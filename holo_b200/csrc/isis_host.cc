@@ -517,21 +517,29 @@ struct SrView {
     }
 };
 
-// Next-hop Vecs of a `local = true` SPT for every SPT vertex (indexed by vertex).
-int local_nexthops(const hspf_isis_flat &f, const hl_isis_instance *in, uint8_t mt_id, uint32_t root,
-                   const uint32_t *dist, const uint16_t *hops, std::vector<std::vector<LNh>> &out) {
-    const uint32_t V = (uint32_t)f.ids.size();
-    const uint8_t level_bit = in->level == 1 ? 1 : 2;
-    // pop order
-    std::vector<uint32_t> pop;
+// The SPT's pop order (distance, then vertex id) and each vertex's position in it.
+void pop_order(uint32_t V, const uint32_t *dist, std::vector<uint32_t> &pop, std::vector<uint32_t> &pos) {
+    pop.clear();
     for (uint32_t v = 0; v < V; ++v) if (dist[v] != HSPF_DIST_INF) pop.push_back(v);
     std::sort(pop.begin(), pop.end(), [&](uint32_t a, uint32_t b) { return dist[a] != dist[b] ? dist[a] < dist[b] : a < b; });
-    std::vector<uint32_t> pos(V, kNone);
+    pos.assign(V, kNone);
     for (uint32_t i = 0; i < pop.size(); ++i) pos[pop[i]] = i;
-    auto relax_ok = [&](uint32_t u, uint32_t e) {     // would the reference relax this edge at all?
-        if (dist[u] == HSPF_DIST_INF || !expands(f.vflags[u], u, root)) return false;
-        return (uint64_t)dist[u] + f.cost[e] <= f.reject_above;
-    };
+}
+
+// would the reference relax edge e out of u at all?  `cost` is the job's edge cost array
+// (HSPF_COST_DISABLED: the edge is gone)
+inline bool relax_ok(const hspf_isis_flat &f, uint32_t root, const uint32_t *dist, const uint32_t *cost, uint32_t u,
+                     uint32_t e) {
+    if (dist[u] == HSPF_DIST_INF || !expands(f.vflags[u], u, root) || cost[e] == HSPF_COST_DISABLED) return false;
+    return (uint64_t)dist[u] + cost[e] <= f.reject_above;
+}
+
+// The resolved next hop of every final DAG edge out of a hops==0 vertex (the root and the pseudonodes
+// attached to it), keyed by forward edge id: resolve_nexthop replayed in pop order.
+std::map<uint32_t, LNh> first_hop_replay(const hspf_isis_flat &f, const hl_isis_instance *in, uint8_t mt_id,
+                                         uint32_t root, const uint32_t *dist, const uint16_t *hops, const uint32_t *cost,
+                                         const std::vector<uint32_t> &pop, const std::vector<uint32_t> &pos) {
+    const uint8_t level_bit = in->level == 1 ? 1 : 2;
     std::set<std::array<uint8_t, 6>> used;
     auto resolve = [&](uint32_t P, uint32_t e, uint32_t R) {
         LNh nh{f.ids[R] >> 8, false, 0, false, 0, false, hl_ip_addr{}};
@@ -545,7 +553,7 @@ int local_nexthops(const hspf_isis_flat &f, const hl_isis_instance *in, uint8_t 
                     if (in->adjs[iface.adj_off + k].system_id == nh.sysid) adj = &in->adjs[iface.adj_off + k];
                 if (adj && (!(mt_id == HL_ISIS_MT_STANDARD ? adj->topo_std : adj->topo_ipv6) || !adj->up)) adj = nullptr;
             } else {
-                if (iface.metric != f.cost[e] || !iface.n_adj) continue;
+                if (iface.metric != cost[e] || !iface.n_adj) continue;
                 const auto &a = in->adjs[iface.adj_off];
                 if ((mt_id == HL_ISIS_MT_STANDARD ? a.topo_std : a.topo_ipv6) && (a.level_usage & level_bit) &&
                     a.system_id == nh.sysid && a.up)
@@ -569,15 +577,16 @@ int local_nexthops(const hspf_isis_flat &f, const hl_isis_instance *in, uint8_t 
         for (uint32_t e = f.row[P]; e < f.row[P + 1]; ++e) {
             const uint32_t R = f.col[e];
             if (pos[R] != kNone && pos[R] < pos[P]) continue;            // already on the SPT
-            const uint64_t d = (uint64_t)dist[P] + f.cost[e];
+            if (cost[e] == HSPF_COST_DISABLED) continue;
+            const uint64_t d = (uint64_t)dist[P] + cost[e];
             if (d > f.reject_above) continue;
             // candidate distance of R at this moment
             uint64_t cb = ~0ull;
             for (uint32_t i = f.irow[R]; i < f.irow[R + 1]; ++i) {
                 const uint32_t u = f.isrc[i], e2 = f.ieid[i];
-                if (!relax_ok(u, e2)) continue;
+                if (!relax_ok(f, root, dist, cost, u, e2)) continue;
                 const bool earlier = (u == P) ? (e2 < e) : (pos[u] < pos[P]);
-                if (earlier) cb = std::min<uint64_t>(cb, (uint64_t)dist[u] + f.cost[e2]);
+                if (earlier) cb = std::min<uint64_t>(cb, (uint64_t)dist[u] + cost[e2]);
             }
             if (d > cb) continue;
             if (!(f.vflags[R] & HSPF_VF_HOP)) continue;                  // pseudonode: nothing is pushed
@@ -585,6 +594,16 @@ int local_nexthops(const hspf_isis_flat &f, const hl_isis_instance *in, uint8_t 
             if (d == dist[R]) first_hop[e] = nh;
         }
     }
+    return first_hop;
+}
+
+// Next-hop Vecs of a `local = true` SPT for every SPT vertex (indexed by vertex).
+int local_nexthops(const hspf_isis_flat &f, const hl_isis_instance *in, uint8_t mt_id, uint32_t root,
+                   const uint32_t *dist, const uint16_t *hops, const uint32_t *cost, std::vector<std::vector<LNh>> &out) {
+    const uint32_t V = (uint32_t)f.ids.size();
+    std::vector<uint32_t> pop, pos;
+    pop_order(V, dist, pop, pos);
+    const std::map<uint32_t, LNh> first_hop = first_hop_replay(f, in, mt_id, root, dist, hops, cost, pop, pos);
     // final Vecs in pop order: parents in (pop position, edge order)
     out.assign(V, {});
     std::vector<std::pair<uint64_t, uint32_t>> tmp;
@@ -593,7 +612,7 @@ int local_nexthops(const hspf_isis_flat &f, const hl_isis_instance *in, uint8_t 
         tmp.clear();
         for (uint32_t i = f.irow[v]; i < f.irow[v + 1]; ++i) {
             const uint32_t u = f.isrc[i], e = f.ieid[i];
-            if (!relax_ok(u, e) || (uint64_t)dist[u] + f.cost[e] != dist[v]) continue;
+            if (!relax_ok(f, root, dist, cost, u, e) || (uint64_t)dist[u] + cost[e] != dist[v]) continue;
             tmp.emplace_back(((uint64_t)pos[u] << 32) | e, u);
         }
         std::sort(tmp.begin(), tmp.end());
@@ -632,115 +651,132 @@ int topology_flat(const hl_isis_instance *in, uint8_t mt_id, hspf_isis_flat &f, 
     return HSPF_OK;
 }
 
-// compute_routes (spf.rs:838-941) for one topology, over that topology's SPT planes
-// (vertex order of `f`).
-int topology_routes(const hl_isis_instance *in, const hspf_isis_flat &f, uint8_t mt_id, uint32_t root,
-                    const uint32_t *dist_p, const uint16_t *hops_p, std::map<NetKey, RouteE> &rib) {
+// The contributions compute_routes (spf.rs:838-941) makes in one topology, in its order: every
+// vertex `visit(v)` accepts, in id_tree (= vertex index) order, with a valid zeroth LSP; its valid
+// fragments in LspId order; per fragment the ATT-bit default routes, then TLV 128, 130, 135 and
+// 236/237 entries.  emit(v, prefix, len, entry metric, external, entry with its Prefix-SID or NULL).
+// Which contributions there are depends only on the LSDB and the instance configuration.
+template <class Visit, class Emit>
+void for_each_contribution(const hl_isis_instance *in, const hspf_isis_flat &f, uint8_t mt_id, Visit visit, Emit emit) {
     const hl_isis_level &l0 = in->lvl;
     const bool std_en = l0.metric_type == HL_ISIS_METRIC_STANDARD || l0.metric_type == HL_ISIS_METRIC_BOTH;
     const bool wide_en = l0.metric_type == HL_ISIS_METRIC_WIDE || l0.metric_type == HL_ISIS_METRIC_BOTH;
     const uint32_t V = (uint32_t)f.ids.size();
-    const uint32_t *dist = dist_p;
-    const uint16_t *hops = hops_p;
-    int rc = HSPF_OK;
-    const SrView sr(l0);
-        std::vector<std::vector<LNh>> vnh;
-        rc = local_nexthops(f, in, mt_id, root, dist, hops, vnh);
-        if (rc) return rc;
-
-        // ---- compute_routes over the SPT in id_tree (= vertex index) order -------------
-        bool attached = false;
-        for (uint32_t i = 0; i < in->n_adjs; ++i) {
-            const auto &a = in->adjs[i];
-            if ((mt_id == HL_ISIS_MT_STANDARD ? a.topo_std : a.topo_ipv6) && a.up && (a.level_usage & 2) && a.area_disjoint) attached = true;
-        }
-        const bool ipv4_enabled = l0.ipv4_enabled && mt_id == HL_ISIS_MT_STANDARD;
-        const bool ipv6_enabled = l0.ipv6_enabled && (mt_id == HL_ISIS_MT_STANDARD ? !in->mt_ipv6_enabled : true);
-        // fragments per LAN id in LspId order
-        std::vector<uint32_t> order(l0.n_lsps);
-        for (uint32_t i = 0; i < l0.n_lsps; ++i) order[i] = i;
-        std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
-            const auto &x = l0.lsps[a], &y = l0.lsps[b];
-            return x.lan_id != y.lan_id ? x.lan_id < y.lan_id : x.fragment < y.fragment;
-        });
-        std::unordered_map<uint64_t, std::vector<uint32_t>> frags;
-        for (uint32_t i : order) frags[l0.lsps[i].lan_id].push_back(i);
-        for (uint32_t v = 0; v < V; ++v) {
-            if (dist[v] == HSPF_DIST_INF) continue;
-            const auto &fr = frags[f.ids[v]];
-            const hl_isis_lsp *z = nullptr;
-            for (uint32_t i : fr)
-                if (l0.lsps[i].fragment == 0) { if (l0.lsps[i].seqno && l0.lsps[i].rem_lifetime) z = &l0.lsps[i]; break; }
-            if (!z) continue;
-            const bool att_bit = !in->att_ignore &&
-                                 (mt_id == HL_ISIS_MT_STANDARD ? (z->flags & HL_LSPF_ATT) : (z->flags & HL_LSPF_MT_IPV6_ATT));
-            auto add = [&](const hl_ip_addr &prefix, uint8_t len, uint32_t nmetric, bool external, const hl_isis_ipreach *src = nullptr) {
-                auto build = [&](std::map<hl_ip_addr, RNh, IpLess> &m) {
-                    for (const LNh &nh : vnh[v]) {
-                        hl_ip_addr addr{};
-                        if (!prefix.is_v6) {
-                            if (!nh.has4) continue;
-                            addr.bytes[0] = (uint8_t)(nh.ipv4 >> 24); addr.bytes[1] = (uint8_t)(nh.ipv4 >> 16);
-                            addr.bytes[2] = (uint8_t)(nh.ipv4 >> 8); addr.bytes[3] = (uint8_t)nh.ipv4;
-                        } else {
-                            if (!nh.has6) continue;
-                            addr = nh.ipv6; addr.is_v6 = 1;
-                        }
-                        m[addr] = RNh{nh.sysid, nh.iface, addr};
-                    }
-                };
-                const uint32_t metric = dist[v] + nmetric;
-                NetKey key{prefix, len};
-                auto rit = rib.find(key);
-                RouteE *route;
-                if (rit == rib.end() || metric < rit->second.metric) {
-                    RouteE r{};
-                    r.flags = hops[v] == 0 ? HL_ROUTE_CONNECTED : 0;
-                    r.type = in->level == 1 ? (external ? HL_ISIS_RT_L1_EXT : HL_ISIS_RT_L1_INTRA)
-                                            : (external ? HL_ISIS_RT_L2_EXT : HL_ISIS_RT_L2_INTRA);
-                    r.metric = metric;
-                    build(r.nh);
-                    if (src && src->has_psid) r.psid = PrefixSid{true, src->psid_flags, src->psid_is_label != 0, src->psid_value};
-                    if (rit == rib.end()) route = &rib.emplace(key, std::move(r)).first->second;
-                    else { rit->second = std::move(r); route = &rit->second; }
-                } else if (metric == rit->second.metric) {
-                    build(rit->second.nh);
-                    route = &rit->second;
-                } else {
-                    return;
-                }
-                while (route->nh.size() > in->max_paths) route->nh.erase(std::prev(route->nh.end()));
-                if (in->sr_enabled && route->psid.present)      // spf.rs:923-939
-                    sr.update(*route, in->system_id, f.ids[v], prefix.is_v6 != 0, hops[v] == 0, hops[v] == 1);
-            };
-            for (uint32_t i : fr) {
-                const auto &lsp = l0.lsps[i];
-                if (!lsp.seqno || !lsp.rem_lifetime) continue;
-                if (att_bit && in->level == 1 && (in->level_type == 1 || !attached)) {
-                    if (ipv4_enabled) add(hl_ip_addr{}, 0, 0, false);
-                    if (ipv6_enabled) { hl_ip_addr z6{}; z6.is_v6 = 1; add(z6, 0, 0, false); }
-                }
-                const hl_isis_ipreach *ip = l0.ipreaches + lsp.ipreach_off;
-                if (mt_id == HL_ISIS_MT_STANDARD && ipv4_enabled) {
-                    if (std_en) {
-                        for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
-                            if (ip[k].kind == HL_ISIS_IP_V4_INTERNAL) add(ip[k].prefix, ip[k].len, ip[k].metric, false);
-                        for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
-                            if (ip[k].kind == HL_ISIS_IP_V4_EXTERNAL) add(ip[k].prefix, ip[k].len, ip[k].metric, true);
-                    }
-                    if (wide_en)
-                        for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
-                            if (ip[k].kind == HL_ISIS_IP_V4_EXT && ip[k].metric <= kMaxWide)
-                                add(ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external, &ip[k]);
-                }
-                if (ipv6_enabled)
-                    for (uint32_t k = 0; k < lsp.n_ipreach; ++k) {
-                        const bool take = mt_id == HL_ISIS_MT_IPV6 ? (ip[k].kind == HL_ISIS_IP_MT_V6 && ip[k].mt_id == HL_ISIS_MT_IPV6)
-                                                                   : (ip[k].kind == HL_ISIS_IP_V6);
-                        if (take) add(ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external, &ip[k]);
-                    }
+    bool attached = false;
+    for (uint32_t i = 0; i < in->n_adjs; ++i) {
+        const auto &a = in->adjs[i];
+        if ((mt_id == HL_ISIS_MT_STANDARD ? a.topo_std : a.topo_ipv6) && a.up && (a.level_usage & 2) && a.area_disjoint) attached = true;
+    }
+    const bool ipv4_enabled = l0.ipv4_enabled && mt_id == HL_ISIS_MT_STANDARD;
+    const bool ipv6_enabled = l0.ipv6_enabled && (mt_id == HL_ISIS_MT_STANDARD ? !in->mt_ipv6_enabled : true);
+    // fragments per LAN id in LspId order
+    std::vector<uint32_t> order(l0.n_lsps);
+    for (uint32_t i = 0; i < l0.n_lsps; ++i) order[i] = i;
+    std::stable_sort(order.begin(), order.end(), [&](uint32_t a, uint32_t b) {
+        const auto &x = l0.lsps[a], &y = l0.lsps[b];
+        return x.lan_id != y.lan_id ? x.lan_id < y.lan_id : x.fragment < y.fragment;
+    });
+    std::unordered_map<uint64_t, std::vector<uint32_t>> frags;
+    for (uint32_t i : order) frags[l0.lsps[i].lan_id].push_back(i);
+    for (uint32_t v = 0; v < V; ++v) {
+        if (!visit(v)) continue;
+        const auto &fr = frags[f.ids[v]];
+        const hl_isis_lsp *z = nullptr;
+        for (uint32_t i : fr)
+            if (l0.lsps[i].fragment == 0) { if (l0.lsps[i].seqno && l0.lsps[i].rem_lifetime) z = &l0.lsps[i]; break; }
+        if (!z) continue;
+        const bool att_bit = !in->att_ignore &&
+                             (mt_id == HL_ISIS_MT_STANDARD ? (z->flags & HL_LSPF_ATT) : (z->flags & HL_LSPF_MT_IPV6_ATT));
+        for (uint32_t i : fr) {
+            const auto &lsp = l0.lsps[i];
+            if (!lsp.seqno || !lsp.rem_lifetime) continue;
+            if (att_bit && in->level == 1 && (in->level_type == 1 || !attached)) {
+                if (ipv4_enabled) emit(v, hl_ip_addr{}, 0, 0, false, nullptr);
+                if (ipv6_enabled) { hl_ip_addr z6{}; z6.is_v6 = 1; emit(v, z6, 0, 0, false, nullptr); }
             }
+            const hl_isis_ipreach *ip = l0.ipreaches + lsp.ipreach_off;
+            if (mt_id == HL_ISIS_MT_STANDARD && ipv4_enabled) {
+                if (std_en) {
+                    for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
+                        if (ip[k].kind == HL_ISIS_IP_V4_INTERNAL) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, false, nullptr);
+                    for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
+                        if (ip[k].kind == HL_ISIS_IP_V4_EXTERNAL) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, true, nullptr);
+                }
+                if (wide_en)
+                    for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
+                        if (ip[k].kind == HL_ISIS_IP_V4_EXT && ip[k].metric <= kMaxWide)
+                            emit(v, ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external != 0, &ip[k]);
+            }
+            if (ipv6_enabled)
+                for (uint32_t k = 0; k < lsp.n_ipreach; ++k) {
+                    const bool take = mt_id == HL_ISIS_MT_IPV6 ? (ip[k].kind == HL_ISIS_IP_MT_V6 && ip[k].mt_id == HL_ISIS_MT_IPV6)
+                                                               : (ip[k].kind == HL_ISIS_IP_V6);
+                    if (take) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external != 0, &ip[k]);
+                }
         }
+    }
+}
+
+// RouteE.type of a contribution
+inline uint8_t route_type(const hl_isis_instance *in, bool external) {
+    return in->level == 1 ? (external ? HL_ISIS_RT_L1_EXT : HL_ISIS_RT_L1_INTRA)
+                          : (external ? HL_ISIS_RT_L2_EXT : HL_ISIS_RT_L2_INTRA);
+}
+
+// A next hop's address in the prefix's family; false when the adjacency has none.
+inline bool nh_addr(const LNh &nh, bool v6, hl_ip_addr &addr) {
+    addr = hl_ip_addr{};
+    if (!v6) {
+        if (!nh.has4) return false;
+        addr.bytes[0] = (uint8_t)(nh.ipv4 >> 24); addr.bytes[1] = (uint8_t)(nh.ipv4 >> 16);
+        addr.bytes[2] = (uint8_t)(nh.ipv4 >> 8); addr.bytes[3] = (uint8_t)nh.ipv4;
+    } else {
+        if (!nh.has6) return false;
+        addr = nh.ipv6; addr.is_v6 = 1;
+    }
+    return true;
+}
+
+// compute_routes (spf.rs:838-941) for one topology, over that topology's SPT planes
+// (vertex order of `f`).
+int topology_routes(const hl_isis_instance *in, const hspf_isis_flat &f, uint8_t mt_id, uint32_t root,
+                    const uint32_t *dist, const uint16_t *hops, std::map<NetKey, RouteE> &rib) {
+    const SrView sr(in->lvl);
+    std::vector<std::vector<LNh>> vnh;
+    int rc = local_nexthops(f, in, mt_id, root, dist, hops, f.cost.data(), vnh);
+    if (rc) return rc;
+    auto add = [&](uint32_t v, const hl_ip_addr &prefix, uint8_t len, uint32_t nmetric, bool external,
+                   const hl_isis_ipreach *src) {
+        auto build = [&](std::map<hl_ip_addr, RNh, IpLess> &m) {
+            for (const LNh &nh : vnh[v]) {
+                hl_ip_addr addr;
+                if (nh_addr(nh, prefix.is_v6 != 0, addr)) m[addr] = RNh{nh.sysid, nh.iface, addr};
+            }
+        };
+        const uint32_t metric = dist[v] + nmetric;
+        NetKey key{prefix, len};
+        auto rit = rib.find(key);
+        RouteE *route;
+        if (rit == rib.end() || metric < rit->second.metric) {
+            RouteE r{};
+            r.flags = hops[v] == 0 ? HL_ROUTE_CONNECTED : 0;
+            r.type = route_type(in, external);
+            r.metric = metric;
+            build(r.nh);
+            if (src && src->has_psid) r.psid = PrefixSid{true, src->psid_flags, src->psid_is_label != 0, src->psid_value};
+            if (rit == rib.end()) route = &rib.emplace(key, std::move(r)).first->second;
+            else { rit->second = std::move(r); route = &rit->second; }
+        } else if (metric == rit->second.metric) {
+            build(rit->second.nh);
+            route = &rit->second;
+        } else {
+            return;
+        }
+        while (route->nh.size() > in->max_paths) route->nh.erase(std::prev(route->nh.end()));
+        if (in->sr_enabled && route->psid.present)      // spf.rs:923-939
+            sr.update(*route, in->system_id, f.ids[v], prefix.is_v6 != 0, hops[v] == 0, hops[v] == 1);
+    };
+    for_each_contribution(in, f, mt_id, [&](uint32_t v) { return dist[v] != HSPF_DIST_INF; }, add);
     return HSPF_OK;
 }
 
@@ -833,3 +869,188 @@ extern "C" int hspf_isis_routes_from_planes(const hl_isis_instance *in, const ui
         return emit_rib(rib, out);
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
 }
+
+/* ---- batched route stage: the table and the per-job decode (isis_route_cells.h) ------------- */
+#include <memory>
+
+#include "isis_route_cells.h"
+
+namespace {
+const uint8_t kTopologies[2] = {HL_ISIS_MT_STANDARD, HL_ISIS_MT_IPV6};    // table topology 0, 1
+}  // namespace
+
+extern "C" {
+
+void hspf_isis_rtable_free(hspf_isis_rtable *rt) {
+    if (!rt) return;
+    hspf_isis_rtable_release_device(rt);
+    delete rt;
+}
+
+int hspf_isis_rtable_create(const hl_isis_instance *in, hspf_isis_rtable **out) {
+    if (!in || !out) return HSPF_E_INVAL;
+    *out = nullptr;
+    try {
+        auto rt = std::make_unique<hspf_isis_rtable>();
+        struct Raw { NetKey key; hspf::IsisContrib c; int32_t src; };
+        std::vector<Raw> raw;
+        for (uint32_t t = 0; t < 2; ++t) {
+            const uint8_t mt_id = kTopologies[t];
+            if (mt_id == HL_ISIS_MT_IPV6 && !in->mt_ipv6_enabled) continue;
+            hspf_isis_flat f;
+            uint32_t root = 0;
+            bool have_root = false;
+            const int rc = topology_flat(in, mt_id, f, root, have_root);
+            if (rc) return rc;
+            rt->n_vertices[t] = (uint32_t)f.ids.size();
+            if (!have_root) continue;
+            rt->root[t] = root;
+            // every vertex: whether a contributor is on the SPT is the job's business
+            for_each_contribution(in, f, mt_id, [](uint32_t) { return true; },
+                                  [&](uint32_t v, const hl_ip_addr &prefix, uint8_t len, uint32_t nmetric, bool external,
+                                      const hl_isis_ipreach *src) {
+                                      Raw r{};
+                                      r.key = NetKey{prefix, len};
+                                      r.c.vertex = v; r.c.metric = nmetric; r.c.topology = (uint8_t)t;
+                                      r.c.external = external ? 1 : 0;
+                                      r.c.has_psid = (src && src->has_psid) ? 1 : 0;
+                                      r.c.sr = (r.c.has_psid && in->sr_enabled) ? 1 : 0;
+                                      r.src = src ? (int32_t)(src - in->lvl.ipreaches) : -1;
+                                      raw.push_back(r);
+                                  });
+        }
+        // NetKey order, walk order within a prefix
+        std::stable_sort(raw.begin(), raw.end(), [](const Raw &a, const Raw &b) { return a.key < b.key; });
+        for (size_t i = 0; i < raw.size(); ++i) {
+            if (i == 0 || raw[i - 1].key < raw[i].key) {
+                rt->prefix.push_back(raw[i].key.a); rt->len.push_back(raw[i].key.len); rt->off.push_back((uint32_t)i);
+            }
+            rt->contribs.push_back(raw[i].c);
+            rt->src.push_back(raw[i].src);
+        }
+        rt->off.push_back((uint32_t)raw.size());
+        *out = rt.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+uint32_t hspf_isis_rtable_prefixes(const hspf_isis_rtable *rt) { return rt ? (uint32_t)rt->prefix.size() : 0; }
+uint32_t hspf_isis_rtable_contributors(const hspf_isis_rtable *rt) { return rt ? (uint32_t)rt->contribs.size() : 0; }
+
+int hspf_isis_rtable_topology(const hspf_isis_rtable *rt, uint32_t topology, uint32_t *n_vertices, uint32_t *root) {
+    if (!rt || topology > 1) return HSPF_E_INVAL;
+    if (n_vertices) *n_vertices = rt->n_vertices[topology];
+    if (root) *root = rt->root[topology];
+    return HSPF_OK;
+}
+
+int hspf_isis_rtable_arrays(const hspf_isis_rtable *rt, const hl_ip_addr **prefix, const uint32_t **len,
+                            const uint32_t **off, const void **contribs) {
+    if (!rt) return HSPF_E_INVAL;
+    if (prefix) *prefix = rt->prefix.data();
+    if (len) *len = rt->len.data();
+    if (off) *off = rt->off.data();
+    if (contribs) *contribs = rt->contribs.data();
+    return HSPF_OK;
+}
+
+int hspf_isis_routes_from_cells(const hl_isis_instance *in, const hspf_isis_rtable *rt, const hl_isis_route_cell *cells,
+                                const uint32_t *dist_std, const uint16_t *hops_std,
+                                const uint32_t *dist_mt6, const uint16_t *hops_mt6,
+                                uint32_t n_ov_std, const uint32_t *ov_edge_std, const uint32_t *ov_cost_std,
+                                uint32_t n_ov_mt6, const uint32_t *ov_edge_mt6, const uint32_t *ov_cost_mt6,
+                                hl_isis_rib *out) {
+    if (!in || !rt || !out || (!cells && !rt->prefix.empty())) return HSPF_E_INVAL;
+    try {
+        // per topology: the flat, the job's planes, and what each first-hop atom resolves to
+        struct Topo {
+            hspf_isis_flat f;
+            const uint16_t *hops = nullptr;
+            bool live = false;
+            LNh atom_nh[64];
+            bool atom_has[64] = {};
+        };
+        auto tp = std::make_unique<Topo[]>(2);
+        for (uint32_t t = 0; t < 2; ++t) {
+            const uint8_t mt_id = kTopologies[t];
+            if (mt_id == HL_ISIS_MT_IPV6 && !in->mt_ipv6_enabled) continue;
+            Topo &T = tp[t];
+            uint32_t root = 0;
+            bool have_root = false;
+            int rc = topology_flat(in, mt_id, T.f, root, have_root);
+            if (rc) return rc;
+            // not the instance the table was built from
+            if (T.f.ids.size() != rt->n_vertices[t] || (have_root ? root : kNone) != rt->root[t]) return HSPF_E_INVAL;
+            if (!have_root) continue;
+            const uint32_t *dist = t ? dist_mt6 : dist_std;
+            T.hops = t ? hops_mt6 : hops_std;
+            const uint32_t n_ov = t ? n_ov_mt6 : n_ov_std;
+            const uint32_t *ov_edge = t ? ov_edge_mt6 : ov_edge_std, *ov_cost = t ? ov_cost_mt6 : ov_cost_std;
+            if (!dist || !T.hops || (n_ov && (!ov_edge || !ov_cost))) return HSPF_E_INVAL;
+            std::vector<uint32_t> cost(T.f.cost);
+            for (uint32_t k = 0; k < n_ov; ++k) {
+                if (ov_edge[k] >= cost.size()) return HSPF_E_INVAL;
+                cost[ov_edge[k]] = ov_cost[k];
+            }
+            std::vector<uint32_t> pop, pos;
+            pop_order((uint32_t)T.f.ids.size(), dist, pop, pos);
+            const std::map<uint32_t, LNh> first_hop = first_hop_replay(T.f, in, mt_id, root, dist, T.hops, cost.data(), pop, pos);
+            hspf_csr csr;
+            fill_csr(T.f, &csr);
+            uint32_t n_atoms = 0;
+            if (hspf_atom_count(&csr, root, &n_atoms) != HSPF_OK) return HSPF_E_INVAL;
+            for (uint32_t a = 0; a < std::min<uint32_t>(n_atoms, 64); ++a) {
+                uint32_t tail = 0, edge = 0;
+                if (hspf_atom_decode(&csr, root, a, &tail, &edge) != HSPF_OK) continue;
+                auto it = first_hop.find(edge);
+                if (it == first_hop.end()) continue;
+                T.atom_nh[a] = it->second;
+                T.atom_has[a] = true;
+            }
+            T.live = true;
+        }
+        const SrView sr(in->lvl);
+        std::map<NetKey, RouteE> rib;
+        const uint32_t P = (uint32_t)rt->prefix.size();
+        for (uint32_t p = 0; p < P; ++p) {
+            const hl_isis_route_cell &c = cells[p];
+            if (!(c.flags & HL_CELL_PRESENT)) continue;
+            if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
+            if (c.winner < rt->off[p] || c.winner >= rt->off[p + 1]) return HSPF_E_INVAL;
+            const hspf::IsisContrib &k = rt->contribs[c.winner];
+            const Topo &T = tp[k.topology];
+            if (!T.live || k.vertex >= T.f.ids.size()) return HSPF_E_INVAL;
+            const bool v6 = rt->prefix[p].is_v6 != 0;
+            RouteE r{};
+            r.flags = (c.flags & HL_CELL_CONNECTED) ? HL_ROUTE_CONNECTED : 0;
+            r.type = route_type(in, k.external != 0);
+            r.metric = c.metric;
+            // the union of the best-metric contributors' next hops; an address reached over two different
+            // adjacencies keeps whichever `add` wrote last, which the cell cannot tell
+            for (uint64_t m = c.nh_mask; m; m &= m - 1) {
+                const uint32_t a = (uint32_t)__builtin_ctzll(m);
+                hl_ip_addr addr;
+                if (!T.atom_has[a] || !nh_addr(T.atom_nh[a], v6, addr)) continue;
+                const RNh x{T.atom_nh[a].sysid, T.atom_nh[a].iface, addr};
+                auto ins = r.nh.emplace(addr, x);
+                if (!ins.second && (ins.first->second.sysid != x.sysid || ins.first->second.iface != x.iface))
+                    return HSPF_E_UNSUPPORTED;
+            }
+            while (r.nh.size() > in->max_paths) r.nh.erase(std::prev(r.nh.end()));
+            if (k.has_psid) {
+                const int32_t s = rt->src[c.winner];
+                if (s < 0 || (uint32_t)s >= in->lvl.n_ipreaches) return HSPF_E_INVAL;
+                const hl_isis_ipreach &e = in->lvl.ipreaches[s];
+                r.psid = PrefixSid{true, e.psid_flags, e.psid_is_label != 0, e.psid_value};
+            }
+            // all best-metric contributions come from the winner's vertex (else the cell is flagged):
+            // one update with its context gives the labels every repeated update would
+            if (in->sr_enabled && r.psid.present)
+                sr.update(r, in->system_id, T.f.ids[k.vertex], v6, T.hops[k.vertex] == 0, T.hops[k.vertex] == 1);
+            rib.emplace_hint(rib.end(), NetKey{rt->prefix[p], (uint8_t)rt->len[p]}, std::move(r));
+        }
+        return emit_rib(rib, out);
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+}  // extern "C"

@@ -408,6 +408,7 @@ int hspf_abi_sizes(uint32_t *out, uint32_t cap) {
         (uint32_t)sizeof(hl_ospfv2_rtr_tables),
         (uint32_t)sizeof(hl_isis_lsp_trigger), (uint32_t)sizeof(hl_ip_prefix), (uint32_t)sizeof(hl_lsa_trigger6),
         (uint32_t)sizeof(hl_spf_computation6),
+        (uint32_t)sizeof(hl_isis_route_cell),
     };
     static_assert(sizeof(hl_rib_action) == 12, "hl_rib_action layout");
     const uint32_t n = sizeof(v) / sizeof(v[0]);

@@ -419,6 +419,118 @@ def routes_from_planes(inst: dict, spf) -> IsisRib:
     return res
 
 
+# ---- batched route stage (include/holo_spf_lsdb.h: hspf_isis_rtable_*, hspf_isis_routes_batch*) --------
+CELL_DT = np.dtype([("nh_mask", "<u8"), ("winner", "<u4"), ("metric", "<u4"), ("flags", "u1"), ("_pad", "u1", (7,))])
+CONTRIB_DT = np.dtype([("vertex", "<u4"), ("metric", "<u4"), ("topology", "u1"), ("external", "u1"), ("has_psid", "u1"),
+                       ("sr", "u1"), ("_pad", "<u4")])
+CELL_PRESENT, CELL_CONNECTED, CELL_MIXED_SID = 1, 2, 4
+TOPO_STD, TOPO_MT6 = 0, 1
+NO_ROOT = 0xFFFFFFFF
+
+
+class RouteTable:
+    """hspf_isis_rtable: the instance's prefixes in NetKey order and their contributors (host);
+    `upload(ctx)` copies it to the device for hspf_isis_routes_batch.  `n_vertices[t]` / `root[t]` per
+    topology (TOPO_STD, TOPO_MT6; root NO_ROOT: the topology has no routes)."""
+
+    def __init__(self, inst: dict):
+        lib = capi.load_library()
+        lib.hspf_isis_rtable_create.argtypes = [C.POINTER(InstanceStruct), C.POINTER(C.c_void_p)]
+        lib.hspf_isis_rtable_free.argtypes = [C.c_void_p]
+        lib.hspf_isis_rtable_free.restype = None
+        lib.hspf_isis_rtable_prefixes.argtypes = [C.c_void_p]
+        lib.hspf_isis_rtable_prefixes.restype = C.c_uint32
+        lib.hspf_isis_rtable_contributors.argtypes = [C.c_void_p]
+        lib.hspf_isis_rtable_contributors.restype = C.c_uint32
+        lib.hspf_isis_rtable_topology.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
+        lib.hspf_isis_rtable_arrays.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint32)),
+                                                C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_void_p)]
+        lib.hspf_isis_rtable_upload.argtypes = [C.c_void_p, C.c_void_p]
+        self.lib = lib
+        s = instance_struct(inst)
+        h = C.c_void_p()
+        rc = lib.hspf_isis_rtable_create(C.byref(s), C.byref(h))
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, "hspf_isis_rtable_create failed")
+        self.handle = h
+        self.n_prefixes = int(lib.hspf_isis_rtable_prefixes(h))
+        self.n_contributors = int(lib.hspf_isis_rtable_contributors(h))
+        self.n_vertices, self.root = [], []
+        for t in (TOPO_STD, TOPO_MT6):
+            nv, r = C.c_uint32(), C.c_uint32()
+            lib.hspf_isis_rtable_topology(h, t, C.byref(nv), C.byref(r))
+            self.n_vertices.append(nv.value)
+            self.root.append(r.value)
+        pp, pl, po, pc = C.c_void_p(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.c_void_p()
+        lib.hspf_isis_rtable_arrays(h, C.byref(pp), C.byref(pl), C.byref(po), C.byref(pc))
+        P, K = self.n_prefixes, self.n_contributors
+        self.prefix = (np.frombuffer(C.string_at(pp.value, P * IP_DT.itemsize), IP_DT).copy() if P else np.zeros(0, IP_DT))
+        self.len = np.ctypeslib.as_array(pl, shape=(P,)).copy() if P else np.zeros(0, np.uint32)
+        self.off = np.ctypeslib.as_array(po, shape=(P + 1,)).copy()
+        self.contribs = (np.frombuffer(C.string_at(pc.value, K * CONTRIB_DT.itemsize), CONTRIB_DT).copy()
+                         if K else np.zeros(0, CONTRIB_DT))
+
+    def upload(self, ctx: capi.Context):
+        rc = self.lib.hspf_isis_rtable_upload(ctx.handle, self.handle)
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, ctx.last_error())
+
+    def __del__(self):
+        try:
+            if self.handle:
+                self.lib.hspf_isis_rtable_free(self.handle)
+                self.handle = None
+        except Exception:
+            pass
+
+
+def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, rs_mt6, cells_ptr: int):
+    """hspf_isis_routes_batch / _batch16 over DEVICE planes (rs_*: capi.ResultStruct or capi.Result16Struct holding
+    device pointers, one per topology; rs_mt6 may be None unless the table has an MT-IPv6 root); cells_ptr: device
+    buffer of n_jobs * rt.n_prefixes cells.  Enqueued on the ctx stream; the table must have been uploaded."""
+    lib = ctx.lib
+    narrow = isinstance(rs_std if rs_std is not None else rs_mt6, capi.Result16Struct)
+    fn = lib.hspf_isis_routes_batch16 if narrow else lib.hspf_isis_routes_batch
+    fn.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
+    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs_std) if rs_std is not None else None,
+            C.byref(rs_mt6) if rs_mt6 is not None else None, cells_ptr)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
+def routes_from_cells(inst: dict, rt: RouteTable, cells: np.ndarray, std=None, mt6=None, ov_std=(), ov_mt6=()) -> IsisRib:
+    """hspf_isis_routes_from_cells (host): one job's cells -> the table hspf_isis_routes_from_planes gives for the
+    same planes.  std / mt6: that job's (dist u32[V], hops u16[V]) per topology; ov_*: its [(edge, cost), ...]
+    overrides.  rc HSPF_E_UNSUPPORTED is returned in the result (caller: routes_from_planes)."""
+    lib = capi.load_library()
+    u32p, u16p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16)
+    lib.hspf_isis_routes_from_cells.argtypes = [C.POINTER(InstanceStruct), C.c_void_p, C.c_void_p, u32p, u16p, u32p, u16p,
+                                                C.c_uint32, u32p, u32p, C.c_uint32, u32p, u32p, C.POINTER(RibStruct)]
+    cells = np.ascontiguousarray(cells, CELL_DT)
+    assert cells.shape == (rt.n_prefixes,)
+    keep = [cells]
+
+    def arr(a, dt, ty):
+        if a is None:
+            return C.cast(None, ty)
+        a = np.ascontiguousarray(a, dt)
+        keep.append(a)
+        return a.ctypes.data_as(ty)
+
+    def planes(p):
+        return (arr(None, None, u32p), arr(None, None, u16p)) if p is None else (arr(p[0], np.uint32, u32p), arr(p[1], np.uint16, u16p))
+
+    def ov(o):
+        o = list(o)
+        return (len(o), arr([e for e, _ in o] or [0], np.uint32, u32p), arr([c for _, c in o] or [0], np.uint32, u32p))
+
+    tail = (rt.handle, cells.ctypes.data, *planes(std), *planes(mt6), *ov(ov_std), *ov(ov_mt6))
+    res = _call_rib(lib.hspf_isis_routes_from_cells, inst, (), tail_args=tail)
+    if res.rc not in (capi.HSPF_OK, capi.HSPF_E_UNSUPPORTED):
+        raise capi.HspfError(res.rc, "hspf_isis_routes_from_cells failed")
+    return res
+
+
 # ---- flooding reduction over hop-count SPTs (holo-isis/src/flooding/manet.rs) ------------------
 def _spt_struct(spt: IsisSpt, keep: list) -> SptStruct:
     r = SptStruct()

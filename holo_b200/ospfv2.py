@@ -89,7 +89,7 @@ def abi_sizes_expected():
             [isis.RNL_DT.itemsize, CELL_DT.itemsize, TRIGGER_DT.itemsize, C.sizeof(SpfComputationStruct),
              ospf_rib.RIB_RTR_DT.itemsize, C.sizeof(ospf_rib.RtrTablesStruct),
              isis.LSP_TRIGGER_DT.itemsize, ospfv3.IP_PREFIX_DT.itemsize, ospfv3.TRIGGER6_DT.itemsize,
-             C.sizeof(ospfv3.SpfComputation6Struct)])
+             C.sizeof(ospfv3.SpfComputation6Struct), isis.CELL_DT.itemsize])
 
 
 def abi_sizes_from_library():

@@ -840,6 +840,21 @@ typedef struct hl_isis_spt {
     uint32_t second_hops_cap, n_second_hops;  uint32_t *second_hops;
 } hl_isis_spt;
 
+/* One (job, prefix) cell of the IS-IS device route stage (hspf_isis_routes_batch): what compute_routes
+ * (holo-isis/src/spf.rs:838-941) leaves for that prefix in the SPT of that job, next hops still as
+ * first-hop atoms of the prefix's topology (hspf_atom_decode for the job's root).  Prefixes are those
+ * of the instance's route table (hspf_isis_rtable_prefixes), in NetKey order.  flags: HL_CELL_PRESENT,
+ * HL_CELL_CONNECTED (the winner's vertex has hops == 0), HL_CELL_MIXED_SID (SR enabled, the route has
+ * a Prefix-SID and its best-metric contributions come from two or more vertices: redo this job through
+ * hspf_isis_routes_from_planes). */
+typedef struct hl_isis_route_cell {
+    uint64_t nh_mask;       /* union of the best-metric contributors' atom sets                         */
+    uint32_t winner;        /* contributor that set type, CONNECTED and Prefix-SID (table index)        */
+    uint32_t metric;        /* distance + entry metric, u32 as compute_routes adds them                 */
+    uint8_t  flags;         /* HL_CELL_*                                                                */
+    uint8_t  _pad[7];
+} hl_isis_route_cell;
+
 #ifdef __cplusplus
 }
 #endif

@@ -316,6 +316,56 @@ int hspf_isis_compute_routes(hspf_ctx *ctx, const hl_isis_instance *inst, hl_isi
 int hspf_isis_routes_from_planes(const hl_isis_instance *inst, const uint32_t *dist_std, const uint16_t *hops_std,
                                  const uint32_t *dist_mt6, const uint16_t *hops_mt6, hl_isis_rib *out);
 
+/*
+ * Batched IS-IS route stage on the device (compute_routes, holo-isis/src/spf.rs:838-941, for every job of a
+ * what-if batch).
+ *
+ *   hspf_isis_rtable_create   per instance: the prefixes of the enabled topologies in NetKey order and, per
+ *                             prefix, its contributors in the order compute_routes meets them (vertex order,
+ *                             fragments in LspId order, ATT default, TLV 128, 130, 135, 236/237).  Each prefix
+ *                             is fed by one topology: IPv4 by the standard one, IPv6 by the standard one or,
+ *                             with inst->mt_ipv6_enabled, by MT-IPv6 only.  Vertex numbering per topology is
+ *                             that of hspf_isis_flatten with lvl.mt_id set and HL_ISIS_MODE_NORMAL.  Host only;
+ *                             `inst` must outlive the call only.
+ *   hspf_isis_rtable_topology vertex count and root vertex (0xFFFFFFFF: the root owns no LSP there, or the
+ *                             topology is not enabled) of topology 0 (standard) or 1 (MT-IPv6).
+ *   hspf_isis_rtable_upload   copies the table to the ctx's device.
+ *   hspf_isis_routes_batch    one thread per (job, prefix) over DEVICE planes [n_jobs][V] of each topology
+ *   hspf_isis_routes_batch16  written by hspf_run_batch_async / hspf_run_batch16_async with nh_words == 1:
+ *                             cells[n_jobs][P] (device).  `mt6` may be NULL unless the table has an MT-IPv6
+ *                             root.  A job whose status word is non-zero in either topology gets empty cells.
+ *                             Enqueued on the ctx stream behind the batches; no synchronisation.
+ *   hspf_isis_routes_from_cells   host: one job's cells -> exactly the hl_isis_rib hspf_isis_routes_from_planes
+ *                             returns for the same planes (routes, next hops, SR labels).  dist_* / hops_*: that
+ *                             job's planes (the first-hop replay around the root reads them); ov_*: that job's
+ *                             edge overrides per topology (HSPF_COST_DISABLED: the edge relaxes nothing), so
+ *                             that a what-if job decodes to the routes of an LSDB carrying those metrics.
+ *                             HSPF_E_UNSUPPORTED: a cell is flagged HL_CELL_MIXED_SID, or two atoms resolve to
+ *                             the same address with different attributes: take this job through
+ *                             hspf_isis_routes_from_planes.
+ */
+typedef struct hspf_isis_rtable hspf_isis_rtable;
+int hspf_isis_rtable_create(const hl_isis_instance *inst, hspf_isis_rtable **out);
+void hspf_isis_rtable_free(hspf_isis_rtable *rt);
+uint32_t hspf_isis_rtable_prefixes(const hspf_isis_rtable *rt);
+uint32_t hspf_isis_rtable_contributors(const hspf_isis_rtable *rt);
+int hspf_isis_rtable_topology(const hspf_isis_rtable *rt, uint32_t topology, uint32_t *n_vertices, uint32_t *root);
+/* prefix[P], len[P], off[P+1], contribs[K] (16-byte records {vertex, metric, topology, external, Prefix-SID
+ * present, SR-relevant}, isis_route_cells.h); any pointer may be NULL */
+int hspf_isis_rtable_arrays(const hspf_isis_rtable *rt, const hl_ip_addr **prefix, const uint32_t **len,
+                            const uint32_t **off, const void **contribs);
+int hspf_isis_rtable_upload(hspf_ctx *ctx, hspf_isis_rtable *rt);
+int hspf_isis_routes_batch(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result *std_planes,
+                           const hspf_result *mt6_planes, hl_isis_route_cell *cells);
+int hspf_isis_routes_batch16(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result16 *std_planes,
+                             const hspf_result16 *mt6_planes, hl_isis_route_cell *cells);
+int hspf_isis_routes_from_cells(const hl_isis_instance *inst, const hspf_isis_rtable *rt, const hl_isis_route_cell *cells,
+                                const uint32_t *dist_std, const uint16_t *hops_std,
+                                const uint32_t *dist_mt6, const uint16_t *hops_mt6,
+                                uint32_t n_ov_std, const uint32_t *ov_edge_std, const uint32_t *ov_cost_std,
+                                uint32_t n_ov_mt6, const uint32_t *ov_edge_mt6, const uint32_t *ov_cost_mt6,
+                                hl_isis_rib *out);
+
 /* sizeof() of the ABI structs in declaration order (hspf_csr, hspf_jobs,
  * hspf_result, then every struct of holo_lsdb.h); returns the count.  Lets a
  * foreign binding verify its struct layouts at load time. */
