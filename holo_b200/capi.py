@@ -153,6 +153,8 @@ def load_library(path: Path | None = None) -> C.CDLL:
     lib.hspf_run_batch16.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(JobsStruct), C.POINTER(Result16Struct), C.c_uint32]
     lib.hspf_run_batch16_async.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(JobsStruct), C.POINTER(Result16Struct)]
     lib.hspf_graph_info.argtypes = [C.c_void_p, C.POINTER(C.c_uint32)]
+    from . import route_table
+    route_table.declare(lib)
     if path is None:
         _lib = lib
     return lib

@@ -883,7 +883,7 @@ extern "C" {
 
 void hspf_isis_rtable_free(hspf_isis_rtable *rt) {
     if (!rt) return;
-    hspf_isis_rtable_release_device(rt);
+    hspf::release_route_table(rt->dev);
     delete rt;
 }
 

@@ -94,12 +94,5 @@ struct hspf_isis_rtable {
     std::vector<int32_t> src;                // per contributor: index into lvl.ipreaches, -1 for an ATT default route
     uint32_t n_vertices[2] = {0, 0};         // per topology (0 standard, 1 MT-IPv6)
     uint32_t root[2] = {0xFFFFFFFFu, 0xFFFFFFFFu};
-    // device copies (hspf_isis_rtable_upload)
-    void *d_blob = nullptr;
-    const uint32_t *d_off = nullptr;
-    const hspf::IsisContrib *d_contribs = nullptr;
-    int device = -1;
+    hspf::DeviceRouteTable dev;              // hspf_isis_rtable_upload
 };
-
-// frees the device copy (isis_routes.cu); called by hspf_isis_rtable_free
-void hspf_isis_rtable_release_device(hspf_isis_rtable *rt);

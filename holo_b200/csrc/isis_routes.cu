@@ -5,12 +5,9 @@
 // contributors (isis_route_cells.h: isis_route_cell_eval) and writes one 24-byte cell.  Prefix is the fast
 // index: contributor records and cells are read / written coalesced, the plane values are gathers inside
 // the job's own rows of the prefix's topology.  The stage is bounded by the cell writes.
-#include <cuda_runtime.h>
-
-#include <algorithm>
-
 #include "../../include/holo_spf_lsdb.h"
 #include "isis_route_cells.h"
+#include "route_stage.cuh"
 
 namespace {
 
@@ -27,106 +24,49 @@ struct TopoPlanes {
     __device__ __forceinline__ bool refused(uint32_t j) const { return status && status[j] != 0; }
 };
 
+// The cell of (job, prefix): isis_route_cell_eval over the job's rows of both topologies' planes.
 template <class Planes, class D, class N>
-__global__ void __launch_bounds__(256)
+struct IsisCell {
+    const uint32_t *off; const IsisContrib *contribs; TopoPlanes<Planes, D, N> std_pl, mt6_pl;
+    __device__ __forceinline__ bool refused(uint32_t j) const { return std_pl.refused(j) || mt6_pl.refused(j); }
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        const hl_isis_route_cell c = hspf::isis_route_cell_eval(std_pl.job(j), mt6_pl.job(j), contribs, off[p], off[p + 1]);
+        return {c.nh_mask, (uint64_t)c.winner | ((uint64_t)c.metric << 32), c.flags};
+    }
+};
+
+template <class Planes, class D, class N>
+__global__ void __launch_bounds__(hspf::kRouteThreads)
 isis_route_cells_kernel(uint32_t n_jobs, uint32_t P, const uint32_t *__restrict__ off,
                         const IsisContrib *__restrict__ contribs, TopoPlanes<Planes, D, N> std_pl,
                         TopoPlanes<Planes, D, N> mt6_pl, hl_isis_route_cell *__restrict__ cells, bool aligned16) {
-    // a warp owns 32 consecutive cells = one contiguous 768-byte span of the output: the cells are staged in
-    // shared memory and leave as 48 16-byte stores (full sectors) instead of 96 scattered 8-byte ones
-    __shared__ __align__(16) uint64_t stage[8][96];
-    const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const uint64_t total = (uint64_t)n_jobs * P;
-    const uint64_t n_tiles = (total + 31) / 32;
-    const uint64_t wstride = (uint64_t)gridDim.x * 8;
-    for (uint64_t tile = (uint64_t)blockIdx.x * 8 + wib; tile < n_tiles; tile += wstride) {
-        const uint64_t idx = tile * 32 + lane;
-        uint64_t w0 = 0, w1 = 0xFFFFFFFFull, w2 = 0;         // an empty cell: no route, winner none
-        if (idx < total) {
-            const uint32_t job = (uint32_t)(idx / P), p = (uint32_t)(idx - (uint64_t)job * P);
-            // planes of a refused job are undefined: empty cells
-            if (!std_pl.refused(job) && !mt6_pl.refused(job)) {
-                const hl_isis_route_cell c =
-                    hspf::isis_route_cell_eval(std_pl.job(job), mt6_pl.job(job), contribs, off[p], off[p + 1]);
-                w0 = c.nh_mask;
-                w1 = (uint64_t)c.winner | ((uint64_t)c.metric << 32);
-                w2 = c.flags;
-            }
-        }
-        if (aligned16 && tile * 32 + 32 <= total) {
-            uint64_t *s = stage[wib];
-            s[lane * 3 + 0] = w0; s[lane * 3 + 1] = w1; s[lane * 3 + 2] = w2;
-            __syncwarp();
-            const uint4 *s4 = reinterpret_cast<const uint4 *>(s);
-            uint4 *o4 = reinterpret_cast<uint4 *>(cells + tile * 32);
-            o4[lane] = s4[lane];
-            if (lane < 16) o4[32 + lane] = s4[32 + lane];
-            __syncwarp();
-        } else if (idx < total) {
-            uint64_t *o = reinterpret_cast<uint64_t *>(cells + idx);
-            o[0] = w0; o[1] = w1; o[2] = w2;
-        }
-    }
+    const IsisCell<Planes, D, N> cell{off, contribs, std_pl, mt6_pl};
+    hspf::store_route_cells(n_jobs, P, cell, hspf::CellWords{0, 0xFFFFFFFFu, 0}, cells, aligned16);   // empty: winner none
 }
-static_assert(sizeof(hl_isis_route_cell) == 24, "hl_isis_route_cell layout");
 
 template <class Planes, class D, class N>
 int launch_isis_cells(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, TopoPlanes<Planes, D, N> std_pl,
                       TopoPlanes<Planes, D, N> mt6_pl, hl_isis_route_cell *cells) {
-    if (!ctx || !rt || !rt->d_blob || !cells) return HSPF_E_INVAL;
+    if (!ctx || !rt || !rt->dev.blob || !cells) return HSPF_E_INVAL;
     // every topology the table reads needs its planes
     if (rt->root[0] != 0xFFFFFFFFu && (!std_pl.dist || !std_pl.hops || !std_pl.nh)) return HSPF_E_INVAL;
     if (rt->root[1] != 0xFFFFFFFFu && (!mt6_pl.dist || !mt6_pl.hops || !mt6_pl.nh)) return HSPF_E_INVAL;
     const uint32_t P = (uint32_t)rt->prefix.size();
     const uint64_t total = (uint64_t)n_jobs * P;
     if (total == 0) return HSPF_OK;
-    const int dev = hspf_ctx_device(ctx);
-    if (rt->device != dev) return HSPF_E_INVAL;               // the table was uploaded to another device
-    int sms = 0;
-    if (cudaSetDevice(dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-        return HSPF_E_CUDA;
-    // one resident wave (8 blocks of 256 per SM), warp-tile-stride beyond that
-    const uint64_t want = std::max<uint64_t>((total + 255) / 256, 1);
-    const uint32_t blocks = (uint32_t)std::min<uint64_t>(want, (uint64_t)sms * 8);
-    const bool aligned16 = (reinterpret_cast<uintptr_t>(cells) & 15u) == 0;
-    cudaStream_t st = static_cast<cudaStream_t>(hspf_stream(ctx));
-    isis_route_cells_kernel<Planes, D, N><<<blocks, 256, 0, st>>>(n_jobs, P, rt->d_off, rt->d_contribs, std_pl, mt6_pl,
-                                                                  cells, aligned16);
-    if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
-    hspf_note_launches(ctx, 1);
-    return HSPF_OK;
+    return hspf::launch_route_stage(ctx, rt->dev, total, cells, [&](uint32_t blocks, cudaStream_t st, bool aligned16) {
+        isis_route_cells_kernel<Planes, D, N><<<blocks, hspf::kRouteThreads, 0, st>>>(
+            n_jobs, P, rt->dev.off, static_cast<const IsisContrib *>(rt->dev.contribs), std_pl, mt6_pl, cells, aligned16);
+    });
 }
 
 }  // namespace
 
-void hspf_isis_rtable_release_device(hspf_isis_rtable *rt) {
-    if (rt && rt->d_blob) {
-        cudaFree(rt->d_blob);
-        rt->d_blob = nullptr; rt->d_off = nullptr; rt->d_contribs = nullptr;
-    }
-}
-
 extern "C" {
 
 int hspf_isis_rtable_upload(hspf_ctx *ctx, hspf_isis_rtable *rt) {
-    if (!ctx || !rt) return HSPF_E_INVAL;
-    hspf_isis_rtable_release_device(rt);
-    if (cudaSetDevice(hspf_ctx_device(ctx)) != cudaSuccess) return HSPF_E_CUDA;
-    const size_t off_bytes = (rt->off.size() * sizeof(uint32_t) + 15) & ~(size_t)15;
-    const size_t con_bytes = rt->contribs.size() * sizeof(IsisContrib);
-    void *blob = nullptr;
-    if (cudaMalloc(&blob, off_bytes + std::max<size_t>(con_bytes, 16)) != cudaSuccess) return HSPF_E_NOMEM;
-    cudaStream_t st = static_cast<cudaStream_t>(hspf_stream(ctx));
-    cudaError_t e = cudaMemcpyAsync(blob, rt->off.data(), rt->off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess && con_bytes)
-        e = cudaMemcpyAsync(static_cast<char *>(blob) + off_bytes, rt->contribs.data(), con_bytes, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);      // the host vectors may go away after the call
-    if (e != cudaSuccess) { cudaFree(blob); return HSPF_E_CUDA; }
-    rt->d_blob = blob;
-    rt->device = hspf_ctx_device(ctx);
-    rt->d_off = static_cast<const uint32_t *>(blob);
-    rt->d_contribs = reinterpret_cast<const IsisContrib *>(static_cast<char *>(blob) + off_bytes);
-    return HSPF_OK;
+    return rt ? hspf::upload_route_table(ctx, rt->dev, rt->off, rt->contribs.data(), rt->contribs.size() * sizeof(IsisContrib))
+              : HSPF_E_INVAL;
 }
 
 int hspf_isis_routes_batch(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result *std_planes,

@@ -738,7 +738,7 @@ int hspf_ospfv2_area_from_planes(const hl_ospfv2_area *a, const uint32_t *dist, 
 
 void hspf_ospfv2_rtable_free(hspf_ospfv2_rtable *rt) {
     if (!rt) return;
-    hspf_rtable_release_device(rt);
+    hspf::release_route_table(rt->dev);
     delete rt;
 }
 

@@ -7,8 +7,6 @@
 // the job's own rows (200 KB at 10k vertices: L2 hits).  HBM traffic per job is the cells
 // (24 B x prefixes) plus one pass over the three planes; the walk itself is a handful of integer
 // instructions per advertiser, so the stage is bounded by the cell writes.
-#include <cuda_runtime.h>
-
 #include <algorithm>
 #include <cstring>
 #include <memory>
@@ -16,86 +14,57 @@
 #include <vector>
 
 #include "../../include/holo_spf_lsdb.h"
-#include "route_cells.h"
+#include "route_stage.cuh"
 
 namespace {
 
 using hspf::RouteContrib;
 
+// The cell of (job, prefix): route_cell_eval over the job's rows of the planes.
 template <class Planes, class D, class N>
-__global__ void __launch_bounds__(256)
+struct OspfCell {
+    const uint32_t *off; const RouteContrib *contribs; const D *dist; const uint16_t *hops; const N *nh;
+    const uint32_t *status; uint32_t V;
+    __device__ __forceinline__ bool refused(uint32_t j) const { return status && status[j] != 0; }
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        const size_t base = (size_t)j * V;
+        const hl_route_cell c = hspf::route_cell_eval(Planes{dist + base, hops + base, nh + base}, contribs, off[p], off[p + 1]);
+        return {c.nh_mask, c.lasthop_mask, (uint64_t)c.winner | ((uint64_t)c.metric << 32) | ((uint64_t)c.flags << 48)};
+    }
+};
+
+// the bound keeps the walk in 32 registers, so the whole grid launch_route_stage sizes is resident at once
+template <class Planes, class D, class N>
+__global__ void __launch_bounds__(hspf::kRouteThreads, hspf::kRouteBlocksPerSM)
 route_cells_kernel(uint32_t n_jobs, uint32_t P, uint32_t V, const uint32_t *__restrict__ off,
                    const RouteContrib *__restrict__ contribs, const D *__restrict__ dist,
                    const uint16_t *__restrict__ hops, const N *__restrict__ nh, const uint32_t *__restrict__ job_status,
                    hl_route_cell *__restrict__ cells, bool aligned16, uint32_t n_gather,
                    const uint32_t *__restrict__ gather_job, const uint32_t *__restrict__ gather_v,
                    uint64_t *__restrict__ gather_nh) {
-    // a warp owns 32 consecutive cells = one contiguous 768-byte span of the output: the cells are staged in
-    // shared memory and leave as 48 16-byte stores (full sectors) instead of 96 scattered 8-byte ones
-    __shared__ __align__(16) uint64_t stage[8][96];
-    const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const uint64_t total = (uint64_t)n_jobs * P;
-    const uint64_t n_tiles = (total + 31) / 32;
-    const uint64_t wstride = (uint64_t)gridDim.x * 8;
-    for (uint64_t tile = (uint64_t)blockIdx.x * 8 + wib; tile < n_tiles; tile += wstride) {
-        const uint64_t idx = tile * 32 + lane;
-        hl_route_cell c;
-        c.nh_mask = 0; c.lasthop_mask = 0; c.winner = 0xFFFFFFFFu; c.metric = 0; c.flags = 0; c._pad = 0;
-        if (idx < total) {
-            const uint32_t job = (uint32_t)(idx / P), p = (uint32_t)(idx - (uint64_t)job * P);
-            if (!(job_status && job_status[job] != 0)) {      // planes of a refused job are undefined: empty cells
-                const size_t base = (size_t)job * V;
-                const Planes pl{dist + base, hops + base, nh + base};
-                c = hspf::route_cell_eval(pl, contribs, off[p], off[p + 1]);
-            }
-        }
-        const uint64_t w2 = (uint64_t)c.winner | ((uint64_t)c.metric << 32) | ((uint64_t)c.flags << 48);
-        if (aligned16 && tile * 32 + 32 <= total) {
-            uint64_t *s = stage[wib];
-            s[lane * 3 + 0] = c.nh_mask; s[lane * 3 + 1] = c.lasthop_mask; s[lane * 3 + 2] = w2;
-            __syncwarp();
-            const uint4 *s4 = reinterpret_cast<const uint4 *>(s);
-            uint4 *o4 = reinterpret_cast<uint4 *>(cells + tile * 32);
-            o4[lane] = s4[lane];
-            if (lane < 16) o4[32 + lane] = s4[32 + lane];
-            __syncwarp();
-        } else if (idx < total) {
-            uint64_t *o = reinterpret_cast<uint64_t *>(cells + idx);
-            o[0] = c.nh_mask; o[1] = c.lasthop_mask; o[2] = w2;
-        }
-    }
+    const OspfCell<Planes, D, N> cell{off, contribs, dist, hops, nh, job_status, V};
+    hspf::store_route_cells(n_jobs, P, cell, hspf::CellWords{0, 0, 0xFFFFFFFFu}, cells, aligned16);   // empty: winner none
     // the few plane values the host decode needs
     for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_gather; g += (uint64_t)gridDim.x * blockDim.x) {
         const uint32_t job = gather_job[g], v = gather_v[g];
         gather_nh[g] = (job < n_jobs && v < V) ? (uint64_t)nh[(size_t)job * V + v] : 0;
     }
 }
-static_assert(sizeof(hl_route_cell) == 24, "hl_route_cell layout");
 
 template <class Planes, class D, class N>
 int launch_cells(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const D *dist, const uint16_t *hops,
                  const N *nh, const uint32_t *status, hl_route_cell *cells, uint32_t n_gather,
                  const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh) {
-    if (!ctx || !rt || !rt->d_blob || !dist || !hops || !nh || !cells) return HSPF_E_INVAL;
+    if (!ctx || !rt || !rt->dev.blob || !dist || !hops || !nh || !cells) return HSPF_E_INVAL;
     if (n_gather && (!gather_job || !gather_v || !gather_nh)) return HSPF_E_INVAL;
     const uint32_t P = (uint32_t)rt->t.prefix.size();
     const uint64_t total = (uint64_t)n_jobs * P;
     if (total + n_gather == 0) return HSPF_OK;
-    const int dev = hspf_ctx_device(ctx);
-    if (rt->device != dev) return HSPF_E_INVAL;               // the table was uploaded to another device
-    int sms = 0;
-    if (cudaSetDevice(dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-        return HSPF_E_CUDA;
-    // one resident wave (8 blocks of 256 per SM), warp-tile-stride beyond that
-    const uint64_t want = std::max<uint64_t>((total + 255) / 256, 1);
-    const uint32_t blocks = (uint32_t)std::min<uint64_t>(want, (uint64_t)sms * 8);
-    const bool aligned16 = (reinterpret_cast<uintptr_t>(cells) & 15u) == 0;
-    cudaStream_t st = static_cast<cudaStream_t>(hspf_stream(ctx));
-    route_cells_kernel<Planes, D, N><<<blocks, 256, 0, st>>>(n_jobs, P, rt->t.n_vertices, rt->d_off, rt->d_contribs, dist, hops,
-                                                             nh, status, cells, aligned16, n_gather, gather_job, gather_v, gather_nh);
-    if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
-    hspf_note_launches(ctx, 1);
-    return HSPF_OK;
+    return hspf::launch_route_stage(ctx, rt->dev, total, cells, [&](uint32_t blocks, cudaStream_t st, bool aligned16) {
+        route_cells_kernel<Planes, D, N><<<blocks, hspf::kRouteThreads, 0, st>>>(
+            n_jobs, P, rt->t.n_vertices, rt->dev.off, static_cast<const RouteContrib *>(rt->dev.contribs), dist, hops, nh,
+            status, cells, aligned16, n_gather, gather_job, gather_v, gather_nh);
+    });
 }
 
 struct DevBuf {
@@ -107,34 +76,11 @@ struct DevBuf {
 
 }  // namespace
 
-void hspf_rtable_release_device(hspf_ospfv2_rtable *rt) {
-    if (rt && rt->d_blob) {
-        cudaFree(rt->d_blob);
-        rt->d_blob = nullptr; rt->d_off = nullptr; rt->d_contribs = nullptr;
-    }
-}
-
 extern "C" {
 
 int hspf_ospfv2_rtable_upload(hspf_ctx *ctx, hspf_ospfv2_rtable *rt) {
-    if (!ctx || !rt) return HSPF_E_INVAL;
-    hspf_rtable_release_device(rt);
-    if (cudaSetDevice(hspf_ctx_device(ctx)) != cudaSuccess) return HSPF_E_CUDA;
-    const size_t off_bytes = (rt->t.off.size() * sizeof(uint32_t) + 15) & ~(size_t)15;
-    const size_t con_bytes = rt->t.contribs.size() * sizeof(RouteContrib);
-    void *blob = nullptr;
-    if (cudaMalloc(&blob, off_bytes + std::max<size_t>(con_bytes, 16)) != cudaSuccess) return HSPF_E_NOMEM;
-    cudaStream_t st = static_cast<cudaStream_t>(hspf_stream(ctx));
-    cudaError_t e = cudaMemcpyAsync(blob, rt->t.off.data(), rt->t.off.size() * sizeof(uint32_t), cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess && con_bytes)
-        e = cudaMemcpyAsync(static_cast<char *>(blob) + off_bytes, rt->t.contribs.data(), con_bytes, cudaMemcpyHostToDevice, st);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(st);      // the host vectors may go away after the call
-    if (e != cudaSuccess) { cudaFree(blob); return HSPF_E_CUDA; }
-    rt->d_blob = blob;
-    rt->device = hspf_ctx_device(ctx);
-    rt->d_off = static_cast<const uint32_t *>(blob);
-    rt->d_contribs = reinterpret_cast<const RouteContrib *>(static_cast<char *>(blob) + off_bytes);
-    return HSPF_OK;
+    return rt ? hspf::upload_route_table(ctx, rt->dev, rt->t.off, rt->t.contribs.data(), rt->t.contribs.size() * sizeof(RouteContrib))
+              : HSPF_E_INVAL;
 }
 
 int hspf_ospfv2_routes_batch(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result *pl,

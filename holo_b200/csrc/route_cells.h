@@ -12,10 +12,13 @@
 // to interface next hops (needs the root's interface / neighbour state), SR labels per next hop
 // (needs the neighbour's SRGB), max_paths truncation in next-hop order.
 #pragma once
+#include <cstddef>
 #include <cstdint>
 #include <vector>
 
 #include "holo_lsdb.h"
+
+struct hspf_ctx;
 
 #if defined(__CUDACC__)
 #define HSPF_HD __host__ __device__ __forceinline__
@@ -131,22 +134,23 @@ HSPF_HD hl_route_cell route_cell_eval(const Planes &pl, const RouteContrib *cont
     return c;
 }
 
+// Device copy of a route table's `off` and contributor records, one allocation (route_stage.cu).  The
+// functions are defined in the CUDA library only: the CPU test harnesses include this header without linking it.
+struct DeviceRouteTable {
+    void *blob = nullptr;
+    const uint32_t *off = nullptr;
+    const void *contribs = nullptr;
+    int device = -1;
+};
+int upload_route_table(hspf_ctx *ctx, DeviceRouteTable &d, const std::vector<uint32_t> &off, const void *contribs,
+                       size_t contrib_bytes);
+void release_route_table(DeviceRouteTable &d);
+
 }  // namespace hspf
 
 // Host + device image of a flattened area's route table (include/holo_spf_lsdb.h).
 struct hspf_ospfv2_rtable {
     hspf::RouteTable t;
     std::vector<int32_t> ext_of;       // per contributor: index of its Extended-Prefix entry, -1 if none usable
-    // device copies (hspf_ospfv2_rtable_upload)
-    void *d_blob = nullptr;
-    const uint32_t *d_off = nullptr;
-    const hspf::RouteContrib *d_contribs = nullptr;
-    int device = -1;
+    hspf::DeviceRouteTable dev;        // hspf_ospfv2_rtable_upload
 };
-
-// frees the device copy (ospfv2_routes.cu); called by hspf_ospfv2_rtable_free
-void hspf_rtable_release_device(hspf_ospfv2_rtable *rt);
-// counts kernels this translation unit enqueues on the ctx stream (hspf_capi.cu, hspf_launch_count)
-struct hspf_ctx;
-extern "C" void hspf_note_launches(hspf_ctx *ctx, uint32_t n);
-extern "C" int hspf_ctx_device(const hspf_ctx *ctx);     // the CUDA device the ctx and its stream belong to

@@ -8,7 +8,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import capi
+from . import capi, route_table
 from .synth import Topology
 
 REACH_LEGACY, REACH_EXT, REACH_MT = 0, 1, 2
@@ -428,60 +428,26 @@ TOPO_STD, TOPO_MT6 = 0, 1
 NO_ROOT = 0xFFFFFFFF
 
 
-class RouteTable:
+class RouteTable(route_table.RouteTable):
     """hspf_isis_rtable: the instance's prefixes in NetKey order and their contributors (host);
     `upload(ctx)` copies it to the device for hspf_isis_routes_batch.  `n_vertices[t]` / `root[t]` per
     topology (TOPO_STD, TOPO_MT6; root NO_ROOT: the topology has no routes)."""
 
+    api, contrib_dt = "hspf_isis", CONTRIB_DT
+
     def __init__(self, inst: dict):
-        lib = capi.load_library()
-        lib.hspf_isis_rtable_create.argtypes = [C.POINTER(InstanceStruct), C.POINTER(C.c_void_p)]
-        lib.hspf_isis_rtable_free.argtypes = [C.c_void_p]
-        lib.hspf_isis_rtable_free.restype = None
-        lib.hspf_isis_rtable_prefixes.argtypes = [C.c_void_p]
-        lib.hspf_isis_rtable_prefixes.restype = C.c_uint32
-        lib.hspf_isis_rtable_contributors.argtypes = [C.c_void_p]
-        lib.hspf_isis_rtable_contributors.restype = C.c_uint32
-        lib.hspf_isis_rtable_topology.argtypes = [C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32)]
-        lib.hspf_isis_rtable_arrays.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint32)),
-                                                C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_void_p)]
-        lib.hspf_isis_rtable_upload.argtypes = [C.c_void_p, C.c_void_p]
-        self.lib = lib
         s = instance_struct(inst)
-        h = C.c_void_p()
-        rc = lib.hspf_isis_rtable_create(C.byref(s), C.byref(h))
-        if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, "hspf_isis_rtable_create failed")
-        self.handle = h
-        self.n_prefixes = int(lib.hspf_isis_rtable_prefixes(h))
-        self.n_contributors = int(lib.hspf_isis_rtable_contributors(h))
+        super().__init__(capi.load_library().hspf_isis_rtable_create, C.byref(s))
         self.n_vertices, self.root = [], []
         for t in (TOPO_STD, TOPO_MT6):
             nv, r = C.c_uint32(), C.c_uint32()
-            lib.hspf_isis_rtable_topology(h, t, C.byref(nv), C.byref(r))
+            self._call("topology", t, C.byref(nv), C.byref(r))
             self.n_vertices.append(nv.value)
             self.root.append(r.value)
-        pp, pl, po, pc = C.c_void_p(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.c_void_p()
-        lib.hspf_isis_rtable_arrays(h, C.byref(pp), C.byref(pl), C.byref(po), C.byref(pc))
-        P, K = self.n_prefixes, self.n_contributors
-        self.prefix = (np.frombuffer(C.string_at(pp.value, P * IP_DT.itemsize), IP_DT).copy() if P else np.zeros(0, IP_DT))
-        self.len = np.ctypeslib.as_array(pl, shape=(P,)).copy() if P else np.zeros(0, np.uint32)
-        self.off = np.ctypeslib.as_array(po, shape=(P + 1,)).copy()
-        self.contribs = (np.frombuffer(C.string_at(pc.value, K * CONTRIB_DT.itemsize), CONTRIB_DT).copy()
-                         if K else np.zeros(0, CONTRIB_DT))
-
-    def upload(self, ctx: capi.Context):
-        rc = self.lib.hspf_isis_rtable_upload(ctx.handle, self.handle)
-        if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, ctx.last_error())
-
-    def __del__(self):
-        try:
-            if self.handle:
-                self.lib.hspf_isis_rtable_free(self.handle)
-                self.handle = None
-        except Exception:
-            pass
+        pp, pl = C.c_void_p(), C.POINTER(C.c_uint32)()
+        self._call("arrays", C.byref(pp), C.byref(pl), None, None)
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, IP_DT)
+        self.len = route_table.copy_records(pl, self.n_prefixes, np.uint32)
 
 
 def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, rs_mt6, cells_ptr: int):
@@ -491,7 +457,6 @@ def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, 
     lib = ctx.lib
     narrow = isinstance(rs_std if rs_std is not None else rs_mt6, capi.Result16Struct)
     fn = lib.hspf_isis_routes_batch16 if narrow else lib.hspf_isis_routes_batch
-    fn.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
     rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs_std) if rs_std is not None else None,
             C.byref(rs_mt6) if rs_mt6 is not None else None, cells_ptr)
     if rc != capi.HSPF_OK:
@@ -504,8 +469,6 @@ def routes_from_cells(inst: dict, rt: RouteTable, cells: np.ndarray, std=None, m
     overrides.  rc HSPF_E_UNSUPPORTED is returned in the result (caller: routes_from_planes)."""
     lib = capi.load_library()
     u32p, u16p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16)
-    lib.hspf_isis_routes_from_cells.argtypes = [C.POINTER(InstanceStruct), C.c_void_p, C.c_void_p, u32p, u16p, u32p, u16p,
-                                                C.c_uint32, u32p, u32p, C.c_uint32, u32p, u32p, C.POINTER(RibStruct)]
     cells = np.ascontiguousarray(cells, CELL_DT)
     assert cells.shape == (rt.n_prefixes,)
     keep = [cells]

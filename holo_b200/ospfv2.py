@@ -10,7 +10,7 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import capi
+from . import capi, route_table
 from .synth import Topology
 
 LINK_P2P, LINK_TRANSIT, LINK_STUB, LINK_VLINK = 1, 2, 3, 4
@@ -331,51 +331,19 @@ CONTRIB_DT = np.dtype([("vertex", "<u4"), ("origin_id", "<u4"), ("metric", "<u2"
 CELL_PRESENT, CELL_CONNECTED, CELL_MIXED_SID = 1, 2, 4
 
 
-class RouteTable:
+class RouteTable(route_table.RouteTable):
     """hspf_ospfv2_rtable: the area's prefixes in route-table order and their advertisers (host);
     `upload(ctx)` copies it to the device for hspf_ospfv2_routes_batch."""
 
+    api, contrib_dt = "hspf_ospfv2", CONTRIB_DT
+
     def __init__(self, flat: Flat):
-        lib = capi.load_library()
-        lib.hspf_ospfv2_rtable_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-        lib.hspf_ospfv2_rtable_free.argtypes = [C.c_void_p]
-        lib.hspf_ospfv2_rtable_free.restype = None
-        lib.hspf_ospfv2_rtable_prefixes.argtypes = [C.c_void_p]
-        lib.hspf_ospfv2_rtable_prefixes.restype = C.c_uint32
-        lib.hspf_ospfv2_rtable_contributors.argtypes = [C.c_void_p]
-        lib.hspf_ospfv2_rtable_contributors.restype = C.c_uint32
-        lib.hspf_ospfv2_rtable_arrays.argtypes = [C.c_void_p, C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.POINTER(C.c_uint32)),
-                                                  C.POINTER(C.POINTER(C.c_uint32)), C.POINTER(C.c_void_p)]
-        lib.hspf_ospfv2_rtable_upload.argtypes = [C.c_void_p, C.c_void_p]
-        self.lib = lib
         self.flat = flat                      # the table is built from the flat's area image
-        h = C.c_void_p()
-        rc = lib.hspf_ospfv2_rtable_create(flat.handle, C.byref(h))
-        if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, "hspf_ospfv2_rtable_create failed")
-        self.handle = h
-        self.n_prefixes = int(lib.hspf_ospfv2_rtable_prefixes(h))
-        self.n_contributors = int(lib.hspf_ospfv2_rtable_contributors(h))
-        pp, pl, po, pc = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.c_void_p()
-        lib.hspf_ospfv2_rtable_arrays(h, C.byref(pp), C.byref(pl), C.byref(po), C.byref(pc))
-        P, K = self.n_prefixes, self.n_contributors
-        as_np = lambda p, n: np.ctypeslib.as_array(p, shape=(n,)).copy() if n else np.zeros(0, np.uint32)
-        self.prefix, self.plen, self.off = as_np(pp, P), as_np(pl, P), as_np(po, P + 1)
-        self.contribs = (np.frombuffer(C.string_at(pc.value, K * CONTRIB_DT.itemsize), CONTRIB_DT).copy()
-                         if K else np.zeros(0, CONTRIB_DT))
-
-    def upload(self, ctx: capi.Context):
-        rc = self.lib.hspf_ospfv2_rtable_upload(ctx.handle, self.handle)
-        if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, ctx.last_error())
-
-    def __del__(self):
-        try:
-            if self.handle:
-                self.lib.hspf_ospfv2_rtable_free(self.handle)
-                self.handle = None
-        except Exception:
-            pass
+        super().__init__(capi.load_library().hspf_ospfv2_rtable_create, flat.handle)
+        pp, pl = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)()
+        self._call("arrays", C.byref(pp), C.byref(pl), None, None)
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, np.uint32)
+        self.plen = route_table.copy_records(pl, self.n_prefixes, np.uint32)
 
 
 @dataclass
@@ -396,10 +364,6 @@ class BatchRoutes:
 def run_area_batch(ctx: capi.Context, area: Ospfv2Area, root_router_ids, n_prefixes=None) -> BatchRoutes:
     """hspf_ospfv2_run_area_batch: SPT + intra-area route cells of every listed root router, on the device."""
     lib = ctx.lib
-    lib.hspf_ospfv2_run_area_batch.argtypes = [C.c_void_p, C.POINTER(AreaStruct), C.POINTER(C.c_uint32), C.c_uint32,
-                                               C.c_void_p, C.c_uint64, C.POINTER(C.c_uint32), C.POINTER(C.c_uint32),
-                                               C.POINTER(C.c_uint32), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64),
-                                               C.c_uint32, C.POINTER(C.c_double)]
     roots = np.ascontiguousarray(root_router_ids, np.uint32)
     n = len(roots)
     s = area.as_struct()
@@ -437,7 +401,6 @@ def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs, cell
     lib = ctx.lib
     narrow = isinstance(rs, capi.Result16Struct)
     fn = lib.hspf_ospfv2_routes_batch16 if narrow else lib.hspf_ospfv2_routes_batch
-    fn.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]
     rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), cells_ptr, n_gather, gather_job_ptr or None,
             gather_v_ptr or None, gather_nh_ptr or None)
     if rc != capi.HSPF_OK:
@@ -448,8 +411,6 @@ def routes_from_cells(area: Ospfv2Area, rt: RouteTable, cells: np.ndarray, gathe
     """hspf_ospfv2_routes_from_cells (host): one job's cells -> routes and next hops as run_area returns them
     for area.router_id.  rc HSPF_E_UNSUPPORTED is returned in the result (caller: area_from_planes)."""
     lib = capi.load_library()
-    lib.hspf_ospfv2_routes_from_cells.argtypes = [C.POINTER(AreaStruct), C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32),
-                                                  C.POINTER(C.c_uint64), C.c_uint32, C.POINTER(ResultStruct)]
     cells = np.ascontiguousarray(cells, CELL_DT)
     assert cells.shape == (rt.n_prefixes,)
     gv = np.ascontiguousarray(gather_v, np.uint32)

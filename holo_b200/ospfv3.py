@@ -9,8 +9,8 @@ from dataclasses import dataclass, field
 
 import numpy as np
 
-from . import capi
-from .ospfv2 import ROUTE_RTR_DT, IF_P2P, IF_BROADCAST, LINK_P2P, LINK_TRANSIT, MAX_AGE
+from . import capi, route_table
+from .ospfv2 import CONTRIB_DT, ROUTE_RTR_DT, IF_P2P, IF_BROADCAST, LINK_P2P, LINK_TRANSIT, MAX_AGE
 from .synth import Topology
 
 OPT_R, OPT_V6 = 0x01, 0x02
@@ -186,59 +186,25 @@ def area_from_planes(area: Ospfv3Area, spf) -> Ospfv3Result:
     return res
 
 
-class RouteTable:
+class RouteTable(route_table.RouteTable):
     """hspf_ospfv3_rtable_create: the route table of an OSPFv3 area for the batched route stage (the object
     ospfv2.RouteTable wraps; upload and hspf_ospfv2_routes_batch[16] work on it unchanged)."""
 
+    api, contrib_dt = "hspf_ospfv2", CONTRIB_DT
+
     def __init__(self, flat: "Flat"):
-        lib = capi.load_library()
-        lib.hspf_ospfv3_rtable_create.argtypes = [C.c_void_p, C.POINTER(C.c_void_p)]
-        lib.hspf_ospfv2_rtable_free.argtypes = [C.c_void_p]
-        lib.hspf_ospfv2_rtable_free.restype = None
-        lib.hspf_ospfv2_rtable_prefixes.argtypes = [C.c_void_p]
-        lib.hspf_ospfv2_rtable_prefixes.restype = C.c_uint32
-        lib.hspf_ospfv2_rtable_contributors.argtypes = [C.c_void_p]
-        lib.hspf_ospfv2_rtable_contributors.restype = C.c_uint32
-        lib.hspf_ospfv2_rtable_upload.argtypes = [C.c_void_p, C.c_void_p]
-        lib.hspf_ospfv3_rtable_prefixes6.argtypes = [C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.POINTER(C.c_uint32))]
-        self.lib, self.flat = lib, flat
-        h = C.c_void_p()
-        rc = lib.hspf_ospfv3_rtable_create(flat.handle, C.byref(h))
-        if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, "hspf_ospfv3_rtable_create failed")
-        self.handle = h
-        self.n_prefixes = int(lib.hspf_ospfv2_rtable_prefixes(h))
-        self.n_contributors = int(lib.hspf_ospfv2_rtable_contributors(h))
+        self.flat = flat
+        super().__init__(capi.load_library().hspf_ospfv3_rtable_create, flat.handle)
         pp, pl = C.c_void_p(), C.POINTER(C.c_uint32)()
-        lib.hspf_ospfv3_rtable_prefixes6(h, C.byref(pp), C.byref(pl))
-        P = self.n_prefixes
-        self.prefix = np.frombuffer(C.string_at(pp.value, P * IP_DT.itemsize), IP_DT).copy() if P else np.zeros(0, IP_DT)
-        self.plen = np.ctypeslib.as_array(pl, shape=(P,)).copy() if P else np.zeros(0, np.uint32)
-        lib.hspf_ospfv2_rtable_arrays.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.POINTER(C.c_uint32)), C.c_void_p]
-        po = C.POINTER(C.c_uint32)()
-        lib.hspf_ospfv2_rtable_arrays(h, None, None, C.byref(po), None)
-        self.off = np.ctypeslib.as_array(po, shape=(P + 1,)).copy()
-
-    def upload(self, ctx: capi.Context):
-        rc = self.lib.hspf_ospfv2_rtable_upload(ctx.handle, self.handle)
-        if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, ctx.last_error())
-
-    def __del__(self):
-        try:
-            if self.handle:
-                self.lib.hspf_ospfv2_rtable_free(self.handle)
-                self.handle = None
-        except Exception:
-            pass
+        self.lib.hspf_ospfv3_rtable_prefixes6(self.handle, C.byref(pp), C.byref(pl))
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, IP_DT)
+        self.plen = route_table.copy_records(pl, self.n_prefixes, np.uint32)
 
 
 def routes_from_cells(area: Ospfv3Area, rt: RouteTable, cells: np.ndarray, gather_v, gather_nh) -> Ospfv3Result:
     """hspf_ospfv3_routes_from_cells (host): one job's cells -> the routes / next hops of hspf_ospfv3_run_area."""
     from . import ospfv2
     lib = capi.load_library()
-    lib.hspf_ospfv3_routes_from_cells.argtypes = [C.POINTER(AreaStruct), C.c_void_p, C.c_void_p, C.POINTER(C.c_uint32),
-                                                  C.POINTER(C.c_uint64), C.c_uint32, C.POINTER(ResultStruct)]
     cells = np.ascontiguousarray(cells, ospfv2.CELL_DT)
     assert cells.shape == (rt.n_prefixes,)
     gv = np.ascontiguousarray(gather_v, np.uint32)
