@@ -52,6 +52,7 @@ struct hspf_ctx {
     void *stage = nullptr;   size_t stage_bytes = 0;    // device staging of results (host-pointer mode)
     void *h_pin = nullptr;   size_t h_pin_bytes = 0;    // pinned bounce buffer
     void *scratch = nullptr; size_t scratch_bytes = 0;  // planes the caller did not ask for
+    void *route_ws = nullptr; size_t route_ws_bytes = 0; // tile counts / offsets of the route-delta stage
     unsigned long long *d_prof = nullptr; int prof_rows = 0;  // optional phase counters (debug)
     bool prof_enabled = false;
     // progress counters of the pipelined host-pointer call (see run_any)
@@ -583,6 +584,7 @@ void hspf_ctx_destroy(hspf_ctx *ctx) {
     if (ctx->ws) cudaFree(ctx->ws);
     if (ctx->stage) cudaFree(ctx->stage);
     if (ctx->scratch) cudaFree(ctx->scratch);
+    if (ctx->route_ws) cudaFree(ctx->route_ws);
     if (ctx->h_pin) cudaFreeHost(ctx->h_pin);
     delete ctx;
 }
@@ -595,6 +597,10 @@ uint64_t hspf_launch_count(const hspf_ctx *ctx) { return ctx ? ctx->launches : 0
 /* kernels other translation units of the library enqueue on the ctx stream (route_cells.h) */
 void hspf_note_launches(hspf_ctx *ctx, uint32_t n) { if (ctx) ctx->launches += n; }
 int hspf_ctx_device(const hspf_ctx *ctx) { return ctx ? ctx->device : -1; }
+void *hspf_ctx_route_workspace(hspf_ctx *ctx, size_t bytes) {
+    if (!ctx) return nullptr;
+    return grow(ctx, &ctx->route_ws, &ctx->route_ws_bytes, bytes) == HSPF_OK ? ctx->route_ws : nullptr;
+}
 
 int hspf_ctx_set_peer_slots(hspf_ctx *ctx, uint32_t n_peers, const int64_t *deltas) {
     if (!ctx || n_peers > 7 || (n_peers && !deltas)) return HSPF_E_INVAL;

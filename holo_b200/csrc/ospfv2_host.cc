@@ -409,7 +409,9 @@ int hspf_abi_sizes(uint32_t *out, uint32_t cap) {
         (uint32_t)sizeof(hl_isis_lsp_trigger), (uint32_t)sizeof(hl_ip_prefix), (uint32_t)sizeof(hl_lsa_trigger6),
         (uint32_t)sizeof(hl_spf_computation6),
         (uint32_t)sizeof(hl_isis_route_cell),
+        (uint32_t)sizeof(hl_route_delta), (uint32_t)sizeof(hl_route_delta_job),
     };
+    static_assert(sizeof(hl_route_delta) == 16 && sizeof(hl_route_delta_job) == 32, "route delta layout");
     static_assert(sizeof(hl_rib_action) == 12, "hl_rib_action layout");
     const uint32_t n = sizeof(v) / sizeof(v[0]);
     if (!out || cap < n) return (int)n;

@@ -26,6 +26,7 @@ struct OspfCell {
     const uint32_t *off; const RouteContrib *contribs; const D *dist; const uint16_t *hops; const N *nh;
     const uint32_t *status; uint32_t V;
     __device__ __forceinline__ bool refused(uint32_t j) const { return status && status[j] != 0; }
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const { return status ? status[j] : 0; }
     __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
         const size_t base = (size_t)j * V;
         const hl_route_cell c = hspf::route_cell_eval(Planes{dist + base, hops + base, nh + base}, contribs, off[p], off[p + 1]);
@@ -67,6 +68,32 @@ int launch_cells(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, c
     });
 }
 
+// The route-delta stage over the same walk (route_stage.cuh: launch_route_delta), under the bound of route_cells_kernel
+// so that the grid launch_route_stage sizes is resident at once: 32 registers, with a few bytes of spill in pass A.
+template <class Planes, class D, class N>
+int launch_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const D *dist, const uint16_t *hops,
+                 const N *nh, const uint32_t *status, const hl_route_cell *base_cells, uint32_t n_base,
+                 const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                 uint64_t *n_records) {
+    if (!ctx || !rt || !rt->dev.blob || !dist || !hops || !nh) return HSPF_E_INVAL;
+    using Cell = OspfCell<Planes, D, N>;
+    const Cell cell{rt->dev.off, static_cast<const RouteContrib *>(rt->dev.contribs), dist, hops, nh, status, rt->t.n_vertices};
+    hspf::DeltaArgs a{};
+    a.n_jobs = n_jobs; a.P = (uint32_t)rt->t.prefix.size();
+    a.base = reinterpret_cast<const uint64_t *>(base_cells); a.n_base = n_base; a.base_of = base_of;
+    a.job_out = job_out; a.n_records = reinterpret_cast<unsigned long long *>(n_records);
+    a.records = records; a.cap = cap;
+    return hspf::launch_route_delta(ctx, rt->dev, a,
+        [&](uint32_t blocks, cudaStream_t st, const hspf::DeltaArgs &args) {
+            hspf::route_delta_count_kernel<hspf::OspfCellLayout, Cell, hspf::kRouteBlocksPerSM>
+                <<<blocks, hspf::kRouteThreads, 0, st>>>(cell, args);
+        },
+        [&](uint32_t blocks, cudaStream_t st, const hspf::DeltaArgs &args) {
+            hspf::route_delta_store_kernel<hspf::OspfCellLayout, Cell, hspf::kRouteBlocksPerSM>
+                <<<blocks, hspf::kRouteThreads, 0, st>>>(cell, args);
+        });
+}
+
 struct DevBuf {
     void *p = nullptr;
     ~DevBuf() { if (p) cudaFree(p); }
@@ -97,6 +124,22 @@ int hspf_ospfv2_routes_batch16(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint
     if (!pl) return HSPF_E_INVAL;
     return launch_cells<hspf::PlanesNarrow, uint16_t, uint16_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask, pl->job_status,
                                                                 cells, n_gather, gather_job, gather_v, gather_nh);
+}
+
+int hspf_ospfv2_routes_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result *pl,
+                             const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                             hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    if (!pl || pl->nh_words != 1) return HSPF_E_INVAL;
+    return launch_delta<hspf::PlanesWide, uint32_t, uint64_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask, pl->job_status,
+                                                              base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+int hspf_ospfv2_routes_delta16(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
+                               const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                               hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    if (!pl) return HSPF_E_INVAL;
+    return launch_delta<hspf::PlanesNarrow, uint16_t, uint16_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask, pl->job_status,
+                                                                base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
 int hspf_ospfv2_run_area_batch(hspf_ctx *ctx, const hl_ospfv2_area *area, const uint32_t *root_router_ids, uint32_t n_roots,

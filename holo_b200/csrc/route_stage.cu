@@ -1,4 +1,8 @@
-// Device copies of the route tables (route_cells.h: DeviceRouteTable), for both route stages.
+// Device copies of the route tables (route_cells.h: DeviceRouteTable), for both route stages, and the scan of the
+// route-delta stage (route_stage.cuh).
+#include <cub/device/device_scan.cuh>
+#include <cuda/std/functional>
+
 #include "route_stage.cuh"
 
 namespace hspf {
@@ -29,6 +33,19 @@ int upload_route_table(hspf_ctx *ctx, DeviceRouteTable &d, const std::vector<uin
     d.off = static_cast<const uint32_t *>(blob);
     d.contribs = static_cast<char *>(blob) + off_bytes;
     return HSPF_OK;
+}
+
+// u8 tile counts -> u64 offsets: the initial value makes the scan accumulate in 64 bits
+size_t route_delta_scan_bytes(uint64_t n_tiles) {
+    size_t bytes = 0;
+    cub::DeviceScan::ExclusiveScan(nullptr, bytes, static_cast<const uint8_t *>(nullptr), static_cast<uint64_t *>(nullptr),
+                                   cuda::std::plus<>{}, (uint64_t)0, (int64_t)n_tiles);
+    return bytes;
+}
+
+cudaError_t route_delta_scan(void *temp, size_t temp_bytes, const uint8_t *cnt, uint64_t *off, uint64_t n_tiles,
+                             cudaStream_t st) {
+    return cub::DeviceScan::ExclusiveScan(temp, temp_bytes, cnt, off, cuda::std::plus<>{}, (uint64_t)0, (int64_t)n_tiles, st);
 }
 
 }  // namespace hspf

@@ -463,6 +463,23 @@ def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, 
         raise capi.HspfError(rc, ctx.last_error())
 
 
+def routes_delta_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, rs_mt6, base_ptr: int, n_base: int,
+                        base_of_ptr: int, job_out_ptr: int, records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_isis_routes_delta / _delta16 over DEVICE planes (rs_* as for routes_batch_device): each job's cells compared
+    with its base row of base_ptr ([n_base, rt.n_prefixes] cells; base_of_ptr: [n_jobs] u32 rows, 0 for row 0 of
+    every job), without storing them.  job_out_ptr: [n_jobs] route_table.DELTA_JOB_DT; records_ptr: [cap]
+    route_table.DELTA_DT in (job, prefix) order (0 or cap 0: summaries only); n_records_ptr: u64 total.  All device
+    pointers; enqueued on the ctx stream."""
+    lib = ctx.lib
+    narrow = isinstance(rs_std if rs_std is not None else rs_mt6, capi.Result16Struct)
+    fn = lib.hspf_isis_routes_delta16 if narrow else lib.hspf_isis_routes_delta
+    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs_std) if rs_std is not None else None,
+            C.byref(rs_mt6) if rs_mt6 is not None else None, base_ptr or None, n_base, base_of_ptr or None,
+            job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
 def routes_from_cells(inst: dict, rt: RouteTable, cells: np.ndarray, std=None, mt6=None, ov_std=(), ov_mt6=()) -> IsisRib:
     """hspf_isis_routes_from_cells (host): one job's cells -> the table hspf_isis_routes_from_planes gives for the
     same planes.  std / mt6: that job's (dist u32[V], hops u16[V]) per topology; ov_*: its [(edge, cost), ...]

@@ -89,7 +89,8 @@ def abi_sizes_expected():
             [isis.RNL_DT.itemsize, CELL_DT.itemsize, TRIGGER_DT.itemsize, C.sizeof(SpfComputationStruct),
              ospf_rib.RIB_RTR_DT.itemsize, C.sizeof(ospf_rib.RtrTablesStruct),
              isis.LSP_TRIGGER_DT.itemsize, ospfv3.IP_PREFIX_DT.itemsize, ospfv3.TRIGGER6_DT.itemsize,
-             C.sizeof(ospfv3.SpfComputation6Struct), isis.CELL_DT.itemsize])
+             C.sizeof(ospfv3.SpfComputation6Struct), isis.CELL_DT.itemsize,
+             route_table.DELTA_DT.itemsize, route_table.DELTA_JOB_DT.itemsize])
 
 
 def abi_sizes_from_library():
@@ -403,6 +404,22 @@ def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs, cell
     fn = lib.hspf_ospfv2_routes_batch16 if narrow else lib.hspf_ospfv2_routes_batch
     rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), cells_ptr, n_gather, gather_job_ptr or None,
             gather_v_ptr or None, gather_nh_ptr or None)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
+def routes_delta_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs, base_ptr: int, n_base: int, base_of_ptr: int,
+                        job_out_ptr: int, records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_ospfv2_routes_delta / _delta16 over DEVICE planes (rs as for routes_batch_device): each job's cells compared
+    with its base row of base_ptr ([n_base, rt.n_prefixes] cells; base_of_ptr: [n_jobs] u32 rows, 0 for row 0 of
+    every job), without storing them.  job_out_ptr: [n_jobs] route_table.DELTA_JOB_DT; records_ptr: [cap]
+    route_table.DELTA_DT in (job, prefix) order (0 or cap 0: summaries only); n_records_ptr: u64 total.  All device
+    pointers; enqueued on the ctx stream."""
+    lib = ctx.lib
+    narrow = isinstance(rs, capi.Result16Struct)
+    fn = lib.hspf_ospfv2_routes_delta16 if narrow else lib.hspf_ospfv2_routes_delta
+    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), base_ptr or None, n_base, base_of_ptr or None, job_out_ptr or None,
+            records_ptr or None, cap, n_records_ptr or None)
     if rc != capi.HSPF_OK:
         raise capi.HspfError(rc, ctx.last_error())
 

@@ -9,6 +9,13 @@ import numpy as np
 from . import capi
 
 
+# route-delta stage (include/holo_lsdb.h: hl_route_delta, hl_route_delta_job, HL_DELTA_*)
+DELTA_DT = np.dtype([("job", "<u4"), ("prefix", "<u4"), ("metric", "<u4"), ("kind", "u1"), ("_pad", "u1", (3,))])
+DELTA_JOB_DT = np.dtype([("n_changed", "<u4"), ("n_lost", "<u4"), ("n_gained", "<u4"), ("n_metric", "<u4"),
+                         ("n_nexthops", "<u4"), ("n_other", "<u4"), ("status", "<u4"), ("_pad", "<u4")])
+DELTA_LOST, DELTA_GAINED, DELTA_METRIC, DELTA_NEXTHOPS, DELTA_OTHER = 0x01, 0x02, 0x04, 0x08, 0x10
+
+
 def copy_records(ptr, n: int, dt) -> np.ndarray:
     """n records of dtype dt at a native pointer, copied out of the table that owns them."""
     dt = np.dtype(dt)
@@ -81,6 +88,10 @@ def declare(lib: C.CDLL):
         "hspf_isis_rtable_upload": [vp, vp],
         "hspf_isis_routes_batch": [vp, vp, u32, res, res, vp],
         "hspf_isis_routes_batch16": [vp, vp, u32, res16, res16, vp],
+        "hspf_ospfv2_routes_delta": [vp, vp, u32, res, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_routes_delta16": [vp, vp, u32, res16, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_isis_routes_delta": [vp, vp, u32, res, res, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_isis_routes_delta16": [vp, vp, u32, res16, res16, vp, u32, vp, vp, vp, u64, vp],
         "hspf_isis_routes_from_cells": [C.POINTER(isis.InstanceStruct), vp, vp, u32p, u16p, u32p, u16p, u32, u32p, u32p,
                                         u32, u32p, u32p, C.POINTER(isis.RibStruct)],
     }

@@ -855,6 +855,32 @@ typedef struct hl_isis_route_cell {
     uint8_t  _pad[7];
 } hl_isis_route_cell;
 
+/* ------------------------------------------------------------ route deltas -- */
+/* What the route-delta stage (hspf_ospfv2_routes_delta, hspf_isis_routes_delta) reports for one (job, prefix)
+ * whose cell differs from the job's base cell, compared word for word (for a fixed root, atom numbering does not
+ * depend on the job).  B = base cell, J = job cell: */
+#define HL_DELTA_LOST      0x01u   /* B is present, J is not                                                   */
+#define HL_DELTA_GAINED    0x02u   /* J is present, B is not                                                   */
+#define HL_DELTA_METRIC    0x04u   /* both present, the metric differs                                         */
+#define HL_DELTA_NEXTHOPS  0x08u   /* both present, nh_mask differs                                            */
+#define HL_DELTA_OTHER     0x10u   /* both present, winner or flags differ (OSPF: or lasthop_mask); a new
+                                      winner can mean a new origin, route type or SR label                     */
+typedef struct hl_route_delta {
+    uint32_t job;
+    uint32_t prefix;        /* index in the route table                                                   */
+    uint32_t metric;        /* J's metric; B's when kind is HL_DELTA_LOST                                  */
+    uint8_t  kind;          /* HL_DELTA_* (never 0)                                                        */
+    uint8_t  _pad[3];
+} hl_route_delta;
+
+typedef struct hl_route_delta_job {
+    uint32_t n_changed;     /* prefixes with any HL_DELTA_* bit                                           */
+    uint32_t n_lost, n_gained, n_metric, n_nexthops, n_other;   /* prefixes carrying that bit            */
+    uint32_t status;        /* the job's status word (IS-IS: both topologies'), HSPF_JS_INVALID for a base
+                               row out of range; non-zero: not compared, counts 0, no records             */
+    uint32_t _pad;
+} hl_route_delta_job;
+
 #ifdef __cplusplus
 }
 #endif

@@ -366,6 +366,49 @@ int hspf_isis_routes_from_cells(const hl_isis_instance *inst, const hspf_isis_rt
                                 uint32_t n_ov_mt6, const uint32_t *ov_edge_mt6, const uint32_t *ov_cost_mt6,
                                 hl_isis_rib *out);
 
+/*
+ * Route-delta stage on the device: which prefixes each job of a what-if batch loses, gains, or reaches at another
+ * metric or over another next-hop set, against a base route table — without storing the n_jobs x P cell matrix.
+ * Per (job, prefix) it runs the same walk as hspf_*_routes_batch[16] and compares the cell with the job's base cell
+ * word for word (for a fixed root, atom a is always the same first hop, whatever the job's overrides).  Enqueued on
+ * the ctx stream behind the SPT batches; no synchronisation.
+ *
+ *   hspf_ospfv2_routes_delta[16]  OSPFv2 and OSPFv3 tables (as hspf_ospfv2_routes_batch[16]).
+ *   hspf_isis_routes_delta[16]    IS-IS tables (as hspf_isis_routes_batch[16]).
+ *
+ *   base_cells  DEVICE [n_base][P] cells, 8-byte aligned: typically written by hspf_*_routes_batch[16] for the
+ *               unperturbed job of each root.  n_base == 0 is HSPF_E_INVAL.
+ *   base_of     DEVICE [n_jobs] base row of each job, or NULL: every job uses row 0.
+ *   job_out     DEVICE [n_jobs] hl_route_delta_job (required).  status: the job's status word (IS-IS: both
+ *               topologies' OR-ed), or HSPF_JS_INVALID when base_of[j] >= n_base.  A job with a non-zero status
+ *               is not compared: counts 0, no records.
+ *   records     DEVICE hl_route_delta[cap], ordered by (job, prefix), identical from run to run.  Only the first
+ *               min(total, cap) are written.  records NULL or cap 0: the summaries only.
+ *   n_records   DEVICE uint64_t (required): the total number of changed (job, prefix), whatever cap is.
+ *
+ * Kinds (include/holo_lsdb.h, HL_DELTA_*), with B the base cell and J the job cell: LOST (B present, J not),
+ * GAINED (J present, B not); both present: METRIC, NEXTHOPS (nh_mask), OTHER (winner or flags; OSPF: also
+ * lasthop_mask) in any combination; neither present: no change.  What is not promised: an unchanged cell does not
+ * guarantee unchanged next-hop addresses.  IS-IS addresses come from a replay of the first hops that depends on
+ * the order in which the root's neighbours leave the heap; OSPF addresses also read the atom sets of the transit
+ * networks attached to the root.  A caller who needs addresses decodes the reported jobs
+ * (hspf_*_routes_from_cells).
+ */
+int hspf_ospfv2_routes_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result *planes,
+                             const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                             hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_ospfv2_routes_delta16(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result16 *planes,
+                               const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                               hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_isis_routes_delta(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result *std_planes,
+                           const hspf_result *mt6_planes, const hl_isis_route_cell *base_cells, uint32_t n_base,
+                           const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                           uint64_t *n_records);
+int hspf_isis_routes_delta16(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result16 *std_planes,
+                             const hspf_result16 *mt6_planes, const hl_isis_route_cell *base_cells, uint32_t n_base,
+                             const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                             uint64_t *n_records);
+
 /* sizeof() of the ABI structs in declaration order (hspf_csr, hspf_jobs,
  * hspf_result, then every struct of holo_lsdb.h); returns the count.  Lets a
  * foreign binding verify its struct layouts at load time. */
