@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "holo_spf_lsdb.h"
+#include "ospf_rib_cells.h"
 #include "route_cells.h"
 
 namespace {
@@ -410,9 +411,11 @@ int hspf_abi_sizes(uint32_t *out, uint32_t cap) {
         (uint32_t)sizeof(hl_spf_computation6),
         (uint32_t)sizeof(hl_isis_route_cell),
         (uint32_t)sizeof(hl_route_delta), (uint32_t)sizeof(hl_route_delta_job),
+        (uint32_t)sizeof(hl_ospf_rib_cell),
     };
     static_assert(sizeof(hl_route_delta) == 16 && sizeof(hl_route_delta_job) == 32, "route delta layout");
     static_assert(sizeof(hl_rib_action) == 12, "hl_rib_action layout");
+    static_assert(sizeof(hl_ospf_rib_cell) == 24, "hl_ospf_rib_cell layout");
     const uint32_t n = sizeof(v) / sizeof(v[0]);
     if (!out || cap < n) return (int)n;
     for (uint32_t i = 0; i < n; ++i) out[i] = v[i];
@@ -868,6 +871,153 @@ int hspf_ospfv2_rtable_arrays(const hspf_ospfv2_rtable *rt, const uint32_t **pre
     return HSPF_OK;
 }
 
+}  // extern "C" (reopened below)
+
+namespace {
+
+// One job's decode state: the flattened area, its root, and atoms -> next hops (Resolver) over the nh_mask of the
+// transit networks next to the root, the only plane values Resolver::resolve looks up.
+struct JobDecode {
+    hspf_ospfv2_flat f;
+    uint32_t root = kNone;
+    std::vector<uint64_t> sparse_nh;
+    std::unique_ptr<Resolver> rs;
+    // HSPF_OK with root == kNone when area->router_id is not a router of the area
+    int init(const hl_ospfv2_area *a, uint32_t n_vertices, const uint32_t *gather_v, const uint64_t *gather_nh,
+             uint32_t n_gather) {
+        int rc = flatten(a, f);
+        if (rc) return rc;
+        const uint32_t V = (uint32_t)f.ids.size();
+        if (V != n_vertices) return HSPF_E_INVAL;                      // not the LSDB the table was built from
+        auto rit = f.rtr_vertex.find(a->router_id);
+        if (rit == f.rtr_vertex.end()) return HSPF_OK;
+        root = rit->second;
+        sparse_nh.assign(V, 0);
+        for (uint32_t i = 0; i < n_gather; ++i) {
+            if (gather_v[i] >= V) return HSPF_E_INVAL;
+            sparse_nh[gather_v[i]] = gather_nh[i];
+        }
+        rs.reset(new Resolver{f, a, root, sparse_nh.data(), 1, {}, {}, {}});
+        rs->atom_nh.resize(64);
+        rs->atom_done.assign(64, 0);
+        for (uint32_t i = 0; i < a->n_ifaces; ++i)
+            if (a->ifaces[i].n_nbrs > 0) rs->ifaces_with_nbrs.push_back((int)i);
+        return HSPF_OK;
+    }
+};
+
+// Intra-area routes of one job's cells (hspf_ospfv2_routes_from_cells after its checks).
+int intra_from_cells(JobDecode &jd, const hl_ospfv2_area *a, const hspf_ospfv2_rtable *rt, const hl_route_cell *cells,
+                     hl_ospfv2_result *out) {
+    Resolver &rs = *jd.rs;
+    // SRGBs per router (area_router_information, ospfv2/spf.rs:617-654)
+    std::unordered_map<uint32_t, RouterInfo> ri_cache;
+    const RouterInfo no_ri;
+    if (a->sr_enabled) {
+        for (uint32_t i = 0; i < a->n_ri_lsas; ++i) {
+            const auto &l = a->ri_lsas[i];
+            if (l.age == HL_LSA_MAX_AGE) continue;
+            RouterInfo &ri = ri_cache[l.adv_rtr];
+            if (l.has_sr_algo) ri.has_sr_algo = true;
+            for (uint32_t k = 0; k < l.n_srgb; ++k) ri.srgb.push_back(&a->srgbs[l.srgb_off + k]);
+        }
+    }
+    auto cached_ri = [&](uint32_t rid) -> const RouterInfo & {
+        auto it = ri_cache.find(rid);
+        return it == ri_cache.end() ? no_ri : it->second;
+    };
+    const RouterInfo &local_ri = cached_ri(a->router_id);
+
+    const auto &t = rt->t;
+    const uint32_t P = (uint32_t)t.prefix.size();
+    uint32_t n_routes = 0, n_nh = 0;
+    std::vector<Nh> set;
+    for (uint32_t p = 0; p < P; ++p) {
+        const hl_route_cell &c = cells[p];
+        if (!(c.flags & HL_CELL_PRESENT)) continue;
+        if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
+        if (c.winner < t.off[p] || c.winner >= t.off[p + 1]) return HSPF_E_INVAL;
+        const hspf::RouteContrib &w = t.contribs[c.winner];
+        const hl_ospfv2_ext_prefix *ep = nullptr;
+        if (w.sid_class) {
+            const int32_t e = rt->ext_of[c.winner];
+            if (e < 0 || (uint32_t)e >= a->n_ext_prefixes) return HSPF_E_INVAL;
+            ep = &a->ext_prefixes[e];
+        }
+        const bool local = (c.flags & HL_CELL_CONNECTED) != 0;
+        hl_route_net o{};
+        o.prefix = t.prefix[p]; o.mask = t.plen[p] == 0 ? 0 : 0xFFFFFFFFu << (32 - t.plen[p]);
+        o.metric = c.metric; o.flags = local ? HL_ROUTE_CONNECTED : 0; o.origin_type = t.origin_type[c.winner];
+        o.origin_adv_rtr = t.origin_adv[c.winner]; o.origin_lsa_id = w.origin_id;
+        if (ep) {
+            o.has_prefix_sid = 1; o.prefix_sid_value = ep->sid_value; o.prefix_sid_flags = ep->sid_flags;
+            o.prefix_sid_is_label = ep->sid_is_label;
+            if (!(local && (!(ep->sid_flags & HL_PSID_NP) || (ep->sid_flags & HL_PSID_E)))) {
+                if (!ep->sid_is_label) {
+                    uint32_t lab;
+                    if (!local_ri.srgb.empty() && index_to_label(ep->sid_value, local_ri.srgb, &lab)) { o.has_sr_label = 1; o.sr_label = lab; }
+                } else {
+                    o.has_sr_label = 1; o.sr_label = ep->sid_value;
+                }
+            }
+        }
+        set.clear();
+        uint64_t m = c.nh_mask;
+        while (m) {
+            const uint32_t atom = (uint32_t)__builtin_ctzll(m);
+            m &= m - 1;
+            const bool last_hop = (c.lasthop_mask >> atom) & 1u;
+            for (Nh x : rs.resolve(atom)) {
+                if (ep && x.has_nbr) {
+                    uint32_t lab = 0; bool ok = false, decided = false;
+                    if (last_hop) {
+                        if (!(ep->sid_flags & HL_PSID_NP)) { lab = 3; ok = decided = true; }
+                        else if (ep->sid_flags & HL_PSID_E) { lab = 0; ok = decided = true; }
+                    }
+                    if (!decided) {
+                        if (!ep->sid_is_label) {
+                            const RouterInfo &nri = cached_ri(x.nbr);
+                            if (!nri.srgb.empty()) ok = index_to_label(ep->sid_value, nri.srgb, &lab);
+                        } else {
+                            lab = last_hop ? ep->sid_value : 3u; ok = true;
+                        }
+                    }
+                    if (ok) { x.has_label = 1; x.label = lab; }
+                }
+                auto it = std::lower_bound(set.begin(), set.end(), x, nh_less);
+                if (it != set.end() && nh_same_key(*it, x)) {
+                    // two atoms, one next hop: the reference keeps whichever advertiser came last; the
+                    // cell cannot tell unless both agree
+                    if (it->iface != x.iface || it->nbr != x.nbr || it->has_nbr != x.has_nbr ||
+                        it->has_label != x.has_label || it->label != x.label) return HSPF_E_UNSUPPORTED;
+                } else {
+                    set.insert(it, x);
+                }
+            }
+        }
+        if (set.size() > a->max_paths) set.resize(a->max_paths);
+        o.nh_off = n_nh; o.n_nh = (uint32_t)set.size();
+        if (n_routes < out->routes_cap && n_nh + set.size() <= out->nexthops_cap) {
+            out->routes[n_routes] = o;
+            for (const Nh &x : set) {
+                hl_nexthop h{};
+                h.iface = x.iface; h.addr = x.has_addr ? x.addr : 0; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
+                h.sr_label = x.has_label ? x.label : 0;
+                h.has_addr = x.has_addr; h.has_nbr = x.has_nbr; h.has_label = x.has_label;
+                out->nexthops[n_nh + (&x - set.data())] = h;
+            }
+        }
+        ++n_routes; n_nh += (uint32_t)set.size();
+    }
+    out->n_routes = n_routes; out->n_nexthops = n_nh;
+    if (n_routes > out->routes_cap || n_nh > out->nexthops_cap) return HSPF_E_NOMEM;
+    return HSPF_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
 int hspf_ospfv2_routes_from_cells(const hl_ospfv2_area *a, const hspf_ospfv2_rtable *rt, const hl_route_cell *cells,
                                   const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather,
                                   hl_ospfv2_result *out) {
@@ -876,127 +1026,257 @@ int hspf_ospfv2_routes_from_cells(const hl_ospfv2_area *a, const hspf_ospfv2_rta
         out->n_vertices = out->n_routers = out->n_routes = out->n_nexthops = 0;
         out->transit_capability = 0;
         out->root_found = 0;
-        hspf_ospfv2_flat f;
-        int rc = flatten(a, f);
-        if (rc) return rc;
-        const uint32_t V = (uint32_t)f.ids.size();
-        if (V != rt->t.n_vertices) return HSPF_E_INVAL;          // not the LSDB the table was built from
-        auto rit = f.rtr_vertex.find(a->router_id);
-        if (rit == f.rtr_vertex.end()) return HSPF_OK;
+        JobDecode jd;
+        const int rc = jd.init(a, rt->t.n_vertices, gather_v, gather_nh, n_gather);
+        if (rc || jd.root == kNone) return rc;
         out->root_found = 1;
-        const uint32_t root = rit->second;
-        // atoms -> next hops: only the transit networks next to the root are ever looked up (Resolver::resolve)
-        std::vector<uint64_t> sparse_nh(V, 0);
-        for (uint32_t i = 0; i < n_gather; ++i) {
-            if (gather_v[i] >= V) return HSPF_E_INVAL;
-            sparse_nh[gather_v[i]] = gather_nh[i];
-        }
-        Resolver rs{f, a, root, sparse_nh.data(), 1, {}, {}, {}};
-        rs.atom_nh.resize(64);
-        rs.atom_done.assign(64, 0);
-        for (uint32_t i = 0; i < a->n_ifaces; ++i)
-            if (a->ifaces[i].n_nbrs > 0) rs.ifaces_with_nbrs.push_back((int)i);
-        // SRGBs per router (area_router_information, ospfv2/spf.rs:617-654)
-        std::unordered_map<uint32_t, RouterInfo> ri_cache;
-        const RouterInfo no_ri;
-        if (a->sr_enabled) {
-            for (uint32_t i = 0; i < a->n_ri_lsas; ++i) {
-                const auto &l = a->ri_lsas[i];
-                if (l.age == HL_LSA_MAX_AGE) continue;
-                RouterInfo &ri = ri_cache[l.adv_rtr];
-                if (l.has_sr_algo) ri.has_sr_algo = true;
-                for (uint32_t k = 0; k < l.n_srgb; ++k) ri.srgb.push_back(&a->srgbs[l.srgb_off + k]);
-            }
-        }
-        auto cached_ri = [&](uint32_t rid) -> const RouterInfo & {
-            auto it = ri_cache.find(rid);
-            return it == ri_cache.end() ? no_ri : it->second;
-        };
-        const RouterInfo &local_ri = cached_ri(a->router_id);
+        return intra_from_cells(jd, a, rt, cells, out);
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
+}
 
-        const auto &t = rt->t;
-        const uint32_t P = (uint32_t)t.prefix.size();
-        uint32_t n_routes = 0, n_nh = 0;
+
+/* ---- batched routing-table stage for roots attached to one area (ospf_rib_cells.h) ----------------- */
+
+void hspf_ospfv2_ribtable_free(hspf_ospfv2_ribtable *rt) {
+    if (!rt) return;
+    hspf::release_route_table(rt->dev);
+    hspf_ospfv2_rtable_free(rt->intra);
+    delete rt;
+}
+
+int hspf_ospfv2_ribtable_create(const hspf_ospfv2_flat *flat, uint32_t area_id, const hl_ospfv2_summary_lsa *sums,
+                                uint32_t n_sums, const hl_ospfv2_external_lsa *ext, uint32_t n_ext,
+                                hspf_ospfv2_ribtable **out) {
+    if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext)) return HSPF_E_INVAL;
+    *out = nullptr;
+    // the largest metric a cell holds: a type-1 external behind a type-4 entry, over a distance below saturation
+    static_assert(0xFFFEull + 2ull * (HL_LSA_INFINITY - 1) <= HL_RIB_CELL_METRIC_MAX, "cell metric field");
+    try {
+        using hspf::RibRec;
+        const hspf_ospfv2_flat &f = *flat;
+        const hl_ospfv2_area *a = f.area;
+        const uint32_t V = (uint32_t)f.ids.size();
+        std::unique_ptr<hspf_ospfv2_ribtable, void (*)(hspf_ospfv2_ribtable *)> rt(new hspf_ospfv2_ribtable(),
+                                                                                   hspf_ospfv2_ribtable_free);
+        rt->area_id = area_id;
+        rt->vflags.assign(V, 0);
+        for (uint32_t v = 0; v < V; ++v)
+            if (f.is_router[v]) rt->vflags[v] = a->router_lsas[f.lsa_of[v]].flags;
+        // rib_full step 3 (transit areas) can rewrite the backbone's intra-area routes when it has virtual links
+        if (area_id == 0)
+            for (uint32_t v = 0; v < V; ++v)
+                if (rt->vflags[v] & HL_RTR_FLAG_V) return HSPF_E_UNSUPPORTED;
+        auto router_vertex = [&](uint32_t id) {
+            auto it = f.rtr_vertex.find(id);
+            return it == f.rtr_vertex.end() ? kNone : it->second;
+        };
+        auto has_flag = [&](uint32_t v, uint8_t flag) { return v != kNone && (rt->vflags[v] & flag) != 0; };
+        auto live = [](uint8_t maxage, uint32_t metric) { return !maxage && metric < HL_LSA_INFINITY; };
+        int rc = hspf_ospfv2_rtable_create(flat, &rt->intra);
+        if (rc) return rc;
+        const hspf::RouteTable &it = rt->intra->t;
+
+        struct Keyed { uint64_t key; RibRec r; uint32_t tag; };
+        std::vector<Keyed> t3, t5;
+        std::unordered_map<uint32_t, uint32_t> slot_of;        // ASBR router id -> slot
+        std::vector<uint32_t> slot_id;
+        std::vector<std::vector<RibRec>> t4;                    // per slot, LSDB order
+        auto slot = [&](uint32_t id) {
+            auto ins = slot_of.emplace(id, (uint32_t)slot_id.size());
+            if (ins.second) { slot_id.push_back(id); t4.emplace_back(); }
+            return ins.first->second;
+        };
+        for (uint32_t i = 0; i < n_sums; ++i) {
+            const auto &l = sums[i];
+            if (!live(l.maxage, l.metric)) continue;
+            const uint32_t abr = router_vertex(l.adv_rtr);
+            if (!has_flag(abr, HL_RTR_FLAG_B)) continue;                 // abr(): a router entry with the B flag
+            if (l.lsa_type == 3) {
+                t3.push_back({pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)), RibRec{abr, l.metric, 0, 0}, 0});
+            } else if (l.lsa_type == 4) {
+                // the entry a type-4 LSA writes replaces the named router's: were that an ABR, later type-4 LSAs
+                // would see abr() change under them
+                if (has_flag(router_vertex(l.lsa_id), HL_RTR_FLAG_B)) return HSPF_E_UNSUPPORTED;
+                t4[slot(l.lsa_id)].push_back(RibRec{abr, l.metric, 0, 0});
+            }
+        }
+        for (uint32_t i = 0; i < n_ext; ++i) {
+            const auto &l = ext[i];
+            if (!live(l.maxage, l.metric)) continue;
+            t5.push_back({pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)), RibRec{slot(l.adv_rtr), l.metric,
+                          l.e_bit ? 1u : 0u, 0}, l.tag});
+        }
+        auto by_key = [](const Keyed &x, const Keyed &y) { return x.key < y.key; };
+        std::stable_sort(t3.begin(), t3.end(), by_key);        // LSDB order within a prefix
+        std::stable_sort(t5.begin(), t5.end(), by_key);
+        std::vector<uint64_t> keys;
+        keys.reserve(it.prefix.size() + t3.size() + t5.size());
+        for (size_t k = 0; k < it.prefix.size(); ++k) keys.push_back(pkey(it.prefix[k], it.plen[k]));
+        for (const Keyed &x : t3) keys.push_back(x.key);
+        for (const Keyed &x : t5) keys.push_back(x.key);
+        std::sort(keys.begin(), keys.end());
+        keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+        const uint32_t P = (uint32_t)keys.size(), PI = (uint32_t)it.prefix.size();
+        rt->n_intra = (uint32_t)it.contribs.size();
+        const uint64_t n_slots = slot_id.size(), slot_base = (uint64_t)rt->n_intra + t3.size() + t5.size();
+        uint64_t n_t4 = 0;
+        for (const auto &l : t4) n_t4 += l.size();
+        if (slot_base + n_slots + n_t4 >= kNone) return HSPF_E_UNSUPPORTED;      // record indices are u32
+        rt->recs.resize(rt->n_intra);
+        if (rt->n_intra) std::memcpy(rt->recs.data(), it.contribs.data(), rt->n_intra * sizeof(RibRec));
+        rt->prefix.resize(P); rt->plen.resize(P); rt->intra_of.assign(P, kNone);
+        rt->off.assign(3 * ((size_t)P + 1), 0);
+        uint32_t *oi = rt->off.data(), *o3 = oi + P + 1, *o5 = o3 + P + 1;
+        uint32_t k = 0;
+        for (uint32_t u = 0; u < P; ++u) {
+            rt->prefix[u] = (uint32_t)(keys[u] >> 8); rt->plen[u] = (uint32_t)(keys[u] & 0xFF);
+            oi[u] = it.off[k];                                  // an empty range where the prefix has no intra record
+            if (k < PI && pkey(it.prefix[k], it.plen[k]) == keys[u]) rt->intra_of[u] = k++;
+        }
+        oi[P] = rt->n_intra;
+        size_t q = 0;
+        for (uint32_t u = 0; u < P; ++u) {
+            o3[u] = (uint32_t)rt->recs.size();
+            for (; q < t3.size() && t3[q].key == keys[u]; ++q) rt->recs.push_back(t3[q].r);
+        }
+        o3[P] = (uint32_t)rt->recs.size();
+        rt->ext_base = o3[P];
+        q = 0;
+        for (uint32_t u = 0; u < P; ++u) {
+            o5[u] = (uint32_t)rt->recs.size();
+            for (; q < t5.size() && t5[q].key == keys[u]; ++q) {
+                RibRec r = t5[q].r;
+                r.x += (uint32_t)slot_base;
+                rt->recs.push_back(r);
+                rt->ext_tag.push_back(t5[q].tag);
+            }
+        }
+        o5[P] = (uint32_t)rt->recs.size();
+        rt->ext_end = o5[P];
+        uint32_t t4_at = (uint32_t)(slot_base + n_slots);
+        for (uint32_t s = 0; s < n_slots; ++s) {
+            const uint32_t v = router_vertex(slot_id[s]);
+            rt->recs.push_back(RibRec{v, has_flag(v, HL_RTR_FLAG_E) ? 1u : 0u, t4_at, t4_at + (uint32_t)t4[s].size()});
+            t4_at += (uint32_t)t4[s].size();
+        }
+        for (const auto &l : t4) rt->recs.insert(rt->recs.end(), l.begin(), l.end());
+        *out = rt.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_UNSUPPORTED;
+    }
+}
+
+uint32_t hspf_ospfv2_ribtable_prefixes(const hspf_ospfv2_ribtable *rt) { return rt ? (uint32_t)rt->prefix.size() : 0; }
+uint32_t hspf_ospfv2_ribtable_contributors(const hspf_ospfv2_ribtable *rt) { return rt ? (uint32_t)rt->recs.size() : 0; }
+
+int hspf_ospfv2_ribtable_arrays(const hspf_ospfv2_ribtable *rt, const uint32_t **prefix, const uint32_t **plen,
+                                const uint32_t **off, const void **records) {
+    if (!rt) return HSPF_E_INVAL;
+    if (prefix) *prefix = rt->prefix.data();
+    if (plen) *plen = rt->plen.data();
+    if (off) *off = rt->off.data();
+    if (records) *records = rt->recs.data();
+    return HSPF_OK;
+}
+
+int hspf_ospfv2_rib_from_cells(const hl_ospfv2_area *a, const hspf_ospfv2_ribtable *rt, const hl_ospf_rib_cell *cells,
+                               const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv2_rib *out) {
+    if (!a || !rt || !rt->intra || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
+    try {
+        out->n_routes = out->n_nexthops = 0;
+        JobDecode jd;
+        int rc = jd.init(a, (uint32_t)rt->vflags.size(), gather_v, gather_nh, n_gather);
+        if (rc) return rc;
+        if (jd.root == kNone) return HSPF_E_INVAL;                  // not the root of any job over this table
+        const uint32_t P = (uint32_t)rt->prefix.size(), PI = (uint32_t)rt->intra->t.prefix.size();
+        const uint32_t *o3 = rt->off.data() + P + 1, *o5 = o3 + P + 1;
+        // 1. the intra-area cells, through the intra-area decode
+        std::vector<hl_route_cell> ic(PI, hl_route_cell{0, 0, kNone, 0, 0, 0});
+        for (uint32_t u = 0; u < P; ++u) {
+            const hl_ospf_rib_cell &c = cells[u];
+            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(c) != HL_PATH_INTRA_AREA) continue;
+            if (rt->intra_of[u] == kNone || HL_RIB_CELL_METRIC(c) > 0xFFFFu) return HSPF_E_INVAL;
+            ic[rt->intra_of[u]] = hl_route_cell{c.nh_mask, c.aux, c.winner, (uint16_t)HL_RIB_CELL_METRIC(c),
+                                                (uint8_t)HL_RIB_CELL_FLAGS(c), 0};
+        }
+        std::vector<hl_route_net> nets(PI);
+        std::vector<hl_nexthop> nh(std::max<size_t>(64, (size_t)PI * 2));
+        hl_ospfv2_result res{};
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            res = hl_ospfv2_result{};
+            res.routes_cap = PI; res.routes = nets.data();
+            res.nexthops_cap = (uint32_t)nh.size(); res.nexthops = nh.data();
+            rc = intra_from_cells(jd, a, rt->intra, ic.data(), &res);
+            if (rc != HSPF_E_NOMEM) break;
+            nh.resize(res.n_nexthops);
+        }
+        if (rc) return rc;
+        // 2. every route in prefix order; inter-area and external next hops from the cell's atoms
+        std::vector<hl_rib_route> routes;
+        std::vector<hl_nexthop> hops;
         std::vector<Nh> set;
-        for (uint32_t p = 0; p < P; ++p) {
-            const hl_route_cell &c = cells[p];
-            if (!(c.flags & HL_CELL_PRESENT)) continue;
-            if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
-            if (c.winner < t.off[p] || c.winner >= t.off[p + 1]) return HSPF_E_INVAL;
-            const hspf::RouteContrib &w = t.contribs[c.winner];
-            const hl_ospfv2_ext_prefix *ep = nullptr;
-            if (w.sid_class) {
-                const int32_t e = rt->ext_of[c.winner];
-                if (e < 0 || (uint32_t)e >= a->n_ext_prefixes) return HSPF_E_INVAL;
-                ep = &a->ext_prefixes[e];
-            }
-            const bool local = (c.flags & HL_CELL_CONNECTED) != 0;
-            hl_route_net o{};
-            o.prefix = t.prefix[p]; o.mask = t.plen[p] == 0 ? 0 : 0xFFFFFFFFu << (32 - t.plen[p]);
-            o.metric = c.metric; o.flags = local ? HL_ROUTE_CONNECTED : 0; o.origin_type = t.origin_type[c.winner];
-            o.origin_adv_rtr = t.origin_adv[c.winner]; o.origin_lsa_id = w.origin_id;
-            if (ep) {
-                o.has_prefix_sid = 1; o.prefix_sid_value = ep->sid_value; o.prefix_sid_flags = ep->sid_flags;
-                o.prefix_sid_is_label = ep->sid_is_label;
-                if (!(local && (!(ep->sid_flags & HL_PSID_NP) || (ep->sid_flags & HL_PSID_E)))) {
-                    if (!ep->sid_is_label) {
-                        uint32_t lab;
-                        if (!local_ri.srgb.empty() && index_to_label(ep->sid_value, local_ri.srgb, &lab)) { o.has_sr_label = 1; o.sr_label = lab; }
-                    } else {
-                        o.has_sr_label = 1; o.sr_label = ep->sid_value;
+        auto sort_key = [&](uint32_t iface) { return iface < a->n_ifaces ? a->ifaces[iface].sort_key : 0xFFFFFFFFu; };
+        uint32_t ri = 0;
+        for (uint32_t u = 0; u < P; ++u) {
+            const hl_ospf_rib_cell &c = cells[u];
+            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT)) continue;
+            const uint32_t path = HL_RIB_CELL_PATH(c);
+            hl_rib_route o;
+            std::memset(&o, 0, sizeof(o));
+            o.prefix = rt->prefix[u]; o.mask = rt->plen[u] == 0 ? 0 : 0xFFFFFFFFu << (32 - rt->plen[u]);
+            o.path_type = (uint8_t)path;
+            o.nh_off = (uint32_t)hops.size();
+            if (path == HL_PATH_INTRA_AREA) {
+                if (ri >= res.n_routes) return HSPF_E_INVAL;
+                const hl_route_net &r = nets[ri++];
+                o.metric = r.metric; o.area_id = rt->area_id; o.has_area = 1; o.flags = r.flags;
+                o.has_sr_label = r.has_sr_label; o.sr_label = r.has_sr_label ? r.sr_label : 0;
+                for (uint32_t k = 0; k < r.n_nh; ++k) {
+                    hl_nexthop h = nh[r.nh_off + k];
+                    h.iface = sort_key(h.iface);                      // the merged table names interfaces by sort key
+                    hops.push_back(h);
+                }
+            } else {
+                const bool inter = path == HL_PATH_INTER_AREA;
+                if (inter ? (c.winner < o3[u] || c.winner >= o3[u + 1]) : (c.winner < o5[u] || c.winner >= o5[u + 1]))
+                    return HSPF_E_INVAL;
+                o.metric = HL_RIB_CELL_METRIC(c);
+                if (inter) { o.area_id = rt->area_id; o.has_area = 1; }
+                else o.tag = rt->ext_tag[c.winner - rt->ext_base];
+                if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
+                set.clear();
+                for (uint64_t m = c.nh_mask; m; m &= m - 1) {
+                    for (const Nh &x : jd.rs->resolve((uint32_t)__builtin_ctzll(m))) {
+                        auto at = std::lower_bound(set.begin(), set.end(), x, nh_less);
+                        if (at == set.end() || !nh_same_key(*at, x)) { set.insert(at, x); continue; }
+                        // two atoms, one next hop: which router's entry gave it depends on the merge order
+                        if (at->iface != x.iface || at->nbr != x.nbr || at->has_nbr != x.has_nbr) return HSPF_E_UNSUPPORTED;
                     }
                 }
-            }
-            set.clear();
-            uint64_t m = c.nh_mask;
-            while (m) {
-                const uint32_t atom = (uint32_t)__builtin_ctzll(m);
-                m &= m - 1;
-                const bool last_hop = (c.lasthop_mask >> atom) & 1u;
-                for (Nh x : rs.resolve(atom)) {
-                    if (ep && x.has_nbr) {
-                        uint32_t lab = 0; bool ok = false, decided = false;
-                        if (last_hop) {
-                            if (!(ep->sid_flags & HL_PSID_NP)) { lab = 3; ok = decided = true; }
-                            else if (ep->sid_flags & HL_PSID_E) { lab = 0; ok = decided = true; }
-                        }
-                        if (!decided) {
-                            if (!ep->sid_is_label) {
-                                const RouterInfo &nri = cached_ri(x.nbr);
-                                if (!nri.srgb.empty()) ok = index_to_label(ep->sid_value, nri.srgb, &lab);
-                            } else {
-                                lab = last_hop ? ep->sid_value : 3u; ok = true;
-                            }
-                        }
-                        if (ok) { x.has_label = 1; x.label = lab; }
-                    }
-                    auto it = std::lower_bound(set.begin(), set.end(), x, nh_less);
-                    if (it != set.end() && nh_same_key(*it, x)) {
-                        // two atoms, one next hop: the reference keeps whichever advertiser came last; the
-                        // cell cannot tell unless both agree
-                        if (it->iface != x.iface || it->nbr != x.nbr || it->has_nbr != x.has_nbr ||
-                            it->has_label != x.has_label || it->label != x.label) return HSPF_E_UNSUPPORTED;
-                    } else {
-                        set.insert(it, x);
-                    }
-                }
-            }
-            if (set.size() > a->max_paths) set.resize(a->max_paths);
-            o.nh_off = n_nh; o.n_nh = (uint32_t)set.size();
-            if (n_routes < out->routes_cap && n_nh + set.size() <= out->nexthops_cap) {
-                out->routes[n_routes] = o;
+                if (set.size() > a->max_paths) set.resize(a->max_paths);
                 for (const Nh &x : set) {
                     hl_nexthop h{};
-                    h.iface = x.iface; h.addr = x.has_addr ? x.addr : 0; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
-                    h.sr_label = x.has_label ? x.label : 0;
-                    h.has_addr = x.has_addr; h.has_nbr = x.has_nbr; h.has_label = x.has_label;
-                    out->nexthops[n_nh + (&x - set.data())] = h;
+                    h.iface = sort_key(x.iface); h.addr = x.has_addr ? x.addr : 0; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
+                    h.has_addr = x.has_addr; h.has_nbr = x.has_nbr;
+                    hops.push_back(h);
                 }
             }
-            ++n_routes; n_nh += (uint32_t)set.size();
+            o.n_nh = (uint32_t)hops.size() - o.nh_off;
+            routes.push_back(o);
         }
-        out->n_routes = n_routes; out->n_nexthops = n_nh;
-        if (n_routes > out->routes_cap || n_nh > out->nexthops_cap) return HSPF_E_NOMEM;
+        out->n_routes = (uint32_t)routes.size();
+        out->n_nexthops = (uint32_t)hops.size();
+        if (out->n_routes > out->routes_cap || out->n_nexthops > out->nexthops_cap) return HSPF_E_NOMEM;
+        if ((out->n_routes && !out->routes) || (out->n_nexthops && !out->nexthops)) return HSPF_E_INVAL;
+        std::copy(routes.begin(), routes.end(), out->routes);
+        std::copy(hops.begin(), hops.end(), out->nexthops);
         return HSPF_OK;
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;

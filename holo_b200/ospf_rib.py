@@ -10,7 +10,7 @@ from dataclasses import dataclass
 
 import numpy as np
 
-from . import capi, ospfv2
+from . import capi, ospfv2, route_table
 
 PATH_INTRA, PATH_INTER, PATH_TYPE1, PATH_TYPE2 = 0, 1, 2, 3
 PATH_NAMES = {PATH_INTRA: "intra-area", PATH_INTER: "inter-area", PATH_TYPE1: "external-1", PATH_TYPE2: "external-2"}
@@ -314,3 +314,86 @@ def update_rib_partial(router_id: int, max_paths: int, areas: list, externals, t
         raise capi.HspfError(rc, "update_rib_partial failed")
     return (Rib(routes[: out.n_routes].copy(), nhs[: out.n_nexthops].copy()), RtrTables(rt[: ts.n_rtrs].copy(), tnh[: ts.n_nexthops].copy()),
             acts[: n.value].copy())
+
+
+# ---- batched routing-table stage for roots attached to one area (include/holo_spf_lsdb.h) ------------------
+RIB_CELL_DT = np.dtype([("nh_mask", "<u8"), ("aux", "<u8"), ("winner", "<u4"), ("mpf", "<u4")])
+RIB_RECORD_DT = np.dtype([("x", "<u4"), ("y", "<u4"), ("z", "<u4"), ("w", "<u4")])   # ospf_rib_cells.h: RibRec
+JS_NOT_INTERNAL = 0x40            # HSPF_JS_NOT_INTERNAL: the job's root is an ABR
+NO_RECORD = 0xFFFFFFFF
+
+
+def cell_metric(cells):
+    return cells["mpf"] & 0x03FFFFFF
+
+
+def cell_path(cells):
+    return (cells["mpf"] >> 26) & 0x3
+
+
+def cell_flags(cells):
+    return cells["mpf"] >> 28
+
+
+class RibTable(route_table.RouteTable):
+    """hspf_ospfv2_ribtable: the area's intra-area, type-3 and type-5 prefixes in prefix order and, per prefix,
+    its intra-area advertisers, type-3 and type-5 records (host); `off` holds the three ranges per prefix
+    ([3, P + 1]).  `upload(ctx)` copies it to the device for hspf_ospfv2_rib_cells."""
+
+    api, kind, contrib_dt = "hspf_ospfv2", "ribtable", RIB_RECORD_DT
+
+    def __init__(self, flat: ospfv2.Flat, area_id: int, summaries=None, externals=None):
+        self.flat = flat
+        sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        self.area_id, self.summaries, self.externals = area_id, sm, ext
+        super().__init__(capi.load_library().hspf_ospfv2_ribtable_create, flat.handle, area_id,
+                         sm.ctypes.data if len(sm) else None, len(sm), ext.ctypes.data if len(ext) else None, len(ext))
+        pp, pl, po = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)()
+        self._call("arrays", C.byref(pp), C.byref(pl), C.byref(po), None)
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, np.uint32)
+        self.plen = route_table.copy_records(pl, self.n_prefixes, np.uint32)
+        self.off = route_table.copy_records(po, 3 * (self.n_prefixes + 1), np.uint32).reshape(3, self.n_prefixes + 1)
+
+
+def rib_cells_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr: int, cells_ptr: int,
+                     status_out_ptr: int = 0, n_gather: int = 0, gather_job_ptr: int = 0, gather_v_ptr: int = 0,
+                     gather_nh_ptr: int = 0):
+    """hspf_ospfv2_rib_cells / _cells16 over DEVICE planes (rs: capi.ResultStruct or capi.Result16Struct holding
+    device pointers); roots_ptr: device u32[n_jobs] root vertices; cells_ptr: device buffer of n_jobs * rt.n_prefixes
+    RIB_CELL_DT; status_out_ptr: device u32[n_jobs] or 0.  Enqueued on the ctx stream; the table must have been
+    uploaded."""
+    lib = ctx.lib
+    narrow = isinstance(rs, capi.Result16Struct)
+    fn = lib.hspf_ospfv2_rib_cells16 if narrow else lib.hspf_ospfv2_rib_cells
+    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), roots_ptr or None, cells_ptr, status_out_ptr or None, n_gather,
+            gather_job_ptr or None, gather_v_ptr or None, gather_nh_ptr or None)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
+def rib_from_cells(area: ospfv2.Ospfv2Area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv2_rib_from_cells (host): one job's cells -> the routing table update_rib_full gives for
+    area.router_id over its one area.  rc HSPF_E_UNSUPPORTED is returned in the result (caller: the host
+    stages over that job's planes)."""
+    lib = capi.load_library()
+    cells = np.ascontiguousarray(cells, RIB_CELL_DT)
+    assert cells.shape == (rt.n_prefixes,)
+    gv = np.ascontiguousarray(gather_v, np.uint32)
+    gn = np.ascontiguousarray(gather_nh, np.uint64)
+    s = area.as_struct()
+    caps = [max(rt.n_prefixes, 1), max(4 * rt.n_prefixes, 64)]
+    for _ in range(2):
+        routes, nhs = np.zeros(caps[0], RIB_ROUTE_DT), np.zeros(caps[1], ospfv2.NEXTHOP_DT)
+        r = RibStruct(caps[0], 0, routes.ctypes.data, caps[1], 0, nhs.ctypes.data)
+        rc = lib.hspf_ospfv2_rib_from_cells(C.byref(s), rt.handle, cells.ctypes.data, gv.ctypes.data_as(C.POINTER(C.c_uint32)),
+                                            gn.ctypes.data_as(C.POINTER(C.c_uint64)), len(gv), C.byref(r))
+        if rc == capi.HSPF_E_NOMEM:
+            caps = [max(caps[0], r.n_routes), max(caps[1], r.n_nexthops)]
+            continue
+        break
+    if rc not in (capi.HSPF_OK, capi.HSPF_E_UNSUPPORTED):
+        raise capi.HspfError(rc, "hspf_ospfv2_rib_from_cells failed")
+    if rc != capi.HSPF_OK:
+        return Rib(np.zeros(0, RIB_ROUTE_DT), np.zeros(0, ospfv2.NEXTHOP_DT), rc)
+    return Rib(routes[: r.n_routes].copy(), nhs[: r.n_nexthops].copy(), rc)

@@ -90,7 +90,7 @@ def abi_sizes_expected():
              ospf_rib.RIB_RTR_DT.itemsize, C.sizeof(ospf_rib.RtrTablesStruct),
              isis.LSP_TRIGGER_DT.itemsize, ospfv3.IP_PREFIX_DT.itemsize, ospfv3.TRIGGER6_DT.itemsize,
              C.sizeof(ospfv3.SpfComputation6Struct), isis.CELL_DT.itemsize,
-             route_table.DELTA_DT.itemsize, route_table.DELTA_JOB_DT.itemsize])
+             route_table.DELTA_DT.itemsize, route_table.DELTA_JOB_DT.itemsize, ospf_rib.RIB_CELL_DT.itemsize])
 
 
 def abi_sizes_from_library():
@@ -523,3 +523,64 @@ def synth_area(t: Topology, root: int = 0, sr: bool = False, max_paths: int = 16
             ep[i] = (rid(i), rid(i), 0xFFFFFFFF, 1, 1, 1, PSID_NP, 0, (0, 0), i % 8000)
         area.ri_lsas, area.srgbs, area.ext_prefixes = ri, sg, ep
     return area
+
+
+def inter_area_view(area: Ospfv2Area, seed: int, n_abr: int = 4, n_asbr: int = 3, n_inter: int = 60, n_ext: int = 50,
+                    unreachable_abr: bool = True, n_overlap: int = 8, n_fresh: int = 10, n_ext_only: int = 8):
+    """A single-area LSDB as one area of a multi-area domain: returns (area, summaries, externals) for
+    ospf_rib (hl_ospfv2_summary_lsa[] in LsaKey order, hl_ospfv2_external_lsa[] in LSDB order).  Seeded and
+    independent of area.router_id, so every root of one topology sees the same LSDB.
+      * n_abr routers get the B flag, n_asbr others the E flag; with unreachable_abr a router with B|E and no
+        adjacency is added (its LSAs exist, no job reaches it);
+      * type-3 LSAs from the ABRs (and from a router without the B flag and an unknown router, which no job may
+        use) for intra-area prefixes, new prefixes, prefixes with host bits and the default route; type-4 LSAs
+        for in-area ASBRs (the last one usable replaces the ASBR's intra-area entry) and ASBRs outside the area;
+        type-5 LSAs of type 1 and 2 from those ASBRs, from routers without the E flag, from unknown routers and
+        from ordinary routers (self-originated for the job rooted there);
+      * metrics from small sets, so that ties are common; some LSAs at maxage or at LSInfinity.
+    Prefixes: n_overlap of the area's own, n_fresh new /24s (< 2048) and three with host bits or the default route,
+    for both LSA types; n_ext_only /24s named by type-5 LSAs only, the first four by type-2 LSAs only."""
+    from . import ospf_rib
+    rng = np.random.default_rng(seed)
+    a = Ospfv2Area(**{k: getattr(area, k) for k in area.__dataclass_fields__})
+    rl, links = area.router_lsas.copy(), area.links.copy()
+    rids = [int(x) for x in rl["adv_rtr"]]
+    pick = [int(x) for x in rng.permutation(rids)]
+    abrs, asbrs, plain = pick[:n_abr], pick[n_abr:n_abr + n_asbr], pick[n_abr + n_asbr:]
+    for i, r in enumerate(rids):
+        rl["flags"][i] |= (0x01 if r in abrs else 0) | (0x02 if r in asbrs else 0)
+    lost = []
+    if unreachable_abr:
+        lost = [max(rids) + 0x100]
+        rl = np.concatenate([rl, np.array([(lost[0], lost[0], 1, 0x03, 0x02, len(links), 1)], ROUTER_LSA_DT)])
+        links = np.concatenate([links, np.array([(lost[0], 0xFFFFFFFF, 0, LINK_STUB, 0)], LINK_DT)])
+    a.router_lsas, a.links = rl, links
+    stubs = sorted({(int(l["link_id"]) & int(l["link_data"]), int(l["link_data"])) for l in links if l["link_type"] == LINK_STUB})
+    nets = [(int(n["lsa_id"]) & int(n["mask"]), int(n["mask"])) for n in area.network_lsas]
+    intra = [stubs[int(i)] for i in rng.choice(len(stubs), min(len(stubs), n_overlap), replace=False)] + nets[:2]
+    fresh = [(0x0AC80000 + (i << 8), 0xFFFFFF00) for i in range(n_fresh)]
+    pool = intra + fresh + [(0x0AC80005, 0xFFFFFF00), (0x0AC80105, 0xFFFFFF00), (0, 0)]
+    metric = lambda: int(rng.choice([1, 10, 10, 20, 30])) if rng.random() > 0.05 else ospf_rib.LSA_INFINITY
+    maxage = lambda: int(rng.random() < 0.06)
+    sums = []
+    advs3 = abrs + lost + plain[:1] + [0x7F000001]                # the last two: never an ABR of the area
+    for _ in range(n_inter):
+        p, m = pool[int(rng.integers(0, len(pool)))]
+        sums.append((int(rng.choice(advs3)), p, m, metric(), 3, maxage(), (0, 0)))
+    outside = [0x0B000001 + i for i in range(3)]                  # ASBRs in other areas
+    for asbr in asbrs[:2] + outside:
+        for abr in rng.choice(abrs + lost, int(rng.integers(1, 4)), replace=False):
+            sums.append((int(abr), asbr, 0, metric(), 4, maxage(), (0, 0)))
+    sums.sort(key=lambda x: (x[4], x[0], x[1]))
+    summaries = np.asarray(sums, ospf_rib.SUMMARY_LSA_DT)
+    ext = []
+    advs5 = asbrs + outside + lost + plain[:3] + abrs[:1] + [0x7F000002]
+    pool5 = pool + [(0x0C000000 + (i << 8), 0xFFFFFF00) for i in range(n_ext_only)]     # prefixes only externals name
+    for _ in range(n_ext):
+        p, m = pool5[int(rng.integers(0, len(pool5)))]
+        e_bit = 1 if 0x0C000000 <= p < 0x0C000400 else int(rng.integers(0, 2))   # four prefixes of type-2 LSAs only
+        ext.append((int(rng.choice(advs5)), p, m, int(rng.choice([1, 5, 5, 20])) if rng.random() > 0.05 else ospf_rib.LSA_INFINITY,
+                    0, int(rng.integers(0, 4)), e_bit, maxage(), (0, 0)))
+    ext.sort(key=lambda x: (x[0], x[1]))
+    externals = np.asarray(ext, ospf_rib.EXTERNAL_LSA_DT)
+    return a, summaries, externals

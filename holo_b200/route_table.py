@@ -27,7 +27,8 @@ class RouteTable:
     16-byte contributor records `contribs`, and `upload(ctx)`, which copies the table to the device.  Subclasses
     name the table type's functions (`api`), their record dtype, and read the prefixes."""
 
-    api = ""                  # "hspf_ospfv2" or "hspf_isis": prefix of the table type's rtable_* functions
+    api = ""                  # "hspf_ospfv2" or "hspf_isis": prefix of the table type's functions
+    kind = "rtable"           # the table type's functions are {api}_{kind}_*
     contrib_dt = None
 
     def __init__(self, create, *args):
@@ -45,10 +46,10 @@ class RouteTable:
         self.contribs = copy_records(pc, self.n_contributors, self.contrib_dt)
 
     def _call(self, name, *args):
-        return getattr(self.lib, f"{self.api}_rtable_{name}")(self.handle, *args)
+        return getattr(self.lib, f"{self.api}_{self.kind}_{name}")(self.handle, *args)
 
     def upload(self, ctx: capi.Context):
-        rc = getattr(self.lib, f"{self.api}_rtable_upload")(ctx.handle, self.handle)
+        rc = getattr(self.lib, f"{self.api}_{self.kind}_upload")(ctx.handle, self.handle)
         if rc != capi.HSPF_OK:
             raise capi.HspfError(rc, ctx.last_error())
 
@@ -64,7 +65,7 @@ class RouteTable:
 def declare(lib: C.CDLL):
     """The route stage's C signatures, set once when the library is loaded.  Every caller shares one CDLL, so a
     signature set per call would change how the function is marshalled for all of them."""
-    from . import isis, ospfv2, ospfv3
+    from . import isis, ospf_rib, ospfv2, ospfv3
     vp, u32, u64 = C.c_void_p, C.c_uint32, C.c_uint64
     pvp, u16p, u32p, u64p = C.POINTER(vp), C.POINTER(C.c_uint16), C.POINTER(u32), C.POINTER(u64)
     res, res16 = C.POINTER(capi.ResultStruct), C.POINTER(capi.Result16Struct)
@@ -94,12 +95,18 @@ def declare(lib: C.CDLL):
         "hspf_isis_routes_delta16": [vp, vp, u32, res16, res16, vp, u32, vp, vp, vp, u64, vp],
         "hspf_isis_routes_from_cells": [C.POINTER(isis.InstanceStruct), vp, vp, u32p, u16p, u32p, u16p, u32, u32p, u32p,
                                         u32, u32p, u32p, C.POINTER(isis.RibStruct)],
+        "hspf_ospfv2_ribtable_create": [vp, u32, vp, u32, vp, u32, pvp],
+        "hspf_ospfv2_ribtable_arrays": [vp, C.POINTER(u32p), C.POINTER(u32p), C.POINTER(u32p), pvp],
+        "hspf_ospfv2_ribtable_upload": [vp, vp],
+        "hspf_ospfv2_rib_cells": [vp, vp, u32, res, vp, vp, vp, u32, vp, vp, vp],
+        "hspf_ospfv2_rib_cells16": [vp, vp, u32, res16, vp, vp, vp, u32, vp, vp, vp],
+        "hspf_ospfv2_rib_from_cells": [C.POINTER(ospfv2.AreaStruct), vp, vp, u32p, u64p, u32, C.POINTER(ospf_rib.RibStruct)],
     }
     for name, argtypes in sigs.items():
         getattr(lib, name).argtypes = argtypes
-    for api in ("hspf_ospfv2", "hspf_isis"):
-        getattr(lib, api + "_rtable_free").argtypes = [vp]
-        getattr(lib, api + "_rtable_free").restype = None
+    for table in ("hspf_ospfv2_rtable", "hspf_isis_rtable", "hspf_ospfv2_ribtable"):
+        getattr(lib, table + "_free").argtypes = [vp]
+        getattr(lib, table + "_free").restype = None
         for name in ("prefixes", "contributors"):
-            getattr(lib, f"{api}_rtable_{name}").argtypes = [vp]
-            getattr(lib, f"{api}_rtable_{name}").restype = u32
+            getattr(lib, f"{table}_{name}").argtypes = [vp]
+            getattr(lib, f"{table}_{name}").restype = u32

@@ -881,6 +881,29 @@ typedef struct hl_route_delta_job {
     uint32_t _pad;
 } hl_route_delta_job;
 
+/* ------------------------------------------------------- batched OSPFv2 route-table cells -- */
+/* One (job, prefix) cell of the device routing-table stage (hspf_ospfv2_rib_cells): what update_rib_full
+ * (route.rs:146-193) leaves for that prefix when the job's root is attached to one area only — intra-area
+ * route, else the best inter-area route (type-3), else the best AS-external route (type-5 through the
+ * ASBR's entry) — with the next hops still as first-hop atoms.  Prefixes are those of the table
+ * (hspf_ospfv2_ribtable_prefixes), in prefix order.  `mpf` packs the metric (bits 0-25: at most
+ * 0xFFFE + 2 * 0xFFFFFE, a type-1 external behind a type-4 entry), the HL_PATH_* type (bits 26-27)
+ * and the HL_CELL_* flags (bits 28-31). */
+typedef struct hl_ospf_rib_cell {
+    uint64_t nh_mask;       /* atoms of the winner, equal-cost candidates OR-ed together                  */
+    uint64_t aux;           /* intra-area: last-hop atoms (hl_route_cell.lasthop_mask); type-2 external:
+                               the type-2 metric; else 0                                                   */
+    uint32_t winner;        /* record index in the table, 0xFFFFFFFF: no route                              */
+    uint32_t mpf;           /* metric | path type << 26 | flags << 28                                       */
+} hl_ospf_rib_cell;
+#define HL_RIB_CELL_METRIC_BITS  26u
+#define HL_RIB_CELL_METRIC_MAX   0x03FFFFFFu
+#define HL_RIB_CELL_MPF(metric, path, flags) \
+    ((uint32_t)(metric) | ((uint32_t)(path) << 26) | ((uint32_t)(flags) << 28))
+#define HL_RIB_CELL_METRIC(c)    ((c).mpf & HL_RIB_CELL_METRIC_MAX)
+#define HL_RIB_CELL_PATH(c)      (((c).mpf >> 26) & 0x3u)
+#define HL_RIB_CELL_FLAGS(c)     ((c).mpf >> 28)
+
 #ifdef __cplusplus
 }
 #endif

@@ -100,6 +100,8 @@ extern "C" {
 #define HSPF_JS_NARROW         0x20u /* hspf_run_batch16 only: the result does not fit 16-bit planes */
 #define HSPF_JS_INTERNAL       0x10u /* a device loop hit a bound that cannot be reached on a
                                         valid graph (defensive; please report): planes undefined */
+#define HSPF_JS_NOT_INTERNAL   0x40u /* hspf_ospfv2_rib_cells only: the job's root is an area border
+                                        router (B flag), whose table spans other areas: no cells   */
 
 /*
  * Flattened link-state graph of one area / level / topology.

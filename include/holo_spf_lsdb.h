@@ -180,6 +180,59 @@ int hspf_ospfv2_routes_from_cells(const hl_ospfv2_area *area, const hspf_ospfv2_
                                   uint32_t n_gather, hl_ospfv2_result *out);
 
 /*
+ * Batched routing-table stage on the device, for roots attached to one area (every internal router of the
+ * area): update_rib_full (holo-ospf/src/route.rs:146-193) — intra-area, inter-area and AS-external routes —
+ * for every job of a batch.  For job j with root router r over area A, the decoded cells of j equal
+ *     hspf_ospfv2_update_rib_full(r, A.max_paths, [{A.area_id, spf_j, A.ifaces, summaries, active = 1}], externals)
+ * with spf_j = hspf_ospfv2_area_from_planes(A with router_id = r, j's planes): routes and next hops.
+ *
+ *   hspf_ospfv2_ribtable_create  per flattened area: the prefixes of its intra-area routes, type-3 and type-5
+ *                                LSAs (type-3 / type-5 prefixes keep their host bits, as update_rib_full does) in
+ *                                prefix order, and per prefix three record ranges: its intra-area advertisers
+ *                                (the records of hspf_ospfv2_rtable_create), its type-3 LSAs, its type-5 LSAs, in
+ *                                LSDB order.  summaries: the area's type-3 / type-4 LSAs (LsaKey order); externals:
+ *                                the instance's AS-external LSAs.  LSAs that no job can use (maxage, metric at
+ *                                infinity, a type-3 / type-4 LSA from a router that is not an ABR of the area) are
+ *                                left out here.  HSPF_E_UNSUPPORTED when the answer would depend on more than one
+ *                                area's SPT: area 0 with a virtual-link endpoint (V flag: the transit-area stage
+ *                                could rewrite intra-area routes), or a usable type-4 LSA naming an ABR (its entry
+ *                                would replace the ABR's for later type-4 LSAs).  Host only.
+ *   hspf_ospfv2_ribtable_arrays  prefix[P], plen[P], off[3 (P + 1)] (intra, type-3, type-5 ranges), the 16-byte
+ *                                records (ospf_rib_cells.h); any pointer may be NULL.
+ *   hspf_ospfv2_ribtable_upload  copies the table to the ctx's device.
+ *   hspf_ospfv2_rib_cells        one thread per (job, prefix) over DEVICE planes as hspf_ospfv2_routes_batch[16];
+ *   hspf_ospfv2_rib_cells16      roots: device u32[n_jobs], each job's root vertex; cells[n_jobs][P] (device).
+ *                                job_status_out (device u32[n_jobs], may be NULL): the planes' status word, plus
+ *                                HSPF_JS_INVALID for a root >= V and HSPF_JS_NOT_INTERNAL for a root with the B
+ *                                flag (an ABR: its table spans other areas).  A job with a non-zero word gets empty
+ *                                cells.  gather_* as hspf_ospfv2_routes_batch.  Enqueued on the ctx stream.
+ *   hspf_ospfv2_rib_from_cells   host: one job's cells -> the table above (out->routes in prefix order, next hops
+ *                                named by interface sort key in NexthopKey order, HSPF_E_NOMEM with the counts when
+ *                                out is too small).  `area` as for hspf_ospfv2_routes_from_cells, with router_id =
+ *                                the job's root.  HSPF_E_UNSUPPORTED in the cases of hspf_ospfv2_routes_from_cells:
+ *                                take that job through its planes and hspf_ospfv2_update_rib_full.
+ */
+typedef struct hspf_ospfv2_ribtable hspf_ospfv2_ribtable;
+int hspf_ospfv2_ribtable_create(const hspf_ospfv2_flat *flat, uint32_t area_id, const hl_ospfv2_summary_lsa *summaries,
+                                uint32_t n_summaries, const hl_ospfv2_external_lsa *externals, uint32_t n_externals,
+                                hspf_ospfv2_ribtable **out);
+void hspf_ospfv2_ribtable_free(hspf_ospfv2_ribtable *rt);
+uint32_t hspf_ospfv2_ribtable_prefixes(const hspf_ospfv2_ribtable *rt);
+uint32_t hspf_ospfv2_ribtable_contributors(const hspf_ospfv2_ribtable *rt);
+int hspf_ospfv2_ribtable_arrays(const hspf_ospfv2_ribtable *rt, const uint32_t **prefix, const uint32_t **plen,
+                                const uint32_t **off, const void **records);
+int hspf_ospfv2_ribtable_upload(hspf_ctx *ctx, hspf_ospfv2_ribtable *rt);
+int hspf_ospfv2_rib_cells(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result *planes,
+                          const uint32_t *roots, hl_ospf_rib_cell *cells, uint32_t *job_status_out,
+                          uint32_t n_gather, const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh);
+int hspf_ospfv2_rib_cells16(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result16 *planes,
+                            const uint32_t *roots, hl_ospf_rib_cell *cells, uint32_t *job_status_out,
+                            uint32_t n_gather, const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh);
+int hspf_ospfv2_rib_from_cells(const hl_ospfv2_area *area, const hspf_ospfv2_ribtable *rt, const hl_ospf_rib_cell *cells,
+                               const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather,
+                               hl_ospfv2_rib *out);
+
+/*
  * The stages of update_rib_full that follow the per-area SPFs (holo-ospf/src/route.rs:146-193):
  * merges the intra-area routes of the attached areas (route_update / route_compare,
  * route.rs:895-971), adds inter-area network routes and inter-area router entries from the
