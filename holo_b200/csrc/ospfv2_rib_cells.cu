@@ -27,6 +27,10 @@ struct OspfRibCell {
     __device__ __forceinline__ bool refused(uint32_t j) const {
         return (status && status[j] != 0) || hspf::rib_job_refusal(t, roots[j]) != 0;
     }
+    // what job_status_out of ospf_rib_cells_kernel holds for job j
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
+        return (status ? status[j] : 0u) | hspf::rib_job_refusal(t, roots[j]);
+    }
     __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
         const size_t base = (size_t)j * t.V;
         return hspf::ospf_rib_cell_eval(Planes{dist + base, hops + base, nh + base}, roots[j], t, p);
@@ -73,6 +77,41 @@ int launch_rib_cells(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_j
     });
 }
 
+// Blocks per SM of the route-delta passes over this walk: their launch bound and their grid.  At the cell kernels'
+// 8 the walk plus the base compare spills 68 bytes in pass A; from 5 down neither pass spills, and of the bounds
+// timed on an H100 this one was fastest (DESIGN.md §4.4, §6).
+constexpr uint32_t kRibDeltaBlocksPerSM = 4;
+
+// The route-delta stage over the same walk (route_stage.cuh: launch_route_delta), its grid one wave of
+// kRibDeltaBlocksPerSM blocks per SM.
+template <class Planes, class D, class N>
+int launch_rib_delta(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const D *dist, const uint16_t *hops,
+                     const N *nh, const uint32_t *status, const uint32_t *roots, const hl_ospf_rib_cell *base_cells,
+                     uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
+                     uint64_t cap, uint64_t *n_records) {
+    if (!ctx || !rt || !rt->dev.blob || !dist || !hops || !nh || (n_jobs && !roots)) return HSPF_E_INVAL;
+    using Cell = OspfRibCell<Planes, D, N>;
+    const uint32_t P = (uint32_t)rt->prefix.size(), V = (uint32_t)rt->vflags.size();
+    const RibRec *recs = static_cast<const RibRec *>(rt->dev.contribs);
+    const Cell cell{hspf::RibView{rt->dev.off, recs, reinterpret_cast<const uint8_t *>(recs + rt->recs.size()), P, V},
+                    dist, hops, nh, status, roots};
+    hspf::DeltaArgs a{};
+    a.n_jobs = n_jobs; a.P = P;
+    a.base = reinterpret_cast<const uint64_t *>(base_cells); a.n_base = n_base; a.base_of = base_of;
+    a.job_out = job_out; a.n_records = reinterpret_cast<unsigned long long *>(n_records);
+    a.records = records; a.cap = cap;
+    return hspf::launch_route_delta(ctx, rt->dev, a,
+        [&](uint32_t blocks, cudaStream_t st, const hspf::DeltaArgs &args) {
+            hspf::route_delta_count_kernel<hspf::OspfRibCellLayout, Cell, kRibDeltaBlocksPerSM>
+                <<<blocks, hspf::kRouteThreads, 0, st>>>(cell, args);
+        },
+        [&](uint32_t blocks, cudaStream_t st, const hspf::DeltaArgs &args) {
+            hspf::route_delta_store_kernel<hspf::OspfRibCellLayout, Cell, kRibDeltaBlocksPerSM>
+                <<<blocks, hspf::kRouteThreads, 0, st>>>(cell, args);
+        },
+        kRibDeltaBlocksPerSM);
+}
+
 }  // namespace
 
 extern "C" {
@@ -102,6 +141,26 @@ int hspf_ospfv2_rib_cells16(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint3
     return launch_rib_cells<hspf::PlanesNarrow, uint16_t, uint16_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask,
                                                                     pl->job_status, roots, cells, job_status_out, n_gather,
                                                                     gather_job, gather_v, gather_nh);
+}
+
+int hspf_ospfv2_rib_delta(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result *pl,
+                          const uint32_t *roots, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                          const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                          uint64_t *n_records) {
+    if (!pl || pl->nh_words != 1) return HSPF_E_INVAL;
+    return launch_rib_delta<hspf::PlanesWide, uint32_t, uint64_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask,
+                                                                  pl->job_status, roots, base_cells, n_base, base_of,
+                                                                  job_out, records, cap, n_records);
+}
+
+int hspf_ospfv2_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
+                            const uint32_t *roots, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                            const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                            uint64_t *n_records) {
+    if (!pl) return HSPF_E_INVAL;
+    return launch_rib_delta<hspf::PlanesNarrow, uint16_t, uint16_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask,
+                                                                    pl->job_status, roots, base_cells, n_base, base_of,
+                                                                    job_out, records, cap, n_records);
 }
 
 }  // extern "C"

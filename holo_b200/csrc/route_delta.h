@@ -1,10 +1,13 @@
 // Route-delta classification: how one (job, prefix) cell differs from its base cell (include/holo_lsdb.h,
 // HL_DELTA_*).  Host and device: the fused route-delta stage (route_stage.cuh) and the CPU test harness compile
-// this same function.  Both cell layouts are three 8-byte words with the next-hop atom set in word 0; they differ
-// in where the HL_CELL_* flags byte and the metric sit:
+// this same function.  Every cell layout is three 8-byte words with the next-hop atom set in word 0; they differ
+// in where the HL_CELL_* flags and the metric sit:
 //   OSPF  (hl_route_cell)      w1 lasthop_mask,               w2 winner | metric:16 << 32 | flags << 48
 //   IS-IS (hl_isis_route_cell) w1 winner | metric:32 << 32,   w2 flags
-// Everything outside word 0 and the metric field (winner, flags, OSPF lasthop_mask) counts as HL_DELTA_OTHER.
+//   OSPF routing table (hl_ospf_rib_cell)
+//                              w1 aux,                        w2 winner | metric:26 << 32 | path:2 << 58 | flags:4 << 60
+// Everything outside word 0 and the metric field (winner, flags, OSPF lasthop_mask, routing-table path type and aux)
+// counts as HL_DELTA_OTHER.
 #pragma once
 #include <cstdint>
 
@@ -31,6 +34,11 @@ struct OspfCellLayout {
 struct IsisCellLayout {
     static constexpr uint32_t flags_word = 2, flags_shift = 0, metric_word = 1, metric_shift = 32;
     static constexpr uint64_t metric_mask = 0xFFFFFFFFull << 32;
+};
+// flags are 4 bits here: the shifted word holds nothing above them
+struct OspfRibCellLayout {
+    static constexpr uint32_t flags_word = 2, flags_shift = 60, metric_word = 2, metric_shift = 32;
+    static constexpr uint64_t metric_mask = 0x3FFFFFFull << 32;
 };
 
 HSPF_HD uint64_t cell_word(const CellWords &c, uint32_t i) { return i == 0 ? c.w0 : (i == 1 ? c.w1 : c.w2); }

@@ -59,17 +59,19 @@ __device__ __forceinline__ void store_route_cells(uint32_t n_jobs, uint32_t P, c
     }
 }
 
-// Enqueues one route kernel on the ctx stream over `total` cells: one wave of kRouteBlocksPerSM blocks per SM,
-// warp-tile-stride beyond that.  `launch(blocks, stream, aligned16)` makes the <<<blocks, kRouteThreads>>> call.
+// Enqueues one route kernel on the ctx stream over `total` cells: one wave of `blocks_per_sm` blocks per SM (the
+// kernel's __launch_bounds__ minimum), warp-tile-stride beyond that.  `launch(blocks, stream, aligned16)` makes the
+// <<<blocks, kRouteThreads>>> call.
 template <class Launch>
-int launch_route_stage(hspf_ctx *ctx, const DeviceRouteTable &table, uint64_t total, const void *cells, Launch launch) {
+int launch_route_stage(hspf_ctx *ctx, const DeviceRouteTable &table, uint64_t total, const void *cells, Launch launch,
+                       uint32_t blocks_per_sm = kRouteBlocksPerSM) {
     const int dev = hspf_ctx_device(ctx);
     if (table.device != dev) return HSPF_E_INVAL;             // the table was uploaded to another device
     int sms = 0;
     if (cudaSetDevice(dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
         return HSPF_E_CUDA;
     const uint64_t want = std::max<uint64_t>((total + kRouteThreads - 1) / kRouteThreads, 1);
-    const uint32_t blocks = (uint32_t)std::min<uint64_t>(want, (uint64_t)sms * kRouteBlocksPerSM);
+    const uint32_t blocks = (uint32_t)std::min<uint64_t>(want, (uint64_t)sms * blocks_per_sm);
     const bool aligned16 = (reinterpret_cast<uintptr_t>(cells) & 15u) == 0;
     launch(blocks, static_cast<cudaStream_t>(hspf_stream(ctx)), aligned16);
     if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
@@ -189,9 +191,11 @@ cudaError_t route_delta_scan(void *temp, size_t temp_bytes, const uint8_t *cnt, 
 
 // Validates the arguments every route-delta call shares and enqueues the stage on the ctx stream: the summaries and
 // the total are zeroed, then `count(blocks, stream, args)` launches pass A; with records, the scan and
-// `store(blocks, stream, args)` (pass B) follow.  `a.base` is the caller's base cell buffer.
+// `store(blocks, stream, args)` (pass B) follow.  `a.base` is the caller's base cell buffer; `blocks_per_sm` is
+// the kMinBlocks both passes were instantiated with.
 template <class Count, class Store>
-int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, DeltaArgs a, Count count, Store store) {
+int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, DeltaArgs a, Count count, Store store,
+                       uint32_t blocks_per_sm = kRouteBlocksPerSM) {
     if (!a.base || !a.job_out || !a.n_records || a.n_base == 0) return HSPF_E_INVAL;
     // device buffers at their struct alignment
     if ((reinterpret_cast<uintptr_t>(a.base) & 7u) || (reinterpret_cast<uintptr_t>(a.job_out) & 3u) ||
@@ -231,7 +235,7 @@ int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, DeltaArgs a
         if (scan != cudaSuccess) return;
         store(blocks, s, a);
         hspf_note_launches(ctx, 2);                            // the scan (counted as one) and pass B
-    });
+    }, blocks_per_sm);
     return rc != HSPF_OK ? rc : (scan != cudaSuccess ? HSPF_E_CUDA : HSPF_OK);
 }
 

@@ -372,6 +372,22 @@ def rib_cells_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr
         raise capi.HspfError(rc, ctx.last_error())
 
 
+def rib_delta_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr: int, base_ptr: int, n_base: int,
+                     base_of_ptr: int, job_out_ptr: int, records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_ospfv2_rib_delta / _delta16 over DEVICE planes (rs and roots_ptr as for rib_cells_device): each job's cells
+    compared with its base row of base_ptr ([n_base, rt.n_prefixes] RIB_CELL_DT, normally rib_cells_device over the
+    unperturbed job of the same root; base_of_ptr: [n_jobs] u32 rows, 0 for row 0 of every job), without storing them.
+    job_out_ptr: [n_jobs] route_table.DELTA_JOB_DT; records_ptr: [cap] route_table.DELTA_DT in (job, prefix) order
+    (0 or cap 0: summaries only); n_records_ptr: u64 total.  All device pointers; enqueued on the ctx stream."""
+    lib = ctx.lib
+    narrow = isinstance(rs, capi.Result16Struct)
+    fn = lib.hspf_ospfv2_rib_delta16 if narrow else lib.hspf_ospfv2_rib_delta
+    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), roots_ptr or None, base_ptr or None, n_base, base_of_ptr or None,
+            job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
 def rib_from_cells(area: ospfv2.Ospfv2Area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
     """hspf_ospfv2_rib_from_cells (host): one job's cells -> the routing table update_rib_full gives for
     area.router_id over its one area.  rc HSPF_E_UNSUPPORTED is returned in the result (caller: the host

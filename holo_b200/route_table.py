@@ -100,6 +100,8 @@ def declare(lib: C.CDLL):
         "hspf_ospfv2_ribtable_upload": [vp, vp],
         "hspf_ospfv2_rib_cells": [vp, vp, u32, res, vp, vp, vp, u32, vp, vp, vp],
         "hspf_ospfv2_rib_cells16": [vp, vp, u32, res16, vp, vp, vp, u32, vp, vp, vp],
+        "hspf_ospfv2_rib_delta": [vp, vp, u32, res, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_rib_delta16": [vp, vp, u32, res16, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv2_rib_from_cells": [C.POINTER(ospfv2.AreaStruct), vp, vp, u32p, u64p, u32, C.POINTER(ospf_rib.RibStruct)],
     }
     for name, argtypes in sigs.items():

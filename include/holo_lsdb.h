@@ -863,8 +863,9 @@ typedef struct hl_isis_route_cell {
 #define HL_DELTA_GAINED    0x02u   /* J is present, B is not                                                   */
 #define HL_DELTA_METRIC    0x04u   /* both present, the metric differs                                         */
 #define HL_DELTA_NEXTHOPS  0x08u   /* both present, nh_mask differs                                            */
-#define HL_DELTA_OTHER     0x10u   /* both present, winner or flags differ (OSPF: or lasthop_mask); a new
-                                      winner can mean a new origin, route type or SR label                     */
+#define HL_DELTA_OTHER     0x10u   /* both present, winner or flags differ (OSPF: or lasthop_mask; routing-
+                                      table cell: or path type or aux); a new winner can mean a new origin,
+                                      route type or SR label                                                   */
 typedef struct hl_route_delta {
     uint32_t job;
     uint32_t prefix;        /* index in the route table                                                   */

@@ -211,6 +211,8 @@ int hspf_ospfv2_routes_from_cells(const hl_ospfv2_area *area, const hspf_ospfv2_
  *                                out is too small).  `area` as for hspf_ospfv2_routes_from_cells, with router_id =
  *                                the job's root.  HSPF_E_UNSUPPORTED in the cases of hspf_ospfv2_routes_from_cells:
  *                                take that job through its planes and hspf_ospfv2_update_rib_full.
+ *   hspf_ospfv2_rib_delta[16]    what-if batches: each job's cells compared with a base row on the device, without
+ *                                storing them (route-delta stage, below).
  */
 typedef struct hspf_ospfv2_ribtable hspf_ospfv2_ribtable;
 int hspf_ospfv2_ribtable_create(const hspf_ospfv2_flat *flat, uint32_t area_id, const hl_ospfv2_summary_lsa *summaries,
@@ -428,20 +430,28 @@ int hspf_isis_routes_from_cells(const hl_isis_instance *inst, const hspf_isis_rt
  *
  *   hspf_ospfv2_routes_delta[16]  OSPFv2 and OSPFv3 tables (as hspf_ospfv2_routes_batch[16]).
  *   hspf_isis_routes_delta[16]    IS-IS tables (as hspf_isis_routes_batch[16]).
- *
+ *   hspf_ospfv2_rib_delta[16]     OSPFv2 routing tables (as hspf_ospfv2_rib_cells[16]: the wide call needs
+ *                                 nh_words == 1; roots: device u32[n_jobs], required when n_jobs > 0).  A job and
+ *                                 its base row must share a root: atoms compare word for word only then.  The base
+ *                                 row is normally hspf_ospfv2_rib_cells over the root's unperturbed job.
  *   base_cells  DEVICE [n_base][P] cells, 8-byte aligned: typically written by hspf_*_routes_batch[16] for the
  *               unperturbed job of each root.  n_base == 0 is HSPF_E_INVAL.
  *   base_of     DEVICE [n_jobs] base row of each job, or NULL: every job uses row 0.
  *   job_out     DEVICE [n_jobs] hl_route_delta_job (required).  status: the job's status word (IS-IS: both
- *               topologies' OR-ed), or HSPF_JS_INVALID when base_of[j] >= n_base.  A job with a non-zero status
- *               is not compared: counts 0, no records.
+ *               topologies' OR-ed; routing tables: what job_status_out of hspf_ospfv2_rib_cells holds), or
+ *               HSPF_JS_INVALID when base_of[j] >= n_base.  A job with a non-zero status is not compared: counts 0,
+ *               no records.
  *   records     DEVICE hl_route_delta[cap], ordered by (job, prefix), identical from run to run.  Only the first
  *               min(total, cap) are written.  records NULL or cap 0: the summaries only.
  *   n_records   DEVICE uint64_t (required): the total number of changed (job, prefix), whatever cap is.
  *
  * Kinds (include/holo_lsdb.h, HL_DELTA_*), with B the base cell and J the job cell: LOST (B present, J not),
  * GAINED (J present, B not); both present: METRIC, NEXTHOPS (nh_mask), OTHER (winner or flags; OSPF: also
- * lasthop_mask) in any combination; neither present: no change.  What is not promised: an unchanged cell does not
+ * lasthop_mask) in any combination; neither present: no change.  Routing-table cells (hl_ospf_rib_cell): METRIC is
+ * the 26-bit cell metric (for a type-2 external, the forwarding metric to the ASBR, not the type-2 metric); OTHER is
+ * a changed winner, path type, HL_CELL_* flags or aux (intra-area last-hop atoms, or the type-2 metric, which the
+ * winner fixes).  A new path type always comes with a new winner, so it is OTHER; a caller who needs the path type
+ * decodes the job (hspf_ospfv2_rib_from_cells).  What is not promised: an unchanged cell does not
  * guarantee unchanged next-hop addresses.  IS-IS addresses come from a replay of the first hops that depends on
  * the order in which the root's neighbours leave the heap; OSPF addresses also read the atom sets of the transit
  * networks attached to the root.  A caller who needs addresses decodes the reported jobs
@@ -461,6 +471,14 @@ int hspf_isis_routes_delta16(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t
                              const hspf_result16 *mt6_planes, const hl_isis_route_cell *base_cells, uint32_t n_base,
                              const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                              uint64_t *n_records);
+int hspf_ospfv2_rib_delta(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result *planes,
+                          const uint32_t *roots, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                          const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
+                          uint64_t cap, uint64_t *n_records);
+int hspf_ospfv2_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result16 *planes,
+                            const uint32_t *roots, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                            const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
+                            uint64_t cap, uint64_t *n_records);
 
 /* sizeof() of the ABI structs in declaration order (hspf_csr, hspf_jobs,
  * hspf_result, then every struct of holo_lsdb.h); returns the count.  Lets a
