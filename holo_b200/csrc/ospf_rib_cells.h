@@ -126,7 +126,13 @@ struct hspf_ospfv2_ribtable {
     std::vector<uint8_t> vflags;             // [V] Router-LSA flags of router vertices
     uint32_t n_intra = 0, ext_base = 0, ext_end = 0;
     std::vector<uint32_t> ext_tag;           // per type-5 record (index - ext_base): the LSA's tag
-    hspf::DeviceRouteTable dev;              // hspf_ospfv2_ribtable_upload: off, then records + vflags
+    // OSPFv3 tables (hspf_ospfv3_ribtable_create): `intra` is an OSPFv3 rtable, `prefix` is zero-filled (the prefixes
+    // are intra->t.prefix6 merged with the LSAs' in prefix6), and options6 holds the prefix options per type-3 /
+    // type-5 record (index - n_intra)
+    bool v3 = false;
+    std::vector<hl_ip_addr> prefix6;
+    std::vector<uint8_t> options6;
+    hspf::DeviceRouteTable dev;             // hspf_ospfv2_ribtable_upload: off, then records + vflags
     hspf::RibView host_view() const {
         return hspf::RibView{off.data(), recs.data(), vflags.data(), (uint32_t)prefix.size(), (uint32_t)vflags.size()};
     }

@@ -21,6 +21,7 @@
 
 #include "holo_spf_lsdb.h"
 #include "ospf_rib_cells.h"
+#include "ospf_ribtable.h"
 #include "route_cells.h"
 
 namespace {
@@ -322,6 +323,23 @@ struct Route {
 };
 
 inline uint64_t pkey(uint32_t prefix, uint32_t plen) { return ((uint64_t)prefix << 8) | plen; }
+
+// the OSPFv2 side of hspf::build_rib_records (ospf_ribtable.h)
+struct RibV2 {
+    using Key = uint64_t;
+    using Sum = hl_ospfv2_summary_lsa;
+    using Ext = hl_ospfv2_external_lsa;
+    static constexpr bool kV3 = false;
+    static Key key(const Sum &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
+    static Key key(const Ext &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
+    static Key intra_key(const hspf::RouteTable &t, uint32_t k) { return pkey(t.prefix[k], t.plen[k]); }
+    static bool skip(const Sum &) { return false; }
+    static bool skip(const Ext &) { return false; }
+    static uint32_t asbr_id(const Sum &l) { return l.lsa_id; }
+    static uint8_t options(const Sum &) { return 0; }
+    static uint8_t options(const Ext &) { return 0; }
+    static void set_prefix(hspf_ospfv2_ribtable &rt, uint32_t u, Key k) { rt.prefix[u] = (uint32_t)(k >> 8); rt.plen[u] = (uint32_t)(k & 0xFF); }
+};
 
 }  // namespace
 
@@ -1053,117 +1071,23 @@ int hspf_ospfv2_ribtable_create(const hspf_ospfv2_flat *flat, uint32_t area_id, 
                                 hspf_ospfv2_ribtable **out) {
     if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext)) return HSPF_E_INVAL;
     *out = nullptr;
-    // the largest metric a cell holds: a type-1 external behind a type-4 entry, over a distance below saturation
-    static_assert(0xFFFEull + 2ull * (HL_LSA_INFINITY - 1) <= HL_RIB_CELL_METRIC_MAX, "cell metric field");
     try {
-        using hspf::RibRec;
         const hspf_ospfv2_flat &f = *flat;
         const hl_ospfv2_area *a = f.area;
         const uint32_t V = (uint32_t)f.ids.size();
         std::unique_ptr<hspf_ospfv2_ribtable, void (*)(hspf_ospfv2_ribtable *)> rt(new hspf_ospfv2_ribtable(),
                                                                                    hspf_ospfv2_ribtable_free);
-        rt->area_id = area_id;
         rt->vflags.assign(V, 0);
         for (uint32_t v = 0; v < V; ++v)
             if (f.is_router[v]) rt->vflags[v] = a->router_lsas[f.lsa_of[v]].flags;
-        // rib_full step 3 (transit areas) can rewrite the backbone's intra-area routes when it has virtual links
-        if (area_id == 0)
-            for (uint32_t v = 0; v < V; ++v)
-                if (rt->vflags[v] & HL_RTR_FLAG_V) return HSPF_E_UNSUPPORTED;
+        int rc = hspf_ospfv2_rtable_create(flat, &rt->intra);
+        if (rc) return rc;
         auto router_vertex = [&](uint32_t id) {
             auto it = f.rtr_vertex.find(id);
             return it == f.rtr_vertex.end() ? kNone : it->second;
         };
-        auto has_flag = [&](uint32_t v, uint8_t flag) { return v != kNone && (rt->vflags[v] & flag) != 0; };
-        auto live = [](uint8_t maxage, uint32_t metric) { return !maxage && metric < HL_LSA_INFINITY; };
-        int rc = hspf_ospfv2_rtable_create(flat, &rt->intra);
+        rc = hspf::build_rib_records<RibV2>(*rt, area_id, router_vertex, sums, n_sums, ext, n_ext);
         if (rc) return rc;
-        const hspf::RouteTable &it = rt->intra->t;
-
-        struct Keyed { uint64_t key; RibRec r; uint32_t tag; };
-        std::vector<Keyed> t3, t5;
-        std::unordered_map<uint32_t, uint32_t> slot_of;        // ASBR router id -> slot
-        std::vector<uint32_t> slot_id;
-        std::vector<std::vector<RibRec>> t4;                    // per slot, LSDB order
-        auto slot = [&](uint32_t id) {
-            auto ins = slot_of.emplace(id, (uint32_t)slot_id.size());
-            if (ins.second) { slot_id.push_back(id); t4.emplace_back(); }
-            return ins.first->second;
-        };
-        for (uint32_t i = 0; i < n_sums; ++i) {
-            const auto &l = sums[i];
-            if (!live(l.maxage, l.metric)) continue;
-            const uint32_t abr = router_vertex(l.adv_rtr);
-            if (!has_flag(abr, HL_RTR_FLAG_B)) continue;                 // abr(): a router entry with the B flag
-            if (l.lsa_type == 3) {
-                t3.push_back({pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)), RibRec{abr, l.metric, 0, 0}, 0});
-            } else if (l.lsa_type == 4) {
-                // the entry a type-4 LSA writes replaces the named router's: were that an ABR, later type-4 LSAs
-                // would see abr() change under them
-                if (has_flag(router_vertex(l.lsa_id), HL_RTR_FLAG_B)) return HSPF_E_UNSUPPORTED;
-                t4[slot(l.lsa_id)].push_back(RibRec{abr, l.metric, 0, 0});
-            }
-        }
-        for (uint32_t i = 0; i < n_ext; ++i) {
-            const auto &l = ext[i];
-            if (!live(l.maxage, l.metric)) continue;
-            t5.push_back({pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)), RibRec{slot(l.adv_rtr), l.metric,
-                          l.e_bit ? 1u : 0u, 0}, l.tag});
-        }
-        auto by_key = [](const Keyed &x, const Keyed &y) { return x.key < y.key; };
-        std::stable_sort(t3.begin(), t3.end(), by_key);        // LSDB order within a prefix
-        std::stable_sort(t5.begin(), t5.end(), by_key);
-        std::vector<uint64_t> keys;
-        keys.reserve(it.prefix.size() + t3.size() + t5.size());
-        for (size_t k = 0; k < it.prefix.size(); ++k) keys.push_back(pkey(it.prefix[k], it.plen[k]));
-        for (const Keyed &x : t3) keys.push_back(x.key);
-        for (const Keyed &x : t5) keys.push_back(x.key);
-        std::sort(keys.begin(), keys.end());
-        keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
-        const uint32_t P = (uint32_t)keys.size(), PI = (uint32_t)it.prefix.size();
-        rt->n_intra = (uint32_t)it.contribs.size();
-        const uint64_t n_slots = slot_id.size(), slot_base = (uint64_t)rt->n_intra + t3.size() + t5.size();
-        uint64_t n_t4 = 0;
-        for (const auto &l : t4) n_t4 += l.size();
-        if (slot_base + n_slots + n_t4 >= kNone) return HSPF_E_UNSUPPORTED;      // record indices are u32
-        rt->recs.resize(rt->n_intra);
-        if (rt->n_intra) std::memcpy(rt->recs.data(), it.contribs.data(), rt->n_intra * sizeof(RibRec));
-        rt->prefix.resize(P); rt->plen.resize(P); rt->intra_of.assign(P, kNone);
-        rt->off.assign(3 * ((size_t)P + 1), 0);
-        uint32_t *oi = rt->off.data(), *o3 = oi + P + 1, *o5 = o3 + P + 1;
-        uint32_t k = 0;
-        for (uint32_t u = 0; u < P; ++u) {
-            rt->prefix[u] = (uint32_t)(keys[u] >> 8); rt->plen[u] = (uint32_t)(keys[u] & 0xFF);
-            oi[u] = it.off[k];                                  // an empty range where the prefix has no intra record
-            if (k < PI && pkey(it.prefix[k], it.plen[k]) == keys[u]) rt->intra_of[u] = k++;
-        }
-        oi[P] = rt->n_intra;
-        size_t q = 0;
-        for (uint32_t u = 0; u < P; ++u) {
-            o3[u] = (uint32_t)rt->recs.size();
-            for (; q < t3.size() && t3[q].key == keys[u]; ++q) rt->recs.push_back(t3[q].r);
-        }
-        o3[P] = (uint32_t)rt->recs.size();
-        rt->ext_base = o3[P];
-        q = 0;
-        for (uint32_t u = 0; u < P; ++u) {
-            o5[u] = (uint32_t)rt->recs.size();
-            for (; q < t5.size() && t5[q].key == keys[u]; ++q) {
-                RibRec r = t5[q].r;
-                r.x += (uint32_t)slot_base;
-                rt->recs.push_back(r);
-                rt->ext_tag.push_back(t5[q].tag);
-            }
-        }
-        o5[P] = (uint32_t)rt->recs.size();
-        rt->ext_end = o5[P];
-        uint32_t t4_at = (uint32_t)(slot_base + n_slots);
-        for (uint32_t s = 0; s < n_slots; ++s) {
-            const uint32_t v = router_vertex(slot_id[s]);
-            rt->recs.push_back(RibRec{v, has_flag(v, HL_RTR_FLAG_E) ? 1u : 0u, t4_at, t4_at + (uint32_t)t4[s].size()});
-            t4_at += (uint32_t)t4[s].size();
-        }
-        for (const auto &l : t4) rt->recs.insert(rt->recs.end(), l.begin(), l.end());
         *out = rt.release();
         return HSPF_OK;
     } catch (const std::bad_alloc &) {
@@ -1188,7 +1112,7 @@ int hspf_ospfv2_ribtable_arrays(const hspf_ospfv2_ribtable *rt, const uint32_t *
 
 int hspf_ospfv2_rib_from_cells(const hl_ospfv2_area *a, const hspf_ospfv2_ribtable *rt, const hl_ospf_rib_cell *cells,
                                const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv2_rib *out) {
-    if (!a || !rt || !rt->intra || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
+    if (!a || !rt || rt->v3 || !rt->intra || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
     try {
         out->n_routes = out->n_nexthops = 0;
         JobDecode jd;

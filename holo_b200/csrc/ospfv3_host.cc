@@ -23,6 +23,8 @@
 #include <vector>
 
 #include "holo_spf_lsdb.h"
+#include "ospf_rib_cells.h"
+#include "ospf_ribtable.h"
 #include "route_cells.h"
 
 namespace {
@@ -635,6 +637,120 @@ int hspf_ospfv3_rtable_prefixes6(const hspf_ospfv2_rtable *rt, const hl_ip_addr 
     return HSPF_OK;
 }
 
+}  // extern "C" (reopened below)
+
+namespace {
+
+// One job's decode state: the flattened area, its root, and atoms -> next hops (Resolver) over the nh_mask of the
+// transit networks next to the root, the only plane values Resolver::resolve looks up.
+struct JobDecode {
+    hspf_ospfv3_flat f;
+    uint32_t root = kNone;
+    std::vector<uint64_t> sparse_nh;
+    std::unique_ptr<Resolver> rs;
+    // HSPF_OK with root == kNone when area->router_id is not a router of the area
+    int init(const hl_ospfv3_area *a, uint32_t n_vertices, const uint32_t *gather_v, const uint64_t *gather_nh,
+             uint32_t n_gather) {
+        int rc = flatten(a, f);
+        if (rc) return rc;
+        const uint32_t V = (uint32_t)f.rid.size();
+        if (V != n_vertices) return HSPF_E_INVAL;                      // not the LSDB the table was built from
+        auto rit = f.rtr_vertex.find(a->router_id);
+        if (rit == f.rtr_vertex.end()) return HSPF_OK;
+        root = rit->second;
+        sparse_nh.assign(V, 0);
+        for (uint32_t i = 0; i < n_gather; ++i) {
+            if (gather_v[i] >= V) return HSPF_E_INVAL;
+            sparse_nh[gather_v[i]] = gather_nh[i];
+        }
+        rs.reset(new Resolver{f, a, root, sparse_nh.data(), 1, {}, {}});
+        rs->atom_nh.resize(64);
+        rs->atom_done.assign(64, 0);
+        return HSPF_OK;
+    }
+};
+
+// The atoms of `mask` resolved into one next-hop set in NexthopKey order; false when two atoms give one next hop with
+// different attributes (the reference keeps the later advertiser's, which the cell cannot tell).
+bool atom_hops(Resolver &rs, uint64_t mask, std::vector<Nh6> &set) {
+    set.clear();
+    for (uint64_t m = mask; m; m &= m - 1) {
+        for (const Nh6 &x : rs.resolve((uint32_t)__builtin_ctzll(m))) {
+            auto it = std::lower_bound(set.begin(), set.end(), x, nh_less);
+            if (it == set.end() || !nh_same(*it, x)) { set.insert(it, x); continue; }
+            if (it->iface != x.iface || it->has_nbr != x.has_nbr || (x.has_nbr && it->nbr != x.nbr)) return false;
+        }
+    }
+    return true;
+}
+
+// Intra-area routes of one job's cells (hspf_ospfv3_routes_from_cells after its checks).
+int intra_from_cells(JobDecode &jd, const hl_ospfv3_area *a, const hspf_ospfv2_rtable *rt, const hl_route_cell *cells,
+                     hl_ospfv3_result *out) {
+    const auto &t = rt->t;
+    const uint32_t P = (uint32_t)t.prefix6.size();
+    uint32_t n_routes = 0, n_nh = 0;
+    std::vector<Nh6> set;
+    for (uint32_t p = 0; p < P; ++p) {
+        const hl_route_cell &c = cells[p];
+        if (!(c.flags & HL_CELL_PRESENT)) continue;
+        if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
+        if (c.winner < t.off[p] || c.winner >= t.off[p + 1]) return HSPF_E_INVAL;
+        hl_route_net6 o{};
+        o.prefix = t.prefix6[p]; o.len = (uint8_t)t.plen[p];
+        o.flags = (c.flags & HL_CELL_CONNECTED) ? HL_ROUTE_CONNECTED : 0;
+        o.origin_type = t.origin_type[c.winner]; o.prefix_options = t.options6[c.winner]; o.metric = c.metric;
+        o.origin_adv_rtr = t.origin_adv[c.winner]; o.origin_lsa_id = t.contribs[c.winner].origin_id;
+        if (!atom_hops(*jd.rs, c.nh_mask, set)) return HSPF_E_UNSUPPORTED;
+        if (set.size() > a->max_paths) set.resize(a->max_paths);
+        o.nh_off = n_nh; o.n_nh = (uint32_t)set.size();
+        if (n_routes < out->routes_cap && n_nh + set.size() <= out->nexthops_cap) {
+            out->routes[n_routes] = o;
+            uint32_t h = n_nh;
+            for (const Nh6 &x : set) {
+                hl_nexthop6 q{};
+                q.iface = x.iface; q.nbr_router_id = x.has_nbr ? x.nbr : 0;
+                if (x.has_addr) q.addr = x.addr;
+                q.has_addr = x.has_addr; q.has_nbr = x.has_nbr;
+                out->nexthops[h++] = q;
+            }
+        }
+        ++n_routes; n_nh += (uint32_t)set.size();
+    }
+    out->n_routes = n_routes; out->n_nexthops = n_nh;
+    if (n_routes > out->routes_cap || n_nh > out->nexthops_cap) return HSPF_E_NOMEM;
+    return HSPF_OK;
+}
+
+// the OSPFv3 side of hspf::build_rib_records (ospf_ribtable.h): rib_full<V3> of ospf_rib_host.cc
+struct RibV3 {
+    using Key = std::array<uint8_t, 17>;                  // 16 address bytes, then the length
+    using Sum = hl_ospfv3_inter_area_lsa;
+    using Ext = hl_ospfv3_external_lsa;
+    static constexpr bool kV3 = true;
+    static Key mk(const hl_ip_addr &a, uint8_t len) { Key k; std::memcpy(k.data(), a.bytes, 16); k[16] = len; return k; }
+    static Key key(const Sum &l) { return mk(l.prefix, l.len); }
+    static Key key(const Ext &l) { return mk(l.prefix, l.len); }
+    static Key intra_key(const hspf::RouteTable &t, uint32_t k) { return mk(t.prefix6[k], (uint8_t)t.plen[k]); }
+    static bool skip(const Sum &l) { return l.lsa_type == 3 && (l.prefix_options & HL_PFX_OPT_NU); }
+    static bool skip(const Ext &l) { return (l.prefix_options & HL_PFX_OPT_NU) != 0; }
+    static uint32_t asbr_id(const Sum &l) { return l.router_id; }
+    static uint8_t options(const Sum &l) { return l.prefix_options; }
+    static uint8_t options(const Ext &l) { return l.prefix_options; }
+    // the merged table names every prefix as an IPv6 network, as update_rib_full does
+    static void set_prefix(hspf_ospfv2_ribtable &rt, uint32_t u, const Key &k) {
+        hl_ip_addr &p = rt.prefix6[u];
+        std::memset(&p, 0, sizeof(p));
+        std::memcpy(p.bytes, k.data(), 16);
+        p.is_v6 = 1;
+        rt.prefix[u] = 0; rt.plen[u] = k[16];
+    }
+};
+
+}  // namespace
+
+extern "C" {
+
 int hspf_ospfv3_routes_from_cells(const hl_ospfv3_area *a, const hspf_ospfv2_rtable *rt, const hl_route_cell *cells,
                                   const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv3_result *out) {
     if (!a || !rt || !rt->t.v3 || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
@@ -642,68 +758,137 @@ int hspf_ospfv3_routes_from_cells(const hl_ospfv3_area *a, const hspf_ospfv2_rta
         out->n_vertices = out->n_routers = out->n_routes = out->n_nexthops = 0;
         out->transit_capability = 0;
         out->root_found = 0;
-        hspf_ospfv3_flat f;
-        int rc = flatten(a, f);
-        if (rc) return rc;
-        const uint32_t V = (uint32_t)f.rid.size();
-        if (V != rt->t.n_vertices) return HSPF_E_INVAL;                   // not the LSDB the table was built from
-        auto rit = f.rtr_vertex.find(a->router_id);
-        if (rit == f.rtr_vertex.end()) return HSPF_OK;
+        JobDecode jd;
+        const int rc = jd.init(a, rt->t.n_vertices, gather_v, gather_nh, n_gather);
+        if (rc || jd.root == kNone) return rc;
         out->root_found = 1;
-        std::vector<uint64_t> sparse_nh(V, 0);                             // only the transit networks next to the root are read
-        for (uint32_t i = 0; i < n_gather; ++i) {
-            if (gather_v[i] >= V) return HSPF_E_INVAL;
-            sparse_nh[gather_v[i]] = gather_nh[i];
+        return intra_from_cells(jd, a, rt, cells, out);
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+
+/* ---- batched routing-table stage for roots attached to one OSPFv3 area (ospf_rib_cells.h) ------------------- */
+
+int hspf_ospfv3_ribtable_create(const hspf_ospfv3_flat *flat, uint32_t area_id, const hl_ospfv3_inter_area_lsa *sums,
+                                uint32_t n_sums, const hl_ospfv3_external_lsa *ext, uint32_t n_ext,
+                                hspf_ospfv2_ribtable **out) {
+    if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext)) return HSPF_E_INVAL;
+    *out = nullptr;
+    try {
+        const hspf_ospfv3_flat &f = *flat;
+        const hl_ospfv3_area *a = f.area;
+        const uint32_t V = (uint32_t)f.rid.size();
+        std::unique_ptr<hspf_ospfv2_ribtable, void (*)(hspf_ospfv2_ribtable *)> rt(new hspf_ospfv2_ribtable(),
+                                                                                   hspf_ospfv2_ribtable_free);
+        // a router vertex's flags are its first fragment's, as the intra-area stage reads them
+        rt->vflags.assign(V, 0);
+        for (uint32_t v = 0; v < V; ++v)
+            if (f.is_router[v]) rt->vflags[v] = a->router_lsas[f.first_lsa[v]].flags;
+        int rc = hspf_ospfv3_rtable_create(flat, &rt->intra);
+        if (rc) return rc;
+        auto router_vertex = [&](uint32_t id) {
+            auto it = f.rtr_vertex.find(id);
+            return it == f.rtr_vertex.end() ? kNone : it->second;
+        };
+        rc = hspf::build_rib_records<RibV3>(*rt, area_id, router_vertex, sums, n_sums, ext, n_ext);
+        if (rc) return rc;
+        *out = rt.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_UNSUPPORTED; }
+}
+
+int hspf_ospfv3_ribtable_prefixes6(const hspf_ospfv2_ribtable *rt, const hl_ip_addr **prefixes, const uint32_t **lens) {
+    if (!rt || !rt->v3) return HSPF_E_INVAL;
+    if (prefixes) *prefixes = rt->prefix6.data();
+    if (lens) *lens = rt->plen.data();
+    return HSPF_OK;
+}
+
+int hspf_ospfv3_rib_from_cells(const hl_ospfv3_area *a, const hspf_ospfv2_ribtable *rt, const hl_ospf_rib_cell *cells,
+                               const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv3_rib *out) {
+    if (!a || !rt || !rt->v3 || !rt->intra || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
+    try {
+        out->n_routes = out->n_nexthops = 0;
+        JobDecode jd;
+        int rc = jd.init(a, (uint32_t)rt->vflags.size(), gather_v, gather_nh, n_gather);
+        if (rc) return rc;
+        if (jd.root == kNone) return HSPF_E_INVAL;                  // not the root of any job over this table
+        const uint32_t P = (uint32_t)rt->prefix6.size(), PI = (uint32_t)rt->intra->t.prefix6.size();
+        const uint32_t *o3 = rt->off.data() + P + 1, *o5 = o3 + P + 1;
+        // 1. the intra-area cells, through the intra-area decode
+        std::vector<hl_route_cell> ic(PI, hl_route_cell{0, 0, kNone, 0, 0, 0});
+        for (uint32_t u = 0; u < P; ++u) {
+            const hl_ospf_rib_cell &c = cells[u];
+            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(c) != HL_PATH_INTRA_AREA) continue;
+            if (rt->intra_of[u] == kNone || HL_RIB_CELL_METRIC(c) > 0xFFFFu) return HSPF_E_INVAL;
+            ic[rt->intra_of[u]] = hl_route_cell{c.nh_mask, c.aux, c.winner, (uint16_t)HL_RIB_CELL_METRIC(c),
+                                                (uint8_t)HL_RIB_CELL_FLAGS(c), 0};
         }
-        Resolver rs{f, a, rit->second, sparse_nh.data(), 1, {}, {}};
-        rs.atom_nh.resize(64);
-        rs.atom_done.assign(64, 0);
-        const auto &t = rt->t;
-        const uint32_t P = (uint32_t)t.prefix6.size();
-        uint32_t n_routes = 0, n_nh = 0;
+        std::vector<hl_route_net6> nets(PI);
+        std::vector<hl_nexthop6> nh(std::max<size_t>(64, (size_t)PI * 2));
+        hl_ospfv3_result res{};
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            res = hl_ospfv3_result{};
+            res.routes_cap = PI; res.routes = nets.data();
+            res.nexthops_cap = (uint32_t)nh.size(); res.nexthops = nh.data();
+            rc = intra_from_cells(jd, a, rt->intra, ic.data(), &res);
+            if (rc != HSPF_E_NOMEM) break;
+            nh.resize(res.n_nexthops);
+        }
+        if (rc) return rc;
+        // 2. every route in prefix order; inter-area and external next hops from the cell's atoms
+        std::vector<hl_rib_route6> routes;
+        std::vector<hl_nexthop6> hops;
         std::vector<Nh6> set;
-        for (uint32_t p = 0; p < P; ++p) {
-            const hl_route_cell &c = cells[p];
-            if (!(c.flags & HL_CELL_PRESENT)) continue;
-            if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
-            if (c.winner < t.off[p] || c.winner >= t.off[p + 1]) return HSPF_E_INVAL;
-            hl_route_net6 o{};
-            o.prefix = t.prefix6[p]; o.len = (uint8_t)t.plen[p];
-            o.flags = (c.flags & HL_CELL_CONNECTED) ? HL_ROUTE_CONNECTED : 0;
-            o.origin_type = t.origin_type[c.winner]; o.prefix_options = t.options6[c.winner]; o.metric = c.metric;
-            o.origin_adv_rtr = t.origin_adv[c.winner]; o.origin_lsa_id = t.contribs[c.winner].origin_id;
-            set.clear();
-            uint64_t m = c.nh_mask;
-            while (m) {
-                const uint32_t atom = (uint32_t)__builtin_ctzll(m);
-                m &= m - 1;
-                for (const Nh6 &x : rs.resolve(atom)) {
-                    auto it = std::lower_bound(set.begin(), set.end(), x, nh_less);
-                    if (it != set.end() && nh_same(*it, x)) {
-                        // same NexthopKey from another atom: the reference keeps the later advertiser's; both must agree
-                        if (it->iface != x.iface || it->has_nbr != x.has_nbr || (x.has_nbr && it->nbr != x.nbr)) return HSPF_E_UNSUPPORTED;
-                    } else {
-                        set.insert(it, x);
-                    }
+        auto sort_key = [&](uint32_t iface) { return iface < a->n_ifaces ? a->ifaces[iface].sort_key : 0xFFFFFFFFu; };
+        uint32_t ri = 0;
+        for (uint32_t u = 0; u < P; ++u) {
+            const hl_ospf_rib_cell &c = cells[u];
+            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT)) continue;
+            const uint32_t path = HL_RIB_CELL_PATH(c);
+            hl_rib_route6 o;
+            std::memset(&o, 0, sizeof(o));
+            o.prefix = rt->prefix6[u]; o.len = (uint8_t)rt->plen[u];
+            o.path_type = (uint8_t)path;
+            o.nh_off = (uint32_t)hops.size();
+            if (path == HL_PATH_INTRA_AREA) {
+                if (ri >= res.n_routes) return HSPF_E_INVAL;
+                const hl_route_net6 &r = nets[ri++];
+                o.metric = r.metric; o.area_id = rt->area_id; o.has_area = 1; o.flags = r.flags;
+                o.prefix_options = r.prefix_options;
+                for (uint32_t k = 0; k < r.n_nh; ++k) {
+                    hl_nexthop6 h = nh[r.nh_off + k];
+                    h.iface = sort_key(h.iface);                      // the merged table names interfaces by sort key
+                    hops.push_back(h);
                 }
-            }
-            if (set.size() > a->max_paths) set.resize(a->max_paths);
-            o.nh_off = n_nh; o.n_nh = (uint32_t)set.size();
-            if (n_routes < out->routes_cap && n_nh + set.size() <= out->nexthops_cap) {
-                out->routes[n_routes] = o;
-                uint32_t h = n_nh;
+            } else {
+                const bool inter = path == HL_PATH_INTER_AREA;
+                if (inter ? (c.winner < o3[u] || c.winner >= o3[u + 1]) : (c.winner < o5[u] || c.winner >= o5[u + 1]))
+                    return HSPF_E_INVAL;
+                o.metric = HL_RIB_CELL_METRIC(c);
+                o.prefix_options = rt->options6[c.winner - rt->n_intra];
+                if (inter) { o.area_id = rt->area_id; o.has_area = 1; }
+                else o.tag = rt->ext_tag[c.winner - rt->ext_base];
+                if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
+                if (!atom_hops(*jd.rs, c.nh_mask, set)) return HSPF_E_UNSUPPORTED;
+                if (set.size() > a->max_paths) set.resize(a->max_paths);
                 for (const Nh6 &x : set) {
-                    hl_nexthop6 q{};
-                    q.iface = x.iface; q.nbr_router_id = x.has_nbr ? x.nbr : 0;
-                    if (x.has_addr) q.addr = x.addr;
-                    q.has_addr = x.has_addr; q.has_nbr = x.has_nbr;
-                    out->nexthops[h++] = q;
+                    hl_nexthop6 h{};
+                    h.iface = sort_key(x.iface); h.nbr_router_id = x.has_nbr ? x.nbr : 0;
+                    if (x.has_addr) h.addr = x.addr;
+                    h.has_addr = x.has_addr; h.has_nbr = x.has_nbr;
+                    hops.push_back(h);
                 }
             }
-            ++n_routes; n_nh += (uint32_t)set.size();
+            o.n_nh = (uint32_t)hops.size() - o.nh_off;
+            routes.push_back(o);
         }
-        out->n_routes = n_routes; out->n_nexthops = n_nh;
-        if (n_routes > out->routes_cap || n_nh > out->nexthops_cap) return HSPF_E_NOMEM;
+        out->n_routes = (uint32_t)routes.size();
+        out->n_nexthops = (uint32_t)hops.size();
+        if (out->n_routes > out->routes_cap || out->n_nexthops > out->nexthops_cap) return HSPF_E_NOMEM;
+        if ((out->n_routes && !out->routes) || (out->n_nexthops && !out->nexthops)) return HSPF_E_INVAL;
+        std::copy(routes.begin(), routes.end(), out->routes);
+        std::copy(hops.begin(), hops.end(), out->nexthops);
         return HSPF_OK;
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
 }

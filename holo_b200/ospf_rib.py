@@ -338,22 +338,36 @@ def cell_flags(cells):
 class RibTable(route_table.RouteTable):
     """hspf_ospfv2_ribtable: the area's intra-area, type-3 and type-5 prefixes in prefix order and, per prefix,
     its intra-area advertisers, type-3 and type-5 records (host); `off` holds the three ranges per prefix
-    ([3, P + 1]).  `upload(ctx)` copies it to the device for hspf_ospfv2_rib_cells."""
+    ([3, P + 1]).  `upload(ctx)` copies it to the device for hspf_ospfv2_rib_cells.
+
+    From an ospfv3.Flat the table is hspf_ospfv3_ribtable_create's (summaries: INTER_AREA_LSA_DT, externals:
+    EXTERNAL6_LSA_DT); `prefix` then holds the IPv6 prefixes (ospfv3.IP_DT) and `v3` is set."""
 
     api, kind, contrib_dt = "hspf_ospfv2", "ribtable", RIB_RECORD_DT
 
-    def __init__(self, flat: ospfv2.Flat, area_id: int, summaries=None, externals=None):
+    def __init__(self, flat, area_id: int, summaries=None, externals=None):
+        from . import ospfv3
         self.flat = flat
-        sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
-        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        self.v3 = isinstance(flat, ospfv3.Flat)
+        sum_dt, ext_dt = (INTER_AREA_LSA_DT, EXTERNAL6_LSA_DT) if self.v3 else (SUMMARY_LSA_DT, EXTERNAL_LSA_DT)
+        sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, sum_dt), sum_dt)
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, ext_dt), ext_dt)
         self.area_id, self.summaries, self.externals = area_id, sm, ext
-        super().__init__(capi.load_library().hspf_ospfv2_ribtable_create, flat.handle, area_id,
-                         sm.ctypes.data if len(sm) else None, len(sm), ext.ctypes.data if len(ext) else None, len(ext))
+        lib = capi.load_library()
+        super().__init__(lib.hspf_ospfv3_ribtable_create if self.v3 else lib.hspf_ospfv2_ribtable_create, flat.handle,
+                         area_id, sm.ctypes.data if len(sm) else None, len(sm), ext.ctypes.data if len(ext) else None,
+                         len(ext))
         pp, pl, po = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)()
         self._call("arrays", C.byref(pp), C.byref(pl), C.byref(po), None)
         self.prefix = route_table.copy_records(pp, self.n_prefixes, np.uint32)
         self.plen = route_table.copy_records(pl, self.n_prefixes, np.uint32)
         self.off = route_table.copy_records(po, 3 * (self.n_prefixes + 1), np.uint32).reshape(3, self.n_prefixes + 1)
+        if self.v3:
+            p6 = C.c_void_p()
+            rc = lib.hspf_ospfv3_ribtable_prefixes6(self.handle, C.byref(p6), None)
+            if rc != capi.HSPF_OK:
+                raise capi.HspfError(rc, "hspf_ospfv3_ribtable_prefixes6 failed")
+            self.prefix = route_table.copy_records(p6, self.n_prefixes, ospfv3.IP_DT)
 
 
 def rib_cells_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr: int, cells_ptr: int,
@@ -374,8 +388,8 @@ def rib_cells_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr
 
 def rib_delta_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr: int, base_ptr: int, n_base: int,
                      base_of_ptr: int, job_out_ptr: int, records_ptr: int, cap: int, n_records_ptr: int):
-    """hspf_ospfv2_rib_delta / _delta16 over DEVICE planes (rs and roots_ptr as for rib_cells_device): each job's cells
-    compared with its base row of base_ptr ([n_base, rt.n_prefixes] RIB_CELL_DT, normally rib_cells_device over the
+    """hspf_ospfv2_rib_delta / _delta16 over DEVICE planes (rs and roots_ptr as for rib_cells_device; rt an OSPFv2 or
+    OSPFv3 RibTable): each job's cells compared with its base row of base_ptr ([n_base, rt.n_prefixes] RIB_CELL_DT, normally rib_cells_device over the
     unperturbed job of the same root; base_of_ptr: [n_jobs] u32 rows, 0 for row 0 of every job), without storing them.
     job_out_ptr: [n_jobs] route_table.DELTA_JOB_DT; records_ptr: [cap] route_table.DELTA_DT in (job, prefix) order
     (0 or cap 0: summaries only); n_records_ptr: u64 total.  All device pointers; enqueued on the ctx stream."""
@@ -388,11 +402,7 @@ def rib_delta_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr
         raise capi.HspfError(rc, ctx.last_error())
 
 
-def rib_from_cells(area: ospfv2.Ospfv2Area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
-    """hspf_ospfv2_rib_from_cells (host): one job's cells -> the routing table update_rib_full gives for
-    area.router_id over its one area.  rc HSPF_E_UNSUPPORTED is returned in the result (caller: the host
-    stages over that job's planes)."""
-    lib = capi.load_library()
+def _call_rib_from_cells(fn, area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh, route_dt, nh_dt) -> Rib:
     cells = np.ascontiguousarray(cells, RIB_CELL_DT)
     assert cells.shape == (rt.n_prefixes,)
     gv = np.ascontiguousarray(gather_v, np.uint32)
@@ -400,16 +410,33 @@ def rib_from_cells(area: ospfv2.Ospfv2Area, rt: RibTable, cells: np.ndarray, gat
     s = area.as_struct()
     caps = [max(rt.n_prefixes, 1), max(4 * rt.n_prefixes, 64)]
     for _ in range(2):
-        routes, nhs = np.zeros(caps[0], RIB_ROUTE_DT), np.zeros(caps[1], ospfv2.NEXTHOP_DT)
+        routes, nhs = np.zeros(caps[0], route_dt), np.zeros(caps[1], nh_dt)
         r = RibStruct(caps[0], 0, routes.ctypes.data, caps[1], 0, nhs.ctypes.data)
-        rc = lib.hspf_ospfv2_rib_from_cells(C.byref(s), rt.handle, cells.ctypes.data, gv.ctypes.data_as(C.POINTER(C.c_uint32)),
-                                            gn.ctypes.data_as(C.POINTER(C.c_uint64)), len(gv), C.byref(r))
+        rc = fn(C.byref(s), rt.handle, cells.ctypes.data, gv.ctypes.data_as(C.POINTER(C.c_uint32)),
+                gn.ctypes.data_as(C.POINTER(C.c_uint64)), len(gv), C.byref(r))
         if rc == capi.HSPF_E_NOMEM:
             caps = [max(caps[0], r.n_routes), max(caps[1], r.n_nexthops)]
             continue
         break
     if rc not in (capi.HSPF_OK, capi.HSPF_E_UNSUPPORTED):
-        raise capi.HspfError(rc, "hspf_ospfv2_rib_from_cells failed")
+        raise capi.HspfError(rc, fn.__name__ + " failed")
     if rc != capi.HSPF_OK:
-        return Rib(np.zeros(0, RIB_ROUTE_DT), np.zeros(0, ospfv2.NEXTHOP_DT), rc)
+        return Rib(np.zeros(0, route_dt), np.zeros(0, nh_dt), rc)
     return Rib(routes[: r.n_routes].copy(), nhs[: r.n_nexthops].copy(), rc)
+
+
+def rib_from_cells(area: ospfv2.Ospfv2Area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv2_rib_from_cells (host): one job's cells -> the routing table update_rib_full gives for
+    area.router_id over its one area.  rc HSPF_E_UNSUPPORTED is returned in the result (caller: the host
+    stages over that job's planes)."""
+    return _call_rib_from_cells(capi.load_library().hspf_ospfv2_rib_from_cells, area, rt, cells, gather_v, gather_nh,
+                                RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)
+
+
+def rib_from_cells_v3(area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv3_rib_from_cells (host): one job's cells over an OSPFv3 RibTable -> the routing table
+    update_rib_full_v3 gives for area.router_id (an ospfv3.Ospfv3Area) over its one area (RIB_ROUTE6_DT routes,
+    ospfv3.NEXTHOP6_DT next hops).  rc HSPF_E_UNSUPPORTED is returned in the result, as rib_from_cells."""
+    from . import ospfv3
+    return _call_rib_from_cells(capi.load_library().hspf_ospfv3_rib_from_cells, area, rt, cells, gather_v, gather_nh,
+                                RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)

@@ -417,3 +417,76 @@ def synth_area(t: Topology, root: int = 0, max_links_per_fragment: int = 0, max_
     area.link_lsas = la
     area.ifnames = [f"if{int(x[0])}" for x in ifaces]
     return area
+
+
+def inter_area_view(area: Ospfv3Area, seed: int, n_abr: int = 4, n_asbr: int = 3, n_inter: int = 60, n_ext: int = 50,
+                    unreachable_abr: bool = True, n_overlap: int = 8, n_fresh: int = 10, n_ext_only: int = 8,
+                    nu_fraction: float = 0.08):
+    """The OSPFv3 twin of ospfv2.inter_area_view: a single-area LSDB as one area of a multi-area domain, returned as
+    (area, inter-area LSAs, AS-external LSAs) for ospf_rib (ospf_rib.INTER_AREA_LSA_DT in LsaKey order,
+    ospf_rib.EXTERNAL6_LSA_DT in LSDB order).  Seeded and independent of area.router_id.
+      * n_abr routers get the B flag, n_asbr others the E flag (on every Router-LSA fragment of the router); with
+        unreachable_abr a router with B|E and no links is added;
+      * Inter-Area-Prefix LSAs from the ABRs (and from a router without the B flag and an unknown router) for
+        intra-area prefixes, new prefixes, prefixes with host bits and the default route; Inter-Area-Router LSAs for
+        in-area ASBRs and ASBRs outside the area, naming the ASBR in router_id (lsa_id is an unrelated number);
+        AS-external LSAs of type 1 and 2 from those ASBRs, from routers without the E flag, from unknown routers and
+        from ordinary routers;
+      * a nu_fraction of the Inter-Area-Prefix, Inter-Area-Router and AS-external LSAs carry the NU option (only the
+        first and last kinds are skipped for it);
+      * metrics from small sets, so that ties are common; some LSAs at maxage or at LSInfinity."""
+    from . import ospf_rib
+    rng = np.random.default_rng(seed)
+    a = Ospfv3Area(**{k: getattr(area, k) for k in area.__dataclass_fields__})
+    rl = area.router_lsas.copy()
+    rids = sorted({int(x) for x in rl["adv_rtr"]})
+    pick = [int(x) for x in rng.permutation(rids)]
+    abrs, asbrs, plain = pick[:n_abr], pick[n_abr:n_abr + n_asbr], pick[n_abr + n_asbr:]
+    for i in range(len(rl)):
+        r = int(rl["adv_rtr"][i])
+        rl["flags"][i] |= (0x01 if r in abrs else 0) | (0x02 if r in asbrs else 0)
+    lost = []
+    if unreachable_abr:
+        lost = [max(rids) + 0x100]
+        rl = np.concatenate([rl, np.array([(lost[0], 0, 1, 0x03, OPT_R | OPT_V6, len(area.links), 0)], ROUTER_LSA_DT)])
+    a.router_lsas = rl
+    own = sorted({(bytes(int(b) for b in p["addr"]["bytes"]), int(p["len"])) for p in area.prefixes
+                  if not int(p["options"]) & PFX_NU})
+    six = lambda hi, lo=0: ipaddress.IPv6Address((0x20010DB8 << 96) | (hi << 64) | lo).packed
+    intra = [own[int(i)] for i in rng.choice(len(own), min(len(own), n_overlap), replace=False)]
+    fresh = [(six(0xC8_0000 + i), 64) for i in range(n_fresh)]
+    pool = intra + fresh + [(six(0xC8_0000, 5), 64), (six(0xC8_0001, 5), 64), (bytes(16), 0)]
+    metric = lambda: int(rng.choice([1, 10, 10, 20, 30])) if rng.random() > 0.05 else ospf_rib.LSA_INFINITY
+    maxage = lambda: int(rng.random() < 0.06)
+    nu = lambda: PFX_NU if rng.random() < nu_fraction else 0
+    rec = lambda b: (tuple(b), 1, (0, 0, 0))
+    sums, ids = [], {}
+    next_id = lambda adv: ids.__setitem__(adv, ids.get(adv, 0) + 1) or ids[adv]
+    advs3 = abrs + lost + plain[:1] + [0x7F000001]                # the last two: never an ABR of the area
+    for _ in range(n_inter):
+        p, ln = pool[int(rng.integers(0, len(pool)))]
+        adv = int(rng.choice(advs3))
+        sums.append((adv, next_id(adv), metric(), 0, rec(p), ln, nu(), 3, maxage()))
+    outside = [0x0B000001 + i for i in range(3)]                  # ASBRs in other areas
+    for asbr in asbrs[:2] + outside:
+        for abr in rng.choice(abrs + lost, int(rng.integers(1, 4)), replace=False):
+            sums.append((int(abr), next_id(int(abr)), metric(), asbr, rec(bytes(16)), 0, nu(), 4, maxage()))
+    sums.sort(key=lambda x: (x[7], x[0], x[1]))
+    summaries = np.zeros(len(sums), ospf_rib.INTER_AREA_LSA_DT)
+    for i, x in enumerate(sums):
+        summaries[i] = x
+    ext = []
+    advs5 = asbrs + outside + lost + plain[:3] + abrs[:1] + [0x7F000002]
+    only5 = [(six(0xC0_0000 + i), 64) for i in range(n_ext_only)]  # prefixes only externals name
+    pool5 = pool + only5
+    for _ in range(n_ext):
+        p, ln = pool5[int(rng.integers(0, len(pool5)))]
+        e_bit = 1 if (p, ln) in only5[:4] else int(rng.integers(0, 2))   # four prefixes of type-2 LSAs only
+        adv = int(rng.choice(advs5))
+        ext.append((adv, next_id(adv), int(rng.choice([1, 5, 5, 20])) if rng.random() > 0.05 else ospf_rib.LSA_INFINITY,
+                    int(rng.integers(0, 4)), rec(p), ln, nu(), e_bit, maxage()))
+    ext.sort(key=lambda x: (x[0], x[1]))
+    externals = np.zeros(len(ext), ospf_rib.EXTERNAL6_LSA_DT)
+    for i, x in enumerate(ext):
+        externals[i] = x
+    return a, summaries, externals

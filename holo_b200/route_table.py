@@ -103,6 +103,9 @@ def declare(lib: C.CDLL):
         "hspf_ospfv2_rib_delta": [vp, vp, u32, res, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv2_rib_delta16": [vp, vp, u32, res16, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv2_rib_from_cells": [C.POINTER(ospfv2.AreaStruct), vp, vp, u32p, u64p, u32, C.POINTER(ospf_rib.RibStruct)],
+        "hspf_ospfv3_ribtable_create": [vp, u32, vp, u32, vp, u32, pvp],
+        "hspf_ospfv3_ribtable_prefixes6": [vp, pvp, C.POINTER(u32p)],
+        "hspf_ospfv3_rib_from_cells": [C.POINTER(ospfv3.AreaStruct), vp, vp, u32p, u64p, u32, C.POINTER(ospf_rib.RibStruct)],
     }
     for name, argtypes in sigs.items():
         getattr(lib, name).argtypes = argtypes

@@ -200,7 +200,8 @@ int hspf_ospfv2_routes_from_cells(const hl_ospfv2_area *area, const hspf_ospfv2_
  *   hspf_ospfv2_ribtable_arrays  prefix[P], plen[P], off[3 (P + 1)] (intra, type-3, type-5 ranges), the 16-byte
  *                                records (ospf_rib_cells.h); any pointer may be NULL.
  *   hspf_ospfv2_ribtable_upload  copies the table to the ctx's device.
- *   hspf_ospfv2_rib_cells        one thread per (job, prefix) over DEVICE planes as hspf_ospfv2_routes_batch[16];
+ *   hspf_ospfv2_rib_cells        one thread per (job, prefix) over DEVICE planes as hspf_ospfv2_routes_batch[16],
+ *                                for OSPFv2 tables and the OSPFv3 tables of hspf_ospfv3_ribtable_create;
  *   hspf_ospfv2_rib_cells16      roots: device u32[n_jobs], each job's root vertex; cells[n_jobs][P] (device).
  *                                job_status_out (device u32[n_jobs], may be NULL): the planes' status word, plus
  *                                HSPF_JS_INVALID for a root >= V and HSPF_JS_NOT_INTERNAL for a root with the B
@@ -292,6 +293,32 @@ int hspf_ospfv3_rtable_prefixes6(const hspf_ospfv2_rtable *rt, const hl_ip_addr 
 int hspf_ospfv3_routes_from_cells(const hl_ospfv3_area *area, const hspf_ospfv2_rtable *rt, const hl_route_cell *cells,
                                   const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather,
                                   hl_ospfv3_result *out);
+/* The batched routing-table stage for OSPFv3 areas (see "Batched routing-table stage" above): for job j with root
+ * router r over area A, the decoded cells of j equal
+ *     hspf_ospfv3_update_rib_full(r, A.max_paths, [{A.area_id, spf_j, A.ifaces, summaries, active = 1}], externals)
+ * with spf_j = hspf_ospfv3_area_from_planes(A with router_id = r, j's planes): routes (prefix options, tag, type-2
+ * metric, area) and next hops.
+ *   hspf_ospfv3_ribtable_create   the same hspf_ospfv2_ribtable: the intra-area records of hspf_ospfv3_rtable_create,
+ *                                 then the type-3 / type-5 / ASBR-slot / type-4 records, as hspf_ospfv2_ribtable_create
+ *                                 builds them, with the rules of hspf_ospfv3_update_rib_full: an Inter-Area-Prefix or
+ *                                 AS-external LSA with the NU option is left out, an Inter-Area-Router LSA names its
+ *                                 ASBR in router_id, and prefixes are ordered by their 16 address bytes, then length.
+ *                                 summaries: the area's Inter-Area-Prefix / Inter-Area-Router LSAs (LsaKey order);
+ *                                 externals: the instance's AS-external LSAs.  A router vertex's flags are those of its
+ *                                 first Router-LSA fragment.  The same two HSPF_E_UNSUPPORTED refusals as OSPFv2.
+ *                                 hspf_ospfv2_ribtable_free / _prefixes / _contributors / _arrays (prefix[] all zero) /
+ *                                 _upload and hspf_ospfv2_rib_cells[16] / hspf_ospfv2_rib_delta[16] take it unchanged.
+ *   hspf_ospfv3_ribtable_prefixes6  the table's prefixes (IPv6 networks, as update_rib_full names them) and lengths.
+ *   hspf_ospfv3_rib_from_cells    host: one job's cells -> the table above, as hspf_ospfv2_rib_from_cells (next hops
+ *                                 named by interface sort key in NexthopKey order, HSPF_E_NOMEM with the counts,
+ *                                 HSPF_E_UNSUPPORTED in the cases of hspf_ospfv3_routes_from_cells).  HSPF_E_INVAL for
+ *                                 an OSPFv2 table, as hspf_ospfv2_rib_from_cells gives for an OSPFv3 one. */
+int hspf_ospfv3_ribtable_create(const hspf_ospfv3_flat *flat, uint32_t area_id, const hl_ospfv3_inter_area_lsa *summaries,
+                                uint32_t n_summaries, const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
+                                hspf_ospfv2_ribtable **out);
+int hspf_ospfv3_ribtable_prefixes6(const hspf_ospfv2_ribtable *rt, const hl_ip_addr **prefixes, const uint32_t **lens);
+int hspf_ospfv3_rib_from_cells(const hl_ospfv3_area *area, const hspf_ospfv2_ribtable *rt, const hl_ospf_rib_cell *cells,
+                               const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv3_rib *out);
 /* Ospfv3::spf_computation_type (holo-ospf/src/ospfv3/spf.rs:96-162): Router-, Network-, Link- and Router-Information
  * LSAs ask for a full run; otherwise the run is partial over the prefixes of the changed Intra-Area-Prefix (old and
  * new instance), Inter-Area-Prefix and AS-external LSAs and the routers of the changed Inter-Area-Router LSAs.
@@ -430,7 +457,7 @@ int hspf_isis_routes_from_cells(const hl_isis_instance *inst, const hspf_isis_rt
  *
  *   hspf_ospfv2_routes_delta[16]  OSPFv2 and OSPFv3 tables (as hspf_ospfv2_routes_batch[16]).
  *   hspf_isis_routes_delta[16]    IS-IS tables (as hspf_isis_routes_batch[16]).
- *   hspf_ospfv2_rib_delta[16]     OSPFv2 routing tables (as hspf_ospfv2_rib_cells[16]: the wide call needs
+ *   hspf_ospfv2_rib_delta[16]     OSPFv2 and OSPFv3 routing tables (as hspf_ospfv2_rib_cells[16]: the wide call needs
  *                                 nh_words == 1; roots: device u32[n_jobs], required when n_jobs > 0).  A job and
  *                                 its base row must share a root: atoms compare word for word only then.  The base
  *                                 row is normally hspf_ospfv2_rib_cells over the root's unperturbed job.
