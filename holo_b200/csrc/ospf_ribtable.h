@@ -26,10 +26,11 @@
 namespace hspf {
 
 // rt arrives with vflags filled and rt.intra built; `router_vertex(id)` is the vertex of router `id`, or
-// 0xFFFFFFFF.  Fills everything else; HSPF_E_UNSUPPORTED for the tables the walk cannot answer.
+// 0xFFFFFFFF.  Fills everything else; HSPF_E_UNSUPPORTED for the tables the walk cannot answer.  `transit_walk`:
+// the table is one area of an ABR's table (ospf_abr_rib_cells.h), whose walk has the transit-area step.
 template <class T, class RouterVertex>
 int build_rib_records(hspf_ospfv2_ribtable &rt, uint32_t area_id, RouterVertex router_vertex, const typename T::Sum *sums,
-                      uint32_t n_sums, const typename T::Ext *ext, uint32_t n_ext) {
+                      uint32_t n_sums, const typename T::Ext *ext, uint32_t n_ext, bool transit_walk = false) {
     using Key = typename T::Key;
     constexpr uint32_t kNone = 0xFFFFFFFFu;
     // the largest metric a cell holds: a type-1 external behind a type-4 entry, over a distance below saturation
@@ -38,7 +39,7 @@ int build_rib_records(hspf_ospfv2_ribtable &rt, uint32_t area_id, RouterVertex r
     rt.v3 = T::kV3;
     const uint32_t V = (uint32_t)rt.vflags.size();
     // rib_full step 3 (transit areas) can rewrite the backbone's intra-area routes when it has virtual links
-    if (area_id == 0)
+    if (area_id == 0 && !transit_walk)
         for (uint32_t v = 0; v < V; ++v)
             if (rt.vflags[v] & HL_RTR_FLAG_V) return HSPF_E_UNSUPPORTED;
     auto has_flag = [&](uint32_t v, uint8_t flag) { return v != kNone && (rt.vflags[v] & flag) != 0; };

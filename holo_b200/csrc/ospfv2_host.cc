@@ -20,6 +20,7 @@
 #include <vector>
 
 #include "holo_spf_lsdb.h"
+#include "ospf_abr_rib_cells.h"
 #include "ospf_rib_cells.h"
 #include "ospf_ribtable.h"
 #include "route_cells.h"
@@ -1066,30 +1067,44 @@ void hspf_ospfv2_ribtable_free(hspf_ospfv2_ribtable *rt) {
     delete rt;
 }
 
+}  // extern "C" (reopened below)
+
+namespace {
+
+// hspf_ospfv2_ribtable_create after its argument checks; `transit_walk` as for hspf::build_rib_records
+int make_ribtable(const hspf_ospfv2_flat *flat, uint32_t area_id, const hl_ospfv2_summary_lsa *sums, uint32_t n_sums,
+                  const hl_ospfv2_external_lsa *ext, uint32_t n_ext, bool transit_walk, hspf_ospfv2_ribtable **out) {
+    const hspf_ospfv2_flat &f = *flat;
+    const hl_ospfv2_area *a = f.area;
+    const uint32_t V = (uint32_t)f.ids.size();
+    std::unique_ptr<hspf_ospfv2_ribtable, void (*)(hspf_ospfv2_ribtable *)> rt(new hspf_ospfv2_ribtable(),
+                                                                               hspf_ospfv2_ribtable_free);
+    rt->vflags.assign(V, 0);
+    for (uint32_t v = 0; v < V; ++v)
+        if (f.is_router[v]) rt->vflags[v] = a->router_lsas[f.lsa_of[v]].flags;
+    int rc = hspf_ospfv2_rtable_create(flat, &rt->intra);
+    if (rc) return rc;
+    auto router_vertex = [&](uint32_t id) {
+        auto it = f.rtr_vertex.find(id);
+        return it == f.rtr_vertex.end() ? kNone : it->second;
+    };
+    rc = hspf::build_rib_records<RibV2>(*rt, area_id, router_vertex, sums, n_sums, ext, n_ext, transit_walk);
+    if (rc) return rc;
+    *out = rt.release();
+    return HSPF_OK;
+}
+
+}  // namespace
+
+extern "C" {
+
 int hspf_ospfv2_ribtable_create(const hspf_ospfv2_flat *flat, uint32_t area_id, const hl_ospfv2_summary_lsa *sums,
                                 uint32_t n_sums, const hl_ospfv2_external_lsa *ext, uint32_t n_ext,
                                 hspf_ospfv2_ribtable **out) {
     if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext)) return HSPF_E_INVAL;
     *out = nullptr;
     try {
-        const hspf_ospfv2_flat &f = *flat;
-        const hl_ospfv2_area *a = f.area;
-        const uint32_t V = (uint32_t)f.ids.size();
-        std::unique_ptr<hspf_ospfv2_ribtable, void (*)(hspf_ospfv2_ribtable *)> rt(new hspf_ospfv2_ribtable(),
-                                                                                   hspf_ospfv2_ribtable_free);
-        rt->vflags.assign(V, 0);
-        for (uint32_t v = 0; v < V; ++v)
-            if (f.is_router[v]) rt->vflags[v] = a->router_lsas[f.lsa_of[v]].flags;
-        int rc = hspf_ospfv2_rtable_create(flat, &rt->intra);
-        if (rc) return rc;
-        auto router_vertex = [&](uint32_t id) {
-            auto it = f.rtr_vertex.find(id);
-            return it == f.rtr_vertex.end() ? kNone : it->second;
-        };
-        rc = hspf::build_rib_records<RibV2>(*rt, area_id, router_vertex, sums, n_sums, ext, n_ext);
-        if (rc) return rc;
-        *out = rt.release();
-        return HSPF_OK;
+        return make_ribtable(flat, area_id, sums, n_sums, ext, n_ext, false, out);
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;
     } catch (...) {
@@ -1191,6 +1206,342 @@ int hspf_ospfv2_rib_from_cells(const hl_ospfv2_area *a, const hspf_ospfv2_ribtab
                     h.has_addr = x.has_addr; h.has_nbr = x.has_nbr;
                     hops.push_back(h);
                 }
+            }
+            o.n_nh = (uint32_t)hops.size() - o.nh_off;
+            routes.push_back(o);
+        }
+        out->n_routes = (uint32_t)routes.size();
+        out->n_nexthops = (uint32_t)hops.size();
+        if (out->n_routes > out->routes_cap || out->n_nexthops > out->nexthops_cap) return HSPF_E_NOMEM;
+        if ((out->n_routes && !out->routes) || (out->n_nexthops && !out->nexthops)) return HSPF_E_INVAL;
+        std::copy(routes.begin(), routes.end(), out->routes);
+        std::copy(hops.begin(), hops.end(), out->nexthops);
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
+}
+
+
+/* ---- batched routing-table stage for area border routers (ospf_abr_rib_cells.h) --------------------- */
+
+void hspf_ospfv2_abr_ribtable_free(hspf_ospfv2_abr_ribtable *t) {
+    if (!t) return;
+    hspf::release_route_table(t->dev);
+    for (hspf_ospfv2_ribtable *a : t->area) hspf_ospfv2_ribtable_free(a);
+    delete t;
+}
+
+int hspf_ospfv2_abr_ribtable_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv2_flat *const *flats,
+                                    const uint32_t *area_ids, const hl_ospfv2_summary_lsa *const *summaries,
+                                    const uint32_t *n_summaries, const uint8_t *active,
+                                    const hl_ospfv2_external_lsa *ext, uint32_t n_ext, hspf_ospfv2_abr_ribtable **out) {
+    if (!out || !flats || !area_ids || n_areas == 0 || (n_ext && !ext)) return HSPF_E_INVAL;
+    *out = nullptr;
+    if (n_areas > hspf::kAbrMaxAreas) return HSPF_E_UNSUPPORTED;
+    for (uint32_t i = 0; i < n_areas; ++i) {
+        if (!flats[i] || !flats[i]->area) return HSPF_E_INVAL;
+        if (n_summaries && n_summaries[i] && (!summaries || !summaries[i])) return HSPF_E_INVAL;
+    }
+    try {
+        std::unique_ptr<hspf_ospfv2_abr_ribtable, void (*)(hspf_ospfv2_abr_ribtable *)> t(
+            new hspf_ospfv2_abr_ribtable(), hspf_ospfv2_abr_ribtable_free);
+        const uint32_t A = n_areas;
+        t->router_id = router_id;
+        t->n_areas = A;
+        uint32_t n_active = 0;
+        for (uint32_t i = 0; i < A; ++i) n_active += (!active || active[i]) ? 1u : 0u;
+        uint32_t atoms = 0;
+        for (uint32_t i = 0; i < A; ++i) {
+            const hspf_ospfv2_flat &f = *flats[i];
+            if (i == 0) t->max_paths = f.area->max_paths;
+            else if (f.area->max_paths != t->max_paths) return HSPF_E_INVAL;   // one instance, one max_paths
+            auto rit = f.rtr_vertex.find(router_id);
+            if (rit == f.rtr_vertex.end()) return HSPF_E_INVAL;                // the caller leaves that area out
+            const uint32_t root = rit->second;
+            hspf_csr c;
+            fill_csr(f, &c);
+            uint32_t na = 0;
+            int rc = hspf_atom_count(&c, root, &na);
+            if (rc) return rc;
+            t->base.push_back(na ? atoms : 0);
+            t->n_atoms.push_back(na);
+            atoms += na;
+            if (atoms > 64) return HSPF_E_UNSUPPORTED;                         // the cell's masks are 64 bits
+            // rib_full step 2 reads every area's summaries with one active area, else only the backbone's; the
+            // other areas' type-3 LSAs are still offered by the transit-area step
+            const bool step2 = n_active <= 1 || area_ids[i] == 0;
+            if (step2) t->step2 |= 1u << i;
+            const uint32_t ns = n_summaries ? n_summaries[i] : 0;
+            std::vector<hl_ospfv2_summary_lsa> sums;
+            for (uint32_t k = 0; k < ns; ++k)
+                if (step2 || summaries[i][k].lsa_type == 3) sums.push_back(summaries[i][k]);
+            hspf_ospfv2_ribtable *rt = nullptr;
+            rc = make_ribtable(flats[i], area_ids[i], sums.data(), (uint32_t)sums.size(), ext, n_ext, true, &rt);
+            if (rc) return rc;
+            t->area.push_back(rt);
+            t->area_id.push_back(area_ids[i]);
+            t->root.push_back(root);
+            t->n_vertices.push_back((uint32_t)f.ids.size());
+        }
+        // the prefixes: the union of the areas' in prefix order
+        std::vector<uint64_t> keys;
+        for (const hspf_ospfv2_ribtable *rt : t->area)
+            for (size_t u = 0; u < rt->prefix.size(); ++u) keys.push_back(pkey(rt->prefix[u], rt->plen[u]));
+        std::sort(keys.begin(), keys.end());
+        keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+        const uint32_t P = (uint32_t)keys.size(), S = P + 1;
+        t->prefix.resize(P); t->plen.resize(P);
+        for (uint32_t u = 0; u < P; ++u) { t->prefix[u] = (uint32_t)(keys[u] >> 8); t->plen[u] = (uint32_t)(keys[u] & 0xFF); }
+        t->area_prefix.assign(A, std::vector<uint32_t>(P, kNone));
+        std::vector<std::vector<uint32_t>> first_at(A, std::vector<uint32_t>(P));   // first area prefix >= keys[u]
+        for (uint32_t i = 0; i < A; ++i) {
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            uint32_t q = 0;
+            for (uint32_t u = 0; u < P; ++u) {
+                first_at[i][u] = q;
+                if (q < rt.prefix.size() && pkey(rt.prefix[q], rt.plen[q]) == keys[u]) t->area_prefix[i][u] = q++;
+            }
+        }
+        t->off.assign((2 * (size_t)A + 1) * S, 0);
+        uint32_t *o3 = t->off.data() + (size_t)A * S, *o5 = o3 + (size_t)A * S;
+        auto &recs = t->recs;
+        for (uint32_t i = 0; i < A; ++i) {                                  // intra-area records, area by area
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            const uint32_t b = (uint32_t)recs.size();
+            t->intra_base.push_back(b);
+            recs.insert(recs.end(), rt.recs.begin(), rt.recs.begin() + rt.n_intra);
+            for (uint32_t u = 0; u < P; ++u) t->off[i * S + u] = b + rt.off[first_at[i][u]];
+            t->off[i * S + P] = b + rt.n_intra;
+        }
+        for (uint32_t i = 0; i < A; ++i) {                                  // type-3, without the root's own
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            const uint32_t *a3 = rt.off.data() + rt.prefix.size() + 1;
+            t->t3_base.push_back((uint32_t)recs.size());
+            for (uint32_t u = 0; u < P; ++u) {
+                o3[i * S + u] = (uint32_t)recs.size();
+                const uint32_t q = t->area_prefix[i][u];
+                if (q == kNone) continue;
+                for (uint32_t k = a3[q]; k < a3[q + 1]; ++k)
+                    if (rt.recs[k].x != t->root[i]) recs.push_back(rt.recs[k]);
+            }
+            o3[i * S + P] = (uint32_t)recs.size();
+        }
+        t->t3_end = (uint32_t)recs.size();
+        // type-5: every area's table holds the same type-5 records in the same order (one external list, one filter);
+        // area 0's slot of a record names its ASBR, and each area's slot of that record gives that area's entry
+        const hspf_ospfv2_ribtable &r0 = *t->area[0];
+        const uint32_t N5 = r0.ext_end - r0.ext_base;
+        for (const hspf_ospfv2_ribtable *rt : t->area)
+            if (rt->ext_end - rt->ext_base != N5) return HSPF_E_INVAL;
+        std::unordered_map<uint32_t, uint32_t> group_of;                    // area 0's slot record -> group
+        std::vector<uint32_t> group_rep, rec_group;                         // a type-5 record of each group; group per record
+        t->ext_base = (uint32_t)recs.size();
+        const uint32_t *a5 = r0.off.data() + 2 * (r0.prefix.size() + 1);
+        for (uint32_t u = 0; u < P; ++u) {
+            o5[u] = (uint32_t)recs.size();
+            const uint32_t q = t->area_prefix[0][u];
+            if (q == kNone) continue;
+            for (uint32_t k = a5[q]; k < a5[q + 1]; ++k) {
+                const hspf::RibRec r = r0.recs[k];
+                if (r0.recs[r.x].x == t->root[0]) continue;                 // self-originated
+                auto ins = group_of.emplace(r.x, (uint32_t)group_rep.size());
+                if (ins.second) group_rep.push_back(k - r0.ext_base);
+                rec_group.push_back(ins.first->second);
+                recs.push_back(hspf::RibRec{0, r.y, r.z, 0});
+                t->ext_tag.push_back(r0.ext_tag[k - r0.ext_base]);
+            }
+        }
+        o5[P] = (uint32_t)recs.size();
+        t->ext_end = o5[P];
+        const uint32_t group_base = (uint32_t)recs.size(), G = (uint32_t)group_rep.size();
+        for (uint32_t k = 0; k < rec_group.size(); ++k) recs[t->ext_base + k].x = group_base + rec_group[k] * A;
+        recs.resize((size_t)group_base + (size_t)G * A);
+        for (uint32_t g = 0; g < G; ++g)
+            for (uint32_t i = 0; i < A; ++i) {
+                const hspf_ospfv2_ribtable &rt = *t->area[i];
+                const hspf::RibRec s = rt.recs[rt.recs[rt.ext_base + group_rep[g]].x];
+                const uint32_t z = (uint32_t)recs.size();
+                if ((t->step2 >> i) & 1u)
+                    for (uint32_t k = s.z; k < s.w; ++k)
+                        if (rt.recs[k].x != t->root[i]) recs.push_back(rt.recs[k]);
+                recs[group_base + g * A + i] = hspf::RibRec{s.x, s.y, z, (uint32_t)recs.size()};
+            }
+        if (recs.size() >= kNone) return HSPF_E_UNSUPPORTED;               // record indices are u32
+        t->vl_off.push_back(0);
+        for (uint32_t i = 0; i < A; ++i) {
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            for (uint32_t v = 0; v < rt.vflags.size(); ++v)
+                if (rt.vflags[v] & HL_RTR_FLAG_V) t->v_flagged.push_back(v);
+            t->vl_off.push_back((uint32_t)t->v_flagged.size());
+        }
+        *out = t.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_UNSUPPORTED;
+    }
+}
+
+uint32_t hspf_ospfv2_abr_ribtable_prefixes(const hspf_ospfv2_abr_ribtable *t) { return t ? (uint32_t)t->prefix.size() : 0; }
+uint32_t hspf_ospfv2_abr_ribtable_contributors(const hspf_ospfv2_abr_ribtable *t) { return t ? (uint32_t)t->recs.size() : 0; }
+
+int hspf_ospfv2_abr_ribtable_arrays(const hspf_ospfv2_abr_ribtable *t, const uint32_t **prefix, const uint32_t **plen,
+                                    const uint32_t **off, const void **records) {
+    if (!t) return HSPF_E_INVAL;
+    if (prefix) *prefix = t->prefix.data();
+    if (plen) *plen = t->plen.data();
+    if (off) *off = t->off.data();
+    if (records) *records = t->recs.data();
+    return HSPF_OK;
+}
+
+int hspf_ospfv2_abr_ribtable_areas(const hspf_ospfv2_abr_ribtable *t, uint32_t *root, uint32_t *n_vertices,
+                                   uint32_t *atom_base, uint32_t *n_atoms) {
+    if (!t) return HSPF_E_INVAL;
+    for (uint32_t i = 0; i < t->n_areas; ++i) {
+        if (root) root[i] = t->root[i];
+        if (n_vertices) n_vertices[i] = t->n_vertices[i];
+        if (atom_base) atom_base[i] = t->base[i];
+        if (n_atoms) n_atoms[i] = t->n_atoms[i];
+    }
+    return (int)t->n_areas;
+}
+
+int hspf_ospfv2_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_ospfv2_area *areas, uint32_t n_areas,
+                                   const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
+                                   const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv2_rib *out) {
+    if (!t || !areas || !cells || !out || n_areas != t->n_areas ||
+        (n_gather && (!gather_area || !gather_v || !gather_nh)))
+        return HSPF_E_INVAL;
+    try {
+        out->n_routes = out->n_nexthops = 0;
+        const uint32_t A = n_areas, P = (uint32_t)t->prefix.size(), S = P + 1;
+        const uint32_t *o3 = t->off.data() + (size_t)A * S, *o5 = o3 + (size_t)A * S;
+        std::vector<JobDecode> jd(A);
+        std::vector<uint64_t> amask(A);
+        for (uint32_t i = 0; i < A; ++i) {
+            const hl_ospfv2_area &a = areas[i];
+            if (a.router_id != t->router_id || a.area_id != t->area_id[i] || a.max_paths != t->max_paths) return HSPF_E_INVAL;
+            std::vector<uint32_t> gv;
+            std::vector<uint64_t> gn;
+            for (uint32_t g = 0; g < n_gather; ++g) {
+                if (gather_area[g] >= A) return HSPF_E_INVAL;
+                if (gather_area[g] == i) { gv.push_back(gather_v[g]); gn.push_back(gather_nh[g]); }
+            }
+            const int rc = jd[i].init(&a, t->n_vertices[i], gv.data(), gn.data(), (uint32_t)gv.size());
+            if (rc) return rc;
+            if (jd[i].root != t->root[i]) return HSPF_E_INVAL;
+            const uint32_t na = t->n_atoms[i];
+            amask[i] = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << t->base[i]);
+        }
+        auto intra_area = [&](uint32_t w) {
+            for (uint32_t i = 0; i < A; ++i)
+                if (w >= t->intra_base[i] && w < t->intra_base[i] + t->area[i]->n_intra) return i;
+            return kNone;
+        };
+        // 1. per area, the intra-area cells its records won, through the intra-area decode
+        std::vector<std::vector<hl_route_net>> nets(A);
+        std::vector<std::vector<hl_nexthop>> nh(A);
+        std::vector<hl_ospfv2_result> res(A);
+        for (uint32_t i = 0; i < A; ++i) {
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            const uint32_t PI = (uint32_t)rt.intra->t.prefix.size();
+            std::vector<hl_route_cell> ic(PI, hl_route_cell{0, 0, kNone, 0, 0, 0});
+            for (uint32_t u = 0; u < P; ++u) {
+                const hl_ospf_rib_cell &c = cells[u];
+                if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(c) != HL_PATH_INTRA_AREA) continue;
+                if (intra_area(c.winner) != i) continue;
+                const uint32_t q = t->area_prefix[i][u];
+                if (q == kNone || rt.intra_of[q] == kNone || HL_RIB_CELL_METRIC(c) > 0xFFFFu) return HSPF_E_INVAL;
+                ic[rt.intra_of[q]] = hl_route_cell{(c.nh_mask & amask[i]) >> t->base[i], (c.aux & amask[i]) >> t->base[i],
+                                                   c.winner - t->intra_base[i], (uint16_t)HL_RIB_CELL_METRIC(c),
+                                                   (uint8_t)HL_RIB_CELL_FLAGS(c), 0};
+            }
+            nets[i].resize(PI);
+            nh[i].resize(std::max<size_t>(64, (size_t)PI * 2));
+            int rc = HSPF_OK;
+            for (int attempt = 0; attempt < 2; ++attempt) {
+                res[i] = hl_ospfv2_result{};
+                res[i].routes_cap = PI; res[i].routes = nets[i].data();
+                res[i].nexthops_cap = (uint32_t)nh[i].size(); res[i].nexthops = nh[i].data();
+                rc = intra_from_cells(jd[i], &areas[i], rt.intra, ic.data(), &res[i]);
+                if (rc != HSPF_E_NOMEM) break;
+                nh[i].resize(res[i].n_nexthops);
+            }
+            if (rc) return rc;
+        }
+        // 2. every route in prefix order; atoms of the other areas through their own resolvers
+        std::vector<hl_rib_route> routes;
+        std::vector<hl_nexthop> hops;
+        std::vector<Nh> set;
+        std::vector<uint32_t> ri(A, 0);
+        auto sort_key = [&](uint32_t i, uint32_t iface) {
+            return iface < areas[i].n_ifaces ? areas[i].ifaces[iface].sort_key : 0xFFFFFFFFu;
+        };
+        auto add_atoms = [&](uint64_t m) {
+            for (; m; m &= m - 1) {
+                const uint32_t b = (uint32_t)__builtin_ctzll(m);
+                uint32_t i = 0;
+                while (i < A && !((amask[i] >> b) & 1u)) ++i;
+                if (i == A) return HSPF_E_INVAL;                       // an atom no area has
+                for (const Nh &x : jd[i].rs->resolve(b - t->base[i])) {
+                    auto at = std::lower_bound(set.begin(), set.end(), x, nh_less);
+                    if (at == set.end() || !nh_same_key(*at, x)) { set.insert(at, x); continue; }
+                    // two atoms, one next hop: which entry gave it depends on the merge order
+                    if (at->iface != x.iface || at->nbr != x.nbr || at->has_nbr != x.has_nbr || at->has_label != x.has_label ||
+                        at->label != x.label)
+                        return HSPF_E_UNSUPPORTED;
+                }
+            }
+            return HSPF_OK;
+        };
+        for (uint32_t u = 0; u < P; ++u) {
+            const hl_ospf_rib_cell &c = cells[u];
+            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT)) continue;
+            const uint32_t path = HL_RIB_CELL_PATH(c);
+            hl_rib_route o;
+            std::memset(&o, 0, sizeof(o));
+            o.prefix = t->prefix[u]; o.mask = t->plen[u] == 0 ? 0 : 0xFFFFFFFFu << (32 - t->plen[u]);
+            o.path_type = (uint8_t)path;
+            o.nh_off = (uint32_t)hops.size();
+            set.clear();
+            uint64_t rest = c.nh_mask;
+            if (path == HL_PATH_INTRA_AREA) {
+                const uint32_t w = intra_area(c.winner);
+                if (w == kNone || ri[w] >= res[w].n_routes) return HSPF_E_INVAL;
+                const hl_route_net &r = nets[w][ri[w]++];
+                o.metric = r.metric; o.area_id = t->area_id[w]; o.has_area = 1; o.flags = r.flags;
+                o.has_sr_label = r.has_sr_label; o.sr_label = r.has_sr_label ? r.sr_label : 0;
+                for (uint32_t k = 0; k < r.n_nh; ++k) {
+                    const hl_nexthop &h = nh[w][r.nh_off + k];
+                    set.push_back(Nh{sort_key(w, h.iface), h.iface, h.addr, h.nbr_router_id, h.sr_label, h.has_addr,
+                                     h.has_nbr, h.has_label});
+                }
+                rest &= ~amask[w];
+            } else if (path == HL_PATH_INTER_AREA) {
+                uint32_t w = 0;
+                while (w < A && !(c.winner >= o3[w * S + u] && c.winner < o3[w * S + u + 1])) ++w;
+                if (w == A) return HSPF_E_INVAL;
+                o.metric = HL_RIB_CELL_METRIC(c); o.area_id = t->area_id[w]; o.has_area = 1;
+            } else {
+                if (c.winner < o5[u] || c.winner >= o5[u + 1]) return HSPF_E_INVAL;
+                o.metric = HL_RIB_CELL_METRIC(c);
+                o.tag = t->ext_tag[c.winner - t->ext_base];
+                if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
+            }
+            const int rc = add_atoms(rest);
+            if (rc) return rc;
+            if (set.size() > t->max_paths) set.resize(t->max_paths);
+            for (const Nh &x : set) {
+                hl_nexthop h{};
+                h.iface = x.sort; h.addr = x.has_addr ? x.addr : 0; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
+                h.sr_label = x.has_label ? x.label : 0;
+                h.has_addr = x.has_addr; h.has_nbr = x.has_nbr; h.has_label = x.has_label;
+                hops.push_back(h);
             }
             o.n_nh = (uint32_t)hops.size() - o.nh_off;
             routes.push_back(o);

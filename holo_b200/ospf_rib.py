@@ -440,3 +440,111 @@ def rib_from_cells_v3(area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh
     from . import ospfv3
     return _call_rib_from_cells(capi.load_library().hspf_ospfv3_rib_from_cells, area, rt, cells, gather_v, gather_nh,
                                 RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)
+
+
+# ---- batched routing-table stage for area border routers (include/holo_spf_lsdb.h) --------------------------
+ABR_MAX_AREAS = 8                  # HSPF_ABR_MAX_AREAS
+
+
+class AbrRibTable(route_table.RouteTable):
+    """hspf_ospfv2_abr_ribtable: the routing-table records of one area border router over its attached areas, in
+    the instance's area order.  `flats`: one ospfv2.Flat per area (each with the router as a router vertex);
+    `summaries`: each area's SUMMARY_LSA_DT[] (LsaKey order); `active`: per area (default all); `externals`: the
+    instance's EXTERNAL_LSA_DT[].  `off` is [2 n_areas + 1, P + 1] (intra-area ranges per area, type-3 ranges per
+    area, type-5 ranges); per area `roots`, `n_vertices`, `atom_base`, `n_atoms`."""
+
+    api, kind, contrib_dt = "hspf_ospfv2", "abr_ribtable", RIB_RECORD_DT
+
+    def __init__(self, router_id: int, flats: list, area_ids, summaries=None, active=None, externals=None):
+        n = len(flats)
+        self.router_id, self.flats, self.area_ids = router_id, list(flats), [int(a) for a in area_ids]
+        sums = [np.ascontiguousarray(s if s is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
+                for s in (summaries if summaries is not None else [None] * n)]
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        self.summaries, self.externals = sums, ext
+        self.active = [True] * n if active is None else [bool(a) for a in active]
+        fl = (C.c_void_p * max(n, 1))(*[f.handle.value for f in flats])
+        ids = np.asarray(self.area_ids or [0], np.uint32)
+        sp = (C.c_void_p * max(n, 1))(*[s.ctypes.data if len(s) else None for s in sums])
+        ns = np.asarray([len(s) for s in sums] or [0], np.uint32)
+        act = np.asarray([int(a) for a in self.active] or [0], np.uint8)
+        self._keep = (fl, ids, sp, ns, act, sums, ext, flats)
+        lib = capi.load_library()
+        super().__init__(lib.hspf_ospfv2_abr_ribtable_create, router_id, n, fl, ids.ctypes.data, sp, ns.ctypes.data,
+                         act.ctypes.data, ext.ctypes.data if len(ext) else None, len(ext))
+        self.n_areas = n
+        pp, pl, po = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)()
+        self._call("arrays", C.byref(pp), C.byref(pl), C.byref(po), None)
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, np.uint32)
+        self.plen = route_table.copy_records(pl, self.n_prefixes, np.uint32)
+        self.off = route_table.copy_records(po, (2 * n + 1) * (self.n_prefixes + 1), np.uint32).reshape(2 * n + 1, -1)
+        info = [np.zeros(n, np.uint32) for _ in range(4)]
+        self._call("areas", *[x.ctypes.data for x in info])
+        self.roots, self.n_vertices, self.atom_base, self.n_atoms = [[int(v) for v in x] for x in info]
+
+
+def _planes_array(planes: list):
+    """Host array of capi.ResultStruct / capi.Result16Struct (one per area, device pointers) and whether narrow."""
+    narrow = isinstance(planes[0], capi.Result16Struct)
+    cls = capi.Result16Struct if narrow else capi.ResultStruct
+    arr = (cls * len(planes))(*planes)
+    return arr, narrow
+
+
+def abr_rib_cells_device(ctx: capi.Context, rt: AbrRibTable, n_jobs: int, planes: list, n_rows, rows_ptr: int,
+                         cells_ptr: int, status_out_ptr: int = 0, n_gather: int = 0, gather_job_ptr: int = 0,
+                         gather_area_ptr: int = 0, gather_v_ptr: int = 0, gather_nh_ptr: int = 0):
+    """hspf_ospfv2_abr_rib_cells / _cells16 over DEVICE planes: `planes` one capi.ResultStruct (nh_words 1) or
+    capi.Result16Struct per area, in the table's order; n_rows: rows of each area's planes; rows_ptr: device
+    u32[n_jobs, n_areas]; cells_ptr: device [n_jobs, rt.n_prefixes] RIB_CELL_DT; gathers as (job, area, vertex)
+    triples.  Enqueued on the ctx stream; the table must have been uploaded."""
+    arr, narrow = _planes_array(planes)
+    nr = np.ascontiguousarray(n_rows, np.uint32)
+    fn = ctx.lib.hspf_ospfv2_abr_rib_cells16 if narrow else ctx.lib.hspf_ospfv2_abr_rib_cells
+    rc = fn(ctx.handle, rt.handle, n_jobs, arr, nr.ctypes.data, rows_ptr or None, cells_ptr or None, status_out_ptr or None,
+            n_gather, gather_job_ptr or None, gather_area_ptr or None, gather_v_ptr or None, gather_nh_ptr or None)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
+def abr_rib_delta_device(ctx: capi.Context, rt: AbrRibTable, n_jobs: int, planes: list, n_rows, rows_ptr: int,
+                         base_ptr: int, n_base: int, base_of_ptr: int, job_out_ptr: int, records_ptr: int, cap: int,
+                         n_records_ptr: int):
+    """hspf_ospfv2_abr_rib_delta / _delta16: each job's cells (as abr_rib_cells_device) compared with its base row of
+    base_ptr on the device, as rib_delta_device."""
+    arr, narrow = _planes_array(planes)
+    nr = np.ascontiguousarray(n_rows, np.uint32)
+    fn = ctx.lib.hspf_ospfv2_abr_rib_delta16 if narrow else ctx.lib.hspf_ospfv2_abr_rib_delta
+    rc = fn(ctx.handle, rt.handle, n_jobs, arr, nr.ctypes.data, rows_ptr or None, base_ptr or None, n_base,
+            base_of_ptr or None, job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
+def abr_rib_from_cells(areas: list, rt: AbrRibTable, cells: np.ndarray, gather_area, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv2_abr_rib_from_cells (host): one job's cells -> the routing table update_rib_full gives for
+    rt.router_id over its areas (ospfv2.Ospfv2Area images in the table's order).  rc HSPF_E_UNSUPPORTED is returned
+    in the result, as rib_from_cells."""
+    cells = np.ascontiguousarray(cells, RIB_CELL_DT)
+    assert cells.shape == (rt.n_prefixes,)
+    ga = np.ascontiguousarray(gather_area, np.uint32)
+    gv = np.ascontiguousarray(gather_v, np.uint32)
+    gn = np.ascontiguousarray(gather_nh, np.uint64)
+    structs = [a.as_struct() for a in areas]
+    arr = (ospfv2.AreaStruct * max(len(areas), 1))(*structs)
+    fn = capi.load_library().hspf_ospfv2_abr_rib_from_cells
+    caps = [max(rt.n_prefixes, 1), max(4 * rt.n_prefixes, 64)]
+    for _ in range(2):
+        routes, nhs = np.zeros(caps[0], RIB_ROUTE_DT), np.zeros(caps[1], ospfv2.NEXTHOP_DT)
+        r = RibStruct(caps[0], 0, routes.ctypes.data, caps[1], 0, nhs.ctypes.data)
+        rc = fn(rt.handle, arr, len(areas), cells.ctypes.data, ga.ctypes.data, gv.ctypes.data, gn.ctypes.data, len(gv),
+                C.byref(r))
+        if rc == capi.HSPF_E_NOMEM:
+            caps = [max(caps[0], r.n_routes), max(caps[1], r.n_nexthops)]
+            continue
+        break
+    if rc not in (capi.HSPF_OK, capi.HSPF_E_UNSUPPORTED):
+        raise capi.HspfError(rc, "hspf_ospfv2_abr_rib_from_cells failed")
+    if rc != capi.HSPF_OK:
+        return Rib(np.zeros(0, RIB_ROUTE_DT), np.zeros(0, ospfv2.NEXTHOP_DT), rc)
+    return Rib(routes[: r.n_routes].copy(), nhs[: r.n_nexthops].copy(), rc)

@@ -584,3 +584,183 @@ def inter_area_view(area: Ospfv2Area, seed: int, n_abr: int = 4, n_asbr: int = 3
     ext.sort(key=lambda x: (x[0], x[1]))
     externals = np.asarray(ext, ospf_rib.EXTERNAL_LSA_DT)
     return a, summaries, externals
+
+
+ABR_ROUTER_ID = 0x0AFF0001   # 10.255.0.1: the router abr_view roots every area at
+ABR_TIE_ASBR = 0x0B0000F1    # an ASBR outside the domain that every non-backbone area of abr_view names
+
+
+def _dist_from(flat: Flat, root: int):
+    """Unperturbed SPT distances of `flat` from `root` (the generator's own Dijkstra, to place equal-cost routes)."""
+    import heapq
+    c = flat.csr
+    dist = np.full(c.n_vertices, np.iinfo(np.int64).max, np.int64)
+    dist[root] = 0
+    heap = [(0, root)]
+    while heap:
+        d, v = heapq.heappop(heap)
+        if d > dist[v]:
+            continue
+        for e in range(int(c.row_ptr[v]), int(c.row_ptr[v + 1])):
+            w, nd = int(c.col[e]), d + int(c.cost[e])
+            if nd < dist[w]:
+                dist[w] = nd
+                heapq.heappush(heap, (nd, w))
+    return dist
+
+
+def _with_stubs(area: Ospfv2Area, adds: dict) -> Ospfv2Area:
+    """area with stub links appended to Router-LSAs: adds {router_id: [(prefix, mask, metric)]}.  Appended after each
+    LSA's own links, so the root's non-stub link positions do not move."""
+    rl, links = area.router_lsas.copy(), []
+    for i in range(len(rl)):
+        o, n = int(rl["link_off"][i]), int(rl["n_links"][i])
+        extra = [(p, m, metric, LINK_STUB, 0) for (p, m, metric) in adds.get(int(rl["adv_rtr"][i]), [])]
+        rl["link_off"][i] = len(links)
+        rl["n_links"][i] = n + len(extra)
+        links += [tuple(x) for x in area.links[o: o + n].tolist()] + extra
+    a = Ospfv2Area(**{k: getattr(area, k) for k in area.__dataclass_fields__})
+    a.router_lsas, a.links = rl, np.asarray(links, LINK_DT) if links else np.zeros(0, LINK_DT)
+    return a
+
+
+def abr_view(topos: list, seed: int, area_ids=None, roots=None, max_paths: int = 16, n_shared: int = 6,
+             v_flag_area: int | None = 1, **inter_kw):
+    """A multi-area domain as one ABR sees it: returns (areas [Ospfv2Area], summaries [SUMMARY_LSA_DT[] per area],
+    externals EXTERNAL_LSA_DT[]), the areas in instance order.  Area k is synth_area(topos[k], root=roots[k]) with its
+    router ids, addresses, interface sort keys and ifindexes moved into ranges of its own; the root becomes router
+    ABR_ROUTER_ID in every area, with the B flag.  Seeded.
+      * area 0 (area_ids[0], 0 by default) carries inter_area_view's type-3/4/5 load (type-4 LSAs naming the root
+        dropped); every other area gets type-3 LSAs from two ABRs of its own, for some of area 0's prefixes and new
+        ones (read only while one area is active, and by the transit-area step), and a type-4 LSA;
+      * shared prefixes: area 0's first LAN is also a LAN of area 1 (transit-network overwrite across areas); n_shared
+        stubs of area 0's neighbours of the root are also stubs of a neighbour of the root in the other areas, half at
+        the same metric (atoms merge across areas), half not;
+      * an ASBR in each non-backbone area (its farthest router) with externals of its own, also named by a backbone
+        type-4 LSA at metric 1; an ASBR named by a type-4 LSA of every non-backbone area at one forwarding metric;
+      * with v_flag_area, a router of that area (not the root) gets the V flag."""
+    from . import ospf_rib
+    rng = np.random.default_rng(seed)
+    A = len(topos)
+    area_ids = list(area_ids) if area_ids is not None else list(range(A))
+    roots = list(roots) if roots is not None else [0] * A
+    areas = []
+    for k, (t, r) in enumerate(zip(topos, roots)):
+        a = synth_area(t, root=r, max_paths=max_paths)
+        root_rid = RID_BASE + r
+
+        def rmap(x, k=k, root_rid=root_rid):
+            x = np.asarray(x, np.uint64)
+            out = x.copy()
+            is_rid = (x >> 24) == 10
+            out = np.where(is_rid, x + (k << 20), out)
+            out = np.where(x == root_rid, ABR_ROUTER_ID, out)
+            out = np.where((x >> 20) == (P2P_BASE >> 20), x + (k << 18), out)
+            lan = (x >> 16) == (LAN_BASE >> 16)
+            lan_to = x + (k << 16)
+            if k == 1:                       # area 1's LAN 0 is area 0's LAN 0, hosts moved up by 100
+                lan_to = np.where(lan & (((x - LAN_BASE) >> 8) == 0), x + 100, lan_to)
+            out = np.where(lan, lan_to, out)
+            return out.astype(np.uint32)
+
+        a.router_id = ABR_ROUTER_ID
+        a.area_id = area_ids[k]
+        rl = a.router_lsas.copy()
+        rl["adv_rtr"], rl["lsa_id"] = rmap(rl["adv_rtr"]), rmap(rl["lsa_id"])
+        links = a.links.copy()
+        links["link_id"] = rmap(links["link_id"])
+        non_stub = links["link_type"] != LINK_STUB
+        links["link_data"] = np.where(non_stub, rmap(links["link_data"]), links["link_data"])
+        nl = a.network_lsas.copy()
+        nl["adv_rtr"], nl["lsa_id"] = rmap(nl["adv_rtr"]), rmap(nl["lsa_id"])
+        a.attached = rmap(a.attached)
+        nb = a.nbrs.copy()
+        for f in nb.dtype.names:
+            if nb.dtype[f] == np.uint32:
+                nb[f] = rmap(nb[f])
+        ia = a.iface_addrs.copy()
+        ia["addr"] = rmap(ia["addr"])
+        ifs = a.ifaces.copy()
+        ifs["sort_key"] += 1000 * k
+        ifs["ifindex"] += 1000 * k
+        order = np.lexsort((rl["lsa_id"], rl["adv_rtr"]))
+        rl = rl[order]
+        rl["flags"][rl["adv_rtr"] == ABR_ROUTER_ID] |= 0x01
+        a.router_lsas, a.links, a.nbrs, a.iface_addrs, a.ifaces = rl, links, nb, ia, ifs
+        a.network_lsas = nl[np.lexsort((nl["lsa_id"], nl["adv_rtr"]))] if len(nl) else nl
+        areas.append(a)
+    # type-3/4/5 load of area 0 (the backbone unless area_ids say otherwise)
+    a0, sums0, ext = inter_area_view(areas[0], seed, **inter_kw)
+    a0.router_lsas["flags"][a0.router_lsas["adv_rtr"] == ABR_ROUTER_ID] |= 0x01
+    sums0 = sums0[~((sums0["lsa_type"] == 4) & (sums0["lsa_id"] == ABR_ROUTER_ID))]
+    areas[0] = a0
+    flat0 = Flat(a0)
+    d0 = _dist_from(flat0, flat0.router_vertex(ABR_ROUTER_ID))
+    stubs0 = [(int(l["link_id"]), int(l["link_data"]), int(l["metric"]), int(r["adv_rtr"]))
+              for r in a0.router_lsas for l in a0.links[int(r["link_off"]): int(r["link_off"]) + int(r["n_links"])]
+              if l["link_type"] == LINK_STUB and int(r["adv_rtr"]) != ABR_ROUTER_ID]
+    summaries, ext_rows = [sums0], [tuple(x) for x in ext.tolist()]
+    bb_abrs = [int(r) for r, f in zip(a0.router_lsas["adv_rtr"], a0.router_lsas["flags"])
+               if f & 0x01 and int(r) != ABR_ROUTER_ID and flat0.router_vertex(int(r)) != 0xFFFFFFFF
+               and d0[flat0.router_vertex(int(r))] < 1 << 40]
+    extra4 = []
+    inter_prefixes = sorted({(int(s["lsa_id"]), int(s["mask"])) for s in sums0 if s["lsa_type"] == 3})
+    for k in range(1, A):
+        a = areas[k]
+        flat = Flat(a)
+        rv = flat.router_vertex(ABR_ROUTER_ID)
+        dk = _dist_from(flat, rv)
+        others = [int(x) for x in a.router_lsas["adv_rtr"] if int(x) != ABR_ROUTER_ID]
+        reach = {int(flat.ids[v]): int(dk[v]) for v in range(len(flat.ids)) if flat.is_router[v] and dk[v] < 1 << 40}
+        pick = [int(x) for x in rng.permutation([r for r in others if r in reach])]
+        abrs, vrtr = pick[:2], pick[3]
+        asbr = max((r for r in pick[2:] if r != vrtr), key=lambda r: (reach[r], r))     # the farthest router
+        # shared stubs: the same prefix at a router of this area, half of them at the metric that ties area 0's route
+        adds = {}
+        shared = [stubs0[int(i)] for i in rng.choice(len(stubs0), min(n_shared, len(stubs0)), replace=False)]
+        for j, (p, m, metric, adv) in enumerate(shared):
+            want = int(d0[flat0.router_vertex(adv)]) + metric
+            cand = [(rid, d) for rid, d in reach.items() if rid != ABR_ROUTER_ID and d <= want - 1]
+            if not cand or want > 0xFFFF:
+                continue
+            rid, d = cand[int(rng.integers(0, len(cand)))]
+            m2 = want - d if j % 2 == 0 else want - d + int(rng.choice([-1, 5]))
+            adds.setdefault(rid, []).append((p, m, max(int(m2), 1)))
+        a = _with_stubs(a, adds)
+        rl = a.router_lsas
+        for rid in abrs:
+            rl["flags"][rl["adv_rtr"] == rid] |= 0x01
+        rl["flags"][rl["adv_rtr"] == asbr] |= 0x02
+        if v_flag_area is not None and k == v_flag_area:
+            rl["flags"][rl["adv_rtr"] == vrtr] |= 0x04
+        areas[k] = a
+        pool = [(p, m) for (p, m, _, _) in shared] + inter_prefixes[:6] + [(0x0AD00000 + (k << 12) + (i << 8), 0xFFFFFF00)
+                                                                          for i in range(4)]
+        sums = []
+        for (p, m) in pool:
+            for abr in abrs[: int(rng.integers(1, 3))]:
+                sums.append((abr, p, m, int(rng.choice([1, 5, 10, 20])), 3, 0, (0, 0)))
+        sums.append((abrs[0], 0x0B000001, 0, 10, 4, 0, (0, 0)))
+        # an ASBR outside the area named by every non-backbone area at one forwarding metric: with one active area
+        # the entries tie across areas and the higher area id wins
+        sums.append((abrs[0], ABR_TIE_ASBR, 0, max(1, 1000 - reach[abrs[0]]), 4, 0, (0, 0)))
+        # this area's ASBR, also named by a backbone type-4 LSA through the nearest backbone ABR at metric 1: an
+        # intra-area entry through a non-backbone area beats the (usually shorter) backbone entry
+        if bb_abrs:
+            near = min(bb_abrs, key=lambda r: (int(d0[flat0.router_vertex(r)]), r))
+            extra4.append((near, asbr, 0, 1, 4, 0, (0, 0)))
+        sums.sort(key=lambda x: (x[4], x[0], x[1]))
+        summaries.append(np.asarray(sums, ospf_rib.SUMMARY_LSA_DT))
+        for i in range(3):
+            ext_rows.append((asbr, 0x0E000000 + (k << 16) + (i << 8), 0xFFFFFF00, int(rng.choice([1, 5, 20])), 0, k,
+                             int(i % 2), 0, (0, 0)))
+        if inter_prefixes:                                           # an ASBR of area 0's view seen from this area too
+            ext_rows.append((0x0B000001, 0x0E000000 + (k << 16) + 0xF00, 0xFFFFFF00, 7, 0, 0, 1, 0, (0, 0)))
+    if A > 1:
+        for i in range(2):
+            ext_rows.append((ABR_TIE_ASBR, 0x0E0F0000 + (i << 8), 0xFFFFFF00, 3, 0, 9, i, 0, (0, 0)))
+    if extra4:
+        s0 = sorted([tuple(x) for x in summaries[0].tolist()] + extra4, key=lambda x: (x[4], x[0], x[1]))
+        summaries[0] = np.asarray(s0, ospf_rib.SUMMARY_LSA_DT)
+    ext_rows.sort(key=lambda x: (x[0], x[1]))
+    return areas, summaries, np.asarray(ext_rows, ospf_rib.EXTERNAL_LSA_DT)

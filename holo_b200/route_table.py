@@ -106,10 +106,20 @@ def declare(lib: C.CDLL):
         "hspf_ospfv3_ribtable_create": [vp, u32, vp, u32, vp, u32, pvp],
         "hspf_ospfv3_ribtable_prefixes6": [vp, pvp, C.POINTER(u32p)],
         "hspf_ospfv3_rib_from_cells": [C.POINTER(ospfv3.AreaStruct), vp, vp, u32p, u64p, u32, C.POINTER(ospf_rib.RibStruct)],
+        "hspf_ospfv2_abr_ribtable_create": [u32, u32, vp, vp, vp, vp, vp, vp, u32, pvp],
+        "hspf_ospfv2_abr_ribtable_arrays": [vp, C.POINTER(u32p), C.POINTER(u32p), C.POINTER(u32p), pvp],
+        "hspf_ospfv2_abr_ribtable_areas": [vp, vp, vp, vp, vp],
+        "hspf_ospfv2_abr_ribtable_upload": [vp, vp],
+        "hspf_ospfv2_abr_rib_cells": [vp, vp, u32, vp, vp, vp, vp, vp, u32, vp, vp, vp, vp],
+        "hspf_ospfv2_abr_rib_cells16": [vp, vp, u32, vp, vp, vp, vp, vp, u32, vp, vp, vp, vp],
+        "hspf_ospfv2_abr_rib_delta": [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_abr_rib_delta16": [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_abr_rib_from_cells": [vp, C.POINTER(ospfv2.AreaStruct), u32, vp, vp, vp, vp, u32,
+                                           C.POINTER(ospf_rib.RibStruct)],
     }
     for name, argtypes in sigs.items():
         getattr(lib, name).argtypes = argtypes
-    for table in ("hspf_ospfv2_rtable", "hspf_isis_rtable", "hspf_ospfv2_ribtable"):
+    for table in ("hspf_ospfv2_rtable", "hspf_isis_rtable", "hspf_ospfv2_ribtable", "hspf_ospfv2_abr_ribtable"):
         getattr(lib, table + "_free").argtypes = [vp]
         getattr(lib, table + "_free").restype = None
         for name in ("prefixes", "contributors"):

@@ -236,6 +236,92 @@ int hspf_ospfv2_rib_from_cells(const hl_ospfv2_area *area, const hspf_ospfv2_rib
                                hl_ospfv2_rib *out);
 
 /*
+ * Batched routing-table stage on the device for one area border router (a root with the B flag, which the stage
+ * above refuses): update_rib_full over every area the router is attached to, for every job of a what-if batch.
+ * One table per router.  Job j holds one row per attached area: rows[j][i] is the row of area i's planes (the
+ * SPT of that area's graph rooted at the router).  With attached areas A_0 .. A_{n-1} (flat, area id, type-3/4
+ * summaries in LsaKey order, active) and externals X, the decoded cells of job j equal
+ *     hspf_ospfv2_update_rib_full(r, max_paths,
+ *         [{A_i.area_id, hspf_ospfv2_area_from_planes(A_i, planes_i[rows[j][i]]), A_i.ifaces, summaries_i, active_i}],
+ *         X)
+ * routes and next hops, with the areas in the caller's order (the instance's area order: it decides the
+ * cross-area transit-network rule and the transit-area step) and max_paths the areas' own, which must agree.
+ *
+ *   hspf_ospfv2_abr_ribtable_create  host.  router_id; per area i < n_areas: flats[i], area_ids[i], summaries[i] /
+ *                                n_summaries[i] (n_summaries NULL: none), active[i] (NULL: all active); the
+ *                                instance's AS-external LSAs.  Prefixes: the union over the areas, in prefix order;
+ *                                per prefix, each area's intra-area advertiser range and type-3 range, and the type-5
+ *                                range; per ASBR one entry per area (its vertex with the E flag, its type-4 range,
+ *                                which is empty for an area whose summaries step 2 does not read: every area's with
+ *                                one active area, else the backbone's); per area its root, its atom base (the atom
+ *                                counts of the earlier areas: atom a of area i is bit base_i + a of nh_mask and of an
+ *                                intra-area cell's aux) and its V-flag routers.  Filters as hspf_ospfv2_ribtable_create,
+ *                                plus the LSAs the router originated itself.  HSPF_E_UNSUPPORTED: more than 8 areas
+ *                                (the kernels' bound), more than 64 atoms in all, a usable type-4 LSA naming an ABR in
+ *                                an area step 2 reads.  HSPF_E_INVAL: the router is not a router vertex of some flat
+ *                                (leave that area out, as update_rib_full callers do when root_found is 0), or the
+ *                                areas' max_paths differ.
+ *   hspf_ospfv2_abr_ribtable_arrays / _prefixes / _contributors  as for hspf_ospfv2_ribtable (off[(2 n + 1)(P + 1)]:
+ *                                per area its intra-area ranges, then per area its type-3 ranges, then the type-5).
+ *   hspf_ospfv2_abr_ribtable_areas  per area: root vertex, vertex count, atom base, atom count; returns n_areas.
+ *   hspf_ospfv2_abr_ribtable_upload copies the table to the ctx's device.
+ *   hspf_ospfv2_abr_rib_cells    one thread per (job, prefix).  planes: host array of n_areas hspf_result (device
+ *   hspf_ospfv2_abr_rib_cells16  planes, nh_words == 1) / hspf_result16; n_rows[i] the rows of area i's planes;
+ *                                rows: device u32[n_jobs][n_areas]; cells[n_jobs][P] (device) hl_ospf_rib_cell.
+ *                                job_status_out (device u32[n_jobs], may be NULL): the OR of the status words of the
+ *                                job's rows, plus HSPF_JS_INVALID for a row out of range; a job with a non-zero word
+ *                                gets empty cells.  gather_job / gather_area / gather_v (device u32[n_gather]):
+ *                                gather_nh[g] = nh_mask of vertex gather_v[g] in the job's row of area gather_area[g]
+ *                                (0 when out of range): the transit networks next to the root in each area, which the
+ *                                decode reads.  Enqueued on the ctx stream.
+ *   hspf_ospfv2_abr_rib_from_cells  host: one job's cells -> the table of the contract.  areas[n_areas]: each area's
+ *                                image (router_id = the router), in the table's order; the gathers of the job as
+ *                                (area, vertex, nh_mask).  Virtual-link atoms have no next hop, as in
+ *                                hspf_ospfv2_area_from_planes; the transit-area step gives such routes theirs.
+ *                                HSPF_E_UNSUPPORTED as hspf_ospfv2_rib_from_cells (HL_CELL_MIXED_SID, which also
+ *                                marks an intra-area merge across areas or with a transit-area route where a
+ *                                Prefix-SID is involved; two atoms with one next hop and different attributes).
+ *   hspf_ospfv2_abr_rib_delta[16]   the route-delta stage over the same walk (arguments as hspf_ospfv2_rib_delta, rows
+ *                                as above in place of roots).  The base row is normally the job whose rows are all
+ *                                the unperturbed rows.
+ */
+#define HSPF_ABR_MAX_AREAS 8u
+typedef struct hspf_ospfv2_abr_ribtable hspf_ospfv2_abr_ribtable;
+int hspf_ospfv2_abr_ribtable_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv2_flat *const *flats,
+                                    const uint32_t *area_ids, const hl_ospfv2_summary_lsa *const *summaries,
+                                    const uint32_t *n_summaries, const uint8_t *active,
+                                    const hl_ospfv2_external_lsa *externals, uint32_t n_externals,
+                                    hspf_ospfv2_abr_ribtable **out);
+void hspf_ospfv2_abr_ribtable_free(hspf_ospfv2_abr_ribtable *t);
+uint32_t hspf_ospfv2_abr_ribtable_prefixes(const hspf_ospfv2_abr_ribtable *t);
+uint32_t hspf_ospfv2_abr_ribtable_contributors(const hspf_ospfv2_abr_ribtable *t);
+int hspf_ospfv2_abr_ribtable_arrays(const hspf_ospfv2_abr_ribtable *t, const uint32_t **prefix, const uint32_t **plen,
+                                    const uint32_t **off, const void **records);
+int hspf_ospfv2_abr_ribtable_areas(const hspf_ospfv2_abr_ribtable *t, uint32_t *root, uint32_t *n_vertices,
+                                   uint32_t *atom_base, uint32_t *n_atoms);
+int hspf_ospfv2_abr_ribtable_upload(hspf_ctx *ctx, hspf_ospfv2_abr_ribtable *t);
+int hspf_ospfv2_abr_rib_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs, const hspf_result *planes,
+                              const uint32_t *n_rows, const uint32_t *rows, hl_ospf_rib_cell *cells,
+                              uint32_t *job_status_out, uint32_t n_gather, const uint32_t *gather_job,
+                              const uint32_t *gather_area, const uint32_t *gather_v, uint64_t *gather_nh);
+int hspf_ospfv2_abr_rib_cells16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs,
+                                const hspf_result16 *planes, const uint32_t *n_rows, const uint32_t *rows,
+                                hl_ospf_rib_cell *cells, uint32_t *job_status_out, uint32_t n_gather,
+                                const uint32_t *gather_job, const uint32_t *gather_area, const uint32_t *gather_v,
+                                uint64_t *gather_nh);
+int hspf_ospfv2_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_ospfv2_area *areas, uint32_t n_areas,
+                                   const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
+                                   const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv2_rib *out);
+int hspf_ospfv2_abr_rib_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs, const hspf_result *planes,
+                              const uint32_t *n_rows, const uint32_t *rows, const hl_ospf_rib_cell *base_cells,
+                              uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                              hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_ospfv2_abr_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs,
+                                const hspf_result16 *planes, const uint32_t *n_rows, const uint32_t *rows,
+                                const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+
+/*
  * The stages of update_rib_full that follow the per-area SPFs (holo-ospf/src/route.rs:146-193):
  * merges the intra-area routes of the attached areas (route_update / route_compare,
  * route.rs:895-971), adds inter-area network routes and inter-area router entries from the
