@@ -21,77 +21,50 @@ namespace {
 using hspf::RouteContrib;
 
 // The cell of (job, prefix): route_cell_eval over the job's rows of the planes.
-template <class Planes, class D, class N>
+template <class Planes>
 struct OspfCell {
-    const uint32_t *off; const RouteContrib *contribs; const D *dist; const uint16_t *hops; const N *nh;
-    const uint32_t *status; uint32_t V;
-    __device__ __forceinline__ bool refused(uint32_t j) const { return status && status[j] != 0; }
-    __device__ __forceinline__ uint32_t status_word(uint32_t j) const { return status ? status[j] : 0; }
+    const uint32_t *off; const RouteContrib *contribs; hspf::ResultPlanes<Planes> pl;
+    __device__ __forceinline__ bool refused(uint32_t j) const { return pl.refused(j); }
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const { return pl.status_word(j); }
     __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        const size_t base = (size_t)j * V;
-        const hl_route_cell c = hspf::route_cell_eval(Planes{dist + base, hops + base, nh + base}, contribs, off[p], off[p + 1]);
+        const hl_route_cell c = hspf::route_cell_eval(pl.job(j), contribs, off[p], off[p + 1]);
         return {c.nh_mask, c.lasthop_mask, (uint64_t)c.winner | ((uint64_t)c.metric << 32) | ((uint64_t)c.flags << 48)};
     }
+    // the few plane values the host decode needs
+    __device__ __forceinline__ uint64_t gather(uint32_t j, uint32_t, uint32_t v) const { return pl.gather(j, v); }
+    __device__ static hspf::CellWords empty() { return {0, 0, 0xFFFFFFFFu}; }      // winner none
 };
 
-// the bound keeps the walk in 32 registers, so the whole grid launch_route_stage sizes is resident at once
-template <class Planes, class D, class N>
-__global__ void __launch_bounds__(hspf::kRouteThreads, hspf::kRouteBlocksPerSM)
-route_cells_kernel(uint32_t n_jobs, uint32_t P, uint32_t V, const uint32_t *__restrict__ off,
-                   const RouteContrib *__restrict__ contribs, const D *__restrict__ dist,
-                   const uint16_t *__restrict__ hops, const N *__restrict__ nh, const uint32_t *__restrict__ job_status,
-                   hl_route_cell *__restrict__ cells, bool aligned16, uint32_t n_gather,
-                   const uint32_t *__restrict__ gather_job, const uint32_t *__restrict__ gather_v,
-                   uint64_t *__restrict__ gather_nh) {
-    const OspfCell<Planes, D, N> cell{off, contribs, dist, hops, nh, job_status, V};
-    hspf::store_route_cells(n_jobs, P, cell, hspf::CellWords{0, 0, 0xFFFFFFFFu}, cells, aligned16);   // empty: winner none
-    // the few plane values the host decode needs
-    for (uint64_t g = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; g < n_gather; g += (uint64_t)gridDim.x * blockDim.x) {
-        const uint32_t job = gather_job[g], v = gather_v[g];
-        gather_nh[g] = (job < n_jobs && v < V) ? (uint64_t)nh[(size_t)job * V + v] : 0;
-    }
+template <class R>
+int make_cell(const hspf_ospfv2_rtable *rt, const R *pl, OspfCell<hspf::PlanesOf<R>> &cell) {
+    if (!rt || !rt->dev.blob || hspf::result_planes(pl, rt->t.n_vertices, cell.pl) || !cell.pl.complete())
+        return HSPF_E_INVAL;
+    cell.off = rt->dev.off;
+    cell.contribs = static_cast<const RouteContrib *>(rt->dev.contribs);
+    return HSPF_OK;
 }
 
-template <class Planes, class D, class N>
-int launch_cells(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const D *dist, const uint16_t *hops,
-                 const N *nh, const uint32_t *status, hl_route_cell *cells, uint32_t n_gather,
-                 const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh) {
-    if (!ctx || !rt || !rt->dev.blob || !dist || !hops || !nh || !cells) return HSPF_E_INVAL;
-    if (n_gather && (!gather_job || !gather_v || !gather_nh)) return HSPF_E_INVAL;
-    const uint32_t P = (uint32_t)rt->t.prefix.size();
-    const uint64_t total = (uint64_t)n_jobs * P;
-    if (total + n_gather == 0) return HSPF_OK;
-    return hspf::launch_route_stage(ctx, rt->dev, total, cells, [&](uint32_t blocks, cudaStream_t st, bool aligned16) {
-        route_cells_kernel<Planes, D, N><<<blocks, hspf::kRouteThreads, 0, st>>>(
-            n_jobs, P, rt->t.n_vertices, rt->dev.off, static_cast<const RouteContrib *>(rt->dev.contribs), dist, hops, nh,
-            status, cells, aligned16, n_gather, gather_job, gather_v, gather_nh);
-    });
+// Both the cell kernel and the route-delta passes are bounded to 8 blocks per SM: the walk stays in 32 registers
+// (with a few bytes of spill in delta pass A), so the grid of one wave is resident at once.
+template <class R>
+int routes_batch(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const R *pl, hl_route_cell *cells,
+                 uint32_t n_gather, const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh) {
+    OspfCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_cell(rt, pl, cell)) return rc;
+    return hspf::launch_route_cells<hspf::kRouteBlocksPerSM>(ctx, rt->dev, cell, n_jobs, (uint32_t)rt->t.prefix.size(),
+                                                             cells, nullptr, n_gather, gather_job, nullptr, gather_v,
+                                                             gather_nh);
 }
 
-// The route-delta stage over the same walk (route_stage.cuh: launch_route_delta), under the bound of route_cells_kernel
-// so that the grid launch_route_stage sizes is resident at once: 32 registers, with a few bytes of spill in pass A.
-template <class Planes, class D, class N>
-int launch_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const D *dist, const uint16_t *hops,
-                 const N *nh, const uint32_t *status, const hl_route_cell *base_cells, uint32_t n_base,
-                 const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
-                 uint64_t *n_records) {
-    if (!ctx || !rt || !rt->dev.blob || !dist || !hops || !nh) return HSPF_E_INVAL;
-    using Cell = OspfCell<Planes, D, N>;
-    const Cell cell{rt->dev.off, static_cast<const RouteContrib *>(rt->dev.contribs), dist, hops, nh, status, rt->t.n_vertices};
-    hspf::DeltaArgs a{};
-    a.n_jobs = n_jobs; a.P = (uint32_t)rt->t.prefix.size();
-    a.base = reinterpret_cast<const uint64_t *>(base_cells); a.n_base = n_base; a.base_of = base_of;
-    a.job_out = job_out; a.n_records = reinterpret_cast<unsigned long long *>(n_records);
-    a.records = records; a.cap = cap;
-    return hspf::launch_route_delta(ctx, rt->dev, a,
-        [&](uint32_t blocks, cudaStream_t st, const hspf::DeltaArgs &args) {
-            hspf::route_delta_count_kernel<hspf::OspfCellLayout, Cell, hspf::kRouteBlocksPerSM>
-                <<<blocks, hspf::kRouteThreads, 0, st>>>(cell, args);
-        },
-        [&](uint32_t blocks, cudaStream_t st, const hspf::DeltaArgs &args) {
-            hspf::route_delta_store_kernel<hspf::OspfCellLayout, Cell, hspf::kRouteBlocksPerSM>
-                <<<blocks, hspf::kRouteThreads, 0, st>>>(cell, args);
-        });
+template <class R>
+int routes_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const R *pl,
+                 const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                 hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    OspfCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_cell(rt, pl, cell)) return rc;
+    return hspf::launch_route_delta<hspf::OspfCellLayout, hspf::kRouteBlocksPerSM>(
+        ctx, rt->dev, cell, n_jobs, (uint32_t)rt->t.prefix.size(), base_cells, n_base, base_of, job_out, records, cap,
+        n_records);
 }
 
 struct DevBuf {
@@ -113,33 +86,25 @@ int hspf_ospfv2_rtable_upload(hspf_ctx *ctx, hspf_ospfv2_rtable *rt) {
 int hspf_ospfv2_routes_batch(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result *pl,
                              hl_route_cell *cells, uint32_t n_gather, const uint32_t *gather_job,
                              const uint32_t *gather_v, uint64_t *gather_nh) {
-    if (!pl || pl->nh_words != 1) return HSPF_E_INVAL;
-    return launch_cells<hspf::PlanesWide, uint32_t, uint64_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask, pl->job_status,
-                                                              cells, n_gather, gather_job, gather_v, gather_nh);
+    return routes_batch(ctx, rt, n_jobs, pl, cells, n_gather, gather_job, gather_v, gather_nh);
 }
 
 int hspf_ospfv2_routes_batch16(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
                                hl_route_cell *cells, uint32_t n_gather, const uint32_t *gather_job,
                                const uint32_t *gather_v, uint64_t *gather_nh) {
-    if (!pl) return HSPF_E_INVAL;
-    return launch_cells<hspf::PlanesNarrow, uint16_t, uint16_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask, pl->job_status,
-                                                                cells, n_gather, gather_job, gather_v, gather_nh);
+    return routes_batch(ctx, rt, n_jobs, pl, cells, n_gather, gather_job, gather_v, gather_nh);
 }
 
 int hspf_ospfv2_routes_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result *pl,
                              const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                              hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    if (!pl || pl->nh_words != 1) return HSPF_E_INVAL;
-    return launch_delta<hspf::PlanesWide, uint32_t, uint64_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask, pl->job_status,
-                                                              base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return routes_delta(ctx, rt, n_jobs, pl, base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
 int hspf_ospfv2_routes_delta16(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
                                const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    if (!pl) return HSPF_E_INVAL;
-    return launch_delta<hspf::PlanesNarrow, uint16_t, uint16_t>(ctx, rt, n_jobs, pl->dist, pl->hops, pl->nh_mask, pl->job_status,
-                                                                base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return routes_delta(ctx, rt, n_jobs, pl, base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
 int hspf_ospfv2_run_area_batch(hspf_ctx *ctx, const hl_ospfv2_area *area, const uint32_t *root_router_ids, uint32_t n_roots,

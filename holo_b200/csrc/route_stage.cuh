@@ -1,11 +1,13 @@
-// Device side shared by the batched route stages (ospfv2_routes.cu, isis_routes.cu): the warp-tiled store
-// of 24-byte cells, one thread per (job, prefix), its launch on the ctx stream, and the fused route-delta stage
-// that compares every cell with its job's base cell instead of storing it.  nvcc only.
+// Device side shared by the batched route stages (ospfv2_routes.cu, isis_routes.cu, ospfv2_rib_cells.cu,
+// ospfv2_abr_rib_cells.cu): the warp-tiled store of 24-byte cells, one thread per (job, prefix), the cell kernel and
+// its launch on the ctx stream, and the fused route-delta stage that compares every cell with its job's base cell
+// instead of storing it.  A stage brings its cell functor; nvcc only.
 #pragma once
 #include <cuda_runtime.h>
 
 #include <algorithm>
 #include <cstdint>
+#include <type_traits>
 
 #include "holo_spf.h"
 #include "route_cells.h"
@@ -59,21 +61,101 @@ __device__ __forceinline__ void store_route_cells(uint32_t n_jobs, uint32_t P, c
     }
 }
 
-// Enqueues one route kernel on the ctx stream over `total` cells: one wave of `blocks_per_sm` blocks per SM (the
-// kernel's __launch_bounds__ minimum), warp-tile-stride beyond that.  `launch(blocks, stream, aligned16)` makes the
-// <<<blocks, kRouteThreads>>> call.
-template <class Launch>
-int launch_route_stage(hspf_ctx *ctx, const DeviceRouteTable &table, uint64_t total, const void *cells, Launch launch,
-                       uint32_t blocks_per_sm = kRouteBlocksPerSM) {
+// The planes of one result struct (include/holo_spf.h: hspf_result, hspf_result16), rows of V vertices per job.
+template <class Planes>
+struct ResultPlanes {
+    using D = std::remove_const_t<std::remove_pointer_t<decltype(Planes::dist)>>;
+    using N = std::remove_const_t<std::remove_pointer_t<decltype(Planes::nh)>>;
+    const D *dist; const uint16_t *hops; const N *nh; const uint32_t *status; uint32_t V;
+    bool complete() const { return dist && hops && nh; }
+    __device__ __forceinline__ Planes job(uint32_t j) const {
+        const size_t base = (size_t)j * V;
+        return Planes{dist + base, hops + base, nh + base};
+    }
+    __device__ __forceinline__ bool refused(uint32_t j) const { return status && status[j] != 0; }
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const { return status ? status[j] : 0; }
+    __device__ __forceinline__ uint64_t gather(uint32_t j, uint32_t v) const {
+        return v < V ? (uint64_t)nh[(size_t)j * V + v] : 0;
+    }
+};
+
+// the Planes of a result struct type
+template <class R>
+using PlanesOf = std::conditional_t<std::is_same<R, hspf_result>::value, PlanesWide, PlanesNarrow>;
+
+// The planes of `r` (all NULL when r is NULL: the caller decides whether it needs them).  The route stages read
+// one next-hop word: wide planes of more than one are HSPF_E_INVAL.
+inline int result_planes(const hspf_result *r, uint32_t V, ResultPlanes<PlanesWide> &p) {
+    p = {nullptr, nullptr, nullptr, nullptr, V};
+    if (!r) return HSPF_OK;
+    if (r->nh_words != 1) return HSPF_E_INVAL;
+    p = {r->dist, r->hops, r->nh_mask, r->job_status, V};
+    return HSPF_OK;
+}
+inline int result_planes(const hspf_result16 *r, uint32_t V, ResultPlanes<PlanesNarrow> &p) {
+    p = {nullptr, nullptr, nullptr, nullptr, V};
+    if (r) p = {r->dist, r->hops, r->nh_mask, r->job_status, V};
+    return HSPF_OK;
+}
+
+// The grid of a route kernel over `items` threads on the ctx's device: one wave of `blocks_per_sm` blocks per SM
+// at most (the kernel's __launch_bounds__ minimum), warp-tile-stride beyond that.  Makes the device current.
+inline int route_grid(hspf_ctx *ctx, const DeviceRouteTable &table, uint64_t items, uint32_t blocks_per_sm,
+                      uint32_t &blocks) {
     const int dev = hspf_ctx_device(ctx);
     if (table.device != dev) return HSPF_E_INVAL;             // the table was uploaded to another device
     int sms = 0;
     if (cudaSetDevice(dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
         return HSPF_E_CUDA;
-    const uint64_t want = std::max<uint64_t>((total + kRouteThreads - 1) / kRouteThreads, 1);
-    const uint32_t blocks = (uint32_t)std::min<uint64_t>(want, (uint64_t)sms * blocks_per_sm);
+    const uint64_t want = std::max<uint64_t>((items + kRouteThreads - 1) / kRouteThreads, 1);
+    blocks = (uint32_t)std::min<uint64_t>(want, (uint64_t)sms * blocks_per_sm);
+    return HSPF_OK;
+}
+
+// ---- cell kernel ----------------------------------------------------------------------------------------------
+// A route stage is a cell functor, passed to every kernel by value as one parameter (as __grid_constant__ it costs the
+// IS-IS cell kernel two registers):
+//   refused(j)             the job gets Cell::empty() (its planes are undefined)
+//   status_word(j)         the job's status word
+//   operator()(j, p)       the cell of (job, prefix) as three words
+//   gather(j, area, v)     a plane value the host decode needs, 0 when out of range (j < n_jobs is checked here)
+//   static empty()         the cell of a refused job
+
+// The jobs' status words and the gathers (when asked for), then the cells.
+template <class Cell, int kMinBlocks>
+__global__ void __launch_bounds__(kRouteThreads, kMinBlocks)
+route_cells_kernel(const Cell cell, uint32_t n_jobs, uint32_t P, CellWords *__restrict__ cells,
+                   uint32_t *__restrict__ status_out, bool aligned16, uint32_t n_gather,
+                   const uint32_t *__restrict__ gather_job, const uint32_t *__restrict__ gather_area,
+                   const uint32_t *__restrict__ gather_v, uint64_t *__restrict__ gather_nh) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x, first = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (status_out)
+        for (uint64_t j = first; j < n_jobs; j += stride) status_out[j] = cell.status_word((uint32_t)j);
+    for (uint64_t g = first; g < n_gather; g += stride) {
+        const uint32_t job = gather_job[g];
+        gather_nh[g] = job < n_jobs ? cell.gather(job, gather_area ? gather_area[g] : 0, gather_v[g]) : 0;
+    }
+    store_route_cells(n_jobs, P, cell, Cell::empty(), cells, aligned16);
+}
+
+// Enqueues route_cells_kernel on the ctx stream: n_jobs x P cells, the jobs' status words when status_out is set,
+// n_gather gathers of (gather_job, gather_area (NULL: 0), gather_v).  The grid covers the largest of the three, one
+// wave of kBlocksPerSM blocks per SM at most; kMinBlocks is the kernel's launch bound.
+template <int kMinBlocks, uint32_t kBlocksPerSM = kMinBlocks, class Cell>
+int launch_route_cells(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs, uint32_t P,
+                       void *cells, uint32_t *status_out, uint32_t n_gather, const uint32_t *gather_job,
+                       const uint32_t *gather_area, const uint32_t *gather_v, uint64_t *gather_nh) {
+    if (!ctx || !cells) return HSPF_E_INVAL;
+    if (n_gather && (!gather_job || !gather_v || !gather_nh)) return HSPF_E_INVAL;
+    const uint64_t items = std::max<uint64_t>({(uint64_t)n_jobs * P, status_out ? n_jobs : 0u, n_gather});
+    if (items == 0) return HSPF_OK;
+    uint32_t blocks = 0;
+    const int rc = route_grid(ctx, table, items, kBlocksPerSM, blocks);
+    if (rc != HSPF_OK) return rc;
     const bool aligned16 = (reinterpret_cast<uintptr_t>(cells) & 15u) == 0;
-    launch(blocks, static_cast<cudaStream_t>(hspf_stream(ctx)), aligned16);
+    route_cells_kernel<Cell, kMinBlocks><<<blocks, kRouteThreads, 0, static_cast<cudaStream_t>(hspf_stream(ctx))>>>(
+        cell, n_jobs, P, static_cast<CellWords *>(cells), status_out, aligned16, n_gather, gather_job, gather_area,
+        gather_v, gather_nh);
     if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
     hspf_note_launches(ctx, 1);
     return HSPF_OK;
@@ -89,7 +171,7 @@ int launch_route_stage(hspf_ctx *ctx, const DeviceRouteTable &table, uint64_t to
 
 struct DeltaArgs {
     uint32_t n_jobs, P;
-    double inv_p;                     // 1.0 / P (set by launch_route_delta)
+    double inv_p;                     // 1.0 / P
     const uint64_t *base;             // base cells [n_base][P] as three words each
     uint32_t n_base;
     const uint32_t *base_of;          // [n_jobs] base row of each job; NULL: row 0
@@ -189,29 +271,33 @@ size_t route_delta_scan_bytes(uint64_t n_tiles);
 cudaError_t route_delta_scan(void *temp, size_t temp_bytes, const uint8_t *cnt, uint64_t *off, uint64_t n_tiles,
                              cudaStream_t st);
 
-// Validates the arguments every route-delta call shares and enqueues the stage on the ctx stream: the summaries and
-// the total are zeroed, then `count(blocks, stream, args)` launches pass A; with records, the scan and
-// `store(blocks, stream, args)` (pass B) follow.  `a.base` is the caller's base cell buffer; `blocks_per_sm` is
-// the kMinBlocks both passes were instantiated with.
-template <class Count, class Store>
-int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, DeltaArgs a, Count count, Store store,
-                       uint32_t blocks_per_sm = kRouteBlocksPerSM) {
-    if (!a.base || !a.job_out || !a.n_records || a.n_base == 0) return HSPF_E_INVAL;
+// Enqueues the route-delta stage over `cell` on the ctx stream: the summaries and the total are zeroed, then pass A
+// runs; with records, the scan and pass B follow.  `base` holds the base cells [n_base][P].  Both passes are
+// launch-bounded to kMinBlocks blocks per SM, and the grid is one wave of kBlocksPerSM blocks per SM at most.
+template <class Layout, int kMinBlocks, uint32_t kBlocksPerSM = kMinBlocks, class Cell>
+int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs, uint32_t P,
+                       const void *base, uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                       hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    if (!ctx || !base || !job_out || !n_records || n_base == 0) return HSPF_E_INVAL;
     // device buffers at their struct alignment
-    if ((reinterpret_cast<uintptr_t>(a.base) & 7u) || (reinterpret_cast<uintptr_t>(a.job_out) & 3u) ||
-        (reinterpret_cast<uintptr_t>(a.n_records) & 7u) || (reinterpret_cast<uintptr_t>(a.records) & 3u))
+    if ((reinterpret_cast<uintptr_t>(base) & 7u) || (reinterpret_cast<uintptr_t>(job_out) & 3u) ||
+        (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u))
         return HSPF_E_INVAL;
-    const int dev = hspf_ctx_device(ctx);
-    if (table.device != dev) return HSPF_E_INVAL;
-    if (cudaSetDevice(dev) != cudaSuccess) return HSPF_E_CUDA;
-    cudaStream_t st = static_cast<cudaStream_t>(hspf_stream(ctx));
-    const uint64_t total = (uint64_t)a.n_jobs * a.P, n_tiles = delta_tiles64(a.n_jobs, a.P);
+    const uint64_t total = (uint64_t)n_jobs * P, n_tiles = delta_tiles64(n_jobs, P);
+    // the grid covers the cells, or the jobs' status words when there are more jobs than cells
+    uint32_t blocks = 0;
+    const int rc = route_grid(ctx, table, std::max<uint64_t>(total, n_jobs), kBlocksPerSM, blocks);
+    if (rc != HSPF_OK) return rc;
     if (n_tiles > 0xFFFFFFFFull) return HSPF_E_INVAL;
-    a.inv_p = a.P ? 1.0 / a.P : 0.0;
-    if (cudaMemsetAsync(a.n_records, 0, sizeof(uint64_t), st) != cudaSuccess) return HSPF_E_CUDA;
-    if (a.n_jobs == 0) return HSPF_OK;
-    if (cudaMemsetAsync(a.job_out, 0, (size_t)a.n_jobs * sizeof(hl_route_delta_job), st) != cudaSuccess) return HSPF_E_CUDA;
-    const bool with_records = a.records && a.cap && n_tiles;
+    DeltaArgs a{};
+    a.n_jobs = n_jobs; a.P = P; a.inv_p = P ? 1.0 / P : 0.0;
+    a.base = static_cast<const uint64_t *>(base); a.n_base = n_base; a.base_of = base_of;
+    a.job_out = job_out; a.n_records = reinterpret_cast<unsigned long long *>(n_records);
+    cudaStream_t st = static_cast<cudaStream_t>(hspf_stream(ctx));
+    if (cudaMemsetAsync(n_records, 0, sizeof(uint64_t), st) != cudaSuccess) return HSPF_E_CUDA;
+    if (n_jobs == 0) return HSPF_OK;
+    if (cudaMemsetAsync(job_out, 0, (size_t)n_jobs * sizeof(hl_route_delta_job), st) != cudaSuccess) return HSPF_E_CUDA;
+    const bool with_records = records && cap && n_tiles;
     size_t scan_bytes = 0;
     char *ws = nullptr;
     if (with_records) {
@@ -221,22 +307,19 @@ int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, DeltaArgs a
         if (!ws) return HSPF_E_NOMEM;
         a.tile_off = reinterpret_cast<const uint64_t *>(ws);
         a.tile_cnt = reinterpret_cast<uint8_t *>(ws + off_bytes);
+        a.records = records; a.cap = cap;
         ws += off_bytes + cnt_bytes;
-    } else {
-        a.tile_cnt = nullptr; a.tile_off = nullptr; a.records = nullptr; a.cap = 0;
     }
-    // the grid covers the cells, or the jobs' status words when there are more jobs than cells
-    cudaError_t scan = cudaSuccess;
-    const int rc = launch_route_stage(ctx, table, std::max<uint64_t>(total, a.n_jobs), a.base,
-                                      [&](uint32_t blocks, cudaStream_t s, bool) {
-        count(blocks, s, a);
-        if (!with_records) return;
-        scan = route_delta_scan(ws, scan_bytes, a.tile_cnt, const_cast<uint64_t *>(a.tile_off), n_tiles, s);
-        if (scan != cudaSuccess) return;
-        store(blocks, s, a);
-        hspf_note_launches(ctx, 2);                            // the scan (counted as one) and pass B
-    }, blocks_per_sm);
-    return rc != HSPF_OK ? rc : (scan != cudaSuccess ? HSPF_E_CUDA : HSPF_OK);
+    route_delta_count_kernel<Layout, Cell, kMinBlocks><<<blocks, kRouteThreads, 0, st>>>(cell, a);
+    if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
+    hspf_note_launches(ctx, 1);
+    if (!with_records) return HSPF_OK;
+    if (route_delta_scan(ws, scan_bytes, a.tile_cnt, const_cast<uint64_t *>(a.tile_off), n_tiles, st) != cudaSuccess)
+        return HSPF_E_CUDA;
+    route_delta_store_kernel<Layout, Cell, kMinBlocks><<<blocks, kRouteThreads, 0, st>>>(cell, a);
+    if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
+    hspf_note_launches(ctx, 2);                                 // the scan (counted as one) and pass B
+    return HSPF_OK;
 }
 
 }  // namespace hspf

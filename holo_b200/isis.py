@@ -454,13 +454,9 @@ def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, 
     """hspf_isis_routes_batch / _batch16 over DEVICE planes (rs_*: capi.ResultStruct or capi.Result16Struct holding
     device pointers, one per topology; rs_mt6 may be None unless the table has an MT-IPv6 root); cells_ptr: device
     buffer of n_jobs * rt.n_prefixes cells.  Enqueued on the ctx stream; the table must have been uploaded."""
-    lib = ctx.lib
-    narrow = isinstance(rs_std if rs_std is not None else rs_mt6, capi.Result16Struct)
-    fn = lib.hspf_isis_routes_batch16 if narrow else lib.hspf_isis_routes_batch
-    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs_std) if rs_std is not None else None,
-            C.byref(rs_mt6) if rs_mt6 is not None else None, cells_ptr)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_isis_routes_batch", rs_std if rs_std is not None else rs_mt6, rt.handle, n_jobs,
+                           C.byref(rs_std) if rs_std is not None else None,
+                           C.byref(rs_mt6) if rs_mt6 is not None else None, cells_ptr)
 
 
 def routes_delta_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, rs_mt6, base_ptr: int, n_base: int,
@@ -470,14 +466,10 @@ def routes_delta_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs_std, 
     every job), without storing them.  job_out_ptr: [n_jobs] route_table.DELTA_JOB_DT; records_ptr: [cap]
     route_table.DELTA_DT in (job, prefix) order (0 or cap 0: summaries only); n_records_ptr: u64 total.  All device
     pointers; enqueued on the ctx stream."""
-    lib = ctx.lib
-    narrow = isinstance(rs_std if rs_std is not None else rs_mt6, capi.Result16Struct)
-    fn = lib.hspf_isis_routes_delta16 if narrow else lib.hspf_isis_routes_delta
-    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs_std) if rs_std is not None else None,
-            C.byref(rs_mt6) if rs_mt6 is not None else None, base_ptr or None, n_base, base_of_ptr or None,
-            job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_isis_routes_delta", rs_std if rs_std is not None else rs_mt6, rt.handle, n_jobs,
+                           C.byref(rs_std) if rs_std is not None else None,
+                           C.byref(rs_mt6) if rs_mt6 is not None else None, base_ptr or None, n_base,
+                           base_of_ptr or None, job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
 
 
 def routes_from_cells(inst: dict, rt: RouteTable, cells: np.ndarray, std=None, mt6=None, ov_std=(), ov_mt6=()) -> IsisRib:

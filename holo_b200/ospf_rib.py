@@ -377,13 +377,9 @@ def rib_cells_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr
     device pointers); roots_ptr: device u32[n_jobs] root vertices; cells_ptr: device buffer of n_jobs * rt.n_prefixes
     RIB_CELL_DT; status_out_ptr: device u32[n_jobs] or 0.  Enqueued on the ctx stream; the table must have been
     uploaded."""
-    lib = ctx.lib
-    narrow = isinstance(rs, capi.Result16Struct)
-    fn = lib.hspf_ospfv2_rib_cells16 if narrow else lib.hspf_ospfv2_rib_cells
-    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), roots_ptr or None, cells_ptr, status_out_ptr or None, n_gather,
-            gather_job_ptr or None, gather_v_ptr or None, gather_nh_ptr or None)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_ospfv2_rib_cells", rs, rt.handle, n_jobs, C.byref(rs), roots_ptr or None, cells_ptr,
+                           status_out_ptr or None, n_gather, gather_job_ptr or None, gather_v_ptr or None,
+                           gather_nh_ptr or None)
 
 
 def rib_delta_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr: int, base_ptr: int, n_base: int,
@@ -393,13 +389,9 @@ def rib_delta_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr
     unperturbed job of the same root; base_of_ptr: [n_jobs] u32 rows, 0 for row 0 of every job), without storing them.
     job_out_ptr: [n_jobs] route_table.DELTA_JOB_DT; records_ptr: [cap] route_table.DELTA_DT in (job, prefix) order
     (0 or cap 0: summaries only); n_records_ptr: u64 total.  All device pointers; enqueued on the ctx stream."""
-    lib = ctx.lib
-    narrow = isinstance(rs, capi.Result16Struct)
-    fn = lib.hspf_ospfv2_rib_delta16 if narrow else lib.hspf_ospfv2_rib_delta
-    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), roots_ptr or None, base_ptr or None, n_base, base_of_ptr or None,
-            job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_ospfv2_rib_delta", rs, rt.handle, n_jobs, C.byref(rs), roots_ptr or None,
+                           base_ptr or None, n_base, base_of_ptr or None, job_out_ptr or None, records_ptr or None, cap,
+                           n_records_ptr or None)
 
 
 def _call_rib_from_cells(fn, area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh, route_dt, nh_dt) -> Rib:
@@ -484,11 +476,8 @@ class AbrRibTable(route_table.RouteTable):
 
 
 def _planes_array(planes: list):
-    """Host array of capi.ResultStruct / capi.Result16Struct (one per area, device pointers) and whether narrow."""
-    narrow = isinstance(planes[0], capi.Result16Struct)
-    cls = capi.Result16Struct if narrow else capi.ResultStruct
-    arr = (cls * len(planes))(*planes)
-    return arr, narrow
+    """Host array of capi.ResultStruct / capi.Result16Struct (one per area, device pointers)."""
+    return (type(planes[0]) * len(planes))(*planes)
 
 
 def abr_rib_cells_device(ctx: capi.Context, rt: AbrRibTable, n_jobs: int, planes: list, n_rows, rows_ptr: int,
@@ -498,13 +487,10 @@ def abr_rib_cells_device(ctx: capi.Context, rt: AbrRibTable, n_jobs: int, planes
     capi.Result16Struct per area, in the table's order; n_rows: rows of each area's planes; rows_ptr: device
     u32[n_jobs, n_areas]; cells_ptr: device [n_jobs, rt.n_prefixes] RIB_CELL_DT; gathers as (job, area, vertex)
     triples.  Enqueued on the ctx stream; the table must have been uploaded."""
-    arr, narrow = _planes_array(planes)
     nr = np.ascontiguousarray(n_rows, np.uint32)
-    fn = ctx.lib.hspf_ospfv2_abr_rib_cells16 if narrow else ctx.lib.hspf_ospfv2_abr_rib_cells
-    rc = fn(ctx.handle, rt.handle, n_jobs, arr, nr.ctypes.data, rows_ptr or None, cells_ptr or None, status_out_ptr or None,
-            n_gather, gather_job_ptr or None, gather_area_ptr or None, gather_v_ptr or None, gather_nh_ptr or None)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_ospfv2_abr_rib_cells", planes[0], rt.handle, n_jobs, _planes_array(planes),
+                           nr.ctypes.data, rows_ptr or None, cells_ptr or None, status_out_ptr or None, n_gather,
+                           gather_job_ptr or None, gather_area_ptr or None, gather_v_ptr or None, gather_nh_ptr or None)
 
 
 def abr_rib_delta_device(ctx: capi.Context, rt: AbrRibTable, n_jobs: int, planes: list, n_rows, rows_ptr: int,
@@ -512,13 +498,10 @@ def abr_rib_delta_device(ctx: capi.Context, rt: AbrRibTable, n_jobs: int, planes
                          n_records_ptr: int):
     """hspf_ospfv2_abr_rib_delta / _delta16: each job's cells (as abr_rib_cells_device) compared with its base row of
     base_ptr on the device, as rib_delta_device."""
-    arr, narrow = _planes_array(planes)
     nr = np.ascontiguousarray(n_rows, np.uint32)
-    fn = ctx.lib.hspf_ospfv2_abr_rib_delta16 if narrow else ctx.lib.hspf_ospfv2_abr_rib_delta
-    rc = fn(ctx.handle, rt.handle, n_jobs, arr, nr.ctypes.data, rows_ptr or None, base_ptr or None, n_base,
-            base_of_ptr or None, job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_ospfv2_abr_rib_delta", planes[0], rt.handle, n_jobs, _planes_array(planes),
+                           nr.ctypes.data, rows_ptr or None, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
 
 
 def abr_rib_from_cells(areas: list, rt: AbrRibTable, cells: np.ndarray, gather_area, gather_v, gather_nh) -> Rib:

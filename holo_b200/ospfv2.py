@@ -399,13 +399,8 @@ def routes_batch_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs, cell
     """hspf_ospfv2_routes_batch / _batch16 over DEVICE planes (rs: capi.ResultStruct or capi.Result16Struct
     holding device pointers); cells_ptr: device buffer of n_jobs * rt.n_prefixes cells.  Enqueued on the ctx
     stream; the table must have been uploaded."""
-    lib = ctx.lib
-    narrow = isinstance(rs, capi.Result16Struct)
-    fn = lib.hspf_ospfv2_routes_batch16 if narrow else lib.hspf_ospfv2_routes_batch
-    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), cells_ptr, n_gather, gather_job_ptr or None,
-            gather_v_ptr or None, gather_nh_ptr or None)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_ospfv2_routes_batch", rs, rt.handle, n_jobs, C.byref(rs), cells_ptr, n_gather,
+                           gather_job_ptr or None, gather_v_ptr or None, gather_nh_ptr or None)
 
 
 def routes_delta_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs, base_ptr: int, n_base: int, base_of_ptr: int,
@@ -415,13 +410,8 @@ def routes_delta_device(ctx: capi.Context, rt: RouteTable, n_jobs: int, rs, base
     every job), without storing them.  job_out_ptr: [n_jobs] route_table.DELTA_JOB_DT; records_ptr: [cap]
     route_table.DELTA_DT in (job, prefix) order (0 or cap 0: summaries only); n_records_ptr: u64 total.  All device
     pointers; enqueued on the ctx stream."""
-    lib = ctx.lib
-    narrow = isinstance(rs, capi.Result16Struct)
-    fn = lib.hspf_ospfv2_routes_delta16 if narrow else lib.hspf_ospfv2_routes_delta
-    rc = fn(ctx.handle, rt.handle, n_jobs, C.byref(rs), base_ptr or None, n_base, base_of_ptr or None, job_out_ptr or None,
-            records_ptr or None, cap, n_records_ptr or None)
-    if rc != capi.HSPF_OK:
-        raise capi.HspfError(rc, ctx.last_error())
+    route_table.call_stage(ctx, "hspf_ospfv2_routes_delta", rs, rt.handle, n_jobs, C.byref(rs), base_ptr or None, n_base,
+                           base_of_ptr or None, job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
 
 
 def routes_from_cells(area: Ospfv2Area, rt: RouteTable, cells: np.ndarray, gather_v, gather_nh) -> Ospfv2Result:

@@ -22,6 +22,15 @@ def copy_records(ptr, n: int, dt) -> np.ndarray:
     return np.frombuffer(C.string_at(ptr, n * dt.itemsize), dt).copy() if n else np.zeros(0, dt)
 
 
+def call_stage(ctx: capi.Context, name: str, rs, *args):
+    """Calls route-stage entry point `name` (ctx first, then `args`), or its 16-bit twin `name`16 when the planes
+    are 16-bit (`rs` a capi.Result16Struct); raises HspfError on a return code other than HSPF_OK."""
+    fn = getattr(ctx.lib, name + "16" if isinstance(rs, capi.Result16Struct) else name)
+    rc = fn(ctx.handle, *args)
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, ctx.last_error())
+
+
 class RouteTable:
     """A route table of the batched route stage: prefixes in route-table order, `off` [n_prefixes + 1] into the
     16-byte contributor records `contribs`, and `upload(ctx)`, which copies the table to the device.  Subclasses
