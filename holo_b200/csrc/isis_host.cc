@@ -654,8 +654,9 @@ int topology_flat(const hl_isis_instance *in, uint8_t mt_id, hspf_isis_flat &f, 
 // The contributions compute_routes (spf.rs:838-941) makes in one topology, in its order: every
 // vertex `visit(v)` accepts, in id_tree (= vertex index) order, with a valid zeroth LSP; its valid
 // fragments in LspId order; per fragment the ATT-bit default routes, then TLV 128, 130, 135 and
-// 236/237 entries.  emit(v, prefix, len, entry metric, external, entry with its Prefix-SID or NULL).
-// Which contributions there are depends only on the LSDB and the instance configuration.
+// 236/237 entries.  emit(v, prefix, len, entry metric, external, entry with its Prefix-SID or NULL, index of the
+// entry in lvl.ipreaches or -1 for an ATT-bit default route).  Which contributions there are depends only on the
+// LSDB and the instance configuration.
 template <class Visit, class Emit>
 void for_each_contribution(const hl_isis_instance *in, const hspf_isis_flat &f, uint8_t mt_id, Visit visit, Emit emit) {
     const hl_isis_level &l0 = in->lvl;
@@ -691,27 +692,28 @@ void for_each_contribution(const hl_isis_instance *in, const hspf_isis_flat &f, 
             const auto &lsp = l0.lsps[i];
             if (!lsp.seqno || !lsp.rem_lifetime) continue;
             if (att_bit && in->level == 1 && (in->level_type == 1 || !attached)) {
-                if (ipv4_enabled) emit(v, hl_ip_addr{}, 0, 0, false, nullptr);
-                if (ipv6_enabled) { hl_ip_addr z6{}; z6.is_v6 = 1; emit(v, z6, 0, 0, false, nullptr); }
+                if (ipv4_enabled) emit(v, hl_ip_addr{}, 0, 0, false, nullptr, -1);
+                if (ipv6_enabled) { hl_ip_addr z6{}; z6.is_v6 = 1; emit(v, z6, 0, 0, false, nullptr, -1); }
             }
             const hl_isis_ipreach *ip = l0.ipreaches + lsp.ipreach_off;
+            const auto at = [&](uint32_t k) { return (int32_t)(lsp.ipreach_off + k); };
             if (mt_id == HL_ISIS_MT_STANDARD && ipv4_enabled) {
                 if (std_en) {
                     for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
-                        if (ip[k].kind == HL_ISIS_IP_V4_INTERNAL) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, false, nullptr);
+                        if (ip[k].kind == HL_ISIS_IP_V4_INTERNAL) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, false, nullptr, at(k));
                     for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
-                        if (ip[k].kind == HL_ISIS_IP_V4_EXTERNAL) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, true, nullptr);
+                        if (ip[k].kind == HL_ISIS_IP_V4_EXTERNAL) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, true, nullptr, at(k));
                 }
                 if (wide_en)
                     for (uint32_t k = 0; k < lsp.n_ipreach; ++k)
                         if (ip[k].kind == HL_ISIS_IP_V4_EXT && ip[k].metric <= kMaxWide)
-                            emit(v, ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external != 0, &ip[k]);
+                            emit(v, ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external != 0, &ip[k], at(k));
             }
             if (ipv6_enabled)
                 for (uint32_t k = 0; k < lsp.n_ipreach; ++k) {
                     const bool take = mt_id == HL_ISIS_MT_IPV6 ? (ip[k].kind == HL_ISIS_IP_MT_V6 && ip[k].mt_id == HL_ISIS_MT_IPV6)
                                                                : (ip[k].kind == HL_ISIS_IP_V6);
-                    if (take) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external != 0, &ip[k]);
+                    if (take) emit(v, ip[k].prefix, ip[k].len, ip[k].metric, ip[k].external != 0, &ip[k], at(k));
                 }
         }
     }
@@ -746,7 +748,7 @@ int topology_routes(const hl_isis_instance *in, const hspf_isis_flat &f, uint8_t
     int rc = local_nexthops(f, in, mt_id, root, dist, hops, f.cost.data(), vnh);
     if (rc) return rc;
     auto add = [&](uint32_t v, const hl_ip_addr &prefix, uint8_t len, uint32_t nmetric, bool external,
-                   const hl_isis_ipreach *src) {
+                   const hl_isis_ipreach *src, int32_t) {
         auto build = [&](std::map<hl_ip_addr, RNh, IpLess> &m) {
             for (const LNh &nh : vnh[v]) {
                 hl_ip_addr addr;
@@ -873,10 +875,138 @@ extern "C" int hspf_isis_routes_from_planes(const hl_isis_instance *in, const ui
 /* ---- batched route stage: the table and the per-job decode (isis_route_cells.h) ------------- */
 #include <memory>
 
+#include "isis_l1l2_rib_cells.h"
 #include "isis_route_cells.h"
 
 namespace {
 const uint8_t kTopologies[2] = {HL_ISIS_MT_STANDARD, HL_ISIS_MT_IPV6};    // table topology 0, 1
+
+struct RawContrib { NetKey key; hspf::IsisContrib c; int32_t src; };
+
+// Every contribution compute_routes can make in the instance's enabled topologies, in NetKey order and, within a
+// prefix, in walk order; entries whose lvl.ipreaches byte in `drop` is non-zero are left out (drop NULL: none).
+// Sets each topology's vertex count and root (kNone: the root owns no LSP there, or the topology is off).
+int collect_contributions(const hl_isis_instance *in, const uint8_t *drop, std::vector<RawContrib> &raw,
+                          uint32_t n_vertices[2], uint32_t root_out[2]) {
+    for (uint32_t t = 0; t < 2; ++t) {
+        n_vertices[t] = 0;
+        root_out[t] = kNone;
+        const uint8_t mt_id = kTopologies[t];
+        if (mt_id == HL_ISIS_MT_IPV6 && !in->mt_ipv6_enabled) continue;
+        hspf_isis_flat f;
+        uint32_t root = 0;
+        bool have_root = false;
+        const int rc = topology_flat(in, mt_id, f, root, have_root);
+        if (rc) return rc;
+        n_vertices[t] = (uint32_t)f.ids.size();
+        if (!have_root) continue;
+        root_out[t] = root;
+        // every vertex: whether a contributor is on the SPT is the job's business
+        for_each_contribution(in, f, mt_id, [](uint32_t) { return true; },
+                              [&](uint32_t v, const hl_ip_addr &prefix, uint8_t len, uint32_t nmetric, bool external,
+                                  const hl_isis_ipreach *src, int32_t idx) {
+                                  if (drop && idx >= 0 && drop[idx]) return;
+                                  RawContrib r{};
+                                  r.key = NetKey{prefix, len};
+                                  r.c.vertex = v; r.c.metric = nmetric; r.c.topology = (uint8_t)t;
+                                  r.c.external = external ? 1 : 0;
+                                  r.c.has_psid = (src && src->has_psid) ? 1 : 0;
+                                  r.c.sr = (r.c.has_psid && in->sr_enabled) ? 1 : 0;
+                                  r.src = src ? (int32_t)(src - in->lvl.ipreaches) : -1;
+                                  raw.push_back(r);
+                              });
+    }
+    // NetKey order, walk order within a prefix
+    std::stable_sort(raw.begin(), raw.end(), [](const RawContrib &a, const RawContrib &b) { return a.key < b.key; });
+    return HSPF_OK;
+}
+
+// One job's decode state for one level's topologies: the flat, the job's planes, and what each first-hop atom
+// resolves to (hspf_isis_routes_from_cells, hspf_isis_l1l2_rib_from_cells).
+struct DecodeTopo {
+    hspf_isis_flat f;
+    const uint16_t *hops = nullptr;
+    bool live = false;
+    LNh atom_nh[64];
+    bool atom_has[64] = {};
+};
+
+// The job's planes of topology t of `in` (pl[t]); the table recorded n_vertices[t] and root[t] for that instance.
+int decode_topos(const hl_isis_instance *in, const uint32_t n_vertices[2], const uint32_t table_root[2],
+                 const hspf_isis_job_planes pl[2], DecodeTopo tp[2]) {
+    for (uint32_t t = 0; t < 2; ++t) {
+        const uint8_t mt_id = kTopologies[t];
+        if (mt_id == HL_ISIS_MT_IPV6 && !in->mt_ipv6_enabled) continue;
+        DecodeTopo &T = tp[t];
+        uint32_t root = 0;
+        bool have_root = false;
+        int rc = topology_flat(in, mt_id, T.f, root, have_root);
+        if (rc) return rc;
+        // not the instance the table was built from
+        if (T.f.ids.size() != n_vertices[t] || (have_root ? root : kNone) != table_root[t]) return HSPF_E_INVAL;
+        if (!have_root) continue;
+        const uint32_t *dist = pl[t].dist;
+        T.hops = pl[t].hops;
+        const uint32_t n_ov = pl[t].n_ov;
+        if (!dist || !T.hops || (n_ov && (!pl[t].ov_edge || !pl[t].ov_cost))) return HSPF_E_INVAL;
+        std::vector<uint32_t> cost(T.f.cost);
+        for (uint32_t k = 0; k < n_ov; ++k) {
+            if (pl[t].ov_edge[k] >= cost.size()) return HSPF_E_INVAL;
+            cost[pl[t].ov_edge[k]] = pl[t].ov_cost[k];
+        }
+        std::vector<uint32_t> pop, pos;
+        pop_order((uint32_t)T.f.ids.size(), dist, pop, pos);
+        const std::map<uint32_t, LNh> first_hop = first_hop_replay(T.f, in, mt_id, root, dist, T.hops, cost.data(), pop, pos);
+        hspf_csr csr;
+        fill_csr(T.f, &csr);
+        uint32_t n_atoms = 0;
+        if (hspf_atom_count(&csr, root, &n_atoms) != HSPF_OK) return HSPF_E_INVAL;
+        for (uint32_t a = 0; a < std::min<uint32_t>(n_atoms, 64); ++a) {
+            uint32_t tail = 0, edge = 0;
+            if (hspf_atom_decode(&csr, root, a, &tail, &edge) != HSPF_OK) continue;
+            auto it = first_hop.find(edge);
+            if (it == first_hop.end()) continue;
+            T.atom_nh[a] = it->second;
+            T.atom_has[a] = true;
+        }
+        T.live = true;
+    }
+    return HSPF_OK;
+}
+
+// The route of a present cell won by contributor k (src: its lvl.ipreaches index) of `in`.
+int decode_route(const hl_isis_instance *in, const DecodeTopo tp[2], const SrView &sr, const hspf::IsisContrib &k,
+                 int32_t src, const hl_isis_route_cell &c, bool v6, RouteE &r) {
+    const DecodeTopo &T = tp[k.topology];
+    if (!T.live || k.vertex >= T.f.ids.size()) return HSPF_E_INVAL;
+    r = RouteE{};
+    r.flags = (c.flags & HL_CELL_CONNECTED) ? HL_ROUTE_CONNECTED : 0;
+    r.type = route_type(in, k.external != 0);
+    r.metric = c.metric;
+    // the union of the best-metric contributors' next hops; an address reached over two different
+    // adjacencies keeps whichever `add` wrote last, which the cell cannot tell
+    for (uint64_t m = c.nh_mask; m; m &= m - 1) {
+        const uint32_t a = (uint32_t)__builtin_ctzll(m);
+        hl_ip_addr addr;
+        if (!T.atom_has[a] || !nh_addr(T.atom_nh[a], v6, addr)) continue;
+        const RNh x{T.atom_nh[a].sysid, T.atom_nh[a].iface, addr};
+        auto ins = r.nh.emplace(addr, x);
+        if (!ins.second && (ins.first->second.sysid != x.sysid || ins.first->second.iface != x.iface))
+            return HSPF_E_UNSUPPORTED;
+    }
+    while (r.nh.size() > in->max_paths) r.nh.erase(std::prev(r.nh.end()));
+    if (k.has_psid) {
+        if (src < 0 || (uint32_t)src >= in->lvl.n_ipreaches) return HSPF_E_INVAL;
+        const hl_isis_ipreach &e = in->lvl.ipreaches[src];
+        r.psid = PrefixSid{true, e.psid_flags, e.psid_is_label != 0, e.psid_value};
+    }
+    // all best-metric contributions come from the winner's vertex (else the cell is flagged):
+    // one update with its context gives the labels every repeated update would
+    if (in->sr_enabled && r.psid.present)
+        sr.update(r, in->system_id, T.f.ids[k.vertex], v6, T.hops[k.vertex] == 0, T.hops[k.vertex] == 1);
+    return HSPF_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -892,35 +1022,9 @@ int hspf_isis_rtable_create(const hl_isis_instance *in, hspf_isis_rtable **out) 
     *out = nullptr;
     try {
         auto rt = std::make_unique<hspf_isis_rtable>();
-        struct Raw { NetKey key; hspf::IsisContrib c; int32_t src; };
-        std::vector<Raw> raw;
-        for (uint32_t t = 0; t < 2; ++t) {
-            const uint8_t mt_id = kTopologies[t];
-            if (mt_id == HL_ISIS_MT_IPV6 && !in->mt_ipv6_enabled) continue;
-            hspf_isis_flat f;
-            uint32_t root = 0;
-            bool have_root = false;
-            const int rc = topology_flat(in, mt_id, f, root, have_root);
-            if (rc) return rc;
-            rt->n_vertices[t] = (uint32_t)f.ids.size();
-            if (!have_root) continue;
-            rt->root[t] = root;
-            // every vertex: whether a contributor is on the SPT is the job's business
-            for_each_contribution(in, f, mt_id, [](uint32_t) { return true; },
-                                  [&](uint32_t v, const hl_ip_addr &prefix, uint8_t len, uint32_t nmetric, bool external,
-                                      const hl_isis_ipreach *src) {
-                                      Raw r{};
-                                      r.key = NetKey{prefix, len};
-                                      r.c.vertex = v; r.c.metric = nmetric; r.c.topology = (uint8_t)t;
-                                      r.c.external = external ? 1 : 0;
-                                      r.c.has_psid = (src && src->has_psid) ? 1 : 0;
-                                      r.c.sr = (r.c.has_psid && in->sr_enabled) ? 1 : 0;
-                                      r.src = src ? (int32_t)(src - in->lvl.ipreaches) : -1;
-                                      raw.push_back(r);
-                                  });
-        }
-        // NetKey order, walk order within a prefix
-        std::stable_sort(raw.begin(), raw.end(), [](const Raw &a, const Raw &b) { return a.key < b.key; });
+        std::vector<RawContrib> raw;
+        const int rc = collect_contributions(in, nullptr, raw, rt->n_vertices, rt->root);
+        if (rc) return rc;
         for (size_t i = 0; i < raw.size(); ++i) {
             if (i == 0 || raw[i - 1].key < raw[i].key) {
                 rt->prefix.push_back(raw[i].key.a); rt->len.push_back(raw[i].key.len); rt->off.push_back((uint32_t)i);
@@ -962,53 +1066,11 @@ int hspf_isis_routes_from_cells(const hl_isis_instance *in, const hspf_isis_rtab
                                 hl_isis_rib *out) {
     if (!in || !rt || !out || (!cells && !rt->prefix.empty())) return HSPF_E_INVAL;
     try {
-        // per topology: the flat, the job's planes, and what each first-hop atom resolves to
-        struct Topo {
-            hspf_isis_flat f;
-            const uint16_t *hops = nullptr;
-            bool live = false;
-            LNh atom_nh[64];
-            bool atom_has[64] = {};
-        };
-        auto tp = std::make_unique<Topo[]>(2);
-        for (uint32_t t = 0; t < 2; ++t) {
-            const uint8_t mt_id = kTopologies[t];
-            if (mt_id == HL_ISIS_MT_IPV6 && !in->mt_ipv6_enabled) continue;
-            Topo &T = tp[t];
-            uint32_t root = 0;
-            bool have_root = false;
-            int rc = topology_flat(in, mt_id, T.f, root, have_root);
-            if (rc) return rc;
-            // not the instance the table was built from
-            if (T.f.ids.size() != rt->n_vertices[t] || (have_root ? root : kNone) != rt->root[t]) return HSPF_E_INVAL;
-            if (!have_root) continue;
-            const uint32_t *dist = t ? dist_mt6 : dist_std;
-            T.hops = t ? hops_mt6 : hops_std;
-            const uint32_t n_ov = t ? n_ov_mt6 : n_ov_std;
-            const uint32_t *ov_edge = t ? ov_edge_mt6 : ov_edge_std, *ov_cost = t ? ov_cost_mt6 : ov_cost_std;
-            if (!dist || !T.hops || (n_ov && (!ov_edge || !ov_cost))) return HSPF_E_INVAL;
-            std::vector<uint32_t> cost(T.f.cost);
-            for (uint32_t k = 0; k < n_ov; ++k) {
-                if (ov_edge[k] >= cost.size()) return HSPF_E_INVAL;
-                cost[ov_edge[k]] = ov_cost[k];
-            }
-            std::vector<uint32_t> pop, pos;
-            pop_order((uint32_t)T.f.ids.size(), dist, pop, pos);
-            const std::map<uint32_t, LNh> first_hop = first_hop_replay(T.f, in, mt_id, root, dist, T.hops, cost.data(), pop, pos);
-            hspf_csr csr;
-            fill_csr(T.f, &csr);
-            uint32_t n_atoms = 0;
-            if (hspf_atom_count(&csr, root, &n_atoms) != HSPF_OK) return HSPF_E_INVAL;
-            for (uint32_t a = 0; a < std::min<uint32_t>(n_atoms, 64); ++a) {
-                uint32_t tail = 0, edge = 0;
-                if (hspf_atom_decode(&csr, root, a, &tail, &edge) != HSPF_OK) continue;
-                auto it = first_hop.find(edge);
-                if (it == first_hop.end()) continue;
-                T.atom_nh[a] = it->second;
-                T.atom_has[a] = true;
-            }
-            T.live = true;
-        }
+        const hspf_isis_job_planes pl[2] = {{dist_std, hops_std, n_ov_std, ov_edge_std, ov_cost_std},
+                                            {dist_mt6, hops_mt6, n_ov_mt6, ov_edge_mt6, ov_cost_mt6}};
+        auto tp = std::make_unique<DecodeTopo[]>(2);
+        int rc = decode_topos(in, rt->n_vertices, rt->root, pl, tp.get());
+        if (rc) return rc;
         const SrView sr(in->lvl);
         std::map<NetKey, RouteE> rib;
         const uint32_t P = (uint32_t)rt->prefix.size();
@@ -1017,37 +1079,221 @@ int hspf_isis_routes_from_cells(const hl_isis_instance *in, const hspf_isis_rtab
             if (!(c.flags & HL_CELL_PRESENT)) continue;
             if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
             if (c.winner < rt->off[p] || c.winner >= rt->off[p + 1]) return HSPF_E_INVAL;
-            const hspf::IsisContrib &k = rt->contribs[c.winner];
-            const Topo &T = tp[k.topology];
-            if (!T.live || k.vertex >= T.f.ids.size()) return HSPF_E_INVAL;
-            const bool v6 = rt->prefix[p].is_v6 != 0;
-            RouteE r{};
-            r.flags = (c.flags & HL_CELL_CONNECTED) ? HL_ROUTE_CONNECTED : 0;
-            r.type = route_type(in, k.external != 0);
-            r.metric = c.metric;
-            // the union of the best-metric contributors' next hops; an address reached over two different
-            // adjacencies keeps whichever `add` wrote last, which the cell cannot tell
-            for (uint64_t m = c.nh_mask; m; m &= m - 1) {
-                const uint32_t a = (uint32_t)__builtin_ctzll(m);
-                hl_ip_addr addr;
-                if (!T.atom_has[a] || !nh_addr(T.atom_nh[a], v6, addr)) continue;
-                const RNh x{T.atom_nh[a].sysid, T.atom_nh[a].iface, addr};
-                auto ins = r.nh.emplace(addr, x);
-                if (!ins.second && (ins.first->second.sysid != x.sysid || ins.first->second.iface != x.iface))
-                    return HSPF_E_UNSUPPORTED;
-            }
-            while (r.nh.size() > in->max_paths) r.nh.erase(std::prev(r.nh.end()));
-            if (k.has_psid) {
-                const int32_t s = rt->src[c.winner];
-                if (s < 0 || (uint32_t)s >= in->lvl.n_ipreaches) return HSPF_E_INVAL;
-                const hl_isis_ipreach &e = in->lvl.ipreaches[s];
-                r.psid = PrefixSid{true, e.psid_flags, e.psid_is_label != 0, e.psid_value};
-            }
-            // all best-metric contributions come from the winner's vertex (else the cell is flagged):
-            // one update with its context gives the labels every repeated update would
-            if (in->sr_enabled && r.psid.present)
-                sr.update(r, in->system_id, T.f.ids[k.vertex], v6, T.hops[k.vertex] == 0, T.hops[k.vertex] == 1);
+            RouteE r;
+            rc = decode_route(in, tp.get(), sr, rt->contribs[c.winner], rt->src[c.winner], c, rt->prefix[p].is_v6 != 0, r);
+            if (rc) return rc;
             rib.emplace_hint(rib.end(), NetKey{rt->prefix[p], (uint8_t)rt->len[p]}, std::move(r));
+        }
+        return emit_rib(rib, out);
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+}  // extern "C"
+
+/* ---- routing table of an L1/L2 router (isis_l1l2_rib_cells.h) -------------------------------- */
+namespace {
+
+// The own-LSP argument of hspf_isis_l1l2_ribtable_create needs every L1 entry that lsp_propagate_l1_to_l2 could
+// carry into the router's L2 LSP (its static filters, holo-isis lsdb.rs:1163-1258, as hspf_isis_l1_to_l2 applies
+// them, up/down bits aside) to be an entry compute_routes feeds into the L1 table (spf.rs:862-882, vertex_networks
+// spf.rs:1141, for_each_contribution above) whenever its originator is on the same topology's SPT.  False when
+// some entry breaks that.
+bool propagation_within_routes(const hl_isis_instance *l1, const hl_isis_instance *l2, const hl_isis_summary *cfg,
+                               uint32_t n_cfg) {
+    const hl_isis_level &lv = l1->lvl;
+    auto std_on = [](uint8_t t) { return t == HL_ISIS_METRIC_STANDARD || t == HL_ISIS_METRIC_BOTH; };
+    auto wide_on = [](uint8_t t) { return t == HL_ISIS_METRIC_WIDE || t == HL_ISIS_METRIC_BOTH; };
+    const bool narrow = std_on(lv.metric_type) && std_on(l2->lvl.metric_type);
+    const bool wide = wide_on(lv.metric_type) && wide_on(l2->lvl.metric_type);
+    const bool mt6 = l1->mt_ipv6_enabled != 0;
+    std::unordered_set<uint64_t> zeroth;          // LAN ids with a valid zeroth LSP
+    for (uint32_t i = 0; i < lv.n_lsps; ++i)
+        if (lv.lsps[i].fragment == 0 && lv.lsps[i].seqno && lv.lsps[i].rem_lifetime) zeroth.insert(lv.lsps[i].lan_id);
+    for (uint32_t i = 0; i < lv.n_lsps; ++i) {
+        const hl_isis_lsp &lsp = lv.lsps[i];
+        if (!lsp.seqno || !lsp.rem_lifetime || is_pn(lsp.lan_id) || (lsp.lan_id >> 8) == l1->system_id) continue;
+        const bool has_zeroth = zeroth.count(lsp.lan_id) != 0;
+        for (uint32_t k = lsp.ipreach_off; k < lsp.ipreach_off + lsp.n_ipreach; ++k) {
+            const hl_isis_ipreach &e = lv.ipreaches[k];
+            bool propagated = false, routed = has_zeroth;
+            switch (e.kind) {
+            case HL_ISIS_IP_V4_INTERNAL: case HL_ISIS_IP_V4_EXTERNAL:
+                propagated = lv.ipv4_enabled && narrow; break;
+            case HL_ISIS_IP_V4_EXT:
+                propagated = lv.ipv4_enabled && wide; routed = routed && e.metric <= kMaxWide; break;
+            case HL_ISIS_IP_V6:
+                propagated = !mt6 && lv.ipv6_enabled; break;
+            case HL_ISIS_IP_MT_V6:
+                propagated = mt6 && e.mt_id == HL_ISIS_MT_IPV6; routed = routed && lv.ipv6_enabled; break;
+            default: break;
+            }
+            if (propagated && !routed && hspf::isis_summary_match(cfg, n_cfg, e.prefix, e.len) < 0) return false;
+        }
+    }
+    return true;
+}
+
+// NetKey of a summary
+NetKey summary_key(const hl_isis_summary &s) { return NetKey{s.prefix, s.len}; }
+
+}  // namespace
+
+extern "C" {
+
+void hspf_isis_l1l2_ribtable_free(hspf_isis_l1l2_ribtable *t) {
+    if (!t) return;
+    hspf::release_route_table(t->dev);
+    delete t;
+}
+
+int hspf_isis_l1l2_ribtable_create(const hl_isis_instance *l1, const hl_isis_instance *l2, const uint8_t *l2_derived,
+                                   const hl_isis_summary *cfg, uint32_t n_cfg, hspf_isis_l1l2_ribtable **out) {
+    if (!out) return HSPF_E_INVAL;
+    *out = nullptr;
+    if (!l1 || !l2 || (n_cfg && !cfg)) return HSPF_E_INVAL;
+    if (l1->level_type != 3 || l2->level_type != 3 || l1->level != 1 || l2->level != 2 ||
+        l1->system_id != l2->system_id || l1->max_paths != l2->max_paths)
+        return HSPF_E_INVAL;
+    for (uint32_t s = 1; s < n_cfg; ++s)
+        if (!(summary_key(cfg[s - 1]) < summary_key(cfg[s]))) return HSPF_E_INVAL;
+    try {
+        // a derived entry is one of the root's own (non-pseudonode) L2 LSPs
+        if (l2_derived) {
+            std::vector<uint8_t> own(l2->lvl.n_ipreaches, 0);
+            for (uint32_t i = 0; i < l2->lvl.n_lsps; ++i) {
+                const hl_isis_lsp &lsp = l2->lvl.lsps[i];
+                if (lsp.lan_id != (l2->system_id << 8)) continue;
+                for (uint32_t k = lsp.ipreach_off; k < lsp.ipreach_off + lsp.n_ipreach && k < l2->lvl.n_ipreaches; ++k) own[k] = 1;
+            }
+            for (uint32_t k = 0; k < l2->lvl.n_ipreaches; ++k)
+                if (l2_derived[k] && !own[k]) return HSPF_E_INVAL;
+        }
+        if (!propagation_within_routes(l1, l2, cfg, n_cfg)) return HSPF_E_UNSUPPORTED;
+        auto t = std::make_unique<hspf_isis_l1l2_ribtable>();
+        std::vector<RawContrib> r1, r2;
+        int rc = collect_contributions(l1, nullptr, r1, t->n_vertices[0], t->root[0]);
+        if (rc) return rc;
+        rc = collect_contributions(l2, l2_derived, r2, t->n_vertices[1], t->root[1]);
+        if (rc) return rc;
+        t->n1 = (uint32_t)r1.size();
+        t->S = n_cfg;
+        t->cfg.assign(cfg, cfg + n_cfg);
+        for (const auto &x : r1) { t->contribs.push_back(x.c); t->src.push_back(x.src); }
+        for (const auto &x : r2) { t->contribs.push_back(x.c); t->src.push_back(x.src); }
+        // the union of the L1, L2 and summary prefixes in NetKey (= hl_isis_rib) order
+        std::vector<uint32_t> off1, off2, sum_of;
+        std::vector<std::vector<uint32_t>> cov(n_cfg);
+        size_t i = 0, j = 0, s = 0;
+        while (i < r1.size() || j < r2.size() || s < n_cfg) {
+            NetKey k{};
+            bool have = false;
+            auto low = [&](const NetKey &x) { if (!have || x < k) { k = x; have = true; } };
+            if (i < r1.size()) low(r1[i].key);
+            if (j < r2.size()) low(r2[j].key);
+            if (s < n_cfg) low(summary_key(cfg[s]));
+            const uint32_t p = (uint32_t)t->prefix.size();
+            t->prefix.push_back(k.a);
+            t->len.push_back(k.len);
+            off1.push_back((uint32_t)i);
+            while (i < r1.size() && !(k < r1[i].key)) ++i;
+            off2.push_back(t->n1 + (uint32_t)j);
+            while (j < r2.size() && !(k < r2[j].key)) ++j;
+            const bool is_summary = s < n_cfg && !(k < summary_key(cfg[s]));
+            sum_of.push_back(is_summary ? (uint32_t)s : hspf::kIsisNoSummary);
+            if (is_summary) ++s;
+            if (off1.back() != i) {          // an L1 prefix: the summary that is its shortest configured match
+                const int m = hspf::isis_summary_match(cfg, n_cfg, k.a, k.len);
+                if (m >= 0) cov[m].push_back(p);
+            }
+        }
+        t->P = (uint32_t)t->prefix.size();
+        off1.push_back((uint32_t)r1.size());
+        off2.push_back(t->n1 + (uint32_t)r2.size());
+        auto &w = t->words;
+        w.insert(w.end(), off1.begin(), off1.end());
+        w.insert(w.end(), off2.begin(), off2.end());
+        w.insert(w.end(), sum_of.begin(), sum_of.end());
+        uint32_t n_cov = 0;
+        for (uint32_t k = 0; k < n_cfg; ++k) { w.push_back(n_cov); n_cov += (uint32_t)cov[k].size(); }
+        w.push_back(n_cov);
+        for (const auto &c : cov) w.insert(w.end(), c.begin(), c.end());
+        t->n_cov = n_cov;
+        for (uint32_t k = 0; k < n_cfg; ++k) { w.push_back(cfg[k].has_cfg_metric ? 1u : 0u); w.push_back(cfg[k].cfg_metric); }
+        *out = t.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+uint32_t hspf_isis_l1l2_ribtable_prefixes(const hspf_isis_l1l2_ribtable *t) { return t ? t->P : 0; }
+uint32_t hspf_isis_l1l2_ribtable_contributors(const hspf_isis_l1l2_ribtable *t) {
+    return t ? (uint32_t)t->contribs.size() : 0;
+}
+
+int hspf_isis_l1l2_ribtable_topology(const hspf_isis_l1l2_ribtable *t, uint32_t level, uint32_t topology,
+                                     uint32_t *n_vertices, uint32_t *root) {
+    if (!t || level < 1 || level > 2 || topology > 1) return HSPF_E_INVAL;
+    if (n_vertices) *n_vertices = t->n_vertices[level - 1][topology];
+    if (root) *root = t->root[level - 1][topology];
+    return HSPF_OK;
+}
+
+int hspf_isis_l1l2_ribtable_arrays(const hspf_isis_l1l2_ribtable *t, const hl_ip_addr **prefix, const uint32_t **len,
+                                   const uint32_t **off, const void **contribs) {
+    if (!t) return HSPF_E_INVAL;
+    if (prefix) *prefix = t->prefix.data();
+    if (len) *len = t->len.data();
+    if (off) *off = t->words.data();
+    if (contribs) *contribs = t->contribs.data();
+    return HSPF_OK;
+}
+
+int hspf_isis_l1l2_ribtable_summaries(const hspf_isis_l1l2_ribtable *t, uint32_t *n_l1, uint32_t *n_summaries,
+                                      const uint32_t **sum_of, const uint32_t **cov_off, const uint32_t **cov) {
+    if (!t) return HSPF_E_INVAL;
+    const hspf::IsisL1L2View v = t->view(t->words.data(), t->contribs.data());
+    if (n_l1) *n_l1 = t->n1;
+    if (n_summaries) *n_summaries = t->S;
+    if (sum_of) *sum_of = v.sum_of;
+    if (cov_off) *cov_off = v.cov_off;
+    if (cov) *cov = v.cov;
+    return HSPF_OK;
+}
+
+int hspf_isis_l1l2_rib_from_cells(const hl_isis_instance *l1, const hl_isis_instance *l2,
+                                  const hspf_isis_l1l2_ribtable *t, const hl_isis_route_cell *cells,
+                                  const uint64_t *summary_words, const hspf_isis_job_planes *planes, hl_isis_rib *out) {
+    if (!l1 || !l2 || !t || !planes || !out || (!cells && t->P) || (!summary_words && t->S)) return HSPF_E_INVAL;
+    if (l1->level != 1 || l2->level != 2) return HSPF_E_INVAL;
+    try {
+        const hl_isis_instance *in[2] = {l1, l2};
+        auto tp = std::make_unique<DecodeTopo[]>(4);
+        for (uint32_t l = 0; l < 2; ++l) {
+            const int rc = decode_topos(in[l], t->n_vertices[l], t->root[l], planes + 2 * l, tp.get() + 2 * l);
+            if (rc) return rc;
+        }
+        const SrView sr[2] = {SrView(l1->lvl), SrView(l2->lvl)};
+        const hspf::IsisL1L2View v = t->view(t->words.data(), t->contribs.data());
+        std::map<NetKey, RouteE> rib;
+        for (uint32_t p = 0; p < t->P; ++p) {
+            const hl_isis_route_cell &c = cells[p];
+            if (!(c.flags & HL_CELL_PRESENT)) continue;
+            if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
+            RouteE r{};
+            if (c.winner >= v.n_contribs) {            // an active summary: a blackhole route
+                const uint32_t s = c.winner - v.n_contribs;
+                if (s != v.sum_of[p] || !(summary_words[s] & hspf::kIsisSummaryActive)) return HSPF_E_INVAL;
+                r.type = HL_ISIS_RT_L2_INTRA;
+                r.flags = HL_ROUTE_SUMMARY;
+                r.metric = c.metric;
+            } else {
+                const uint32_t l = c.winner < t->n1 ? 0 : 1;
+                const uint32_t *off = v.off + l * (t->P + 1);
+                if (c.winner < off[p] || c.winner >= off[p + 1]) return HSPF_E_INVAL;
+                const int rc = decode_route(in[l], tp.get() + 2 * l, sr[l], t->contribs[c.winner], t->src[c.winner], c,
+                                            t->prefix[p].is_v6 != 0, r);
+                if (rc) return rc;
+            }
+            rib.emplace_hint(rib.end(), NetKey{t->prefix[p], (uint8_t)t->len[p]}, std::move(r));
         }
         return emit_rib(rib, out);
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }

@@ -152,6 +152,12 @@ uint32_t summary_metric(const hl_isis_summary &s) { return s.has_cfg_metric ? s.
 
 }  // namespace
 
+namespace hspf {
+int isis_summary_match(const hl_isis_summary *cfg, uint32_t n_cfg, const hl_ip_addr &a, uint8_t len) {
+    return shortest_match(cfg, n_cfg, a, len);
+}
+}  // namespace hspf
+
 extern "C" int hspf_isis_summaries(const hl_isis_rib *l1, const hl_isis_summary *cfg, uint32_t n_cfg,
                                    hl_isis_summary *out, uint32_t *n_out) {
     if (!n_out || (n_cfg && (!cfg || !out)) || !rib_ok(l1)) return HSPF_E_INVAL;

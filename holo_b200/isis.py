@@ -695,3 +695,314 @@ def l1_to_l2(level: IsisLevel, local_system_id: int, spt_std: IsisSpt, spt_v6, l
     if rc != capi.HSPF_OK:
         raise capi.HspfError(rc, name + " failed")
     return out[: n.value].copy()
+
+
+# ---- routing table of an L1/L2 router (include/holo_spf_lsdb.h: hspf_isis_l1l2_*) ----------------
+class JobPlanesStruct(C.Structure):
+    _fields_ = [("dist", C.c_void_p), ("hops", C.c_void_p), ("n_ov", C.c_uint32), ("ov_edge", C.c_void_p),
+                ("ov_cost", C.c_void_p)]
+
+
+NO_SUMMARY = 0xFFFFFFFF
+SUMMARY_ACTIVE = 1 << 32
+
+
+class L1L2RibTable(route_table.RouteTable):
+    """hspf_isis_l1l2_ribtable of one L1/L2 router: its level-1 and level-2 instances (`l1`, `l2`, dicts as for
+    RouteTable), its configured summaries `cfg` (summary_cfg) and `l2_derived` (u8 per l2 IP reachability entry,
+    or None).  `off` [2, n_prefixes + 1]: the L1 and L2 contributor ranges; contributors [0, n_l1) are L1's, the
+    rest L2's, and winner n_contributors + s is summary s.  `sum_of`, `cov_off`, `cov`: each prefix's summary and
+    the L1 prefixes each summary covers.  `n_vertices[level - 1][t]` / `root[level - 1][t]` per topology."""
+
+    api, kind, contrib_dt = "hspf_isis", "l1l2_ribtable", CONTRIB_DT
+
+    def __init__(self, l1: dict, l2: dict, cfg=None, l2_derived=None):
+        s1, s2 = instance_struct(l1), instance_struct(l2)
+        self.cfg = np.ascontiguousarray(cfg if cfg is not None else np.zeros(0, SUMMARY_DT), SUMMARY_DT)
+        der = None if l2_derived is None else np.ascontiguousarray(l2_derived, np.uint8)
+        super().__init__(capi.load_library().hspf_isis_l1l2_ribtable_create, C.byref(s1), C.byref(s2),
+                         der.ctypes.data if der is not None and len(der) else None,
+                         self.cfg.ctypes.data if len(self.cfg) else None, len(self.cfg))
+        self.n_vertices = [[0, 0], [0, 0]]
+        self.root = [[NO_ROOT, NO_ROOT], [NO_ROOT, NO_ROOT]]
+        for level in (1, 2):
+            for t in (TOPO_STD, TOPO_MT6):
+                nv, r = C.c_uint32(), C.c_uint32()
+                self._call("topology", level, t, C.byref(nv), C.byref(r))
+                self.n_vertices[level - 1][t], self.root[level - 1][t] = nv.value, r.value
+        pp, pl, po = C.c_void_p(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)()
+        self._call("arrays", C.byref(pp), C.byref(pl), C.byref(po), None)
+        P = self.n_prefixes
+        self.prefix = route_table.copy_records(pp, P, IP_DT)
+        self.len = route_table.copy_records(pl, P, np.uint32)
+        self.off = route_table.copy_records(po, 2 * (P + 1), np.uint32).reshape(2, P + 1)
+        n1, S = C.c_uint32(), C.c_uint32()
+        so, co, cv = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)()
+        self._call("summaries", C.byref(n1), C.byref(S), C.byref(so), C.byref(co), C.byref(cv))
+        self.n_l1, self.n_summaries = n1.value, S.value
+        self.sum_of = route_table.copy_records(so, P, np.uint32)
+        self.cov_off = route_table.copy_records(co, S.value + 1, np.uint32)
+        self.cov = route_table.copy_records(cv, int(self.cov_off[-1]), np.uint32)
+
+
+def _planes_pair(rs):
+    return C.byref(rs) if rs is not None else None
+
+
+def l1l2_rib_cells_device(ctx: capi.Context, t: L1L2RibTable, n_jobs: int, l1, l2, n_rows, rows_ptr: int,
+                          summary_ptr: int, status_ptr: int, cells_ptr: int):
+    """hspf_isis_l1l2_rib_cells / _cells16 over DEVICE planes.  l1, l2: (rs_std, rs_mt6) of the L1 and of the L2 batch
+    (capi.ResultStruct or capi.Result16Struct holding device pointers; rs_mt6 may be None unless that level has an
+    MT-IPv6 root); n_rows: (rows of the L1 batch, rows of the L2 batch); rows_ptr: device u32 [n_jobs, 2];
+    summary_ptr: device u64 [n_jobs, t.n_summaries]; status_ptr: device u32 [n_jobs] or 0; cells_ptr: device
+    [n_jobs, t.n_prefixes] cells.  Enqueued on the ctx stream; the table must have been uploaded."""
+    nr = (C.c_uint32 * 2)(*[int(x) for x in n_rows])
+    rs = next((x for x in (*l1, *l2) if x is not None), None)      # none at all: the call refuses the arguments
+    route_table.call_stage(ctx, "hspf_isis_l1l2_rib_cells", rs, t.handle, n_jobs, *map(_planes_pair, (*l1, *l2)), nr,
+                           rows_ptr or None, summary_ptr or None, status_ptr or None, cells_ptr or None)
+
+
+def l1l2_rib_delta_device(ctx: capi.Context, t: L1L2RibTable, n_jobs: int, l1, l2, n_rows, rows_ptr: int,
+                          summary_ptr: int, base_ptr: int, n_base: int, base_of_ptr: int, job_out_ptr: int,
+                          records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_isis_l1l2_rib_delta / _delta16: the summary pass, then the route-delta stage over the same walk (arguments
+    as l1l2_rib_cells_device and routes_delta_device)."""
+    nr = (C.c_uint32 * 2)(*[int(x) for x in n_rows])
+    rs = next((x for x in (*l1, *l2) if x is not None), None)      # none at all: the call refuses the arguments
+    route_table.call_stage(ctx, "hspf_isis_l1l2_rib_delta", rs, t.handle, n_jobs, *map(_planes_pair, (*l1, *l2)), nr,
+                           rows_ptr or None, summary_ptr or None, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+
+
+def l1l2_rib_from_cells(l1: dict, l2: dict, t: L1L2RibTable, cells: np.ndarray, words: np.ndarray, planes, ovs=None) -> IsisRib:
+    """hspf_isis_l1l2_rib_from_cells (host): one job's cells and summary words -> its merged routing table.  planes:
+    four (dist u32[V], hops u16[V]) or None, for L1 std, L1 MT-IPv6, L2 std, L2 MT-IPv6; ovs: four [(edge, cost)]
+    lists.  rc HSPF_E_UNSUPPORTED is returned in the result."""
+    lib = capi.load_library()
+    cells = np.ascontiguousarray(cells, CELL_DT)
+    words = np.ascontiguousarray(words, np.uint64)
+    assert cells.shape == (t.n_prefixes,) and words.shape == (t.n_summaries,)
+    keep = [cells, words]
+    jp = (JobPlanesStruct * 4)()
+    for k in range(4):
+        p = planes[k]
+        ov = list((ovs or [(), (), (), ()])[k])
+        if p is not None:
+            d, h = np.ascontiguousarray(p[0], np.uint32), np.ascontiguousarray(p[1], np.uint16)
+            keep += [d, h]
+            jp[k].dist, jp[k].hops = d.ctypes.data, h.ctypes.data
+        e = np.asarray([x for x, _ in ov] or [0], np.uint32)
+        c = np.asarray([x for _, x in ov] or [0], np.uint32)
+        keep += [e, c]
+        jp[k].n_ov, jp[k].ov_edge, jp[k].ov_cost = len(ov), e.ctypes.data, c.ctypes.data
+    s1 = instance_struct(l1)
+    tail = (t.handle, cells.ctypes.data if len(cells) else None, words.ctypes.data if len(words) else None, jp)
+    res = _call_rib(lib.hspf_isis_l1l2_rib_from_cells, l2, (C.byref(s1),), tail_args=tail)
+    if res.rc not in (capi.HSPF_OK, capi.HSPF_E_UNSUPPORTED):
+        raise capi.HspfError(res.rc, "hspf_isis_l1l2_rib_from_cells failed")
+    return res
+
+
+def _adjacencies(t: Topology, root: int, sys_of, usage: int):
+    """Local interfaces and adjacencies of router `root` of topology t (router i is system sys_of(i))."""
+    from . import ospfv3
+    ifaces, adjs = [], []
+    for k in range(t.n_p2p):
+        a, b = int(t.p2p_a[k]), int(t.p2p_b[k])
+        for me, other, cost in ((a, b, int(t.p2p_cost_ab[k])), (b, a, int(t.p2p_cost_ba[k]))):
+            if me == root:
+                n = len(adjs) + 1
+                adjs.append((sys_of(other), (2, 0, 0, 1, n >> 8, n & 255), 1, usage, 1, 1, 1, 1, 0, (0, 0, 0),
+                             0xAC100000 + 4 * k + (2 if me == a else 1), ospfv3.ip_rec(f"fe80::{n:x}")))
+                ifaces.append((len(ifaces) + 1, cost, 0, (0, 0, 0), len(adjs) - 1, 1))
+    for members, costs in t.lans:
+        if root in members:
+            off = len(adjs)
+            for m in sorted(members):
+                if m != root:
+                    n = len(adjs) + 1
+                    adjs.append((sys_of(m), (2, 0, 0, 2, n >> 8, n & 255), 1, usage, 1, 1, 1, 1, 0, (0, 0, 0),
+                                 0xC0A80000 + 256 * len(ifaces) + m % 250, ospfv3.ip_rec(f"fe80::1:{n:x}")))
+            ifaces.append((len(ifaces) + 1, costs[members.index(root)], 1, (0, 0, 0), off, len(adjs) - off))
+    return ifaces, adjs
+
+
+def _with_ipreach(level: IsisLevel, entries: dict) -> IsisLevel:
+    """`level` with entries[lan_id] (IPREACH_DT tuples) appended to each LAN id's zeroth fragment."""
+    import copy
+    lv = copy.copy(level)
+    lsps, old = lv.lsps.copy(), lv.ipreaches
+    new = []
+    for i in range(len(lsps)):
+        a, n = int(lsps["ipreach_off"][i]), int(lsps["n_ipreach"][i])
+        ent = [tuple(x.tolist()) for x in old[a:a + n]]
+        if int(lsps["fragment"][i]) == 0:
+            ent += entries.get(int(lsps["lan_id"][i]), [])
+        lsps["ipreach_off"][i], lsps["n_ipreach"][i] = len(new), len(ent)
+        new += ent
+    lv.lsps = lsps
+    lv.ipreaches = np.array(new, IPREACH_DT) if new else np.zeros(0, IPREACH_DT)
+    return lv
+
+
+def _distances(flat: "Flat", root: int) -> np.ndarray:
+    """Shortest distances from `root` over a flattened level (u32, 0xFFFFFFFF: unreached)."""
+    import heapq
+    row, col, cost, vf = flat.csr.row_ptr, flat.csr.col, flat.csr.cost, flat.csr.vflags
+    V = flat.csr.n_vertices
+    d = np.full(V, 0xFFFFFFFF, np.uint64)
+    d[root] = 0
+    heap, done = [(0, root)], np.zeros(V, bool)
+    while heap:
+        du, u = heapq.heappop(heap)
+        if done[u]:
+            continue
+        done[u] = True
+        if u != root and (vf[u] & 0x6):          # HSPF_VF_LEAF / LEAF_UNLESS_ROOT: a leaf relaxes nothing
+            continue
+        for e in range(int(row[u]), int(row[u + 1])):
+            v, nd = int(col[e]), du + int(cost[e])
+            if nd < d[v]:
+                d[v] = nd
+                heapq.heappush(heap, (nd, v))
+    return d.astype(np.uint32)
+
+
+def _spt_of(flat: "Flat", dist: np.ndarray) -> IsisSpt:
+    """An IsisSpt holding only what hspf_isis_l1_to_l2 reads: the reached vertices' LAN ids and distances."""
+    reached = np.nonzero(dist != 0xFFFFFFFF)[0]
+    v = np.zeros(len(reached), VERTEX_DT)
+    v["lan_id"], v["distance"] = flat.ids[reached], dist[reached]
+    z = np.zeros(0, np.uint32)
+    return IsisSpt(v, z, np.zeros(0, np.uint64), z, z)
+
+
+def l1l2_view(seed: int, n_l1: int = 150, n_l2: int = 120, n_border: int = 3, root: int = 0,
+              metric_type: int = METRIC_WIDE, mt6: bool = False, sr: bool = False, max_paths: int = 4,
+              attached: bool = True, summaries=(("10.1.0.0/16", None),), cost_choices=None, l1_degree: int = 4,
+              l2_topology=None) -> dict:
+    """A seeded two-level domain: an L1 area of n_l1 routers (systems sysid(0 .. n_l1 - 1)) and an L2 backbone of n_l2
+    routers joined by the L1/L2 routers 0 .. n_border - 1 (backbone router i >= n_border is sysid(n_l1 + i)).  L1
+    router r advertises 10.1.r/32 (every third one also 10.2.(r % 16).0/24, and with mt6 an MT-IPv6 /128); backbone
+    router i advertises 10.200.i/32.  `l2_topology` (a synth.Topology) replaces the generated backbone; n_l2 is then
+    its router count.  The L1 area has l1_degree * n_l1 / 2 adjacencies (2: a tree and a few more).  Every L1/L2 router sets the ATT bit in its L1 LSP (the root only when
+    `attached`) and carries in its own L2 LSP what lsp_propagate_l1_to_l2 puts there from its own L1 SPT with the
+    configured `summaries`: the propagated entries and its active summaries.  Returns dict(l1, l2: the instance
+    images of L1/L2 router `root`, cfg, l2_derived: the mask of root's derived L2 entries, borders)."""
+    from . import ospfv3, synth
+    kw = dict(cost_choices=cost_choices) if cost_choices else dict(cost_lo=1, cost_hi=20)
+    t1 = synth.random_topology(n_l1, l1_degree * n_l1, synth.SEED_BASE + 1000 + seed, lan_fraction=0.1, **kw)
+    t2 = l2_topology or synth.random_topology(n_l2, 4 * n_l2, synth.SEED_BASE + 2000 + seed, lan_fraction=0.1, **kw)
+    n_l2 = t2.n_routers
+    sys2 = lambda i: sysid(i) if i < n_border else sysid(n_l1 + i)
+    cfg = summary_cfg(list(summaries))
+    narrow, wide = metric_type in (METRIC_STANDARD, METRIC_BOTH), metric_type in (METRIC_WIDE, METRIC_BOTH)
+
+    def v4(net, plen, metric, psid=None):
+        out = []
+        if narrow:
+            out.append(ipreach_rec(ospfv3.ip_rec(net), min(metric, 63), 0, plen, IP_V4_INTERNAL))
+        if wide:
+            out.append(ipreach_rec(ospfv3.ip_rec(net), metric, 0, plen, IP_V4_EXT, 0, psid if sr else None))
+        return out
+
+    def finish(lv):
+        """SR capabilities, NLPIDs and ATT bits of a level"""
+        lsps = lv.lsps.copy()
+        lsps["flags"] |= np.where(lsps["fragment"] == 0, LSPF_NLPID_IPV6 if mt6 else 0, 0).astype(np.uint8)
+        if sr:
+            zero = (lsps["fragment"] == 0) & ((lsps["lan_id"] & 0xFF) == 0)
+            lsps["sr_flags"] = np.where(zero, LSP_SR_HAS_CAP | LSP_SR_CAP_I | LSP_SR_CAP_V | LSP_SR_ALGO_SPF, 0)
+            lsps["srgb_off"], lsps["n_srgb"] = 0, np.where(zero, 1, 0)
+            lv.srgbs = np.array([(16000, 8000, 0, (0, 0, 0))], SRGB_DT)
+        lv.lsps = lsps
+        lv.ipv6_enabled = bool(mt6)
+        return lv
+
+    # level 1 (with mt6, synth_level's MT-IPv6 level carries the standard adjacencies beside the MT ones)
+    lv1 = synth_level(t1, metric_type=metric_type, mt_id=MT_IPV6 if mt6 else MT_STANDARD)
+    ent1 = {}
+    for r in range(n_l1):
+        e = v4(f"10.1.{r >> 8}.{r & 255}", 32, 1, (PSID_P, 0, r))
+        if r % 3 == 0:
+            e += v4(f"10.2.{r % 16}.0", 24, 5)
+        if mt6:
+            e.append(ipreach_rec(ospfv3.ip_rec(f"2001:db8:1::{r + 1:x}"), 2, MT_IPV6, 128, IP_MT_V6))
+        ent1[sysid(r) << 8] = e
+    lv1 = finish(_with_ipreach(lv1, ent1))
+    lv1.mt_id = MT_STANDARD
+    att = (lv1.lsps["fragment"] == 0) & np.isin(lv1.lsps["lan_id"], [sysid(b) << 8 for b in range(n_border)
+                                                                      if attached or b != root])
+    lv1.lsps["flags"] |= np.where(att, LSPF_ATT | (LSPF_MT_IPV6_ATT if mt6 else 0), 0).astype(np.uint8)
+    # level 2: configured prefixes, then each L1/L2 router's propagated entries and active summaries
+    lv2 = synth_level(t2, metric_type=metric_type, mt_id=MT_IPV6 if mt6 else MT_STANDARD)
+    remap = lambda lid: (sys2(((int(lid) >> 8) - SYSID_BASE)) << 8) | (int(lid) & 0xFF)
+    lsps = lv2.lsps.copy()
+    lsps["lan_id"] = [remap(x) for x in lsps["lan_id"]]
+    lv2.reaches = lv2.reaches.copy()
+    lv2.reaches["neighbor"] = [remap(x) for x in lv2.reaches["neighbor"]]
+    lv2.lsps = lsps[np.lexsort((lsps["fragment"], lsps["lan_id"]))]
+    lv2.mt_id = MT_STANDARD
+    ent2 = {}
+    for i in range(n_l2):
+        ent2[sys2(i) << 8] = v4(f"10.200.{i >> 8}.{i & 255}", 32, 1, (PSID_P, 0, 5000 + i))
+    f1 = Flat(lv1)
+    f6 = None
+    if mt6:
+        import copy
+        l6 = copy.copy(lv1)
+        l6.mt_id = MT_IPV6
+        f6 = Flat(l6)
+    derived = {}
+    for b in range(n_border):
+        d = _distances(f1, f1.vertex(sysid(b) << 8))
+        d6 = _distances(f6, f6.vertex(sysid(b) << 8)) if mt6 else None
+        spt6 = _spt_of(f6, d6) if mt6 else None
+        # the router's L1 routes (contributions of reached vertices; ATT defaults only when not attached)
+        low = {}
+        for i in range(len(lv1.lsps)):
+            lid, v = int(lv1.lsps["lan_id"][i]), f1.vertex(int(lv1.lsps["lan_id"][i]))
+            a, n = int(lv1.lsps["ipreach_off"][i]), int(lv1.lsps["n_ipreach"][i])
+            for r in lv1.ipreaches[a:a + n]:
+                dv = d[v] if int(r["kind"]) != IP_MT_V6 else d6[f6.vertex(lid)]
+                if dv == 0xFFFFFFFF:
+                    continue
+                key = (int(r["prefix"]["is_v6"]), bytes(r["prefix"]["bytes"]), int(r["len"]))
+                low[key] = min(low.get(key, 1 << 40), int(dv) + int(r["metric"]))
+        if not (attached or b != root):
+            for i in np.nonzero(att)[0]:
+                v = f1.vertex(int(lv1.lsps["lan_id"][i]))
+                if d[v] != 0xFFFFFFFF:
+                    key = (0, bytes(16), 0)
+                    low[key] = min(low.get(key, 1 << 40), int(d[v]))
+        rib = np.zeros(len(low), ROUTE_DT)
+        for k, (key, m) in enumerate(sorted(low.items())):
+            rib[k]["prefix"]["is_v6"], rib[k]["prefix"]["bytes"], rib[k]["len"], rib[k]["metric"] = key[0], list(key[1]), key[2], m
+        act = summaries_of(rib, cfg)
+        prop = l1_to_l2(lv1, sysid(b), _spt_of(f1, d), spt6, metric_type, metric_type, cfg, act)
+        prop = [tuple(x.tolist()) for x in prop]
+        derived[sysid(b) << 8] = len(prop)
+        ent2[sysid(b) << 8] = ent2[sysid(b) << 8] + prop
+    lv2 = finish(_with_ipreach(lv2, ent2))
+    mask = np.zeros(len(lv2.ipreaches), np.uint8)
+    for i in range(len(lv2.lsps)):
+        lid = int(lv2.lsps["lan_id"][i])
+        if lid == sysid(root) << 8 and int(lv2.lsps["fragment"][i]) == 0:
+            end = int(lv2.lsps["ipreach_off"][i]) + int(lv2.lsps["n_ipreach"][i])
+            mask[end - derived[lid]: end] = 1
+    i1, a1 = _adjacencies(t1, root, sysid, 1)
+    if attached:                  # an up L2 adjacency into another area: is_l2_attached_to_backbone
+        a1.append((sys2(n_border), (2, 0, 0, 9, 0, 1), 1, 2, 1, 1, 1, 1, 1, (0, 0, 0), 0xAC1F0001,
+                   ospfv3.ip_rec("fe80::9:1")))
+        i1.append((len(i1) + 1, 10, 0, (0, 0, 0), len(a1) - 1, 1))
+    r2 = next(i for i in range(n_l2) if sys2(i) == sysid(root))
+    i2, a2 = _adjacencies(t2, r2, sys2, 2)
+    base = dict(system_id=sysid(root), max_paths=max_paths, level_type=3, att_ignore=0, mt_ipv6=int(mt6), sr_enabled=int(sr))
+    l1 = dict(base, level=lv1, level_no=1, ifaces=np.array(i1, IFACE_DT), adjs=np.array(a1, ADJ_DT))
+    l2 = dict(base, level=lv2, level_no=2, ifaces=np.array(i2, IFACE_DT), adjs=np.array(a2, ADJ_DT))
+    return dict(l1=l1, l2=l2, cfg=cfg, l2_derived=mask, borders=list(range(n_border)), t1=t1, t2=t2)
+
+
+def summaries_of(l1_routes: np.ndarray, cfg: np.ndarray) -> np.ndarray:
+    """hspf_isis_summaries over bare L1 routes (ROUTE_DT in prefix order, no next hops)."""
+    return summaries(IsisRib(l1_routes, np.zeros(0, NEXTHOP_DT)), cfg)

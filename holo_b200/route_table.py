@@ -125,10 +125,24 @@ def declare(lib: C.CDLL):
         "hspf_ospfv2_abr_rib_delta16": [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv2_abr_rib_from_cells": [vp, C.POINTER(ospfv2.AreaStruct), u32, vp, vp, vp, vp, u32,
                                            C.POINTER(ospf_rib.RibStruct)],
+        "hspf_isis_l1l2_ribtable_create": [C.POINTER(isis.InstanceStruct), C.POINTER(isis.InstanceStruct), vp, vp, u32,
+                                           pvp],
+        "hspf_isis_l1l2_ribtable_topology": [vp, u32, u32, u32p, u32p],
+        "hspf_isis_l1l2_ribtable_arrays": [vp, pvp, C.POINTER(u32p), C.POINTER(u32p), pvp],
+        "hspf_isis_l1l2_ribtable_summaries": [vp, u32p, u32p, C.POINTER(u32p), C.POINTER(u32p), C.POINTER(u32p)],
+        "hspf_isis_l1l2_ribtable_upload": [vp, vp],
+        "hspf_isis_l1l2_rib_cells": [vp, vp, u32, res, res, res, res, u32p, vp, vp, vp, vp],
+        "hspf_isis_l1l2_rib_cells16": [vp, vp, u32, res16, res16, res16, res16, u32p, vp, vp, vp, vp],
+        "hspf_isis_l1l2_rib_delta": [vp, vp, u32, res, res, res, res, u32p, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_isis_l1l2_rib_delta16": [vp, vp, u32, res16, res16, res16, res16, u32p, vp, vp, vp, u32, vp, vp, vp, u64,
+                                       vp],
+        "hspf_isis_l1l2_rib_from_cells": [C.POINTER(isis.InstanceStruct), C.POINTER(isis.InstanceStruct), vp, vp, vp,
+                                          C.POINTER(isis.JobPlanesStruct), C.POINTER(isis.RibStruct)],
     }
     for name, argtypes in sigs.items():
         getattr(lib, name).argtypes = argtypes
-    for table in ("hspf_ospfv2_rtable", "hspf_isis_rtable", "hspf_ospfv2_ribtable", "hspf_ospfv2_abr_ribtable"):
+    for table in ("hspf_ospfv2_rtable", "hspf_isis_rtable", "hspf_ospfv2_ribtable", "hspf_ospfv2_abr_ribtable",
+                  "hspf_isis_l1l2_ribtable"):
         getattr(lib, table + "_free").argtypes = [vp]
         getattr(lib, table + "_free").restype = None
         for name in ("prefixes", "contributors"):

@@ -535,6 +535,110 @@ int hspf_isis_routes_from_cells(const hl_isis_instance *inst, const hspf_isis_rt
                                 hl_isis_rib *out);
 
 /*
+ * Routing table of an IS-IS L1/L2 router on the device, for every job of a what-if batch: update_rib
+ * (holo-isis/src/route.rs:182-249) over the job's SPTs of both levels.  The L1 table, the active summaries it
+ * gives (get_spm: the SHORTEST configured match of each L1 route; metric: the configured one, else the lowest
+ * covered L1 metric), the L2 table in which an active summary replaces the route of its prefix with a blackhole
+ * route, and the two merged with the L1 route preferred (isis_l1l2_rib_cells.h).
+ *
+ *   hspf_isis_l1l2_ribtable_create   per L1/L2 router: `l1` / `l2` its instance images of level 1 and 2 (level_type 3,
+ *                             the same system id and max_paths), `cfg` its n_cfg configured summaries in prefix order
+ *                             (IPv4 before IPv6, address, length).  Each level's contributors are those of
+ *                             hspf_isis_rtable_create.  The prefixes are the union of both levels' prefixes and the
+ *                             summary prefixes, in hl_isis_rib order; per prefix an L1 range, an L2 range and its
+ *                             summary.  Contributor indices (hl_isis_route_cell.winner) share one space: the L1
+ *                             contributors, the L2 contributors, then one index per configured summary.
+ *     l2_derived              one byte per entry of l2->lvl.ipreaches (NULL: none): non-zero marks an entry of the
+ *                             router's own (non-pseudonode) L2 LSPs that is not configured there — lsp_propagate_l1_to_l2 or an
+ *                             advertised summary put it there.  Those entries are left out of the L2 contributors.
+ *                             The L2 LSDB holds the base state's propagation; in a what-if job holo re-originates
+ *                             that LSP from the job's L1 SPT, and a stale entry would become a connected L2 route
+ *                             holo does not have.  Leaving them out is exact: whenever the re-originated LSP
+ *                             carries a propagated entry, its originator is on the job's L1 SPT of the same
+ *                             topology, so the prefix has an L1 route, and the L1 route wins the merge; an active
+ *                             summary replaces the L2 route of its prefix anyway.  That holds when every L1 entry
+ *                             propagation's static filters let through (holo-isis lsdb.rs:1163-1258) is one
+ *                             compute_routes feeds into the L1 table (spf.rs:862-882, 1141): the builder checks
+ *                             it and returns HSPF_E_UNSUPPORTED for a fragment whose system has no valid zeroth
+ *                             LSP, an extended IPv4 entry above the wide-metric limit, or an MT-IPv6 entry under
+ *                             an instance with IPv6 disabled, unless a summary covers it.  What-if jobs change
+ *                             costs only, so the check is exact for every job.
+ *                             HSPF_E_INVAL: levels or level types wrong, system ids or max_paths differ, `cfg` out
+ *                             of order, a non-zero l2_derived byte for an entry outside the router's own
+ *                             (non-pseudonode) L2 LSPs.
+ *   hspf_isis_l1l2_ribtable_topology vertex count and root vertex of level 1 or 2, topology 0 or 1 (as
+ *                             hspf_isis_rtable_topology).
+ *   hspf_isis_l1l2_ribtable_arrays   prefix[P], len[P], off (u32: the L1 ranges [P + 1], the L2 ranges [P + 1], ...),
+ *                             contribs (the L1 then the L2 contributor records); any pointer may be NULL.
+ *   hspf_isis_l1l2_ribtable_summaries n_l1 (the number of L1 contributors), S, sum_of[P] (0xFFFFFFFF: not a summary
+ *                             prefix), cov_off[S + 1] and cov: the L1 prefixes each summary is the shortest match of.
+ *   hspf_isis_l1l2_ribtable_upload   copies the table to the ctx's device.
+ *   hspf_isis_l1l2_rib_cells[16]   DEVICE planes of four topologies: l1_std, l1_mt6 from one L1 batch and l2_std,
+ *                             l2_mt6 from one L2 batch (hspf_run_batch_async / hspf_run_batch16_async, the wide ones
+ *                             with nh_words == 1; *_mt6 may be NULL unless that level's table has an MT-IPv6 root).
+ *                             n_rows[2]: the rows of the L1 and of the L2 batch; rows [n_jobs][2] (device): the
+ *                             job's L1 row and L2 row, so that a job perturbing one level reuses the other level's
+ *                             plain row.  First the summary pass, one warp per (job, summary), writes
+ *                             summary_out (device u64 [n_jobs][S], required when S > 0): 0 inactive,
+ *                             (1 << 32) | lowest covered L1 metric when active — per job, which summaries the router
+ *                             advertises into L2 and at what metric.  Then cells[n_jobs][P] (device).
+ *                             job_status_out (device [n_jobs], or NULL): the OR of the status words of the job's
+ *                             rows (MT-IPv6 planes only where the level has an MT-IPv6 root), HSPF_JS_INVALID for a
+ *                             row out of range.  A job with a non-zero status gets empty cells and summary words 0.
+ *                             Nothing is launched for 0 jobs.  Enqueued on the ctx stream; no synchronisation.
+ *   hspf_isis_l1l2_rib_delta[16]   the summary pass, then the route-delta stage (below) over the same walk.
+ *   hspf_isis_l1l2_rib_from_cells  host: one job's cells and summary words -> exactly the hl_isis_rib of
+ *                             hspf_isis_rib_merge(hspf_isis_rib_add_summaries(L2 routes, hspf_isis_summaries(L1
+ *                             routes, cfg)), L1 routes), the routes of each level as hspf_isis_routes_from_planes
+ *                             gives them over the same planes (the L2 LSDB without the derived entries).
+ *                             planes[4]: the job's planes and overrides of L1 std, L1 MT-IPv6, L2 std, L2 MT-IPv6.
+ *                             HSPF_E_UNSUPPORTED as hspf_isis_routes_from_cells.
+ */
+typedef struct hspf_isis_l1l2_ribtable hspf_isis_l1l2_ribtable;
+/* One topology's planes of one job for the host decode: dist / hops [V], its n_ov edge overrides */
+typedef struct hspf_isis_job_planes {
+    const uint32_t *dist;
+    const uint16_t *hops;
+    uint32_t n_ov;
+    const uint32_t *ov_edge;
+    const uint32_t *ov_cost;
+} hspf_isis_job_planes;
+int hspf_isis_l1l2_ribtable_create(const hl_isis_instance *l1, const hl_isis_instance *l2, const uint8_t *l2_derived,
+                                   const hl_isis_summary *cfg, uint32_t n_cfg, hspf_isis_l1l2_ribtable **out);
+void hspf_isis_l1l2_ribtable_free(hspf_isis_l1l2_ribtable *t);
+uint32_t hspf_isis_l1l2_ribtable_prefixes(const hspf_isis_l1l2_ribtable *t);
+uint32_t hspf_isis_l1l2_ribtable_contributors(const hspf_isis_l1l2_ribtable *t);
+int hspf_isis_l1l2_ribtable_topology(const hspf_isis_l1l2_ribtable *t, uint32_t level, uint32_t topology,
+                                     uint32_t *n_vertices, uint32_t *root);
+int hspf_isis_l1l2_ribtable_arrays(const hspf_isis_l1l2_ribtable *t, const hl_ip_addr **prefix, const uint32_t **len,
+                                   const uint32_t **off, const void **contribs);
+int hspf_isis_l1l2_ribtable_summaries(const hspf_isis_l1l2_ribtable *t, uint32_t *n_l1, uint32_t *n_summaries,
+                                      const uint32_t **sum_of, const uint32_t **cov_off, const uint32_t **cov);
+int hspf_isis_l1l2_ribtable_upload(hspf_ctx *ctx, hspf_isis_l1l2_ribtable *t);
+int hspf_isis_l1l2_rib_cells(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs, const hspf_result *l1_std,
+                             const hspf_result *l1_mt6, const hspf_result *l2_std, const hspf_result *l2_mt6,
+                             const uint32_t *n_rows, const uint32_t *rows, uint64_t *summary_out,
+                             uint32_t *job_status_out, hl_isis_route_cell *cells);
+int hspf_isis_l1l2_rib_cells16(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs,
+                               const hspf_result16 *l1_std, const hspf_result16 *l1_mt6, const hspf_result16 *l2_std,
+                               const hspf_result16 *l2_mt6, const uint32_t *n_rows, const uint32_t *rows,
+                               uint64_t *summary_out, uint32_t *job_status_out, hl_isis_route_cell *cells);
+int hspf_isis_l1l2_rib_delta(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs, const hspf_result *l1_std,
+                             const hspf_result *l1_mt6, const hspf_result *l2_std, const hspf_result *l2_mt6,
+                             const uint32_t *n_rows, const uint32_t *rows, uint64_t *summary_out,
+                             const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                             hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_isis_l1l2_rib_delta16(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs,
+                               const hspf_result16 *l1_std, const hspf_result16 *l1_mt6, const hspf_result16 *l2_std,
+                               const hspf_result16 *l2_mt6, const uint32_t *n_rows, const uint32_t *rows,
+                               uint64_t *summary_out, const hl_isis_route_cell *base_cells, uint32_t n_base,
+                               const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
+                               uint64_t cap, uint64_t *n_records);
+int hspf_isis_l1l2_rib_from_cells(const hl_isis_instance *l1, const hl_isis_instance *l2,
+                                  const hspf_isis_l1l2_ribtable *t, const hl_isis_route_cell *cells,
+                                  const uint64_t *summary_words, const hspf_isis_job_planes *planes, hl_isis_rib *out);
+
+/*
  * Route-delta stage on the device: which prefixes each job of a what-if batch loses, gains, or reaches at another
  * metric or over another next-hop set, against a base route table — without storing the n_jobs x P cell matrix.
  * Per (job, prefix) it runs the same walk as hspf_*_routes_batch[16] and compares the cell with the job's base cell
