@@ -873,9 +873,12 @@ extern "C" int hspf_isis_routes_from_planes(const hl_isis_instance *in, const ui
 }
 
 /* ---- batched route stage: the table and the per-job decode (isis_route_cells.h) ------------- */
+#include <cassert>
 #include <memory>
 
+#include "isis_l1_to_l2_cells.h"
 #include "isis_l1l2_rib_cells.h"
+#include "isis_propagation.h"
 #include "isis_route_cells.h"
 
 namespace {
@@ -1101,36 +1104,18 @@ namespace {
 bool propagation_within_routes(const hl_isis_instance *l1, const hl_isis_instance *l2, const hl_isis_summary *cfg,
                                uint32_t n_cfg) {
     const hl_isis_level &lv = l1->lvl;
-    auto std_on = [](uint8_t t) { return t == HL_ISIS_METRIC_STANDARD || t == HL_ISIS_METRIC_BOTH; };
-    auto wide_on = [](uint8_t t) { return t == HL_ISIS_METRIC_WIDE || t == HL_ISIS_METRIC_BOTH; };
-    const bool narrow = std_on(lv.metric_type) && std_on(l2->lvl.metric_type);
-    const bool wide = wide_on(lv.metric_type) && wide_on(l2->lvl.metric_type);
-    const bool mt6 = l1->mt_ipv6_enabled != 0;
     std::unordered_set<uint64_t> zeroth;          // LAN ids with a valid zeroth LSP
     for (uint32_t i = 0; i < lv.n_lsps; ++i)
         if (lv.lsps[i].fragment == 0 && lv.lsps[i].seqno && lv.lsps[i].rem_lifetime) zeroth.insert(lv.lsps[i].lan_id);
-    for (uint32_t i = 0; i < lv.n_lsps; ++i) {
-        const hl_isis_lsp &lsp = lv.lsps[i];
-        if (!lsp.seqno || !lsp.rem_lifetime || is_pn(lsp.lan_id) || (lsp.lan_id >> 8) == l1->system_id) continue;
-        const bool has_zeroth = zeroth.count(lsp.lan_id) != 0;
-        for (uint32_t k = lsp.ipreach_off; k < lsp.ipreach_off + lsp.n_ipreach; ++k) {
-            const hl_isis_ipreach &e = lv.ipreaches[k];
-            bool propagated = false, routed = has_zeroth;
-            switch (e.kind) {
-            case HL_ISIS_IP_V4_INTERNAL: case HL_ISIS_IP_V4_EXTERNAL:
-                propagated = lv.ipv4_enabled && narrow; break;
-            case HL_ISIS_IP_V4_EXT:
-                propagated = lv.ipv4_enabled && wide; routed = routed && e.metric <= kMaxWide; break;
-            case HL_ISIS_IP_V6:
-                propagated = !mt6 && lv.ipv6_enabled; break;
-            case HL_ISIS_IP_MT_V6:
-                propagated = mt6 && e.mt_id == HL_ISIS_MT_IPV6; routed = routed && lv.ipv6_enabled; break;
-            default: break;
-            }
-            if (propagated && !routed && hspf::isis_summary_match(cfg, n_cfg, e.prefix, e.len) < 0) return false;
-        }
-    }
-    return true;
+    bool within = true;
+    hspf::for_each_propagation(lv, l1->system_id, lv.metric_type, l2->lvl.metric_type, l1->mt_ipv6_enabled != 0, nullptr,
+                               cfg, n_cfg, [&](const hl_isis_lsp &lsp, uint32_t k, uint8_t, uint32_t, bool) {
+        const hl_isis_ipreach &e = lv.ipreaches[k];
+        const bool routed = zeroth.count(lsp.lan_id) != 0 && (e.kind != HL_ISIS_IP_V4_EXT || e.metric <= kMaxWide) &&
+                            (e.kind != HL_ISIS_IP_MT_V6 || lv.ipv6_enabled);
+        if (!routed) within = false;
+    });
+    return within;
 }
 
 // NetKey of a summary
@@ -1296,6 +1281,160 @@ int hspf_isis_l1l2_rib_from_cells(const hl_isis_instance *l1, const hl_isis_inst
             rib.emplace_hint(rib.end(), NetKey{t->prefix[p], (uint8_t)t->len[p]}, std::move(r));
         }
         return emit_rib(rib, out);
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+}  // extern "C"
+
+/* ---- what an L1/L2 router propagates into its L2 LSP (isis_l1_to_l2_cells.h) --------------------- */
+namespace {
+
+// hspf_isis_l1_to_l2's output order: kind, then prefix
+bool key_less(uint8_t ka, const NetKey &a, uint8_t kb, const NetKey &b) { return ka != kb ? ka < kb : a < b; }
+
+}  // namespace
+
+extern "C" {
+
+void hspf_isis_l1_to_l2_table_free(hspf_isis_l1_to_l2_table *t) {
+    if (!t) return;
+    hspf::release_route_table(t->dev);
+    delete t;
+}
+
+int hspf_isis_l1_to_l2_table_create(const hl_isis_instance *l1, const hl_isis_instance *l2, const uint8_t *up_down,
+                                    const hspf_isis_l1l2_ribtable *rib, hspf_isis_l1_to_l2_table **out) {
+    if (!out) return HSPF_E_INVAL;
+    *out = nullptr;
+    if (!l1 || !l2 || !rib) return HSPF_E_INVAL;
+    if (l1->level != 1 || l2->level != 2 || l1->level_type != 3 || l2->level_type != 3 || l1->system_id != l2->system_id)
+        return HSPF_E_INVAL;
+    try {
+        // the L1 flats of the rib table's instance: same vertex counts and roots
+        hspf_isis_flat f[2];
+        for (uint32_t t = 0; t < 2; ++t) {
+            uint32_t root = 0;
+            bool have_root = false;
+            if (kTopologies[t] == HL_ISIS_MT_STANDARD || l1->mt_ipv6_enabled) {
+                const int rc = topology_flat(l1, kTopologies[t], f[t], root, have_root);
+                if (rc) return rc;
+            }
+            if (f[t].ids.size() != rib->n_vertices[0][t] || (have_root ? root : kNone) != rib->root[0][t])
+                return HSPF_E_INVAL;
+        }
+        auto t = std::make_unique<hspf_isis_l1_to_l2_table>();
+        struct Raw { uint8_t kind; NetKey key; hspf::IsisPropRecord r; uint32_t src; };
+        std::vector<Raw> raw;
+        const hl_isis_level &lv = l1->lvl;
+        hspf::for_each_propagation(lv, l1->system_id, lv.metric_type, l2->lvl.metric_type, l1->mt_ipv6_enabled != 0,
+                                   up_down, rib->cfg.data(), rib->S,
+                                   [&](const hl_isis_lsp &lsp, uint32_t k, uint8_t kind, uint32_t topology, bool narrow) {
+            if (rib->root[0][topology] == kNone) return;             // no SPT in that topology: never reached
+            auto it = f[topology].index.find(lsp.lan_id);
+            if (it == f[topology].index.end()) return;               // not a vertex: never on the SPT
+            Raw x{};
+            x.kind = kind;
+            x.key = NetKey{lv.ipreaches[k].prefix, lv.ipreaches[k].len};
+            x.r.vertex = it->second; x.r.metric = lv.ipreaches[k].metric;
+            x.r.topology = (uint8_t)topology; x.r.narrow = narrow ? 1 : 0;
+            x.src = k;
+            raw.push_back(x);
+        });
+        std::stable_sort(raw.begin(), raw.end(), [](const Raw &a, const Raw &b) { return key_less(a.kind, a.key, b.kind, b.key); });
+        // the summary keys, as hspf_isis_l1_to_l2 adds an active summary
+        struct SumKey { uint8_t kind; NetKey key; uint32_t word; };
+        std::vector<SumKey> sk;
+        auto std_on = [](uint8_t m) { return m == HL_ISIS_METRIC_STANDARD || m == HL_ISIS_METRIC_BOTH; };
+        auto wide_on = [](uint8_t m) { return m == HL_ISIS_METRIC_WIDE || m == HL_ISIS_METRIC_BOTH; };
+        for (uint32_t s = 0; s < rib->S; ++s) {
+            const NetKey key{rib->cfg[s].prefix, rib->cfg[s].len};
+            if (!key.a.is_v6) {
+                if (!lv.ipv4_enabled) continue;
+                if (std_on(l2->lvl.metric_type)) sk.push_back(SumKey{HL_ISIS_IP_V4_INTERNAL, key, (s << 1) | 1u});
+                if (wide_on(l2->lvl.metric_type)) sk.push_back(SumKey{HL_ISIS_IP_V4_EXT, key, s << 1});
+            } else if (lv.ipv6_enabled) {
+                sk.push_back(SumKey{HL_ISIS_IP_V6, key, s << 1});
+            }
+        }
+        std::stable_sort(sk.begin(), sk.end(), [](const SumKey &a, const SumKey &b) { return key_less(a.kind, a.key, b.kind, b.key); });
+        // merge: the keys in output order, each propagated key with its records
+        std::vector<uint32_t> off, sum;
+        size_t i = 0, j = 0;
+        while (i < raw.size() || j < sk.size()) {
+            const bool take_sum = i == raw.size() || (j < sk.size() && key_less(sk[j].kind, sk[j].key, raw[i].kind, raw[i].key));
+            // a summary covers its own prefix, so no propagated entry shares a summary key
+            assert(take_sum || j == sk.size() || key_less(raw[i].kind, raw[i].key, sk[j].kind, sk[j].key));
+            const uint8_t kind = take_sum ? sk[j].kind : raw[i].kind;
+            const NetKey key = take_sum ? sk[j].key : raw[i].key;
+            t->kind.push_back(kind);
+            t->prefix.push_back(key.a);
+            t->len.push_back(key.len);
+            off.push_back((uint32_t)t->recs.size());
+            if (take_sum) {
+                sum.push_back(sk[j++].word);
+                continue;
+            }
+            sum.push_back(hspf::kIsisNoSummary);
+            for (; i < raw.size() && raw[i].kind == kind && !(key < raw[i].key) && !(raw[i].key < key); ++i) {
+                t->recs.push_back(raw[i].r);
+                t->src.push_back(raw[i].src);
+            }
+        }
+        off.push_back((uint32_t)t->recs.size());
+        t->K = (uint32_t)t->kind.size();
+        t->words = off;
+        t->words.insert(t->words.end(), sum.begin(), sum.end());
+        t->n_ipreaches = lv.n_ipreaches;
+        t->rib = rib;
+        *out = t.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+int hspf_isis_l1_to_l2_table_keys(const hspf_isis_l1_to_l2_table *t, uint32_t *n_keys, uint32_t *n_records,
+                                  const uint8_t **kind, const hl_ip_addr **prefix, const uint8_t **len) {
+    if (!t) return HSPF_E_INVAL;
+    if (n_keys) *n_keys = t->K;
+    if (n_records) *n_records = (uint32_t)t->recs.size();
+    if (kind) *kind = t->kind.data();
+    if (prefix) *prefix = t->prefix.data();
+    if (len) *len = t->len.data();
+    return HSPF_OK;
+}
+
+int hspf_isis_l1_to_l2_from_cells(const hl_isis_instance *l1, const hspf_isis_l1_to_l2_table *t,
+                                  const hl_isis_route_cell *cells, const uint64_t *summary_words, hl_isis_ipreach *out,
+                                  uint32_t cap, uint32_t *n_out) {
+    if (!l1 || !t || !n_out || (!cells && t->K) || (!summary_words && t->rib->S) || (cap && !out)) return HSPF_E_INVAL;
+    if (l1->level != 1 || l1->lvl.n_ipreaches != t->n_ipreaches) return HSPF_E_INVAL;    // not the table's instance
+    try {
+        const hspf::IsisL1ToL2View v = t->view(t->words.data(), t->recs.data());
+        std::vector<hl_isis_ipreach> got;
+        for (uint32_t k = 0; k < t->K; ++k) {
+            const hl_isis_route_cell &c = cells[k];
+            if (!(c.flags & HL_CELL_PRESENT)) continue;
+            hl_isis_ipreach e;
+            if (v.sum[k] != hspf::kIsisNoSummary) {               // an active summary
+                const uint32_t s = v.sum[k] >> 1;
+                if (c.winner != v.n_records + s || !(summary_words[s] & hspf::kIsisSummaryActive)) return HSPF_E_INVAL;
+                std::memset(&e, 0, sizeof(e));
+                e.prefix = t->prefix[k];
+                e.len = t->len[k];
+                e.kind = t->kind[k];
+            } else {
+                if (c.winner < v.off[k] || c.winner >= v.off[k + 1]) return HSPF_E_INVAL;
+                e = l1->lvl.ipreaches[t->src[c.winner]];
+                e.kind = t->kind[k];
+                if (e.kind != l1->lvl.ipreaches[t->src[c.winner]].kind) e.mt_id = 0;   // MT-IPv6 into IPv6
+                hspf::isis_propagated_sid(e);
+            }
+            e.metric = c.metric;
+            got.push_back(e);
+        }
+        *n_out = (uint32_t)got.size();
+        if (got.size() > cap) return HSPF_E_NOMEM;
+        std::copy(got.begin(), got.end(), out);
+        return HSPF_OK;
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
 }
 

@@ -1,13 +1,14 @@
 // Device routing-table stage for IS-IS L1/L2 routers (include/holo_spf_lsdb.h, "routing table of an IS-IS L1/L2
 // router"): update_rib (holo-isis/src/route.rs:182-249) over both levels, for every job of a what-if batch.
 //
-// Two launches on the ctx stream.  The summary pass gives one warp to each (job, summary): the lanes stride over
-// the L1 prefixes the summary covers, each runs the prefix's L1 walk, and the warp reduces presence and the lowest
-// metric into the job's summary word.  Then one thread per (job, prefix) runs isis_l1l2_cell_eval
+// Two launches on the ctx stream.  The summary pass (isis_summary.cuh) gives one warp to each (job, summary): the
+// lanes stride over the L1 prefixes the summary covers, each runs the prefix's L1 walk, and the warp reduces presence
+// and the lowest metric into the job's summary word.  Then one thread per (job, prefix) runs isis_l1l2_cell_eval
 // (isis_l1l2_rib_cells.h) over the job's L1 row and L2 row, reading the words the first pass wrote, and the shared
 // cell kernel or the route-delta stage (route_stage.cuh) stores or compares the 24-byte cells.
 #include "../../include/holo_spf_lsdb.h"
 #include "isis_l1l2_rib_cells.h"
+#include "isis_summary.cuh"
 #include "route_stage.cuh"
 
 namespace {
@@ -38,20 +39,11 @@ struct IsisL1L2Cell {
                                                                pl[1][1].job(r2), t, p, words + (size_t)j * t.S);
         return {c.nh_mask, (uint64_t)c.winner | ((uint64_t)c.metric << 32), c.flags};
     }
-    // the summary word of (job j, summary s): lane-strided L1 walks of the covered prefixes, reduced over the warp
+    __host__ __device__ __forceinline__ uint32_t n_summaries() const { return t.S; }
+    // the summary word of (job j, summary s) over the job's L1 row (isis_summary.cuh)
     __device__ __forceinline__ uint64_t summary_word(uint32_t j, uint32_t s, uint32_t lane) const {
         const uint32_t r1 = rows[2 * j];
-        const Planes s1 = pl[0][0].job(r1), m1 = pl[0][1].job(r1);
-        bool any = false;
-        uint32_t low = 0xFFFFFFFFu;
-        for (uint32_t i = t.cov_off[s] + lane; i < t.cov_off[s + 1]; i += 32) {
-            uint32_t m;
-            if (!hspf::isis_l1_metric(s1, m1, t, __ldg(t.cov + i), m)) continue;
-            any = true;
-            low = min(low, m);
-        }
-        low = __reduce_min_sync(0xFFFFFFFFu, low);
-        return __any_sync(0xFFFFFFFFu, any) ? (hspf::kIsisSummaryActive | low) : 0;
+        return hspf::isis_summary_word(pl[0][0].job(r1), pl[0][1].job(r1), t, s, lane);
     }
     __device__ __forceinline__ uint64_t gather(uint32_t, uint32_t, uint32_t) const { return 0; }   // the decode needs none
     __device__ static hspf::CellWords empty() { return {0, 0xFFFFFFFFu, 0}; }                      // winner none
@@ -61,34 +53,6 @@ struct IsisL1L2Cell {
 // registers and spills a little; on an H100, timed against 4 in one run, 8 was faster for the summary kernel, the
 // cell kernel and both delta passes, with byte-identical cells and words (DESIGN.md §4.4, §6).
 constexpr uint32_t kL1L2BlocksPerSM = 8;
-
-template <class Cell, int kMinBlocks>
-__global__ void __launch_bounds__(hspf::kRouteThreads, kMinBlocks)
-isis_summary_kernel(const Cell cell, uint32_t n_jobs, uint64_t *__restrict__ out) {
-    const uint32_t lane = threadIdx.x & 31;
-    const uint64_t n = (uint64_t)n_jobs * cell.t.S;
-    const uint64_t wstride = (uint64_t)gridDim.x * (hspf::kRouteThreads / 32);
-    for (uint64_t w = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) / 32; w < n; w += wstride) {
-        const uint32_t j = (uint32_t)(w / cell.t.S), s = (uint32_t)(w - (uint64_t)j * cell.t.S);
-        const uint64_t word = cell.refused(j) ? 0 : cell.summary_word(j, s, lane);   // warp-uniform branch
-        if (lane == 0) out[w] = word;
-    }
-}
-
-// Enqueues the summary pass on the ctx stream: nothing for 0 jobs or no summaries.
-template <class Cell>
-int launch_summaries(hspf_ctx *ctx, const hspf::DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs,
-                     uint64_t *out) {
-    const uint64_t n = (uint64_t)n_jobs * cell.t.S;
-    if (n == 0) return HSPF_OK;
-    uint32_t blocks = 0;
-    if (const int rc = hspf::route_grid(ctx, table, n * 32, kL1L2BlocksPerSM, blocks)) return rc;
-    isis_summary_kernel<Cell, kL1L2BlocksPerSM>
-        <<<blocks, hspf::kRouteThreads, 0, static_cast<cudaStream_t>(hspf_stream(ctx))>>>(cell, n_jobs, out);
-    if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
-    hspf_note_launches(ctx, 1);
-    return HSPF_OK;
-}
 
 // A topology the table has no root in is not read: its planes are ignored.
 template <class R>
@@ -120,7 +84,7 @@ int l1l2_rib_cells(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_j
     IsisL1L2Cell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(t, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, n_jobs, rows, summary_out, cell)) return rc;
     if (!ctx || !cells) return HSPF_E_INVAL;                  // launch_route_cells' checks, before the first launch
-    if (const int rc = launch_summaries(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
+    if (const int rc = hspf::launch_isis_summaries<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
     return hspf::launch_route_cells<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P, cells, job_status_out, 0, nullptr,
                                                       nullptr, nullptr, nullptr);
 }
@@ -138,7 +102,7 @@ int l1l2_rib_delta(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_j
         (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u) ||
         hspf::delta_tiles64(n_jobs, t->P) > 0xFFFFFFFFull)
         return HSPF_E_INVAL;
-    if (const int rc = launch_summaries(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
+    if (const int rc = hspf::launch_isis_summaries<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
     return hspf::launch_route_delta<hspf::IsisCellLayout, kL1L2BlocksPerSM>(
         ctx, t->dev, cell, n_jobs, t->P, base_cells, n_base, base_of, job_out, records, cap, n_records);
 }

@@ -14,6 +14,7 @@
 #include "../../include/holo_lsdb.h"
 #include "../../include/holo_spf.h"
 #include "../../include/holo_spf_lsdb.h"
+#include "isis_propagation.h"
 
 namespace {
 
@@ -240,8 +241,6 @@ extern "C" int hspf_isis_l1_to_l2(const hl_isis_level *l1, const uint8_t *up_dow
         };
         auto std_on = [](uint8_t t) { return t == HL_ISIS_METRIC_STANDARD || t == HL_ISIS_METRIC_BOTH; };
         auto wide_on = [](uint8_t t) { return t == HL_ISIS_METRIC_WIDE || t == HL_ISIS_METRIC_BOTH; };
-        const bool narrow = std_on(l1_metric_type) && std_on(l2_metric_type);
-        const bool wide = wide_on(l1_metric_type) && wide_on(l2_metric_type);
         const bool mt6 = spt_v6 != nullptr;           // IPv6 unicast topology enabled
         std::vector<hl_isis_ipreach> best;            // kept sorted by (kind, prefix)
         auto key_cmp = [](const hl_isis_ipreach &a, const hl_isis_ipreach &b) {
@@ -254,42 +253,17 @@ extern "C" int hspf_isis_l1_to_l2(const hl_isis_level *l1, const uint8_t *up_dow
             if (lo < best.size() && key_cmp(best[lo], e) == 0) { if (e.metric < best[lo].metric) best[lo] = e; }
             else best.insert(best.begin() + (long)lo, e);
         };
-        for (uint32_t li = 0; li < l1->n_lsps; ++li) {
-            const hl_isis_lsp &lsp = l1->lsps[li];
-            if (lsp.seqno == 0 || lsp.rem_lifetime == 0) continue;
-            if ((lsp.lan_id & 0xFF) != 0) continue;                     // pseudonode LSP
-            if ((lsp.lan_id >> 8) == local_system_id) continue;
-            const uint32_t d_std = dist_of(dmap_std, lsp.lan_id);
-            const uint32_t d_v6 = dist_of(dmap_v6, lsp.lan_id);
-            for (uint32_t k = lsp.ipreach_off; k < lsp.ipreach_off + lsp.n_ipreach; ++k) {
-                hl_isis_ipreach e = l1->ipreaches[k];
-                uint32_t d;
-                bool is_narrow = false;
-                switch (e.kind) {
-                case HL_ISIS_IP_V4_INTERNAL: case HL_ISIS_IP_V4_EXTERNAL:
-                    if (!l1->ipv4_enabled || !narrow) continue;
-                    d = d_std; is_narrow = true; break;
-                case HL_ISIS_IP_V4_EXT:
-                    if (!l1->ipv4_enabled || !wide) continue;
-                    d = d_std; break;
-                case HL_ISIS_IP_V6:
-                    if (mt6 || !l1->ipv6_enabled) continue;
-                    d = d_std; break;
-                case HL_ISIS_IP_MT_V6:
-                    if (e.mt_id != HL_ISIS_MT_IPV6) continue;
-                    d = d_v6; e.kind = HL_ISIS_IP_V6; e.mt_id = 0;      // lands in the L2 LSP's IPv6 reachability
-                    break;
-                default: continue;
-                }
-                if (d == HSPF_DIST_INF) continue;                       // originator not on the L1 SPT
-                if (up_down && up_down[k]) continue;
-                if (shortest_match(cfg, n_cfg, e.prefix, e.len) >= 0) continue;
-                const uint64_t sum = (uint64_t)e.metric + d;
-                e.metric = is_narrow ? (uint32_t)std::min<uint64_t>(sum, 63) : (uint32_t)std::min<uint64_t>(sum, 0xFFFFFFFFull);
-                if (e.has_psid) { e.psid_flags |= HL_ISIS_PSID_R | HL_ISIS_PSID_P; e.psid_flags &= (uint8_t)~HL_ISIS_PSID_E; }
-                offer(e);
-            }
-        }
+        hspf::for_each_propagation(*l1, local_system_id, l1_metric_type, l2_metric_type, mt6, up_down, cfg, n_cfg,
+                                   [&](const hl_isis_lsp &lsp, uint32_t k, uint8_t kind, uint32_t topology, bool is_narrow) {
+            const uint32_t d = dist_of(topology ? dmap_v6 : dmap_std, lsp.lan_id);
+            if (d == HSPF_DIST_INF) return;                             // originator not on the L1 SPT
+            hl_isis_ipreach e = l1->ipreaches[k];
+            if (e.kind != kind) { e.kind = kind; e.mt_id = 0; }         // MT-IPv6 into the L2 LSP's IPv6 reachability
+            const uint64_t sum = (uint64_t)e.metric + d;
+            e.metric = is_narrow ? (uint32_t)std::min<uint64_t>(sum, 63) : (uint32_t)std::min<uint64_t>(sum, 0xFFFFFFFFull);
+            hspf::isis_propagated_sid(e);
+            offer(e);
+        });
         for (uint32_t j = 0; j < n_active; ++j) {       // active summaries (inserted: they replace an equal prefix)
             hl_isis_ipreach e;
             std::memset(&e, 0, sizeof(e));

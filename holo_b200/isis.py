@@ -803,6 +803,90 @@ def l1l2_rib_from_cells(l1: dict, l2: dict, t: L1L2RibTable, cells: np.ndarray, 
     return res
 
 
+# ---- L1 -> L2 propagation of an L1/L2 router (include/holo_spf_lsdb.h: hspf_isis_l1_to_l2_*) -------------
+class L1ToL2Table:
+    """hspf_isis_l1_to_l2_table of one L1/L2 router: what lsp_propagate_l1_to_l2 may put into its L2 LSP in any job.
+    `l1`, `l2`: its instance images; `rib`: its L1L2RibTable (kept alive with this table; upload it before the
+    device calls); `up_down`: u8 per l1 IP reachability entry, or None.  `kind`, `prefix`, `len` [n_keys]: the keys
+    in hspf_isis_l1_to_l2's output order; a cell's winner < n_records is a record, n_records + s is summary s."""
+
+    def __init__(self, l1: dict, l2: dict, rib: L1L2RibTable, up_down=None):
+        self.lib = capi.load_library()
+        self.rib = rib
+        s1, s2 = instance_struct(l1), instance_struct(l2)
+        ud = None if up_down is None else np.ascontiguousarray(up_down, np.uint8)
+        h = C.c_void_p()
+        rc = self.lib.hspf_isis_l1_to_l2_table_create(C.byref(s1), C.byref(s2),
+                                                      ud.ctypes.data if ud is not None and len(ud) else None,
+                                                      rib.handle, C.byref(h))
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, "hspf_isis_l1_to_l2_table_create failed")
+        self.handle = h
+        nk, nr = C.c_uint32(), C.c_uint32()
+        pk, pp, pl = C.c_void_p(), C.c_void_p(), C.c_void_p()
+        assert self.lib.hspf_isis_l1_to_l2_table_keys(h, C.byref(nk), C.byref(nr), C.byref(pk), C.byref(pp),
+                                                      C.byref(pl)) == capi.HSPF_OK
+        self.n_keys, self.n_records = nk.value, nr.value
+        self.kind = route_table.copy_records(pk, self.n_keys, np.uint8)
+        self.prefix = route_table.copy_records(pp, self.n_keys, IP_DT)
+        self.len = route_table.copy_records(pl, self.n_keys, np.uint8)
+        self.n_summaries = rib.n_summaries
+
+    def upload(self, ctx: capi.Context):
+        rc = self.lib.hspf_isis_l1_to_l2_table_upload(ctx.handle, self.handle)
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, ctx.last_error())
+
+    def __del__(self):
+        try:
+            if self.handle:
+                self.lib.hspf_isis_l1_to_l2_table_free(self.handle)
+                self.handle = None
+        except Exception:
+            pass
+
+
+def l1_to_l2_cells_device(ctx: capi.Context, t: L1ToL2Table, n_jobs: int, l1, n_rows: int, rows_ptr: int,
+                          summary_ptr: int, status_ptr: int, cells_ptr: int):
+    """hspf_isis_l1_to_l2_cells / _cells16 over DEVICE planes.  l1: (rs_std, rs_mt6) of the L1 batch
+    (capi.ResultStruct or capi.Result16Struct holding device pointers; rs_mt6 may be None unless L1 has an MT-IPv6
+    root); n_rows: rows of the L1 batch; rows_ptr: device u32 [n_jobs]; summary_ptr: device u64
+    [n_jobs, t.n_summaries]; status_ptr: device u32 [n_jobs] or 0; cells_ptr: device [n_jobs, t.n_keys] cells.
+    Enqueued on the ctx stream; both tables must have been uploaded."""
+    rs = next((x for x in l1 if x is not None), None)      # none at all: the call refuses the arguments
+    route_table.call_stage(ctx, "hspf_isis_l1_to_l2_cells", rs, t.handle, n_jobs, *map(_planes_pair, l1), n_rows,
+                           rows_ptr or None, summary_ptr or None, status_ptr or None, cells_ptr or None)
+
+
+def l1_to_l2_delta_device(ctx: capi.Context, t: L1ToL2Table, n_jobs: int, l1, n_rows: int, rows_ptr: int,
+                          summary_ptr: int, base_ptr: int, n_base: int, base_of_ptr: int, job_out_ptr: int,
+                          records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_isis_l1_to_l2_delta / _delta16: the summary pass, then the route-delta stage over the same walk
+    (arguments as l1_to_l2_cells_device and routes_delta_device)."""
+    rs = next((x for x in l1 if x is not None), None)
+    route_table.call_stage(ctx, "hspf_isis_l1_to_l2_delta", rs, t.handle, n_jobs, *map(_planes_pair, l1), n_rows,
+                           rows_ptr or None, summary_ptr or None, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+
+
+def l1_to_l2_from_cells(l1: dict, t: L1ToL2Table, cells: np.ndarray, words: np.ndarray) -> np.ndarray:
+    """hspf_isis_l1_to_l2_from_cells (host): one job's cells and summary words -> the IPREACH_DT entries
+    hspf_isis_l1_to_l2 gives over the job's L1 SPTs and active summaries."""
+    lib = capi.load_library()
+    cells = np.ascontiguousarray(cells, CELL_DT)
+    words = np.ascontiguousarray(words, np.uint64)
+    assert cells.shape == (t.n_keys,) and words.shape == (t.n_summaries,)
+    s1 = instance_struct(l1)
+    out = np.zeros(max(t.n_keys, 1), IPREACH_DT)
+    n = C.c_uint32()
+    rc = lib.hspf_isis_l1_to_l2_from_cells(C.byref(s1), t.handle, cells.ctypes.data if len(cells) else None,
+                                           words.ctypes.data if len(words) else None, out.ctypes.data, len(out),
+                                           C.byref(n))
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, "hspf_isis_l1_to_l2_from_cells failed")
+    return out[: n.value].copy()
+
+
 def _adjacencies(t: Topology, root: int, sys_of, usage: int):
     """Local interfaces and adjacencies of router `root` of topology t (router i is system sys_of(i))."""
     from . import ospfv3

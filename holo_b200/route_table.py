@@ -138,6 +138,15 @@ def declare(lib: C.CDLL):
                                        vp],
         "hspf_isis_l1l2_rib_from_cells": [C.POINTER(isis.InstanceStruct), C.POINTER(isis.InstanceStruct), vp, vp, vp,
                                           C.POINTER(isis.JobPlanesStruct), C.POINTER(isis.RibStruct)],
+        "hspf_isis_l1_to_l2_table_create": [C.POINTER(isis.InstanceStruct), C.POINTER(isis.InstanceStruct), vp, vp,
+                                            pvp],
+        "hspf_isis_l1_to_l2_table_keys": [vp, u32p, u32p, pvp, pvp, pvp],
+        "hspf_isis_l1_to_l2_table_upload": [vp, vp],
+        "hspf_isis_l1_to_l2_cells": [vp, vp, u32, res, res, u32, vp, vp, vp, vp],
+        "hspf_isis_l1_to_l2_cells16": [vp, vp, u32, res16, res16, u32, vp, vp, vp, vp],
+        "hspf_isis_l1_to_l2_delta": [vp, vp, u32, res, res, u32, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_isis_l1_to_l2_delta16": [vp, vp, u32, res16, res16, u32, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_isis_l1_to_l2_from_cells": [C.POINTER(isis.InstanceStruct), vp, vp, vp, vp, u32, u32p],
     }
     for name, argtypes in sigs.items():
         getattr(lib, name).argtypes = argtypes
@@ -148,3 +157,5 @@ def declare(lib: C.CDLL):
         for name in ("prefixes", "contributors"):
             getattr(lib, f"{table}_{name}").argtypes = [vp]
             getattr(lib, f"{table}_{name}").restype = u32
+    lib.hspf_isis_l1_to_l2_table_free.argtypes = [vp]
+    lib.hspf_isis_l1_to_l2_table_free.restype = None

@@ -639,6 +639,76 @@ int hspf_isis_l1l2_rib_from_cells(const hl_isis_instance *l1, const hl_isis_inst
                                   const uint64_t *summary_words, const hspf_isis_job_planes *planes, hl_isis_rib *out);
 
 /*
+ * L1 -> L2 propagation of an IS-IS L1/L2 router on the device, for every job of a what-if batch: the IP reachability
+ * lsp_propagate_l1_to_l2 (holo-isis lsdb.rs:1149-1357) puts into the router's L2 LSP over the job's L1 SPT — what
+ * every other L2 router of the domain sees of the area (isis_l1_to_l2_cells.h).  It tells whether an L1 failure
+ * stays inside the area (absorbed by a summary, or leaving the metrics unchanged) or reaches every backbone router.
+ *
+ *   hspf_isis_l1_to_l2_table_create  per L1/L2 router: `l1` / `l2` its instance images of level 1 and 2, `up_down`
+ *                             one byte per entry of l1->lvl.ipreaches (NULL: none set; as hspf_isis_l1_to_l2), `rib`
+ *                             the router's hspf_isis_l1l2_ribtable, which supplies the configured summaries and the
+ *                             summary pass; it must outlive the table and be uploaded before the device calls.  The
+ *                             keys are (kind, prefix) in hspf_isis_l1_to_l2's output order: every key an entry could
+ *                             be propagated into in some job, and the summary keys (IPv4: narrow and/or extended,
+ *                             after the L2 metric type; IPv6).  Each propagated key keeps its records in the host
+ *                             loop's order (LSP order, then entry order): the originator's L1 vertex, the entry
+ *                             metric, narrow or not.  Propagation's static filters (valid non-pseudonode LSPs other
+ *                             than the router's own, kinds enabled by the address families and both metric types,
+ *                             MT-IPv6, up/down bits, no covering summary) hold for every job, since what-if jobs
+ *                             change costs only; per job a record only asks whether its originator is reached.
+ *                             HSPF_E_INVAL: levels or level types wrong, system ids differ, an l1 whose L1 vertex
+ *                             counts or roots differ from the rib table's.
+ *   hspf_isis_l1_to_l2_table_keys    K, the number of records, kind[K], prefix[K], len[K]; any pointer may be NULL.
+ *   hspf_isis_l1_to_l2_table_upload  copies the table to the ctx's device.
+ *   hspf_isis_l1_to_l2_cells[16]  DEVICE planes of the L1 batch (l1_std; l1_mt6 may be NULL unless L1 has an MT-IPv6
+ *                             root; the wide ones with nh_words == 1), n_l1_rows its rows, rows [n_jobs] (device) the
+ *                             job's L1 row.  L2 planes are not read.  First the summary pass of
+ *                             hspf_isis_l1l2_rib_cells writes summary_out (device u64 [n_jobs][S], required when
+ *                             S > 0); then cells[n_jobs][K] (device), hl_isis_route_cell: nh_mask 0, winner the
+ *                             record (summary s: n_records + s), metric the advertised one (narrow totals capped at
+ *                             63, wide ones at 2^32 - 1; an active summary's configured metric, else its lowest
+ *                             covered L1 metric, capped at 63 for the narrow key), HL_CELL_PRESENT.  On equal totals
+ *                             the first record in LSP order wins.  job_status_out (device [n_jobs], or NULL): the OR
+ *                             of the job's L1 row status words, HSPF_JS_INVALID for a row out of range; such a job
+ *                             gets empty cells and summary words 0.  Nothing is launched for 0 jobs.  Enqueued on the
+ *                             ctx stream; no synchronisation.
+ *   hspf_isis_l1_to_l2_delta[16]  the summary pass, then the route-delta stage (below) over the same walk: LOST (an
+ *                             originator cut off, a summary gone inactive), GAINED, METRIC (the advertised metric),
+ *                             OTHER (another originator at the same metric: the Prefix-SID may change); never NEXTHOPS.
+ *   hspf_isis_l1_to_l2_from_cells  host: one job's cells and summary words -> exactly the hl_isis_ipreach list of
+ *                             hspf_isis_l1_to_l2 over the job's L1 SPTs (hspf_isis_spt_from_planes of the same planes)
+ *                             and the job's active summaries.  *n_out is set; HSPF_E_NOMEM when it exceeds cap.
+ */
+typedef struct hspf_isis_l1_to_l2_table hspf_isis_l1_to_l2_table;
+int hspf_isis_l1_to_l2_table_create(const hl_isis_instance *l1, const hl_isis_instance *l2, const uint8_t *up_down,
+                                    const hspf_isis_l1l2_ribtable *rib, hspf_isis_l1_to_l2_table **out);
+void hspf_isis_l1_to_l2_table_free(hspf_isis_l1_to_l2_table *t);
+int hspf_isis_l1_to_l2_table_keys(const hspf_isis_l1_to_l2_table *t, uint32_t *n_keys, uint32_t *n_records,
+                                  const uint8_t **kind, const hl_ip_addr **prefix, const uint8_t **len);
+int hspf_isis_l1_to_l2_table_upload(hspf_ctx *ctx, hspf_isis_l1_to_l2_table *t);
+int hspf_isis_l1_to_l2_cells(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs,
+                             const hspf_result *l1_std, const hspf_result *l1_mt6, uint32_t n_l1_rows,
+                             const uint32_t *rows, uint64_t *summary_out, uint32_t *job_status_out,
+                             hl_isis_route_cell *cells);
+int hspf_isis_l1_to_l2_cells16(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs,
+                               const hspf_result16 *l1_std, const hspf_result16 *l1_mt6, uint32_t n_l1_rows,
+                               const uint32_t *rows, uint64_t *summary_out, uint32_t *job_status_out,
+                               hl_isis_route_cell *cells);
+int hspf_isis_l1_to_l2_delta(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs,
+                             const hspf_result *l1_std, const hspf_result *l1_mt6, uint32_t n_l1_rows,
+                             const uint32_t *rows, uint64_t *summary_out, const hl_isis_route_cell *base_cells,
+                             uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                             hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_isis_l1_to_l2_delta16(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs,
+                               const hspf_result16 *l1_std, const hspf_result16 *l1_mt6, uint32_t n_l1_rows,
+                               const uint32_t *rows, uint64_t *summary_out, const hl_isis_route_cell *base_cells,
+                               uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                               hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_isis_l1_to_l2_from_cells(const hl_isis_instance *l1, const hspf_isis_l1_to_l2_table *t,
+                                  const hl_isis_route_cell *cells, const uint64_t *summary_words, hl_isis_ipreach *out,
+                                  uint32_t cap, uint32_t *n_out);
+
+/*
  * Route-delta stage on the device: which prefixes each job of a what-if batch loses, gains, or reaches at another
  * metric or over another next-hop set, against a base route table — without storing the n_jobs x P cell matrix.
  * Per (job, prefix) it runs the same walk as hspf_*_routes_batch[16] and compares the cell with the job's base cell
