@@ -1,9 +1,14 @@
-// The record-building half of hspf_ospfv2_ribtable_create / hspf_ospfv3_ribtable_create (include/holo_spf_lsdb.h),
-// written once over a small version trait, as rib_full is in ospf_rib_host.cc.  The versions differ only in the prefix
-// key, in which field of an inter-area-router LSA names the ASBR, and in the NU-bit LSAs OSPFv3 skips; the records the
-// walk reads (ospf_rib_cells.h) are the same.  Host only.
+// The two host halves of the OSPF routing-table stage, each written once over a small version trait, as rib_full is
+// in ospf_rib_host.cc.  Host only.
+//   build_rib_records  the record-building half of hspf_ospfv2_ribtable_create / hspf_ospfv3_ribtable_create
+//                      (include/holo_spf_lsdb.h).  The versions differ only in the prefix key, in which field of an
+//                      inter-area-router LSA names the ASBR, and in the NU-bit LSAs OSPFv3 skips; the records the walk
+//                      reads (ospf_rib_cells.h) are the same.
+//   decode_rib         one job's cells -> its routing table, for hspf_ospfv2_rib_from_cells,
+//                      hspf_ospfv3_rib_from_cells and hspf_ospfv2_abr_rib_from_cells.  A one-area table decodes as an
+//                      area border router's table with a single area.
 //
-// A version trait T provides:
+// For build_rib_records a version trait T provides:
 //   Key                        prefix key; its order is the table's prefix order (update_rib_full's IpNetwork order)
 //   Sum, Ext                   the summary / inter-area LSA and the AS-external LSA
 //   key(Sum), key(Ext)         the LSA's prefix key (host bits kept, as update_rib_full keeps them)
@@ -13,10 +18,25 @@
 //   options(Sum), options(Ext) prefix options a route through the LSA carries
 //   set_prefix(rt, u, Key)     writes prefix u of the table
 //   kV3                        the table carries OSPFv3 prefixes and per-record prefix options
+//
+// For decode_rib it also provides:
+//   Area, Rib                  the area image and the caller's output
+//   Route, Hop                 a route and a next hop of that output
+//   Result, Net                intra_from_cells' output and one route of it
+//   Nh, JobDecode              a resolved next hop; one job's decode state over one area (flattened area, root,
+//                              Resolver `rs`)
+//   intra_from_cells           the intra-area decode of one area's cells (hspf_ospfv{2,3}_routes_from_cells' body)
+//   nh_less, nh_same           next-hop order (NexthopKey) and same key
+//   nh_conflict(a, b)          a and b have one key, but attributes the cell cannot choose between
+//   route_prefix(o, d, u)      writes prefix u of the decode into the route (v2 prefix / mask, v3 prefix6 / len)
+//   from_intra(o, net)         what a route takes from its intra-area route (v2 SR label, v3 prefix options)
+//   from_record(o, rt, rec)    what it takes from type-3 / type-5 record `rec` of one-area table rt (v3 prefix options)
+//   to_nh(hop, sort), to_hop   a next hop into the merged set, naming its interface's sort key, and back out
 #pragma once
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <numeric>
 #include <unordered_map>
 #include <vector>
 
@@ -140,6 +160,179 @@ int build_rib_records(hspf_ospfv2_ribtable &rt, uint32_t area_id, RouterVertex r
     }
     for (const auto &l : t4) rt.recs.insert(rt.recs.end(), l.begin(), l.end());
     return HSPF_OK;
+}
+
+// One area of a decode: record and prefix indices are the decoded table's unless said otherwise.
+template <class T>
+struct RibDecodeArea {
+    const typename T::Area *a;
+    const hspf_ospfv2_ribtable *rt;      // the area's one-area table
+    const uint32_t *prefix_of;           // per prefix: its index in rt, 0xFFFFFFFF if none
+    uint32_t intra_first;                // the first of the area's intra-area records, which are rt's in rt's order
+    uint64_t intra_end;                  // one past the last record an intra-area cell of the area may name
+    const uint32_t *o3;                  // [P + 1] the area's type-3 record ranges
+    uint32_t base;                       // atom a of the area is bit base + a of the cell's masks ...
+    uint64_t mask;                       // ... and these are its bits
+    uint32_t area_id;
+    typename T::JobDecode *jd;           // the job's decode state over the area
+};
+
+template <class T>
+struct RibDecode {
+    std::vector<RibDecodeArea<T>> area;
+    uint32_t P;
+    const uint32_t *prefix, *plen;       // [P] (OSPFv3: prefix6)
+    const hl_ip_addr *prefix6;
+    const uint32_t *o5;                  // [P + 1] type-5 record ranges
+    const uint32_t *ext_tag;             // per type-5 record (index - ext_base): the LSA's tag
+    uint32_t ext_base;
+    uint32_t max_paths;
+};
+
+// One job's cells -> its routing table, in prefix order, into `out` (HSPF_E_NOMEM with the counts when it does not
+// fit).  1. Each area's intra-area winners go through that area's intra-area decode, every area before step 2, so
+// that its refusals come before step 2's.  2. A route is the intra-area route, or the type-3 / type-5 winner checked
+// against its record range; every other atom of the cell resolves through its own area's resolver; the union of the
+// next hops in next-hop order, cut to max_paths, is what rib_full's merge-then-clip leaves.  Two atoms that give one
+// next hop with different attributes refuse the job (HSPF_E_UNSUPPORTED): the reference keeps whichever came last.
+template <class T>
+int decode_rib(const RibDecode<T> &d, const hl_ospf_rib_cell *cells, typename T::Rib *out) {
+    using Nh = typename T::Nh;
+    constexpr uint32_t kNone = 0xFFFFFFFFu;
+    const uint32_t A = (uint32_t)d.area.size(), P = d.P;
+    auto intra_area = [&](uint32_t w) {
+        for (uint32_t i = 0; i < A; ++i)
+            if (w >= d.area[i].intra_first && w < d.area[i].intra_end) return i;
+        return kNone;
+    };
+    // 1. per area, the intra-area cells its records won, through the intra-area decode
+    std::vector<std::vector<typename T::Net>> nets(A);
+    std::vector<std::vector<typename T::Hop>> nh(A);
+    std::vector<typename T::Result> res(A);
+    for (uint32_t i = 0; i < A; ++i) {
+        const RibDecodeArea<T> &ar = d.area[i];
+        const hspf_ospfv2_ribtable &rt = *ar.rt;
+        const uint32_t PI = (uint32_t)rt.intra->t.plen.size();
+        std::vector<hl_route_cell> ic(PI, hl_route_cell{0, 0, kNone, 0, 0, 0});
+        for (uint32_t u = 0; u < P; ++u) {
+            const hl_ospf_rib_cell &c = cells[u];
+            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(c) != HL_PATH_INTRA_AREA) continue;
+            if (intra_area(c.winner) != i) continue;
+            const uint32_t q = ar.prefix_of[u];
+            if (q == kNone || rt.intra_of[q] == kNone || HL_RIB_CELL_METRIC(c) > 0xFFFFu) return HSPF_E_INVAL;
+            ic[rt.intra_of[q]] = hl_route_cell{(c.nh_mask & ar.mask) >> ar.base, (c.aux & ar.mask) >> ar.base,
+                                               c.winner - ar.intra_first, (uint16_t)HL_RIB_CELL_METRIC(c),
+                                               (uint8_t)HL_RIB_CELL_FLAGS(c), 0};
+        }
+        nets[i].resize(PI);
+        nh[i].resize(std::max<size_t>(64, (size_t)PI * 2));
+        int rc = HSPF_OK;
+        for (int attempt = 0; attempt < 2; ++attempt) {
+            res[i] = typename T::Result{};
+            res[i].routes_cap = PI; res[i].routes = nets[i].data();
+            res[i].nexthops_cap = (uint32_t)nh[i].size(); res[i].nexthops = nh[i].data();
+            rc = T::intra_from_cells(*ar.jd, ar.a, rt.intra, ic.data(), &res[i]);
+            if (rc != HSPF_E_NOMEM) break;
+            nh[i].resize(res[i].n_nexthops);
+        }
+        if (rc) return rc;
+    }
+    // 2. every route in prefix order; the atoms no intra-area route gave through their own area's resolver
+    std::vector<typename T::Route> routes;
+    std::vector<typename T::Hop> hops;
+    std::vector<Nh> set;
+    std::vector<uint32_t> ri(A, 0);
+    auto sort_key = [&](uint32_t i, uint32_t iface) {
+        const typename T::Area &a = *d.area[i].a;
+        return iface < a.n_ifaces ? a.ifaces[iface].sort_key : 0xFFFFFFFFu;
+    };
+    auto add_atoms = [&](uint64_t m) {
+        for (; m; m &= m - 1) {
+            const uint32_t b = (uint32_t)__builtin_ctzll(m);
+            uint32_t i = 0;
+            while (i < A && !((d.area[i].mask >> b) & 1u)) ++i;
+            if (i == A) return HSPF_E_INVAL;                       // an atom no area has
+            for (const Nh &x : d.area[i].jd->rs->resolve(b - d.area[i].base)) {
+                auto at = std::lower_bound(set.begin(), set.end(), x, T::nh_less);
+                if (at == set.end() || !T::nh_same(*at, x)) { set.insert(at, x); continue; }
+                if (T::nh_conflict(*at, x)) return HSPF_E_UNSUPPORTED;
+            }
+        }
+        return HSPF_OK;
+    };
+    for (uint32_t u = 0; u < P; ++u) {
+        const hl_ospf_rib_cell &c = cells[u];
+        if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT)) continue;
+        const uint32_t path = HL_RIB_CELL_PATH(c);
+        typename T::Route o;
+        std::memset(&o, 0, sizeof(o));
+        T::route_prefix(o, d, u);
+        o.path_type = (uint8_t)path;
+        o.nh_off = (uint32_t)hops.size();
+        set.clear();
+        uint64_t rest = c.nh_mask;
+        if (path == HL_PATH_INTRA_AREA) {
+            const uint32_t w = intra_area(c.winner);
+            if (w == kNone || ri[w] >= res[w].n_routes) return HSPF_E_INVAL;
+            const typename T::Net &r = nets[w][ri[w]++];
+            o.metric = r.metric; o.area_id = d.area[w].area_id; o.has_area = 1; o.flags = r.flags;
+            T::from_intra(o, r);
+            rest &= ~d.area[w].mask;
+            for (uint32_t k = 0; k < r.n_nh; ++k) {
+                typename T::Hop h = nh[w][r.nh_off + k];
+                const uint32_t sort = sort_key(w, h.iface);
+                // with no other area's atoms the area's decode has merged and cut them: straight to the output
+                if (rest) set.push_back(T::to_nh(h, sort));
+                else { h.iface = sort; hops.push_back(h); }
+            }
+        } else {
+            if (path == HL_PATH_INTER_AREA) {
+                uint32_t w = 0;
+                while (w < A && !(c.winner >= d.area[w].o3[u] && c.winner < d.area[w].o3[u + 1])) ++w;
+                if (w == A) return HSPF_E_INVAL;
+                o.metric = HL_RIB_CELL_METRIC(c); o.area_id = d.area[w].area_id; o.has_area = 1;
+            } else {
+                if (c.winner < d.o5[u] || c.winner >= d.o5[u + 1]) return HSPF_E_INVAL;
+                o.metric = HL_RIB_CELL_METRIC(c);
+                o.tag = d.ext_tag[c.winner - d.ext_base];
+                if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
+            }
+            T::from_record(o, *d.area[0].rt, c.winner);            // only OSPFv3 reads it, whose tables have one area
+        }
+        const int rc = add_atoms(rest);
+        if (rc) return rc;
+        if (set.size() > d.max_paths) set.resize(d.max_paths);
+        for (const Nh &x : set) hops.push_back(T::to_hop(x));
+        o.n_nh = (uint32_t)hops.size() - o.nh_off;
+        routes.push_back(o);
+    }
+    out->n_routes = (uint32_t)routes.size();
+    out->n_nexthops = (uint32_t)hops.size();
+    if (out->n_routes > out->routes_cap || out->n_nexthops > out->nexthops_cap) return HSPF_E_NOMEM;
+    if ((out->n_routes && !out->routes) || (out->n_nexthops && !out->nexthops)) return HSPF_E_INVAL;
+    std::copy(routes.begin(), routes.end(), out->routes);
+    std::copy(hops.begin(), hops.end(), out->nexthops);
+    return HSPF_OK;
+}
+
+// hspf_ospfv2_rib_from_cells / hspf_ospfv3_rib_from_cells after their argument checks: the decode of a table with
+// one area whose prefixes, records and atoms are all the table's own.  Every intra-area cell is the area's, so that
+// the intra-area decode refuses a winner outside the intra-area records, as it does for the area's own cells.
+template <class T>
+int decode_one_area_rib(const typename T::Area *a, const hspf_ospfv2_ribtable &rt, const hl_ospf_rib_cell *cells,
+                        const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out) {
+    typename T::JobDecode jd;
+    const int rc = jd.init(a, (uint32_t)rt.vflags.size(), gather_v, gather_nh, n_gather);
+    if (rc) return rc;
+    if (jd.root == 0xFFFFFFFFu) return HSPF_E_INVAL;               // not the root of any job over this table
+    const uint32_t P = (uint32_t)rt.plen.size();
+    const uint32_t *o3 = rt.off.data() + P + 1;
+    std::vector<uint32_t> same(P);
+    std::iota(same.begin(), same.end(), 0u);
+    RibDecode<T> d{{RibDecodeArea<T>{a, &rt, same.data(), 0, ~0ull, o3, 0, ~0ull, rt.area_id, &jd}},
+                   P, rt.prefix.data(), rt.plen.data(), rt.prefix6.data(), o3 + P + 1, rt.ext_tag.data(), rt.ext_base,
+                   a->max_paths};
+    return decode_rib(d, cells, out);
 }
 
 }  // namespace hspf

@@ -39,6 +39,10 @@ inline bool nh_less(const Nh &a, const Nh &b) {
     return a.addr < b.addr;
 }
 inline bool nh_same_key(const Nh &a, const Nh &b) { return a.sort == b.sort && a.has_addr == b.has_addr && a.addr == b.addr; }
+// two atoms, one next hop: the reference keeps whichever advertiser came last; the cell cannot tell unless both agree
+inline bool nh_conflict(const Nh &a, const Nh &b) {
+    return a.iface != b.iface || a.nbr != b.nbr || a.has_nbr != b.has_nbr || a.has_label != b.has_label || a.label != b.label;
+}
 
 // sorted-unique insert; an existing key is overwritten (BTreeMap::insert/extend)
 void nh_insert(std::vector<Nh> &set, const Nh &x) {
@@ -324,23 +328,6 @@ struct Route {
 };
 
 inline uint64_t pkey(uint32_t prefix, uint32_t plen) { return ((uint64_t)prefix << 8) | plen; }
-
-// the OSPFv2 side of hspf::build_rib_records (ospf_ribtable.h)
-struct RibV2 {
-    using Key = uint64_t;
-    using Sum = hl_ospfv2_summary_lsa;
-    using Ext = hl_ospfv2_external_lsa;
-    static constexpr bool kV3 = false;
-    static Key key(const Sum &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
-    static Key key(const Ext &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
-    static Key intra_key(const hspf::RouteTable &t, uint32_t k) { return pkey(t.prefix[k], t.plen[k]); }
-    static bool skip(const Sum &) { return false; }
-    static bool skip(const Ext &) { return false; }
-    static uint32_t asbr_id(const Sum &l) { return l.lsa_id; }
-    static uint8_t options(const Sum &) { return 0; }
-    static uint8_t options(const Ext &) { return 0; }
-    static void set_prefix(hspf_ospfv2_ribtable &rt, uint32_t u, Key k) { rt.prefix[u] = (uint32_t)(k >> 8); rt.plen[u] = (uint32_t)(k & 0xFF); }
-};
 
 }  // namespace
 
@@ -1005,10 +992,7 @@ int intra_from_cells(JobDecode &jd, const hl_ospfv2_area *a, const hspf_ospfv2_r
                 }
                 auto it = std::lower_bound(set.begin(), set.end(), x, nh_less);
                 if (it != set.end() && nh_same_key(*it, x)) {
-                    // two atoms, one next hop: the reference keeps whichever advertiser came last; the
-                    // cell cannot tell unless both agree
-                    if (it->iface != x.iface || it->nbr != x.nbr || it->has_nbr != x.has_nbr ||
-                        it->has_label != x.has_label || it->label != x.label) return HSPF_E_UNSUPPORTED;
+                    if (nh_conflict(*it, x)) return HSPF_E_UNSUPPORTED;
                 } else {
                     set.insert(it, x);
                 }
@@ -1071,6 +1055,51 @@ void hspf_ospfv2_ribtable_free(hspf_ospfv2_ribtable *rt) {
 
 namespace {
 
+// the OSPFv2 side of hspf::build_rib_records and hspf::decode_rib (ospf_ribtable.h)
+struct RibV2 {
+    using Key = uint64_t;
+    using Sum = hl_ospfv2_summary_lsa;
+    using Ext = hl_ospfv2_external_lsa;
+    static constexpr bool kV3 = false;
+    static Key key(const Sum &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
+    static Key key(const Ext &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
+    static Key intra_key(const hspf::RouteTable &t, uint32_t k) { return pkey(t.prefix[k], t.plen[k]); }
+    static bool skip(const Sum &) { return false; }
+    static bool skip(const Ext &) { return false; }
+    static uint32_t asbr_id(const Sum &l) { return l.lsa_id; }
+    static uint8_t options(const Sum &) { return 0; }
+    static uint8_t options(const Ext &) { return 0; }
+    static void set_prefix(hspf_ospfv2_ribtable &rt, uint32_t u, Key k) { rt.prefix[u] = (uint32_t)(k >> 8); rt.plen[u] = (uint32_t)(k & 0xFF); }
+
+    using Area = hl_ospfv2_area;
+    using Rib = hl_ospfv2_rib;
+    using Route = hl_rib_route;
+    using Hop = hl_nexthop;
+    using Result = hl_ospfv2_result;
+    using Net = hl_route_net;
+    using Nh = ::Nh;
+    using JobDecode = ::JobDecode;
+    static constexpr auto intra_from_cells = ::intra_from_cells;
+    static constexpr auto nh_less = ::nh_less;
+    static constexpr auto nh_same = nh_same_key;
+    static constexpr auto nh_conflict = ::nh_conflict;
+    static void route_prefix(Route &o, const hspf::RibDecode<RibV2> &d, uint32_t u) {
+        o.prefix = d.prefix[u]; o.mask = d.plen[u] == 0 ? 0 : 0xFFFFFFFFu << (32 - d.plen[u]);
+    }
+    static void from_intra(Route &o, const Net &r) { o.has_sr_label = r.has_sr_label; o.sr_label = r.has_sr_label ? r.sr_label : 0; }
+    static void from_record(Route &, const hspf_ospfv2_ribtable &, uint32_t) {}
+    static Nh to_nh(const Hop &h, uint32_t sort) {
+        return Nh{sort, h.iface, h.addr, h.nbr_router_id, h.sr_label, h.has_addr, h.has_nbr, h.has_label};
+    }
+    static Hop to_hop(const Nh &x) {
+        Hop h{};
+        h.iface = x.sort; h.addr = x.has_addr ? x.addr : 0; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
+        h.sr_label = x.has_label ? x.label : 0;
+        h.has_addr = x.has_addr; h.has_nbr = x.has_nbr; h.has_label = x.has_label;
+        return h;
+    }
+};
+
 // hspf_ospfv2_ribtable_create after its argument checks; `transit_walk` as for hspf::build_rib_records
 int make_ribtable(const hspf_ospfv2_flat *flat, uint32_t area_id, const hl_ospfv2_summary_lsa *sums, uint32_t n_sums,
                   const hl_ospfv2_external_lsa *ext, uint32_t n_ext, bool transit_walk, hspf_ospfv2_ribtable **out) {
@@ -1130,93 +1159,7 @@ int hspf_ospfv2_rib_from_cells(const hl_ospfv2_area *a, const hspf_ospfv2_ribtab
     if (!a || !rt || rt->v3 || !rt->intra || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
     try {
         out->n_routes = out->n_nexthops = 0;
-        JobDecode jd;
-        int rc = jd.init(a, (uint32_t)rt->vflags.size(), gather_v, gather_nh, n_gather);
-        if (rc) return rc;
-        if (jd.root == kNone) return HSPF_E_INVAL;                  // not the root of any job over this table
-        const uint32_t P = (uint32_t)rt->prefix.size(), PI = (uint32_t)rt->intra->t.prefix.size();
-        const uint32_t *o3 = rt->off.data() + P + 1, *o5 = o3 + P + 1;
-        // 1. the intra-area cells, through the intra-area decode
-        std::vector<hl_route_cell> ic(PI, hl_route_cell{0, 0, kNone, 0, 0, 0});
-        for (uint32_t u = 0; u < P; ++u) {
-            const hl_ospf_rib_cell &c = cells[u];
-            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(c) != HL_PATH_INTRA_AREA) continue;
-            if (rt->intra_of[u] == kNone || HL_RIB_CELL_METRIC(c) > 0xFFFFu) return HSPF_E_INVAL;
-            ic[rt->intra_of[u]] = hl_route_cell{c.nh_mask, c.aux, c.winner, (uint16_t)HL_RIB_CELL_METRIC(c),
-                                                (uint8_t)HL_RIB_CELL_FLAGS(c), 0};
-        }
-        std::vector<hl_route_net> nets(PI);
-        std::vector<hl_nexthop> nh(std::max<size_t>(64, (size_t)PI * 2));
-        hl_ospfv2_result res{};
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            res = hl_ospfv2_result{};
-            res.routes_cap = PI; res.routes = nets.data();
-            res.nexthops_cap = (uint32_t)nh.size(); res.nexthops = nh.data();
-            rc = intra_from_cells(jd, a, rt->intra, ic.data(), &res);
-            if (rc != HSPF_E_NOMEM) break;
-            nh.resize(res.n_nexthops);
-        }
-        if (rc) return rc;
-        // 2. every route in prefix order; inter-area and external next hops from the cell's atoms
-        std::vector<hl_rib_route> routes;
-        std::vector<hl_nexthop> hops;
-        std::vector<Nh> set;
-        auto sort_key = [&](uint32_t iface) { return iface < a->n_ifaces ? a->ifaces[iface].sort_key : 0xFFFFFFFFu; };
-        uint32_t ri = 0;
-        for (uint32_t u = 0; u < P; ++u) {
-            const hl_ospf_rib_cell &c = cells[u];
-            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT)) continue;
-            const uint32_t path = HL_RIB_CELL_PATH(c);
-            hl_rib_route o;
-            std::memset(&o, 0, sizeof(o));
-            o.prefix = rt->prefix[u]; o.mask = rt->plen[u] == 0 ? 0 : 0xFFFFFFFFu << (32 - rt->plen[u]);
-            o.path_type = (uint8_t)path;
-            o.nh_off = (uint32_t)hops.size();
-            if (path == HL_PATH_INTRA_AREA) {
-                if (ri >= res.n_routes) return HSPF_E_INVAL;
-                const hl_route_net &r = nets[ri++];
-                o.metric = r.metric; o.area_id = rt->area_id; o.has_area = 1; o.flags = r.flags;
-                o.has_sr_label = r.has_sr_label; o.sr_label = r.has_sr_label ? r.sr_label : 0;
-                for (uint32_t k = 0; k < r.n_nh; ++k) {
-                    hl_nexthop h = nh[r.nh_off + k];
-                    h.iface = sort_key(h.iface);                      // the merged table names interfaces by sort key
-                    hops.push_back(h);
-                }
-            } else {
-                const bool inter = path == HL_PATH_INTER_AREA;
-                if (inter ? (c.winner < o3[u] || c.winner >= o3[u + 1]) : (c.winner < o5[u] || c.winner >= o5[u + 1]))
-                    return HSPF_E_INVAL;
-                o.metric = HL_RIB_CELL_METRIC(c);
-                if (inter) { o.area_id = rt->area_id; o.has_area = 1; }
-                else o.tag = rt->ext_tag[c.winner - rt->ext_base];
-                if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
-                set.clear();
-                for (uint64_t m = c.nh_mask; m; m &= m - 1) {
-                    for (const Nh &x : jd.rs->resolve((uint32_t)__builtin_ctzll(m))) {
-                        auto at = std::lower_bound(set.begin(), set.end(), x, nh_less);
-                        if (at == set.end() || !nh_same_key(*at, x)) { set.insert(at, x); continue; }
-                        // two atoms, one next hop: which router's entry gave it depends on the merge order
-                        if (at->iface != x.iface || at->nbr != x.nbr || at->has_nbr != x.has_nbr) return HSPF_E_UNSUPPORTED;
-                    }
-                }
-                if (set.size() > a->max_paths) set.resize(a->max_paths);
-                for (const Nh &x : set) {
-                    hl_nexthop h{};
-                    h.iface = sort_key(x.iface); h.addr = x.has_addr ? x.addr : 0; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
-                    h.has_addr = x.has_addr; h.has_nbr = x.has_nbr;
-                    hops.push_back(h);
-                }
-            }
-            o.n_nh = (uint32_t)hops.size() - o.nh_off;
-            routes.push_back(o);
-        }
-        out->n_routes = (uint32_t)routes.size();
-        out->n_nexthops = (uint32_t)hops.size();
-        if (out->n_routes > out->routes_cap || out->n_nexthops > out->nexthops_cap) return HSPF_E_NOMEM;
-        if ((out->n_routes && !out->routes) || (out->n_nexthops && !out->nexthops)) return HSPF_E_INVAL;
-        std::copy(routes.begin(), routes.end(), out->routes);
-        std::copy(hops.begin(), hops.end(), out->nexthops);
-        return HSPF_OK;
+        return hspf::decode_one_area_rib<RibV2>(a, *rt, cells, gather_v, gather_nh, n_gather, out);
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;
     } catch (...) {
@@ -1420,9 +1363,9 @@ int hspf_ospfv2_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_o
     try {
         out->n_routes = out->n_nexthops = 0;
         const uint32_t A = n_areas, P = (uint32_t)t->prefix.size(), S = P + 1;
-        const uint32_t *o3 = t->off.data() + (size_t)A * S, *o5 = o3 + (size_t)A * S;
         std::vector<JobDecode> jd(A);
-        std::vector<uint64_t> amask(A);
+        hspf::RibDecode<RibV2> d{{}, P, t->prefix.data(), t->plen.data(), nullptr, t->off.data() + 2 * (size_t)A * S,
+                                 t->ext_tag.data(), t->ext_base, t->max_paths};
         for (uint32_t i = 0; i < A; ++i) {
             const hl_ospfv2_area &a = areas[i];
             if (a.router_id != t->router_id || a.area_id != t->area_id[i] || a.max_paths != t->max_paths) return HSPF_E_INVAL;
@@ -1436,123 +1379,12 @@ int hspf_ospfv2_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_o
             if (rc) return rc;
             if (jd[i].root != t->root[i]) return HSPF_E_INVAL;
             const uint32_t na = t->n_atoms[i];
-            amask[i] = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << t->base[i]);
+            const uint64_t mask = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << t->base[i]);
+            d.area.push_back({&a, t->area[i], t->area_prefix[i].data(), t->intra_base[i],
+                              (uint64_t)t->intra_base[i] + t->area[i]->n_intra, t->off.data() + (A + i) * (size_t)S,
+                              t->base[i], mask, t->area_id[i], &jd[i]});
         }
-        auto intra_area = [&](uint32_t w) {
-            for (uint32_t i = 0; i < A; ++i)
-                if (w >= t->intra_base[i] && w < t->intra_base[i] + t->area[i]->n_intra) return i;
-            return kNone;
-        };
-        // 1. per area, the intra-area cells its records won, through the intra-area decode
-        std::vector<std::vector<hl_route_net>> nets(A);
-        std::vector<std::vector<hl_nexthop>> nh(A);
-        std::vector<hl_ospfv2_result> res(A);
-        for (uint32_t i = 0; i < A; ++i) {
-            const hspf_ospfv2_ribtable &rt = *t->area[i];
-            const uint32_t PI = (uint32_t)rt.intra->t.prefix.size();
-            std::vector<hl_route_cell> ic(PI, hl_route_cell{0, 0, kNone, 0, 0, 0});
-            for (uint32_t u = 0; u < P; ++u) {
-                const hl_ospf_rib_cell &c = cells[u];
-                if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(c) != HL_PATH_INTRA_AREA) continue;
-                if (intra_area(c.winner) != i) continue;
-                const uint32_t q = t->area_prefix[i][u];
-                if (q == kNone || rt.intra_of[q] == kNone || HL_RIB_CELL_METRIC(c) > 0xFFFFu) return HSPF_E_INVAL;
-                ic[rt.intra_of[q]] = hl_route_cell{(c.nh_mask & amask[i]) >> t->base[i], (c.aux & amask[i]) >> t->base[i],
-                                                   c.winner - t->intra_base[i], (uint16_t)HL_RIB_CELL_METRIC(c),
-                                                   (uint8_t)HL_RIB_CELL_FLAGS(c), 0};
-            }
-            nets[i].resize(PI);
-            nh[i].resize(std::max<size_t>(64, (size_t)PI * 2));
-            int rc = HSPF_OK;
-            for (int attempt = 0; attempt < 2; ++attempt) {
-                res[i] = hl_ospfv2_result{};
-                res[i].routes_cap = PI; res[i].routes = nets[i].data();
-                res[i].nexthops_cap = (uint32_t)nh[i].size(); res[i].nexthops = nh[i].data();
-                rc = intra_from_cells(jd[i], &areas[i], rt.intra, ic.data(), &res[i]);
-                if (rc != HSPF_E_NOMEM) break;
-                nh[i].resize(res[i].n_nexthops);
-            }
-            if (rc) return rc;
-        }
-        // 2. every route in prefix order; atoms of the other areas through their own resolvers
-        std::vector<hl_rib_route> routes;
-        std::vector<hl_nexthop> hops;
-        std::vector<Nh> set;
-        std::vector<uint32_t> ri(A, 0);
-        auto sort_key = [&](uint32_t i, uint32_t iface) {
-            return iface < areas[i].n_ifaces ? areas[i].ifaces[iface].sort_key : 0xFFFFFFFFu;
-        };
-        auto add_atoms = [&](uint64_t m) {
-            for (; m; m &= m - 1) {
-                const uint32_t b = (uint32_t)__builtin_ctzll(m);
-                uint32_t i = 0;
-                while (i < A && !((amask[i] >> b) & 1u)) ++i;
-                if (i == A) return HSPF_E_INVAL;                       // an atom no area has
-                for (const Nh &x : jd[i].rs->resolve(b - t->base[i])) {
-                    auto at = std::lower_bound(set.begin(), set.end(), x, nh_less);
-                    if (at == set.end() || !nh_same_key(*at, x)) { set.insert(at, x); continue; }
-                    // two atoms, one next hop: which entry gave it depends on the merge order
-                    if (at->iface != x.iface || at->nbr != x.nbr || at->has_nbr != x.has_nbr || at->has_label != x.has_label ||
-                        at->label != x.label)
-                        return HSPF_E_UNSUPPORTED;
-                }
-            }
-            return HSPF_OK;
-        };
-        for (uint32_t u = 0; u < P; ++u) {
-            const hl_ospf_rib_cell &c = cells[u];
-            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT)) continue;
-            const uint32_t path = HL_RIB_CELL_PATH(c);
-            hl_rib_route o;
-            std::memset(&o, 0, sizeof(o));
-            o.prefix = t->prefix[u]; o.mask = t->plen[u] == 0 ? 0 : 0xFFFFFFFFu << (32 - t->plen[u]);
-            o.path_type = (uint8_t)path;
-            o.nh_off = (uint32_t)hops.size();
-            set.clear();
-            uint64_t rest = c.nh_mask;
-            if (path == HL_PATH_INTRA_AREA) {
-                const uint32_t w = intra_area(c.winner);
-                if (w == kNone || ri[w] >= res[w].n_routes) return HSPF_E_INVAL;
-                const hl_route_net &r = nets[w][ri[w]++];
-                o.metric = r.metric; o.area_id = t->area_id[w]; o.has_area = 1; o.flags = r.flags;
-                o.has_sr_label = r.has_sr_label; o.sr_label = r.has_sr_label ? r.sr_label : 0;
-                for (uint32_t k = 0; k < r.n_nh; ++k) {
-                    const hl_nexthop &h = nh[w][r.nh_off + k];
-                    set.push_back(Nh{sort_key(w, h.iface), h.iface, h.addr, h.nbr_router_id, h.sr_label, h.has_addr,
-                                     h.has_nbr, h.has_label});
-                }
-                rest &= ~amask[w];
-            } else if (path == HL_PATH_INTER_AREA) {
-                uint32_t w = 0;
-                while (w < A && !(c.winner >= o3[w * S + u] && c.winner < o3[w * S + u + 1])) ++w;
-                if (w == A) return HSPF_E_INVAL;
-                o.metric = HL_RIB_CELL_METRIC(c); o.area_id = t->area_id[w]; o.has_area = 1;
-            } else {
-                if (c.winner < o5[u] || c.winner >= o5[u + 1]) return HSPF_E_INVAL;
-                o.metric = HL_RIB_CELL_METRIC(c);
-                o.tag = t->ext_tag[c.winner - t->ext_base];
-                if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
-            }
-            const int rc = add_atoms(rest);
-            if (rc) return rc;
-            if (set.size() > t->max_paths) set.resize(t->max_paths);
-            for (const Nh &x : set) {
-                hl_nexthop h{};
-                h.iface = x.sort; h.addr = x.has_addr ? x.addr : 0; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
-                h.sr_label = x.has_label ? x.label : 0;
-                h.has_addr = x.has_addr; h.has_nbr = x.has_nbr; h.has_label = x.has_label;
-                hops.push_back(h);
-            }
-            o.n_nh = (uint32_t)hops.size() - o.nh_off;
-            routes.push_back(o);
-        }
-        out->n_routes = (uint32_t)routes.size();
-        out->n_nexthops = (uint32_t)hops.size();
-        if (out->n_routes > out->routes_cap || out->n_nexthops > out->nexthops_cap) return HSPF_E_NOMEM;
-        if ((out->n_routes && !out->routes) || (out->n_nexthops && !out->nexthops)) return HSPF_E_INVAL;
-        std::copy(routes.begin(), routes.end(), out->routes);
-        std::copy(hops.begin(), hops.end(), out->nexthops);
-        return HSPF_OK;
+        return hspf::decode_rib(d, cells, out);
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;
     } catch (...) {

@@ -44,6 +44,9 @@ inline bool nh_less(const Nh6 &a, const Nh6 &b) {
 inline bool nh_same(const Nh6 &a, const Nh6 &b) {
     return a.sort == b.sort && a.has_addr == b.has_addr && (!a.has_addr || addr_cmp(a.addr, b.addr) == 0);
 }
+inline bool nh_conflict(const Nh6 &a, const Nh6 &b) {
+    return a.iface != b.iface || a.has_nbr != b.has_nbr || (b.has_nbr && a.nbr != b.nbr);
+}
 void nh_insert(std::vector<Nh6> &set, const Nh6 &x) {
     auto it = std::lower_bound(set.begin(), set.end(), x, nh_less);
     if (it != set.end() && nh_same(*it, x)) *it = x; else set.insert(it, x);
@@ -678,7 +681,7 @@ bool atom_hops(Resolver &rs, uint64_t mask, std::vector<Nh6> &set) {
         for (const Nh6 &x : rs.resolve((uint32_t)__builtin_ctzll(m))) {
             auto it = std::lower_bound(set.begin(), set.end(), x, nh_less);
             if (it == set.end() || !nh_same(*it, x)) { set.insert(it, x); continue; }
-            if (it->iface != x.iface || it->has_nbr != x.has_nbr || (x.has_nbr && it->nbr != x.nbr)) return false;
+            if (nh_conflict(*it, x)) return false;
         }
     }
     return true;
@@ -722,7 +725,7 @@ int intra_from_cells(JobDecode &jd, const hl_ospfv3_area *a, const hspf_ospfv2_r
     return HSPF_OK;
 }
 
-// the OSPFv3 side of hspf::build_rib_records (ospf_ribtable.h): rib_full<V3> of ospf_rib_host.cc
+// the OSPFv3 side of hspf::build_rib_records and hspf::decode_rib (ospf_ribtable.h): rib_full<V3> of ospf_rib_host.cc
 struct RibV3 {
     using Key = std::array<uint8_t, 17>;                  // 16 address bytes, then the length
     using Sum = hl_ospfv3_inter_area_lsa;
@@ -744,6 +747,32 @@ struct RibV3 {
         std::memcpy(p.bytes, k.data(), 16);
         p.is_v6 = 1;
         rt.prefix[u] = 0; rt.plen[u] = k[16];
+    }
+
+    using Area = hl_ospfv3_area;
+    using Rib = hl_ospfv3_rib;
+    using Route = hl_rib_route6;
+    using Hop = hl_nexthop6;
+    using Result = hl_ospfv3_result;
+    using Net = hl_route_net6;
+    using Nh = Nh6;
+    using JobDecode = ::JobDecode;
+    static constexpr auto intra_from_cells = ::intra_from_cells;
+    static constexpr auto nh_less = ::nh_less;
+    static constexpr auto nh_same = ::nh_same;
+    static constexpr auto nh_conflict = ::nh_conflict;
+    static void route_prefix(Route &o, const hspf::RibDecode<RibV3> &d, uint32_t u) {
+        o.prefix = d.prefix6[u]; o.len = (uint8_t)d.plen[u];
+    }
+    static void from_intra(Route &o, const Net &r) { o.prefix_options = r.prefix_options; }
+    static void from_record(Route &o, const hspf_ospfv2_ribtable &rt, uint32_t rec) { o.prefix_options = rt.options6[rec - rt.n_intra]; }
+    static Nh to_nh(const Hop &h, uint32_t sort) { return Nh{sort, h.iface, h.nbr_router_id, h.addr, h.has_addr, h.has_nbr}; }
+    static Hop to_hop(const Nh &x) {
+        Hop h{};
+        h.iface = x.sort; h.nbr_router_id = x.has_nbr ? x.nbr : 0;
+        if (x.has_addr) h.addr = x.addr;
+        h.has_addr = x.has_addr; h.has_nbr = x.has_nbr;
+        return h;
     }
 };
 
@@ -809,87 +838,7 @@ int hspf_ospfv3_rib_from_cells(const hl_ospfv3_area *a, const hspf_ospfv2_ribtab
     if (!a || !rt || !rt->v3 || !rt->intra || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
     try {
         out->n_routes = out->n_nexthops = 0;
-        JobDecode jd;
-        int rc = jd.init(a, (uint32_t)rt->vflags.size(), gather_v, gather_nh, n_gather);
-        if (rc) return rc;
-        if (jd.root == kNone) return HSPF_E_INVAL;                  // not the root of any job over this table
-        const uint32_t P = (uint32_t)rt->prefix6.size(), PI = (uint32_t)rt->intra->t.prefix6.size();
-        const uint32_t *o3 = rt->off.data() + P + 1, *o5 = o3 + P + 1;
-        // 1. the intra-area cells, through the intra-area decode
-        std::vector<hl_route_cell> ic(PI, hl_route_cell{0, 0, kNone, 0, 0, 0});
-        for (uint32_t u = 0; u < P; ++u) {
-            const hl_ospf_rib_cell &c = cells[u];
-            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(c) != HL_PATH_INTRA_AREA) continue;
-            if (rt->intra_of[u] == kNone || HL_RIB_CELL_METRIC(c) > 0xFFFFu) return HSPF_E_INVAL;
-            ic[rt->intra_of[u]] = hl_route_cell{c.nh_mask, c.aux, c.winner, (uint16_t)HL_RIB_CELL_METRIC(c),
-                                                (uint8_t)HL_RIB_CELL_FLAGS(c), 0};
-        }
-        std::vector<hl_route_net6> nets(PI);
-        std::vector<hl_nexthop6> nh(std::max<size_t>(64, (size_t)PI * 2));
-        hl_ospfv3_result res{};
-        for (int attempt = 0; attempt < 2; ++attempt) {
-            res = hl_ospfv3_result{};
-            res.routes_cap = PI; res.routes = nets.data();
-            res.nexthops_cap = (uint32_t)nh.size(); res.nexthops = nh.data();
-            rc = intra_from_cells(jd, a, rt->intra, ic.data(), &res);
-            if (rc != HSPF_E_NOMEM) break;
-            nh.resize(res.n_nexthops);
-        }
-        if (rc) return rc;
-        // 2. every route in prefix order; inter-area and external next hops from the cell's atoms
-        std::vector<hl_rib_route6> routes;
-        std::vector<hl_nexthop6> hops;
-        std::vector<Nh6> set;
-        auto sort_key = [&](uint32_t iface) { return iface < a->n_ifaces ? a->ifaces[iface].sort_key : 0xFFFFFFFFu; };
-        uint32_t ri = 0;
-        for (uint32_t u = 0; u < P; ++u) {
-            const hl_ospf_rib_cell &c = cells[u];
-            if (!(HL_RIB_CELL_FLAGS(c) & HL_CELL_PRESENT)) continue;
-            const uint32_t path = HL_RIB_CELL_PATH(c);
-            hl_rib_route6 o;
-            std::memset(&o, 0, sizeof(o));
-            o.prefix = rt->prefix6[u]; o.len = (uint8_t)rt->plen[u];
-            o.path_type = (uint8_t)path;
-            o.nh_off = (uint32_t)hops.size();
-            if (path == HL_PATH_INTRA_AREA) {
-                if (ri >= res.n_routes) return HSPF_E_INVAL;
-                const hl_route_net6 &r = nets[ri++];
-                o.metric = r.metric; o.area_id = rt->area_id; o.has_area = 1; o.flags = r.flags;
-                o.prefix_options = r.prefix_options;
-                for (uint32_t k = 0; k < r.n_nh; ++k) {
-                    hl_nexthop6 h = nh[r.nh_off + k];
-                    h.iface = sort_key(h.iface);                      // the merged table names interfaces by sort key
-                    hops.push_back(h);
-                }
-            } else {
-                const bool inter = path == HL_PATH_INTER_AREA;
-                if (inter ? (c.winner < o3[u] || c.winner >= o3[u + 1]) : (c.winner < o5[u] || c.winner >= o5[u + 1]))
-                    return HSPF_E_INVAL;
-                o.metric = HL_RIB_CELL_METRIC(c);
-                o.prefix_options = rt->options6[c.winner - rt->n_intra];
-                if (inter) { o.area_id = rt->area_id; o.has_area = 1; }
-                else o.tag = rt->ext_tag[c.winner - rt->ext_base];
-                if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
-                if (!atom_hops(*jd.rs, c.nh_mask, set)) return HSPF_E_UNSUPPORTED;
-                if (set.size() > a->max_paths) set.resize(a->max_paths);
-                for (const Nh6 &x : set) {
-                    hl_nexthop6 h{};
-                    h.iface = sort_key(x.iface); h.nbr_router_id = x.has_nbr ? x.nbr : 0;
-                    if (x.has_addr) h.addr = x.addr;
-                    h.has_addr = x.has_addr; h.has_nbr = x.has_nbr;
-                    hops.push_back(h);
-                }
-            }
-            o.n_nh = (uint32_t)hops.size() - o.nh_off;
-            routes.push_back(o);
-        }
-        out->n_routes = (uint32_t)routes.size();
-        out->n_nexthops = (uint32_t)hops.size();
-        if (out->n_routes > out->routes_cap || out->n_nexthops > out->nexthops_cap) return HSPF_E_NOMEM;
-        if ((out->n_routes && !out->routes) || (out->n_nexthops && !out->nexthops)) return HSPF_E_INVAL;
-        std::copy(routes.begin(), routes.end(), out->routes);
-        std::copy(hops.begin(), hops.end(), out->nexthops);
-        return HSPF_OK;
+        return hspf::decode_one_area_rib<RibV3>(a, *rt, cells, gather_v, gather_nh, n_gather, out);
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
 }
 

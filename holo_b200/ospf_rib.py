@@ -394,18 +394,13 @@ def rib_delta_device(ctx: capi.Context, rt: RibTable, n_jobs: int, rs, roots_ptr
                            n_records_ptr or None)
 
 
-def _call_rib_from_cells(fn, area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh, route_dt, nh_dt) -> Rib:
-    cells = np.ascontiguousarray(cells, RIB_CELL_DT)
-    assert cells.shape == (rt.n_prefixes,)
-    gv = np.ascontiguousarray(gather_v, np.uint32)
-    gn = np.ascontiguousarray(gather_nh, np.uint64)
-    s = area.as_struct()
-    caps = [max(rt.n_prefixes, 1), max(4 * rt.n_prefixes, 64)]
+def _call_rib(fn, args, n_prefixes: int, route_dt, nh_dt) -> Rib:
+    """fn(*args, &rib), the buffers grown once to the counts an HSPF_E_NOMEM reports."""
+    caps = [max(n_prefixes, 1), max(4 * n_prefixes, 64)]
     for _ in range(2):
         routes, nhs = np.zeros(caps[0], route_dt), np.zeros(caps[1], nh_dt)
         r = RibStruct(caps[0], 0, routes.ctypes.data, caps[1], 0, nhs.ctypes.data)
-        rc = fn(C.byref(s), rt.handle, cells.ctypes.data, gv.ctypes.data_as(C.POINTER(C.c_uint32)),
-                gn.ctypes.data_as(C.POINTER(C.c_uint64)), len(gv), C.byref(r))
+        rc = fn(*args, C.byref(r))
         if rc == capi.HSPF_E_NOMEM:
             caps = [max(caps[0], r.n_routes), max(caps[1], r.n_nexthops)]
             continue
@@ -415,6 +410,16 @@ def _call_rib_from_cells(fn, area, rt: RibTable, cells: np.ndarray, gather_v, ga
     if rc != capi.HSPF_OK:
         return Rib(np.zeros(0, route_dt), np.zeros(0, nh_dt), rc)
     return Rib(routes[: r.n_routes].copy(), nhs[: r.n_nexthops].copy(), rc)
+
+
+def _call_rib_from_cells(fn, area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh, route_dt, nh_dt) -> Rib:
+    cells = np.ascontiguousarray(cells, RIB_CELL_DT)
+    assert cells.shape == (rt.n_prefixes,)
+    gv = np.ascontiguousarray(gather_v, np.uint32)
+    gn = np.ascontiguousarray(gather_nh, np.uint64)
+    s = area.as_struct()
+    return _call_rib(fn, (C.byref(s), rt.handle, cells.ctypes.data, gv.ctypes.data_as(C.POINTER(C.c_uint32)),
+                          gn.ctypes.data_as(C.POINTER(C.c_uint64)), len(gv)), rt.n_prefixes, route_dt, nh_dt)
 
 
 def rib_from_cells(area: ospfv2.Ospfv2Area, rt: RibTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
@@ -515,19 +520,6 @@ def abr_rib_from_cells(areas: list, rt: AbrRibTable, cells: np.ndarray, gather_a
     gn = np.ascontiguousarray(gather_nh, np.uint64)
     structs = [a.as_struct() for a in areas]
     arr = (ospfv2.AreaStruct * max(len(areas), 1))(*structs)
-    fn = capi.load_library().hspf_ospfv2_abr_rib_from_cells
-    caps = [max(rt.n_prefixes, 1), max(4 * rt.n_prefixes, 64)]
-    for _ in range(2):
-        routes, nhs = np.zeros(caps[0], RIB_ROUTE_DT), np.zeros(caps[1], ospfv2.NEXTHOP_DT)
-        r = RibStruct(caps[0], 0, routes.ctypes.data, caps[1], 0, nhs.ctypes.data)
-        rc = fn(rt.handle, arr, len(areas), cells.ctypes.data, ga.ctypes.data, gv.ctypes.data, gn.ctypes.data, len(gv),
-                C.byref(r))
-        if rc == capi.HSPF_E_NOMEM:
-            caps = [max(caps[0], r.n_routes), max(caps[1], r.n_nexthops)]
-            continue
-        break
-    if rc not in (capi.HSPF_OK, capi.HSPF_E_UNSUPPORTED):
-        raise capi.HspfError(rc, "hspf_ospfv2_abr_rib_from_cells failed")
-    if rc != capi.HSPF_OK:
-        return Rib(np.zeros(0, RIB_ROUTE_DT), np.zeros(0, ospfv2.NEXTHOP_DT), rc)
-    return Rib(routes[: r.n_routes].copy(), nhs[: r.n_nexthops].copy(), rc)
+    return _call_rib(capi.load_library().hspf_ospfv2_abr_rib_from_cells,
+                     (rt.handle, arr, len(areas), cells.ctypes.data, ga.ctypes.data, gv.ctypes.data, gn.ctypes.data,
+                      len(gv)), rt.n_prefixes, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)
