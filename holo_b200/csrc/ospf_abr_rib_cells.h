@@ -207,6 +207,12 @@ struct hspf_ospfv2_abr_ribtable {
     std::vector<hspf::RibRec> recs;
     std::vector<uint32_t> v_flagged, vl_off;
     std::vector<uint32_t> ext_tag;                 // per type-5 record (index - ext_base)
+    // OSPFv3 tables (hspf_ospfv3_abr_ribtable_create): each area's table is an OSPFv3 one-area table, `prefix` is
+    // zero-filled (the prefixes are prefix6), and options6 holds the prefix options per type-3 / type-5 record
+    // (index - t3_base[0], the first type-3 record)
+    bool v3 = false;
+    std::vector<hl_ip_addr> prefix6;
+    std::vector<uint8_t> options6;
     hspf::DeviceRouteTable dev;                    // off, then records + v_flagged
     hspf::AbrRibView view(const uint32_t *o, const hspf::RibRec *r, const uint32_t *vf) const {
         hspf::AbrRibView t{};

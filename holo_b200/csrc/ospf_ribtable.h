@@ -4,9 +4,11 @@
 //                      (include/holo_spf_lsdb.h).  The versions differ only in the prefix key, in which field of an
 //                      inter-area-router LSA names the ASBR, and in the NU-bit LSAs OSPFv3 skips; the records the walk
 //                      reads (ospf_rib_cells.h) are the same.
+//   build_abr_ribtable hspf_ospfv2_abr_ribtable_create / hspf_ospfv3_abr_ribtable_create: an area border router's
+//                      records over the one-area tables of its areas (ospf_abr_rib_cells.h)
 //   decode_rib         one job's cells -> its routing table, for hspf_ospfv2_rib_from_cells,
-//                      hspf_ospfv3_rib_from_cells and hspf_ospfv2_abr_rib_from_cells.  A one-area table decodes as an
-//                      area border router's table with a single area.
+//                      hspf_ospfv3_rib_from_cells and hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib).  A
+//                      one-area table decodes as an area border router's table with a single area.
 //
 // For build_rib_records a version trait T provides:
 //   Key                        prefix key; its order is the table's prefix order (update_rib_full's IpNetwork order)
@@ -16,8 +18,16 @@
 //   skip(Sum), skip(Ext)       LSAs update_rib_full never uses whatever the job (OSPFv3: NU bit)
 //   asbr_id(Sum)               the ASBR a type-4 LSA names
 //   options(Sum), options(Ext) prefix options a route through the LSA carries
-//   set_prefix(rt, u, Key)     writes prefix u of the table
+//   set_prefix(rt, u, Key)     writes prefix u of the table (a one-area or an ABR table)
 //   kV3                        the table carries OSPFv3 prefixes and per-record prefix options
+//
+// For build_abr_ribtable it also provides:
+//   Flat                       the version's flattened area; its `area` is the area's image
+//   root_vertex(f, id)         the router vertex of router `id` in f, or 0xFFFFFFFF
+//   n_vertices(f)              f's vertex count
+//   atom_count(f, root, &n)    hspf_atom_count over f's CSR
+//   area_table(f, id, sums, n_sums, ext, n_ext, &rt)  the area's one-area table, built with the transit-area walk
+//   table_key(rt, u)           the key of prefix u of a one-area table
 //
 // For decode_rib it also provides:
 //   Area, Rib                  the area image and the caller's output
@@ -30,17 +40,20 @@
 //   nh_conflict(a, b)          a and b have one key, but attributes the cell cannot choose between
 //   route_prefix(o, d, u)      writes prefix u of the decode into the route (v2 prefix / mask, v3 prefix6 / len)
 //   from_intra(o, net)         what a route takes from its intra-area route (v2 SR label, v3 prefix options)
-//   from_record(o, rt, rec)    what it takes from type-3 / type-5 record `rec` of one-area table rt (v3 prefix options)
+//   from_record(o, d, rec)     what it takes from type-3 / type-5 record `rec` of the decoded table (v3: d.options)
 //   to_nh(hop, sort), to_hop   a next hop into the merged set, naming its interface's sort key, and back out
 #pragma once
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <memory>
+#include <new>
 #include <numeric>
 #include <unordered_map>
 #include <vector>
 
 #include "holo_spf_lsdb.h"
+#include "ospf_abr_rib_cells.h"
 #include "ospf_rib_cells.h"
 
 namespace hspf {
@@ -162,6 +175,165 @@ int build_rib_records(hspf_ospfv2_ribtable &rt, uint32_t area_id, RouterVertex r
     return HSPF_OK;
 }
 
+// hspf_ospfv2_abr_ribtable_create / hspf_ospfv3_abr_ribtable_create, argument checks included: each area's one-area
+// table with the transit-area walk, then the router's records over all of them (ospf_abr_rib_cells.h).
+template <class T>
+int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::Flat *const *flats,
+                       const uint32_t *area_ids, const typename T::Sum *const *summaries, const uint32_t *n_summaries,
+                       const uint8_t *active, const typename T::Ext *ext, uint32_t n_ext,
+                       hspf_ospfv2_abr_ribtable **out) {
+    using Key = typename T::Key;
+    if (!out || !flats || !area_ids || n_areas == 0 || (n_ext && !ext)) return HSPF_E_INVAL;
+    *out = nullptr;
+    if (n_areas > kAbrMaxAreas) return HSPF_E_UNSUPPORTED;
+    for (uint32_t i = 0; i < n_areas; ++i) {
+        if (!flats[i] || !flats[i]->area) return HSPF_E_INVAL;
+        if (n_summaries && n_summaries[i] && (!summaries || !summaries[i])) return HSPF_E_INVAL;
+    }
+    try {
+        std::unique_ptr<hspf_ospfv2_abr_ribtable, void (*)(hspf_ospfv2_abr_ribtable *)> t(
+            new hspf_ospfv2_abr_ribtable(), hspf_ospfv2_abr_ribtable_free);
+        const uint32_t A = n_areas;
+        t->router_id = router_id;
+        t->n_areas = A;
+        t->v3 = T::kV3;
+        uint32_t n_active = 0;
+        for (uint32_t i = 0; i < A; ++i) n_active += (!active || active[i]) ? 1u : 0u;
+        uint32_t atoms = 0;
+        for (uint32_t i = 0; i < A; ++i) {
+            const typename T::Flat &f = *flats[i];
+            if (i == 0) t->max_paths = f.area->max_paths;
+            else if (f.area->max_paths != t->max_paths) return HSPF_E_INVAL;   // one instance, one max_paths
+            const uint32_t root = T::root_vertex(f, router_id);
+            if (root == kNoRecord) return HSPF_E_INVAL;                        // the caller leaves that area out
+            uint32_t na = 0;
+            int rc = T::atom_count(f, root, &na);
+            if (rc) return rc;
+            t->base.push_back(na ? atoms : 0);
+            t->n_atoms.push_back(na);
+            atoms += na;
+            if (atoms > 64) return HSPF_E_UNSUPPORTED;                         // the cell's masks are 64 bits
+            // rib_full step 2 reads every area's summaries with one active area, else only the backbone's; the
+            // other areas' type-3 LSAs are still offered by the transit-area step
+            const bool step2 = n_active <= 1 || area_ids[i] == 0;
+            if (step2) t->step2 |= 1u << i;
+            const uint32_t ns = n_summaries ? n_summaries[i] : 0;
+            std::vector<typename T::Sum> sums;
+            for (uint32_t k = 0; k < ns; ++k)
+                if (step2 || summaries[i][k].lsa_type == 3) sums.push_back(summaries[i][k]);
+            hspf_ospfv2_ribtable *rt = nullptr;
+            rc = T::area_table(flats[i], area_ids[i], sums.data(), (uint32_t)sums.size(), ext, n_ext, &rt);
+            if (rc) return rc;
+            t->area.push_back(rt);
+            t->area_id.push_back(area_ids[i]);
+            t->root.push_back(root);
+            t->n_vertices.push_back(T::n_vertices(f));
+        }
+        // the prefixes: the union of the areas' in prefix order
+        std::vector<Key> keys;
+        for (const hspf_ospfv2_ribtable *rt : t->area)
+            for (uint32_t u = 0; u < (uint32_t)rt->plen.size(); ++u) keys.push_back(T::table_key(*rt, u));
+        std::sort(keys.begin(), keys.end());
+        keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
+        const uint32_t P = (uint32_t)keys.size(), S = P + 1;
+        t->prefix.resize(P); t->plen.resize(P);
+        if (T::kV3) t->prefix6.resize(P);
+        for (uint32_t u = 0; u < P; ++u) T::set_prefix(*t, u, keys[u]);
+        t->area_prefix.assign(A, std::vector<uint32_t>(P, kNoRecord));
+        std::vector<std::vector<uint32_t>> first_at(A, std::vector<uint32_t>(P));   // first area prefix >= keys[u]
+        for (uint32_t i = 0; i < A; ++i) {
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            uint32_t q = 0;
+            for (uint32_t u = 0; u < P; ++u) {
+                first_at[i][u] = q;
+                if (q < rt.plen.size() && T::table_key(rt, q) == keys[u]) t->area_prefix[i][u] = q++;
+            }
+        }
+        t->off.assign((2 * (size_t)A + 1) * S, 0);
+        uint32_t *o3 = t->off.data() + (size_t)A * S, *o5 = o3 + (size_t)A * S;
+        auto &recs = t->recs;
+        for (uint32_t i = 0; i < A; ++i) {                                  // intra-area records, area by area
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            const uint32_t b = (uint32_t)recs.size();
+            t->intra_base.push_back(b);
+            recs.insert(recs.end(), rt.recs.begin(), rt.recs.begin() + rt.n_intra);
+            for (uint32_t u = 0; u < P; ++u) t->off[i * S + u] = b + rt.off[first_at[i][u]];
+            t->off[i * S + P] = b + rt.n_intra;
+        }
+        for (uint32_t i = 0; i < A; ++i) {                                  // type-3, without the root's own
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            const uint32_t *a3 = rt.off.data() + rt.plen.size() + 1;
+            t->t3_base.push_back((uint32_t)recs.size());
+            for (uint32_t u = 0; u < P; ++u) {
+                o3[i * S + u] = (uint32_t)recs.size();
+                const uint32_t q = t->area_prefix[i][u];
+                if (q == kNoRecord) continue;
+                for (uint32_t k = a3[q]; k < a3[q + 1]; ++k)
+                    if (rt.recs[k].x != t->root[i]) {
+                        recs.push_back(rt.recs[k]);
+                        if (T::kV3) t->options6.push_back(rt.options6[k - rt.n_intra]);
+                    }
+            }
+            o3[i * S + P] = (uint32_t)recs.size();
+        }
+        t->t3_end = (uint32_t)recs.size();
+        // type-5: every area's table holds the same type-5 records in the same order (one external list, one filter);
+        // area 0's slot of a record names its ASBR, and each area's slot of that record gives that area's entry
+        const hspf_ospfv2_ribtable &r0 = *t->area[0];
+        const uint32_t N5 = r0.ext_end - r0.ext_base;
+        for (const hspf_ospfv2_ribtable *rt : t->area)
+            if (rt->ext_end - rt->ext_base != N5) return HSPF_E_INVAL;
+        std::unordered_map<uint32_t, uint32_t> group_of;                    // area 0's slot record -> group
+        std::vector<uint32_t> group_rep, rec_group;                         // a type-5 record of each group; group per record
+        t->ext_base = (uint32_t)recs.size();
+        const uint32_t *a5 = r0.off.data() + 2 * (r0.plen.size() + 1);
+        for (uint32_t u = 0; u < P; ++u) {
+            o5[u] = (uint32_t)recs.size();
+            const uint32_t q = t->area_prefix[0][u];
+            if (q == kNoRecord) continue;
+            for (uint32_t k = a5[q]; k < a5[q + 1]; ++k) {
+                const RibRec r = r0.recs[k];
+                if (r0.recs[r.x].x == t->root[0]) continue;                 // self-originated
+                auto ins = group_of.emplace(r.x, (uint32_t)group_rep.size());
+                if (ins.second) group_rep.push_back(k - r0.ext_base);
+                rec_group.push_back(ins.first->second);
+                recs.push_back(RibRec{0, r.y, r.z, 0});
+                t->ext_tag.push_back(r0.ext_tag[k - r0.ext_base]);
+                if (T::kV3) t->options6.push_back(r0.options6[k - r0.n_intra]);
+            }
+        }
+        o5[P] = (uint32_t)recs.size();
+        t->ext_end = o5[P];
+        const uint32_t group_base = (uint32_t)recs.size(), G = (uint32_t)group_rep.size();
+        for (uint32_t k = 0; k < rec_group.size(); ++k) recs[t->ext_base + k].x = group_base + rec_group[k] * A;
+        recs.resize((size_t)group_base + (size_t)G * A);
+        for (uint32_t g = 0; g < G; ++g)
+            for (uint32_t i = 0; i < A; ++i) {
+                const hspf_ospfv2_ribtable &rt = *t->area[i];
+                const RibRec s = rt.recs[rt.recs[rt.ext_base + group_rep[g]].x];
+                const uint32_t z = (uint32_t)recs.size();
+                if ((t->step2 >> i) & 1u)
+                    for (uint32_t k = s.z; k < s.w; ++k)
+                        if (rt.recs[k].x != t->root[i]) recs.push_back(rt.recs[k]);
+                recs[group_base + g * A + i] = RibRec{s.x, s.y, z, (uint32_t)recs.size()};
+            }
+        if (recs.size() >= kNoRecord) return HSPF_E_UNSUPPORTED;           // record indices are u32
+        t->vl_off.push_back(0);
+        for (uint32_t i = 0; i < A; ++i) {
+            const hspf_ospfv2_ribtable &rt = *t->area[i];
+            for (uint32_t v = 0; v < rt.vflags.size(); ++v)
+                if (rt.vflags[v] & HL_RTR_FLAG_V) t->v_flagged.push_back(v);
+            t->vl_off.push_back((uint32_t)t->v_flagged.size());
+        }
+        *out = t.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_UNSUPPORTED;
+    }
+}
+
 // One area of a decode: record and prefix indices are the decoded table's unless said otherwise.
 template <class T>
 struct RibDecodeArea {
@@ -187,6 +359,8 @@ struct RibDecode {
     const uint32_t *ext_tag;             // per type-5 record (index - ext_base): the LSA's tag
     uint32_t ext_base;
     uint32_t max_paths;
+    const uint8_t *options;              // OSPFv3: per type-3 / type-5 record (index - options_base), its prefix options
+    uint32_t options_base;
 };
 
 // One job's cells -> its routing table, in prefix order, into `out` (HSPF_E_NOMEM with the counts when it does not
@@ -297,7 +471,7 @@ int decode_rib(const RibDecode<T> &d, const hl_ospf_rib_cell *cells, typename T:
                 o.tag = d.ext_tag[c.winner - d.ext_base];
                 if (path == HL_PATH_TYPE2_EXTERNAL) { o.has_type2 = 1; o.type2_metric = (uint32_t)c.aux; }
             }
-            T::from_record(o, *d.area[0].rt, c.winner);            // only OSPFv3 reads it, whose tables have one area
+            T::from_record(o, d, c.winner);
         }
         const int rc = add_atoms(rest);
         if (rc) return rc;
@@ -331,8 +505,50 @@ int decode_one_area_rib(const typename T::Area *a, const hspf_ospfv2_ribtable &r
     std::iota(same.begin(), same.end(), 0u);
     RibDecode<T> d{{RibDecodeArea<T>{a, &rt, same.data(), 0, ~0ull, o3, 0, ~0ull, rt.area_id, &jd}},
                    P, rt.prefix.data(), rt.plen.data(), rt.prefix6.data(), o3 + P + 1, rt.ext_tag.data(), rt.ext_base,
-                   a->max_paths};
+                   a->max_paths, rt.options6.data(), rt.n_intra};
     return decode_rib(d, cells, out);
+}
+
+// hspf_ospfv2_abr_rib_from_cells / hspf_ospfv3_abr_rib_from_cells, argument checks included: each area's job
+// decode over its own gathers, and the decode of the router's table over them.  A table of the other version is
+// refused (HSPF_E_INVAL).
+template <class T>
+int decode_abr_rib(const hspf_ospfv2_abr_ribtable *t, const typename T::Area *areas, uint32_t n_areas,
+                   const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
+                   const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out) {
+    if (!t || t->v3 != T::kV3 || !areas || !cells || !out || n_areas != t->n_areas ||
+        (n_gather && (!gather_area || !gather_v || !gather_nh)))
+        return HSPF_E_INVAL;
+    try {
+        out->n_routes = out->n_nexthops = 0;
+        const uint32_t A = n_areas, P = (uint32_t)t->plen.size(), S = P + 1;
+        std::vector<typename T::JobDecode> jd(A);
+        RibDecode<T> d{{}, P, t->prefix.data(), t->plen.data(), t->prefix6.data(), t->off.data() + 2 * (size_t)A * S,
+                       t->ext_tag.data(), t->ext_base, t->max_paths, t->options6.data(), t->t3_base[0]};
+        for (uint32_t i = 0; i < A; ++i) {
+            const typename T::Area &a = areas[i];
+            if (a.router_id != t->router_id || a.area_id != t->area_id[i] || a.max_paths != t->max_paths) return HSPF_E_INVAL;
+            std::vector<uint32_t> gv;
+            std::vector<uint64_t> gn;
+            for (uint32_t g = 0; g < n_gather; ++g) {
+                if (gather_area[g] >= A) return HSPF_E_INVAL;
+                if (gather_area[g] == i) { gv.push_back(gather_v[g]); gn.push_back(gather_nh[g]); }
+            }
+            const int rc = jd[i].init(&a, t->n_vertices[i], gv.data(), gn.data(), (uint32_t)gv.size());
+            if (rc) return rc;
+            if (jd[i].root != t->root[i]) return HSPF_E_INVAL;
+            const uint32_t na = t->n_atoms[i];
+            const uint64_t mask = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << t->base[i]);
+            d.area.push_back({&a, t->area[i], t->area_prefix[i].data(), t->intra_base[i],
+                              (uint64_t)t->intra_base[i] + t->area[i]->n_intra, t->off.data() + (A + i) * (size_t)S,
+                              t->base[i], mask, t->area_id[i], &jd[i]});
+        }
+        return decode_rib(d, cells, out);
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
 }
 
 }  // namespace hspf

@@ -1055,7 +1055,10 @@ void hspf_ospfv2_ribtable_free(hspf_ospfv2_ribtable *rt) {
 
 namespace {
 
-// the OSPFv2 side of hspf::build_rib_records and hspf::decode_rib (ospf_ribtable.h)
+int make_ribtable(const hspf_ospfv2_flat *flat, uint32_t area_id, const hl_ospfv2_summary_lsa *sums, uint32_t n_sums,
+                  const hl_ospfv2_external_lsa *ext, uint32_t n_ext, bool transit_walk, hspf_ospfv2_ribtable **out);
+
+// the OSPFv2 side of hspf::build_rib_records, hspf::build_abr_ribtable and hspf::decode_rib (ospf_ribtable.h)
 struct RibV2 {
     using Key = uint64_t;
     using Sum = hl_ospfv2_summary_lsa;
@@ -1069,7 +1072,25 @@ struct RibV2 {
     static uint32_t asbr_id(const Sum &l) { return l.lsa_id; }
     static uint8_t options(const Sum &) { return 0; }
     static uint8_t options(const Ext &) { return 0; }
-    static void set_prefix(hspf_ospfv2_ribtable &rt, uint32_t u, Key k) { rt.prefix[u] = (uint32_t)(k >> 8); rt.plen[u] = (uint32_t)(k & 0xFF); }
+    template <class Table>
+    static void set_prefix(Table &rt, uint32_t u, Key k) { rt.prefix[u] = (uint32_t)(k >> 8); rt.plen[u] = (uint32_t)(k & 0xFF); }
+
+    using Flat = hspf_ospfv2_flat;
+    static uint32_t root_vertex(const Flat &f, uint32_t id) {
+        auto it = f.rtr_vertex.find(id);
+        return it == f.rtr_vertex.end() ? kNone : it->second;
+    }
+    static uint32_t n_vertices(const Flat &f) { return (uint32_t)f.ids.size(); }
+    static int atom_count(const Flat &f, uint32_t root, uint32_t *n) {
+        hspf_csr c;
+        fill_csr(f, &c);
+        return hspf_atom_count(&c, root, n);
+    }
+    static int area_table(const Flat *f, uint32_t area_id, const Sum *sums, uint32_t n_sums, const Ext *ext,
+                          uint32_t n_ext, hspf_ospfv2_ribtable **out) {
+        return make_ribtable(f, area_id, sums, n_sums, ext, n_ext, true, out);
+    }
+    static Key table_key(const hspf_ospfv2_ribtable &rt, uint32_t u) { return pkey(rt.prefix[u], rt.plen[u]); }
 
     using Area = hl_ospfv2_area;
     using Rib = hl_ospfv2_rib;
@@ -1087,7 +1108,7 @@ struct RibV2 {
         o.prefix = d.prefix[u]; o.mask = d.plen[u] == 0 ? 0 : 0xFFFFFFFFu << (32 - d.plen[u]);
     }
     static void from_intra(Route &o, const Net &r) { o.has_sr_label = r.has_sr_label; o.sr_label = r.has_sr_label ? r.sr_label : 0; }
-    static void from_record(Route &, const hspf_ospfv2_ribtable &, uint32_t) {}
+    static void from_record(Route &, const hspf::RibDecode<RibV2> &, uint32_t) {}
     static Nh to_nh(const Hop &h, uint32_t sort) {
         return Nh{sort, h.iface, h.addr, h.nbr_router_id, h.sr_label, h.has_addr, h.has_nbr, h.has_label};
     }
@@ -1181,152 +1202,8 @@ int hspf_ospfv2_abr_ribtable_create(uint32_t router_id, uint32_t n_areas, const 
                                     const uint32_t *area_ids, const hl_ospfv2_summary_lsa *const *summaries,
                                     const uint32_t *n_summaries, const uint8_t *active,
                                     const hl_ospfv2_external_lsa *ext, uint32_t n_ext, hspf_ospfv2_abr_ribtable **out) {
-    if (!out || !flats || !area_ids || n_areas == 0 || (n_ext && !ext)) return HSPF_E_INVAL;
-    *out = nullptr;
-    if (n_areas > hspf::kAbrMaxAreas) return HSPF_E_UNSUPPORTED;
-    for (uint32_t i = 0; i < n_areas; ++i) {
-        if (!flats[i] || !flats[i]->area) return HSPF_E_INVAL;
-        if (n_summaries && n_summaries[i] && (!summaries || !summaries[i])) return HSPF_E_INVAL;
-    }
-    try {
-        std::unique_ptr<hspf_ospfv2_abr_ribtable, void (*)(hspf_ospfv2_abr_ribtable *)> t(
-            new hspf_ospfv2_abr_ribtable(), hspf_ospfv2_abr_ribtable_free);
-        const uint32_t A = n_areas;
-        t->router_id = router_id;
-        t->n_areas = A;
-        uint32_t n_active = 0;
-        for (uint32_t i = 0; i < A; ++i) n_active += (!active || active[i]) ? 1u : 0u;
-        uint32_t atoms = 0;
-        for (uint32_t i = 0; i < A; ++i) {
-            const hspf_ospfv2_flat &f = *flats[i];
-            if (i == 0) t->max_paths = f.area->max_paths;
-            else if (f.area->max_paths != t->max_paths) return HSPF_E_INVAL;   // one instance, one max_paths
-            auto rit = f.rtr_vertex.find(router_id);
-            if (rit == f.rtr_vertex.end()) return HSPF_E_INVAL;                // the caller leaves that area out
-            const uint32_t root = rit->second;
-            hspf_csr c;
-            fill_csr(f, &c);
-            uint32_t na = 0;
-            int rc = hspf_atom_count(&c, root, &na);
-            if (rc) return rc;
-            t->base.push_back(na ? atoms : 0);
-            t->n_atoms.push_back(na);
-            atoms += na;
-            if (atoms > 64) return HSPF_E_UNSUPPORTED;                         // the cell's masks are 64 bits
-            // rib_full step 2 reads every area's summaries with one active area, else only the backbone's; the
-            // other areas' type-3 LSAs are still offered by the transit-area step
-            const bool step2 = n_active <= 1 || area_ids[i] == 0;
-            if (step2) t->step2 |= 1u << i;
-            const uint32_t ns = n_summaries ? n_summaries[i] : 0;
-            std::vector<hl_ospfv2_summary_lsa> sums;
-            for (uint32_t k = 0; k < ns; ++k)
-                if (step2 || summaries[i][k].lsa_type == 3) sums.push_back(summaries[i][k]);
-            hspf_ospfv2_ribtable *rt = nullptr;
-            rc = make_ribtable(flats[i], area_ids[i], sums.data(), (uint32_t)sums.size(), ext, n_ext, true, &rt);
-            if (rc) return rc;
-            t->area.push_back(rt);
-            t->area_id.push_back(area_ids[i]);
-            t->root.push_back(root);
-            t->n_vertices.push_back((uint32_t)f.ids.size());
-        }
-        // the prefixes: the union of the areas' in prefix order
-        std::vector<uint64_t> keys;
-        for (const hspf_ospfv2_ribtable *rt : t->area)
-            for (size_t u = 0; u < rt->prefix.size(); ++u) keys.push_back(pkey(rt->prefix[u], rt->plen[u]));
-        std::sort(keys.begin(), keys.end());
-        keys.erase(std::unique(keys.begin(), keys.end()), keys.end());
-        const uint32_t P = (uint32_t)keys.size(), S = P + 1;
-        t->prefix.resize(P); t->plen.resize(P);
-        for (uint32_t u = 0; u < P; ++u) { t->prefix[u] = (uint32_t)(keys[u] >> 8); t->plen[u] = (uint32_t)(keys[u] & 0xFF); }
-        t->area_prefix.assign(A, std::vector<uint32_t>(P, kNone));
-        std::vector<std::vector<uint32_t>> first_at(A, std::vector<uint32_t>(P));   // first area prefix >= keys[u]
-        for (uint32_t i = 0; i < A; ++i) {
-            const hspf_ospfv2_ribtable &rt = *t->area[i];
-            uint32_t q = 0;
-            for (uint32_t u = 0; u < P; ++u) {
-                first_at[i][u] = q;
-                if (q < rt.prefix.size() && pkey(rt.prefix[q], rt.plen[q]) == keys[u]) t->area_prefix[i][u] = q++;
-            }
-        }
-        t->off.assign((2 * (size_t)A + 1) * S, 0);
-        uint32_t *o3 = t->off.data() + (size_t)A * S, *o5 = o3 + (size_t)A * S;
-        auto &recs = t->recs;
-        for (uint32_t i = 0; i < A; ++i) {                                  // intra-area records, area by area
-            const hspf_ospfv2_ribtable &rt = *t->area[i];
-            const uint32_t b = (uint32_t)recs.size();
-            t->intra_base.push_back(b);
-            recs.insert(recs.end(), rt.recs.begin(), rt.recs.begin() + rt.n_intra);
-            for (uint32_t u = 0; u < P; ++u) t->off[i * S + u] = b + rt.off[first_at[i][u]];
-            t->off[i * S + P] = b + rt.n_intra;
-        }
-        for (uint32_t i = 0; i < A; ++i) {                                  // type-3, without the root's own
-            const hspf_ospfv2_ribtable &rt = *t->area[i];
-            const uint32_t *a3 = rt.off.data() + rt.prefix.size() + 1;
-            t->t3_base.push_back((uint32_t)recs.size());
-            for (uint32_t u = 0; u < P; ++u) {
-                o3[i * S + u] = (uint32_t)recs.size();
-                const uint32_t q = t->area_prefix[i][u];
-                if (q == kNone) continue;
-                for (uint32_t k = a3[q]; k < a3[q + 1]; ++k)
-                    if (rt.recs[k].x != t->root[i]) recs.push_back(rt.recs[k]);
-            }
-            o3[i * S + P] = (uint32_t)recs.size();
-        }
-        t->t3_end = (uint32_t)recs.size();
-        // type-5: every area's table holds the same type-5 records in the same order (one external list, one filter);
-        // area 0's slot of a record names its ASBR, and each area's slot of that record gives that area's entry
-        const hspf_ospfv2_ribtable &r0 = *t->area[0];
-        const uint32_t N5 = r0.ext_end - r0.ext_base;
-        for (const hspf_ospfv2_ribtable *rt : t->area)
-            if (rt->ext_end - rt->ext_base != N5) return HSPF_E_INVAL;
-        std::unordered_map<uint32_t, uint32_t> group_of;                    // area 0's slot record -> group
-        std::vector<uint32_t> group_rep, rec_group;                         // a type-5 record of each group; group per record
-        t->ext_base = (uint32_t)recs.size();
-        const uint32_t *a5 = r0.off.data() + 2 * (r0.prefix.size() + 1);
-        for (uint32_t u = 0; u < P; ++u) {
-            o5[u] = (uint32_t)recs.size();
-            const uint32_t q = t->area_prefix[0][u];
-            if (q == kNone) continue;
-            for (uint32_t k = a5[q]; k < a5[q + 1]; ++k) {
-                const hspf::RibRec r = r0.recs[k];
-                if (r0.recs[r.x].x == t->root[0]) continue;                 // self-originated
-                auto ins = group_of.emplace(r.x, (uint32_t)group_rep.size());
-                if (ins.second) group_rep.push_back(k - r0.ext_base);
-                rec_group.push_back(ins.first->second);
-                recs.push_back(hspf::RibRec{0, r.y, r.z, 0});
-                t->ext_tag.push_back(r0.ext_tag[k - r0.ext_base]);
-            }
-        }
-        o5[P] = (uint32_t)recs.size();
-        t->ext_end = o5[P];
-        const uint32_t group_base = (uint32_t)recs.size(), G = (uint32_t)group_rep.size();
-        for (uint32_t k = 0; k < rec_group.size(); ++k) recs[t->ext_base + k].x = group_base + rec_group[k] * A;
-        recs.resize((size_t)group_base + (size_t)G * A);
-        for (uint32_t g = 0; g < G; ++g)
-            for (uint32_t i = 0; i < A; ++i) {
-                const hspf_ospfv2_ribtable &rt = *t->area[i];
-                const hspf::RibRec s = rt.recs[rt.recs[rt.ext_base + group_rep[g]].x];
-                const uint32_t z = (uint32_t)recs.size();
-                if ((t->step2 >> i) & 1u)
-                    for (uint32_t k = s.z; k < s.w; ++k)
-                        if (rt.recs[k].x != t->root[i]) recs.push_back(rt.recs[k]);
-                recs[group_base + g * A + i] = hspf::RibRec{s.x, s.y, z, (uint32_t)recs.size()};
-            }
-        if (recs.size() >= kNone) return HSPF_E_UNSUPPORTED;               // record indices are u32
-        t->vl_off.push_back(0);
-        for (uint32_t i = 0; i < A; ++i) {
-            const hspf_ospfv2_ribtable &rt = *t->area[i];
-            for (uint32_t v = 0; v < rt.vflags.size(); ++v)
-                if (rt.vflags[v] & HL_RTR_FLAG_V) t->v_flagged.push_back(v);
-            t->vl_off.push_back((uint32_t)t->v_flagged.size());
-        }
-        *out = t.release();
-        return HSPF_OK;
-    } catch (const std::bad_alloc &) {
-        return HSPF_E_NOMEM;
-    } catch (...) {
-        return HSPF_E_UNSUPPORTED;
-    }
+    return hspf::build_abr_ribtable<RibV2>(router_id, n_areas, flats, area_ids, summaries, n_summaries, active, ext,
+                                           n_ext, out);
 }
 
 uint32_t hspf_ospfv2_abr_ribtable_prefixes(const hspf_ospfv2_abr_ribtable *t) { return t ? (uint32_t)t->prefix.size() : 0; }
@@ -1357,39 +1234,7 @@ int hspf_ospfv2_abr_ribtable_areas(const hspf_ospfv2_abr_ribtable *t, uint32_t *
 int hspf_ospfv2_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_ospfv2_area *areas, uint32_t n_areas,
                                    const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
                                    const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv2_rib *out) {
-    if (!t || !areas || !cells || !out || n_areas != t->n_areas ||
-        (n_gather && (!gather_area || !gather_v || !gather_nh)))
-        return HSPF_E_INVAL;
-    try {
-        out->n_routes = out->n_nexthops = 0;
-        const uint32_t A = n_areas, P = (uint32_t)t->prefix.size(), S = P + 1;
-        std::vector<JobDecode> jd(A);
-        hspf::RibDecode<RibV2> d{{}, P, t->prefix.data(), t->plen.data(), nullptr, t->off.data() + 2 * (size_t)A * S,
-                                 t->ext_tag.data(), t->ext_base, t->max_paths};
-        for (uint32_t i = 0; i < A; ++i) {
-            const hl_ospfv2_area &a = areas[i];
-            if (a.router_id != t->router_id || a.area_id != t->area_id[i] || a.max_paths != t->max_paths) return HSPF_E_INVAL;
-            std::vector<uint32_t> gv;
-            std::vector<uint64_t> gn;
-            for (uint32_t g = 0; g < n_gather; ++g) {
-                if (gather_area[g] >= A) return HSPF_E_INVAL;
-                if (gather_area[g] == i) { gv.push_back(gather_v[g]); gn.push_back(gather_nh[g]); }
-            }
-            const int rc = jd[i].init(&a, t->n_vertices[i], gv.data(), gn.data(), (uint32_t)gv.size());
-            if (rc) return rc;
-            if (jd[i].root != t->root[i]) return HSPF_E_INVAL;
-            const uint32_t na = t->n_atoms[i];
-            const uint64_t mask = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << t->base[i]);
-            d.area.push_back({&a, t->area[i], t->area_prefix[i].data(), t->intra_base[i],
-                              (uint64_t)t->intra_base[i] + t->area[i]->n_intra, t->off.data() + (A + i) * (size_t)S,
-                              t->base[i], mask, t->area_id[i], &jd[i]});
-        }
-        return hspf::decode_rib(d, cells, out);
-    } catch (const std::bad_alloc &) {
-        return HSPF_E_NOMEM;
-    } catch (...) {
-        return HSPF_E_INVAL;
-    }
+    return hspf::decode_abr_rib<RibV2>(t, areas, n_areas, cells, gather_area, gather_v, gather_nh, n_gather, out);
 }
 
 

@@ -725,7 +725,11 @@ int intra_from_cells(JobDecode &jd, const hl_ospfv3_area *a, const hspf_ospfv2_r
     return HSPF_OK;
 }
 
-// the OSPFv3 side of hspf::build_rib_records and hspf::decode_rib (ospf_ribtable.h): rib_full<V3> of ospf_rib_host.cc
+int make_ribtable(const hspf_ospfv3_flat *flat, uint32_t area_id, const hl_ospfv3_inter_area_lsa *sums, uint32_t n_sums,
+                  const hl_ospfv3_external_lsa *ext, uint32_t n_ext, bool transit_walk, hspf_ospfv2_ribtable **out);
+
+// the OSPFv3 side of hspf::build_rib_records, hspf::build_abr_ribtable and hspf::decode_rib (ospf_ribtable.h):
+// rib_full<V3> of ospf_rib_host.cc
 struct RibV3 {
     using Key = std::array<uint8_t, 17>;                  // 16 address bytes, then the length
     using Sum = hl_ospfv3_inter_area_lsa;
@@ -741,13 +745,31 @@ struct RibV3 {
     static uint8_t options(const Sum &l) { return l.prefix_options; }
     static uint8_t options(const Ext &l) { return l.prefix_options; }
     // the merged table names every prefix as an IPv6 network, as update_rib_full does
-    static void set_prefix(hspf_ospfv2_ribtable &rt, uint32_t u, const Key &k) {
+    template <class Table>
+    static void set_prefix(Table &rt, uint32_t u, const Key &k) {
         hl_ip_addr &p = rt.prefix6[u];
         std::memset(&p, 0, sizeof(p));
         std::memcpy(p.bytes, k.data(), 16);
         p.is_v6 = 1;
         rt.prefix[u] = 0; rt.plen[u] = k[16];
     }
+
+    using Flat = hspf_ospfv3_flat;
+    static uint32_t root_vertex(const Flat &f, uint32_t id) {
+        auto it = f.rtr_vertex.find(id);
+        return it == f.rtr_vertex.end() ? kNone : it->second;
+    }
+    static uint32_t n_vertices(const Flat &f) { return (uint32_t)f.rid.size(); }
+    static int atom_count(const Flat &f, uint32_t root, uint32_t *n) {
+        hspf_csr c;
+        fill_csr(f, &c);
+        return hspf_atom_count(&c, root, n);
+    }
+    static int area_table(const Flat *f, uint32_t area_id, const Sum *sums, uint32_t n_sums, const Ext *ext,
+                          uint32_t n_ext, hspf_ospfv2_ribtable **out) {
+        return make_ribtable(f, area_id, sums, n_sums, ext, n_ext, true, out);
+    }
+    static Key table_key(const hspf_ospfv2_ribtable &rt, uint32_t u) { return mk(rt.prefix6[u], (uint8_t)rt.plen[u]); }
 
     using Area = hl_ospfv3_area;
     using Rib = hl_ospfv3_rib;
@@ -765,7 +787,7 @@ struct RibV3 {
         o.prefix = d.prefix6[u]; o.len = (uint8_t)d.plen[u];
     }
     static void from_intra(Route &o, const Net &r) { o.prefix_options = r.prefix_options; }
-    static void from_record(Route &o, const hspf_ospfv2_ribtable &rt, uint32_t rec) { o.prefix_options = rt.options6[rec - rt.n_intra]; }
+    static void from_record(Route &o, const hspf::RibDecode<RibV3> &d, uint32_t rec) { o.prefix_options = d.options[rec - d.options_base]; }
     static Nh to_nh(const Hop &h, uint32_t sort) { return Nh{sort, h.iface, h.nbr_router_id, h.addr, h.has_addr, h.has_nbr}; }
     static Hop to_hop(const Nh &x) {
         Hop h{};
@@ -775,6 +797,27 @@ struct RibV3 {
         return h;
     }
 };
+
+// hspf_ospfv3_ribtable_create after its argument checks; `transit_walk` as for hspf::build_rib_records
+int make_ribtable(const hspf_ospfv3_flat *flat, uint32_t area_id, const hl_ospfv3_inter_area_lsa *sums, uint32_t n_sums,
+                  const hl_ospfv3_external_lsa *ext, uint32_t n_ext, bool transit_walk, hspf_ospfv2_ribtable **out) {
+    const hspf_ospfv3_flat &f = *flat;
+    const hl_ospfv3_area *a = f.area;
+    const uint32_t V = (uint32_t)f.rid.size();
+    std::unique_ptr<hspf_ospfv2_ribtable, void (*)(hspf_ospfv2_ribtable *)> rt(new hspf_ospfv2_ribtable(),
+                                                                               hspf_ospfv2_ribtable_free);
+    // a router vertex's flags are its first fragment's, as the intra-area stage reads them
+    rt->vflags.assign(V, 0);
+    for (uint32_t v = 0; v < V; ++v)
+        if (f.is_router[v]) rt->vflags[v] = a->router_lsas[f.first_lsa[v]].flags;
+    int rc = hspf_ospfv3_rtable_create(flat, &rt->intra);
+    if (rc) return rc;
+    rc = hspf::build_rib_records<RibV3>(*rt, area_id, [&](uint32_t id) { return RibV3::root_vertex(f, id); }, sums,
+                                        n_sums, ext, n_ext, transit_walk);
+    if (rc) return rc;
+    *out = rt.release();
+    return HSPF_OK;
+}
 
 }  // namespace
 
@@ -804,25 +847,7 @@ int hspf_ospfv3_ribtable_create(const hspf_ospfv3_flat *flat, uint32_t area_id, 
     if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext)) return HSPF_E_INVAL;
     *out = nullptr;
     try {
-        const hspf_ospfv3_flat &f = *flat;
-        const hl_ospfv3_area *a = f.area;
-        const uint32_t V = (uint32_t)f.rid.size();
-        std::unique_ptr<hspf_ospfv2_ribtable, void (*)(hspf_ospfv2_ribtable *)> rt(new hspf_ospfv2_ribtable(),
-                                                                                   hspf_ospfv2_ribtable_free);
-        // a router vertex's flags are its first fragment's, as the intra-area stage reads them
-        rt->vflags.assign(V, 0);
-        for (uint32_t v = 0; v < V; ++v)
-            if (f.is_router[v]) rt->vflags[v] = a->router_lsas[f.first_lsa[v]].flags;
-        int rc = hspf_ospfv3_rtable_create(flat, &rt->intra);
-        if (rc) return rc;
-        auto router_vertex = [&](uint32_t id) {
-            auto it = f.rtr_vertex.find(id);
-            return it == f.rtr_vertex.end() ? kNone : it->second;
-        };
-        rc = hspf::build_rib_records<RibV3>(*rt, area_id, router_vertex, sums, n_sums, ext, n_ext);
-        if (rc) return rc;
-        *out = rt.release();
-        return HSPF_OK;
+        return make_ribtable(flat, area_id, sums, n_sums, ext, n_ext, false, out);
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_UNSUPPORTED; }
 }
 
@@ -840,6 +865,31 @@ int hspf_ospfv3_rib_from_cells(const hl_ospfv3_area *a, const hspf_ospfv2_ribtab
         out->n_routes = out->n_nexthops = 0;
         return hspf::decode_one_area_rib<RibV3>(a, *rt, cells, gather_v, gather_nh, n_gather, out);
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+
+/* ---- batched routing-table stage for OSPFv3 area border routers (ospf_abr_rib_cells.h) ------------------------ */
+
+int hspf_ospfv3_abr_ribtable_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv3_flat *const *flats,
+                                    const uint32_t *area_ids, const hl_ospfv3_inter_area_lsa *const *summaries,
+                                    const uint32_t *n_summaries, const uint8_t *active,
+                                    const hl_ospfv3_external_lsa *ext, uint32_t n_ext, hspf_ospfv2_abr_ribtable **out) {
+    return hspf::build_abr_ribtable<RibV3>(router_id, n_areas, flats, area_ids, summaries, n_summaries, active, ext,
+                                           n_ext, out);
+}
+
+int hspf_ospfv3_abr_ribtable_prefixes6(const hspf_ospfv2_abr_ribtable *t, const hl_ip_addr **prefixes,
+                                       const uint32_t **lens) {
+    if (!t || !t->v3) return HSPF_E_INVAL;
+    if (prefixes) *prefixes = t->prefix6.data();
+    if (lens) *lens = t->plen.data();
+    return HSPF_OK;
+}
+
+int hspf_ospfv3_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_ospfv3_area *areas, uint32_t n_areas,
+                                   const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
+                                   const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv3_rib *out) {
+    return hspf::decode_abr_rib<RibV3>(t, areas, n_areas, cells, gather_area, gather_v, gather_nh, n_gather, out);
 }
 
 }  // extern "C"

@@ -448,16 +448,22 @@ class AbrRibTable(route_table.RouteTable):
     the instance's area order.  `flats`: one ospfv2.Flat per area (each with the router as a router vertex);
     `summaries`: each area's SUMMARY_LSA_DT[] (LsaKey order); `active`: per area (default all); `externals`: the
     instance's EXTERNAL_LSA_DT[].  `off` is [2 n_areas + 1, P + 1] (intra-area ranges per area, type-3 ranges per
-    area, type-5 ranges); per area `roots`, `n_vertices`, `atom_base`, `n_atoms`."""
+    area, type-5 ranges); per area `roots`, `n_vertices`, `atom_base`, `n_atoms`.
+
+    From ospfv3.Flat areas the table is hspf_ospfv3_abr_ribtable_create's (summaries: INTER_AREA_LSA_DT, externals:
+    EXTERNAL6_LSA_DT); `prefix` and `prefixes6` then hold the IPv6 prefixes (ospfv3.IP_DT) and `v3` is set."""
 
     api, kind, contrib_dt = "hspf_ospfv2", "abr_ribtable", RIB_RECORD_DT
 
     def __init__(self, router_id: int, flats: list, area_ids, summaries=None, active=None, externals=None):
+        from . import ospfv3
         n = len(flats)
         self.router_id, self.flats, self.area_ids = router_id, list(flats), [int(a) for a in area_ids]
-        sums = [np.ascontiguousarray(s if s is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
+        self.v3 = bool(flats) and isinstance(flats[0], ospfv3.Flat)
+        sum_dt, ext_dt = (INTER_AREA_LSA_DT, EXTERNAL6_LSA_DT) if self.v3 else (SUMMARY_LSA_DT, EXTERNAL_LSA_DT)
+        sums = [np.ascontiguousarray(s if s is not None else np.zeros(0, sum_dt), sum_dt)
                 for s in (summaries if summaries is not None else [None] * n)]
-        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, ext_dt), ext_dt)
         self.summaries, self.externals = sums, ext
         self.active = [True] * n if active is None else [bool(a) for a in active]
         fl = (C.c_void_p * max(n, 1))(*[f.handle.value for f in flats])
@@ -467,8 +473,9 @@ class AbrRibTable(route_table.RouteTable):
         act = np.asarray([int(a) for a in self.active] or [0], np.uint8)
         self._keep = (fl, ids, sp, ns, act, sums, ext, flats)
         lib = capi.load_library()
-        super().__init__(lib.hspf_ospfv2_abr_ribtable_create, router_id, n, fl, ids.ctypes.data, sp, ns.ctypes.data,
-                         act.ctypes.data, ext.ctypes.data if len(ext) else None, len(ext))
+        create = lib.hspf_ospfv3_abr_ribtable_create if self.v3 else lib.hspf_ospfv2_abr_ribtable_create
+        super().__init__(create, router_id, n, fl, ids.ctypes.data, sp, ns.ctypes.data, act.ctypes.data,
+                         ext.ctypes.data if len(ext) else None, len(ext))
         self.n_areas = n
         pp, pl, po = C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)(), C.POINTER(C.c_uint32)()
         self._call("arrays", C.byref(pp), C.byref(pl), C.byref(po), None)
@@ -478,6 +485,13 @@ class AbrRibTable(route_table.RouteTable):
         info = [np.zeros(n, np.uint32) for _ in range(4)]
         self._call("areas", *[x.ctypes.data for x in info])
         self.roots, self.n_vertices, self.atom_base, self.n_atoms = [[int(v) for v in x] for x in info]
+        if self.v3:
+            p6 = C.c_void_p()
+            rc = lib.hspf_ospfv3_abr_ribtable_prefixes6(self.handle, C.byref(p6), None)
+            if rc != capi.HSPF_OK:
+                raise capi.HspfError(rc, "hspf_ospfv3_abr_ribtable_prefixes6 failed")
+            self.prefixes6 = route_table.copy_records(p6, self.n_prefixes, ospfv3.IP_DT)
+            self.prefix = self.prefixes6
 
 
 def _planes_array(planes: list):
@@ -509,17 +523,32 @@ def abr_rib_delta_device(ctx: capi.Context, rt: AbrRibTable, n_jobs: int, planes
                            job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
 
 
-def abr_rib_from_cells(areas: list, rt: AbrRibTable, cells: np.ndarray, gather_area, gather_v, gather_nh) -> Rib:
-    """hspf_ospfv2_abr_rib_from_cells (host): one job's cells -> the routing table update_rib_full gives for
-    rt.router_id over its areas (ospfv2.Ospfv2Area images in the table's order).  rc HSPF_E_UNSUPPORTED is returned
-    in the result, as rib_from_cells."""
+def _call_abr_rib_from_cells(fn, area_struct, areas: list, rt: AbrRibTable, cells: np.ndarray, gather_area, gather_v,
+                             gather_nh, route_dt, nh_dt) -> Rib:
     cells = np.ascontiguousarray(cells, RIB_CELL_DT)
     assert cells.shape == (rt.n_prefixes,)
     ga = np.ascontiguousarray(gather_area, np.uint32)
     gv = np.ascontiguousarray(gather_v, np.uint32)
     gn = np.ascontiguousarray(gather_nh, np.uint64)
     structs = [a.as_struct() for a in areas]
-    arr = (ospfv2.AreaStruct * max(len(areas), 1))(*structs)
-    return _call_rib(capi.load_library().hspf_ospfv2_abr_rib_from_cells,
-                     (rt.handle, arr, len(areas), cells.ctypes.data, ga.ctypes.data, gv.ctypes.data, gn.ctypes.data,
-                      len(gv)), rt.n_prefixes, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)
+    arr = (area_struct * max(len(areas), 1))(*structs)
+    return _call_rib(fn, (rt.handle, arr, len(areas), cells.ctypes.data, ga.ctypes.data, gv.ctypes.data, gn.ctypes.data,
+                          len(gv)), rt.n_prefixes, route_dt, nh_dt)
+
+
+def abr_rib_from_cells(areas: list, rt: AbrRibTable, cells: np.ndarray, gather_area, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv2_abr_rib_from_cells (host): one job's cells -> the routing table update_rib_full gives for
+    rt.router_id over its areas (ospfv2.Ospfv2Area images in the table's order).  rc HSPF_E_UNSUPPORTED is returned
+    in the result, as rib_from_cells."""
+    return _call_abr_rib_from_cells(capi.load_library().hspf_ospfv2_abr_rib_from_cells, ospfv2.AreaStruct, areas, rt,
+                                    cells, gather_area, gather_v, gather_nh, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)
+
+
+def abr_rib_from_cells_v3(areas: list, rt: AbrRibTable, cells: np.ndarray, gather_area, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv3_abr_rib_from_cells (host): one job's cells over an OSPFv3 AbrRibTable -> the routing table
+    update_rib_full_v3 gives for rt.router_id over its areas (ospfv3.Ospfv3Area images in the table's order;
+    RIB_ROUTE6_DT routes, ospfv3.NEXTHOP6_DT next hops).  rc HSPF_E_UNSUPPORTED is returned in the result, as
+    rib_from_cells."""
+    from . import ospfv3
+    return _call_abr_rib_from_cells(capi.load_library().hspf_ospfv3_abr_rib_from_cells, ospfv3.AreaStruct, areas, rt,
+                                    cells, gather_area, gather_v, gather_nh, RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)

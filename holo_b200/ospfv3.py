@@ -490,3 +490,160 @@ def inter_area_view(area: Ospfv3Area, seed: int, n_abr: int = 4, n_asbr: int = 3
     for i, x in enumerate(ext):
         externals[i] = x
     return a, summaries, externals
+
+
+ABR_ROUTER_ID = 0x0AFF0001   # the router abr_view roots every area at (ospfv2.ABR_ROUTER_ID)
+ABR_TIE_ASBR = 0x0B0000F1    # an ASBR outside the domain that every non-backbone area of abr_view names
+PFX_LA, PFX_P = 0x02, 0x08   # prefix options carried to the routing table unchanged (RFC 5340 A.4.1.1)
+
+
+def _with_prefixes(area: Ospfv3Area, adds: dict) -> Ospfv3Area:
+    """area with one more Intra-Area-Prefix-LSA per router of `adds` {router_id: [(addr bytes, len, options, metric)]},
+    referencing the router's Router-LSA; LsaKey order kept."""
+    a = Ospfv3Area(**{k: getattr(area, k) for k in area.__dataclass_fields__})
+    iaps, prefixes = [tuple(x) for x in area.iap_lsas.tolist()], [tuple(x) for x in area.prefixes.tolist()]
+    for rid, ps in adds.items():
+        off = len(prefixes)
+        prefixes += [((tuple(b), 1, (0, 0, 0)), ln, opt, metric) for (b, ln, opt, metric) in ps]
+        iaps.append((rid, 0x7000_0000, 1, REF_ROUTER, 0, 0, rid, off, len(ps)))
+    ia = np.zeros(len(iaps), IAP_LSA_DT)
+    for i, x in enumerate(iaps):
+        ia[i] = x
+    pa = np.zeros(len(prefixes), PREFIX_DT)
+    for i, x in enumerate(prefixes):
+        pa[i] = x
+    a.iap_lsas, a.prefixes = ia[np.lexsort((ia["lsa_id"], ia["adv_rtr"]))], pa
+    return a
+
+
+def abr_view(topos: list, seed: int, area_ids=None, roots=None, max_paths: int = 16, n_shared: int = 6,
+             v_flag_area: int | None = 1, **inter_kw):
+    """The OSPFv3 twin of ospfv2.abr_view: a multi-area domain as one ABR sees it, returned as (areas [Ospfv3Area],
+    inter-area LSAs [ospf_rib.INTER_AREA_LSA_DT[] per area, LsaKey order], AS-external LSAs ospf_rib.EXTERNAL6_LSA_DT[]),
+    the areas in instance order.  Area k is synth_area(topos[k], root=roots[k]) with router ids, prefixes and interface
+    sort keys in ranges of its own; the root is router ABR_ROUTER_ID in every area, with the B flag.  Seeded.
+      * area 0 (area_ids[0], 0 by default) carries inter_area_view's load (NU-option LSAs, Inter-Area-Router LSAs whose
+        lsa_id is not the ASBR; those naming the root dropped); every other area gets Inter-Area-Prefix LSAs from two
+        ABRs of its own, for some of area 0's prefixes and new ones, some with the NU option, and Inter-Area-Router
+        LSAs (lsa_id a counter, never the ASBR);
+      * shared prefixes: area 0's first LAN prefix is also area 1's (a transit network in both areas); n_shared
+        router prefixes of area 0 are also advertised by a router of each other area, half at the metric that ties
+        area 0's route and with other prefix options, half not;
+      * an ASBR in each non-backbone area (its farthest router) with externals of its own, also named by a backbone
+        Inter-Area-Router LSA at metric 1; an ASBR outside the domain named by every non-backbone area at one
+        forwarding metric;
+      * with v_flag_area, a router of that area (not the root) gets the V flag."""
+    from . import ospf_rib
+    from .ospfv2 import _dist_from
+    rng = np.random.default_rng(seed)
+    A = len(topos)
+    area_ids = list(area_ids) if area_ids is not None else list(range(A))
+    roots = list(roots) if roots is not None else [0] * A
+    six = lambda hi, lo=0: ipaddress.IPv6Address((0x20010DB8 << 96) | (hi << 64) | lo).packed
+    rec = lambda b: (tuple(b), 1, (0, 0, 0))
+    areas = []
+    for k, (t, r) in enumerate(zip(topos, roots)):
+        rids = [ABR_ROUTER_ID if i == r else RID_BASE + i + (k << 20) for i in range(t.n_routers)]
+        a = synth_area(t, root=r, max_paths=max_paths, rids=rids, area_id=area_ids[k])
+        pb = a.prefixes["addr"]["bytes"]
+        keep = np.zeros(len(pb), bool)
+        if k == 1:                       # area 1's first LAN prefix is area 0's
+            keep = (pb[:, 4] == 0x30) & (pb[:, 5] == 0) & (pb[:, 6] == 0) & (pb[:, 7] == 0)
+        pb[:, 5] = np.where(keep, pb[:, 5], pb[:, 5] + k)
+        a.prefixes["addr"]["bytes"] = pb
+        ifs = a.ifaces.copy()
+        ifs["sort_key"] += 1000 * k
+        ifs["ifindex"] += 1000 * k
+        a.ifaces = ifs
+        a.router_lsas["flags"][a.router_lsas["adv_rtr"] == ABR_ROUTER_ID] |= 0x01
+        areas.append(a)
+    a0, sums0, ext = inter_area_view(areas[0], seed, **inter_kw)
+    a0.router_lsas["flags"][a0.router_lsas["adv_rtr"] == ABR_ROUTER_ID] |= 0x01
+    sums0 = sums0[~((sums0["lsa_type"] == 4) & (sums0["router_id"] == ABR_ROUTER_ID))]
+    areas[0] = a0
+    flat0 = Flat(a0)
+    d0 = _dist_from(flat0, flat0.router_vertex(ABR_ROUTER_ID))
+    stubs0 = []                           # (addr bytes, len, metric, router) of area 0's router prefixes
+    for l in a0.iap_lsas:
+        if int(l["ref_type"]) != REF_ROUTER or int(l["adv_rtr"]) == ABR_ROUTER_ID:
+            continue
+        for p in a0.prefixes[int(l["prefix_off"]): int(l["prefix_off"]) + int(l["n_prefixes"])]:
+            stubs0.append((bytes(int(b) for b in p["addr"]["bytes"]), int(p["len"]), int(p["metric"]), int(l["adv_rtr"])))
+    flags0 = {}
+    for rr, f in zip(a0.router_lsas["adv_rtr"], a0.router_lsas["flags"]):
+        flags0.setdefault(int(rr), int(f))
+    bb_abrs = [rr for rr, f in flags0.items() if f & 0x01 and rr != ABR_ROUTER_ID and flat0.router_vertex(rr) != 0xFFFFFFFF
+               and d0[flat0.router_vertex(rr)] < 1 << 40]
+    inter_prefixes = sorted({(bytes(int(b) for b in s["prefix"]["bytes"]), int(s["len"])) for s in sums0
+                             if s["lsa_type"] == 3})
+    summaries, ext_rows, extra4 = [sums0], [tuple(x) for x in ext.tolist()], []
+    ids = {}
+    next_id = lambda adv: ids.__setitem__(adv, ids.get(adv, 0x100) + 1) or ids[adv]
+    for k in range(1, A):
+        a = areas[k]
+        flat = Flat(a)
+        dk = _dist_from(flat, flat.router_vertex(ABR_ROUTER_ID))
+        reach = {int(flat.router_ids[v]): int(dk[v]) for v in range(len(flat.router_ids))
+                 if flat.is_router[v] and dk[v] < 1 << 40}
+        others = sorted({int(x) for x in a.router_lsas["adv_rtr"]} - {ABR_ROUTER_ID})
+        pick = [int(x) for x in rng.permutation([rr for rr in others if rr in reach])]
+        abrs, vrtr = pick[:2], pick[3]
+        asbr = max((rr for rr in pick[2:] if rr != vrtr), key=lambda rr: (reach[rr], rr))     # the farthest router
+        adds = {}
+        shared = [stubs0[int(i)] for i in rng.choice(len(stubs0), min(n_shared, len(stubs0)), replace=False)]
+        for j, (p, ln, metric, adv) in enumerate(shared):
+            want = int(d0[flat0.router_vertex(adv)]) + metric
+            cand = [(rid, d) for rid, d in reach.items() if rid != ABR_ROUTER_ID and d <= want - 1]
+            if not cand or want > 0xFFFF:
+                continue
+            rid, d = cand[int(rng.integers(0, len(cand)))]
+            m2 = want - d if j % 2 == 0 else want - d + int(rng.choice([-1, 5]))
+            adds.setdefault(rid, []).append((p, ln, PFX_LA if j % 2 == 0 else PFX_P, max(int(m2), 1)))
+        a = _with_prefixes(a, adds)
+        rl = a.router_lsas
+        for rid in abrs:
+            rl["flags"][rl["adv_rtr"] == rid] |= 0x01
+        rl["flags"][rl["adv_rtr"] == asbr] |= 0x02
+        if v_flag_area is not None and k == v_flag_area:
+            rl["flags"][rl["adv_rtr"] == vrtr] |= 0x04
+        areas[k] = a
+        pool = [(p, ln) for (p, ln, _, _) in shared] + inter_prefixes[:6] + [(six(0xD0_0000 + (k << 4) + i), 64)
+                                                                              for i in range(4)]
+        sums = []
+        for n, (p, ln) in enumerate(pool):
+            for abr in abrs[: int(rng.integers(1, 3))]:
+                sums.append((abr, next_id(abr), int(rng.choice([1, 5, 10, 20])), 0, rec(p), ln,
+                             PFX_NU if n % 7 == 3 else 0, 3, 0))
+        sums.append((abrs[0], next_id(abrs[0]), 10, 0x0B000001, rec(bytes(16)), 0, 0, 4, 0))
+        # the ASBR outside the domain every non-backbone area names at one forwarding metric: with one active area the
+        # entries tie across areas and the higher area id wins
+        sums.append((abrs[0], next_id(abrs[0]), max(1, 1000 - reach[abrs[0]]), ABR_TIE_ASBR, rec(bytes(16)), 0, 0, 4, 0))
+        # this area's ASBR, also named by a backbone Inter-Area-Router LSA through the nearest backbone ABR at metric 1
+        if bb_abrs:
+            near = min(bb_abrs, key=lambda rr: (int(d0[flat0.router_vertex(rr)]), rr))
+            extra4.append((near, next_id(near), 1, asbr, rec(bytes(16)), 0, 0, 4, 0))
+        sums.sort(key=lambda x: (x[7], x[0], x[1]))
+        s = np.zeros(len(sums), ospf_rib.INTER_AREA_LSA_DT)
+        for i, x in enumerate(sums):
+            s[i] = x
+        summaries.append(s)
+        for i in range(3):
+            ext_rows.append((asbr, next_id(asbr), int(rng.choice([1, 5, 20])), k, rec(six(0xE0_0000 + (k << 8) + i)), 64,
+                             PFX_P if i == 1 else 0, int(i % 2), 0))
+        ext_rows.append((asbr, next_id(asbr), 5, k, rec(six(0xE0_0000 + (k << 8) + 9)), 64, PFX_NU, 0, 0))
+        if inter_prefixes:                   # an ASBR of area 0's view seen from this area too
+            ext_rows.append((0x0B000001, next_id(0x0B000001), 7, 0, rec(six(0xE0_0000 + (k << 8) + 0xF)), 64, 0, 1, 0))
+    if A > 1:
+        for i in range(2):
+            ext_rows.append((ABR_TIE_ASBR, next_id(ABR_TIE_ASBR), 3, 9, rec(six(0xEF_0000 + i)), 64, 0, i, 0))
+    if extra4:
+        s0 = sorted([tuple(x) for x in summaries[0].tolist()] + extra4, key=lambda x: (x[7], x[0], x[1]))
+        s = np.zeros(len(s0), ospf_rib.INTER_AREA_LSA_DT)
+        for i, x in enumerate(s0):
+            s[i] = x
+        summaries[0] = s
+    ext_rows.sort(key=lambda x: (x[0], x[1]))
+    externals = np.zeros(len(ext_rows), ospf_rib.EXTERNAL6_LSA_DT)
+    for i, x in enumerate(ext_rows):
+        externals[i] = x
+    return areas, summaries, externals

@@ -125,6 +125,10 @@ def declare(lib: C.CDLL):
         "hspf_ospfv2_abr_rib_delta16": [vp, vp, u32, vp, vp, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv2_abr_rib_from_cells": [vp, C.POINTER(ospfv2.AreaStruct), u32, vp, vp, vp, vp, u32,
                                            C.POINTER(ospf_rib.RibStruct)],
+        "hspf_ospfv3_abr_ribtable_create": [u32, u32, vp, vp, vp, vp, vp, vp, u32, pvp],
+        "hspf_ospfv3_abr_ribtable_prefixes6": [vp, pvp, C.POINTER(u32p)],
+        "hspf_ospfv3_abr_rib_from_cells": [vp, C.POINTER(ospfv3.AreaStruct), u32, vp, vp, vp, vp, u32,
+                                           C.POINTER(ospf_rib.RibStruct)],
         "hspf_isis_l1l2_ribtable_create": [C.POINTER(isis.InstanceStruct), C.POINTER(isis.InstanceStruct), vp, vp, u32,
                                            pvp],
         "hspf_isis_l1l2_ribtable_topology": [vp, u32, u32, u32p, u32p],

@@ -281,6 +281,7 @@ int hspf_ospfv2_rib_from_cells(const hl_ospfv2_area *area, const hspf_ospfv2_rib
  *                                HSPF_E_UNSUPPORTED as hspf_ospfv2_rib_from_cells (HL_CELL_MIXED_SID, which also
  *                                marks an intra-area merge across areas or with a transit-area route where a
  *                                Prefix-SID is involved; two atoms with one next hop and different attributes).
+ *                                HSPF_E_INVAL for an OSPFv3 table (hspf_ospfv3_abr_rib_from_cells decodes those).
  *   hspf_ospfv2_abr_rib_delta[16]   the route-delta stage over the same walk (arguments as hspf_ospfv2_rib_delta, rows
  *                                as above in place of roots).  The base row is normally the job whose rows are all
  *                                the unperturbed rows.
@@ -405,6 +406,38 @@ int hspf_ospfv3_ribtable_create(const hspf_ospfv3_flat *flat, uint32_t area_id, 
 int hspf_ospfv3_ribtable_prefixes6(const hspf_ospfv2_ribtable *rt, const hl_ip_addr **prefixes, const uint32_t **lens);
 int hspf_ospfv3_rib_from_cells(const hl_ospfv3_area *area, const hspf_ospfv2_ribtable *rt, const hl_ospf_rib_cell *cells,
                                const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv3_rib *out);
+/* The batched routing-table stage for OSPFv3 area border routers (see "Batched routing-table stage on the device for
+ * one area border router" above): with attached areas A_0 .. A_{n-1} (flat, area id, Inter-Area-Prefix /
+ * Inter-Area-Router LSAs in LsaKey order, active) and AS-external LSAs X, the decoded cells of job j equal
+ *     hspf_ospfv3_update_rib_full(r, max_paths,
+ *         [{A_i.area_id, hspf_ospfv3_area_from_planes(A_i, planes_i[rows[j][i]]), A_i.ifaces, summaries_i, active_i}],
+ *         X)
+ * routes (prefix options, tag, type-2 metric, area) and next hops, the areas in the caller's order.
+ *   hspf_ospfv3_abr_ribtable_create  the same hspf_ospfv2_abr_ribtable, built as hspf_ospfv2_abr_ribtable_create builds
+ *                                 it (same arguments per area, same refusals) over each area's
+ *                                 hspf_ospfv3_ribtable_create table, with that call's OSPFv3 rules (NU-option LSAs left
+ *                                 out, an Inter-Area-Router LSA names its ASBR in router_id, IPv6 prefix order).  An
+ *                                 area 0 with V-flag routers is accepted here: the walk's transit-area step covers it.
+ *                                 The table carries its prefixes as IPv6 networks and the prefix options of every
+ *                                 Inter-Area-Prefix and AS-external record.  hspf_ospfv2_abr_ribtable_free / _prefixes /
+ *                                 _contributors / _arrays (prefix[] all zero) / _areas / _upload and
+ *                                 hspf_ospfv2_abr_rib_cells[16] / hspf_ospfv2_abr_rib_delta[16] take it unchanged.
+ *   hspf_ospfv3_abr_ribtable_prefixes6  the table's prefixes and lengths; HSPF_E_INVAL for an OSPFv2 table.
+ *   hspf_ospfv3_abr_rib_from_cells  host: one job's cells -> the table above, as hspf_ospfv2_abr_rib_from_cells (areas:
+ *                                 each area's image with router_id = the router, in the table's order).  When
+ *                                 intra-area routes of two areas tie, the route keeps the prefix options of the first
+ *                                 area in that order, as update_rib_full keeps the first route it met.  HSPF_E_INVAL
+ *                                 for an OSPFv2 table, as hspf_ospfv2_abr_rib_from_cells gives for an OSPFv3 one. */
+int hspf_ospfv3_abr_ribtable_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv3_flat *const *flats,
+                                    const uint32_t *area_ids, const hl_ospfv3_inter_area_lsa *const *summaries,
+                                    const uint32_t *n_summaries, const uint8_t *active,
+                                    const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
+                                    hspf_ospfv2_abr_ribtable **out);
+int hspf_ospfv3_abr_ribtable_prefixes6(const hspf_ospfv2_abr_ribtable *t, const hl_ip_addr **prefixes,
+                                       const uint32_t **lens);
+int hspf_ospfv3_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_ospfv3_area *areas, uint32_t n_areas,
+                                   const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
+                                   const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv3_rib *out);
 /* Ospfv3::spf_computation_type (holo-ospf/src/ospfv3/spf.rs:96-162): Router-, Network-, Link- and Router-Information
  * LSAs ask for a full run; otherwise the run is partial over the prefixes of the changed Intra-Area-Prefix (old and
  * new instance), Inter-Area-Prefix and AS-external LSAs and the routers of the changed Inter-Area-Router LSAs.
