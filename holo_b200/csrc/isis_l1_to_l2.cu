@@ -94,7 +94,7 @@ int l1_to_l2_delta(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_
     if (!ctx || !base_cells || !job_out || !n_records || n_base == 0 ||
         (reinterpret_cast<uintptr_t>(base_cells) & 7u) || (reinterpret_cast<uintptr_t>(job_out) & 3u) ||
         (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u) ||
-        hspf::delta_tiles64(n_jobs, t->K) > 0xFFFFFFFFull)
+        !hspf::delta_batch_fits(n_jobs, t->K))
         return HSPF_E_INVAL;
     if (const int rc = hspf::launch_isis_summaries<kL1ToL2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
     return hspf::launch_route_delta<hspf::IsisCellLayout, kL1ToL2BlocksPerSM>(

@@ -21,12 +21,12 @@ struct IsisL1L2Cell {
     hspf::IsisL1L2View t;
     Rows pl[2][2];                   // [level - 1][topology]; MT-IPv6 planes NULL where the level has no MT-IPv6 root
     uint32_t n_rows[2];
-    const uint32_t *rows;            // [n_jobs][2]: the job's L1 row, L2 row
+    const uint32_t *rows;            // [n_jobs][2]: the job's L1 row, L2 row (indexed in size_t: 2 * j wraps at 2^31)
     const uint64_t *words;           // [n_jobs][S], written by the summary pass
     __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
         uint32_t st = 0;
         for (uint32_t l = 0; l < 2; ++l) {
-            const uint32_t r = rows[2 * j + l];
+            const uint32_t r = rows[2 * (size_t)j + l];
             if (r >= n_rows[l]) st |= HSPF_JS_INVALID;
             else st |= pl[l][0].status_word(r) | pl[l][1].status_word(r);
         }
@@ -34,7 +34,7 @@ struct IsisL1L2Cell {
     }
     __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
     __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        const uint32_t r1 = rows[2 * j], r2 = rows[2 * j + 1];
+        const uint32_t r1 = rows[2 * (size_t)j], r2 = rows[2 * (size_t)j + 1];
         const hl_isis_route_cell c = hspf::isis_l1l2_cell_eval(pl[0][0].job(r1), pl[0][1].job(r1), pl[1][0].job(r2),
                                                                pl[1][1].job(r2), t, p, words + (size_t)j * t.S);
         return {c.nh_mask, (uint64_t)c.winner | ((uint64_t)c.metric << 32), c.flags};
@@ -42,7 +42,7 @@ struct IsisL1L2Cell {
     __host__ __device__ __forceinline__ uint32_t n_summaries() const { return t.S; }
     // the summary word of (job j, summary s) over the job's L1 row (isis_summary.cuh)
     __device__ __forceinline__ uint64_t summary_word(uint32_t j, uint32_t s, uint32_t lane) const {
-        const uint32_t r1 = rows[2 * j];
+        const uint32_t r1 = rows[2 * (size_t)j];
         return hspf::isis_summary_word(pl[0][0].job(r1), pl[0][1].job(r1), t, s, lane);
     }
     __device__ __forceinline__ uint64_t gather(uint32_t, uint32_t, uint32_t) const { return 0; }   // the decode needs none
@@ -100,7 +100,7 @@ int l1l2_rib_delta(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_j
     if (!ctx || !base_cells || !job_out || !n_records || n_base == 0 ||
         (reinterpret_cast<uintptr_t>(base_cells) & 7u) || (reinterpret_cast<uintptr_t>(job_out) & 3u) ||
         (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u) ||
-        hspf::delta_tiles64(n_jobs, t->P) > 0xFFFFFFFFull)
+        !hspf::delta_batch_fits(n_jobs, t->P))
         return HSPF_E_INVAL;
     if (const int rc = hspf::launch_isis_summaries<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
     return hspf::launch_route_delta<hspf::IsisCellLayout, kL1L2BlocksPerSM>(

@@ -183,10 +183,17 @@ struct DeltaArgs {
     uint64_t cap;
 };
 
-// warp tiles of the stage; launch_route_delta refuses a batch with 2^32 or more
+// warp tiles of the stage
 __host__ __device__ __forceinline__ uint64_t delta_tiles64(uint32_t n_jobs, uint32_t P) {
     return ((uint64_t)n_jobs * P + 31) / 32;
 }
+
+// The largest batch of one route-delta call: n_jobs x P <= 2^36 cells, at most 2^31 warp tiles.  The delta kernels
+// walk tiles with a 32-bit counter and a stride of the grid's warp count (< 2^31), so tile + stride < 2^32 never
+// wraps; the reciprocal in delta_eval is exact below 2^37.  Every delta entry point refuses a larger batch before
+// its first launch.
+constexpr uint64_t kDeltaMaxCells = 1ull << 36;
+inline bool delta_batch_fits(uint32_t n_jobs, uint32_t P) { return (uint64_t)n_jobs * P <= kDeltaMaxCells; }
 __device__ __forceinline__ uint32_t delta_tiles(const DeltaArgs &a) { return (uint32_t)delta_tiles64(a.n_jobs, a.P); }
 
 // The kind of the cell of `lane` in warp tile `tile` (0 past the end, for a job without a valid base row, and for a
@@ -223,7 +230,8 @@ __global__ void __launch_bounds__(kRouteThreads, kMinBlocks) route_delta_count_k
     }
     const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const uint32_t n_tiles = delta_tiles(a);
-    uint32_t warp_changes = 0;      // < 2^32: at most 32 per tile, and a warp walks at most 2^26 of the < 2^32 tiles
+    uint32_t warp_changes = 0;      // < 2^32: at most 32 per tile, and a warp walks at most 2^26 of the <= 2^31 tiles
+    // no wrap: n_tiles <= 2^31 (delta_batch_fits) and the stride, the grid's warp count, is far below 2^31
     for (uint32_t tile = blockIdx.x * kWarps + wib; tile < n_tiles; tile += gridDim.x * kWarps) {
         uint32_t job, p, metric;
         const uint32_t kind = delta_eval<L>(cell, a, tile, lane, job, p, metric);
@@ -249,6 +257,7 @@ __global__ void __launch_bounds__(kRouteThreads, kMinBlocks) route_delta_store_k
     constexpr uint32_t kWarps = kRouteThreads / 32;
     const uint32_t lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const uint32_t n_tiles = delta_tiles(a);
+    // no wrap, as in pass A
     for (uint32_t tile = blockIdx.x * kWarps + wib; tile < n_tiles; tile += gridDim.x * kWarps) {
         if (a.tile_cnt[tile] == 0) continue;
         const uint64_t first = a.tile_off[tile];
@@ -278,7 +287,7 @@ template <class Layout, int kMinBlocks, uint32_t kBlocksPerSM = kMinBlocks, clas
 int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs, uint32_t P,
                        const void *base, uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                        hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    if (!ctx || !base || !job_out || !n_records || n_base == 0) return HSPF_E_INVAL;
+    if (!ctx || !base || !job_out || !n_records || n_base == 0 || !delta_batch_fits(n_jobs, P)) return HSPF_E_INVAL;
     // device buffers at their struct alignment
     if ((reinterpret_cast<uintptr_t>(base) & 7u) || (reinterpret_cast<uintptr_t>(job_out) & 3u) ||
         (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u))
@@ -288,7 +297,6 @@ int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell 
     uint32_t blocks = 0;
     const int rc = route_grid(ctx, table, std::max<uint64_t>(total, n_jobs), kBlocksPerSM, blocks);
     if (rc != HSPF_OK) return rc;
-    if (n_tiles > 0xFFFFFFFFull) return HSPF_E_INVAL;
     DeltaArgs a{};
     a.n_jobs = n_jobs; a.P = P; a.inv_p = P ? 1.0 / P : 0.0;
     a.base = static_cast<const uint64_t *>(base); a.n_base = n_base; a.base_of = base_of;

@@ -746,7 +746,10 @@ int hspf_isis_l1_to_l2_from_cells(const hl_isis_instance *l1, const hspf_isis_l1
  * metric or over another next-hop set, against a base route table — without storing the n_jobs x P cell matrix.
  * Per (job, prefix) it runs the same walk as hspf_*_routes_batch[16] and compares the cell with the job's base cell
  * word for word (for a fixed root, atom a is always the same first hop, whatever the job's overrides).  Enqueued on
- * the ctx stream behind the SPT batches; no synchronisation.
+ * the ctx stream behind the SPT batches; no synchronisation.  One call covers at most 2^36 cells: every route-delta
+ * entry point (hspf_*_delta[16], here and above) returns HSPF_E_INVAL and enqueues nothing when n_jobs x P > 2^36,
+ * P being the table's prefixes (its keys for hspf_isis_l1_to_l2_delta); a caller splits a larger sweep into several
+ * calls.
  *
  *   hspf_ospfv2_routes_delta[16]  OSPFv2 and OSPFv3 tables (as hspf_ospfv2_routes_batch[16]).
  *   hspf_isis_routes_delta[16]    IS-IS tables (as hspf_isis_routes_batch[16]).
