@@ -876,6 +876,7 @@ extern "C" int hspf_isis_routes_from_planes(const hl_isis_instance *in, const ui
 #include <cassert>
 #include <memory>
 
+#include "isis_backbone_cells.h"
 #include "isis_l1_to_l2_cells.h"
 #include "isis_l1l2_rib_cells.h"
 #include "isis_propagation.h"
@@ -884,7 +885,9 @@ extern "C" int hspf_isis_routes_from_planes(const hl_isis_instance *in, const ui
 namespace {
 const uint8_t kTopologies[2] = {HL_ISIS_MT_STANDARD, HL_ISIS_MT_IPV6};    // table topology 0, 1
 
-struct RawContrib { NetKey key; hspf::IsisContrib c; int32_t src; };
+// src: the lvl.ipreaches index of an entry that can carry a Prefix-SID, else -1; idx: the entry's index, -1 for an
+// ATT-bit default route
+struct RawContrib { NetKey key; hspf::IsisContrib c; int32_t src, idx; };
 
 // Every contribution compute_routes can make in the instance's enabled topologies, in NetKey order and, within a
 // prefix, in walk order; entries whose lvl.ipreaches byte in `drop` is non-zero are left out (drop NULL: none).
@@ -916,6 +919,7 @@ int collect_contributions(const hl_isis_instance *in, const uint8_t *drop, std::
                                   r.c.has_psid = (src && src->has_psid) ? 1 : 0;
                                   r.c.sr = (r.c.has_psid && in->sr_enabled) ? 1 : 0;
                                   r.src = src ? (int32_t)(src - in->lvl.ipreaches) : -1;
+                                  r.idx = idx;
                                   raw.push_back(r);
                               });
     }
@@ -977,9 +981,10 @@ int decode_topos(const hl_isis_instance *in, const uint32_t n_vertices[2], const
     return HSPF_OK;
 }
 
-// The route of a present cell won by contributor k (src: its lvl.ipreaches index) of `in`.
+// The route of a present cell won by contributor k of `in`; psid: the entry whose Prefix-SID the route takes when
+// k.has_psid.
 int decode_route(const hl_isis_instance *in, const DecodeTopo tp[2], const SrView &sr, const hspf::IsisContrib &k,
-                 int32_t src, const hl_isis_route_cell &c, bool v6, RouteE &r) {
+                 const hl_isis_ipreach *psid, const hl_isis_route_cell &c, bool v6, RouteE &r) {
     const DecodeTopo &T = tp[k.topology];
     if (!T.live || k.vertex >= T.f.ids.size()) return HSPF_E_INVAL;
     r = RouteE{};
@@ -998,16 +1003,21 @@ int decode_route(const hl_isis_instance *in, const DecodeTopo tp[2], const SrVie
             return HSPF_E_UNSUPPORTED;
     }
     while (r.nh.size() > in->max_paths) r.nh.erase(std::prev(r.nh.end()));
-    if (k.has_psid) {
-        if (src < 0 || (uint32_t)src >= in->lvl.n_ipreaches) return HSPF_E_INVAL;
-        const hl_isis_ipreach &e = in->lvl.ipreaches[src];
-        r.psid = PrefixSid{true, e.psid_flags, e.psid_is_label != 0, e.psid_value};
-    }
+    if (k.has_psid) r.psid = PrefixSid{true, psid->psid_flags, psid->psid_is_label != 0, psid->psid_value};
     // all best-metric contributions come from the winner's vertex (else the cell is flagged):
     // one update with its context gives the labels every repeated update would
     if (in->sr_enabled && r.psid.present)
         sr.update(r, in->system_id, T.f.ids[k.vertex], v6, T.hops[k.vertex] == 0, T.hops[k.vertex] == 1);
     return HSPF_OK;
+}
+
+// ... won by contributor k whose entry is src (its lvl.ipreaches index)
+int decode_route(const hl_isis_instance *in, const DecodeTopo tp[2], const SrView &sr, const hspf::IsisContrib &k,
+                 int32_t src, const hl_isis_route_cell &c, bool v6, RouteE &r) {
+    const DecodeTopo &T = tp[k.topology];
+    if (!T.live || k.vertex >= T.f.ids.size()) return HSPF_E_INVAL;
+    if (k.has_psid && (src < 0 || (uint32_t)src >= in->lvl.n_ipreaches)) return HSPF_E_INVAL;
+    return decode_route(in, tp, sr, k, k.has_psid ? &in->lvl.ipreaches[src] : nullptr, c, v6, r);
 }
 
 }  // namespace
@@ -1378,6 +1388,7 @@ int hspf_isis_l1_to_l2_table_create(const hl_isis_instance *l1, const hl_isis_in
             for (; i < raw.size() && raw[i].kind == kind && !(key < raw[i].key) && !(raw[i].key < key); ++i) {
                 t->recs.push_back(raw[i].r);
                 t->src.push_back(raw[i].src);
+                t->has_psid.push_back(lv.ipreaches[raw[i].src].has_psid);
             }
         }
         off.push_back((uint32_t)t->recs.size());
@@ -1385,6 +1396,7 @@ int hspf_isis_l1_to_l2_table_create(const hl_isis_instance *l1, const hl_isis_in
         t->words = off;
         t->words.insert(t->words.end(), sum.begin(), sum.end());
         t->n_ipreaches = lv.n_ipreaches;
+        t->system_id = l1->system_id;
         t->rib = rib;
         *out = t.release();
         return HSPF_OK;
@@ -1435,6 +1447,238 @@ int hspf_isis_l1_to_l2_from_cells(const hl_isis_instance *l1, const hspf_isis_l1
         if (got.size() > cap) return HSPF_E_NOMEM;
         std::copy(got.begin(), got.end(), out);
         return HSPF_OK;
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+}  // extern "C"
+
+/* ---- routing table of a backbone router over the L1 jobs of an area (isis_backbone_cells.h) ------------------- */
+namespace {
+
+static_assert(hspf::kIsisMaxWide == kMaxWide, "the device walk and compute_routes read TLV 135 up to one limit");
+
+using BorderKey = std::pair<uint8_t, NetKey>;
+
+BorderKey border_key(const hspf_isis_l1_to_l2_table *b, uint32_t k) { return {b->kind[k], NetKey{b->prefix[k], b->len[k]}}; }
+
+// the key's records in the border's cells: its first winner and how many (a summary key: its one summary winner)
+void key_records(const hspf_isis_l1_to_l2_table *b, uint32_t k, uint32_t &first, uint32_t &count) {
+    const hspf::IsisL1ToL2View v = b->view(b->words.data(), b->recs.data());
+    if (v.sum[k] != hspf::kIsisNoSummary) { first = v.n_records + (v.sum[k] >> 1); count = 1; }
+    else { first = v.off[k]; count = v.off[k + 1] - v.off[k]; }
+}
+
+// How compute_routes takes an entry of kind `kind` as `emit` passes it (for_each_contribution): whether it carries a
+// Prefix-SID (TLV 128 / 130 never do) and its external bit.
+inline bool kind_has_psid(uint8_t kind) { return kind != HL_ISIS_IP_V4_INTERNAL && kind != HL_ISIS_IP_V4_EXTERNAL; }
+inline bool kind_external(uint8_t kind, const hl_isis_ipreach &e) {
+    return kind_has_psid(kind) ? e.external != 0 : kind == HL_ISIS_IP_V4_EXTERNAL;
+}
+
+}  // namespace
+
+extern "C" {
+
+void hspf_isis_backbone_table_free(hspf_isis_backbone_table *t) {
+    if (!t) return;
+    hspf::release_route_table(t->dev);
+    delete t;
+}
+
+int hspf_isis_backbone_table_create(const hl_isis_instance *l2, const uint8_t *derived, uint32_t n_borders,
+                                    const hspf_isis_l1_to_l2_table *const *borders, hspf_isis_backbone_table **out) {
+    if (!out) return HSPF_E_INVAL;
+    *out = nullptr;
+    if (!l2 || !borders || n_borders == 0 || n_borders > hspf::kIsisBackboneMaxBorders) return HSPF_E_INVAL;
+    if (l2->level != 2 || (l2->level_type != 2 && l2->level_type != 3)) return HSPF_E_INVAL;
+    for (uint32_t b = 0; b < n_borders; ++b) {
+        if (!borders[b] || borders[b]->system_id == l2->system_id) return HSPF_E_INVAL;
+        for (uint32_t c = 0; c < b; ++c)
+            if (borders[c]->system_id == borders[b]->system_id) return HSPF_E_INVAL;
+    }
+    try {
+        const hl_isis_level &lv = l2->lvl;
+        // each entry's border (-1: none), each border's valid zeroth fragment of its non-pseudonode LSP
+        std::vector<int32_t> owner(lv.n_ipreaches, -1), zeroth(n_borders, -1);
+        for (uint32_t i = 0; i < lv.n_lsps; ++i) {
+            const hl_isis_lsp &lsp = lv.lsps[i];
+            if (is_pn(lsp.lan_id)) continue;
+            for (uint32_t b = 0; b < n_borders; ++b) {
+                if ((lsp.lan_id >> 8) != borders[b]->system_id) continue;
+                if (lsp.fragment == 0 && lsp.seqno && lsp.rem_lifetime) zeroth[b] = (int32_t)i;
+                for (uint32_t k = lsp.ipreach_off; k < lsp.ipreach_off + lsp.n_ipreach && k < lv.n_ipreaches; ++k)
+                    owner[k] = (int32_t)b;
+            }
+        }
+        std::vector<std::map<BorderKey, uint32_t>> keys(n_borders);
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            if (zeroth[b] < 0) return HSPF_E_INVAL;
+            for (uint32_t k = 0; k < borders[b]->K; ++k) keys[b][border_key(borders[b], k)] = k;
+        }
+        // a derived entry is a key of its border; a summary key overwrites an entry of the border's own, which the
+        // splice below cannot express
+        for (uint32_t k = 0; k < lv.n_ipreaches; ++k) {
+            const int32_t b = owner[k];
+            const bool der = derived && derived[k];
+            if (der && b < 0) return HSPF_E_INVAL;
+            if (b < 0) continue;
+            const auto it = keys[b].find(BorderKey{lv.ipreaches[k].kind, NetKey{lv.ipreaches[k].prefix, lv.ipreaches[k].len}});
+            if (der && it == keys[b].end()) return HSPF_E_INVAL;
+            if (!der && it != keys[b].end()) {
+                const hspf::IsisL1ToL2View v = borders[b]->view(borders[b]->words.data(), borders[b]->recs.data());
+                if (v.sum[it->second] != hspf::kIsisNoSummary) return HSPF_E_UNSUPPORTED;
+            }
+        }
+        // The spliced image: the derived entries dropped, one placeholder per border key appended to the border's
+        // zeroth fragment.  collect_contributions over it meets static entries and slots in walk order.
+        std::vector<hl_isis_lsp> lsps(lv.lsps, lv.lsps + lv.n_lsps);
+        std::vector<hl_isis_ipreach> ips;
+        std::vector<int64_t> origin;              // per spliced entry: its lvl.ipreaches index, or -1 - slot
+        std::vector<std::pair<uint32_t, uint32_t>> slot_key;     // (border, key)
+        for (uint32_t i = 0; i < lv.n_lsps; ++i) {
+            const uint32_t at = (uint32_t)ips.size();
+            for (uint32_t k = lsps[i].ipreach_off; k < lsps[i].ipreach_off + lsps[i].n_ipreach && k < lv.n_ipreaches; ++k) {
+                if (derived && derived[k]) continue;
+                ips.push_back(lv.ipreaches[k]);
+                origin.push_back(k);
+            }
+            for (uint32_t b = 0; b < n_borders; ++b) {
+                if (zeroth[b] != (int32_t)i) continue;
+                for (uint32_t k = 0; k < borders[b]->K; ++k) {
+                    hl_isis_ipreach e{};
+                    e.prefix = borders[b]->prefix[k];
+                    e.len = borders[b]->len[k];
+                    e.kind = borders[b]->kind[k];
+                    ips.push_back(e);
+                    origin.push_back(-1 - (int64_t)slot_key.size());
+                    slot_key.emplace_back(b, k);
+                }
+            }
+            lsps[i].ipreach_off = at;
+            lsps[i].n_ipreach = (uint32_t)ips.size() - at;
+        }
+        hl_isis_instance sp = *l2;
+        sp.lvl.lsps = lsps.data();
+        sp.lvl.ipreaches = ips.data();
+        sp.lvl.n_ipreaches = (uint32_t)ips.size();
+        auto t = std::make_unique<hspf_isis_backbone_table>();
+        std::vector<RawContrib> raw;
+        const int rc = collect_contributions(&sp, nullptr, raw, t->n_vertices, t->root);
+        if (rc) return rc;
+        // the affected prefixes, each with its contributions
+        std::set<NetKey> affected;
+        for (uint32_t b = 0; b < n_borders; ++b)
+            for (uint32_t k = 0; k < borders[b]->K; ++k) affected.insert(NetKey{borders[b]->prefix[k], borders[b]->len[k]});
+        std::vector<uint32_t> off, sr;
+        size_t i = 0;
+        for (const NetKey &p : affected) {
+            t->prefix.push_back(p.a);
+            t->len.push_back(p.len);
+            off.push_back((uint32_t)t->contribs.size());
+            for (; i < raw.size() && raw[i].key < p; ++i) {}
+            for (; i < raw.size() && !(p < raw[i].key); ++i) {
+                const RawContrib &r = raw[i];
+                hspf::IsisBackboneContrib c{};
+                c.vertex = r.c.vertex;
+                c.topology = r.c.topology;
+                const int64_t o = r.idx >= 0 ? origin[r.idx] : -1;
+                if (r.idx < 0 || o >= 0) {                 // a static contribution
+                    c.metric = r.c.metric;
+                    c.border = hspf::kIsisBackboneStatic;
+                    c.sr = r.c.sr;
+                    t->stat.push_back(r.c);
+                    t->src.push_back((int32_t)(r.src >= 0 ? o : -1));
+                } else {
+                    const uint32_t b = slot_key[-1 - o].first, k = slot_key[-1 - o].second;
+                    uint32_t first, count;
+                    key_records(borders[b], k, first, count);
+                    c.metric = k;
+                    c.base = (uint32_t)sr.size() - first;
+                    c.border = (uint8_t)b;
+                    c.wide = borders[b]->kind[k] == HL_ISIS_IP_V4_EXT;
+                    for (uint32_t w = 0; w < count; ++w) {
+                        const bool rec = first + w < borders[b]->recs.size();
+                        sr.push_back(rec && kind_has_psid(borders[b]->kind[k]) && borders[b]->has_psid[first + w] &&
+                                     l2->sr_enabled);
+                        t->slot_of.push_back((uint32_t)t->contribs.size());
+                    }
+                    t->stat.push_back(hspf::IsisContrib{});
+                    t->src.push_back(-1);
+                }
+                t->contribs.push_back(c);
+            }
+        }
+        t->P = (uint32_t)t->prefix.size();
+        off.push_back((uint32_t)t->contribs.size());
+        t->n_slot_records = (uint32_t)sr.size();
+        t->words = off;
+        t->words.insert(t->words.end(), sr.begin(), sr.end());
+        t->n_borders = n_borders;
+        t->n_ipreaches = lv.n_ipreaches;
+        std::copy(borders, borders + n_borders, t->borders);
+        *out = t.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+int hspf_isis_backbone_table_prefixes(const hspf_isis_backbone_table *t, uint32_t *n_prefixes, const hl_ip_addr **prefix,
+                                      const uint8_t **len) {
+    if (!t) return HSPF_E_INVAL;
+    if (n_prefixes) *n_prefixes = t->P;
+    if (prefix) *prefix = t->prefix.data();
+    if (len) *len = t->len.data();
+    return HSPF_OK;
+}
+
+int hspf_isis_backbone_from_cells(const hl_isis_instance *l2, const hspf_isis_backbone_table *t,
+                                  const hl_isis_route_cell *cells, const hspf_isis_job_planes *planes,
+                                  const hl_isis_ipreach *const *entries, const uint32_t *n_entries, hl_isis_rib *out) {
+    if (!l2 || !t || !planes || !out || (!cells && t->P) || !entries || !n_entries) return HSPF_E_INVAL;
+    if (l2->level != 2 || l2->lvl.n_ipreaches != t->n_ipreaches) return HSPF_E_INVAL;     // not the table's instance
+    try {
+        auto tp = std::make_unique<DecodeTopo[]>(2);
+        int rc = decode_topos(l2, t->n_vertices, t->root, planes, tp.get());
+        if (rc) return rc;
+        // each border's job entries by key
+        std::vector<std::map<BorderKey, const hl_isis_ipreach *>> job(t->n_borders);
+        for (uint32_t b = 0; b < t->n_borders; ++b) {
+            if (n_entries[b] && !entries[b]) return HSPF_E_INVAL;
+            for (uint32_t e = 0; e < n_entries[b]; ++e)
+                job[b][BorderKey{entries[b][e].kind, NetKey{entries[b][e].prefix, entries[b][e].len}}] = &entries[b][e];
+        }
+        const SrView sr(l2->lvl);
+        const hspf::IsisBackboneView v = t->view(t->words.data(), t->contribs.data());
+        std::map<NetKey, RouteE> rib;
+        for (uint32_t p = 0; p < t->P; ++p) {
+            const hl_isis_route_cell &c = cells[p];
+            if (!(c.flags & HL_CELL_PRESENT)) continue;
+            if (c.flags & HL_CELL_MIXED_SID) return HSPF_E_UNSUPPORTED;
+            const bool v6 = t->prefix[p].is_v6 != 0;
+            RouteE r;
+            if (c.winner < v.n_contribs) {             // a static contribution
+                if (c.winner < v.off[p] || c.winner >= v.off[p + 1] || t->contribs[c.winner].border != hspf::kIsisBackboneStatic)
+                    return HSPF_E_INVAL;
+                rc = decode_route(l2, tp.get(), sr, t->stat[c.winner], t->src[c.winner], c, v6, r);
+            } else {                                   // a slot: the border's entry of the job
+                const uint32_t g = c.winner - v.n_contribs;
+                if (g >= t->n_slot_records) return HSPF_E_INVAL;
+                const uint32_t i = t->slot_of[g];
+                if (i < v.off[p] || i >= v.off[p + 1]) return HSPF_E_INVAL;
+                const hspf::IsisBackboneContrib &s = t->contribs[i];
+                const auto it = job[s.border].find(border_key(t->borders[s.border], s.metric));
+                if (it == job[s.border].end()) return HSPF_E_INVAL;
+                const hl_isis_ipreach &e = *it->second;
+                hspf::IsisContrib k{};
+                k.vertex = s.vertex;
+                k.topology = s.topology;
+                k.external = kind_external(e.kind, e);
+                k.has_psid = kind_has_psid(e.kind) && e.has_psid;
+                rc = decode_route(l2, tp.get(), sr, k, &e, c, v6, r);
+            }
+            if (rc) return rc;
+            rib.emplace_hint(rib.end(), NetKey{t->prefix[p], t->len[p]}, std::move(r));
+        }
+        return emit_rib(rib, out);
     } catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
 }
 

@@ -100,7 +100,9 @@ struct hspf_isis_l1_to_l2_table {
     std::vector<uint32_t> words;             // the view's u32 arrays: off [K + 1], sum [K]
     std::vector<hspf::IsisPropRecord> recs;
     std::vector<uint32_t> src;               // per record: index of its entry in the L1 ipreaches
+    std::vector<uint8_t> has_psid;           // per record: its entry carries a Prefix-SID
     uint32_t K = 0, n_ipreaches = 0;
+    uint64_t system_id = 0;                  // the router's
     const hspf_isis_l1l2_ribtable *rib = nullptr;   // the summaries, their metrics and cover lists
     hspf::DeviceRouteTable dev;              // hspf_isis_l1_to_l2_table_upload
 

@@ -55,6 +55,25 @@ HSPF_HD IsisContrib load_isis_contrib(const IsisContrib *p) {
 // the host needs, except for SR labels: every SrView::update relabels with the latest contributor's
 // context.  When the route has an SR-relevant Prefix-SID and its best-metric contributions come from two
 // or more vertices the cell is flagged: the host redoes that job from its planes.
+//
+// One `add` of the walk (isis_backbone_cell_eval): the contribution of `vertex` (reached in `pl`) at total metric m,
+// recorded as `winner`; `sr`: its Prefix-SID is SR-relevant.  cur_vertex / cur_sr: the current winner's.
+template <class Planes>
+HSPF_HD void isis_route_add(hl_isis_route_cell &c, uint32_t &cur_vertex, bool &cur_sr, const Planes &pl,
+                            uint32_t vertex, uint32_t m, uint32_t winner, bool sr) {
+    if (!(c.flags & HL_CELL_PRESENT) || m < c.metric) {
+        c.metric = m;
+        c.winner = winner;
+        c.flags = (uint8_t)(HL_CELL_PRESENT | (pl.h(vertex) == 0 ? HL_CELL_CONNECTED : 0));
+        c.nh_mask = pl.n(vertex);
+        cur_vertex = vertex;
+        cur_sr = sr;
+    } else if (m == c.metric) {
+        if (cur_sr && vertex != cur_vertex) c.flags |= HL_CELL_MIXED_SID;
+        c.nh_mask |= pl.n(vertex);
+    }
+}
+
 template <class Planes>
 HSPF_HD hl_isis_route_cell isis_route_cell_eval(const Planes &std_pl, const Planes &mt6_pl, const IsisContrib *contribs,
                                                 uint32_t begin, uint32_t end) {
@@ -67,6 +86,9 @@ HSPF_HD hl_isis_route_cell isis_route_cell_eval(const Planes &std_pl, const Plan
         const IsisContrib k = load_isis_contrib(contribs + i);
         const Planes pl = k.topology ? mt6_pl : std_pl;     // a copy: selecting a reference puts both on the stack
         if (!pl.reached(k.vertex)) continue;
+        // isis_route_add written out: calling it gives the IS-IS route stage's kernels other SASS (delta passes 44 / 46
+        // registers instead of 45 / 47), untimed; written out, all three IS-IS stages keep their SASS.  Both copies are
+        // held to hspf_isis_routes_from_planes by the route-cell and backbone tests.
         const uint32_t m = pl.d(k.vertex) + k.metric;
         if (!(c.flags & HL_CELL_PRESENT) || m < c.metric) {
             c.metric = m;

@@ -887,6 +887,100 @@ def l1_to_l2_from_cells(l1: dict, t: L1ToL2Table, cells: np.ndarray, words: np.n
     return out[: n.value].copy()
 
 
+# ---- backbone routers over L1 what-if jobs (include/holo_spf_lsdb.h: hspf_isis_backbone_*) ------------------------
+class BackboneTable:
+    """hspf_isis_backbone_table of one backbone router R: its affected prefixes over an area's L1 jobs.  `l2`: R's
+    level-2 instance image; `borders`: the area's L1ToL2Table list (kept alive with this table); `derived`: u8 per l2
+    IP reachability entry marking the borders' propagated and summary entries, or None.  `prefix`, `len`
+    [n_prefixes]: the affected prefixes in hl_isis_rib order."""
+
+    def __init__(self, l2: dict, borders, derived=None):
+        self.lib = capi.load_library()
+        self.borders = list(borders)
+        s2 = instance_struct(l2)
+        der = None if derived is None else np.ascontiguousarray(derived, np.uint8)
+        assert der is None or len(der) == len(l2["level"].ipreaches), "one derived byte per IP reachability entry"
+        arr = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
+        h = C.c_void_p()
+        rc = self.lib.hspf_isis_backbone_table_create(C.byref(s2), der.ctypes.data if der is not None and len(der) else None,
+                                                      len(self.borders), arr, C.byref(h))
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, "hspf_isis_backbone_table_create failed")
+        self.handle = h
+        n, pp, pl = C.c_uint32(), C.c_void_p(), C.c_void_p()
+        assert self.lib.hspf_isis_backbone_table_prefixes(h, C.byref(n), C.byref(pp), C.byref(pl)) == capi.HSPF_OK
+        self.n_prefixes = n.value
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, IP_DT)
+        self.len = route_table.copy_records(pl, self.n_prefixes, np.uint8)
+
+    def upload(self, ctx: capi.Context):
+        rc = self.lib.hspf_isis_backbone_table_upload(ctx.handle, self.handle)
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, ctx.last_error())
+
+    def __del__(self):
+        try:
+            if self.handle:
+                self.lib.hspf_isis_backbone_table_free(self.handle)
+                self.handle = None
+        except Exception:
+            pass
+
+
+def _device_ptrs(ptrs):
+    return (C.c_void_p * max(len(ptrs), 1))(*[int(p) or None for p in ptrs])
+
+
+def backbone_cells_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, l2, border_cells, border_status,
+                          status_ptr: int, cells_ptr: int):
+    """hspf_isis_backbone_cells / _cells16 over DEVICE planes.  l2: (rs_std, rs_mt6) of R's L2 batch (only row 0 is
+    read; rs_mt6 may be None unless R has an MT-IPv6 root); border_cells: per border a device pointer to its
+    [n_jobs, K_b] L1 -> L2 cells; border_status: per border a device u32 [n_jobs] pointer or 0 (None: none);
+    status_ptr: device u32 [n_jobs] or 0; cells_ptr: device [n_jobs, t.n_prefixes] cells.  Enqueued on the ctx
+    stream; the table must have been uploaded."""
+    rs = next((x for x in l2 if x is not None), None)      # none at all: the call refuses the arguments
+    st = _device_ptrs(border_status) if border_status is not None else None
+    route_table.call_stage(ctx, "hspf_isis_backbone_cells", rs, t.handle, n_jobs, *map(_planes_pair, l2),
+                           _device_ptrs(border_cells), st, status_ptr or None, cells_ptr or None)
+
+
+def backbone_delta_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, l2, border_cells, border_status,
+                          base_ptr: int, n_base: int, base_of_ptr: int, job_out_ptr: int, records_ptr: int, cap: int,
+                          n_records_ptr: int):
+    """hspf_isis_backbone_delta / _delta16: the route-delta stage over the same walk (arguments as
+    backbone_cells_device and routes_delta_device)."""
+    rs = next((x for x in l2 if x is not None), None)
+    st = _device_ptrs(border_status) if border_status is not None else None
+    route_table.call_stage(ctx, "hspf_isis_backbone_delta", rs, t.handle, n_jobs, *map(_planes_pair, l2),
+                           _device_ptrs(border_cells), st, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+
+
+def backbone_from_cells(l2: dict, t: BackboneTable, cells: np.ndarray, planes, entries) -> IsisRib:
+    """hspf_isis_backbone_from_cells (host): one job's cells -> the routes of the affected prefixes.  planes: R's two
+    (dist u32[V], hops u16[V]) or None (std, MT-IPv6; row 0); entries: per border the job's IPREACH_DT list
+    (l1_to_l2_from_cells).  rc HSPF_E_UNSUPPORTED is returned in the result."""
+    lib = capi.load_library()
+    cells = np.ascontiguousarray(cells, CELL_DT)
+    assert cells.shape == (t.n_prefixes,) and len(entries) == len(t.borders)
+    keep = [cells]
+    jp = (JobPlanesStruct * 2)()
+    for k in range(2):
+        if planes[k] is not None:
+            d, h = np.ascontiguousarray(planes[k][0], np.uint32), np.ascontiguousarray(planes[k][1], np.uint16)
+            keep += [d, h]
+            jp[k].dist, jp[k].hops = d.ctypes.data, h.ctypes.data
+    ents = [np.ascontiguousarray(e, IPREACH_DT) for e in entries]
+    keep += ents
+    ep = (C.c_void_p * len(ents))(*[e.ctypes.data if len(e) else None for e in ents])
+    ne = (C.c_uint32 * len(ents))(*[len(e) for e in ents])
+    tail = (t.handle, cells.ctypes.data if len(cells) else None, jp, ep, ne)
+    res = _call_rib(lib.hspf_isis_backbone_from_cells, l2, (), tail_args=tail)
+    if res.rc not in (capi.HSPF_OK, capi.HSPF_E_UNSUPPORTED):
+        raise capi.HspfError(res.rc, "hspf_isis_backbone_from_cells failed")
+    return res
+
+
 def _adjacencies(t: Topology, root: int, sys_of, usage: int):
     """Local interfaces and adjacencies of router `root` of topology t (router i is system sys_of(i))."""
     from . import ospfv3
@@ -972,7 +1066,8 @@ def l1l2_view(seed: int, n_l1: int = 150, n_l2: int = 120, n_border: int = 3, ro
     its router count.  The L1 area has l1_degree * n_l1 / 2 adjacencies (2: a tree and a few more).  Every L1/L2 router sets the ATT bit in its L1 LSP (the root only when
     `attached`) and carries in its own L2 LSP what lsp_propagate_l1_to_l2 puts there from its own L1 SPT with the
     configured `summaries`: the propagated entries and its active summaries.  Returns dict(l1, l2: the instance
-    images of L1/L2 router `root`, cfg, l2_derived: the mask of root's derived L2 entries, borders)."""
+    images of L1/L2 router `root`, cfg, l2_derived: the mask of root's derived L2 entries, borders, derived_all: the
+    mask of every border's derived L2 entries).  l1l2_backbone gives a backbone router's L2 image."""
     from . import ospfv3, synth
     kw = dict(cost_choices=cost_choices) if cost_choices else dict(cost_lo=1, cost_hi=20)
     t1 = synth.random_topology(n_l1, l1_degree * n_l1, synth.SEED_BASE + 1000 + seed, lan_fraction=0.1, **kw)
@@ -1069,11 +1164,14 @@ def l1l2_view(seed: int, n_l1: int = 150, n_l2: int = 120, n_border: int = 3, ro
         ent2[sysid(b) << 8] = ent2[sysid(b) << 8] + prop
     lv2 = finish(_with_ipreach(lv2, ent2))
     mask = np.zeros(len(lv2.ipreaches), np.uint8)
+    mask_all = np.zeros(len(lv2.ipreaches), np.uint8)
     for i in range(len(lv2.lsps)):
         lid = int(lv2.lsps["lan_id"][i])
-        if lid == sysid(root) << 8 and int(lv2.lsps["fragment"][i]) == 0:
+        if lid in derived and int(lv2.lsps["fragment"][i]) == 0:
             end = int(lv2.lsps["ipreach_off"][i]) + int(lv2.lsps["n_ipreach"][i])
-            mask[end - derived[lid]: end] = 1
+            mask_all[end - derived[lid]: end] = 1
+            if lid == sysid(root) << 8:
+                mask[end - derived[lid]: end] = 1
     i1, a1 = _adjacencies(t1, root, sysid, 1)
     if attached:                  # an up L2 adjacency into another area: is_l2_attached_to_backbone
         a1.append((sys2(n_border), (2, 0, 0, 9, 0, 1), 1, 2, 1, 1, 1, 1, 1, (0, 0, 0), 0xAC1F0001,
@@ -1084,7 +1182,18 @@ def l1l2_view(seed: int, n_l1: int = 150, n_l2: int = 120, n_border: int = 3, ro
     base = dict(system_id=sysid(root), max_paths=max_paths, level_type=3, att_ignore=0, mt_ipv6=int(mt6), sr_enabled=int(sr))
     l1 = dict(base, level=lv1, level_no=1, ifaces=np.array(i1, IFACE_DT), adjs=np.array(a1, ADJ_DT))
     l2 = dict(base, level=lv2, level_no=2, ifaces=np.array(i2, IFACE_DT), adjs=np.array(a2, ADJ_DT))
-    return dict(l1=l1, l2=l2, cfg=cfg, l2_derived=mask, borders=list(range(n_border)), t1=t1, t2=t2)
+    return dict(l1=l1, l2=l2, cfg=cfg, l2_derived=mask, borders=list(range(n_border)), t1=t1, t2=t2,
+                derived_all=mask_all)
+
+
+def l1l2_backbone(v: dict, i: int) -> dict:
+    """The level-2 instance image of backbone router i (>= the view's border count) of an l1l2_view domain: the same
+    L2 LSDB, level_type 2.  v["derived_all"] marks every border's derived entries in it."""
+    n_border, n_l1 = len(v["borders"]), v["t1"].n_routers
+    assert n_border <= i < v["t2"].n_routers
+    sys2 = lambda k: sysid(k) if k < n_border else sysid(n_l1 + k)
+    ifaces, adjs = _adjacencies(v["t2"], i, sys2, 2)
+    return dict(v["l2"], system_id=sys2(i), level_type=2, ifaces=np.array(ifaces, IFACE_DT), adjs=np.array(adjs, ADJ_DT))
 
 
 def summaries_of(l1_routes: np.ndarray, cfg: np.ndarray) -> np.ndarray:

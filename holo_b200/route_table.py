@@ -151,6 +151,15 @@ def declare(lib: C.CDLL):
         "hspf_isis_l1_to_l2_delta": [vp, vp, u32, res, res, u32, vp, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_isis_l1_to_l2_delta16": [vp, vp, u32, res16, res16, u32, vp, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_isis_l1_to_l2_from_cells": [C.POINTER(isis.InstanceStruct), vp, vp, vp, vp, u32, u32p],
+        "hspf_isis_backbone_table_create": [C.POINTER(isis.InstanceStruct), vp, u32, vp, pvp],
+        "hspf_isis_backbone_table_prefixes": [vp, u32p, pvp, pvp],
+        "hspf_isis_backbone_table_upload": [vp, vp],
+        "hspf_isis_backbone_cells": [vp, vp, u32, res, res, vp, vp, vp, vp],
+        "hspf_isis_backbone_cells16": [vp, vp, u32, res16, res16, vp, vp, vp, vp],
+        "hspf_isis_backbone_delta": [vp, vp, u32, res, res, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_isis_backbone_delta16": [vp, vp, u32, res16, res16, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_isis_backbone_from_cells": [C.POINTER(isis.InstanceStruct), vp, vp, C.POINTER(isis.JobPlanesStruct), vp,
+                                          vp, C.POINTER(isis.RibStruct)],
     }
     for name, argtypes in sigs.items():
         getattr(lib, name).argtypes = argtypes
@@ -161,5 +170,6 @@ def declare(lib: C.CDLL):
         for name in ("prefixes", "contributors"):
             getattr(lib, f"{table}_{name}").argtypes = [vp]
             getattr(lib, f"{table}_{name}").restype = u32
-    lib.hspf_isis_l1_to_l2_table_free.argtypes = [vp]
-    lib.hspf_isis_l1_to_l2_table_free.restype = None
+    for table in ("hspf_isis_l1_to_l2_table", "hspf_isis_backbone_table"):
+        getattr(lib, table + "_free").argtypes = [vp]
+        getattr(lib, table + "_free").restype = None

@@ -742,6 +742,86 @@ int hspf_isis_l1_to_l2_from_cells(const hl_isis_instance *l1, const hspf_isis_l1
                                   uint32_t cap, uint32_t *n_out);
 
 /*
+ * Backbone routers over L1 what-if jobs: the routes a level-2 router R outside an area gets from the area's L1/L2
+ * routers ("borders") when a job changes costs inside the area (isis_backbone_cells.h).  Each border re-originates
+ * its L2 LSP with the same IS reachability, so R's L2 SPT is its unperturbed one in every job, and only the
+ * prefixes that are keys of a border's L1 -> L2 table can route differently: the affected prefixes.  Every other
+ * prefix of R's table is the same in every job (hspf_isis_routes_batch over R's one row, or the host).  Out of
+ * scope: R a border of the area, and jobs that also change the L2 LSDB.
+ *
+ *   hspf_isis_backbone_table_create  `l2` R's level-2 instance image (level_type 2, or 3 when R is an L1/L2 router
+ *                             of another area); `derived` one byte per entry of l2->lvl.ipreaches (NULL: none set): a
+ *                             set byte marks an entry of a border's L2 LSP that propagation or an active summary put
+ *                             there; `borders` 1..8 L1 -> L2 tables (hspf_isis_l1_to_l2_table_create), which must
+ *                             outlive the table.  The table holds the affected prefixes in hl_isis_rib order, each
+ *                             with R's contributors in compute_routes' walk order over the LSDB where each border's
+ *                             derived entries are dropped and its job's entries are appended to its zeroth fragment:
+ *                             static entries read R's planes, and one slot per (border, key), at the border's vertex,
+ *                             reads that border's cell of the job.  L1 -> L2 keys are plain IPv6 (MT-IPv6 entries
+ *                             propagate as IPv6), so with MT-IPv6 enabled at R an IPv6 key gets no slot, as
+ *                             compute_routes reads no such entry there.
+ *                             HSPF_E_INVAL: wrong level or level type; 0 or more than 8 borders; R one of the
+ *                             borders; two tables of the same router; a border without a valid zeroth fragment of its
+ *                             non-pseudonode LSP in R's image; a derived byte outside a border's own non-pseudonode
+ *                             LSP, or on an entry whose (kind, prefix) is not among that border's keys.
+ *                             HSPF_E_UNSUPPORTED: a summary key of a border equal to a non-derived entry of its own
+ *                             LSP (propagation would overwrite that entry).
+ *   hspf_isis_backbone_table_prefixes  P, prefix[P], len[P]; any pointer may be NULL.
+ *   hspf_isis_backbone_table_upload  copies the table to the ctx's device.
+ *   hspf_isis_backbone_cells[16]  DEVICE planes of R's L2 batch (l2_std; l2_mt6 may be NULL unless R has an MT-IPv6
+ *                             root; the wide ones with nh_words == 1): only row 0, R's unperturbed SPT, is read.
+ *                             border_cells: host array of n_borders device pointers, border b's [n_jobs][K_b] cells
+ *                             as hspf_isis_l1_to_l2_cells[16] wrote them for the same job order (8-byte aligned);
+ *                             border_status: host array of n_borders device [n_jobs] status words (entries may be
+ *                             NULL), or NULL.  cells[n_jobs][P] (device): hl_isis_route_cell as
+ *                             hspf_isis_routes_batch's (lowest metric wins, equal metrics OR the next-hop atoms,
+ *                             HL_CELL_CONNECTED for the root, HL_CELL_MIXED_SID for SR-relevant best contributions
+ *                             from two vertices, e.g. two tying borders); winner: a static contributor's index, or
+ *                             for a slot the table's contributor count + one index per (slot, border record), so a
+ *                             new winning record at an equal metric is a new winner.  job_status_out (device
+ *                             [n_jobs], or NULL): the OR of R's row-0 status words and the job's border status words;
+ *                             a job with a non-zero status gets empty cells.  Nothing is launched for 0 jobs.
+ *                             Enqueued on the ctx stream; no synchronisation.
+ *   hspf_isis_backbone_delta[16]  the route-delta stage (below) over the same walk: LOST, GAINED, METRIC, NEXTHOPS
+ *                             (another border takes over), OTHER.
+ *   hspf_isis_backbone_from_cells  host: one job's cells -> exactly the routes of the affected prefixes that
+ *                             hspf_isis_routes_from_planes gives over R's planes in the LSDB where each border's
+ *                             derived entries are replaced by entries[b] (n_entries[b] of them), that border's
+ *                             hspf_isis_l1_to_l2_from_cells output for the job, appended to its zeroth fragment.
+ *                             planes[2]: R's planes of the standard and MT-IPv6 topologies (row 0, no overrides).
+ *                             A slot's route takes its external bit and Prefix-SID from the border's entry.
+ *                             HSPF_E_UNSUPPORTED for an HL_CELL_MIXED_SID cell, as hspf_isis_routes_from_cells.
+ */
+typedef struct hspf_isis_backbone_table hspf_isis_backbone_table;
+int hspf_isis_backbone_table_create(const hl_isis_instance *l2, const uint8_t *derived, uint32_t n_borders,
+                                    const hspf_isis_l1_to_l2_table *const *borders, hspf_isis_backbone_table **out);
+void hspf_isis_backbone_table_free(hspf_isis_backbone_table *t);
+int hspf_isis_backbone_table_prefixes(const hspf_isis_backbone_table *t, uint32_t *n_prefixes,
+                                      const hl_ip_addr **prefix, const uint8_t **len);
+int hspf_isis_backbone_table_upload(hspf_ctx *ctx, hspf_isis_backbone_table *t);
+int hspf_isis_backbone_cells(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs,
+                             const hspf_result *l2_std, const hspf_result *l2_mt6,
+                             const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
+                             uint32_t *job_status_out, hl_isis_route_cell *cells);
+int hspf_isis_backbone_cells16(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs,
+                               const hspf_result16 *l2_std, const hspf_result16 *l2_mt6,
+                               const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
+                               uint32_t *job_status_out, hl_isis_route_cell *cells);
+int hspf_isis_backbone_delta(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs,
+                             const hspf_result *l2_std, const hspf_result *l2_mt6,
+                             const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
+                             const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                             hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_isis_backbone_delta16(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs,
+                               const hspf_result16 *l2_std, const hspf_result16 *l2_mt6,
+                               const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
+                               const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                               hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_isis_backbone_from_cells(const hl_isis_instance *l2, const hspf_isis_backbone_table *t,
+                                  const hl_isis_route_cell *cells, const hspf_isis_job_planes *planes,
+                                  const hl_isis_ipreach *const *entries, const uint32_t *n_entries, hl_isis_rib *out);
+
+/*
  * Route-delta stage on the device: which prefixes each job of a what-if batch loses, gains, or reaches at another
  * metric or over another next-hop set, against a base route table — without storing the n_jobs x P cell matrix.
  * Per (job, prefix) it runs the same walk as hspf_*_routes_batch[16] and compares the cell with the job's base cell
