@@ -1,0 +1,159 @@
+// Routing table of an OSPFv2 backbone router R for a batch of what-if jobs inside other areas, one cell per (job,
+// affected prefix) (include/holo_spf_lsdb.h, hspf_ospfv2_backbone_table_create).
+//
+// A job changes costs only in the non-backbone areas of the area border routers given as "borders".  R is an
+// internal router of area 0, so its area-0 SPT is its unperturbed one in every job, and only the type-3 LSAs the
+// borders originate into area 0 change.  Only a prefix some border can advertise (one with an intra-area record in
+// one of the border's non-backbone areas) can route differently at R.  Per such prefix the walk is
+// ospf_rib_cell_eval (ospf_rib_cells.h) over R's row 0, with each border's type-3 LSA for the prefix replaced by a
+// slot at that border's place in LsaKey order:
+//   * a static type-3 record reads R's planes as before (dist[abr] + metric);
+//   * a slot reads the border's routing-table cell of the job (ospf_abr_rib_cells.h) and stands for the LSA
+//     compute_net_summaries (holo-ospf area.rs:561-659) originates into the backbone: the cell is present and
+//     intra-area, its winner is not one of area 0's intra-area records (route.area_id != 0), none of its atoms is an
+//     area-0 atom (nexthops_area_check, area.rs:742) and its metric is below LSInfinity.  Then it offers
+//     dist[border] + the cell's metric.
+// The lowest metric wins and equal metrics OR their atoms, the first record staying the winner.  A slot's winner
+// is n_recs + its slot index, so the decode can tell it from a static record.
+#pragma once
+#include <cstdint>
+#include <vector>
+
+#include "ospf_abr_rib_cells.h"
+
+namespace hspf {
+
+constexpr uint32_t kOspfBackboneMaxBorders = 8;
+constexpr uint32_t kOspfBackboneStatic = 0xFFFFFFFFu;   // RibRec::z of a static type-3 record
+
+// Type-3 records of the backbone table, beside R's one-area records (ospf_rib_cells.h):
+//   static: x ABR vertex, y LSA metric, z kOspfBackboneStatic
+//   slot:   x the border's vertex, y the prefix's index in the border's table, z the border, w the slot index
+
+// What the walk reads of a table.  Per border b, border[4 b ..]: its area-0 intra-area records [lo, hi) and its
+// area-0 atom bits (low word, high word).
+struct OspfBackboneView {
+    const uint32_t *oi;           // [PR + 1] R's intra-area ranges (R's one-area table)
+    const uint32_t *q;            // [P] the prefix's index in R's one-area table, kNoRecord if none
+    const uint32_t *o3;           // [P + 1] type-3 ranges (statics and slots)
+    const uint32_t *o5;           // [P + 1] type-5 ranges
+    const uint32_t *border;       // [4 n_borders]
+    const RibRec *recs;
+    uint32_t P, n_recs, root;
+};
+
+// One job's row of every border's cells.
+struct OspfBorderRows {
+    const hl_ospf_rib_cell *row[kOspfBackboneMaxBorders];
+};
+
+// What border b advertises into area 0 for the prefix of its cell c: false when nothing, else its metric.
+HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, uint32_t b, uint32_t &metric) {
+#if defined(__CUDA_ARCH__)
+    const unsigned long long *w = reinterpret_cast<const unsigned long long *>(c);
+    const uint64_t wm = __ldg(w + 2), nh = __ldg(w);
+    const uint4 bb = __ldg(reinterpret_cast<const uint4 *>(border) + b);
+#else
+    const uint64_t wm = (uint64_t)c->winner | ((uint64_t)c->mpf << 32), nh = c->nh_mask;
+    const struct { uint32_t x, y, z, w; } bb = {border[4 * b], border[4 * b + 1], border[4 * b + 2], border[4 * b + 3]};
+#endif
+    const uint32_t winner = (uint32_t)wm, mpf = (uint32_t)(wm >> 32);
+    const uint64_t atoms0 = (uint64_t)bb.z | ((uint64_t)bb.w << 32);
+    metric = mpf & HL_RIB_CELL_METRIC_MAX;
+    return ((mpf >> 28) & HL_CELL_PRESENT) && ((mpf >> 26) & 0x3u) == HL_PATH_INTRA_AREA &&
+           (winner < bb.x || winner >= bb.y) && !(nh & atoms0) && metric < HL_LSA_INFINITY;
+}
+
+template <class Planes>
+HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneView &t, uint32_t p,
+                                          const OspfBorderRows &rows) {
+    const RouteContrib *contribs = reinterpret_cast<const RouteContrib *>(t.recs);
+    const uint32_t q = t.q[p];
+    if (q != kNoRecord) {                                               // 1. intra-area
+        const hl_route_cell c = route_cell_eval(pl, contribs, t.oi[q], t.oi[q + 1]);
+        if (c.flags & HL_CELL_PRESENT)
+            return {c.nh_mask, c.lasthop_mask, (uint64_t)c.winner | ((uint64_t)rib_mpf(c.metric, HL_PATH_INTRA_AREA, c.flags) << 32)};
+    }
+    uint64_t mask = 0;
+    uint32_t win = kNoRecord, metric = 0;
+    for (uint32_t i = t.o3[p]; i < t.o3[p + 1]; ++i) {                  // 2. inter-area, slots in LsaKey order
+        const RibRec r = load_rib_rec(t.recs + i);
+        if (!pl.reached(r.x)) continue;
+        uint32_t y = r.y, w = i;
+        if (r.z != kOspfBackboneStatic) {
+            if (!border_summary(rows.row[r.z] + r.y, t.border, r.z, y)) continue;
+            w = t.n_recs + r.w;
+        }
+        const uint32_t m = pl.d(r.x) + y;
+        if (win == kNoRecord || m < metric) { win = w; metric = m; mask = pl.n(r.x); }
+        else if (m == metric) mask |= pl.n(r.x);
+    }
+    if (win != kNoRecord)
+        return {mask, 0, (uint64_t)win | ((uint64_t)rib_mpf(metric, HL_PATH_INTER_AREA, HL_CELL_PRESENT) << 32)};
+    uint32_t path = 0, type2 = 0;
+    for (uint32_t i = t.o5[p]; i < t.o5[p + 1]; ++i) {                  // 3. AS-external, as ospf_rib_cell_eval
+        const RibRec r = load_rib_rec(t.recs + i);
+        const RibRec s = load_rib_rec(t.recs + r.x);
+        if (s.x == t.root) continue;
+        uint32_t em = 0;
+        uint64_t en = 0;
+        bool have = false;
+        for (uint32_t k = s.w; k > s.z; --k) {
+            const RibRec f = load_rib_rec(t.recs + k - 1);
+            if (f.x == t.root || !pl.reached(f.x)) continue;
+            em = pl.d(f.x) + f.y; en = pl.n(f.x); have = true;
+            break;
+        }
+        if (!have) {
+            if (!s.y || !pl.reached(s.x)) continue;
+            em = pl.d(s.x); en = pl.n(s.x);
+        }
+        const uint32_t cp = r.z ? HL_PATH_TYPE2_EXTERNAL : HL_PATH_TYPE1_EXTERNAL;
+        const uint32_t cm = r.z ? em : em + r.y, c2 = r.z ? r.y : 0;
+        int cmp = -1;
+        if (win != kNoRecord) {
+            if (cp != path) cmp = cp < path ? -1 : 1;
+            else if (cp == HL_PATH_TYPE2_EXTERNAL && c2 != type2) cmp = c2 < type2 ? -1 : 1;
+            else cmp = cm < metric ? -1 : (cm == metric ? 0 : 1);
+        }
+        if (cmp < 0) { win = i; path = cp; metric = cm; type2 = c2; mask = en; }
+        else if (cmp == 0) mask |= en;
+    }
+    if (win == kNoRecord) return {0, 0, (uint64_t)kNoRecord};
+    return {mask, type2, (uint64_t)win | ((uint64_t)rib_mpf(metric, path, HL_CELL_PRESENT) << 32)};
+}
+
+}  // namespace hspf
+
+// Host + device image of a backbone router's affected prefixes (include/holo_spf_lsdb.h).
+struct hspf_ospfv2_backbone_table {
+    hspf_ospfv2_ribtable *r = nullptr;           // R's one-area table over area 0 without the borders' type-3 LSAs
+    uint32_t router_id = 0, root = 0, n_vertices = 0, n_borders = 0, max_paths = 0;
+    std::vector<uint32_t> prefix, plen;          // [P] prefix order
+    std::vector<uint32_t> words;                 // oi [PR + 1], q [P], o3 [P + 1], o5 [P + 1], padding, border [4 n_borders]
+    std::vector<hspf::RibRec> recs;              // R's records, then the type-3 and type-5 records of the view
+    std::vector<uint32_t> slot_rec;              // [n_slots] the record of each slot
+    std::vector<uint32_t> ext_tag;               // per type-5 record of the view (index - ext_base)
+    uint32_t ext_base = 0;
+    const hspf_ospfv2_abr_ribtable *borders[hspf::kOspfBackboneMaxBorders] = {};
+    hspf::DeviceRouteTable dev;                  // hspf_ospfv2_backbone_table_upload: words, then records
+
+    uint32_t P() const { return (uint32_t)prefix.size(); }
+    // the border words start on a 16-byte boundary (one 16-byte load per border)
+    size_t border_at() const { return ((r->prefix.size() + 1 + 3 * (size_t)P() + 2) + 3) & ~(size_t)3; }
+    hspf::OspfBackboneView view(const uint32_t *w, const hspf::RibRec *rc) const {
+        const uint32_t PR = (uint32_t)r->prefix.size(), n = P();
+        hspf::OspfBackboneView v;
+        v.oi = w;
+        v.q = w + PR + 1;
+        v.o3 = v.q + n;
+        v.o5 = v.o3 + n + 1;
+        v.border = w + border_at();
+        v.recs = rc;
+        v.P = n;
+        v.n_recs = (uint32_t)recs.size();
+        v.root = root;
+        return v;
+    }
+    hspf::OspfBackboneView host_view() const { return view(words.data(), recs.data()); }
+};

@@ -16,6 +16,7 @@
 #include <array>
 #include <cstdint>
 #include <cstring>
+#include <map>
 #include <new>
 #include <unordered_map>
 #include <vector>
@@ -448,6 +449,77 @@ extern "C" int hspf_ospfv3_update_rib_full(uint32_t router_id, uint32_t max_path
                                            uint32_t n_areas, const hl_ospfv3_external_lsa *ext, uint32_t n_ext,
                                            hl_ospfv3_rib *out) {
     return guarded<V3>(router_id, max_paths, areas, n_areas, ext, n_ext, out);
+}
+
+// compute_net_summaries / compute_rtr_summaries (holo-ospf area.rs:561-740) of an ABR for one target area, without
+// area ranges and without LSA ids: each map keyed as the reference's summary tables, a later entry replacing
+// an earlier one
+extern "C" int hspf_ospfv2_net_summaries(uint32_t router_id, const hl_ospfv2_rib *rib, const hl_ospfv2_rtr_tables *rtrs,
+                                         const hl_ospfv2_rib_area *areas, const hl_ospf_area_config *config,
+                                         uint32_t n_areas, uint32_t target, hl_ospfv2_summary_lsa *out, uint32_t cap,
+                                         uint32_t *n_out) {
+    if (!rib || !rtrs || !areas || !config || !n_out || target >= n_areas || (cap && !out)) return HSPF_E_INVAL;
+    if ((rib->n_routes && !rib->routes) || (rib->n_nexthops && !rib->nexthops)) return HSPF_E_INVAL;
+    if ((rtrs->n_rtrs && !rtrs->rtrs) || (rtrs->n_nexthops && !rtrs->nexthops)) return HSPF_E_INVAL;
+    for (uint32_t i = 0; i < rib->n_routes; ++i)
+        if ((uint64_t)rib->routes[i].nh_off + rib->routes[i].n_nh > rib->n_nexthops) return HSPF_E_INVAL;
+    for (uint32_t i = 0; i < rtrs->n_rtrs; ++i)
+        if ((uint64_t)rtrs->rtrs[i].nh_off + rtrs->rtrs[i].n_nh > rtrs->n_nexthops) return HSPF_E_INVAL;
+    for (uint32_t i = 0; i < n_areas; ++i)
+        if (areas[i].n_ifaces && !areas[i].ifaces) return HSPF_E_INVAL;
+    try {
+        *n_out = 0;
+        std::map<std::pair<uint32_t, uint32_t>, uint32_t> net;        // (prefix, mask) -> metric
+        std::map<uint32_t, uint32_t> rtr;                             // ASBR id -> metric
+        uint32_t n_active = 0;
+        for (uint32_t i = 0; i < n_areas; ++i) n_active += areas[i].active ? 1u : 0u;
+        const hl_ospfv2_rib_area &ta = areas[target];
+        const hl_ospf_area_config &cfg = config[target];
+        const bool backbone = ta.area_id == 0;
+        // nexthops_area_check: a next hop on one of the target area's interfaces (next hops name them by sort key)
+        auto on_area = [&](const hl_nexthop *h, uint32_t n) {
+            for (uint32_t k = 0; k < n; ++k)
+                for (uint32_t i = 0; i < ta.n_ifaces; ++i)
+                    if (h[k].iface == ta.ifaces[i].sort_key) return true;
+            return false;
+        };
+        if (n_active > 1) {                                           // only ABRs originate summaries
+            if (cfg.summary)
+                for (uint32_t i = 0; i < rib->n_routes; ++i) {
+                    const hl_rib_route &r = rib->routes[i];
+                    if (r.path_type >= HL_PATH_TYPE1_EXTERNAL || r.metric >= HL_LSA_INFINITY) continue;
+                    if (r.has_area && r.area_id == ta.area_id) continue;
+                    if (backbone && r.path_type != HL_PATH_INTRA_AREA) continue;
+                    if (on_area(rib->nexthops + r.nh_off, r.n_nh)) continue;
+                    net[{r.prefix, r.mask}] = r.metric;
+                }
+            if (cfg.area_type != HL_AREA_NORMAL) net[{0u, 0u}] = cfg.default_cost;
+            if (cfg.area_type == HL_AREA_NORMAL)
+                for (uint32_t i = 0; i < rtrs->n_rtrs; ++i) {
+                    const hl_rib_rtr &r = rtrs->rtrs[i];
+                    if (r.area_id == ta.area_id || !(r.flags & HL_RTR_FLAG_E) || r.metric >= HL_LSA_INFINITY) continue;
+                    if (backbone && r.path_type != HL_PATH_INTRA_AREA) continue;
+                    if (on_area(rtrs->nexthops + r.nh_off, r.n_nh)) continue;
+                    rtr[r.router_id] = r.metric;
+                }
+        }
+        *n_out = (uint32_t)(net.size() + rtr.size());
+        if (*n_out > cap) return HSPF_E_NOMEM;
+        uint32_t k = 0;
+        auto put = [&](uint8_t type, uint32_t id, uint32_t mask, uint32_t metric) {
+            hl_ospfv2_summary_lsa l;
+            std::memset(&l, 0, sizeof(l));
+            l.adv_rtr = router_id; l.lsa_id = id; l.mask = mask; l.metric = metric; l.lsa_type = type;
+            out[k++] = l;
+        };
+        for (const auto &e : net) put(3, e.first.first, e.first.second, e.second);
+        for (const auto &e : rtr) put(4, e.first, 0, e.second);
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
 }
 
 extern "C" int hspf_ospfv2_rib_diff(const hl_ospfv2_rib *old_rib, hl_ospfv2_rib *new_rib, hl_rib_action *out, uint32_t cap,

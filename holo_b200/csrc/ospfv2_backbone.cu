@@ -1,0 +1,127 @@
+// Device stage for the routing table of an OSPFv2 backbone router over what-if jobs inside other areas
+// (include/holo_spf_lsdb.h, "backbone router over what-if jobs inside other areas"): update_rib_full at the router,
+// for its affected prefixes, with every border's type-3 LSAs in area 0 re-originated for the job.
+//
+// One launch on the ctx stream: one thread per (job, prefix) runs ospf_backbone_cell_eval (ospf_backbone_cells.h)
+// over the router's unperturbed area-0 planes (row 0) and the job's row of each border's routing-table cells, and
+// the shared cell kernel or the route-delta stage (route_stage.cuh) stores or compares the 24-byte cells.
+#include <cstring>
+#include <vector>
+
+#include "../../include/holo_spf_lsdb.h"
+#include "ospf_backbone_cells.h"
+#include "route_stage.cuh"
+
+namespace {
+
+using hspf::kOspfBackboneMaxBorders;
+
+template <class Planes>
+struct OspfBackboneCell {
+    using Rows = hspf::ResultPlanes<Planes>;
+    hspf::OspfBackboneView t;
+    Rows pl;                                                      // R's area-0 batch; only row 0 is read
+    const hl_ospf_rib_cell *cells[kOspfBackboneMaxBorders];       // [n_jobs][K_b] per border
+    const uint32_t *status[kOspfBackboneMaxBorders];              // [n_jobs] per border, or NULL
+    uint32_t K[kOspfBackboneMaxBorders];
+    uint32_t n_borders;
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
+        uint32_t s = pl.status_word(0);
+        for (uint32_t b = 0; b < n_borders; ++b)
+            if (status[b]) s |= status[b][j];
+        return s;
+    }
+    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = cells[b] + (size_t)j * K[b];
+        return hspf::ospf_backbone_cell_eval(pl.job(0), t, p, rows);
+    }
+    __device__ __forceinline__ uint64_t gather(uint32_t, uint32_t, uint32_t) const { return 0; }   // row 0: host side
+    __device__ static hspf::CellWords empty() { return {0, 0, hspf::kNoRecord}; }
+};
+
+// Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6).
+constexpr uint32_t kBackboneBlocksPerSM = 4;
+
+template <class R>
+int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
+              const uint32_t *const *border_status, OspfBackboneCell<hspf::PlanesOf<R>> &cell) {
+    if (!t || !t->dev.blob || !border_cells) return HSPF_E_INVAL;
+    if (hspf::result_planes(planes, t->n_vertices, cell.pl) || !cell.pl.complete()) return HSPF_E_INVAL;
+    for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
+        cell.cells[b] = nullptr; cell.status[b] = nullptr; cell.K[b] = 0;
+        if (b >= t->n_borders) continue;
+        // the border's cells, 8-byte words of 24-byte cells
+        if (!border_cells[b] || (reinterpret_cast<uintptr_t>(border_cells[b]) & 7u)) return HSPF_E_INVAL;
+        cell.cells[b] = border_cells[b];
+        cell.status[b] = border_status ? border_status[b] : nullptr;
+        cell.K[b] = (uint32_t)t->borders[b]->prefix.size();
+    }
+    cell.n_borders = t->n_borders;
+    cell.t = t->view(t->dev.off, static_cast<const hspf::RibRec *>(t->dev.contribs));
+    return HSPF_OK;
+}
+
+template <class R>
+int backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    OspfBackboneCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
+    return hspf::launch_route_cells<kBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out, 0,
+                                                          nullptr, nullptr, nullptr, nullptr);
+}
+
+template <class R>
+int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    OspfBackboneCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
+    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBackboneBlocksPerSM>(
+        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+}  // namespace
+
+extern "C" {
+
+int hspf_ospfv2_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_backbone_table *t) {
+    if (!t) return HSPF_E_INVAL;
+    return hspf::upload_route_table(ctx, t->dev, t->words, t->recs.data(), t->recs.size() * sizeof(hspf::RibRec));
+}
+
+int hspf_ospfv2_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                               const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                               const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+}
+
+int hspf_ospfv2_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+}
+
+int hspf_ospfv2_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                               const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                               const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                               const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
+                               uint64_t cap, uint64_t *n_records) {
+    return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
+                          records, cap, n_records);
+}
+
+int hspf_ospfv2_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells,
+                                 uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                                 hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
+                          records, cap, n_records);
+}
+
+}  // extern "C"

@@ -552,3 +552,127 @@ def abr_rib_from_cells_v3(areas: list, rt: AbrRibTable, cells: np.ndarray, gathe
     from . import ospfv3
     return _call_abr_rib_from_cells(capi.load_library().hspf_ospfv3_abr_rib_from_cells, ospfv3.AreaStruct, areas, rt,
                                     cells, gather_area, gather_v, gather_nh, RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)
+
+
+# ---- Summary-LSA origination of an area border router (include/holo_spf_lsdb.h) ----------------------------------
+AREA_NORMAL, AREA_STUB, AREA_NSSA = 0, 1, 2
+AREA_CONFIG_DT = np.dtype([("default_cost", "<u4"), ("area_type", "u1"), ("summary", "u1"), ("_pad", "u1", (2,))],
+                          align=True)
+
+
+def area_config(area_type: int = AREA_NORMAL, summary: bool = True, default_cost: int = 10):
+    """One hl_ospf_area_config: the reference's defaults are a normal area with summaries and default cost 10."""
+    return (default_cost, area_type, int(summary), (0, 0))
+
+
+def net_summaries(router_id: int, rib: Rib, rtrs: RtrTables, areas: list, configs: list, target: int) -> np.ndarray:
+    """hspf_ospfv2_net_summaries (host): the type-3 and type-4 contents the router originates into areas[target]
+    (compute_net_summaries / compute_rtr_summaries), as SUMMARY_LSA_DT[] with adv_rtr = router_id and lsa_id the
+    prefix address (type 3) or the ASBR id (type 4): type 3 in prefix order, then type 4 in router-id order.
+    rib: update_rib_full's table; rtrs: router_tables' over the same areas (RibArea list); configs: one area_config()
+    per area."""
+    lib = capi.load_library()
+    keep = []
+    arr = _area_array(areas, keep, False)
+    cfg = np.asarray(list(configs) or [area_config()], AREA_CONFIG_DT)
+    rs = _rib_struct(rib, keep, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)
+    prt = np.ascontiguousarray(rtrs.rtrs, RIB_RTR_DT)
+    pnh = np.ascontiguousarray(rtrs.nexthops, ospfv2.NEXTHOP_DT)
+    ts = RtrTablesStruct(len(prt), len(prt), prt.ctypes.data if len(prt) else None, len(pnh), len(pnh),
+                         pnh.ctypes.data if len(pnh) else None)
+    cap = len(rib.routes) + len(prt) + 1
+    out = np.zeros(cap, SUMMARY_LSA_DT)
+    n = C.c_uint32()
+    rc = lib.hspf_ospfv2_net_summaries(router_id, C.byref(rs), C.byref(ts), arr, cfg.ctypes.data, len(areas), target,
+                                       out.ctypes.data, cap, C.byref(n))
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, "hspf_ospfv2_net_summaries failed")
+    return out[: n.value].copy()
+
+
+# ---- backbone router over what-if jobs inside other areas (include/holo_spf_lsdb.h) -----------------------------
+BACKBONE_MAX_BORDERS = 8           # HSPF_BACKBONE_MAX_BORDERS
+
+
+class BackboneTable:
+    """hspf_ospfv2_backbone_table of one internal backbone router R: its affected prefixes over what-if jobs inside
+    the borders' other areas.  `flat`: R's area-0 ospfv2.Flat; `summaries`: area 0's SUMMARY_LSA_DT[] in LsaKey order;
+    `externals`: EXTERNAL_LSA_DT[]; `borders`: the borders' AbrRibTable list (kept alive with this table).  `prefix`,
+    `plen` [n_prefixes]: the affected prefixes in prefix order; a slot's winner is n_records + its slot index
+    (n_slots in all)."""
+
+    def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=()):
+        self.lib = capi.load_library()
+        self.flat, self.router_id, self.borders = flat, router_id, list(borders)
+        sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        self.summaries, self.externals = sm, ext
+        arr = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
+        h = C.c_void_p()
+        rc = self.lib.hspf_ospfv2_backbone_table_create(flat.handle, router_id, sm.ctypes.data if len(sm) else None,
+                                                        len(sm), ext.ctypes.data if len(ext) else None, len(ext), arr,
+                                                        len(self.borders), C.byref(h))
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, "hspf_ospfv2_backbone_table_create failed")
+        self.handle = h
+        n, pp, pl = C.c_uint32(), C.c_void_p(), C.c_void_p()
+        assert self.lib.hspf_ospfv2_backbone_table_prefixes(h, C.byref(n), C.byref(pp), C.byref(pl)) == capi.HSPF_OK
+        self.n_prefixes = n.value
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, np.uint32)
+        self.plen = route_table.copy_records(pl, self.n_prefixes, np.uint32)
+        nr, ns = C.c_uint32(), C.c_uint32()
+        assert self.lib.hspf_ospfv2_backbone_table_records(h, C.byref(nr), C.byref(ns)) == capi.HSPF_OK
+        self.n_records, self.n_slots = nr.value, ns.value
+
+    def upload(self, ctx: capi.Context):
+        rc = self.lib.hspf_ospfv2_backbone_table_upload(ctx.handle, self.handle)
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, ctx.last_error())
+
+    def __del__(self):
+        try:
+            if self.handle:
+                self.lib.hspf_ospfv2_backbone_table_free(self.handle)
+                self.handle = None
+        except Exception:
+            pass
+
+
+def _device_ptrs(ptrs):
+    return (C.c_void_p * max(len(ptrs), 1))(*[int(p) or None for p in ptrs])
+
+
+def backbone_cells_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
+                          status_ptr: int, cells_ptr: int):
+    """hspf_ospfv2_backbone_cells / _cells16 over DEVICE planes.  rs: R's area-0 capi.ResultStruct (nh_words 1) or
+    capi.Result16Struct, only row 0 read; border_cells: per border a device pointer to its [n_jobs, K_b] RIB_CELL_DT
+    ABR cells; border_status: per border a device u32 [n_jobs] pointer or 0 (None: none); status_ptr: device u32
+    [n_jobs] or 0; cells_ptr: device [n_jobs, t.n_prefixes] RIB_CELL_DT.  Enqueued on the ctx stream; the table must
+    have been uploaded."""
+    st = _device_ptrs(border_status) if border_status is not None else None
+    route_table.call_stage(ctx, "hspf_ospfv2_backbone_cells", rs, t.handle, n_jobs, C.byref(rs),
+                           _device_ptrs(border_cells), st, status_ptr or None, cells_ptr or None)
+
+
+def backbone_delta_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
+                          base_ptr: int, n_base: int, base_of_ptr: int, job_out_ptr: int, records_ptr: int, cap: int,
+                          n_records_ptr: int):
+    """hspf_ospfv2_backbone_delta / _delta16: the route-delta stage over the same walk (arguments as
+    backbone_cells_device and rib_delta_device)."""
+    st = _device_ptrs(border_status) if border_status is not None else None
+    route_table.call_stage(ctx, "hspf_ospfv2_backbone_delta", rs, t.handle, n_jobs, C.byref(rs),
+                           _device_ptrs(border_cells), st, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+
+
+def backbone_from_cells(area: ospfv2.Ospfv2Area, t: BackboneTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv2_backbone_from_cells (host): one job's cells -> R's routes for the affected prefixes.  area: R's
+    area-0 image; gathers of R's row 0.  rc HSPF_E_UNSUPPORTED is returned in the result, as rib_from_cells."""
+    cells = np.ascontiguousarray(cells, RIB_CELL_DT)
+    assert cells.shape == (t.n_prefixes,)
+    gv = np.ascontiguousarray(gather_v, np.uint32)
+    gn = np.ascontiguousarray(gather_nh, np.uint64)
+    s = area.as_struct()
+    return _call_rib(capi.load_library().hspf_ospfv2_backbone_from_cells,
+                     (t.handle, C.byref(s), cells.ctypes.data, gv.ctypes.data, gn.ctypes.data, len(gv)),
+                     t.n_prefixes, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)

@@ -754,3 +754,131 @@ def abr_view(topos: list, seed: int, area_ids=None, roots=None, max_paths: int =
         summaries[0] = np.asarray(s0, ospf_rib.SUMMARY_LSA_DT)
     ext_rows.sort(key=lambda x: (x[0], x[1]))
     return areas, summaries, np.asarray(ext_rows, ospf_rib.EXTERNAL_LSA_DT)
+
+
+def _area_remap(a: Ospfv2Area, k: int, idmap: dict) -> Ospfv2Area:
+    """A copy of synth_area's image as area k of a multi-area domain: router ids moved up by k << 20, then renamed by
+    idmap (the routers of this area that are also routers of area 0 keep their area-0 ids), p2p and LAN addresses,
+    interface sort keys and ifindexes moved into ranges of area k."""
+    a = Ospfv2Area(**{f: getattr(a, f) for f in a.__dataclass_fields__})
+
+    def rmap(x):
+        x = np.asarray(x, np.uint64)
+        out = np.where((x >> 24) == 10, x + (k << 20), x)
+        for old, new in idmap.items():
+            out = np.where(out == old + (k << 20), new, out)
+        out = np.where((x >> 20) == (P2P_BASE >> 20), x + (k << 18), out)
+        out = np.where((x >> 16) == (LAN_BASE >> 16), x + (k << 16), out)
+        return out.astype(np.uint32)
+
+    a.router_id = int(rmap([a.router_id])[0])
+    a.area_id = k
+    rl = a.router_lsas.copy()
+    rl["adv_rtr"], rl["lsa_id"] = rmap(rl["adv_rtr"]), rmap(rl["lsa_id"])
+    links = a.links.copy()
+    links["link_id"] = rmap(links["link_id"])
+    non_stub = links["link_type"] != LINK_STUB
+    links["link_data"] = np.where(non_stub, rmap(links["link_data"]), links["link_data"])
+    nl = a.network_lsas.copy()
+    nl["adv_rtr"], nl["lsa_id"] = rmap(nl["adv_rtr"]), rmap(nl["lsa_id"])
+    a.attached = rmap(a.attached)
+    nb = a.nbrs.copy()
+    for f in nb.dtype.names:
+        if nb.dtype[f] == np.uint32:
+            nb[f] = rmap(nb[f])
+    ia = a.iface_addrs.copy()
+    ia["addr"] = rmap(ia["addr"])
+    ifs = a.ifaces.copy()
+    ifs["sort_key"] += 1000 * k
+    ifs["ifindex"] += 1000 * k
+    order = np.lexsort((rl["lsa_id"], rl["adv_rtr"]))
+    a.router_lsas, a.links, a.nbrs, a.iface_addrs, a.ifaces = rl[order], links, nb, ia, ifs
+    a.network_lsas = nl[np.lexsort((nl["lsa_id"], nl["adv_rtr"]))] if len(nl) else nl
+    return a
+
+
+def _set_flags(a: Ospfv2Area, flags: dict) -> Ospfv2Area:
+    rl = a.router_lsas.copy()
+    for rid, f in flags.items():
+        rl["flags"][rl["adv_rtr"] == rid] |= f
+    a.router_lsas = rl
+    return a
+
+
+def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1, 0), (2, 1), (3, 2)),
+                  max_paths: int = 16, n_ext_keys: int = 3):
+    """A backbone router R of area 0 and the area border routers ("borders") of one other area 1, each as its own
+    image.  Seeded.  Area 0 is synth_area(t0) (router i is RID_BASE + i), area 1 synth_area(t1) moved into ranges of
+    its own, except that border (i0, i1) is router i0 of t0 and router i1 of t1, with one router id and the B flag in
+    both areas.  Returns a dict:
+      r_area        R's area-0 image (router r of t0);
+      summaries0    area 0's type-3 LSAs (LsaKey order): each border's for the area-1 stub prefixes it reaches, at
+                    its distance plus the stub metric (what a job replaces);
+      externals     an ASBR of area 0 (the E flag) with type-5 LSAs for n_ext_keys area-1 loopbacks (prefixes that
+                    are also keys) and for one prefix of its own;
+      borders       per border (areas [area 0 image, area 1 image], area ids, summaries per area) in that area order,
+                    except that the first border lists area 1 first;
+      shared        a /24 that is a stub of a neighbour of the first border in area 0 and in area 1, at metrics that
+                    tie at that border (its route there is intra-area in both areas and carries area-0 atoms)."""
+    from . import ospf_rib
+    rng = np.random.default_rng(seed)
+    rid0 = lambda i: RID_BASE + int(i)
+    idmap = {rid0(i1): rid0(i0) for i0, i1 in borders}
+    bids = [rid0(i0) for i0, _ in borders]
+    cand = [i for i in range(t0.n_routers) if i != r and rid0(i) not in bids]
+    asbr = rid0(cand[int(rng.integers(0, len(cand)))])
+    f0 = {b: 0x01 for b in bids}
+    f0[asbr] = 0x02
+    img0 = lambda i: _set_flags(synth_area(t0, root=i, max_paths=max_paths), f0)
+    img1 = lambda i: _set_flags(_area_remap(synth_area(t1, root=i, max_paths=max_paths), 1, idmap), {b: 0x01 for b in bids})
+    r_area = img0(r)
+    b0 = [img0(i0) for i0, _ in borders]
+    b1 = [img1(i1) for _, i1 in borders]
+    # the shared prefix: a nearest neighbour of the first border in each area, at metrics that tie there
+    def nearest(a):
+        fl = Flat(a)
+        d = _dist_from(fl, fl.router_vertex(a.router_id))
+        vs = [v for v in range(len(fl.ids)) if fl.is_router[v] and 0 < d[v] < 1 << 40]
+        v = min(vs, key=lambda v: (int(d[v]), int(fl.ids[v])))
+        return int(fl.ids[v]), int(d[v])
+    (n0, d0), (n1, d1) = nearest(b0[0]), nearest(b1[0])
+    shared = (0x0AEE0000, 0xFFFFFF00)
+    m0, m1 = 10 + max(0, d1 - d0), 10 + max(0, d0 - d1)
+    add0, add1 = {n0: [(shared[0], shared[1], m0)]}, {n1: [(shared[0], shared[1], m1)]}
+    r_area = _with_stubs(r_area, add0)
+    b0 = [_with_stubs(a, add0) for a in b0]
+    b1 = [_with_stubs(a, add1) for a in b1]
+    # the borders' type-3 LSAs into area 0: area-1 stubs that are not area-0 prefixes
+    stubs0 = {(int(l["link_id"]), int(l["link_data"])) for l in r_area.links if l["link_type"] == LINK_STUB}
+    sums0 = []
+    for bid, a in zip(bids, b1):
+        fl = Flat(a)
+        d = _dist_from(fl, fl.router_vertex(bid))
+        seen = set()
+        for x in a.router_lsas:
+            v = fl.router_vertex(int(x["adv_rtr"]))
+            if v == 0xFFFFFFFF or d[v] >= 1 << 40:
+                continue
+            for l in a.links[int(x["link_off"]): int(x["link_off"]) + int(x["n_links"])]:
+                key = (int(l["link_id"]), int(l["link_data"]))
+                if l["link_type"] != LINK_STUB or key in stubs0 or key in seen:
+                    continue
+                seen.add(key)
+                sums0.append((bid, key[0], key[1], int(d[v]) + int(l["metric"]), 3, 0, (0, 0)))
+    sums0.sort(key=lambda x: (x[4], x[0], x[1]))
+    summaries0 = np.asarray(sums0, ospf_rib.SUMMARY_LSA_DT)
+    loops = sorted({int(x["adv_rtr"]) for x in b1[0].router_lsas} - set(bids))
+    keys = [loops[int(i)] for i in rng.choice(len(loops), min(n_ext_keys, len(loops)), replace=False)]
+    ext = [(asbr, k, 0xFFFFFFFF, int(rng.choice([5, 30])), 0, 7, int(j % 2), 0, (0, 0)) for j, k in enumerate(keys)]
+    ext.append((asbr, 0x0E0A0000, 0xFFFFFF00, 12, 0, 8, 1, 0, (0, 0)))
+    ext.sort(key=lambda x: (x[0], x[1]))
+    externals = np.asarray(ext, ospf_rib.EXTERNAL_LSA_DT)
+    empty = np.zeros(0, ospf_rib.SUMMARY_LSA_DT)
+    out_borders = []
+    for j, (a0, a1) in enumerate(zip(b0, b1)):
+        pair = [(a0, 0, summaries0[summaries0["adv_rtr"] != a0.router_id]), (a1, 1, empty)]
+        if j == 0:
+            pair = pair[::-1]
+        out_borders.append(([p[0] for p in pair], [p[1] for p in pair], [p[2] for p in pair]))
+    return {"r_area": r_area, "summaries0": summaries0, "externals": externals, "borders": out_borders,
+            "shared": shared, "asbr": asbr}

@@ -158,6 +158,18 @@ def declare(lib: C.CDLL):
         "hspf_isis_backbone_cells16": [vp, vp, u32, res16, res16, vp, vp, vp, vp],
         "hspf_isis_backbone_delta": [vp, vp, u32, res, res, vp, vp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_isis_backbone_delta16": [vp, vp, u32, res16, res16, vp, vp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_net_summaries": [u32, C.POINTER(ospf_rib.RibStruct), C.POINTER(ospf_rib.RtrTablesStruct),
+                                      C.POINTER(ospf_rib.RibAreaStruct), vp, u32, u32, vp, u32, u32p],
+        "hspf_ospfv2_backbone_table_create": [vp, u32, vp, u32, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv2_backbone_table_prefixes": [vp, u32p, pvp, pvp],
+        "hspf_ospfv2_backbone_table_records": [vp, u32p, u32p],
+        "hspf_ospfv2_backbone_table_upload": [vp, vp],
+        "hspf_ospfv2_backbone_cells": [vp, vp, u32, res, pvp, pvp, vp, vp],
+        "hspf_ospfv2_backbone_cells16": [vp, vp, u32, res16, pvp, pvp, vp, vp],
+        "hspf_ospfv2_backbone_delta": [vp, vp, u32, res, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_backbone_delta16": [vp, vp, u32, res16, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_backbone_from_cells": [vp, C.POINTER(ospfv2.AreaStruct), vp, vp, vp, u32,
+                                            C.POINTER(ospf_rib.RibStruct)],
         "hspf_isis_backbone_from_cells": [C.POINTER(isis.InstanceStruct), vp, vp, C.POINTER(isis.JobPlanesStruct), vp,
                                           vp, C.POINTER(isis.RibStruct)],
     }
@@ -170,6 +182,6 @@ def declare(lib: C.CDLL):
         for name in ("prefixes", "contributors"):
             getattr(lib, f"{table}_{name}").argtypes = [vp]
             getattr(lib, f"{table}_{name}").restype = u32
-    for table in ("hspf_isis_l1_to_l2_table", "hspf_isis_backbone_table"):
+    for table in ("hspf_isis_l1_to_l2_table", "hspf_isis_backbone_table", "hspf_ospfv2_backbone_table"):
         getattr(lib, table + "_free").argtypes = [vp]
         getattr(lib, table + "_free").restype = None

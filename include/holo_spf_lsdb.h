@@ -323,6 +323,82 @@ int hspf_ospfv2_abr_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t
                                 hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records);
 
 /*
+ * Batched routing-table stage for a backbone router over what-if jobs inside other areas.  R is an internal router
+ * of area 0 (no B flag); the "borders" are 1..8 area border routers with area 0 among their areas, each with its
+ * ABR table above.  A job changes costs only in the borders' non-backbone areas: R's area-0 SPT is the same in every
+ * job (row 0 of R's planes is read) and only the type-3 LSAs the borders originate into area 0 change.  Every area
+ * border router of a perturbed area must be given as a border: another one keeps its base type-3 LSAs as static
+ * records, and the table cannot tell.  The table
+ * holds R's affected prefixes: those with an intra-area record in a non-backbone area of some border.  Every other
+ * prefix of R's table is R's base route in every job.  For job j, with border b's ABR cells of j decoded to rib_b
+ * (hspf_ospfv2_abr_rib_from_cells), the decoded cells of j equal the affected-prefix routes of
+ *     hspf_ospfv2_update_rib_full(R, max_paths, [{0, area_from_planes(area 0, R's row 0), ifaces, S_j, 1}], X)
+ * where S_j is area 0's type-3/4 LSAs with each border's type-3 LSAs replaced by hspf_ospfv2_net_summaries(rib_b,
+ * target area 0), in LsaKey order.  A border advertises a route of its cell when the cell is present and intra-area,
+ * its winner is not one of area 0's intra-area records, no atom is an area-0 atom, and the metric is below
+ * LSInfinity.  A border route that ties across areas and whose area-0 next hops max_paths would cut is outside the
+ * contract (the cell still counts them).
+ *
+ *   hspf_ospfv2_backbone_table_create  host.  flat: R's area-0 flat; router_id: R; summaries: area 0's type-3/4 LSAs
+ *                                in LsaKey order, as in R's LSDB; externals: the instance's AS-external LSAs; borders:
+ *                                the borders' OSPFv2 ABR tables, which must outlive the table.  Per affected prefix:
+ *                                R's intra-area records (hspf_ospfv2_ribtable_create's), R's type-3 records with each
+ *                                border's LSA replaced by one slot per (border, prefix) at the border's place in
+ *                                LsaKey order (also for a border without an LSA for the prefix), and the type-5 range.
+ *                                HSPF_E_INVAL: R missing from the flat, R with the B flag or one of the borders, a
+ *                                border given twice, a border table without area 0 or for OSPFv3, a border that is
+ *                                not a B-flag router vertex of the flat, a usable type-3 LSA of a border for a prefix
+ *                                that is not one of its affected prefixes, 0 or more than 8 borders.
+ *                                HSPF_E_UNSUPPORTED: area 0 with a V-flag router, a usable type-4 LSA from a border, or
+ *                                one naming an ABR (as hspf_ospfv2_ribtable_create).
+ *   hspf_ospfv2_backbone_table_prefixes  P, and the prefixes / lengths in prefix order (pointers may be NULL).
+ *   hspf_ospfv2_backbone_table_records   the record and slot counts: a slot's winner is n_records + its slot index.
+ *   hspf_ospfv2_backbone_table_upload    copies the table to the ctx's device.
+ *   hspf_ospfv2_backbone_cells[16]  one thread per (job, prefix).  planes: R's area-0 planes (device, nh_words 1),
+ *                                row 0 read; border_cells: host array of n_borders device pointers, border b's cells
+ *                                [n_jobs][P_b] in the table's border order (read in place); border_status: host array of
+ *                                n_borders device u32[n_jobs] pointers (NULL, or a NULL entry: none).  job_status_out
+ *                                (device u32[n_jobs], may be NULL): R's row-0 status word ORed with the borders' job
+ *                                words; a job with a non-zero word gets empty cells.  cells[n_jobs][P] (device).
+ *                                Nothing is launched for 0 jobs.  Enqueued on the ctx stream.
+ *   hspf_ospfv2_backbone_delta[16]  the route-delta stage over the same walk (base cells as hspf_ospfv2_rib_delta).
+ *   hspf_ospfv2_backbone_from_cells host: one job's cells -> the table of the contract.  area: R's area-0 image (the
+ *                                one the flat came from); gather_v / gather_nh: nh_mask of the transit networks next to
+ *                                R in row 0.  HSPF_E_UNSUPPORTED as hspf_ospfv2_rib_from_cells.
+ */
+#define HSPF_BACKBONE_MAX_BORDERS 8u
+typedef struct hspf_ospfv2_backbone_table hspf_ospfv2_backbone_table;
+int hspf_ospfv2_backbone_table_create(const hspf_ospfv2_flat *flat, uint32_t router_id,
+                                      const hl_ospfv2_summary_lsa *summaries, uint32_t n_summaries,
+                                      const hl_ospfv2_external_lsa *externals, uint32_t n_externals,
+                                      const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                      hspf_ospfv2_backbone_table **out);
+void hspf_ospfv2_backbone_table_free(hspf_ospfv2_backbone_table *t);
+int hspf_ospfv2_backbone_table_prefixes(const hspf_ospfv2_backbone_table *t, uint32_t *n_prefixes,
+                                        const uint32_t **prefix, const uint32_t **plen);
+int hspf_ospfv2_backbone_table_records(const hspf_ospfv2_backbone_table *t, uint32_t *n_records, uint32_t *n_slots);
+int hspf_ospfv2_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_backbone_table *t);
+int hspf_ospfv2_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                               const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                               const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells);
+int hspf_ospfv2_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells);
+int hspf_ospfv2_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                               const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                               const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                               const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
+                               uint64_t cap, uint64_t *n_records);
+int hspf_ospfv2_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells,
+                                 uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                                 hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_ospfv2_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const hl_ospfv2_area *area,
+                                    const hl_ospf_rib_cell *cells, const uint32_t *gather_v, const uint64_t *gather_nh,
+                                    uint32_t n_gather, hl_ospfv2_rib *out);
+
+/*
  * The stages of update_rib_full that follow the per-area SPFs (holo-ospf/src/route.rs:146-193):
  * merges the intra-area routes of the attached areas (route_update / route_compare,
  * route.rs:895-971), adds inter-area network routes and inter-area router entries from the
@@ -338,6 +414,35 @@ int hspf_ospfv2_abr_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t
 int hspf_ospfv2_update_rib_full(uint32_t router_id, uint32_t max_paths, const hl_ospfv2_rib_area *areas,
                                 uint32_t n_areas, const hl_ospfv2_external_lsa *ext, uint32_t n_ext,
                                 hl_ospfv2_rib *out);
+
+/*
+ * Summary-LSA origination of an area border router (compute_net_summaries / compute_rtr_summaries,
+ * holo-ospf/src/area.rs:561-740), for one target area, over the table update_rib_full left:
+ *   rib       hspf_ospfv2_update_rib_full's output;  rtrs  hspf_ospfv2_rib_router_tables' output (same inputs);
+ *   areas     the router's areas as given to those calls (area_id, ifaces, active are read);
+ *   config    per area: its type, whether it takes regular summaries, the cost of its default route.
+ * out[0, *n_out): the type-3 contents (lsa_type 3, lsa_id = the prefix address, mask, metric) in prefix order, then the
+ * type-4 contents (lsa_type 4, lsa_id = the ASBR's router id, mask 0, metric) in router-id order; adv_rtr = router_id.
+ * Nothing when at most one area is active (not an ABR).  Type 3: every intra- or inter-area route below LSInfinity
+ * that is not of the target area, only intra-area ones into the backbone, none with a next hop on one of the target
+ * area's interfaces; in a stub or NSSA area, the default route at default_cost (and, with summary = 0, nothing else).
+ * Type 4: into a normal area, each other area's router entry with the E flag below LSInfinity, intra-area ones only
+ * into the backbone, under the same next-hop rule; an id in two areas keeps the later area's.  Out of the contract:
+ * LSA ids (the reference keeps them across runs), and area ranges (no range may be configured).  HSPF_E_NOMEM with
+ * *n_out set when cap is too small.  Host only.
+ */
+#define HL_AREA_NORMAL 0u
+#define HL_AREA_STUB   1u
+#define HL_AREA_NSSA   2u
+typedef struct hl_ospf_area_config {
+    uint32_t default_cost;     /* area.config.default_cost (10 by default)                */
+    uint8_t  area_type;        /* HL_AREA_*                                               */
+    uint8_t  summary;          /* area.config.summary (1 by default; 0: totally stubby)   */
+    uint8_t  _pad[2];
+} hl_ospf_area_config;
+int hspf_ospfv2_net_summaries(uint32_t router_id, const hl_ospfv2_rib *rib, const hl_ospfv2_rtr_tables *rtrs,
+                              const hl_ospfv2_rib_area *areas, const hl_ospf_area_config *config, uint32_t n_areas,
+                              uint32_t target, hl_ospfv2_summary_lsa *out, uint32_t cap, uint32_t *n_out);
 
 /*
  * update_global_rib (holo-ospf/src/route.rs:833-893): compares the freshly computed table with
