@@ -1,11 +1,11 @@
-// Routing table of an OSPFv2 backbone router R for a batch of what-if jobs inside other areas, one cell per (job,
-// affected prefix) (include/holo_spf_lsdb.h, hspf_ospfv2_backbone_table_create).
+// Routing table of an OSPF backbone router R for a batch of what-if jobs inside other areas, one cell per (job,
+// affected prefix) (include/holo_spf_lsdb.h, hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create).
 //
 // A job changes costs only in the non-backbone areas of the area border routers given as "borders".  R is an
-// internal router of area 0, so its area-0 SPT is its unperturbed one in every job, and only the type-3 LSAs the
-// borders originate into area 0 change.  Only a prefix some border can advertise (one with an intra-area record in
-// one of the border's non-backbone areas) can route differently at R.  Per such prefix the walk is
-// ospf_rib_cell_eval (ospf_rib_cells.h) over R's row 0, with each border's type-3 LSA for the prefix replaced by a
+// internal router of area 0, so its area-0 SPT is its unperturbed one in every job, and only the type-3 /
+// Inter-Area-Prefix LSAs the borders originate into area 0 change.  Only a prefix some border can advertise (one with
+// an intra-area record in one of the border's non-backbone areas) can route differently at R.  Per such prefix the
+// walk is ospf_rib_cell_eval (ospf_rib_cells.h) over R's row 0, with each border's LSA for the prefix replaced by a
 // slot at that border's place in LsaKey order:
 //   * a static type-3 record reads R's planes as before (dist[abr] + metric);
 //   * a slot reads the border's routing-table cell of the job (ospf_abr_rib_cells.h) and stands for the LSA
@@ -14,7 +14,11 @@
 //     area-0 atom (nexthops_area_check, area.rs:742) and its metric is below LSInfinity.  Then it offers
 //     dist[border] + the cell's metric.
 // The lowest metric wins and equal metrics OR their atoms, the first record staying the winner.  A slot's winner
-// is n_recs + its slot index, so the decode can tell it from a static record.
+// is n_recs + its slot index (OSPFv2), so the decode can tell it from a static record.  An OSPFv3 slot also carries
+// the prefix options the border copies from its route into the LSA (lsa_orig_inter_area_network, ospfv3/lsdb.rs:
+// 341-386): those of the border cell's winning intra-area record.  Its winner is n_recs + (slot << 8 | options), so
+// that a job whose border route changes record at an equal metric, to one with other options, changes R's winner
+// (the route-delta stage reports OTHER), and the decode reads the options from the winner alone.
 #pragma once
 #include <cstdint>
 #include <vector>
@@ -30,8 +34,10 @@ constexpr uint32_t kOspfBackboneStatic = 0xFFFFFFFFu;   // RibRec::z of a static
 //   static: x ABR vertex, y LSA metric, z kOspfBackboneStatic
 //   slot:   x the border's vertex, y the prefix's index in the border's table, z the border, w the slot index
 
-// What the walk reads of a table.  Per border b, border[4 b ..]: its area-0 intra-area records [lo, hi) and its
-// area-0 atom bits (low word, high word).
+// What the walk reads of a table.  Per border b, border[4 b ..] (OSPFv2) or border[8 b ..] (OSPFv3): its area-0
+// intra-area records [lo, hi) and its area-0 atom bits (low word, high word); OSPFv3 adds the byte offset, from
+// `border`, of the border's options bytes, one per intra-area record of its table (the winner of an intra-area cell
+// indexes them), then three zero words.
 struct OspfBackboneView {
     const uint32_t *oi;           // [PR + 1] R's intra-area ranges (R's one-area table)
     const uint32_t *q;            // [P] the prefix's index in R's one-area table, kNoRecord if none
@@ -47,24 +53,41 @@ struct OspfBorderRows {
     const hl_ospf_rib_cell *row[kOspfBackboneMaxBorders];
 };
 
-// What border b advertises into area 0 for the prefix of its cell c: false when nothing, else its metric.
-HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, uint32_t b, uint32_t &metric) {
+// What border b advertises into area 0 for the prefix of its cell c: false when nothing, else its metric and, for
+// OSPFv3 (kV3), the prefix options of the cell's winner.
+template <bool kV3>
+HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, uint32_t b, uint32_t &metric,
+                            uint32_t &options) {
+    constexpr uint32_t kStride = kV3 ? 2 : 1;                          // 16-byte groups per border
 #if defined(__CUDA_ARCH__)
     const unsigned long long *w = reinterpret_cast<const unsigned long long *>(c);
     const uint64_t wm = __ldg(w + 2), nh = __ldg(w);
-    const uint4 bb = __ldg(reinterpret_cast<const uint4 *>(border) + b);
+    const uint4 bb = __ldg(reinterpret_cast<const uint4 *>(border) + kStride * b);
 #else
     const uint64_t wm = (uint64_t)c->winner | ((uint64_t)c->mpf << 32), nh = c->nh_mask;
-    const struct { uint32_t x, y, z, w; } bb = {border[4 * b], border[4 * b + 1], border[4 * b + 2], border[4 * b + 3]};
+    const uint32_t *bw = border + 4 * kStride * b;
+    const struct { uint32_t x, y, z, w; } bb = {bw[0], bw[1], bw[2], bw[3]};
 #endif
     const uint32_t winner = (uint32_t)wm, mpf = (uint32_t)(wm >> 32);
     const uint64_t atoms0 = (uint64_t)bb.z | ((uint64_t)bb.w << 32);
     metric = mpf & HL_RIB_CELL_METRIC_MAX;
-    return ((mpf >> 28) & HL_CELL_PRESENT) && ((mpf >> 26) & 0x3u) == HL_PATH_INTRA_AREA &&
-           (winner < bb.x || winner >= bb.y) && !(nh & atoms0) && metric < HL_LSA_INFINITY;
+    const bool adv = ((mpf >> 28) & HL_CELL_PRESENT) && ((mpf >> 26) & 0x3u) == HL_PATH_INTRA_AREA &&
+                     (winner < bb.x || winner >= bb.y) && !(nh & atoms0) && metric < HL_LSA_INFINITY;
+    if constexpr (kV3) {
+        options = 0;
+        if (adv) {
+#if defined(__CUDA_ARCH__)
+            options = __ldg(reinterpret_cast<const uint8_t *>(border) + __ldg(border + 8 * b + 4) + winner);
+#else
+            options = reinterpret_cast<const uint8_t *>(border)[border[8 * b + 4] + winner];
+#endif
+        }
+    }
+    return adv;
 }
 
-template <class Planes>
+// kV3: the table is an OSPFv3 one (hspf_ospfv3_backbone_table_create), whose slot winners carry prefix options.
+template <bool kV3 = false, class Planes>
 HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneView &t, uint32_t p,
                                           const OspfBorderRows &rows) {
     const RouteContrib *contribs = reinterpret_cast<const RouteContrib *>(t.recs);
@@ -79,10 +102,10 @@ HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneVi
     for (uint32_t i = t.o3[p]; i < t.o3[p + 1]; ++i) {                  // 2. inter-area, slots in LsaKey order
         const RibRec r = load_rib_rec(t.recs + i);
         if (!pl.reached(r.x)) continue;
-        uint32_t y = r.y, w = i;
+        uint32_t y = r.y, w = i, options = 0;
         if (r.z != kOspfBackboneStatic) {
-            if (!border_summary(rows.row[r.z] + r.y, t.border, r.z, y)) continue;
-            w = t.n_recs + r.w;
+            if (!border_summary<kV3>(rows.row[r.z] + r.y, t.border, r.z, y, options)) continue;
+            w = kV3 ? t.n_recs + (r.w << 8 | options) : t.n_recs + r.w;
         }
         const uint32_t m = pl.d(r.x) + y;
         if (win == kNoRecord || m < metric) { win = w; metric = m; mask = pl.n(r.x); }
@@ -130,12 +153,20 @@ struct hspf_ospfv2_backbone_table {
     hspf_ospfv2_ribtable *r = nullptr;           // R's one-area table over area 0 without the borders' type-3 LSAs
     uint32_t router_id = 0, root = 0, n_vertices = 0, n_borders = 0, max_paths = 0;
     std::vector<uint32_t> prefix, plen;          // [P] prefix order
-    std::vector<uint32_t> words;                 // oi [PR + 1], q [P], o3 [P + 1], o5 [P + 1], padding, border [4 n_borders]
+    // oi [PR + 1], q [P], o3 [P + 1], o5 [P + 1], padding, border [4 n_borders] (OSPFv3: [8 n_borders], then each
+    // border's options bytes, each border's padded to a word)
+    std::vector<uint32_t> words;
     std::vector<hspf::RibRec> recs;              // R's records, then the type-3 and type-5 records of the view
     std::vector<uint32_t> slot_rec;              // [n_slots] the record of each slot
     std::vector<uint32_t> ext_tag;               // per type-5 record of the view (index - ext_base)
     uint32_t ext_base = 0;
     const hspf_ospfv2_abr_ribtable *borders[hspf::kOspfBackboneMaxBorders] = {};
+    // OSPFv3 tables (hspf_ospfv3_backbone_table_create): `prefix` is zero-filled (the prefixes are prefix6), and
+    // options6 holds the prefix options of each type-3 / type-5 record of the view (index - o3[0]); a slot's entry is
+    // a placeholder, its options come from its winner
+    bool v3 = false;
+    std::vector<hl_ip_addr> prefix6;
+    std::vector<uint8_t> options6;
     hspf::DeviceRouteTable dev;                  // hspf_ospfv2_backbone_table_upload: words, then records
 
     uint32_t P() const { return (uint32_t)prefix.size(); }

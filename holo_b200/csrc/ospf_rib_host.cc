@@ -85,6 +85,7 @@ struct V2 {
     static bool skip(const Ext &) { return false; }
     static uint32_t asbr_id(const Sum &l) { return l.lsa_id; }
     static uint8_t options(const NetIn &) { return 0; }
+    static uint8_t options(const Out &) { return 0; }
     static uint8_t options(const Sum &) { return 0; }
     static uint8_t options(const Ext &) { return 0; }
     static void label_in(bool &has, uint32_t &label, const NetIn &r) { has = r.has_sr_label != 0; label = r.sr_label; }
@@ -104,6 +105,9 @@ struct V2 {
         kb.fill(0);
         if (n.has_addr) { kb[0] = (uint8_t)(n.addr >> 24); kb[1] = (uint8_t)(n.addr >> 16); kb[2] = (uint8_t)(n.addr >> 8); kb[3] = (uint8_t)n.addr; }
     }
+    // the key of a route in net_summaries' table: (prefix, mask), as the summary LSA names it
+    using SumKey = std::pair<uint32_t, uint32_t>;
+    static SumKey sum_key(const Out &r) { return {r.prefix, r.mask}; }
     static void emit(Out &o, const PKey &k, uint8_t /*options*/) {
         o.prefix = ((uint32_t)k.b[0] << 24) | ((uint32_t)k.b[1] << 16) | ((uint32_t)k.b[2] << 8) | k.b[3];
         o.mask = k.b[16] ? 0xFFFFFFFFu << (32 - k.b[16]) : 0u;
@@ -126,6 +130,7 @@ struct V3 {
     static bool skip(const Ext &l) { return (l.prefix_options & HL_PFX_OPT_NU) != 0; }                   // ospfv3/spf.rs:538
     static uint32_t asbr_id(const Sum &l) { return l.router_id; }
     static uint8_t options(const NetIn &r) { return r.prefix_options; }
+    static uint8_t options(const Out &r) { return r.prefix_options; }
     static uint8_t options(const Sum &l) { return l.prefix_options; }
     static uint8_t options(const Ext &l) { return l.prefix_options; }
     static void label_in(bool &, uint32_t &, const NetIn &) {}
@@ -145,6 +150,8 @@ struct V3 {
         kb.fill(0);
         if (n.has_addr) std::memcpy(kb.data(), n.addr.bytes, 16);
     }
+    using SumKey = PKey;
+    static SumKey sum_key(const Out &r) { return mk(r.prefix, r.len); }
     static void emit(Out &o, const PKey &k, uint8_t options) {
         std::memcpy(o.prefix.bytes, k.b.data(), 16);
         o.prefix.is_v6 = 1;
@@ -451,6 +458,61 @@ extern "C" int hspf_ospfv3_update_rib_full(uint32_t router_id, uint32_t max_path
     return guarded<V3>(router_id, max_paths, areas, n_areas, ext, n_ext, out);
 }
 
+namespace {
+
+// nexthops_area_check (holo-ospf area.rs:742): a next hop on one of area `ta`'s interfaces (next hops name them by
+// sort key)
+template <class Area, class Nh>
+bool nexthops_on_area(const Area &ta, const Nh *h, uint32_t n) {
+    for (uint32_t k = 0; k < n; ++k)
+        for (uint32_t i = 0; i < ta.n_ifaces; ++i)
+            if (h[k].iface == ta.ifaces[i].sort_key) return true;
+    return false;
+}
+
+// The checks both versions' net_summaries make of a routing table and the areas
+template <class Rib, class Area>
+bool net_summaries_args(const Rib *rib, const Area *areas, const hl_ospf_area_config *config, uint32_t n_areas,
+                        uint32_t target) {
+    if (!rib || !areas || !config || target >= n_areas) return false;
+    if ((rib->n_routes && !rib->routes) || (rib->n_nexthops && !rib->nexthops)) return false;
+    for (uint32_t i = 0; i < rib->n_routes; ++i)
+        if ((uint64_t)rib->routes[i].nh_off + rib->routes[i].n_nh > rib->n_nexthops) return false;
+    for (uint32_t i = 0; i < n_areas; ++i)
+        if (areas[i].n_ifaces && !areas[i].ifaces) return false;
+    return true;
+}
+
+// compute_net_summaries (holo-ospf area.rs:561-659) of an ABR for one target area, without area ranges and without
+// LSA ids: the type-3 / Inter-Area-Prefix contents keyed as the reference's summary table (T::sum_key; `dflt` is
+// the default route's key), each (metric, prefix options), a later entry replacing an earlier one.  Empty when at
+// most one area is active (not an ABR).
+template <class T>
+std::map<typename T::SumKey, std::pair<uint32_t, uint8_t>> net_summaries(const typename T::Rib &rib,
+                                                                        const typename T::Area *areas, uint32_t n_areas,
+                                                                        uint32_t target, const hl_ospf_area_config &cfg,
+                                                                        const typename T::SumKey &dflt) {
+    std::map<typename T::SumKey, std::pair<uint32_t, uint8_t>> net;
+    uint32_t n_active = 0;
+    for (uint32_t i = 0; i < n_areas; ++i) n_active += areas[i].active ? 1u : 0u;
+    if (n_active <= 1) return net;
+    const typename T::Area &ta = areas[target];
+    const bool backbone = ta.area_id == 0;
+    if (cfg.summary)
+        for (uint32_t i = 0; i < rib.n_routes; ++i) {
+            const typename T::Out &r = rib.routes[i];
+            if (r.path_type >= HL_PATH_TYPE1_EXTERNAL || r.metric >= HL_LSA_INFINITY) continue;
+            if (r.has_area && r.area_id == ta.area_id) continue;
+            if (backbone && r.path_type != HL_PATH_INTRA_AREA) continue;
+            if (nexthops_on_area(ta, rib.nexthops + r.nh_off, r.n_nh)) continue;
+            net[T::sum_key(r)] = {r.metric, T::options(r)};
+        }
+    if (cfg.area_type != HL_AREA_NORMAL) net[dflt] = {cfg.default_cost, 0};
+    return net;
+}
+
+}  // namespace
+
 // compute_net_summaries / compute_rtr_summaries (holo-ospf area.rs:561-740) of an ABR for one target area, without
 // area ranges and without LSA ids: each map keyed as the reference's summary tables, a later entry replacing
 // an earlier one
@@ -458,51 +520,26 @@ extern "C" int hspf_ospfv2_net_summaries(uint32_t router_id, const hl_ospfv2_rib
                                          const hl_ospfv2_rib_area *areas, const hl_ospf_area_config *config,
                                          uint32_t n_areas, uint32_t target, hl_ospfv2_summary_lsa *out, uint32_t cap,
                                          uint32_t *n_out) {
-    if (!rib || !rtrs || !areas || !config || !n_out || target >= n_areas || (cap && !out)) return HSPF_E_INVAL;
-    if ((rib->n_routes && !rib->routes) || (rib->n_nexthops && !rib->nexthops)) return HSPF_E_INVAL;
+    if (!rtrs || !n_out || (cap && !out) || !net_summaries_args(rib, areas, config, n_areas, target)) return HSPF_E_INVAL;
     if ((rtrs->n_rtrs && !rtrs->rtrs) || (rtrs->n_nexthops && !rtrs->nexthops)) return HSPF_E_INVAL;
-    for (uint32_t i = 0; i < rib->n_routes; ++i)
-        if ((uint64_t)rib->routes[i].nh_off + rib->routes[i].n_nh > rib->n_nexthops) return HSPF_E_INVAL;
     for (uint32_t i = 0; i < rtrs->n_rtrs; ++i)
         if ((uint64_t)rtrs->rtrs[i].nh_off + rtrs->rtrs[i].n_nh > rtrs->n_nexthops) return HSPF_E_INVAL;
-    for (uint32_t i = 0; i < n_areas; ++i)
-        if (areas[i].n_ifaces && !areas[i].ifaces) return HSPF_E_INVAL;
     try {
         *n_out = 0;
-        std::map<std::pair<uint32_t, uint32_t>, uint32_t> net;        // (prefix, mask) -> metric
+        const auto net = net_summaries<V2>(*rib, areas, n_areas, target, config[target], {0u, 0u});
         std::map<uint32_t, uint32_t> rtr;                             // ASBR id -> metric
         uint32_t n_active = 0;
         for (uint32_t i = 0; i < n_areas; ++i) n_active += areas[i].active ? 1u : 0u;
         const hl_ospfv2_rib_area &ta = areas[target];
-        const hl_ospf_area_config &cfg = config[target];
         const bool backbone = ta.area_id == 0;
-        // nexthops_area_check: a next hop on one of the target area's interfaces (next hops name them by sort key)
-        auto on_area = [&](const hl_nexthop *h, uint32_t n) {
-            for (uint32_t k = 0; k < n; ++k)
-                for (uint32_t i = 0; i < ta.n_ifaces; ++i)
-                    if (h[k].iface == ta.ifaces[i].sort_key) return true;
-            return false;
-        };
-        if (n_active > 1) {                                           // only ABRs originate summaries
-            if (cfg.summary)
-                for (uint32_t i = 0; i < rib->n_routes; ++i) {
-                    const hl_rib_route &r = rib->routes[i];
-                    if (r.path_type >= HL_PATH_TYPE1_EXTERNAL || r.metric >= HL_LSA_INFINITY) continue;
-                    if (r.has_area && r.area_id == ta.area_id) continue;
-                    if (backbone && r.path_type != HL_PATH_INTRA_AREA) continue;
-                    if (on_area(rib->nexthops + r.nh_off, r.n_nh)) continue;
-                    net[{r.prefix, r.mask}] = r.metric;
-                }
-            if (cfg.area_type != HL_AREA_NORMAL) net[{0u, 0u}] = cfg.default_cost;
-            if (cfg.area_type == HL_AREA_NORMAL)
-                for (uint32_t i = 0; i < rtrs->n_rtrs; ++i) {
-                    const hl_rib_rtr &r = rtrs->rtrs[i];
-                    if (r.area_id == ta.area_id || !(r.flags & HL_RTR_FLAG_E) || r.metric >= HL_LSA_INFINITY) continue;
-                    if (backbone && r.path_type != HL_PATH_INTRA_AREA) continue;
-                    if (on_area(rtrs->nexthops + r.nh_off, r.n_nh)) continue;
-                    rtr[r.router_id] = r.metric;
-                }
-        }
+        if (n_active > 1 && config[target].area_type == HL_AREA_NORMAL)   // only ABRs originate summaries
+            for (uint32_t i = 0; i < rtrs->n_rtrs; ++i) {
+                const hl_rib_rtr &r = rtrs->rtrs[i];
+                if (r.area_id == ta.area_id || !(r.flags & HL_RTR_FLAG_E) || r.metric >= HL_LSA_INFINITY) continue;
+                if (backbone && r.path_type != HL_PATH_INTRA_AREA) continue;
+                if (nexthops_on_area(ta, rtrs->nexthops + r.nh_off, r.n_nh)) continue;
+                rtr[r.router_id] = r.metric;
+            }
         *n_out = (uint32_t)(net.size() + rtr.size());
         if (*n_out > cap) return HSPF_E_NOMEM;
         uint32_t k = 0;
@@ -512,8 +549,37 @@ extern "C" int hspf_ospfv2_net_summaries(uint32_t router_id, const hl_ospfv2_rib
             l.adv_rtr = router_id; l.lsa_id = id; l.mask = mask; l.metric = metric; l.lsa_type = type;
             out[k++] = l;
         };
-        for (const auto &e : net) put(3, e.first.first, e.first.second, e.second);
+        for (const auto &e : net) put(3, e.first.first, e.first.second, e.second.first);
         for (const auto &e : rtr) put(4, e.first, 0, e.second);
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
+}
+
+// compute_net_summaries for OSPFv3 (Inter-Area-Prefix contents, lsa_orig_inter_area_network, ospfv3/lsdb.rs:341-386):
+// each route's prefix options go into the LSA it originates
+extern "C" int hspf_ospfv3_net_summaries(uint32_t router_id, const hl_ospfv3_rib *rib, const hl_ospfv3_rib_area *areas,
+                                         const hl_ospf_area_config *config, uint32_t n_areas, uint32_t target,
+                                         hl_ospfv3_inter_area_lsa *out, uint32_t cap, uint32_t *n_out) {
+    if (!n_out || (cap && !out) || !net_summaries_args(rib, areas, config, n_areas, target)) return HSPF_E_INVAL;
+    try {
+        *n_out = 0;
+        const auto net = net_summaries<V3>(*rib, areas, n_areas, target, config[target], PKey{});
+        *n_out = (uint32_t)net.size();
+        if (*n_out > cap) return HSPF_E_NOMEM;
+        uint32_t k = 0;
+        for (const auto &e : net) {
+            hl_ospfv3_inter_area_lsa l;
+            std::memset(&l, 0, sizeof(l));
+            l.adv_rtr = router_id; l.metric = e.second.first; l.lsa_type = 3;
+            std::memcpy(l.prefix.bytes, e.first.b.data(), 16);
+            l.prefix.is_v6 = 1;
+            l.len = e.first.b[16]; l.prefix_options = e.second.second;
+            out[k++] = l;
+        }
         return HSPF_OK;
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;

@@ -6,9 +6,12 @@
 //                      reads (ospf_rib_cells.h) are the same.
 //   build_abr_ribtable hspf_ospfv2_abr_ribtable_create / hspf_ospfv3_abr_ribtable_create: an area border router's
 //                      records over the one-area tables of its areas (ospf_abr_rib_cells.h)
+//   build_backbone_table  hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create: a backbone router's
+//                      affected prefixes over its one-area table and its borders' ABR tables (ospf_backbone_cells.h)
 //   decode_rib         one job's cells -> its routing table, for hspf_ospfv2_rib_from_cells,
-//                      hspf_ospfv3_rib_from_cells and hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib).  A
-//                      one-area table decodes as an area border router's table with a single area.
+//                      hspf_ospfv3_rib_from_cells, hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib) and
+//                      hspf_ospfv{2,3}_backbone_from_cells (decode_backbone_rib).  A one-area table decodes as an area
+//                      border router's table with a single area.
 //
 // For build_rib_records a version trait T provides:
 //   Key                        prefix key; its order is the table's prefix order (update_rib_full's IpNetwork order)
@@ -26,8 +29,12 @@
 //   root_vertex(f, id)         the router vertex of router `id` in f, or 0xFFFFFFFF
 //   n_vertices(f)              f's vertex count
 //   atom_count(f, root, &n)    hspf_atom_count over f's CSR
-//   area_table(f, id, sums, n_sums, ext, n_ext, &rt)  the area's one-area table, built with the transit-area walk
-//   table_key(rt, u)           the key of prefix u of a one-area table
+//   area_table(f, id, sums, n_sums, ext, n_ext, transit_walk, &rt)  the area's one-area table (build_rib_records'
+//                              transit_walk)
+//   table_key(rt, u)           the key of prefix u of a one-area or an ABR table
+//
+// For build_backbone_table it also provides:
+//   router_flags(f, v)         the Router-LSA flags of router vertex v of f (its first fragment's)
 //
 // For decode_rib it also provides:
 //   Area, Rib                  the area image and the caller's output
@@ -46,6 +53,7 @@
 #include <algorithm>
 #include <cstdint>
 #include <cstring>
+#include <map>
 #include <memory>
 #include <new>
 #include <numeric>
@@ -54,6 +62,7 @@
 
 #include "holo_spf_lsdb.h"
 #include "ospf_abr_rib_cells.h"
+#include "ospf_backbone_cells.h"
 #include "ospf_rib_cells.h"
 
 namespace hspf {
@@ -222,7 +231,7 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
             for (uint32_t k = 0; k < ns; ++k)
                 if (step2 || summaries[i][k].lsa_type == 3) sums.push_back(summaries[i][k]);
             hspf_ospfv2_ribtable *rt = nullptr;
-            rc = T::area_table(flats[i], area_ids[i], sums.data(), (uint32_t)sums.size(), ext, n_ext, &rt);
+            rc = T::area_table(flats[i], area_ids[i], sums.data(), (uint32_t)sums.size(), ext, n_ext, true, &rt);
             if (rc) return rc;
             t->area.push_back(rt);
             t->area_id.push_back(area_ids[i]);
@@ -324,6 +333,180 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
             for (uint32_t v = 0; v < rt.vflags.size(); ++v)
                 if (rt.vflags[v] & HL_RTR_FLAG_V) t->v_flagged.push_back(v);
             t->vl_off.push_back((uint32_t)t->v_flagged.size());
+        }
+        *out = t.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_UNSUPPORTED;
+    }
+}
+
+// hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create, argument checks included: R's one-area table
+// over area 0 without the borders' type-3 LSAs, and per affected prefix R's intra-area records, its static type-3
+// records with one slot per (border, prefix) at the border's place in LsaKey order, and its type-5 records
+// (ospf_backbone_cells.h).  Border tables of the other version are refused (HSPF_E_INVAL).
+template <class T>
+int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const typename T::Sum *sums, uint32_t n_sums,
+                         const typename T::Ext *ext, uint32_t n_ext, const hspf_ospfv2_abr_ribtable *const *borders,
+                         uint32_t n_borders, hspf_ospfv2_backbone_table **out) {
+    using Key = typename T::Key;
+    using Sum = typename T::Sum;
+    constexpr uint32_t kNone = 0xFFFFFFFFu;
+    if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext) || !borders) return HSPF_E_INVAL;
+    *out = nullptr;
+    if (n_borders == 0 || n_borders > kOspfBackboneMaxBorders) return HSPF_E_INVAL;
+    try {
+        std::unique_ptr<hspf_ospfv2_backbone_table, void (*)(hspf_ospfv2_backbone_table *)> t(
+            new hspf_ospfv2_backbone_table(), hspf_ospfv2_backbone_table_free);
+        const typename T::Flat &f = *flat;
+        auto vertex = [&](uint32_t id) { return T::root_vertex(f, id); };
+        auto flags = [&](uint32_t v) { return v == kNone ? (uint8_t)0 : T::router_flags(f, v); };
+        const uint32_t root = vertex(router_id);
+        if (root == kNone || (flags(root) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
+        t->router_id = router_id; t->root = root; t->n_vertices = T::n_vertices(f);
+        t->max_paths = f.area->max_paths; t->n_borders = n_borders; t->v3 = T::kV3;
+        std::vector<uint32_t> a0(n_borders), bv(n_borders);       // per border: its area-0 index, its vertex
+        std::unordered_map<uint32_t, uint32_t> border_of;           // router id -> border
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            const hspf_ospfv2_abr_ribtable *bt = borders[b];
+            if (!bt || bt->v3 != T::kV3 || bt->router_id == router_id || !border_of.emplace(bt->router_id, b).second)
+                return HSPF_E_INVAL;
+            a0[b] = kNone;
+            for (uint32_t i = 0; i < bt->n_areas; ++i)
+                if (bt->area_id[i] == 0) { a0[b] = i; break; }
+            bv[b] = vertex(bt->router_id);
+            if (a0[b] == kNone || !(flags(bv[b]) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
+            t->borders[b] = bt;
+        }
+        // area 0 without the borders' type-3 LSAs: R's one-area table over the rest
+        auto live = [](const Sum &l) { return !l.maxage && l.metric < HL_LSA_INFINITY && !T::skip(l); };
+        std::vector<Sum> rest;
+        std::vector<std::pair<uint32_t, Key>> border_t3;            // (border, prefix key) of the borders' LSAs
+        for (uint32_t i = 0; i < n_sums; ++i) {
+            const Sum &l = sums[i];
+            auto it = border_of.find(l.adv_rtr);
+            if (it == border_of.end()) { rest.push_back(l); continue; }
+            if (!live(l)) continue;
+            if (l.lsa_type == 4) return HSPF_E_UNSUPPORTED;         // re-originated per job too
+            if (l.lsa_type == 3) border_t3.emplace_back(it->second, T::key(l));
+        }
+        int rc = T::area_table(flat, 0, rest.data(), (uint32_t)rest.size(), ext, n_ext, false, &t->r);
+        if (rc) return rc;
+        const hspf_ospfv2_ribtable &r = *t->r;
+        // the affected prefixes: each border's prefixes with an intra-area record in one of its non-backbone areas
+        std::map<Key, std::vector<std::pair<uint32_t, uint32_t>>> slots;   // key -> (border, its prefix index)
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+            const uint32_t P = (uint32_t)bt.prefix.size(), S = P + 1;
+            for (uint32_t u = 0; u < P; ++u)
+                for (uint32_t i = 0; i < bt.n_areas; ++i)
+                    if (bt.area_id[i] != 0 && bt.off[i * S + u] != bt.off[i * S + u + 1]) {
+                        slots[T::table_key(bt, u)].emplace_back(b, u);
+                        break;
+                    }
+        }
+        for (const auto &x : border_t3) {
+            auto it = slots.find(x.second);
+            bool found = false;
+            if (it != slots.end())
+                for (const auto &s : it->second) found = found || s.first == x.first;
+            if (!found) return HSPF_E_INVAL;                         // the LSDB disagrees with the border's table
+        }
+        // R's static type-3 records per prefix, in LsaKey order: (adv_rtr, ABR vertex, metric, prefix options)
+        std::map<Key, std::vector<std::array<uint32_t, 4>>> statics;
+        for (const Sum &l : rest) {
+            if (l.lsa_type != 3 || !live(l)) continue;
+            const uint32_t v = vertex(l.adv_rtr);
+            if (!(flags(v) & HL_RTR_FLAG_B)) continue;
+            statics[T::key(l)].push_back({l.adv_rtr, v, l.metric, T::options(l)});
+        }
+        std::map<Key, uint32_t> q_of;
+        const uint32_t PR = (uint32_t)r.prefix.size();
+        for (uint32_t u = 0; u < PR; ++u) q_of.emplace(T::table_key(r, u), u);
+        const uint32_t P = (uint32_t)slots.size();
+        std::vector<uint32_t> q(P), o3(P + 1), o5(P + 1);
+        t->recs = r.recs;
+        t->prefix.resize(P); t->plen.resize(P);
+        if (T::kV3) t->prefix6.resize(P);
+        uint32_t u = 0;
+        for (auto &e : slots) {
+            auto &sl = e.second;
+            std::stable_sort(sl.begin(), sl.end(), [&](const std::pair<uint32_t, uint32_t> &x,
+                                                       const std::pair<uint32_t, uint32_t> &y) {
+                return borders[x.first]->router_id < borders[y.first]->router_id;
+            });
+            T::set_prefix(*t, u, e.first);
+            auto qi = q_of.find(e.first);
+            q[u] = qi == q_of.end() ? kNoRecord : qi->second;
+            o3[u] = (uint32_t)t->recs.size();
+            auto st = statics.find(e.first);
+            size_t k = 0;
+            auto put_slot = [&]() {
+                const uint32_t b = sl[k].first;
+                t->slot_rec.push_back((uint32_t)t->recs.size());
+                t->recs.push_back(RibRec{bv[b], sl[k].second, b, (uint32_t)t->slot_rec.size() - 1});
+                if (T::kV3) t->options6.push_back(0);
+                ++k;
+            };
+            if (st != statics.end())
+                for (const auto &s : st->second) {
+                    while (k < sl.size() && borders[sl[k].first]->router_id < s[0]) put_slot();
+                    t->recs.push_back(RibRec{s[1], s[2], kOspfBackboneStatic, 0});
+                    if (T::kV3) t->options6.push_back((uint8_t)s[3]);
+                }
+            while (k < sl.size()) put_slot();
+            ++u;
+        }
+        o3[P] = (uint32_t)t->recs.size();
+        const uint32_t *r5 = r.off.data() + 2 * ((size_t)PR + 1);
+        t->ext_base = (uint32_t)t->recs.size();
+        for (u = 0; u < P; ++u) {
+            o5[u] = (uint32_t)t->recs.size();
+            if (q[u] == kNoRecord) continue;
+            for (uint32_t k = r5[q[u]]; k < r5[q[u] + 1]; ++k) {
+                t->recs.push_back(r.recs[k]);
+                t->ext_tag.push_back(r.ext_tag[k - r.ext_base]);
+                if (T::kV3) t->options6.push_back(r.options6[k - r.n_intra]);
+            }
+        }
+        o5[P] = (uint32_t)t->recs.size();
+        // winners are u32: a slot's is n_recs + its index (OSPFv3: n_recs + (index << 8 | options))
+        const uint64_t n_slots = t->slot_rec.size();
+        if ((uint64_t)t->recs.size() + (T::kV3 ? n_slots << 8 : n_slots) >= kNone) return HSPF_E_UNSUPPORTED;
+        t->words.assign(r.off.begin(), r.off.begin() + PR + 1);
+        t->words.insert(t->words.end(), q.begin(), q.end());
+        t->words.insert(t->words.end(), o3.begin(), o3.end());
+        t->words.insert(t->words.end(), o5.begin(), o5.end());
+        t->words.resize(t->border_at(), 0);
+        uint32_t opt_words = (T::kV3 ? 8 : 4) * n_borders;         // OSPFv3: the options bytes follow the border words
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+            const uint32_t i = a0[b], lo = bt.intra_base[i], na = bt.n_atoms[i];
+            const uint64_t atoms = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << bt.base[i]);
+            t->words.insert(t->words.end(), {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)});
+            if (T::kV3) {
+                t->words.insert(t->words.end(), {4 * opt_words, 0u, 0u, 0u});
+                opt_words += (bt.t3_base[0] + 3) / 4;
+            }
+        }
+        if (T::kV3) {
+            // per border, the prefix options of each intra-area record of its table, as the OSPFv3 intra-area decode
+            // reads them for that winner: the record's entry in its area's intra-area table
+            for (uint32_t b = 0; b < n_borders; ++b) {
+                const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+                std::vector<uint8_t> opt;
+                for (uint32_t i = 0; i < bt.n_areas; ++i) {
+                    const std::vector<uint8_t> &o = bt.area[i]->intra->t.options6;
+                    if (o.size() != bt.area[i]->n_intra || opt.size() != bt.intra_base[i]) return HSPF_E_INVAL;
+                    opt.insert(opt.end(), o.begin(), o.end());
+                }
+                opt.resize(((size_t)bt.t3_base[0] + 3) & ~(size_t)3, 0);
+                const size_t at = t->words.size();
+                t->words.resize(at + opt.size() / 4);
+                if (!opt.empty()) std::memcpy(t->words.data() + at, opt.data(), opt.size());
+            }
         }
         *out = t.release();
         return HSPF_OK;
@@ -544,6 +727,45 @@ int decode_abr_rib(const hspf_ospfv2_abr_ribtable *t, const typename T::Area *ar
                               t->base[i], mask, t->area_id[i], &jd[i]});
         }
         return decode_rib(d, cells, out);
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
+}
+
+// hspf_ospfv2_backbone_from_cells / hspf_ospfv3_backbone_from_cells, argument checks included: the decode of R's
+// one-area table over the affected prefixes, a slot winner naming its type-3 record (and, OSPFv3, carrying the
+// options the route takes).  A table of the other version is refused (HSPF_E_INVAL).
+template <class T>
+int decode_backbone_rib(const hspf_ospfv2_backbone_table *t, const typename T::Area *a, const hl_ospf_rib_cell *cells,
+                        const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out) {
+    if (!t || t->v3 != T::kV3 || !a || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
+    if (a->router_id != t->router_id || a->area_id != 0 || a->max_paths != t->max_paths) return HSPF_E_INVAL;
+    try {
+        out->n_routes = out->n_nexthops = 0;
+        typename T::JobDecode jd;
+        const int rc = jd.init(a, t->n_vertices, gather_v, gather_nh, n_gather);
+        if (rc) return rc;
+        if (jd.root != t->root) return HSPF_E_INVAL;
+        const uint32_t P = t->P(), n_recs = (uint32_t)t->recs.size();
+        const OspfBackboneView v = t->host_view();
+        std::vector<hl_ospf_rib_cell> c(cells, cells + P);
+        std::vector<uint8_t> options(t->options6);                 // OSPFv3: this job's, a slot's from its winner
+        for (hl_ospf_rib_cell &x : c) {
+            if (!(HL_RIB_CELL_FLAGS(x) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(x) != HL_PATH_INTER_AREA || x.winner < n_recs)
+                continue;
+            uint32_t s = x.winner - n_recs, opt = 0;
+            if (T::kV3) { opt = s & 0xFFu; s >>= 8; }
+            if (s >= t->slot_rec.size()) return HSPF_E_INVAL;
+            x.winner = t->slot_rec[s];
+            if (T::kV3) options[x.winner - v.o3[0]] = (uint8_t)opt;
+        }
+        RibDecode<T> d{{RibDecodeArea<T>{a, t->r, v.q, 0, ~0ull, v.o3, 0, ~0ull, 0, &jd}},
+                       P, t->prefix.data(), t->plen.data(), T::kV3 ? t->prefix6.data() : nullptr, v.o5,
+                       t->ext_tag.data(), t->ext_base, t->max_paths, T::kV3 ? options.data() : nullptr,
+                       T::kV3 ? v.o3[0] : 0};
+        return decode_rib(d, c.data(), out);
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;
     } catch (...) {

@@ -1,6 +1,7 @@
-// Device stage for the routing table of an OSPFv2 backbone router over what-if jobs inside other areas
+// Device stage for the routing table of an OSPF backbone router over what-if jobs inside other areas
 // (include/holo_spf_lsdb.h, "backbone router over what-if jobs inside other areas"): update_rib_full at the router,
-// for its affected prefixes, with every border's type-3 LSAs in area 0 re-originated for the job.
+// for its affected prefixes, with every border's type-3 / Inter-Area-Prefix LSAs in area 0 re-originated for the job.
+// The entry points serve OSPFv2 and OSPFv3 tables alike: the table's mark picks the walk's instantiation.
 //
 // One launch on the ctx stream: one thread per (job, prefix) runs ospf_backbone_cell_eval (ospf_backbone_cells.h)
 // over the router's unperturbed area-0 planes (row 0) and the job's row of each border's routing-table cells, and
@@ -16,7 +17,7 @@ namespace {
 
 using hspf::kOspfBackboneMaxBorders;
 
-template <class Planes>
+template <class Planes, bool kV3>
 struct OspfBackboneCell {
     using Rows = hspf::ResultPlanes<Planes>;
     hspf::OspfBackboneView t;
@@ -36,18 +37,20 @@ struct OspfBackboneCell {
         hspf::OspfBorderRows rows;
 #pragma unroll
         for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = cells[b] + (size_t)j * K[b];
-        return hspf::ospf_backbone_cell_eval(pl.job(0), t, p, rows);
+        return hspf::ospf_backbone_cell_eval<kV3>(pl.job(0), t, p, rows);
     }
     __device__ __forceinline__ uint64_t gather(uint32_t, uint32_t, uint32_t) const { return 0; }   // row 0: host side
     __device__ static hspf::CellWords empty() { return {0, 0, hspf::kNoRecord}; }
 };
 
-// Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6).
+// Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
+// and for OSPFv3 tables.
 constexpr uint32_t kBackboneBlocksPerSM = 4;
+constexpr uint32_t kBackboneV3BlocksPerSM = 4;
 
-template <class R>
+template <class R, bool kV3>
 int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
-              const uint32_t *const *border_status, OspfBackboneCell<hspf::PlanesOf<R>> &cell) {
+              const uint32_t *const *border_status, OspfBackboneCell<hspf::PlanesOf<R>, kV3> &cell) {
     if (!t || !t->dev.blob || !border_cells) return HSPF_E_INVAL;
     if (hspf::result_planes(planes, t->n_vertices, cell.pl) || !cell.pl.complete()) return HSPF_E_INVAL;
     for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
@@ -64,14 +67,37 @@ int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_osp
     return HSPF_OK;
 }
 
+template <bool kV3, class R>
+int version_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    constexpr uint32_t kBlocks = kV3 ? kBackboneV3BlocksPerSM : kBackboneBlocksPerSM;
+    OspfBackboneCell<hspf::PlanesOf<R>, kV3> cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
+    return hspf::launch_route_cells<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out, 0, nullptr,
+                                             nullptr, nullptr, nullptr);
+}
+
+template <bool kV3, class R>
+int version_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    constexpr uint32_t kBlocks = kV3 ? kBackboneV3BlocksPerSM : kBackboneBlocksPerSM;
+    OspfBackboneCell<hspf::PlanesOf<R>, kV3> cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
+    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBlocks>(
+        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+// the walk of the table's version
 template <class R>
 int backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
                    const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                    uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    OspfBackboneCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    return hspf::launch_route_cells<kBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out, 0,
-                                                          nullptr, nullptr, nullptr, nullptr);
+    if (!t) return HSPF_E_INVAL;
+    return t->v3 ? version_cells<true>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells)
+                 : version_cells<false>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
 }
 
 template <class R>
@@ -79,10 +105,11 @@ int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t 
                    const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                    const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                    hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    OspfBackboneCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBackboneBlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+    if (!t) return HSPF_E_INVAL;
+    return t->v3 ? version_delta<true>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of,
+                                        job_out, records, cap, n_records)
+                 : version_delta<false>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base,
+                                         base_of, job_out, records, cap, n_records);
 }
 
 }  // namespace

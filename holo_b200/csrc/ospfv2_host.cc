@@ -1090,10 +1090,12 @@ struct RibV2 {
         return hspf_atom_count(&c, root, n);
     }
     static int area_table(const Flat *f, uint32_t area_id, const Sum *sums, uint32_t n_sums, const Ext *ext,
-                          uint32_t n_ext, hspf_ospfv2_ribtable **out) {
-        return make_ribtable(f, area_id, sums, n_sums, ext, n_ext, true, out);
+                          uint32_t n_ext, bool transit_walk, hspf_ospfv2_ribtable **out) {
+        return make_ribtable(f, area_id, sums, n_sums, ext, n_ext, transit_walk, out);
     }
-    static Key table_key(const hspf_ospfv2_ribtable &rt, uint32_t u) { return pkey(rt.prefix[u], rt.plen[u]); }
+    template <class Table>
+    static Key table_key(const Table &rt, uint32_t u) { return pkey(rt.prefix[u], rt.plen[u]); }
+    static uint8_t router_flags(const Flat &f, uint32_t v) { return f.area->router_lsas[f.lsa_of[v]].flags; }
 
     using Area = hl_ospfv2_area;
     using Rib = hl_ospfv2_rib;
@@ -1255,143 +1257,7 @@ int hspf_ospfv2_backbone_table_create(const hspf_ospfv2_flat *flat, uint32_t rou
                                       const hl_ospfv2_external_lsa *ext, uint32_t n_ext,
                                       const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
                                       hspf_ospfv2_backbone_table **out) {
-    using hspf::RibRec;
-    if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext) || !borders) return HSPF_E_INVAL;
-    *out = nullptr;
-    if (n_borders == 0 || n_borders > hspf::kOspfBackboneMaxBorders) return HSPF_E_INVAL;
-    try {
-        std::unique_ptr<hspf_ospfv2_backbone_table, void (*)(hspf_ospfv2_backbone_table *)> t(
-            new hspf_ospfv2_backbone_table(), hspf_ospfv2_backbone_table_free);
-        const hspf_ospfv2_flat &f = *flat;
-        auto vertex = [&](uint32_t id) {
-            auto it = f.rtr_vertex.find(id);
-            return it == f.rtr_vertex.end() ? kNone : it->second;
-        };
-        auto flags = [&](uint32_t v) { return v == kNone ? (uint8_t)0 : f.area->router_lsas[f.lsa_of[v]].flags; };
-        const uint32_t root = vertex(router_id);
-        if (root == kNone || (flags(root) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
-        t->router_id = router_id; t->root = root; t->n_vertices = (uint32_t)f.ids.size();
-        t->max_paths = f.area->max_paths; t->n_borders = n_borders;
-        std::vector<uint32_t> a0(n_borders), bv(n_borders);       // per border: its area-0 index, its vertex
-        std::unordered_map<uint32_t, uint32_t> border_of;           // router id -> border
-        for (uint32_t b = 0; b < n_borders; ++b) {
-            const hspf_ospfv2_abr_ribtable *bt = borders[b];
-            if (!bt || bt->v3 || bt->router_id == router_id || !border_of.emplace(bt->router_id, b).second)
-                return HSPF_E_INVAL;
-            a0[b] = kNone;
-            for (uint32_t i = 0; i < bt->n_areas; ++i)
-                if (bt->area_id[i] == 0) { a0[b] = i; break; }
-            bv[b] = vertex(bt->router_id);
-            if (a0[b] == kNone || !(flags(bv[b]) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
-            t->borders[b] = bt;
-        }
-        // area 0 without the borders' type-3 LSAs: R's one-area table over the rest
-        auto live = [](const hl_ospfv2_summary_lsa &l) { return !l.maxage && l.metric < HL_LSA_INFINITY; };
-        std::vector<hl_ospfv2_summary_lsa> rest;
-        std::vector<std::pair<uint32_t, uint64_t>> border_t3;       // (border, prefix key) of the borders' LSAs
-        for (uint32_t i = 0; i < n_sums; ++i) {
-            const hl_ospfv2_summary_lsa &l = sums[i];
-            auto it = border_of.find(l.adv_rtr);
-            if (it == border_of.end()) { rest.push_back(l); continue; }
-            if (!live(l)) continue;
-            if (l.lsa_type == 4) return HSPF_E_UNSUPPORTED;         // re-originated per job too
-            if (l.lsa_type == 3) border_t3.emplace_back(it->second, RibV2::key(l));
-        }
-        int rc = make_ribtable(flat, 0, rest.data(), (uint32_t)rest.size(), ext, n_ext, false, &t->r);
-        if (rc) return rc;
-        const hspf_ospfv2_ribtable &r = *t->r;
-        // the affected prefixes: each border's prefixes with an intra-area record in one of its non-backbone areas
-        std::map<uint64_t, std::vector<std::pair<uint32_t, uint32_t>>> slots;   // key -> (border, its prefix index)
-        for (uint32_t b = 0; b < n_borders; ++b) {
-            const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-            const uint32_t P = (uint32_t)bt.prefix.size(), S = P + 1;
-            for (uint32_t u = 0; u < P; ++u)
-                for (uint32_t i = 0; i < bt.n_areas; ++i)
-                    if (bt.area_id[i] != 0 && bt.off[i * S + u] != bt.off[i * S + u + 1]) {
-                        slots[pkey(bt.prefix[u], bt.plen[u])].emplace_back(b, u);
-                        break;
-                    }
-        }
-        for (const auto &x : border_t3) {
-            auto it = slots.find(x.second);
-            bool found = false;
-            if (it != slots.end())
-                for (const auto &s : it->second) found = found || s.first == x.first;
-            if (!found) return HSPF_E_INVAL;                         // the LSDB disagrees with the border's table
-        }
-        // R's static type-3 records per prefix, in LsaKey order: (adv_rtr, ABR vertex, metric)
-        std::unordered_map<uint64_t, std::vector<std::array<uint32_t, 3>>> statics;
-        for (const hl_ospfv2_summary_lsa &l : rest) {
-            if (l.lsa_type != 3 || !live(l)) continue;
-            const uint32_t v = vertex(l.adv_rtr);
-            if (!(flags(v) & HL_RTR_FLAG_B)) continue;
-            statics[RibV2::key(l)].push_back({l.adv_rtr, v, l.metric});
-        }
-        std::unordered_map<uint64_t, uint32_t> q_of;
-        const uint32_t PR = (uint32_t)r.prefix.size();
-        for (uint32_t u = 0; u < PR; ++u) q_of.emplace(pkey(r.prefix[u], r.plen[u]), u);
-        const uint32_t P = (uint32_t)slots.size();
-        std::vector<uint32_t> q(P), o3(P + 1), o5(P + 1);
-        t->recs = r.recs;
-        uint32_t u = 0;
-        for (auto &e : slots) {
-            auto &sl = e.second;
-            std::stable_sort(sl.begin(), sl.end(), [&](const std::pair<uint32_t, uint32_t> &x,
-                                                       const std::pair<uint32_t, uint32_t> &y) {
-                return borders[x.first]->router_id < borders[y.first]->router_id;
-            });
-            t->prefix.push_back((uint32_t)(e.first >> 8));
-            t->plen.push_back((uint32_t)(e.first & 0xFF));
-            auto qi = q_of.find(e.first);
-            q[u] = qi == q_of.end() ? hspf::kNoRecord : qi->second;
-            o3[u] = (uint32_t)t->recs.size();
-            auto st = statics.find(e.first);
-            size_t k = 0;
-            auto put_slot = [&]() {
-                const uint32_t b = sl[k].first;
-                t->slot_rec.push_back((uint32_t)t->recs.size());
-                t->recs.push_back(RibRec{bv[b], sl[k].second, b, (uint32_t)t->slot_rec.size() - 1});
-                ++k;
-            };
-            if (st != statics.end())
-                for (const auto &s : st->second) {
-                    while (k < sl.size() && borders[sl[k].first]->router_id < s[0]) put_slot();
-                    t->recs.push_back(RibRec{s[1], s[2], hspf::kOspfBackboneStatic, 0});
-                }
-            while (k < sl.size()) put_slot();
-            ++u;
-        }
-        o3[P] = (uint32_t)t->recs.size();
-        const uint32_t *r5 = r.off.data() + 2 * ((size_t)PR + 1);
-        t->ext_base = (uint32_t)t->recs.size();
-        for (u = 0; u < P; ++u) {
-            o5[u] = (uint32_t)t->recs.size();
-            if (q[u] == hspf::kNoRecord) continue;
-            for (uint32_t k = r5[q[u]]; k < r5[q[u] + 1]; ++k) {
-                t->recs.push_back(r.recs[k]);
-                t->ext_tag.push_back(r.ext_tag[k - r.ext_base]);
-            }
-        }
-        o5[P] = (uint32_t)t->recs.size();
-        if ((uint64_t)t->recs.size() + t->slot_rec.size() >= kNone) return HSPF_E_UNSUPPORTED;   // winners are u32
-        t->words.assign(r.off.begin(), r.off.begin() + PR + 1);
-        t->words.insert(t->words.end(), q.begin(), q.end());
-        t->words.insert(t->words.end(), o3.begin(), o3.end());
-        t->words.insert(t->words.end(), o5.begin(), o5.end());
-        t->words.resize(t->border_at(), 0);
-        for (uint32_t b = 0; b < n_borders; ++b) {
-            const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-            const uint32_t i = a0[b], lo = bt.intra_base[i], na = bt.n_atoms[i];
-            const uint64_t atoms = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << bt.base[i]);
-            t->words.insert(t->words.end(), {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)});
-        }
-        *out = t.release();
-        return HSPF_OK;
-    } catch (const std::bad_alloc &) {
-        return HSPF_E_NOMEM;
-    } catch (...) {
-        return HSPF_E_UNSUPPORTED;
-    }
+    return hspf::build_backbone_table<RibV2>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out);
 }
 
 int hspf_ospfv2_backbone_table_prefixes(const hspf_ospfv2_backbone_table *t, uint32_t *n_prefixes,
@@ -1414,32 +1280,7 @@ int hspf_ospfv2_backbone_table_records(const hspf_ospfv2_backbone_table *t, uint
 int hspf_ospfv2_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const hl_ospfv2_area *a,
                                     const hl_ospf_rib_cell *cells, const uint32_t *gather_v, const uint64_t *gather_nh,
                                     uint32_t n_gather, hl_ospfv2_rib *out) {
-    if (!t || !a || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
-    if (a->router_id != t->router_id || a->area_id != 0 || a->max_paths != t->max_paths) return HSPF_E_INVAL;
-    try {
-        out->n_routes = out->n_nexthops = 0;
-        JobDecode jd;
-        const int rc = jd.init(a, t->n_vertices, gather_v, gather_nh, n_gather);
-        if (rc) return rc;
-        if (jd.root != t->root) return HSPF_E_INVAL;
-        const uint32_t P = t->P(), n_recs = (uint32_t)t->recs.size();
-        std::vector<hl_ospf_rib_cell> c(cells, cells + P);
-        for (hl_ospf_rib_cell &x : c) {
-            if (!(HL_RIB_CELL_FLAGS(x) & HL_CELL_PRESENT) || HL_RIB_CELL_PATH(x) != HL_PATH_INTER_AREA || x.winner < n_recs)
-                continue;
-            if (x.winner - n_recs >= t->slot_rec.size()) return HSPF_E_INVAL;
-            x.winner = t->slot_rec[x.winner - n_recs];
-        }
-        const hspf::OspfBackboneView v = t->host_view();
-        hspf::RibDecode<RibV2> d{{hspf::RibDecodeArea<RibV2>{a, t->r, v.q, 0, ~0ull, v.o3, 0, ~0ull, 0, &jd}},
-                                 P, t->prefix.data(), t->plen.data(), nullptr, v.o5, t->ext_tag.data(), t->ext_base,
-                                 t->max_paths, nullptr, 0};
-        return hspf::decode_rib(d, c.data(), out);
-    } catch (const std::bad_alloc &) {
-        return HSPF_E_NOMEM;
-    } catch (...) {
-        return HSPF_E_INVAL;
-    }
+    return hspf::decode_backbone_rib<RibV2>(t, a, cells, gather_v, gather_nh, n_gather, out);
 }
 
 

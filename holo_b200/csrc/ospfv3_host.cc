@@ -766,10 +766,12 @@ struct RibV3 {
         return hspf_atom_count(&c, root, n);
     }
     static int area_table(const Flat *f, uint32_t area_id, const Sum *sums, uint32_t n_sums, const Ext *ext,
-                          uint32_t n_ext, hspf_ospfv2_ribtable **out) {
-        return make_ribtable(f, area_id, sums, n_sums, ext, n_ext, true, out);
+                          uint32_t n_ext, bool transit_walk, hspf_ospfv2_ribtable **out) {
+        return make_ribtable(f, area_id, sums, n_sums, ext, n_ext, transit_walk, out);
     }
-    static Key table_key(const hspf_ospfv2_ribtable &rt, uint32_t u) { return mk(rt.prefix6[u], (uint8_t)rt.plen[u]); }
+    template <class Table>
+    static Key table_key(const Table &rt, uint32_t u) { return mk(rt.prefix6[u], (uint8_t)rt.plen[u]); }
+    static uint8_t router_flags(const Flat &f, uint32_t v) { return f.area->router_lsas[f.first_lsa[v]].flags; }
 
     using Area = hl_ospfv3_area;
     using Rib = hl_ospfv3_rib;
@@ -890,6 +892,35 @@ int hspf_ospfv3_abr_rib_from_cells(const hspf_ospfv2_abr_ribtable *t, const hl_o
                                    const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
                                    const uint64_t *gather_nh, uint32_t n_gather, hl_ospfv3_rib *out) {
     return hspf::decode_abr_rib<RibV3>(t, areas, n_areas, cells, gather_area, gather_v, gather_nh, n_gather, out);
+}
+
+
+
+/* ---- backbone router over what-if jobs inside other areas (ospf_backbone_cells.h) ------------------------------ */
+
+int hspf_ospfv3_backbone_table_create(const hspf_ospfv3_flat *flat, uint32_t router_id,
+                                      const hl_ospfv3_inter_area_lsa *sums, uint32_t n_sums,
+                                      const hl_ospfv3_external_lsa *ext, uint32_t n_ext,
+                                      const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                      hspf_ospfv2_backbone_table **out) {
+    return hspf::build_backbone_table<RibV3>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out);
+}
+
+int hspf_ospfv3_backbone_table_prefixes6(const hspf_ospfv2_backbone_table *t, uint32_t *n_prefixes,
+                                         const hl_ip_addr **prefixes, const uint32_t **lens) {
+    if (!t || !t->v3) return HSPF_E_INVAL;
+    if (n_prefixes) *n_prefixes = t->P();
+    if (prefixes) *prefixes = t->prefix6.data();
+    if (lens) *lens = t->plen.data();
+    return HSPF_OK;
+}
+
+// The decode of R's one-area table over the affected prefixes: a slot winner names its Inter-Area-Prefix record and
+// carries the route's prefix options.
+int hspf_ospfv3_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const hl_ospfv3_area *a,
+                                    const hl_ospf_rib_cell *cells, const uint32_t *gather_v, const uint64_t *gather_nh,
+                                    uint32_t n_gather, hl_ospfv3_rib *out) {
+    return hspf::decode_backbone_rib<RibV3>(t, a, cells, gather_v, gather_nh, n_gather, out);
 }
 
 }  // extern "C"

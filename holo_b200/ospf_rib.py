@@ -228,11 +228,12 @@ class RtrTables:
     nexthops: np.ndarray
 
 
-def _area_array(areas: list, keep: list, with_results: bool):
+def _area_array(areas: list, keep: list, with_results: bool, v3: bool = False):
+    _cls, _fields, iface_dt, sum_dt = _version(v3)[:4]
     arr = (RibAreaStruct * max(len(areas), 1))()
     for i, a in enumerate(areas):
-        ifs = np.ascontiguousarray(a.ifaces, dtype=ospfv2.IFACE_DT)
-        sm = np.ascontiguousarray(a.summaries, dtype=SUMMARY_LSA_DT)
+        ifs = np.ascontiguousarray(a.ifaces, dtype=iface_dt)
+        sm = np.ascontiguousarray(a.summaries, dtype=sum_dt)
         keep += [ifs, sm]
         arr[i].area_id, arr[i].n_summaries = a.area_id, len(sm)
         if with_results:
@@ -590,6 +591,27 @@ def net_summaries(router_id: int, rib: Rib, rtrs: RtrTables, areas: list, config
     return out[: n.value].copy()
 
 
+def net_summaries_v3(router_id: int, rib: Rib, areas: list, configs: list, target: int) -> np.ndarray:
+    """hspf_ospfv3_net_summaries (host): the Inter-Area-Prefix contents the router originates into areas[target]
+    (compute_net_summaries), as INTER_AREA_LSA_DT[] with adv_rtr = router_id, lsa_id 0, lsa_type 3 and each route's
+    prefix options, in prefix order.  rib: update_rib_full_v3's table over `areas` (RibArea list); configs: one
+    area_config() per area."""
+    from . import ospfv3
+    lib = capi.load_library()
+    keep = []
+    arr = _area_array(areas, keep, False, v3=True)
+    cfg = np.asarray(list(configs) or [area_config()], AREA_CONFIG_DT)
+    rs = _rib_struct(rib, keep, RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)
+    cap = len(rib.routes) + 1
+    out = np.zeros(cap, INTER_AREA_LSA_DT)
+    n = C.c_uint32()
+    rc = lib.hspf_ospfv3_net_summaries(router_id, C.byref(rs), arr, cfg.ctypes.data, len(areas), target,
+                                       out.ctypes.data, cap, C.byref(n))
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, "hspf_ospfv3_net_summaries failed")
+    return out[: n.value].copy()
+
+
 # ---- backbone router over what-if jobs inside other areas (include/holo_spf_lsdb.h) -----------------------------
 BACKBONE_MAX_BORDERS = 8           # HSPF_BACKBONE_MAX_BORDERS
 
@@ -599,21 +621,29 @@ class BackboneTable:
     the borders' other areas.  `flat`: R's area-0 ospfv2.Flat; `summaries`: area 0's SUMMARY_LSA_DT[] in LsaKey order;
     `externals`: EXTERNAL_LSA_DT[]; `borders`: the borders' AbrRibTable list (kept alive with this table).  `prefix`,
     `plen` [n_prefixes]: the affected prefixes in prefix order; a slot's winner is n_records + its slot index
-    (n_slots in all)."""
+    (n_slots in all).
+
+    From an ospfv3.Flat the table is hspf_ospfv3_backbone_table_create's (summaries: INTER_AREA_LSA_DT, externals:
+    EXTERNAL6_LSA_DT, borders: OSPFv3 AbrRibTables); `prefix` and `prefixes6` then hold the IPv6 prefixes
+    (ospfv3.IP_DT), `v3` is set, and a slot's winner is n_records + (slot index << 8 | its prefix options)."""
 
     def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=()):
+        from . import ospfv3
         self.lib = capi.load_library()
         self.flat, self.router_id, self.borders = flat, router_id, list(borders)
-        sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
-        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        self.v3 = isinstance(flat, ospfv3.Flat)
+        sum_dt, ext_dt = (INTER_AREA_LSA_DT, EXTERNAL6_LSA_DT) if self.v3 else (SUMMARY_LSA_DT, EXTERNAL_LSA_DT)
+        sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, sum_dt), sum_dt)
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, ext_dt), ext_dt)
         self.summaries, self.externals = sm, ext
         arr = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
         h = C.c_void_p()
-        rc = self.lib.hspf_ospfv2_backbone_table_create(flat.handle, router_id, sm.ctypes.data if len(sm) else None,
-                                                        len(sm), ext.ctypes.data if len(ext) else None, len(ext), arr,
-                                                        len(self.borders), C.byref(h))
+        create = "hspf_ospfv3_backbone_table_create" if self.v3 else "hspf_ospfv2_backbone_table_create"
+        rc = getattr(self.lib, create)(flat.handle, router_id, sm.ctypes.data if len(sm) else None, len(sm),
+                                       ext.ctypes.data if len(ext) else None, len(ext), arr, len(self.borders),
+                                       C.byref(h))
         if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, "hspf_ospfv2_backbone_table_create failed")
+            raise capi.HspfError(rc, create + " failed")
         self.handle = h
         n, pp, pl = C.c_uint32(), C.c_void_p(), C.c_void_p()
         assert self.lib.hspf_ospfv2_backbone_table_prefixes(h, C.byref(n), C.byref(pp), C.byref(pl)) == capi.HSPF_OK
@@ -623,6 +653,13 @@ class BackboneTable:
         nr, ns = C.c_uint32(), C.c_uint32()
         assert self.lib.hspf_ospfv2_backbone_table_records(h, C.byref(nr), C.byref(ns)) == capi.HSPF_OK
         self.n_records, self.n_slots = nr.value, ns.value
+        if self.v3:
+            p6 = C.c_void_p()
+            rc = self.lib.hspf_ospfv3_backbone_table_prefixes6(h, None, C.byref(p6), None)
+            if rc != capi.HSPF_OK:
+                raise capi.HspfError(rc, "hspf_ospfv3_backbone_table_prefixes6 failed")
+            self.prefixes6 = route_table.copy_records(p6, self.n_prefixes, ospfv3.IP_DT)
+            self.prefix = self.prefixes6
 
     def upload(self, ctx: capi.Context):
         rc = self.lib.hspf_ospfv2_backbone_table_upload(ctx.handle, self.handle)
@@ -676,3 +713,18 @@ def backbone_from_cells(area: ospfv2.Ospfv2Area, t: BackboneTable, cells: np.nda
     return _call_rib(capi.load_library().hspf_ospfv2_backbone_from_cells,
                      (t.handle, C.byref(s), cells.ctypes.data, gv.ctypes.data, gn.ctypes.data, len(gv)),
                      t.n_prefixes, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)
+
+
+def backbone_from_cells_v3(area, t: BackboneTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
+    """hspf_ospfv3_backbone_from_cells (host): one job's cells over an OSPFv3 BackboneTable -> R's routes for the
+    affected prefixes, prefix options included (RIB_ROUTE6_DT routes, ospfv3.NEXTHOP6_DT next hops).  area: R's
+    area-0 ospfv3.Ospfv3Area image; gathers of R's row 0.  rc HSPF_E_UNSUPPORTED is returned in the result."""
+    from . import ospfv3
+    cells = np.ascontiguousarray(cells, RIB_CELL_DT)
+    assert cells.shape == (t.n_prefixes,)
+    gv = np.ascontiguousarray(gather_v, np.uint32)
+    gn = np.ascontiguousarray(gather_nh, np.uint64)
+    s = area.as_struct()
+    return _call_rib(capi.load_library().hspf_ospfv3_backbone_from_cells,
+                     (t.handle, C.byref(s), cells.ctypes.data, gv.ctypes.data, gn.ctypes.data, len(gv)),
+                     t.n_prefixes, RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)

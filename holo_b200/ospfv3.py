@@ -647,3 +647,131 @@ def abr_view(topos: list, seed: int, area_ids=None, roots=None, max_paths: int =
     for i, x in enumerate(ext_rows):
         externals[i] = x
     return areas, summaries, externals
+
+
+def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1, 0), (2, 1), (3, 2)),
+                  max_paths: int = 16, n_ext_keys: int = 3, t2: Topology | None = None):
+    """The OSPFv3 twin of ospfv2.backbone_view: a backbone router R of area 0 and the area border routers ("borders")
+    of one other area 1, each as its own image.  Seeded.  Area 0 is synth_area(t0) (router i is RID_BASE + i), area 1
+    synth_area(t1) with router ids, prefixes and interface sort keys in ranges of its own, except that border (i0, i1)
+    is router i0 of t0 and router i1 of t1, with one router id and the B flag in both areas.  The first border is also
+    attached to a small area 2 (t2, or a seeded 12-router topology; its router 0 is the border).  Returns a dict:
+      r_area        R's area-0 image (router r of t0);
+      summaries0    area 0's Inter-Area-Prefix LSAs (LsaKey order): each border's for the prefixes of its other areas
+                    it reaches, at its distance plus the prefix metric, with that prefix's options (what a job
+                    replaces);
+      externals     an ASBR of area 0 (the E flag) with AS-external LSAs for n_ext_keys area-1 loopbacks (prefixes
+                    that are also keys) and for one prefix of its own;
+      borders       per border (areas, area ids, inter-area LSAs per area): the first border lists area 1, area 0,
+                    area 2; the others area 0, area 1;
+      flip          (address bytes, length) of a /128 two routers of area 1 advertise, one with the LA option and
+                    one with the P option, at metrics that tie at the first border: the first border's route takes the
+                    lower router id's record, and a job that lengthens that router's path alone hands the route to
+                    the other record at the same metric, with other options;
+      shared        (address bytes, length) of a /64 that is intra-area in area 1 (LA) and area 2 (P) at metrics that
+                    tie at the first border (its route there keeps area 1's options, the first of its areas)."""
+    from . import ospf_rib, synth
+    from .ospfv2 import _dist_from
+    rng = np.random.default_rng(seed)
+    six = lambda hi, lo=0: ipaddress.IPv6Address((0x20010DB8 << 96) | (hi << 64) | lo).packed
+    rec = lambda b: (tuple(b), 1, (0, 0, 0))
+    if t2 is None:
+        t2 = synth.random_topology(12, 30, synth.SEED_BASE + 4000 + seed, cost_choices=[5, 10, 20])
+    rid0 = lambda i: RID_BASE + int(i)
+    bids = [rid0(i0) for i0, _ in borders]
+    cand = [i for i in range(t0.n_routers) if i != r and rid0(i) not in bids]
+    asbr = rid0(cand[int(rng.integers(0, len(cand)))])
+
+    def image(t, k, root, border_of):
+        """area k of topology t seen by `root`; border_of {router index: border router id}"""
+        rids = [border_of.get(i, RID_BASE + i + (k << 20)) for i in range(t.n_routers)]
+        a = synth_area(t, root=root, max_paths=max_paths, rids=rids, area_id=k)
+        pb = a.prefixes["addr"]["bytes"]
+        pb[:, 5] = pb[:, 5] + k
+        a.prefixes["addr"]["bytes"] = pb
+        ifs = a.ifaces.copy()
+        ifs["sort_key"] += 1000 * k
+        ifs["ifindex"] += 1000 * k
+        a.ifaces = ifs
+        rl = a.router_lsas.copy()
+        for b in border_of.values():
+            rl["flags"][rl["adv_rtr"] == b] |= 0x01
+        a.router_lsas = rl
+        return a
+
+    b0map = {i0: rid0(i0) for i0, _ in borders}
+    b1map = {i1: rid0(i0) for i0, i1 in borders}
+    b2map = {0: bids[0]}
+    img0 = lambda i: image(t0, 0, i, b0map)
+    r_area = img0(r)
+    a0s = [img0(i0) for i0, _ in borders]
+    a1s = [image(t1, 1, i1, b1map) for _, i1 in borders]
+    a2 = image(t2, 2, 0, b2map)
+    for a in [r_area] + a0s:
+        a.router_lsas["flags"][a.router_lsas["adv_rtr"] == asbr] |= 0x02
+
+    def dists(a):
+        fl = Flat(a)
+        d = _dist_from(fl, fl.router_vertex(a.router_id))
+        return {int(fl.router_ids[v]): int(d[v]) for v in range(len(fl.router_ids)) if fl.is_router[v] and d[v] < 1 << 40}
+    # the flip key: two area-1 routers tying at the first border, the lower id with LA
+    d1 = dists(a1s[0])
+    inner = sorted((d, rr) for rr, d in d1.items() if rr not in bids)
+    y = inner[0][1]                                      # the first border's nearest: its path is one link
+    xs = [rr for d, rr in inner if rr < y] or [rr for d, rr in inner[1:]]
+    x = xs[int(rng.integers(0, len(xs)))]
+    M = max(d1[x], d1[y]) + 5
+    flip = (six(0xF1_0000, 1), 128)
+    adds1 = {x: [(flip[0], 128, PFX_LA, M - d1[x])], y: [(flip[0], 128, PFX_P, M - d1[y])]}
+    # the shared key: area 1 and area 2 tying at the first border
+    d2 = dists(a2)
+    n1 = min((d, rr) for rr, d in d1.items() if rr not in bids)
+    n2 = min((d, rr) for rr, d in d2.items() if rr not in bids)
+    shared = (six(0xF2_0000), 64)
+    adds1.setdefault(n1[1], []).append((shared[0], 64, PFX_LA, 10 + max(0, n2[0] - n1[0])))
+    adds2 = {n2[1]: [(shared[0], 64, PFX_P, 10 + max(0, n1[0] - n2[0]))]}
+    a1s = [_with_prefixes(a, adds1) for a in a1s]
+    a2 = _with_prefixes(a2, adds2)
+    # each border's Inter-Area-Prefix LSAs into area 0: its other areas' prefixes that are not area 0's
+    own0 = {(bytes(int(b) for b in p["addr"]["bytes"]), int(p["len"])) for p in r_area.prefixes}
+    sums0 = []
+    for j, bid in enumerate(bids):
+        best = {}
+        for a in [a1s[j]] + ([a2] if j == 0 else []):
+            fl = Flat(a)
+            d = _dist_from(fl, fl.router_vertex(bid))
+            for l in a.iap_lsas:
+                v = fl.router_vertex(int(l["adv_rtr"])) if int(l["ref_type"]) == REF_ROUTER else 0xFFFFFFFF
+                if v == 0xFFFFFFFF or d[v] >= 1 << 40:
+                    continue
+                for p in a.prefixes[int(l["prefix_off"]): int(l["prefix_off"]) + int(l["n_prefixes"])]:
+                    key = (bytes(int(b) for b in p["addr"]["bytes"]), int(p["len"]))
+                    m = int(d[v]) + int(p["metric"])
+                    if key in own0 or int(p["options"]) & PFX_NU or (key in best and best[key][0] <= m):
+                        continue
+                    best[key] = (m, int(p["options"]))
+        for n, (key, (m, opt)) in enumerate(sorted(best.items())):
+            sums0.append((bid, n + 1, m, 0, rec(key[0]), key[1], opt, 3, 0))
+    sums0.sort(key=lambda x: (x[7], x[0], x[1]))
+    summaries0 = np.zeros(len(sums0), ospf_rib.INTER_AREA_LSA_DT)
+    for i, x in enumerate(sums0):
+        summaries0[i] = x
+    loops = sorted({(bytes(int(b) for b in p["addr"]["bytes"]), int(p["len"])) for p in a1s[0].prefixes
+                    if int(p["len"]) == 128 and (bytes(int(b) for b in p["addr"]["bytes"]), 128) != flip})
+    keys = [loops[int(i)] for i in rng.choice(len(loops), min(n_ext_keys, len(loops)), replace=False)]
+    ext = [(asbr, j + 1, int(rng.choice([5, 30])), 7, rec(k[0]), k[1], PFX_P if j == 1 else 0, int(j % 2), 0)
+           for j, k in enumerate(keys)]
+    ext.append((asbr, len(keys) + 1, 12, 8, rec(six(0xE0_0000)), 64, 0, 1, 0))
+    externals = np.zeros(len(ext), ospf_rib.EXTERNAL6_LSA_DT)
+    for i, x in enumerate(sorted(ext, key=lambda x: (x[0], x[1]))):
+        externals[i] = x
+    empty = np.zeros(0, ospf_rib.INTER_AREA_LSA_DT)
+    out_borders = []
+    for j, (a0, a1) in enumerate(zip(a0s, a1s)):
+        s0 = summaries0[summaries0["adv_rtr"] != a0.router_id]
+        if j == 0:
+            out_borders.append(([a1, a0, a2], [1, 0, 2], [empty, s0, empty]))
+        else:
+            out_borders.append(([a0, a1], [0, 1], [s0, empty]))
+    return {"r_area": r_area, "summaries0": summaries0, "externals": externals, "borders": out_borders,
+            "flip": flip, "shared": shared, "asbr": asbr}

@@ -399,6 +399,41 @@ int hspf_ospfv2_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
                                     uint32_t n_gather, hl_ospfv2_rib *out);
 
 /*
+ * The same stage for OSPFv3.  The table is an hspf_ospfv2_backbone_table marked OSPFv3; the cells and delta calls
+ * above take it (the table's mark picks the walk), and each version's create and decode refuse the other version's
+ * tables (HSPF_E_INVAL).  For job j, with border b's ABR cells of j decoded to rib_b (hspf_ospfv3_abr_rib_from_cells),
+ * the decoded cells of j equal the affected-prefix routes, prefix options included, of
+ *     hspf_ospfv3_update_rib_full(R, max_paths, [{0, area_from_planes(area 0, R's row 0), ifaces, S_j, 1}], X)
+ * where S_j is area 0's Inter-Area-Prefix / Inter-Area-Router LSAs with each border's Inter-Area-Prefix LSAs
+ * replaced by hspf_ospfv3_net_summaries(rib_b, target area 0), in LsaKey order.  A border advertises a route as the
+ * OSPFv2 stage says, and its LSA carries the prefix options of the border cell's winning intra-area record, as the
+ * OSPFv3 intra-area decode reads them.  A slot's winner is n_records + (slot index << 8 | those options): a border
+ * route that changes record at an equal metric, to one with other options, changes R's winner, and the route-delta
+ * stage reports OTHER.
+ *
+ *   hspf_ospfv3_backbone_table_create  host.  As hspf_ospfv2_backbone_table_create, over R's OSPFv3 area-0 flat, area
+ *                                0's Inter-Area-Prefix / Inter-Area-Router LSAs in LsaKey order, the AS-external LSAs
+ *                                and the borders' OSPFv3 ABR tables.  Inter-Area-Prefix LSAs with the NU option are
+ *                                left out, as update_rib_full leaves them out.  Refusals: those of the OSPFv2 call,
+ *                                with an OSPFv2 border table HSPF_E_INVAL, a usable Inter-Area-Router LSA from a border
+ *                                HSPF_E_UNSUPPORTED, and slot winners that would not fit 32 bits HSPF_E_UNSUPPORTED.
+ *   hspf_ospfv3_backbone_table_prefixes6  P, and the IPv6 prefixes / lengths in prefix order (pointers may be NULL);
+ *                                HSPF_E_INVAL for an OSPFv2 table.
+ *   hspf_ospfv3_backbone_from_cells host: one job's cells -> the table of the contract, a slot winner's prefix options
+ *                                read from the winner.  area: R's area-0 image; gathers as hspf_ospfv2_backbone_from_cells.
+ */
+int hspf_ospfv3_backbone_table_create(const struct hspf_ospfv3_flat *flat, uint32_t router_id,
+                                      const hl_ospfv3_inter_area_lsa *summaries, uint32_t n_summaries,
+                                      const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
+                                      const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                      hspf_ospfv2_backbone_table **out);
+int hspf_ospfv3_backbone_table_prefixes6(const hspf_ospfv2_backbone_table *t, uint32_t *n_prefixes,
+                                         const hl_ip_addr **prefixes, const uint32_t **lens);
+int hspf_ospfv3_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const hl_ospfv3_area *area,
+                                    const hl_ospf_rib_cell *cells, const uint32_t *gather_v, const uint64_t *gather_nh,
+                                    uint32_t n_gather, hl_ospfv3_rib *out);
+
+/*
  * The stages of update_rib_full that follow the per-area SPFs (holo-ospf/src/route.rs:146-193):
  * merges the intra-area routes of the attached areas (route_update / route_compare,
  * route.rs:895-971), adds inter-area network routes and inter-area router entries from the
@@ -443,6 +478,17 @@ typedef struct hl_ospf_area_config {
 int hspf_ospfv2_net_summaries(uint32_t router_id, const hl_ospfv2_rib *rib, const hl_ospfv2_rtr_tables *rtrs,
                               const hl_ospfv2_rib_area *areas, const hl_ospf_area_config *config, uint32_t n_areas,
                               uint32_t target, hl_ospfv2_summary_lsa *out, uint32_t cap, uint32_t *n_out);
+/*
+ * The Inter-Area-Prefix contents an OSPFv3 area border router originates into one target area (compute_net_summaries,
+ * lsa_orig_inter_area_network of holo-ospf ospfv3/lsdb.rs:341-386), over hspf_ospfv3_update_rib_full's table: the
+ * type-3 rules of hspf_ospfv2_net_summaries, each LSA carrying its route's prefix options (the default route of a stub
+ * area: ::/0 at default_cost, options 0).  out[0, *n_out): lsa_type 3, adv_rtr = router_id, lsa_id 0, the prefix, its
+ * length, prefix options and metric, in prefix order.  Inter-Area-Router contents are not computed.  HSPF_E_NOMEM
+ * with *n_out set when cap is too small.  Host only.
+ */
+int hspf_ospfv3_net_summaries(uint32_t router_id, const hl_ospfv3_rib *rib, const hl_ospfv3_rib_area *areas,
+                              const hl_ospf_area_config *config, uint32_t n_areas, uint32_t target,
+                              hl_ospfv3_inter_area_lsa *out, uint32_t cap, uint32_t *n_out);
 
 /*
  * update_global_rib (holo-ospf/src/route.rs:833-893): compares the freshly computed table with
