@@ -20,6 +20,7 @@
 // not a B-flag router vertex, self-originated LSAs) are applied when the table is built.
 #pragma once
 #include <cstdint>
+#include <unordered_map>
 
 #include "ospf_rib_cells.h"
 
@@ -207,6 +208,7 @@ struct hspf_ospfv2_abr_ribtable {
     std::vector<hspf::RibRec> recs;
     std::vector<uint32_t> v_flagged, vl_off;
     std::vector<uint32_t> ext_tag;                 // per type-5 record (index - ext_base)
+    std::vector<std::unordered_map<uint32_t, uint32_t>> rtr_vertex;   // per area: router id -> router vertex
     // OSPFv3 tables (hspf_ospfv3_abr_ribtable_create): each area's table is an OSPFv3 one-area table, `prefix` is
     // zero-filled (the prefixes are prefix6), and options6 holds the prefix options per type-3 / type-5 record
     // (index - t3_base[0], the first type-3 record)

@@ -21,6 +21,7 @@
 // (the route-delta stage reports OTHER), and the decode reads the options from the winner alone.
 #pragma once
 #include <cstdint>
+#include <utility>
 #include <vector>
 
 #include "ospf_abr_rib_cells.h"
@@ -51,6 +52,66 @@ struct OspfBackboneView {
 // One job's row of every border's cells.
 struct OspfBorderRows {
     const hl_ospf_rib_cell *row[kOspfBackboneMaxBorders];
+};
+
+// Type-4 slots (OSPFv2, hspf_ospfv2_backbone_asbr_table_create).  A border originates a type-4 LSA into area 0 for an
+// ASBR A (compute_rtr_summaries, ospf_rib_host.cc: hspf_ospfv2_net_summaries) when A is a router of one of its
+// non-backbone areas with the E flag and the border reaches A in that area below LSInfinity; its metric is that
+// distance, and an id in two such areas keeps the later area's entry.  In R's type-4 range for A (walked from the end,
+// as rib_full's step 2 lets the last usable LSA replace the entry) each border has one slot per such area, in area
+// order, at the border's place in LsaKey order:
+//   static: x ABR vertex, y LSA metric, z 0, w 0 (as in ospf_rib_cells.h)
+//   slot:   x the border's vertex, y A's vertex in the slot's area, z the border, w kOspfBackboneAsbrSlot | plane set
+// A plane set is one (border, non-backbone area) pair; a call reads at most kOspfBackboneMaxAsbrSets of them.
+constexpr uint32_t kOspfBackboneMaxAsbrSets = 8;
+constexpr uint32_t kOspfBackboneAsbrSlot = 0x80000000u;
+
+// The plane sets a table's type-4 slots read: set k is area `area[k]` of a border whose rows are rows[k][job][stride[k]]
+// (< n_rows[k]), each row V[k] vertices of dist[k] and a status word (status[k] may be NULL).
+template <class D>
+struct OspfAsbrSets {
+    const D *dist[kOspfBackboneMaxAsbrSets];
+    const uint32_t *status[kOspfBackboneMaxAsbrSets];
+    const uint32_t *rows[kOspfBackboneMaxAsbrSets];
+    uint32_t V[kOspfBackboneMaxAsbrSets], n_rows[kOspfBackboneMaxAsbrSets];
+    uint32_t stride[kOspfBackboneMaxAsbrSets], area[kOspfBackboneMaxAsbrSets];
+    uint32_t n;
+    HSPF_HD uint32_t row(uint32_t k, uint32_t j) const { return rows[k][(size_t)j * stride[k] + area[k]]; }
+};
+
+// The OR of the job's rows' status words over the sets, HSPF_JS_INVALID for a row out of range (read before any plane).
+template <class D>
+HSPF_HD uint32_t asbr_job_status(const OspfAsbrSets<D> &s, uint32_t j) {
+    uint32_t st = 0;
+    for (uint32_t k = 0; k < s.n; ++k) {
+        const uint32_t r = s.row(k, j);
+        if (r >= s.n_rows[k]) st |= HSPF_JS_INVALID;
+        else if (s.status[k]) st |= s.status[k][r];
+    }
+    return st;
+}
+
+// One job of the sets: whether the border of set k originates a type-4 LSA for the ASBR at vertex v of its area, and
+// at what metric.  The intra-area entry of a non-backbone area only has that area's next hops, so the rule that no
+// next hop may be on an area-0 interface (nexthops_area_check) always holds here.
+template <class Planes, class D>
+struct OspfAsbrJob {
+    const OspfAsbrSets<D> &s;
+    uint32_t j;
+    HSPF_HD bool originates(uint32_t k, uint32_t v, uint32_t &metric) const {
+        const Planes pl{s.dist[k] + (size_t)s.row(k, j) * s.V[k], nullptr, nullptr};
+        if (!pl.reached(v)) return false;
+        metric = pl.d(v);
+        return metric < HL_LSA_INFINITY;
+    }
+};
+
+// R's planes of a job over a table with type-4 slots, with the job's plane sets beside them.  (The accessor rides
+// with the planes, which stay in registers, and not with the border rows, which the walk indexes at run time: a
+// reference to the kernel parameter stored there would copy the whole parameter to local memory.)
+template <class Planes, class D>
+struct OspfAsbrPlanes : Planes {
+    OspfAsbrJob<Planes, D> asbr;
 };
 
 // What border b advertises into area 0 for the prefix of its cell c: false when nothing, else its metric and, for
@@ -87,7 +148,8 @@ HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, u
 }
 
 // kV3: the table is an OSPFv3 one (hspf_ospfv3_backbone_table_create), whose slot winners carry prefix options.
-template <bool kV3 = false, class Planes>
+// kAsbr: the table's type-4 ranges hold slots, read through pl.asbr (pl an OspfAsbrPlanes of the job).
+template <bool kV3 = false, bool kAsbr = false, class Planes>
 HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneView &t, uint32_t p,
                                           const OspfBorderRows &rows) {
     const RouteContrib *contribs = reinterpret_cast<const RouteContrib *>(t.recs);
@@ -124,7 +186,14 @@ HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneVi
         for (uint32_t k = s.w; k > s.z; --k) {
             const RibRec f = load_rib_rec(t.recs + k - 1);
             if (f.x == t.root || !pl.reached(f.x)) continue;
-            em = pl.d(f.x) + f.y; en = pl.n(f.x); have = true;
+            if constexpr (kAsbr) {
+                uint32_t fm = f.y;                                      // a border that does not originate: go on
+                if ((f.w & kOspfBackboneAsbrSlot) && !pl.asbr.originates(f.w & ~kOspfBackboneAsbrSlot, f.y, fm)) continue;
+                em = pl.d(f.x) + fm;
+            } else {
+                em = pl.d(f.x) + f.y;
+            }
+            en = pl.n(f.x); have = true;
             break;
         }
         if (!have) {
@@ -161,6 +230,10 @@ struct hspf_ospfv2_backbone_table {
     std::vector<uint32_t> ext_tag;               // per type-5 record of the view (index - ext_base)
     uint32_t ext_base = 0;
     const hspf_ospfv2_abr_ribtable *borders[hspf::kOspfBackboneMaxBorders] = {};
+    // hspf_ospfv2_backbone_asbr_table_create: the type-4 slot count and the plane sets they read, (border, area index
+    // in the border's table); a table with type-4 slots is read only by the asbr calls
+    uint32_t n_asbr_slots = 0;
+    std::vector<std::pair<uint32_t, uint32_t>> asbr_set;
     // OSPFv3 tables (hspf_ospfv3_backbone_table_create): `prefix` is zero-filled (the prefixes are prefix6), and
     // options6 holds the prefix options of each type-3 / type-5 record of the view (index - o3[0]); a slot's entry is
     // a placeholder, its options come from its winner

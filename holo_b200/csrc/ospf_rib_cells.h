@@ -126,6 +126,7 @@ struct hspf_ospfv2_ribtable {
     std::vector<uint8_t> vflags;             // [V] Router-LSA flags of router vertices
     uint32_t n_intra = 0, ext_base = 0, ext_end = 0;
     std::vector<uint32_t> ext_tag;           // per type-5 record (index - ext_base): the LSA's tag
+    std::vector<uint32_t> asbr_id;           // per ASBR record (index - ext_end): the ASBR's router id
     // OSPFv3 tables (hspf_ospfv3_ribtable_create): `intra` is an OSPFv3 rtable, `prefix` is zero-filled (the prefixes
     // are intra->t.prefix6 merged with the LSAs' in prefix6), and options6 holds the prefix options per type-3 /
     // type-5 record (index - n_intra)

@@ -181,6 +181,7 @@ int build_rib_records(hspf_ospfv2_ribtable &rt, uint32_t area_id, RouterVertex r
         t4_at += (uint32_t)t4[s].size();
     }
     for (const auto &l : t4) rt.recs.insert(rt.recs.end(), l.begin(), l.end());
+    rt.asbr_id = slot_id;
     return HSPF_OK;
 }
 
@@ -234,6 +235,7 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
             rc = T::area_table(flats[i], area_ids[i], sums.data(), (uint32_t)sums.size(), ext, n_ext, true, &rt);
             if (rc) return rc;
             t->area.push_back(rt);
+            t->rtr_vertex.push_back(f.rtr_vertex);
             t->area_id.push_back(area_ids[i]);
             t->root.push_back(root);
             t->n_vertices.push_back(T::n_vertices(f));
@@ -346,11 +348,13 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
 // hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create, argument checks included: R's one-area table
 // over area 0 without the borders' type-3 LSAs, and per affected prefix R's intra-area records, its static type-3
 // records with one slot per (border, prefix) at the border's place in LsaKey order, and its type-5 records
-// (ospf_backbone_cells.h).  Border tables of the other version are refused (HSPF_E_INVAL).
+// (ospf_backbone_cells.h).  Border tables of the other version are refused (HSPF_E_INVAL).  `asbr`
+// (hspf_ospfv2_backbone_asbr_table_create): the borders' type-4 LSAs are re-originated per job too, as type-4 slots,
+// and the prefixes of the type-5 LSAs they lead to are affected; else a usable one is HSPF_E_UNSUPPORTED.
 template <class T>
 int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const typename T::Sum *sums, uint32_t n_sums,
                          const typename T::Ext *ext, uint32_t n_ext, const hspf_ospfv2_abr_ribtable *const *borders,
-                         uint32_t n_borders, hspf_ospfv2_backbone_table **out) {
+                         uint32_t n_borders, hspf_ospfv2_backbone_table **out, bool asbr = false) {
     using Key = typename T::Key;
     using Sum = typename T::Sum;
     constexpr uint32_t kNone = 0xFFFFFFFFu;
@@ -384,17 +388,51 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         auto live = [](const Sum &l) { return !l.maxage && l.metric < HL_LSA_INFINITY && !T::skip(l); };
         std::vector<Sum> rest;
         std::vector<std::pair<uint32_t, Key>> border_t3;            // (border, prefix key) of the borders' LSAs
+        std::vector<std::pair<uint32_t, uint32_t>> border_t4;       // (border, ASBR id)
         for (uint32_t i = 0; i < n_sums; ++i) {
             const Sum &l = sums[i];
             auto it = border_of.find(l.adv_rtr);
             if (it == border_of.end()) { rest.push_back(l); continue; }
             if (!live(l)) continue;
-            if (l.lsa_type == 4) return HSPF_E_UNSUPPORTED;         // re-originated per job too
+            if (l.lsa_type == 4) {                                   // re-originated per job too
+                if (!asbr) return HSPF_E_UNSUPPORTED;
+                border_t4.emplace_back(it->second, T::asbr_id(l));
+            }
             if (l.lsa_type == 3) border_t3.emplace_back(it->second, T::key(l));
         }
         int rc = T::area_table(flat, 0, rest.data(), (uint32_t)rest.size(), ext, n_ext, false, &t->r);
         if (rc) return rc;
         const hspf_ospfv2_ribtable &r = *t->r;
+        // type-4 slots: per ASBR id, the (border, area index) pairs of the borders' non-backbone areas where it is a
+        // router with the E flag, each border's in area order
+        std::map<uint32_t, std::vector<std::pair<uint32_t, uint32_t>>> orig;
+        if (asbr) {
+            for (uint32_t b = 0; b < n_borders; ++b) {
+                const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+                for (uint32_t i = 0; i < bt.n_areas; ++i) {
+                    if (bt.area_id[i] == 0) continue;
+                    for (const auto &e : bt.rtr_vertex[i]) {
+                        const uint8_t fl = bt.area[i]->vflags[e.second];
+                        if (!(fl & HL_RTR_FLAG_E)) continue;
+                        // its entry at R would replace an ABR's (as hspf_ospfv2_ribtable_create refuses)
+                        if (fl & HL_RTR_FLAG_B) return HSPF_E_UNSUPPORTED;
+                        orig[e.first].emplace_back(b, i);
+                    }
+                }
+            }
+            for (auto &e : orig)
+                std::stable_sort(e.second.begin(), e.second.end(), [&](const std::pair<uint32_t, uint32_t> &x,
+                                                                       const std::pair<uint32_t, uint32_t> &y) {
+                    return borders[x.first]->router_id < borders[y.first]->router_id;
+                });
+            for (const auto &x : border_t4) {
+                auto it = orig.find(x.second);
+                bool found = false;
+                if (it != orig.end())
+                    for (const auto &o : it->second) found = found || o.first == x.first;
+                if (!found) return HSPF_E_INVAL;                     // the LSDB disagrees with the border's table
+            }
+        }
         // the affected prefixes: each border's prefixes with an intra-area record in one of its non-backbone areas
         std::map<Key, std::vector<std::pair<uint32_t, uint32_t>>> slots;   // key -> (border, its prefix index)
         for (uint32_t b = 0; b < n_borders; ++b) {
@@ -414,6 +452,15 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                 for (const auto &s : it->second) found = found || s.first == x.first;
             if (!found) return HSPF_E_INVAL;                         // the LSDB disagrees with the border's table
         }
+        // ... and the prefixes of the type-5 LSAs of an ASBR some border can originate a type-4 LSA for
+        const uint32_t *rx = r.off.data() + 2 * (r.prefix.size() + 1);
+        if (!orig.empty())
+            for (uint32_t u = 0; u < (uint32_t)r.prefix.size(); ++u)
+                for (uint32_t k = rx[u]; k < rx[u + 1]; ++k)
+                    if (orig.count(r.asbr_id[r.recs[k].x - r.ext_end])) {
+                        slots[T::table_key(r, u)];
+                        break;
+                    }
         // R's static type-3 records per prefix, in LsaKey order: (adv_rtr, ABR vertex, metric, prefix options)
         std::map<Key, std::vector<std::array<uint32_t, 4>>> statics;
         for (const Sum &l : rest) {
@@ -472,6 +519,45 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
             }
         }
         o5[P] = (uint32_t)t->recs.size();
+        if (!orig.empty()) {
+            // each such ASBR's type-4 range again, at the end: its static records (R's one-area table has them in
+            // LSDB order) with the borders' slots at their LsaKey places (by advertising router)
+            std::map<uint32_t, std::vector<std::pair<uint32_t, RibRec>>> t4;   // ASBR id -> (adv_rtr, static record)
+            for (const Sum &l : rest) {
+                if (l.lsa_type != 4 || !live(l)) continue;
+                const uint32_t v = vertex(l.adv_rtr);
+                if (flags(v) & HL_RTR_FLAG_B) t4[T::asbr_id(l)].push_back({l.adv_rtr, RibRec{v, l.metric, 0, 0}});
+            }
+            std::map<std::pair<uint32_t, uint32_t>, uint32_t> set_of;
+            for (uint32_t a = 0; a < (uint32_t)r.asbr_id.size(); ++a) {
+                const uint32_t id = r.asbr_id[a];
+                auto o = orig.find(id);
+                if (o == orig.end()) continue;
+                const auto &ob = o->second;
+                const auto st = t4.find(id);
+                const uint32_t z = (uint32_t)t->recs.size();
+                size_t k = 0;
+                auto put_slot = [&]() {
+                    const uint32_t b = ob[k].first, i = ob[k].second;
+                    auto ins = set_of.emplace(ob[k], (uint32_t)t->asbr_set.size());
+                    if (ins.second) t->asbr_set.push_back(ob[k]);
+                    t->recs.push_back(RibRec{bv[b], borders[b]->rtr_vertex[i].at(id), b,
+                                             kOspfBackboneAsbrSlot | ins.first->second});
+                    ++t->n_asbr_slots;
+                    ++k;
+                };
+                if (st != t4.end())
+                    for (const auto &x : st->second) {
+                        while (k < ob.size() && borders[ob[k].first]->router_id < x.first) put_slot();
+                        t->recs.push_back(x.second);
+                    }
+                while (k < ob.size()) put_slot();
+                RibRec &s = t->recs[r.ext_end + a];
+                s.z = z;
+                s.w = (uint32_t)t->recs.size();
+            }
+            if (t->asbr_set.size() > kOspfBackboneMaxAsbrSets) return HSPF_E_UNSUPPORTED;   // the kernel parameter's
+        }
         // winners are u32: a slot's is n_recs + its index (OSPFv3: n_recs + (index << 8 | options))
         const uint64_t n_slots = t->slot_rec.size();
         if ((uint64_t)t->recs.size() + (T::kV3 ? n_slots << 8 : n_slots) >= kNone) return HSPF_E_UNSUPPORTED;

@@ -43,10 +43,30 @@ struct OspfBackboneCell {
     __device__ static hspf::CellWords empty() { return {0, 0, hspf::kNoRecord}; }
 };
 
+// The walk over a table with type-4 slots (hspf_ospfv2_backbone_asbr_table_create): the same, plus the plane sets the
+// slots read, whose rows enter the job's status word.
+template <class Planes>
+struct OspfBackboneAsbrCell : OspfBackboneCell<Planes, false> {
+    using Base = OspfBackboneCell<Planes, false>;
+    hspf::OspfAsbrSets<typename Base::Rows::D> sets;
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
+        return Base::status_word(j) | hspf::asbr_job_status(sets, j);
+    }
+    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
+        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {sets, j}};
+        return hspf::ospf_backbone_cell_eval<false, true>(pl, this->t, p, rows);
+    }
+};
+
 // Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
-// and for OSPFv3 tables.
+// and for OSPFv3 tables, and for OSPFv2 tables with type-4 slots.
 constexpr uint32_t kBackboneBlocksPerSM = 4;
 constexpr uint32_t kBackboneV3BlocksPerSM = 4;
+constexpr uint32_t kBackboneAsbrBlocksPerSM = 4;
 
 template <class R, bool kV3>
 int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
@@ -90,12 +110,12 @@ int version_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n
         ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
-// the walk of the table's version
+// the walk of the table's version; a table with type-4 slots is the asbr calls'
 template <class R>
 int backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
                    const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                    uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    if (!t) return HSPF_E_INVAL;
+    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
     return t->v3 ? version_cells<true>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells)
                  : version_cells<false>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
 }
@@ -105,11 +125,71 @@ int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t 
                    const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                    const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                    hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    if (!t) return HSPF_E_INVAL;
+    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
     return t->v3 ? version_delta<true>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of,
                                         job_out, records, cap, n_records)
                  : version_delta<false>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base,
                                          base_of, job_out, records, cap, n_records);
+}
+
+// The cell over a table with type-4 slots: the plane sets the slots name, from each border's planes, row counts and
+// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]).
+template <class R>
+int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
+                   const uint32_t *const *border_status, const R *const *border_planes,
+                   const uint32_t *const *border_n_rows, const uint32_t *const *border_rows, uint32_t n_jobs,
+                   OspfBackboneAsbrCell<hspf::PlanesOf<R>> &cell) {
+    if (!t || t->v3) return HSPF_E_INVAL;
+    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
+    if (!border_planes || !border_n_rows || (n_jobs && !border_rows)) return HSPF_E_INVAL;
+    auto &s = cell.sets;
+    s.n = (uint32_t)t->asbr_set.size();
+    for (uint32_t k = 0; k < s.n; ++k) {
+        const uint32_t b = t->asbr_set[k].first, i = t->asbr_set[k].second;
+        if (!border_planes[b] || !border_n_rows[b] || (n_jobs && !border_rows[b])) return HSPF_E_INVAL;
+        hspf::ResultPlanes<hspf::PlanesOf<R>> p;
+        if (hspf::result_planes(&border_planes[b][i], t->borders[b]->n_vertices[i], p) || !p.complete())
+            return HSPF_E_INVAL;
+        s.dist[k] = p.dist; s.status[k] = p.status; s.V[k] = p.V;
+        s.rows[k] = border_rows[b]; s.n_rows[k] = border_n_rows[b][i];
+        s.stride[k] = t->borders[b]->n_areas; s.area[k] = i;
+    }
+    return HSPF_OK;
+}
+
+// A table without type-4 slots takes the calls above (NULL border planes allowed).
+template <class R>
+int backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                        const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                        const R *const *border_planes, const uint32_t *const *border_n_rows,
+                        const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    if (!t || t->v3) return HSPF_E_INVAL;
+    if (!t->n_asbr_slots) return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+    OspfBackboneAsbrCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                      n_jobs, cell))
+        return rc;
+    return hspf::launch_route_cells<kBackboneAsbrBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out,
+                                                              0, nullptr, nullptr, nullptr, nullptr);
+}
+
+template <class R>
+int backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                        const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                        const R *const *border_planes, const uint32_t *const *border_n_rows,
+                        const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                        const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                        uint64_t *n_records) {
+    if (!t || t->v3) return HSPF_E_INVAL;
+    if (!t->n_asbr_slots)
+        return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
+                              records, cap, n_records);
+    OspfBackboneAsbrCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                      n_jobs, cell))
+        return rc;
+    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBackboneAsbrBlocksPerSM>(
+        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
 }  // namespace
@@ -149,6 +229,46 @@ int hspf_ospfv2_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table
                                  hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
     return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
                           records, cap, n_records);
+}
+
+int hspf_ospfv2_backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                    const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                    const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                    const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                    uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    return backbone_asbr_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                               border_rows, job_status_out, cells);
+}
+
+int hspf_ospfv2_backbone_asbr_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                      const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                      const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                      const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                      uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    return backbone_asbr_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                               border_rows, job_status_out, cells);
+}
+
+int hspf_ospfv2_backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                    const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                    const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                    const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                    const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                    hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                    uint64_t *n_records) {
+    return backbone_asbr_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                               border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                      const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                      const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                      const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                      const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                      hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                      uint64_t *n_records) {
+    return backbone_asbr_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                               border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
 }  // extern "C"

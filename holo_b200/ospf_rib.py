@@ -625,20 +625,27 @@ class BackboneTable:
 
     From an ospfv3.Flat the table is hspf_ospfv3_backbone_table_create's (summaries: INTER_AREA_LSA_DT, externals:
     EXTERNAL6_LSA_DT, borders: OSPFv3 AbrRibTables); `prefix` and `prefixes6` then hold the IPv6 prefixes
-    (ospfv3.IP_DT), `v3` is set, and a slot's winner is n_records + (slot index << 8 | its prefix options)."""
+    (ospfv3.IP_DT), `v3` is set, and a slot's winner is n_records + (slot index << 8 | its prefix options).
 
-    def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=()):
+    asbr=True (OSPFv2): hspf_ospfv2_backbone_asbr_table_create, which re-originates the borders' type-4 LSAs per job
+    too; `n_asbr_slots` type-4 slots read `n_asbr_sets` (border, area) plane sets, and a table with type-4 slots is
+    read by backbone_asbr_cells_device / backbone_asbr_delta_device only."""
+
+    def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=(), asbr: bool = False):
         from . import ospfv3
         self.lib = capi.load_library()
         self.flat, self.router_id, self.borders = flat, router_id, list(borders)
         self.v3 = isinstance(flat, ospfv3.Flat)
+        if asbr and self.v3:
+            raise ValueError("type-4 slots are OSPFv2 only")
         sum_dt, ext_dt = (INTER_AREA_LSA_DT, EXTERNAL6_LSA_DT) if self.v3 else (SUMMARY_LSA_DT, EXTERNAL_LSA_DT)
         sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, sum_dt), sum_dt)
         ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, ext_dt), ext_dt)
         self.summaries, self.externals = sm, ext
         arr = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
         h = C.c_void_p()
-        create = "hspf_ospfv3_backbone_table_create" if self.v3 else "hspf_ospfv2_backbone_table_create"
+        create = ("hspf_ospfv3_backbone_table_create" if self.v3 else
+                  "hspf_ospfv2_backbone_asbr_table_create" if asbr else "hspf_ospfv2_backbone_table_create")
         rc = getattr(self.lib, create)(flat.handle, router_id, sm.ctypes.data if len(sm) else None, len(sm),
                                        ext.ctypes.data if len(ext) else None, len(ext), arr, len(self.borders),
                                        C.byref(h))
@@ -653,6 +660,9 @@ class BackboneTable:
         nr, ns = C.c_uint32(), C.c_uint32()
         assert self.lib.hspf_ospfv2_backbone_table_records(h, C.byref(nr), C.byref(ns)) == capi.HSPF_OK
         self.n_records, self.n_slots = nr.value, ns.value
+        na, nsets = C.c_uint32(), C.c_uint32()
+        assert self.lib.hspf_ospfv2_backbone_table_asbr_slots(h, C.byref(na), C.byref(nsets)) == capi.HSPF_OK
+        self.n_asbr_slots, self.n_asbr_sets = na.value, nsets.value
         if self.v3:
             p6 = C.c_void_p()
             rc = self.lib.hspf_ospfv3_backbone_table_prefixes6(h, None, C.byref(p6), None)
@@ -699,6 +709,43 @@ def backbone_delta_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, 
     st = _device_ptrs(border_status) if border_status is not None else None
     route_table.call_stage(ctx, "hspf_ospfv2_backbone_delta", rs, t.handle, n_jobs, C.byref(rs),
                            _device_ptrs(border_cells), st, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+
+
+def _border_plane_args(border_planes, border_n_rows, border_rows, keep: list):
+    """The three per-border arrays of the asbr calls (None: NULL)."""
+    if border_planes is None:
+        return None, None, None
+    pl = [_planes_array(p) for p in border_planes]
+    nr = [np.ascontiguousarray(x, np.uint32) for x in border_n_rows]
+    keep += [pl, nr]
+    return (C.c_void_p * len(pl))(*[C.addressof(p) for p in pl]), (C.c_void_p * len(nr))(*[x.ctypes.data for x in nr]), \
+        _device_ptrs(border_rows)
+
+
+def backbone_asbr_cells_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
+                               border_planes, border_n_rows, border_rows, status_ptr: int, cells_ptr: int):
+    """hspf_ospfv2_backbone_asbr_cells / _cells16: backbone_cells_device over a table with type-4 slots, plus per
+    border its DEVICE planes (one capi.ResultStruct / Result16Struct per area, as given abr_rib_cells_device, of R's
+    width), its row counts per area, and a device pointer to its rows u32 [n_jobs, n_areas].  The three may be None
+    for a table without type-4 slots."""
+    keep = []
+    st = _device_ptrs(border_status) if border_status is not None else None
+    bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)
+    route_table.call_stage(ctx, "hspf_ospfv2_backbone_asbr_cells", rs, t.handle, n_jobs, C.byref(rs),
+                           _device_ptrs(border_cells), st, bp, bn, br, status_ptr or None, cells_ptr or None)
+
+
+def backbone_asbr_delta_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
+                               border_planes, border_n_rows, border_rows, base_ptr: int, n_base: int, base_of_ptr: int,
+                               job_out_ptr: int, records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_ospfv2_backbone_asbr_delta / _delta16: the route-delta stage over the same walk (arguments as
+    backbone_asbr_cells_device and rib_delta_device)."""
+    keep = []
+    st = _device_ptrs(border_status) if border_status is not None else None
+    bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)
+    route_table.call_stage(ctx, "hspf_ospfv2_backbone_asbr_delta", rs, t.handle, n_jobs, C.byref(rs),
+                           _device_ptrs(border_cells), st, bp, bn, br, base_ptr or None, n_base, base_of_ptr or None,
                            job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
 
 

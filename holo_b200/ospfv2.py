@@ -806,7 +806,7 @@ def _set_flags(a: Ospfv2Area, flags: dict) -> Ospfv2Area:
 
 
 def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1, 0), (2, 1), (3, 2)),
-                  max_paths: int = 16, n_ext_keys: int = 3):
+                  max_paths: int = 16, n_ext_keys: int = 3, area1_asbrs: int = 0, area1_ext: int = 4):
     """A backbone router R of area 0 and the area border routers ("borders") of one other area 1, each as its own
     image.  Seeded.  Area 0 is synth_area(t0) (router i is RID_BASE + i), area 1 synth_area(t1) moved into ranges of
     its own, except that border (i0, i1) is router i0 of t0 and router i1 of t1, with one router id and the B flag in
@@ -819,7 +819,12 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
       borders       per border (areas [area 0 image, area 1 image], area ids, summaries per area) in that area order,
                     except that the first border lists area 1 first;
       shared        a /24 that is a stub of a neighbour of the first border in area 0 and in area 1, at metrics that
-                    tie at that border (its route there is intra-area in both areas and carries area-0 atoms)."""
+                    tie at that border (its route there is intra-area in both areas and carries area-0 atoms).
+    area1_asbrs = k > 0 (drawn from a generator of its own, so that every other part is as without it): k routers of
+    area 1 get the E flag ("area1_asbrs" in the dict) and area1_ext type-5 LSAs each, both E-bit values, on /24s that
+    the next ASBR shares in half, plus the area-0 ASBR's own /24 at its type-2 metric; summaries0 then also holds each
+    border's type-4 LSAs for those it reaches in area 1, at that distance.  A border left out of a backbone table keeps
+    its type-3 / type-4 LSAs as another ABR's static ones."""
     from . import ospf_rib
     rng = np.random.default_rng(seed)
     rid0 = lambda i: RID_BASE + int(i)
@@ -834,6 +839,12 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
     r_area = img0(r)
     b0 = [img0(i0) for i0, _ in borders]
     b1 = [img1(i1) for _, i1 in borders]
+    asbrs1 = []
+    if area1_asbrs:
+        rng1 = np.random.default_rng([seed, 0xA5B])
+        cand1 = sorted({int(x["adv_rtr"]) for x in b1[0].router_lsas} - set(bids))
+        asbrs1 = sorted(cand1[int(i)] for i in rng1.choice(len(cand1), min(area1_asbrs, len(cand1)), replace=False))
+        b1 = [_set_flags(a, {x: 0x02 for x in asbrs1}) for a in b1]
     # the shared prefix: a nearest neighbour of the first border in each area, at metrics that tie there
     def nearest(a):
         fl = Flat(a)
@@ -865,12 +876,22 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
                     continue
                 seen.add(key)
                 sums0.append((bid, key[0], key[1], int(d[v]) + int(l["metric"]), 3, 0, (0, 0)))
+    for bid, a in zip(bids, b1) if asbrs1 else ():
+        fl = Flat(a)
+        d = _dist_from(fl, fl.router_vertex(bid))
+        sums0 += [(bid, x, 0, int(d[fl.router_vertex(x)]), 4, 0, (0, 0)) for x in asbrs1
+                  if d[fl.router_vertex(x)] < 1 << 40]
     sums0.sort(key=lambda x: (x[4], x[0], x[1]))
     summaries0 = np.asarray(sums0, ospf_rib.SUMMARY_LSA_DT)
     loops = sorted({int(x["adv_rtr"]) for x in b1[0].router_lsas} - set(bids))
     keys = [loops[int(i)] for i in rng.choice(len(loops), min(n_ext_keys, len(loops)), replace=False)]
     ext = [(asbr, k, 0xFFFFFFFF, int(rng.choice([5, 30])), 0, 7, int(j % 2), 0, (0, 0)) for j, k in enumerate(keys)]
     ext.append((asbr, 0x0E0A0000, 0xFFFFFF00, 12, 0, 8, 1, 0, (0, 0)))
+    for m, x in enumerate(asbrs1):
+        ext.append((x, 0x0E0A0000, 0xFFFFFF00, 12, 0, 9, 1, 0, (0, 0)))
+        for q in range(area1_ext):
+            pfx = 0x0F000000 | ((m * area1_ext // 2 + q) << 8)
+            ext.append((x, pfx, 0xFFFFFF00, int(rng1.integers(1, 40)), 0, 10 + m, (q + m) % 2, 0, (0, 0)))
     ext.sort(key=lambda x: (x[0], x[1]))
     externals = np.asarray(ext, ospf_rib.EXTERNAL_LSA_DT)
     empty = np.zeros(0, ospf_rib.SUMMARY_LSA_DT)
@@ -881,4 +902,4 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
             pair = pair[::-1]
         out_borders.append(([p[0] for p in pair], [p[1] for p in pair], [p[2] for p in pair]))
     return {"r_area": r_area, "summaries0": summaries0, "externals": externals, "borders": out_borders,
-            "shared": shared, "asbr": asbr}
+            "shared": shared, "asbr": asbr, "area1_asbrs": asbrs1}

@@ -399,6 +399,70 @@ int hspf_ospfv2_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
                                     uint32_t n_gather, hl_ospfv2_rib *out);
 
 /*
+ * The same stage with the borders' type-4 LSAs re-originated per job (OSPFv2 only): a border originates one into
+ * area 0 for router A (an ASBR) when A is a router with the E flag in one of its non-backbone areas that it reaches,
+ * below LSInfinity, in the job; its metric is that distance (hspf_ospfv2_net_summaries' type-4 rule; an id in two such
+ * areas keeps the later area's).  For job j the decoded cells equal the affected-prefix routes of the update_rib_full
+ * above, with S_j holding each border's type-3 AND type-4 LSAs from hspf_ospfv2_net_summaries(rib_b, target area 0),
+ * in LsaKey order.  R's entry for A is the last usable type-4 LSA, in LsaKey order, whose ABR R reaches (rib_full step
+ * 2 replaces the entry per LSA), not the cheapest.  The type-4 rules are restated from the reference's code: no
+ * recorded conformance data holds a type-4 or type-5 LSA, so their parity rests on the host restatement alone.
+ *
+ *   hspf_ospfv2_backbone_asbr_table_create  host.  Arguments as hspf_ospfv2_backbone_table_create; the result may hold
+ *                                type-4 slots: per ASBR A some border can originate for, A's type-4 range holds the
+ *                                static type-4 records of other ABRs and one slot per (border, non-backbone area where A
+ *                                is an E-flag router) at the border's place in LsaKey order (also for a border without
+ *                                an LSA for A).  The affected prefixes add every prefix of a usable type-5 LSA of such
+ *                                an A.  The refusals of hspf_ospfv2_backbone_table_create apply, except the one of a
+ *                                border's type-4 LSA, and: HSPF_E_INVAL a usable type-4 LSA of a border for a router it
+ *                                cannot originate for; HSPF_E_UNSUPPORTED a router with the E and the B flag in a
+ *                                border's non-backbone area (its entry would replace an ABR's), or slots reading more
+ *                                than 8 (border, area) plane sets.
+ *   hspf_ospfv2_backbone_table_asbr_slots  the type-4 slot count and the (border, area) plane sets they read (0 and 0
+ *                                for a table of hspf_ospfv2_backbone_table_create).  The cells and delta calls above
+ *                                refuse a table with type-4 slots (HSPF_E_INVAL), before any launch.
+ *   hspf_ospfv2_backbone_asbr_cells[16]  as hspf_ospfv2_backbone_cells[16], plus per border b: border_planes[b] a host
+ *                                array of its n_areas plane structs (device, the arrays given hspf_ospfv2_abr_rib_cells,
+ *                                same width as `planes`), border_n_rows[b] host u32[n_areas], border_rows[b] device
+ *                                u32[n_jobs][n_areas].  Only the plane sets the table's slots name are read.  A job's
+ *                                status word also ORs each read row's word; a row out of range gives HSPF_JS_INVALID
+ *                                (and empty cells).  For a table without type-4 slots the three arrays may be NULL
+ *                                and the output is that of hspf_ospfv2_backbone_cells[16].
+ *   hspf_ospfv2_backbone_asbr_delta[16]  the route-delta stage over the same walk.
+ * hspf_ospfv2_backbone_from_cells decodes both kinds of table: an external cell's winner is its type-5 record.
+ */
+int hspf_ospfv2_backbone_asbr_table_create(const hspf_ospfv2_flat *flat, uint32_t router_id,
+                                           const hl_ospfv2_summary_lsa *summaries, uint32_t n_summaries,
+                                           const hl_ospfv2_external_lsa *externals, uint32_t n_externals,
+                                           const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                           hspf_ospfv2_backbone_table **out);
+int hspf_ospfv2_backbone_table_asbr_slots(const hspf_ospfv2_backbone_table *t, uint32_t *n_slots, uint32_t *n_sets);
+int hspf_ospfv2_backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                    const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                    const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                    const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                    uint32_t *job_status_out, hl_ospf_rib_cell *cells);
+int hspf_ospfv2_backbone_asbr_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                      const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                      const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                      const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                      uint32_t *job_status_out, hl_ospf_rib_cell *cells);
+int hspf_ospfv2_backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                    const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                    const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                    const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                    const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                    hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                    uint64_t *n_records);
+int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                      const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                      const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                      const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                      const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                      hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                      uint64_t *n_records);
+
+/*
  * The same stage for OSPFv3.  The table is an hspf_ospfv2_backbone_table marked OSPFv3; the cells and delta calls
  * above take it (the table's mark picks the walk), and each version's create and decode refuse the other version's
  * tables (HSPF_E_INVAL).  For job j, with border b's ABR cells of j decoded to rib_b (hspf_ospfv3_abr_rib_from_cells),
