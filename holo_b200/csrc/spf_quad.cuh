@@ -19,8 +19,9 @@
 //              predicate dist[u] + c == dist[v] on four records, chain partials combined
 //              with warp shuffles; writes dist / first_parent / n_parents planes.
 //   3. hops and next hops: pointer jumping over the first-parent tree, ECMP vertices as
-//              jump terminals (the scheme of spf_kernel.cuh phase 3J), 16 first-hop atoms
-//              per pass, up to four passes (64 atoms).
+//              jump terminals (the scheme of spf_kernel.cuh phase 3J): one pass for both
+//              when a job has at most 12 first-hop atoms and its ECMP vertices fit the list,
+//              else a hop pass and 16 atoms per next-hop pass, up to four passes (64 atoms).
 //
 // Eligibility (checked by the host, hspf_capi.cu): packed ids and costs (V, quads < 65535,
 // costs <= 65534, degrees <= 128), no LEAF vertex flags, no hop-count mode, one next-hop
@@ -54,6 +55,8 @@ struct QuadDev {
 struct QuadLayout {   // byte offsets into dynamic shared memory
     uint32_t dist, queue, ring, cont, h0, ecmp, elist, total;
     uint32_t qcap;    // queue capacity (entries)
+    uint32_t mhops;   // merged phase 3: hops of ECMP vertices u16[Vp] (0: the merged pass does not fit)
+    uint32_t mcap;    // merged phase 3: ECMP list capacity (entries between elist and mhops)
 };
 
 struct QuadArgs {
@@ -103,6 +106,13 @@ inline QuadLayout make_quad_layout(uint32_t V, uint32_t NQ, uint32_t qcap, uint3
     L.ecmp = o; o += al((size_t)nbv * 4);
     L.total = o;
     L.qcap = qcap;
+    // merged phase 3 (one jumping pass for hops and next hops): the jump words, the ECMP list and the
+    // ECMP vertices' hops u16[Vp] ending at cont (the continuation bits are loaded once per CTA and
+    // stay).  A job whose ECMP vertices do not fit between elist and mhops runs the two-pass code.
+    if (L.cont >= L.elist + al((size_t)Vp * 2)) {
+        L.mhops = L.cont - Vp * 2;        // (Vp * 2 and cont are multiples of 16)
+        L.mcap = (L.mhops - L.elist) / 2;
+    }
     return L;
 }
 
@@ -123,6 +133,8 @@ struct QSmall {
     uint32_t ov_edge[kMaxOv], ov_cost[kMaxOv];          // forward edge, new cost (kInf = disabled)
     uint32_t ov_fq[kMaxOv], ov_iq[kMaxOv];              // quad * 4 + record in fq / iq
     uint32_t n_roottab, root_rb, n_atoms;
+    uint32_t mbad;                                      // merged phase 3 does not apply (hop field overflow, seeded root)
+    uint16_t seed_of[16];                               // merged phase 3: vertex seeded with atom b (0xFFFF: none)
     uint32_t rt_target[kQMaxRoot], rt_base[kQMaxRoot], rt_cost[kQMaxRoot];
 };
 
@@ -575,53 +587,9 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
         // at themselves with an aggregate that is neutral under the update, so the update is
         // unconditional: word[v] = (anc(word[A]), agg(v) (+) agg(word[A])).
         // See spf_kernel.cuh phase 3J for the derivation; the first parents are read back
-        // from the plane just written.
-        // -- hops: sum of HOP flags over (root, v]; the root and unreached vertices are terminals
-        for (uint32_t v = tid; v < Vp; v += T) {      // (padding words are terminals: no bounds checks in the rounds)
-            const uint32_t f = (v < V) ? ld_fp(v) : kInf;
-            word[v] = (f == kInf) ? (v << 16) : ((f << 16) | (is_hop(v) ? 1u : 0u));
-        }
-        __syncthreads();
-        uint32_t jump_rounds = 0;     // rounds in which some vertex still moved
-        for (;;) {
-            uint32_t moved = 0;
-            for (uint32_t v0 = tid; v0 < Vp; v0 += 4 * T) {      // Vp % (4 * T) == 0
-                // two jumps per round (v -> A -> A'): fewer barrier-separated rounds
-                uint32_t w[4], w2[4], w3[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) w[k] = word[v0 + k * T];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) w2[k] = word[w[k] >> 16];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) w3[k] = word[w2[k] >> 16];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    // w2 / w3 are terminals (point at themselves, sum 0: read twice they add nothing)
-                    // or ordinary vertices
-                    word[v0 + k * T] = (w3[k] & 0xFFFF0000u) | ((w[k] + w2[k] + w3[k]) & 0xFFFFu);
-                    moved |= w3[k] ^ w[k];
-                }
-            }
-            if (a.prof && tid == 0) a.prof[(size_t)blockIdx.x * 16 + 13] += 1;
-            if (!__syncthreads_or((moved >> 16) != 0)) break;
-            if (++jump_rounds > 32u) { if (tid == 0) atomicOr(&S.status, kJsInternal); break; }   // depth < 2^32: cannot happen
-        }
-        for (uint32_t v = tid; v < V; v += T) {
-            const uint32_t w = word[v];
-            const uint32_t h = (w >> 16) == v ? 0u : (w & 0xFFFFu);
-            o_hops[v] = (uint16_t)h;
-            // a hops-0 vertex that is not a head of a root edge cannot own atoms
-            if (h == 0 && v != root && (w >> 16) != v && !hops0(v) && g.row[v + 1] != g.row[v])
-                atomicOr(&S.status, kJsTooManyAtoms);
-        }
-        __syncthreads();
-        HSPF_QMARK(5);   // hops
-
-        // -- next hops.  nh[v] = atoms entering v | U nh[p] over DAG parents p that are not at
-        // hops 0.  The tree is cut below hops-0 vertices and AT ECMP vertices (jump terminals):
-        //   word[v] = (top[v], atoms on the segment (top[v], v])
-        // then the ECMP vertices are resolved among themselves (monotone sweeps to the fixpoint)
-        // and every vertex adds the final set of its top.  16 atoms per pass.
+        // from the plane just written.  A job with at most 12 first-hop atoms whose ECMP vertices fit
+        // the layout's list runs both aggregates in one pass over the next-hop tree (tests/
+        // jump_merged_model.py); any other job runs the hop pass, then one next-hop pass per 16 atoms.
         auto is_ecmp = [&](uint32_t v) -> bool { return (ecmpbm[v >> 5] >> (v & 31)) & 1u; };
         // ECMP vertex list (ascending ids), built once
         if (tid == 0) S.cnt[0] = 0;
@@ -674,21 +642,45 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
             });
             cached = n <= 4;
         }
-        for (uint32_t pass = 0; pass * 16u < n_atoms || pass == 0; ++pass) {
-            // terminals (the root, unreached vertices, ECMP vertices) point at themselves
+        bool merged = L.mhops != 0 && n_atoms <= 12u && n_e <= L.mcap;
+        if (merged) {
+            // -- one pass for both aggregates over the next-hop tree (cut below hops-0 vertices and at
+            // ECMP vertices): word[v] = (anc:16 | hsum << n_atoms | atoms), hsum = HOP flags on
+            // (anc, v], atoms = first-hop atoms entering it.  An atom is seeded at one vertex, which a
+            // path crosses once, so on disjoint segments the OR is a sum: the whole aggregate is added.
+            // Terminals (root, unreached and ECMP vertices, padding) carry 0, read twice they add
+            // nothing; an ECMP vertex's seeds wait in S.seed_of.  A carry out of bit 15 (a segment
+            // with 2^(16 - n_atoms) or more HOP vertices) or a seeded root sends the job to the
+            // two-pass code.
+            const uint32_t na = n_atoms;
+            uint32_t ovf = 0;
             for (uint32_t v = tid; v < Vp; v += T) {
-                uint32_t A = v;
-                if (v < V) {
+                uint32_t A = v, h = 0;
+                if (v < V && !is_ecmp(v)) {
                     const uint32_t f = ld_fp(v);
-                    if (f != kInf && !is_ecmp(v)) A = hops0(f) ? root : f;
+                    if (f != kInf) {
+                        h = is_hop(v) ? 1u : 0u;
+                        A = f;
+                        if (hops0(f)) {
+                            // cut: anc = root, but the hops of a hops-0 parent other than the root need
+                            // not be 0 (a HOP vertex at distance 0 above it): walk its first parents
+                            A = root;
+                            for (uint32_t u = f, k = 0; u != root && u < V && k < V; u = ld_fp(u), ++k)
+                                h += is_hop(u) ? 1u : 0u;
+                        }
+                    }
                 }
-                word[v] = A << 16;
+                ovf |= h << na;
+                word[v] = (A << 16) | ((h << na) & 0xFFFFu);
             }
+            if (tid < 16u) S.seed_of[tid] = (uint16_t)min(seed_v, 0xFFFFu);
+            if (tid == 0) S.mbad = 0;
             __syncthreads();
-            if (seed_v != kInf && (tid >> 4) == pass) atomicOr(&word[seed_v], 1u << (tid & 15));
+            if (seed_v != kInf && seed_v == root) ovf |= 1u << 16;
+            else if (seed_v != kInf && !is_ecmp(seed_v)) atomicOr(&word[seed_v], 1u << tid);     // (tid < n_atoms)
             __syncthreads();
-            // the cut tree is no deeper than the first-parent tree: the hop pass's round count suffices
-            for (uint32_t r = 0; r < jump_rounds; ++r) {
+            for (uint32_t rounds = 0;;) {
+                uint32_t moved = 0;
                 for (uint32_t v0 = tid; v0 < Vp; v0 += 4 * T) {
                     uint32_t w[4], w2[4], w3[4];
 #pragma unroll
@@ -698,27 +690,45 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
 #pragma unroll
                     for (int k = 0; k < 4; ++k) w3[k] = word[w2[k] >> 16];
 #pragma unroll
-                    for (int k = 0; k < 4; ++k)   // OR-ing a terminal's own seeds again is harmless (every vertex ORs in its top's set below)
-                        word[v0 + k * T] = (w3[k] & 0xFFFF0000u) | ((w[k] | w2[k] | w3[k]) & 0xFFFFu);
+                    for (int k = 0; k < 4; ++k) {
+                        const uint32_t sum = (w[k] & 0xFFFFu) + (w2[k] & 0xFFFFu) + (w3[k] & 0xFFFFu);
+                        ovf |= sum;
+                        word[v0 + k * T] = (w3[k] & 0xFFFF0000u) | (sum & 0xFFFFu);
+                        moved |= w3[k] ^ w[k];
+                    }
                 }
+                if (ovf >> 16) S.mbad = 1;
                 if (a.prof && tid == 0) a.prof[(size_t)blockIdx.x * 16 + 14] += 1;
-                __syncthreads();
+                if (!__syncthreads_or((moved >> 16) != 0)) break;
+                if (++rounds > 32u) { if (tid == 0) atomicOr(&S.status, kJsInternal); break; }   // depth < 2^32: cannot happen
             }
-            // ECMP vertices: from the self-pointing terminal form to (top, own segment) through the first parent
+            merged = S.mbad == 0;
+            HSPF_QMARK(5);   // hops (set-up and rounds of the merged pass)
+        }
+        if (merged) {
+            const uint32_t na = n_atoms, amask = (1u << na) - 1u;
+            uint16_t *eh = reinterpret_cast<uint16_t *>(qsm + L.mhops);      // hops of ECMP vertices
             if (n_e) {
+                // ECMP vertices: (top, own segment) through the first parent, as in the two-pass code;
+                // hops unresolved (0xFFFF)
+                uint32_t fx = kInf;      // first parent of this thread's ECMP vertex (n_e <= T)
                 for (uint32_t i = tid; i < n_e; i += T) {
                     const uint32_t x = elist[i];
-                    const uint32_t seeds = word[x] & 0xFFFFu;
                     const uint32_t f = ld_fp(x);      // an ECMP vertex has parents
+                    fx = f;
+                    uint32_t seeds = 0;
+                    for (uint32_t b = 0; b < na; ++b) seeds |= (S.seed_of[b] == x) ? 1u << b : 0u;
                     uint32_t nw;
                     if (hops0(f)) nw = (root << 16) | seeds;
                     else if (is_ecmp(f)) nw = (f << 16) | seeds;
-                    else { const uint32_t wf = word[f]; nw = (wf & 0xFFFF0000u) | ((wf | seeds) & 0xFFFFu); }
+                    else { const uint32_t wf = word[f]; nw = (wf & 0xFFFF0000u) | ((wf | seeds) & amask); }
                     // (word[f] of a non-ECMP f is final and is not rewritten here)
                     word[x] = nw;
+                    eh[x] = 0xFFFFu;
                 }
                 __syncthreads();
-                // own segment | final set of own top | the same of every other parent
+                // next hops: own segment | final set of own top | the same of every other parent;
+                // hops(x) = own flag + hops(fp(x)), once the ECMP vertex that decides it is resolved
                 for (uint32_t sweeps = 0;;) {
                     int ch = 0;
                     for (uint32_t i = tid; i < n_e; i += T) {
@@ -736,28 +746,170 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
                         } else {
                             parents(x, pull_parent);
                         }
-                        need &= 0xFFFFu & ~w;
+                        need &= amask & ~w;
                         if (need) { word[x] = w | need; ch = 1; }
+                        if (eh[x] == 0xFFFFu) {
+                            const uint32_t f = (n_e <= (uint32_t)T) ? fx : ld_fp(x);
+                            uint32_t h = is_hop(x) ? 1u : 0u, t = root;
+                            if (is_ecmp(f)) t = f;
+                            else if (f != root) { const uint32_t wf = word[f]; h += (wf & 0xFFFFu) >> na; t = wf >> 16; }
+                            const uint32_t ht = (t == root) ? 0u : eh[t];
+                            if (ht != 0xFFFFu) { eh[x] = (uint16_t)(h + ht); ch = 1; }
+                        }
                     }
                     if (a.prof && tid == 0) a.prof[(size_t)blockIdx.x * 16 + 15] += 1;
                     if (!__syncthreads_or(ch)) break;
-                    if (++sweeps > 16u * n_e + 16u) { if (tid == 0) atomicOr(&S.status, kJsInternal); break; }   // <= 16 bits per vertex
+                    if (++sweeps > 17u * n_e + 16u) { if (tid == 0) atomicOr(&S.status, kJsInternal); break; }
                 }
             }
             for (uint32_t v = tid; v < V; v += T) {
                 const uint32_t w = word[v], Tv = w >> 16;
-                uint32_t m = w;
-                if (Tv != root && Tv != v) m |= word[Tv];
-                if (narrow) {
-                    if (pass == 0) {      // (more than 16 atoms: HSPF_JS_NARROW, set below)
-                        o_nh16[v] = (uint16_t)(m & 0xFFFFu);
-                    }
-                } else {
-                    const uint64_t bits = (uint64_t)(m & 0xFFFFu) << (16 * pass);
-                    if (pass == 0) o_nh[v] = bits; else o_nh[v] |= bits;
-                }
+                const bool up = Tv != root && Tv != v;
+                uint32_t m = w & amask, h;
+                if (up) m |= word[Tv] & amask;
+                if (is_ecmp(v)) h = eh[v];                                   // (n_e > 0)
+                else h = ((w & 0xFFFFu) >> na) + (up ? (uint32_t)eh[Tv] : 0u);  // Tv: the root or an ECMP vertex
+                h &= 0xFFFFu;
+                o_hops[v] = (uint16_t)h;
+                // a hops-0 vertex that is not a head of a root edge cannot own atoms
+                if (h == 0 && v != root && Tv != v && !hops0(v) && g.row[v + 1] != g.row[v])
+                    atomicOr(&S.status, kJsTooManyAtoms);
+                if (narrow) o_nh16[v] = (uint16_t)m;
+                else o_nh[v] = m;
             }
             __syncthreads();
+        } else {
+            // -- hops: sum of HOP flags over (root, v]; the root and unreached vertices are terminals
+            for (uint32_t v = tid; v < Vp; v += T) {      // (padding words are terminals: no bounds checks in the rounds)
+                const uint32_t f = (v < V) ? ld_fp(v) : kInf;
+                word[v] = (f == kInf) ? (v << 16) : ((f << 16) | (is_hop(v) ? 1u : 0u));
+            }
+            __syncthreads();
+            uint32_t jump_rounds = 0;     // rounds in which some vertex still moved
+            for (;;) {
+                uint32_t moved = 0;
+                for (uint32_t v0 = tid; v0 < Vp; v0 += 4 * T) {      // Vp % (4 * T) == 0
+                    // two jumps per round (v -> A -> A'): fewer barrier-separated rounds
+                    uint32_t w[4], w2[4], w3[4];
+    #pragma unroll
+                    for (int k = 0; k < 4; ++k) w[k] = word[v0 + k * T];
+    #pragma unroll
+                    for (int k = 0; k < 4; ++k) w2[k] = word[w[k] >> 16];
+    #pragma unroll
+                    for (int k = 0; k < 4; ++k) w3[k] = word[w2[k] >> 16];
+    #pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        // w2 / w3 are terminals (point at themselves, sum 0: read twice they add nothing)
+                        // or ordinary vertices
+                        word[v0 + k * T] = (w3[k] & 0xFFFF0000u) | ((w[k] + w2[k] + w3[k]) & 0xFFFFu);
+                        moved |= w3[k] ^ w[k];
+                    }
+                }
+                if (a.prof && tid == 0) a.prof[(size_t)blockIdx.x * 16 + 13] += 1;
+                if (!__syncthreads_or((moved >> 16) != 0)) break;
+                if (++jump_rounds > 32u) { if (tid == 0) atomicOr(&S.status, kJsInternal); break; }   // depth < 2^32: cannot happen
+            }
+            for (uint32_t v = tid; v < V; v += T) {
+                const uint32_t w = word[v];
+                const uint32_t h = (w >> 16) == v ? 0u : (w & 0xFFFFu);
+                o_hops[v] = (uint16_t)h;
+                // a hops-0 vertex that is not a head of a root edge cannot own atoms
+                if (h == 0 && v != root && (w >> 16) != v && !hops0(v) && g.row[v + 1] != g.row[v])
+                    atomicOr(&S.status, kJsTooManyAtoms);
+            }
+            __syncthreads();
+            HSPF_QMARK(5);   // hops
+
+            // -- next hops.  nh[v] = atoms entering v | U nh[p] over DAG parents p that are not at
+            // hops 0.  The tree is cut below hops-0 vertices and AT ECMP vertices (jump terminals):
+            //   word[v] = (top[v], atoms on the segment (top[v], v])
+            // then the ECMP vertices are resolved among themselves (monotone sweeps to the fixpoint)
+            // and every vertex adds the final set of its top.  16 atoms per pass.
+            for (uint32_t pass = 0; pass * 16u < n_atoms || pass == 0; ++pass) {
+                // terminals (the root, unreached vertices, ECMP vertices) point at themselves
+                for (uint32_t v = tid; v < Vp; v += T) {
+                    uint32_t A = v;
+                    if (v < V) {
+                        const uint32_t f = ld_fp(v);
+                        if (f != kInf && !is_ecmp(v)) A = hops0(f) ? root : f;
+                    }
+                    word[v] = A << 16;
+                }
+                __syncthreads();
+                if (seed_v != kInf && (tid >> 4) == pass) atomicOr(&word[seed_v], 1u << (tid & 15));
+                __syncthreads();
+                // the cut tree is no deeper than the first-parent tree: the hop pass's round count suffices
+                for (uint32_t r = 0; r < jump_rounds; ++r) {
+                    for (uint32_t v0 = tid; v0 < Vp; v0 += 4 * T) {
+                        uint32_t w[4], w2[4], w3[4];
+    #pragma unroll
+                        for (int k = 0; k < 4; ++k) w[k] = word[v0 + k * T];
+    #pragma unroll
+                        for (int k = 0; k < 4; ++k) w2[k] = word[w[k] >> 16];
+    #pragma unroll
+                        for (int k = 0; k < 4; ++k) w3[k] = word[w2[k] >> 16];
+    #pragma unroll
+                        for (int k = 0; k < 4; ++k)   // OR-ing a terminal's own seeds again is harmless (every vertex ORs in its top's set below)
+                            word[v0 + k * T] = (w3[k] & 0xFFFF0000u) | ((w[k] | w2[k] | w3[k]) & 0xFFFFu);
+                    }
+                    if (a.prof && tid == 0) a.prof[(size_t)blockIdx.x * 16 + 14] += 1;
+                    __syncthreads();
+                }
+                // ECMP vertices: from the self-pointing terminal form to (top, own segment) through the first parent
+                if (n_e) {
+                    for (uint32_t i = tid; i < n_e; i += T) {
+                        const uint32_t x = elist[i];
+                        const uint32_t seeds = word[x] & 0xFFFFu;
+                        const uint32_t f = ld_fp(x);      // an ECMP vertex has parents
+                        uint32_t nw;
+                        if (hops0(f)) nw = (root << 16) | seeds;
+                        else if (is_ecmp(f)) nw = (f << 16) | seeds;
+                        else { const uint32_t wf = word[f]; nw = (wf & 0xFFFF0000u) | ((wf | seeds) & 0xFFFFu); }
+                        // (word[f] of a non-ECMP f is final and is not rewritten here)
+                        word[x] = nw;
+                    }
+                    __syncthreads();
+                    // own segment | final set of own top | the same of every other parent
+                    for (uint32_t sweeps = 0;;) {
+                        int ch = 0;
+                        for (uint32_t i = tid; i < n_e; i += T) {
+                            const uint32_t x = elist[i];
+                            const uint32_t w = word[x], Tx = w >> 16;
+                            uint32_t need = (Tx != root) ? word[Tx] : 0u;
+                            auto pull_parent = [&](uint32_t u) {
+                                const uint32_t wp = word[u], Tp = wp >> 16;
+                                need |= wp;
+                                if (Tp != root && Tp != u) need |= word[Tp];
+                            };
+                            if (cached) {
+    #pragma unroll
+                                for (int k = 0; k < 4; ++k) if (pc[k] != kInf) pull_parent(pc[k]);
+                            } else {
+                                parents(x, pull_parent);
+                            }
+                            need &= 0xFFFFu & ~w;
+                            if (need) { word[x] = w | need; ch = 1; }
+                        }
+                        if (a.prof && tid == 0) a.prof[(size_t)blockIdx.x * 16 + 15] += 1;
+                        if (!__syncthreads_or(ch)) break;
+                        if (++sweeps > 16u * n_e + 16u) { if (tid == 0) atomicOr(&S.status, kJsInternal); break; }   // <= 16 bits per vertex
+                    }
+                }
+                for (uint32_t v = tid; v < V; v += T) {
+                    const uint32_t w = word[v], Tv = w >> 16;
+                    uint32_t m = w;
+                    if (Tv != root && Tv != v) m |= word[Tv];
+                    if (narrow) {
+                        if (pass == 0) {      // (more than 16 atoms: HSPF_JS_NARROW, set below)
+                            o_nh16[v] = (uint16_t)(m & 0xFFFFu);
+                        }
+                    } else {
+                        const uint64_t bits = (uint64_t)(m & 0xFFFFu) << (16 * pass);
+                        if (pass == 0) o_nh[v] = bits; else o_nh[v] |= bits;
+                    }
+                }
+                __syncthreads();
+            }
         }
         if (n_peers) {
             __syncthreads();                      // every plane of this job is written (this CTA wrote them all)

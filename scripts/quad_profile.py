@@ -4,7 +4,10 @@
 Counters (hspf_debug_phase_profile slots, thread 0 of every CTA, summed over CTAs):
 0 init, 1 SSSP, 2 parents, 4 next hops, 5 hops, 7 SSSP rounds, 8 compaction (+ barrier),
 9 expansion (thread 0's share), 10 barrier after the expansion, 12 queue entries,
-13 hop jump rounds, 14 next-hop jump rounds, 15 ECMP sweeps."""
+13 hop jump rounds, 14 next-hop jump rounds, 15 ECMP sweeps.
+A job that runs the merged phase-3 pass counts its set-up and rounds under "hops" and its
+rounds in slot 14; the ECMP sweeps and the result writes fall under "next hops".  Slot 13
+counts rounds of the hop pass, which only the two-pass code runs."""
 import ctypes as C
 import sys
 
