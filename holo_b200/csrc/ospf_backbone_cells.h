@@ -19,6 +19,11 @@
 // 341-386): those of the border cell's winning intra-area record.  Its winner is n_recs + (slot << 8 | options), so
 // that a job whose border route changes record at an equal metric, to one with other options, changes R's winner
 // (the route-delta stage reports OTHER), and the decode reads the options from the winner alone.
+//
+// The same walk serves the opposite direction (kNonBackbone, hspf_ospfv2_nonbackbone_table_create): R is an internal
+// router of a non-backbone area A, a job changes costs in area 0 only, and the borders are A's ABRs attached to area
+// 0.  A slot then stands for the LSA the border originates into A: its cell may also be inter-area, its winner must
+// not be one of A's intra-area records and none of its atoms an A atom.
 #pragma once
 #include <cstdint>
 #include <utility>
@@ -114,9 +119,11 @@ struct OspfAsbrPlanes : Planes {
     OspfAsbrJob<Planes, D> asbr;
 };
 
-// What border b advertises into area 0 for the prefix of its cell c: false when nothing, else its metric and, for
-// OSPFv3 (kV3), the prefix options of the cell's winner.
-template <bool kV3>
+// What border b advertises into the table's target area for the prefix of its cell c: false when nothing, else its
+// metric and, for OSPFv3 (kV3), the prefix options of the cell's winner.  Into area 0 only an intra-area route is
+// advertised; into a non-backbone area (kNonBackbone, hspf_ospfv2_nonbackbone_table_create) an inter-area one too
+// (compute_net_summaries).  The border words name the target area's intra-area records and atoms.
+template <bool kV3, bool kNonBackbone = false>
 HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, uint32_t b, uint32_t &metric,
                             uint32_t &options) {
     constexpr uint32_t kStride = kV3 ? 2 : 1;                          // 16-byte groups per border
@@ -132,7 +139,9 @@ HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, u
     const uint32_t winner = (uint32_t)wm, mpf = (uint32_t)(wm >> 32);
     const uint64_t atoms0 = (uint64_t)bb.z | ((uint64_t)bb.w << 32);
     metric = mpf & HL_RIB_CELL_METRIC_MAX;
-    const bool adv = ((mpf >> 28) & HL_CELL_PRESENT) && ((mpf >> 26) & 0x3u) == HL_PATH_INTRA_AREA &&
+    const uint32_t path = (mpf >> 26) & 0x3u;
+    const bool adv = ((mpf >> 28) & HL_CELL_PRESENT) &&
+                     (path == HL_PATH_INTRA_AREA || (kNonBackbone && path == HL_PATH_INTER_AREA)) &&
                      (winner < bb.x || winner >= bb.y) && !(nh & atoms0) && metric < HL_LSA_INFINITY;
     if constexpr (kV3) {
         options = 0;
@@ -149,7 +158,8 @@ HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, u
 
 // kV3: the table is an OSPFv3 one (hspf_ospfv3_backbone_table_create), whose slot winners carry prefix options.
 // kAsbr: the table's type-4 ranges hold slots, read through pl.asbr (pl an OspfAsbrPlanes of the job).
-template <bool kV3 = false, bool kAsbr = false, class Planes>
+// kNonBackbone: the table's target area is not area 0 (border_summary).
+template <bool kV3 = false, bool kAsbr = false, bool kNonBackbone = false, class Planes>
 HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneView &t, uint32_t p,
                                           const OspfBorderRows &rows) {
     const RouteContrib *contribs = reinterpret_cast<const RouteContrib *>(t.recs);
@@ -166,7 +176,7 @@ HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneVi
         if (!pl.reached(r.x)) continue;
         uint32_t y = r.y, w = i, options = 0;
         if (r.z != kOspfBackboneStatic) {
-            if (!border_summary<kV3>(rows.row[r.z] + r.y, t.border, r.z, y, options)) continue;
+            if (!border_summary<kV3, kNonBackbone>(rows.row[r.z] + r.y, t.border, r.z, y, options)) continue;
             w = kV3 ? t.n_recs + (r.w << 8 | options) : t.n_recs + r.w;
         }
         const uint32_t m = pl.d(r.x) + y;
@@ -219,8 +229,11 @@ HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneVi
 
 // Host + device image of a backbone router's affected prefixes (include/holo_spf_lsdb.h).
 struct hspf_ospfv2_backbone_table {
-    hspf_ospfv2_ribtable *r = nullptr;           // R's one-area table over area 0 without the borders' type-3 LSAs
+    hspf_ospfv2_ribtable *r = nullptr;           // R's one-area table over its area without the borders' type-3 LSAs
     uint32_t router_id = 0, root = 0, n_vertices = 0, n_borders = 0, max_paths = 0;
+    // the target area: R's area, into which the borders' LSAs are re-originated per job (0 but for
+    // hspf_ospfv2_nonbackbone_table_create, whose tables the walk reads with kNonBackbone)
+    uint32_t area_id = 0;
     std::vector<uint32_t> prefix, plen;          // [P] prefix order
     // oi [PR + 1], q [P], o3 [P + 1], o5 [P + 1], padding, border [4 n_borders] (OSPFv3: [8 n_borders], then each
     // border's options bytes, each border's padded to a word)

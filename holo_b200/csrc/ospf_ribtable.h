@@ -7,7 +7,8 @@
 //   build_abr_ribtable hspf_ospfv2_abr_ribtable_create / hspf_ospfv3_abr_ribtable_create: an area border router's
 //                      records over the one-area tables of its areas (ospf_abr_rib_cells.h)
 //   build_backbone_table  hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create: a backbone router's
-//                      affected prefixes over its one-area table and its borders' ABR tables (ospf_backbone_cells.h)
+//                      affected prefixes over its one-area table and its borders' ABR tables (ospf_backbone_cells.h);
+//                      hspf_ospfv2_nonbackbone_table_create: the same for an internal router of a non-backbone area
 //   decode_rib         one job's cells -> its routing table, for hspf_ospfv2_rib_from_cells,
 //                      hspf_ospfv3_rib_from_cells, hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib) and
 //                      hspf_ospfv{2,3}_backbone_from_cells (decode_backbone_rib).  A one-area table decodes as an area
@@ -351,16 +352,31 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
 // (ospf_backbone_cells.h).  Border tables of the other version are refused (HSPF_E_INVAL).  `asbr`
 // (hspf_ospfv2_backbone_asbr_table_create): the borders' type-4 LSAs are re-originated per job too, as type-4 slots,
 // and the prefixes of the type-5 LSAs they lead to are affected; else a usable one is HSPF_E_UNSUPPORTED.
+// `config` (hspf_ospfv2_nonbackbone_table_create, OSPFv2 only): R is an internal router of the non-backbone area of
+// `flat` with that configuration, the target area A.  The borders re-originate into A their intra-area routes of
+// their other areas and their inter-area routes, and type-4 LSAs for the ASBRs they reach intra-area outside A (plane
+// sets of any of those areas, area 0 included); in a stub area the default route stays static and no type-4 LSA is
+// originated, and a totally stubby area has no slot.
 template <class T>
 int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const typename T::Sum *sums, uint32_t n_sums,
                          const typename T::Ext *ext, uint32_t n_ext, const hspf_ospfv2_abr_ribtable *const *borders,
-                         uint32_t n_borders, hspf_ospfv2_backbone_table **out, bool asbr = false) {
+                         uint32_t n_borders, hspf_ospfv2_backbone_table **out, bool asbr = false,
+                         const hl_ospf_area_config *config = nullptr) {
     using Key = typename T::Key;
     using Sum = typename T::Sum;
     constexpr uint32_t kNone = 0xFFFFFFFFu;
     if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext) || !borders) return HSPF_E_INVAL;
     *out = nullptr;
+    const bool nb = config != nullptr;                            // a non-backbone target area
+    const uint32_t ta = nb ? flat->area->area_id : 0;
+    if (nb) {
+        if (T::kV3 || ta == 0) return HSPF_E_INVAL;
+        if (config->area_type == HL_AREA_NSSA || n_borders == 0 || n_borders > kOspfBackboneMaxBorders)
+            return HSPF_E_UNSUPPORTED;
+        asbr = true;
+    }
     if (n_borders == 0 || n_borders > kOspfBackboneMaxBorders) return HSPF_E_INVAL;
+    const bool normal = !nb || config->area_type == HL_AREA_NORMAL;
     try {
         std::unique_ptr<hspf_ospfv2_backbone_table, void (*)(hspf_ospfv2_backbone_table *)> t(
             new hspf_ospfv2_backbone_table(), hspf_ospfv2_backbone_table_free);
@@ -370,21 +386,39 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         const uint32_t root = vertex(router_id);
         if (root == kNone || (flags(root) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
         t->router_id = router_id; t->root = root; t->n_vertices = T::n_vertices(f);
-        t->max_paths = f.area->max_paths; t->n_borders = n_borders; t->v3 = T::kV3;
-        std::vector<uint32_t> a0(n_borders), bv(n_borders);       // per border: its area-0 index, its vertex
+        t->max_paths = f.area->max_paths; t->n_borders = n_borders; t->v3 = T::kV3; t->area_id = ta;
+        // per border: its area-0 index, its target-area index, its vertex
+        std::vector<uint32_t> a0(n_borders), at(n_borders), bv(n_borders);
         std::unordered_map<uint32_t, uint32_t> border_of;           // router id -> border
         for (uint32_t b = 0; b < n_borders; ++b) {
             const hspf_ospfv2_abr_ribtable *bt = borders[b];
             if (!bt || bt->v3 != T::kV3 || bt->router_id == router_id || !border_of.emplace(bt->router_id, b).second)
                 return HSPF_E_INVAL;
-            a0[b] = kNone;
-            for (uint32_t i = 0; i < bt->n_areas; ++i)
-                if (bt->area_id[i] == 0) { a0[b] = i; break; }
+            a0[b] = at[b] = kNone;
+            for (uint32_t i = 0; i < bt->n_areas; ++i) {
+                if (bt->area_id[i] == 0 && a0[b] == kNone) a0[b] = i;
+                if (bt->area_id[i] == ta && at[b] == kNone) at[b] = i;
+            }
             bv[b] = vertex(bt->router_id);
-            if (a0[b] == kNone || !(flags(bv[b]) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
+            if (a0[b] == kNone || at[b] == kNone || !(flags(bv[b]) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
             t->borders[b] = bt;
+            if (nb) {
+                // an inter-area router entry at the border (from another ABR's type-4 LSA in area 0) would be
+                // re-originated into A at a distance the job moves
+                const hspf_ospfv2_ribtable &r0 = *bt->area[a0[b]];
+                for (uint32_t a = 0; a < (uint32_t)r0.asbr_id.size(); ++a) {
+                    const RibRec &s = r0.recs[r0.ext_end + a];
+                    for (uint32_t k = s.z; k < s.w; ++k)
+                        if (r0.recs[k].x != bt->root[a0[b]]) return HSPF_E_UNSUPPORTED;
+                }
+            }
         }
-        // area 0 without the borders' type-3 LSAs: R's one-area table over the rest
+        // the default route a border originates into a stub area, at default_cost whatever the job
+        auto stub_default = [&](const Sum &l) {
+            if constexpr (T::kV3) return false;
+            else return nb && !normal && l.lsa_type == 3 && l.lsa_id == 0 && l.mask == 0;
+        };
+        // R's area without the borders' type-3 LSAs: R's one-area table over the rest
         auto live = [](const Sum &l) { return !l.maxage && l.metric < HL_LSA_INFINITY && !T::skip(l); };
         std::vector<Sum> rest;
         std::vector<std::pair<uint32_t, Key>> border_t3;            // (border, prefix key) of the borders' LSAs
@@ -392,7 +426,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         for (uint32_t i = 0; i < n_sums; ++i) {
             const Sum &l = sums[i];
             auto it = border_of.find(l.adv_rtr);
-            if (it == border_of.end()) { rest.push_back(l); continue; }
+            if (it == border_of.end() || stub_default(l)) { rest.push_back(l); continue; }
             if (!live(l)) continue;
             if (l.lsa_type == 4) {                                   // re-originated per job too
                 if (!asbr) return HSPF_E_UNSUPPORTED;
@@ -400,17 +434,20 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
             }
             if (l.lsa_type == 3) border_t3.emplace_back(it->second, T::key(l));
         }
-        int rc = T::area_table(flat, 0, rest.data(), (uint32_t)rest.size(), ext, n_ext, false, &t->r);
+        int rc = T::area_table(flat, ta, rest.data(), (uint32_t)rest.size(), ext, n_ext, false, &t->r);
         if (rc) return rc;
         const hspf_ospfv2_ribtable &r = *t->r;
-        // type-4 slots: per ASBR id, the (border, area index) pairs of the borders' non-backbone areas where it is a
-        // router with the E flag, each border's in area order
+        if (nb)                                                      // A is a transit area
+            for (uint8_t fl : r.vflags)
+                if (fl & HL_RTR_FLAG_V) return HSPF_E_UNSUPPORTED;
+        // type-4 slots: per ASBR id, the (border, area index) pairs of the borders' areas other than the target where
+        // it is a router with the E flag, each border's in area order (none into a stub area)
         std::map<uint32_t, std::vector<std::pair<uint32_t, uint32_t>>> orig;
-        if (asbr) {
+        if (asbr && normal) {
             for (uint32_t b = 0; b < n_borders; ++b) {
                 const hspf_ospfv2_abr_ribtable &bt = *borders[b];
                 for (uint32_t i = 0; i < bt.n_areas; ++i) {
-                    if (bt.area_id[i] == 0) continue;
+                    if (bt.area_id[i] == ta) continue;
                     for (const auto &e : bt.rtr_vertex[i]) {
                         const uint8_t fl = bt.area[i]->vflags[e.second];
                         if (!(fl & HL_RTR_FLAG_E)) continue;
@@ -433,17 +470,21 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                 if (!found) return HSPF_E_INVAL;                     // the LSDB disagrees with the border's table
             }
         }
-        // the affected prefixes: each border's prefixes with an intra-area record in one of its non-backbone areas
+        // the affected prefixes: each border's prefixes with an intra-area record in one of its areas other than the
+        // target (into a non-backbone area also those with a type-3 record in its area 0; none into a totally stubby
+        // area, and not a stub area's default route)
         std::map<Key, std::vector<std::pair<uint32_t, uint32_t>>> slots;   // key -> (border, its prefix index)
-        for (uint32_t b = 0; b < n_borders; ++b) {
+        for (uint32_t b = 0; b < n_borders && (!nb || config->summary); ++b) {
             const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-            const uint32_t P = (uint32_t)bt.prefix.size(), S = P + 1;
-            for (uint32_t u = 0; u < P; ++u)
-                for (uint32_t i = 0; i < bt.n_areas; ++i)
-                    if (bt.area_id[i] != 0 && bt.off[i * S + u] != bt.off[i * S + u + 1]) {
-                        slots[T::table_key(bt, u)].emplace_back(b, u);
-                        break;
-                    }
+            const uint32_t P = (uint32_t)bt.prefix.size(), S = P + 1, A = bt.n_areas;
+            for (uint32_t u = 0; u < P; ++u) {
+                bool adv = nb && bt.off[(A + a0[b]) * S + u] != bt.off[(A + a0[b]) * S + u + 1];
+                for (uint32_t i = 0; i < A && !adv; ++i)
+                    adv = bt.area_id[i] != ta && bt.off[i * S + u] != bt.off[i * S + u + 1];
+                if constexpr (!T::kV3)
+                    if (nb && !normal && bt.prefix[u] == 0 && bt.plen[u] == 0) adv = false;
+                if (adv) slots[T::table_key(bt, u)].emplace_back(b, u);
+            }
         }
         for (const auto &x : border_t3) {
             auto it = slots.find(x.second);
@@ -569,7 +610,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         uint32_t opt_words = (T::kV3 ? 8 : 4) * n_borders;         // OSPFv3: the options bytes follow the border words
         for (uint32_t b = 0; b < n_borders; ++b) {
             const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-            const uint32_t i = a0[b], lo = bt.intra_base[i], na = bt.n_atoms[i];
+            const uint32_t i = at[b], lo = bt.intra_base[i], na = bt.n_atoms[i];
             const uint64_t atoms = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << bt.base[i]);
             t->words.insert(t->words.end(), {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)});
             if (T::kV3) {
@@ -821,13 +862,13 @@ int decode_abr_rib(const hspf_ospfv2_abr_ribtable *t, const typename T::Area *ar
 }
 
 // hspf_ospfv2_backbone_from_cells / hspf_ospfv3_backbone_from_cells, argument checks included: the decode of R's
-// one-area table over the affected prefixes, a slot winner naming its type-3 record (and, OSPFv3, carrying the
+// one-area table (over the table's target area) over the affected prefixes, a slot winner naming its type-3 record (and, OSPFv3, carrying the
 // options the route takes).  A table of the other version is refused (HSPF_E_INVAL).
 template <class T>
 int decode_backbone_rib(const hspf_ospfv2_backbone_table *t, const typename T::Area *a, const hl_ospf_rib_cell *cells,
                         const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out) {
     if (!t || t->v3 != T::kV3 || !a || !cells || !out || (n_gather && (!gather_v || !gather_nh))) return HSPF_E_INVAL;
-    if (a->router_id != t->router_id || a->area_id != 0 || a->max_paths != t->max_paths) return HSPF_E_INVAL;
+    if (a->router_id != t->router_id || a->area_id != t->area_id || a->max_paths != t->max_paths) return HSPF_E_INVAL;
     try {
         out->n_routes = out->n_nexthops = 0;
         typename T::JobDecode jd;
@@ -847,7 +888,7 @@ int decode_backbone_rib(const hspf_ospfv2_backbone_table *t, const typename T::A
             x.winner = t->slot_rec[s];
             if (T::kV3) options[x.winner - v.o3[0]] = (uint8_t)opt;
         }
-        RibDecode<T> d{{RibDecodeArea<T>{a, t->r, v.q, 0, ~0ull, v.o3, 0, ~0ull, 0, &jd}},
+        RibDecode<T> d{{RibDecodeArea<T>{a, t->r, v.q, 0, ~0ull, v.o3, 0, ~0ull, t->area_id, &jd}},
                        P, t->prefix.data(), t->plen.data(), T::kV3 ? t->prefix6.data() : nullptr, v.o5,
                        t->ext_tag.data(), t->ext_base, t->max_paths, T::kV3 ? options.data() : nullptr,
                        T::kV3 ? v.o3[0] : 0};

@@ -1,7 +1,9 @@
 // Device stage for the routing table of an OSPF backbone router over what-if jobs inside other areas
 // (include/holo_spf_lsdb.h, "backbone router over what-if jobs inside other areas"): update_rib_full at the router,
 // for its affected prefixes, with every border's type-3 / Inter-Area-Prefix LSAs in area 0 re-originated for the job.
-// The entry points serve OSPFv2 and OSPFv3 tables alike: the table's mark picks the walk's instantiation.
+// The entry points serve OSPFv2 and OSPFv3 tables alike, and OSPFv2 tables of an internal router of a non-backbone
+// area over jobs on the backbone (hspf_ospfv2_nonbackbone_table_create): the table's mark picks the walk's
+// instantiation.
 //
 // One launch on the ctx stream: one thread per (job, prefix) runs ospf_backbone_cell_eval (ospf_backbone_cells.h)
 // over the router's unperturbed area-0 planes (row 0) and the job's row of each border's routing-table cells, and
@@ -62,11 +64,26 @@ struct OspfBackboneAsbrCell : OspfBackboneCell<Planes, false> {
     }
 };
 
+// The walk over a table whose target area is not area 0 (hspf_ospfv2_nonbackbone_table_create), with or without
+// type-4 slots (the cells and delta calls of both kinds take it): the borders also advertise their inter-area routes, and a plane set may be a border's area 0.
+template <class Planes>
+struct OspfNonBackboneCell : OspfBackboneAsbrCell<Planes> {
+    using Base = OspfBackboneCell<Planes, false>;
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
+        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {this->sets, j}};
+        return hspf::ospf_backbone_cell_eval<false, true, true>(pl, this->t, p, rows);
+    }
+};
+
 // Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
-// and for OSPFv3 tables, and for OSPFv2 tables with type-4 slots.
+// and for OSPFv3 tables, for OSPFv2 tables with type-4 slots, and for tables of a non-backbone target area.
 constexpr uint32_t kBackboneBlocksPerSM = 4;
 constexpr uint32_t kBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kBackboneAsbrBlocksPerSM = 4;
+constexpr uint32_t kNonBackboneBlocksPerSM = 4;
 
 template <class R, bool kV3>
 int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
@@ -110,30 +127,8 @@ int version_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n
         ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
-// the walk of the table's version; a table with type-4 slots is the asbr calls'
-template <class R>
-int backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
-    return t->v3 ? version_cells<true>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells)
-                 : version_cells<false>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
-}
-
-template <class R>
-int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
-                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
-    return t->v3 ? version_delta<true>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of,
-                                        job_out, records, cap, n_records)
-                 : version_delta<false>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base,
-                                         base_of, job_out, records, cap, n_records);
-}
-
 // The cell over a table with type-4 slots: the plane sets the slots name, from each border's planes, row counts and
-// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]).
+// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when it names none.
 template <class R>
 int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
                    const uint32_t *const *border_status, const R *const *border_planes,
@@ -141,9 +136,9 @@ int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const h
                    OspfBackboneAsbrCell<hspf::PlanesOf<R>> &cell) {
     if (!t || t->v3) return HSPF_E_INVAL;
     if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    if (!border_planes || !border_n_rows || (n_jobs && !border_rows)) return HSPF_E_INVAL;
     auto &s = cell.sets;
     s.n = (uint32_t)t->asbr_set.size();
+    if (s.n && (!border_planes || !border_n_rows || (n_jobs && !border_rows))) return HSPF_E_INVAL;
     for (uint32_t k = 0; k < s.n; ++k) {
         const uint32_t b = t->asbr_set[k].first, i = t->asbr_set[k].second;
         if (!border_planes[b] || !border_n_rows[b] || (n_jobs && !border_rows[b])) return HSPF_E_INVAL;
@@ -157,6 +152,62 @@ int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const h
     return HSPF_OK;
 }
 
+template <class R>
+int nonbackbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                      const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                      const R *const *border_planes, const uint32_t *const *border_n_rows,
+                      const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    OspfNonBackboneCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                      n_jobs, cell))
+        return rc;
+    return hspf::launch_route_cells<kNonBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out,
+                                                             0, nullptr, nullptr, nullptr, nullptr);
+}
+
+template <class R>
+int nonbackbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                      const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                      const R *const *border_planes, const uint32_t *const *border_n_rows,
+                      const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                      const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                      uint64_t *n_records) {
+    OspfNonBackboneCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                      n_jobs, cell))
+        return rc;
+    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kNonBackboneBlocksPerSM>(
+        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+// the walk of the table's version and target area; a table with type-4 slots is the asbr calls'
+template <class R>
+int backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
+    if (t->area_id)
+        return nonbackbone_cells<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr,
+                                    job_status_out, cells);
+    return t->v3 ? version_cells<true>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells)
+                 : version_cells<false>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+}
+
+template <class R>
+int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
+    if (t->area_id)
+        return nonbackbone_delta<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr,
+                                    base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return t->v3 ? version_delta<true>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of,
+                                        job_out, records, cap, n_records)
+                 : version_delta<false>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base,
+                                         base_of, job_out, records, cap, n_records);
+}
+
 // A table without type-4 slots takes the calls above (NULL border planes allowed).
 template <class R>
 int backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
@@ -164,6 +215,9 @@ int backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint
                         const R *const *border_planes, const uint32_t *const *border_n_rows,
                         const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
     if (!t || t->v3) return HSPF_E_INVAL;
+    if (t->area_id)
+        return nonbackbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                                 border_rows, job_status_out, cells);
     if (!t->n_asbr_slots) return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
     OspfBackboneAsbrCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
@@ -181,6 +235,9 @@ int backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint
                         const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                         uint64_t *n_records) {
     if (!t || t->v3) return HSPF_E_INVAL;
+    if (t->area_id)
+        return nonbackbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                                 border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
     if (!t->n_asbr_slots)
         return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
                               records, cap, n_records);

@@ -1268,6 +1268,16 @@ int hspf_ospfv2_backbone_asbr_table_create(const hspf_ospfv2_flat *flat, uint32_
     return hspf::build_backbone_table<RibV2>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out, true);
 }
 
+int hspf_ospfv2_nonbackbone_table_create(const hspf_ospfv2_flat *flat, uint32_t router_id,
+                                         const hl_ospf_area_config *config, const hl_ospfv2_summary_lsa *sums,
+                                         uint32_t n_sums, const hl_ospfv2_external_lsa *ext, uint32_t n_ext,
+                                         const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                         hspf_ospfv2_backbone_table **out) {
+    if (!config) return HSPF_E_INVAL;
+    return hspf::build_backbone_table<RibV2>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out, true,
+                                             config);
+}
+
 int hspf_ospfv2_backbone_table_asbr_slots(const hspf_ospfv2_backbone_table *t, uint32_t *n_slots, uint32_t *n_sets) {
     if (!t) return HSPF_E_INVAL;
     if (n_slots) *n_slots = t->n_asbr_slots;

@@ -629,9 +629,15 @@ class BackboneTable:
 
     asbr=True (OSPFv2): hspf_ospfv2_backbone_asbr_table_create, which re-originates the borders' type-4 LSAs per job
     too; `n_asbr_slots` type-4 slots read `n_asbr_sets` (border, area) plane sets, and a table with type-4 slots is
-    read by backbone_asbr_cells_device / backbone_asbr_delta_device only."""
+    read by backbone_asbr_cells_device / backbone_asbr_delta_device only.
 
-    def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=(), asbr: bool = False):
+    config=area_config(...) (OSPFv2): hspf_ospfv2_nonbackbone_table_create, the table of an internal router R of the
+    non-backbone area of `flat` (the target area, `area_id`) over what-if jobs on the backbone; `summaries` are that
+    area's type-3/4 LSAs, `config` its configuration, and the borders' type-4 LSAs are re-originated per job as with
+    asbr=True.  The device calls of both kinds take it; backbone_from_cells decodes it over R's image of the area."""
+
+    def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=(), asbr: bool = False,
+                 config=None):
         from . import ospfv3
         self.lib = capi.load_library()
         self.flat, self.router_id, self.borders = flat, router_id, list(borders)
@@ -644,11 +650,18 @@ class BackboneTable:
         self.summaries, self.externals = sm, ext
         arr = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
         h = C.c_void_p()
+        self.area_id = int(flat.area.area_id) if config is not None else 0
         create = ("hspf_ospfv3_backbone_table_create" if self.v3 else
+                  "hspf_ospfv2_nonbackbone_table_create" if config is not None else
                   "hspf_ospfv2_backbone_asbr_table_create" if asbr else "hspf_ospfv2_backbone_table_create")
-        rc = getattr(self.lib, create)(flat.handle, router_id, sm.ctypes.data if len(sm) else None, len(sm),
-                                       ext.ctypes.data if len(ext) else None, len(ext), arr, len(self.borders),
-                                       C.byref(h))
+        args = (sm.ctypes.data if len(sm) else None, len(sm), ext.ctypes.data if len(ext) else None, len(ext), arr,
+                len(self.borders), C.byref(h))
+        if config is not None:
+            if self.v3:
+                raise ValueError("the non-backbone table is OSPFv2 only")
+            self.config = np.array([config], AREA_CONFIG_DT)
+            args = (self.config.ctypes.data,) + args
+        rc = getattr(self.lib, create)(flat.handle, router_id, *args)
         if rc != capi.HSPF_OK:
             raise capi.HspfError(rc, create + " failed")
         self.handle = h
@@ -751,7 +764,7 @@ def backbone_asbr_delta_device(ctx: capi.Context, t: BackboneTable, n_jobs: int,
 
 def backbone_from_cells(area: ospfv2.Ospfv2Area, t: BackboneTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
     """hspf_ospfv2_backbone_from_cells (host): one job's cells -> R's routes for the affected prefixes.  area: R's
-    area-0 image; gathers of R's row 0.  rc HSPF_E_UNSUPPORTED is returned in the result, as rib_from_cells."""
+    image of the table's area (area 0, or the target area of a non-backbone table); gathers of R's row 0.  rc HSPF_E_UNSUPPORTED is returned in the result, as rib_from_cells."""
     cells = np.ascontiguousarray(cells, RIB_CELL_DT)
     assert cells.shape == (t.n_prefixes,)
     gv = np.ascontiguousarray(gather_v, np.uint32)

@@ -903,3 +903,54 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
         out_borders.append(([p[0] for p in pair], [p[1] for p in pair], [p[2] for p in pair]))
     return {"r_area": r_area, "summaries0": summaries0, "externals": externals, "borders": out_borders,
             "shared": shared, "asbr": asbr, "area1_asbrs": asbrs1}
+
+
+def nonbackbone_view(t0: Topology, t1: Topology, seed: int, spf, r: int | None = None,
+                     borders=((1, 0), (2, 1), (3, 2)), max_paths: int = 16, n_ext_keys: int = 3, n_ext: int = 0):
+    """An internal router R of area 1 and the area border routers ("borders") between area 0 and area 1, each as its
+    own image: backbone_view's domain seen from area 1.  Seeded.  Areas, borders, the area-0 ASBR (the E flag) with
+    its type-5 LSAs and the shared /24 are backbone_view(t0, t1, seed, ...)'s; R is router r of t1 (default: the first
+    that is not a border).  `spf(csr, root_vertex, nh_words)` gives unperturbed planes, as area_from_planes takes them.
+    Returns a dict:
+      r_area        R's area-1 image;
+      summaries1    area 1's type-3/4 LSAs (LsaKey order): each border's hspf_ospfv2_net_summaries into area 1 over
+                    its update_rib_full at the unperturbed job (type-4: the area-0 ASBR);
+      externals     backbone_view's, plus n_ext /24s of the area-0 ASBR, both E-bit values (drawn from a generator of
+                    its own, so that every other part is as without them);
+      borders       per border (areas, area ids, summaries per area) as backbone_view's (the first border lists area 1
+                    first; a border's area-1 summaries are empty: with two active areas it reads only area 0's);
+      shared        the /24 that ties at the first border between area 0 and area 1;
+      asbr          the area-0 ASBR's router id."""
+    from . import ospf_rib
+    v = backbone_view(t0, t1, seed, borders=borders, max_paths=max_paths, n_ext_keys=n_ext_keys)
+    bids = [RID_BASE + int(i0) for i0, _ in borders]
+    idmap = {RID_BASE + int(i1): RID_BASE + int(i0) for i0, i1 in borders}
+    if r is None:
+        r = next(i for i in range(t1.n_routers) if i not in {int(i1) for _, i1 in borders})
+    ra = _set_flags(_area_remap(synth_area(t1, root=r, max_paths=max_paths), 1, idmap), {b: 0x01 for b in bids})
+    # the shared /24's stub in area 1, as the first border's area-1 image has it
+    a1 = next(a for a in v["borders"][0][0] if a.area_id == 1)
+    add1 = {}
+    for x in a1.router_lsas:
+        for l in a1.links[int(x["link_off"]): int(x["link_off"]) + int(x["n_links"])]:
+            if l["link_type"] == LINK_STUB and (int(l["link_id"]), int(l["link_data"])) == v["shared"]:
+                add1.setdefault(int(x["adv_rtr"]), []).append((v["shared"][0], v["shared"][1], int(l["metric"])))
+    ra = _with_stubs(ra, add1)
+    ext = v["externals"]
+    if n_ext:
+        rng = np.random.default_rng([seed, 0x0E1])
+        more = [(v["asbr"], 0x0F800000 | (q << 8), 0xFFFFFF00, int(rng.integers(1, 40)), 0, 11, q % 2, 0, (0, 0))
+                for q in range(n_ext)]
+        ext = np.asarray(sorted([tuple(x) for x in ext.tolist()] + more, key=lambda x: (x[0], x[1])),
+                         ospf_rib.EXTERNAL_LSA_DT)
+    sums = []
+    for areas, ids, bsums in v["borders"]:
+        rid = areas[0].router_id
+        rib_areas = [ospf_rib.RibArea(a.area_id, area_from_planes(a, spf), a.ifaces, s, True)
+                     for a, s in zip(areas, bsums)]
+        rib = ospf_rib.update_rib_full(rid, max_paths, rib_areas, ext)
+        sums += [tuple(x) for x in ospf_rib.net_summaries(rid, rib, ospf_rib.router_tables(rid, rib_areas), rib_areas,
+                                                          [ospf_rib.area_config()] * len(areas), ids.index(1)).tolist()]
+    sums.sort(key=lambda x: (x[4], x[0], x[1]))
+    return {"r_area": ra, "summaries1": np.asarray(sums, ospf_rib.SUMMARY_LSA_DT), "externals": ext,
+            "borders": v["borders"], "shared": v["shared"], "asbr": v["asbr"]}

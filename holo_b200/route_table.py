@@ -172,6 +172,7 @@ def declare(lib: C.CDLL):
                                             C.POINTER(ospf_rib.RibStruct)],
         "hspf_ospfv2_backbone_asbr_table_create": [vp, u32, vp, u32, vp, u32, pvp, u32, pvp],
         "hspf_ospfv2_backbone_table_asbr_slots": [vp, u32p, u32p],
+        "hspf_ospfv2_nonbackbone_table_create": [vp, u32, vp, vp, u32, vp, u32, pvp, u32, pvp],
         "hspf_ospfv2_backbone_asbr_cells": [vp, vp, u32, res, pvp, pvp, pvp, pvp, pvp, vp, vp],
         "hspf_ospfv2_backbone_asbr_cells16": [vp, vp, u32, res16, pvp, pvp, pvp, pvp, pvp, vp, vp],
         "hspf_ospfv2_backbone_asbr_delta": [vp, vp, u32, res, pvp, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],

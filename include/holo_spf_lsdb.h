@@ -362,9 +362,9 @@ int hspf_ospfv2_abr_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t
  *                                words; a job with a non-zero word gets empty cells.  cells[n_jobs][P] (device).
  *                                Nothing is launched for 0 jobs.  Enqueued on the ctx stream.
  *   hspf_ospfv2_backbone_delta[16]  the route-delta stage over the same walk (base cells as hspf_ospfv2_rib_delta).
- *   hspf_ospfv2_backbone_from_cells host: one job's cells -> the table of the contract.  area: R's area-0 image (the
- *                                one the flat came from); gather_v / gather_nh: nh_mask of the transit networks next to
- *                                R in row 0.  HSPF_E_UNSUPPORTED as hspf_ospfv2_rib_from_cells.
+ *   hspf_ospfv2_backbone_from_cells host: one job's cells -> the table of the contract.  area: R's image of the
+ *                                table's area (area 0 here), the one the flat came from; gather_v / gather_nh: nh_mask
+ *                                of the transit networks next to R in row 0.  HSPF_E_UNSUPPORTED as hspf_ospfv2_rib_from_cells.
  */
 #define HSPF_BACKBONE_MAX_BORDERS 8u
 typedef struct hspf_ospfv2_backbone_table hspf_ospfv2_backbone_table;
@@ -461,6 +461,51 @@ int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_
                                       const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                       hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                                       uint64_t *n_records);
+
+/*
+ * Non-backbone router over what-if jobs on the backbone (OSPFv2 only).  The same stage with source and target area
+ * swapped: R is an internal router of a non-backbone area A, and a job changes costs in area 0 only.  R's area-A SPT
+ * is its unperturbed one; what changes are the type-3 / type-4 LSAs that A's area border routers attached to area 0
+ * (the "borders") originate into A, because each border's routes move with the job.  The caller must give every area
+ * border router of A that is attached to area 0 as a border: another one keeps its base LSAs as static records, and
+ * the table cannot tell.  The borders' cells of job j come from hspf_ospfv2_abr_rib_cells[16], with each border's
+ * area-0 row of the job and row 0 of its other areas.  For job j, with border b's cells decoded to rib_b, the decoded
+ * cells of j equal the affected-prefix routes of
+ *     hspf_ospfv2_update_rib_full(R, max_paths, [{A, area_from_planes(A, R's row 0), ifaces, S_j, 1}], X)
+ * where S_j is A's type-3/4 LSAs with each border's LSAs replaced by hspf_ospfv2_net_summaries(rib_b, rtrs_b, ...,
+ * target A), in LsaKey order.  A border advertises a route of its cell when the cell is present and intra-area or
+ * inter-area, its winner is not one of A's intra-area records, no atom is an A atom, and the metric is below
+ * LSInfinity.  It originates a type-4 LSA for an ASBR it reaches intra-area, below LSInfinity, in one of its areas
+ * other than A (the usual case: an ASBR of area 0, whose distance is read from the border's area-0 row of the job).
+ * The affected prefixes are every prefix a border can advertise into A: one with an intra-area record in one of the
+ * border's areas other than A, or with a type-3 record in its area 0; with type-4 slots also the prefixes of those
+ * ASBRs' type-5 LSAs.  Every other prefix of R's table is R's base route in every job.  In a stub area a border's
+ * default route (0.0.0.0/0 at default_cost) stays a static record and no type-4 LSA is originated; a totally stubby
+ * area (summary 0) gives a table without slots, possibly with no affected prefix.
+ *
+ *   hspf_ospfv2_nonbackbone_table_create  host.  flat: R's area-A flat (A is flat's area id); config: A's
+ *                                configuration; the other arguments as hspf_ospfv2_backbone_table_create, over A's
+ *                                LSDB.  The result is an hspf_ospfv2_backbone_table marked with its target area A;
+ *                                the cells and delta calls above (both kinds) and hspf_ospfv2_backbone_table_* take it,
+ *                                the table's mark picks the walk, and a table with type-4 slots is the asbr calls', as
+ *                                above.  HSPF_E_INVAL: a flat of area 0, a NULL config, R missing from the flat or with
+ *                                the B flag, a border given twice or for OSPFv3, a border table without area 0 or A, a
+ *                                border that is not a B-flag router vertex of the flat, a usable type-3 LSA of a border
+ *                                in A for a prefix it cannot advertise (other than a stub area's default), a usable
+ *                                type-4 LSA of a border in A for a router it cannot originate for.
+ *                                HSPF_E_UNSUPPORTED: an NSSA, a V-flag router in A (A is a transit area), a usable
+ *                                type-4 LSA of another ABR in a border's area-0 summaries (an inter-area router entry
+ *                                at the border, whose per-job re-origination is not modelled), a router with the E and
+ *                                the B flag in a border's area other than A, slots reading more than 8 (border, area)
+ *                                plane sets, 0 or more than 8 borders.
+ * hspf_ospfv2_backbone_from_cells decodes the table over R's image of A.
+ */
+int hspf_ospfv2_nonbackbone_table_create(const hspf_ospfv2_flat *flat, uint32_t router_id,
+                                         const struct hl_ospf_area_config *config,
+                                         const hl_ospfv2_summary_lsa *summaries, uint32_t n_summaries,
+                                         const hl_ospfv2_external_lsa *externals, uint32_t n_externals,
+                                         const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                         hspf_ospfv2_backbone_table **out);
 
 /*
  * The same stage for OSPFv3.  The table is an hspf_ospfv2_backbone_table marked OSPFv3; the cells and delta calls
