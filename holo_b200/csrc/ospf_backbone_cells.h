@@ -36,6 +36,12 @@ namespace hspf {
 constexpr uint32_t kOspfBackboneMaxBorders = 8;
 constexpr uint32_t kOspfBackboneStatic = 0xFFFFFFFFu;   // RibRec::z of a static type-3 record
 
+// Whether a table's cell winners fit their u32 below kNoRecord: a slot's winner is n_recs + its slot index (OSPFv3:
+// n_recs + (slot index << 8 | prefix options)).  A table that does not is refused (HSPF_E_UNSUPPORTED).  Host only.
+inline bool backbone_winners_fit(uint64_t n_recs, uint64_t n_slots, bool v3) {
+    return n_recs + (v3 ? n_slots << 8 : n_slots) < 0xFFFFFFFFull;
+}
+
 // Type-3 records of the backbone table, beside R's one-area records (ospf_rib_cells.h):
 //   static: x ABR vertex, y LSA metric, z kOspfBackboneStatic
 //   slot:   x the border's vertex, y the prefix's index in the border's table, z the border, w the slot index

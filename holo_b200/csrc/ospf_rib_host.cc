@@ -160,12 +160,106 @@ struct V3 {
     }
 };
 
+// ---- router entries (area.state.routers), shared by rib_full and rtr_summaries -------------------
+template <class T> using HopsT = std::vector<HopT<typename T::Nh>>;
+template <class T>
+struct RtrT {
+    uint32_t area, metric;
+    uint8_t path, flags;
+    HopsT<T> hops;
+};
+template <class T> using RtrTable = std::unordered_map<uint32_t, RtrT<T>>;
+
+// the areas' SPF results are consistent with their next-hop arrays
+template <class T>
+bool areas_ok(const typename T::Area *areas, uint32_t n_areas) {
+    if (!areas && n_areas) return false;
+    for (uint32_t ai = 0; ai < n_areas; ++ai) {
+        const auto &a = areas[ai];
+        if (!a.spf || (a.n_ifaces && !a.ifaces) || (a.n_summaries && !a.summaries)) return false;
+        const auto &r = *a.spf;
+        if ((r.n_routers && !r.routers) || (r.n_routes && !r.routes) || (r.n_nexthops && !r.nexthops)) return false;
+        for (uint32_t i = 0; i < r.n_routers; ++i)
+            if ((uint64_t)r.routers[i].nh_off + r.routers[i].n_nh > r.n_nexthops) return false;
+        for (uint32_t i = 0; i < r.n_routes; ++i)
+            if ((uint64_t)r.routes[i].nh_off + r.routes[i].n_nh > r.n_nexthops) return false;
+    }
+    return true;
+}
+
+// an SPF entry's next hops, interfaces named by sort key, in NexthopKey order (same key twice: the later one stays)
+template <class T>
+HopsT<T> hops_of(const typename T::Area &a, uint32_t off, uint32_t n) {
+    HopsT<T> h;
+    h.reserve(n);
+    for (uint32_t i = 0; i < n; ++i) {
+        HopT<typename T::Nh> x;
+        x.nh = a.spf->nexthops[off + i];
+        const uint32_t sk = x.nh.iface < a.n_ifaces ? a.ifaces[x.nh.iface].sort_key : 0xFFFFFFFFu;
+        x.nh.iface = sk;                   // the merged table names interfaces by sort key
+        x.ka = ((uint64_t)sk << 1) | (x.nh.has_addr ? 1u : 0u);
+        T::addr_key(x.nh, x.kb);
+        h.push_back(x);
+    }
+    std::stable_sort(h.begin(), h.end(), key_less<typename T::Nh>);
+    HopsT<T> u;
+    for (const auto &x : h) {
+        if (!u.empty() && key_same(u.back(), x)) u.back() = x;
+        else u.push_back(x);
+    }
+    return u;
+}
+
+template <class T>
+bool summary_usable(uint32_t router_id, const typename T::Sum &l) {
+    return !l.maxage && l.metric < HL_LSA_INFINITY && l.adv_rtr != router_id && !T::skip(l);
+}
+
+// abr(): the area's entry for `adv` when it has the B flag
+template <class T>
+const RtrT<T> *abr_entry(const RtrTable<T> &rtrs, uint32_t adv) {
+    auto it = rtrs.find(adv);
+    return (it != rtrs.end() && (it->second.flags & HL_RTR_FLAG_B)) ? &it->second : nullptr;
+}
+
+// rib_full step 1, routers: the area's intra-area router entries
+template <class T>
+void intra_area_routers(const typename T::Area &a, RtrTable<T> &rtrs) {
+    for (uint32_t i = 0; i < a.spf->n_routers; ++i) {
+        const hl_route_rtr &r = a.spf->routers[i];
+        rtrs[r.router_id] = RtrT<T>{a.area_id, r.metric, HL_PATH_INTRA_AREA, r.flags, hops_of<T>(a, r.nh_off, r.n_nh)};
+    }
+}
+
+// rib_full step 2, ASBRs (update_rib_inter_area_routers): each usable type-4 / Inter-Area-Router LSA of the area
+// whose ABR has an entry writes an inter-area entry for the ASBR it names, replacing any earlier one
+template <class T>
+void inter_area_routers(uint32_t router_id, const typename T::Area &a, RtrTable<T> &rtrs) {
+    for (uint32_t i = 0; i < a.n_summaries; ++i) {
+        const auto &l = a.summaries[i];
+        if (l.lsa_type != 4 || !summary_usable<T>(router_id, l)) continue;
+        const RtrT<T> *br = abr_entry<T>(rtrs, l.adv_rtr);
+        if (!br) continue;
+        RtrT<T> e{a.area_id, br->metric + l.metric, HL_PATH_INTER_AREA, HL_RTR_FLAG_E, br->hops};
+        rtrs[T::asbr_id(l)] = std::move(e);
+    }
+}
+
+// rib_full step 2 reads every area's summaries with one active area, else only the backbone's
+template <class T>
+bool reads_summaries(const typename T::Area *areas, uint32_t n_areas, uint32_t ai) {
+    uint32_t n_active = 0;
+    for (uint32_t i = 0; i < n_areas; ++i) n_active += areas[i].active ? 1u : 0u;
+    return n_active <= 1 || areas[ai].area_id == 0;
+}
+
 // ---- the stages ------------------------------------------------------------------------------
 template <class T>
 int rib_full(uint32_t router_id, uint32_t max_paths, const typename T::Area *areas, uint32_t n_areas,
              const typename T::Ext *ext, uint32_t n_ext, typename T::Rib *out) {
     using Hop = HopT<typename T::Nh>;
-    using Hops = std::vector<Hop>;
+    using Hops = HopsT<T>;
+    using Rtr = RtrT<T>;
     struct Net {
         PKey key;
         uint32_t metric, type2, tag, area;
@@ -176,22 +270,7 @@ int rib_full(uint32_t router_id, uint32_t max_paths, const typename T::Area *are
         uint32_t label = 0;
         uint32_t origin_id = 0;            // LS origin of an intra-area route
     };
-    struct Rtr {
-        uint32_t area, metric;
-        uint8_t path, flags;
-        Hops hops;
-    };
-    if ((!areas && n_areas) || (!ext && n_ext) || !out) return HSPF_E_INVAL;
-    for (uint32_t ai = 0; ai < n_areas; ++ai) {
-        const auto &a = areas[ai];
-        if (!a.spf || (a.n_ifaces && !a.ifaces) || (a.n_summaries && !a.summaries)) return HSPF_E_INVAL;
-        const auto &r = *a.spf;
-        if ((r.n_routers && !r.routers) || (r.n_routes && !r.routes) || (r.n_nexthops && !r.nexthops)) return HSPF_E_INVAL;
-        for (uint32_t i = 0; i < r.n_routers; ++i)
-            if ((uint64_t)r.routers[i].nh_off + r.routers[i].n_nh > r.n_nexthops) return HSPF_E_INVAL;
-        for (uint32_t i = 0; i < r.n_routes; ++i)
-            if ((uint64_t)r.routes[i].nh_off + r.routes[i].n_nh > r.n_nexthops) return HSPF_E_INVAL;
-    }
+    if (!areas_ok<T>(areas, n_areas) || (!ext && n_ext) || !out) return HSPF_E_INVAL;
     auto clip = [&](Hops &h) { if (h.size() > max_paths) h.resize(max_paths); };
     auto prefer = [](const Net &a, const Net &b) -> int {      // route_compare; negative: a wins
         if (a.path != b.path) return a.path < b.path ? -1 : 1;
@@ -221,45 +300,20 @@ int rib_full(uint32_t router_id, uint32_t max_paths, const typename T::Area *are
         }
         clip(cur->hops);
     };
-    auto hops_of = [&](const typename T::Area &a, uint32_t off, uint32_t n) {
-        Hops h;
-        h.reserve(n);
-        for (uint32_t i = 0; i < n; ++i) {
-            Hop x;
-            x.nh = a.spf->nexthops[off + i];
-            const uint32_t sk = x.nh.iface < a.n_ifaces ? a.ifaces[x.nh.iface].sort_key : 0xFFFFFFFFu;
-            x.nh.iface = sk;                   // the merged table names interfaces by sort key
-            x.ka = ((uint64_t)sk << 1) | (x.nh.has_addr ? 1u : 0u);
-            T::addr_key(x.nh, x.kb);
-            h.push_back(x);
-        }
-        std::stable_sort(h.begin(), h.end(), key_less<typename T::Nh>);
-        Hops u;                                // same key twice: the later one stays
-        for (const Hop &x : h) {
-            if (!u.empty() && key_same(u.back(), x)) u.back() = x;
-            else u.push_back(x);
-        }
-        return u;
-    };
-    auto usable = [&](const typename T::Sum &l) {
-        return !l.maxage && l.metric < HL_LSA_INFINITY && l.adv_rtr != router_id && !T::skip(l);
-    };
-    std::vector<std::unordered_map<uint32_t, Rtr>> rtrs(n_areas);
+    auto usable = [&](const typename T::Sum &l) { return summary_usable<T>(router_id, l); };
+    std::vector<RtrTable<T>> rtrs(n_areas);
 
     // 1. per-area router tables; intra-area routes of all areas into one table
     for (uint32_t ai = 0; ai < n_areas; ++ai) {
         const auto &a = areas[ai];
-        for (uint32_t i = 0; i < a.spf->n_routers; ++i) {
-            const hl_route_rtr &r = a.spf->routers[i];
-            rtrs[ai][r.router_id] = Rtr{a.area_id, r.metric, HL_PATH_INTRA_AREA, r.flags, hops_of(a, r.nh_off, r.n_nh)};
-        }
+        intra_area_routers<T>(a, rtrs[ai]);
         for (uint32_t i = 0; i < a.spf->n_routes; ++i) {
             const auto &r = a.spf->routes[i];
             const PKey k = T::key(r);
             Net *cur = find(k);
             if (cur && r.metric > cur->metric) continue;
             Net n{k, r.metric, 0, 0, a.area_id, HL_PATH_INTRA_AREA, r.flags, T::options(r), true, false,
-                  hops_of(a, r.nh_off, r.n_nh)};
+                  hops_of<T>(a, r.nh_off, r.n_nh)};
             T::label_in(n.has_label, n.label, r);
             n.origin_id = r.origin_lsa_id;
             if (cur && r.origin_type == 2) {
@@ -276,15 +330,10 @@ int rib_full(uint32_t router_id, uint32_t max_paths, const typename T::Area *are
     }
 
     // 2. summaries: only the backbone's when more than one area is active
-    uint32_t n_active = 0;
-    for (uint32_t ai = 0; ai < n_areas; ++ai) n_active += areas[ai].active ? 1u : 0u;
-    auto abr = [&](uint32_t ai, uint32_t adv) -> const Rtr * {
-        auto it = rtrs[ai].find(adv);
-        return (it != rtrs[ai].end() && (it->second.flags & HL_RTR_FLAG_B)) ? &it->second : nullptr;
-    };
+    auto abr = [&](uint32_t ai, uint32_t adv) { return abr_entry<T>(rtrs[ai], adv); };
     for (uint32_t ai = 0; ai < n_areas; ++ai) {
         const auto &a = areas[ai];
-        if (n_active > 1 && a.area_id != 0) continue;
+        if (!reads_summaries<T>(areas, n_areas, ai)) continue;
         for (uint32_t i = 0; i < a.n_summaries; ++i) {            // networks
             const auto &l = a.summaries[i];
             if (l.lsa_type != 3 || !usable(l)) continue;
@@ -293,14 +342,7 @@ int rib_full(uint32_t router_id, uint32_t max_paths, const typename T::Area *are
             offer(Net{T::key(l), br->metric + l.metric, 0, 0, a.area_id, HL_PATH_INTER_AREA, 0, T::options(l), true,
                       false, br->hops});
         }
-        for (uint32_t i = 0; i < a.n_summaries; ++i) {            // ASBRs
-            const auto &l = a.summaries[i];
-            if (l.lsa_type != 4 || !usable(l)) continue;
-            const Rtr *br = abr(ai, l.adv_rtr);
-            if (!br) continue;
-            Rtr e{a.area_id, br->metric + l.metric, HL_PATH_INTER_AREA, HL_RTR_FLAG_E, br->hops};
-            rtrs[ai][T::asbr_id(l)] = std::move(e);               // replaces any earlier entry
-        }
+        inter_area_routers<T>(router_id, a, rtrs[ai]);            // ASBRs
     }
 
     // 3. transit areas
@@ -511,6 +553,27 @@ std::map<typename T::SumKey, std::pair<uint32_t, uint8_t>> net_summaries(const t
     return net;
 }
 
+// compute_rtr_summaries (holo-ospf area.rs:699-740) of an ABR for one target area: ASBR id -> metric.  `each(f)` calls
+// f(area_id, router_id, metric, path_type, flags, next hops, n_nh) for every router entry, in the call's area order
+// (an id in two areas keeps the later area's).  Only into a normal area, and only when more than one area is active.
+template <class Area, class Each>
+std::map<uint32_t, uint32_t> rtr_summaries(const Area *areas, uint32_t n_areas, uint32_t target,
+                                           const hl_ospf_area_config &cfg, Each each) {
+    std::map<uint32_t, uint32_t> rtr;
+    uint32_t n_active = 0;
+    for (uint32_t i = 0; i < n_areas; ++i) n_active += areas[i].active ? 1u : 0u;
+    if (n_active <= 1 || cfg.area_type != HL_AREA_NORMAL) return rtr;
+    const Area &ta = areas[target];
+    const bool backbone = ta.area_id == 0;
+    each([&](uint32_t area_id, uint32_t id, uint32_t metric, uint8_t path, uint8_t flags, const auto *nh, uint32_t n_nh) {
+        if (area_id == ta.area_id || !(flags & HL_RTR_FLAG_E) || metric >= HL_LSA_INFINITY) return;
+        if (backbone && path != HL_PATH_INTRA_AREA) return;
+        if (nexthops_on_area(ta, nh, n_nh)) return;
+        rtr[id] = metric;
+    });
+    return rtr;
+}
+
 }  // namespace
 
 // compute_net_summaries / compute_rtr_summaries (holo-ospf area.rs:561-740) of an ABR for one target area, without
@@ -527,19 +590,12 @@ extern "C" int hspf_ospfv2_net_summaries(uint32_t router_id, const hl_ospfv2_rib
     try {
         *n_out = 0;
         const auto net = net_summaries<V2>(*rib, areas, n_areas, target, config[target], {0u, 0u});
-        std::map<uint32_t, uint32_t> rtr;                             // ASBR id -> metric
-        uint32_t n_active = 0;
-        for (uint32_t i = 0; i < n_areas; ++i) n_active += areas[i].active ? 1u : 0u;
-        const hl_ospfv2_rib_area &ta = areas[target];
-        const bool backbone = ta.area_id == 0;
-        if (n_active > 1 && config[target].area_type == HL_AREA_NORMAL)   // only ABRs originate summaries
+        const auto rtr = rtr_summaries(areas, n_areas, target, config[target], [&](auto f) {
             for (uint32_t i = 0; i < rtrs->n_rtrs; ++i) {
                 const hl_rib_rtr &r = rtrs->rtrs[i];
-                if (r.area_id == ta.area_id || !(r.flags & HL_RTR_FLAG_E) || r.metric >= HL_LSA_INFINITY) continue;
-                if (backbone && r.path_type != HL_PATH_INTRA_AREA) continue;
-                if (nexthops_on_area(ta, rtrs->nexthops + r.nh_off, r.n_nh)) continue;
-                rtr[r.router_id] = r.metric;
+                f(r.area_id, r.router_id, r.metric, r.path_type, r.flags, rtrs->nexthops + r.nh_off, r.n_nh);
             }
+        });
         *n_out = (uint32_t)(net.size() + rtr.size());
         if (*n_out > cap) return HSPF_E_NOMEM;
         uint32_t k = 0;
@@ -598,4 +654,47 @@ extern "C" int hspf_ospfv3_rib_diff(const hl_ospfv3_rib *old_rib, hl_ospfv3_rib 
                                     uint32_t *n_out) {
     try { return rib_diff<V3>(old_rib, new_rib, out, cap, n_out); }
     catch (const std::bad_alloc &) { return HSPF_E_NOMEM; } catch (...) { return HSPF_E_INVAL; }
+}
+
+// compute_rtr_summaries for OSPFv3 (Inter-Area-Router contents): the type-4 rule of hspf_ospfv2_net_summaries over
+// the router entries update_rib_full leaves (hspf_ospfv2_rib_router_tables' for OSPFv2), rebuilt from the same areas
+extern "C" int hspf_ospfv3_rtr_summaries(uint32_t router_id, const hl_ospfv3_rib_area *areas,
+                                         const hl_ospf_area_config *config, uint32_t n_areas, uint32_t target,
+                                         hl_ospfv3_inter_area_lsa *out, uint32_t cap, uint32_t *n_out) {
+    if (!n_out || (cap && !out) || !areas || !config || target >= n_areas || !areas_ok<V3>(areas, n_areas))
+        return HSPF_E_INVAL;
+    try {
+        *n_out = 0;
+        std::vector<RtrTable<V3>> rtrs(n_areas);
+        for (uint32_t ai = 0; ai < n_areas; ++ai) intra_area_routers<V3>(areas[ai], rtrs[ai]);
+        for (uint32_t ai = 0; ai < n_areas; ++ai)
+            if (reads_summaries<V3>(areas, n_areas, ai)) inter_area_routers<V3>(router_id, areas[ai], rtrs[ai]);
+        const auto rtr = rtr_summaries(areas, n_areas, target, config[target], [&](auto f) {
+            std::vector<hl_nexthop6> nh;
+            for (const RtrTable<V3> &tab : rtrs) {
+                std::map<uint32_t, const RtrT<V3> *> by_id;             // router-id order
+                for (const auto &e : tab) by_id.emplace(e.first, &e.second);
+                for (const auto &e : by_id) {
+                    const RtrT<V3> &r = *e.second;
+                    nh.clear();
+                    for (const auto &h : r.hops) nh.push_back(h.nh);
+                    f(r.area, e.first, r.metric, r.path, r.flags, nh.data(), (uint32_t)nh.size());
+                }
+            }
+        });
+        *n_out = (uint32_t)rtr.size();
+        if (*n_out > cap) return HSPF_E_NOMEM;
+        uint32_t k = 0;
+        for (const auto &e : rtr) {
+            hl_ospfv3_inter_area_lsa l;
+            std::memset(&l, 0, sizeof(l));
+            l.adv_rtr = router_id; l.router_id = e.first; l.metric = e.second; l.lsa_type = 4;
+            out[k++] = l;
+        }
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
 }

@@ -8,7 +8,8 @@
 //                      records over the one-area tables of its areas (ospf_abr_rib_cells.h)
 //   build_backbone_table  hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create: a backbone router's
 //                      affected prefixes over its one-area table and its borders' ABR tables (ospf_backbone_cells.h);
-//                      hspf_ospfv2_nonbackbone_table_create: the same for an internal router of a non-backbone area
+//                      hspf_ospfv{2,3}_nonbackbone_table_create: the same for an internal router of a non-backbone
+//                      area
 //   decode_rib         one job's cells -> its routing table, for hspf_ospfv2_rib_from_cells,
 //                      hspf_ospfv3_rib_from_cells, hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib) and
 //                      hspf_ospfv{2,3}_backbone_from_cells (decode_backbone_rib).  A one-area table decodes as an area
@@ -36,6 +37,7 @@
 //
 // For build_backbone_table it also provides:
 //   router_flags(f, v)         the Router-LSA flags of router vertex v of f (its first fragment's)
+//   default_key()              the key of the default route (0.0.0.0/0, ::/0)
 //
 // For decode_rib it also provides:
 //   Area, Rib                  the area image and the caller's output
@@ -352,11 +354,12 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
 // (ospf_backbone_cells.h).  Border tables of the other version are refused (HSPF_E_INVAL).  `asbr`
 // (hspf_ospfv2_backbone_asbr_table_create): the borders' type-4 LSAs are re-originated per job too, as type-4 slots,
 // and the prefixes of the type-5 LSAs they lead to are affected; else a usable one is HSPF_E_UNSUPPORTED.
-// `config` (hspf_ospfv2_nonbackbone_table_create, OSPFv2 only): R is an internal router of the non-backbone area of
-// `flat` with that configuration, the target area A.  The borders re-originate into A their intra-area routes of
-// their other areas and their inter-area routes, and type-4 LSAs for the ASBRs they reach intra-area outside A (plane
-// sets of any of those areas, area 0 included); in a stub area the default route stays static and no type-4 LSA is
-// originated, and a totally stubby area has no slot.
+// `config` (hspf_ospfv{2,3}_nonbackbone_table_create): R is an internal router of the non-backbone area of `flat` with
+// that configuration, the target area A.  The borders re-originate into A their intra-area routes of their other
+// areas and their inter-area routes, and type-4 / Inter-Area-Router LSAs for the ASBRs they reach intra-area outside A
+// (plane sets of any of those areas, area 0 included); in a stub area the default route stays static and no type-4
+// LSA is originated, and a totally stubby area has no slot.  OSPFv3: a border's options bytes also cover its type-3
+// records, so that an inter-area cell's winner gives the options of the LSA the border copies them from.
 template <class T>
 int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const typename T::Sum *sums, uint32_t n_sums,
                          const typename T::Ext *ext, uint32_t n_ext, const hspf_ospfv2_abr_ribtable *const *borders,
@@ -370,7 +373,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
     const bool nb = config != nullptr;                            // a non-backbone target area
     const uint32_t ta = nb ? flat->area->area_id : 0;
     if (nb) {
-        if (T::kV3 || ta == 0) return HSPF_E_INVAL;
+        if (ta == 0) return HSPF_E_INVAL;
         if (config->area_type == HL_AREA_NSSA || n_borders == 0 || n_borders > kOspfBackboneMaxBorders)
             return HSPF_E_UNSUPPORTED;
         asbr = true;
@@ -414,10 +417,8 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
             }
         }
         // the default route a border originates into a stub area, at default_cost whatever the job
-        auto stub_default = [&](const Sum &l) {
-            if constexpr (T::kV3) return false;
-            else return nb && !normal && l.lsa_type == 3 && l.lsa_id == 0 && l.mask == 0;
-        };
+        const Key dflt = T::default_key();
+        auto stub_default = [&](const Sum &l) { return nb && !normal && l.lsa_type == 3 && T::key(l) == dflt; };
         // R's area without the borders' type-3 LSAs: R's one-area table over the rest
         auto live = [](const Sum &l) { return !l.maxage && l.metric < HL_LSA_INFINITY && !T::skip(l); };
         std::vector<Sum> rest;
@@ -481,8 +482,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                 bool adv = nb && bt.off[(A + a0[b]) * S + u] != bt.off[(A + a0[b]) * S + u + 1];
                 for (uint32_t i = 0; i < A && !adv; ++i)
                     adv = bt.area_id[i] != ta && bt.off[i * S + u] != bt.off[i * S + u + 1];
-                if constexpr (!T::kV3)
-                    if (nb && !normal && bt.prefix[u] == 0 && bt.plen[u] == 0) adv = false;
+                if (nb && !normal && T::table_key(bt, u) == dflt) adv = false;
                 if (adv) slots[T::table_key(bt, u)].emplace_back(b, u);
             }
         }
@@ -599,15 +599,16 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
             }
             if (t->asbr_set.size() > kOspfBackboneMaxAsbrSets) return HSPF_E_UNSUPPORTED;   // the kernel parameter's
         }
-        // winners are u32: a slot's is n_recs + its index (OSPFv3: n_recs + (index << 8 | options))
-        const uint64_t n_slots = t->slot_rec.size();
-        if ((uint64_t)t->recs.size() + (T::kV3 ? n_slots << 8 : n_slots) >= kNone) return HSPF_E_UNSUPPORTED;
+        if (!backbone_winners_fit(t->recs.size(), t->slot_rec.size(), T::kV3)) return HSPF_E_UNSUPPORTED;
         t->words.assign(r.off.begin(), r.off.begin() + PR + 1);
         t->words.insert(t->words.end(), q.begin(), q.end());
         t->words.insert(t->words.end(), o3.begin(), o3.end());
         t->words.insert(t->words.end(), o5.begin(), o5.end());
         t->words.resize(t->border_at(), 0);
         uint32_t opt_words = (T::kV3 ? 8 : 4) * n_borders;         // OSPFv3: the options bytes follow the border words
+        // OSPFv3: a border's options bytes, one per record an advertised cell's winner can be: its intra-area records,
+        // and into a non-backbone area its type-3 records too
+        auto opt_end = [&](const hspf_ospfv2_abr_ribtable &bt) { return nb ? bt.t3_end : bt.t3_base[0]; };
         for (uint32_t b = 0; b < n_borders; ++b) {
             const hspf_ospfv2_abr_ribtable &bt = *borders[b];
             const uint32_t i = at[b], lo = bt.intra_base[i], na = bt.n_atoms[i];
@@ -615,12 +616,13 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
             t->words.insert(t->words.end(), {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)});
             if (T::kV3) {
                 t->words.insert(t->words.end(), {4 * opt_words, 0u, 0u, 0u});
-                opt_words += (bt.t3_base[0] + 3) / 4;
+                opt_words += (opt_end(bt) + 3) / 4;
             }
         }
         if (T::kV3) {
             // per border, the prefix options of each intra-area record of its table, as the OSPFv3 intra-area decode
-            // reads them for that winner: the record's entry in its area's intra-area table
+            // reads them for that winner: the record's entry in its area's intra-area table; into a non-backbone area
+            // also those of each type-3 record (an inter-area cell's winner), the options of its LSA
             for (uint32_t b = 0; b < n_borders; ++b) {
                 const hspf_ospfv2_abr_ribtable &bt = *borders[b];
                 std::vector<uint8_t> opt;
@@ -629,7 +631,12 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                     if (o.size() != bt.area[i]->n_intra || opt.size() != bt.intra_base[i]) return HSPF_E_INVAL;
                     opt.insert(opt.end(), o.begin(), o.end());
                 }
-                opt.resize(((size_t)bt.t3_base[0] + 3) & ~(size_t)3, 0);
+                if (nb) {
+                    const size_t n3 = bt.t3_end - bt.t3_base[0];
+                    if (opt.size() != bt.t3_base[0] || bt.options6.size() < n3) return HSPF_E_INVAL;
+                    opt.insert(opt.end(), bt.options6.begin(), bt.options6.begin() + n3);
+                }
+                opt.resize(((size_t)opt_end(bt) + 3) & ~(size_t)3, 0);
                 const size_t at = t->words.size();
                 t->words.resize(at + opt.size() / 4);
                 if (!opt.empty()) std::memcpy(t->words.data() + at, opt.data(), opt.size());

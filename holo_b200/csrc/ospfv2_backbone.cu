@@ -1,9 +1,9 @@
 // Device stage for the routing table of an OSPF backbone router over what-if jobs inside other areas
 // (include/holo_spf_lsdb.h, "backbone router over what-if jobs inside other areas"): update_rib_full at the router,
 // for its affected prefixes, with every border's type-3 / Inter-Area-Prefix LSAs in area 0 re-originated for the job.
-// The entry points serve OSPFv2 and OSPFv3 tables alike, and OSPFv2 tables of an internal router of a non-backbone
-// area over jobs on the backbone (hspf_ospfv2_nonbackbone_table_create): the table's mark picks the walk's
-// instantiation.
+// The entry points serve OSPFv2 and OSPFv3 tables alike, and tables of an internal router of a non-backbone area over
+// jobs on the backbone (hspf_ospfv{2,3}_nonbackbone_table_create): the table's marks (version, target area) pick the
+// walk's instantiation.
 //
 // One launch on the ctx stream: one thread per (job, prefix) runs ospf_backbone_cell_eval (ospf_backbone_cells.h)
 // over the router's unperturbed area-0 planes (row 0) and the job's row of each border's routing-table cells, and
@@ -78,12 +78,29 @@ struct OspfNonBackboneCell : OspfBackboneAsbrCell<Planes> {
     }
 };
 
+// The same over an OSPFv3 table (hspf_ospfv3_nonbackbone_table_create): slot winners carry prefix options, and a
+// plane set is a border's area 0 read for an Inter-Area-Router slot.  A type of its own, so that the OSPFv2 kernels
+// above keep their instantiations.
+template <class Planes>
+struct OspfNonBackboneV3Cell : OspfBackboneAsbrCell<Planes> {
+    using Base = OspfBackboneCell<Planes, false>;
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
+        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {this->sets, j}};
+        return hspf::ospf_backbone_cell_eval<true, true, true>(pl, this->t, p, rows);
+    }
+};
+
 // Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
-// and for OSPFv3 tables, for OSPFv2 tables with type-4 slots, and for tables of a non-backbone target area.
+// and for OSPFv3 tables, for OSPFv2 tables with type-4 slots, and for OSPFv2 and OSPFv3 tables of a non-backbone
+// target area.
 constexpr uint32_t kBackboneBlocksPerSM = 4;
 constexpr uint32_t kBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kBackboneAsbrBlocksPerSM = 4;
 constexpr uint32_t kNonBackboneBlocksPerSM = 4;
+constexpr uint32_t kNonBackboneV3BlocksPerSM = 4;
 
 template <class R, bool kV3>
 int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
@@ -128,13 +145,14 @@ int version_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n
 }
 
 // The cell over a table with type-4 slots: the plane sets the slots name, from each border's planes, row counts and
-// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when it names none.
+// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when it names none.  Of OSPFv3
+// tables only those of a non-backbone target area have such slots (Inter-Area-Router slots).
 template <class R>
 int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
                    const uint32_t *const *border_status, const R *const *border_planes,
                    const uint32_t *const *border_n_rows, const uint32_t *const *border_rows, uint32_t n_jobs,
                    OspfBackboneAsbrCell<hspf::PlanesOf<R>> &cell) {
-    if (!t || t->v3) return HSPF_E_INVAL;
+    if (!t || (t->v3 && !t->area_id)) return HSPF_E_INVAL;
     if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
     auto &s = cell.sets;
     s.n = (uint32_t)t->asbr_set.size();
@@ -152,17 +170,47 @@ int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const h
     return HSPF_OK;
 }
 
+template <class Cell, uint32_t kBlocks, class R>
+int nonbackbone_cells_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                         const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                         const R *const *border_planes, const uint32_t *const *border_n_rows,
+                         const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    Cell cell{};
+    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                      n_jobs, cell))
+        return rc;
+    return hspf::launch_route_cells<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out, 0, nullptr,
+                                             nullptr, nullptr, nullptr);
+}
+
+template <class Cell, uint32_t kBlocks, class R>
+int nonbackbone_delta_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                         const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                         const R *const *border_planes, const uint32_t *const *border_n_rows,
+                         const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                         const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                         uint64_t *n_records) {
+    Cell cell{};
+    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                      n_jobs, cell))
+        return rc;
+    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBlocks>(
+        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+// a table of a non-backbone target area: the walk of its version
 template <class R>
 int nonbackbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
                       const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                       const R *const *border_planes, const uint32_t *const *border_n_rows,
                       const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    OspfNonBackboneCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                      n_jobs, cell))
-        return rc;
-    return hspf::launch_route_cells<kNonBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out,
-                                                             0, nullptr, nullptr, nullptr, nullptr);
+    using P = hspf::PlanesOf<R>;
+    return t->v3 ? nonbackbone_cells_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                       job_status_out, cells)
+                 : nonbackbone_cells_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                       job_status_out, cells);
 }
 
 template <class R>
@@ -172,12 +220,13 @@ int nonbackbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32
                       const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
                       const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                       uint64_t *n_records) {
-    OspfNonBackboneCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                      n_jobs, cell))
-        return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kNonBackboneBlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+    using P = hspf::PlanesOf<R>;
+    return t->v3 ? nonbackbone_delta_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                       base_cells, n_base, base_of, job_out, records, cap, n_records)
+                 : nonbackbone_delta_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                       base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
 
 // the walk of the table's version and target area; a table with type-4 slots is the asbr calls'
@@ -208,13 +257,14 @@ int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t 
                                          base_of, job_out, records, cap, n_records);
 }
 
-// A table without type-4 slots takes the calls above (NULL border planes allowed).
+// A table without type-4 slots takes the calls above (NULL border planes allowed).  An OSPFv3 table of area 0 is
+// refused.
 template <class R>
 int backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
                         const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                         const R *const *border_planes, const uint32_t *const *border_n_rows,
                         const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    if (!t || t->v3) return HSPF_E_INVAL;
+    if (!t || (t->v3 && !t->area_id)) return HSPF_E_INVAL;
     if (t->area_id)
         return nonbackbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
                                  border_rows, job_status_out, cells);
@@ -234,7 +284,7 @@ int backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint
                         const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
                         const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                         uint64_t *n_records) {
-    if (!t || t->v3) return HSPF_E_INVAL;
+    if (!t || (t->v3 && !t->area_id)) return HSPF_E_INVAL;
     if (t->area_id)
         return nonbackbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
                                  border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);

@@ -1070,6 +1070,7 @@ struct RibV2 {
     static Key key(const Sum &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
     static Key key(const Ext &l) { return pkey(l.lsa_id, (uint32_t)__builtin_popcount(l.mask)); }
     static Key intra_key(const hspf::RouteTable &t, uint32_t k) { return pkey(t.prefix[k], t.plen[k]); }
+    static Key default_key() { return pkey(0, 0); }
     static bool skip(const Sum &) { return false; }
     static bool skip(const Ext &) { return false; }
     static uint32_t asbr_id(const Sum &l) { return l.lsa_id; }

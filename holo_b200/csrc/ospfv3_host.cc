@@ -739,6 +739,7 @@ struct RibV3 {
     static Key key(const Sum &l) { return mk(l.prefix, l.len); }
     static Key key(const Ext &l) { return mk(l.prefix, l.len); }
     static Key intra_key(const hspf::RouteTable &t, uint32_t k) { return mk(t.prefix6[k], (uint8_t)t.plen[k]); }
+    static Key default_key() { return Key{}; }
     static bool skip(const Sum &l) { return l.lsa_type == 3 && (l.prefix_options & HL_PFX_OPT_NU); }
     static bool skip(const Ext &l) { return (l.prefix_options & HL_PFX_OPT_NU) != 0; }
     static uint32_t asbr_id(const Sum &l) { return l.router_id; }
@@ -904,6 +905,16 @@ int hspf_ospfv3_backbone_table_create(const hspf_ospfv3_flat *flat, uint32_t rou
                                       const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
                                       hspf_ospfv2_backbone_table **out) {
     return hspf::build_backbone_table<RibV3>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out);
+}
+
+int hspf_ospfv3_nonbackbone_table_create(const hspf_ospfv3_flat *flat, uint32_t router_id,
+                                         const hl_ospf_area_config *config, const hl_ospfv3_inter_area_lsa *sums,
+                                         uint32_t n_sums, const hl_ospfv3_external_lsa *ext, uint32_t n_ext,
+                                         const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                         hspf_ospfv2_backbone_table **out) {
+    if (!config) return HSPF_E_INVAL;
+    return hspf::build_backbone_table<RibV3>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out, true,
+                                             config);
 }
 
 int hspf_ospfv3_backbone_table_prefixes6(const hspf_ospfv2_backbone_table *t, uint32_t *n_prefixes,

@@ -237,7 +237,7 @@ def _area_array(areas: list, keep: list, with_results: bool, v3: bool = False):
         keep += [ifs, sm]
         arr[i].area_id, arr[i].n_summaries = a.area_id, len(sm)
         if with_results:
-            rs = _result_struct(a.result, keep)
+            rs = _result_struct(a.result, keep, v3)
             keep.append(rs)
             arr[i].spf = C.addressof(rs)
         arr[i].ifaces = ifs.ctypes.data if len(ifs) else None
@@ -612,6 +612,26 @@ def net_summaries_v3(router_id: int, rib: Rib, areas: list, configs: list, targe
     return out[: n.value].copy()
 
 
+def rtr_summaries_v3(router_id: int, areas: list, configs: list, target: int) -> np.ndarray:
+    """hspf_ospfv3_rtr_summaries (host): the Inter-Area-Router contents the router originates into areas[target]
+    (compute_rtr_summaries), as INTER_AREA_LSA_DT[] with adv_rtr = router_id, lsa_type 4, router_id the ASBR and its
+    metric, in router-id order.  areas: the RibArea list given update_rib_full_v3; configs: one area_config() per
+    area."""
+    lib = capi.load_library()
+    keep = []
+    arr = _area_array(areas, keep, True, v3=True)
+    cfg = np.asarray(list(configs) or [area_config()], AREA_CONFIG_DT)
+    # one entry per id at most: every area's routers, and the ASBRs its Inter-Area-Router LSAs name
+    cap = sum(len(a.result.routers) + int((np.asarray(a.summaries)["lsa_type"] == 4).sum()) for a in areas) + 1
+    out = np.zeros(cap, INTER_AREA_LSA_DT)
+    n = C.c_uint32()
+    rc = lib.hspf_ospfv3_rtr_summaries(router_id, arr, cfg.ctypes.data, len(areas), target, out.ctypes.data, cap,
+                                       C.byref(n))
+    if rc != capi.HSPF_OK:
+        raise capi.HspfError(rc, "hspf_ospfv3_rtr_summaries failed")
+    return out[: n.value].copy()
+
+
 # ---- backbone router over what-if jobs inside other areas (include/holo_spf_lsdb.h) -----------------------------
 BACKBONE_MAX_BORDERS = 8           # HSPF_BACKBONE_MAX_BORDERS
 
@@ -631,10 +651,12 @@ class BackboneTable:
     too; `n_asbr_slots` type-4 slots read `n_asbr_sets` (border, area) plane sets, and a table with type-4 slots is
     read by backbone_asbr_cells_device / backbone_asbr_delta_device only.
 
-    config=area_config(...) (OSPFv2): hspf_ospfv2_nonbackbone_table_create, the table of an internal router R of the
-    non-backbone area of `flat` (the target area, `area_id`) over what-if jobs on the backbone; `summaries` are that
-    area's type-3/4 LSAs, `config` its configuration, and the borders' type-4 LSAs are re-originated per job as with
-    asbr=True.  The device calls of both kinds take it; backbone_from_cells decodes it over R's image of the area."""
+    config=area_config(...): hspf_ospfv2_nonbackbone_table_create (from an ospfv3.Flat:
+    hspf_ospfv3_nonbackbone_table_create), the table of an internal router R of the non-backbone area of `flat` (the
+    target area, `area_id`) over what-if jobs on the backbone; `summaries` are that area's type-3/4 (Inter-Area-Prefix
+    / Inter-Area-Router) LSAs, `config` its configuration, and the borders' type-4 LSAs are re-originated per job as
+    with asbr=True.  The device calls of both kinds take it; backbone_from_cells (backbone_from_cells_v3) decodes it
+    over R's image of the area."""
 
     def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=(), asbr: bool = False,
                  config=None):
@@ -651,14 +673,13 @@ class BackboneTable:
         arr = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
         h = C.c_void_p()
         self.area_id = int(flat.area.area_id) if config is not None else 0
-        create = ("hspf_ospfv3_backbone_table_create" if self.v3 else
+        create = ("hspf_ospfv3_nonbackbone_table_create" if self.v3 and config is not None else
+                  "hspf_ospfv3_backbone_table_create" if self.v3 else
                   "hspf_ospfv2_nonbackbone_table_create" if config is not None else
                   "hspf_ospfv2_backbone_asbr_table_create" if asbr else "hspf_ospfv2_backbone_table_create")
         args = (sm.ctypes.data if len(sm) else None, len(sm), ext.ctypes.data if len(ext) else None, len(ext), arr,
                 len(self.borders), C.byref(h))
         if config is not None:
-            if self.v3:
-                raise ValueError("the non-backbone table is OSPFv2 only")
             self.config = np.array([config], AREA_CONFIG_DT)
             args = (self.config.ctypes.data,) + args
         rc = getattr(self.lib, create)(flat.handle, router_id, *args)
@@ -778,7 +799,8 @@ def backbone_from_cells(area: ospfv2.Ospfv2Area, t: BackboneTable, cells: np.nda
 def backbone_from_cells_v3(area, t: BackboneTable, cells: np.ndarray, gather_v, gather_nh) -> Rib:
     """hspf_ospfv3_backbone_from_cells (host): one job's cells over an OSPFv3 BackboneTable -> R's routes for the
     affected prefixes, prefix options included (RIB_ROUTE6_DT routes, ospfv3.NEXTHOP6_DT next hops).  area: R's
-    area-0 ospfv3.Ospfv3Area image; gathers of R's row 0.  rc HSPF_E_UNSUPPORTED is returned in the result."""
+    ospfv3.Ospfv3Area image of the table's area (area 0, or the target area of a non-backbone table); gathers of R's
+    row 0.  rc HSPF_E_UNSUPPORTED is returned in the result."""
     from . import ospfv3
     cells = np.ascontiguousarray(cells, RIB_CELL_DT)
     assert cells.shape == (t.n_prefixes,)

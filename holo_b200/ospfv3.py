@@ -650,7 +650,7 @@ def abr_view(topos: list, seed: int, area_ids=None, roots=None, max_paths: int =
 
 
 def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1, 0), (2, 1), (3, 2)),
-                  max_paths: int = 16, n_ext_keys: int = 3, t2: Topology | None = None):
+                  max_paths: int = 16, n_ext_keys: int = 3, t2: Topology | None = None, r1: int | None = None):
     """The OSPFv3 twin of ospfv2.backbone_view: a backbone router R of area 0 and the area border routers ("borders")
     of one other area 1, each as its own image.  Seeded.  Area 0 is synth_area(t0) (router i is RID_BASE + i), area 1
     synth_area(t1) with router ids, prefixes and interface sort keys in ranges of its own, except that border (i0, i1)
@@ -669,7 +669,8 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
                     lower router id's record, and a job that lengthens that router's path alone hands the route to
                     the other record at the same metric, with other options;
       shared        (address bytes, length) of a /64 that is intra-area in area 1 (LA) and area 2 (P) at metrics that
-                    tie at the first border (its route there keeps area 1's options, the first of its areas)."""
+                    tie at the first border (its route there keeps area 1's options, the first of its areas);
+      r1_area       with r1: the area-1 image of router r1 of t1, with area 1's prefixes as the borders see them."""
     from . import ospf_rib, synth
     from .ospfv2 import _dist_from
     rng = np.random.default_rng(seed)
@@ -732,6 +733,7 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
     adds2 = {n2[1]: [(shared[0], 64, PFX_P, 10 + max(0, n1[0] - n2[0]))]}
     a1s = [_with_prefixes(a, adds1) for a in a1s]
     a2 = _with_prefixes(a2, adds2)
+    r1_area = _with_prefixes(image(t1, 1, r1, b1map), adds1) if r1 is not None else None
     # each border's Inter-Area-Prefix LSAs into area 0: its other areas' prefixes that are not area 0's
     own0 = {(bytes(int(b) for b in p["addr"]["bytes"]), int(p["len"])) for p in r_area.prefixes}
     sums0 = []
@@ -773,5 +775,101 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
             out_borders.append(([a1, a0, a2], [1, 0, 2], [empty, s0, empty]))
         else:
             out_borders.append(([a0, a1], [0, 1], [s0, empty]))
-    return {"r_area": r_area, "summaries0": summaries0, "externals": externals, "borders": out_borders,
-            "flip": flip, "shared": shared, "asbr": asbr}
+    out = {"r_area": r_area, "summaries0": summaries0, "externals": externals, "borders": out_borders,
+           "flip": flip, "shared": shared, "asbr": asbr}
+    if r1 is not None:
+        out["r1_area"] = r1_area
+    return out
+
+
+def _lsa_array(rows, dt):
+    out = np.zeros(len(rows), dt)
+    for i, x in enumerate(rows):
+        out[i] = x
+    return out
+
+
+def nonbackbone_view(t0: Topology, t1: Topology, seed: int, spf, r: int | None = None,
+                     borders=((1, 0), (2, 1), (3, 2)), max_paths: int = 16, n_ext_keys: int = 3, n_ext: int = 0):
+    """The OSPFv3 twin of ospfv2.nonbackbone_view: an internal router R of area 1 and the area border routers
+    ("borders") between area 0 and area 1, each as its own image: backbone_view's domain seen from area 1.  Seeded.
+    Areas, borders (the first also in area 2), the area-0 ASBR (the E flag) with its AS-external LSAs are
+    backbone_view(t0, t1, seed, ...)'s; R is router r of t1 (default: the first that is not a border).  Two area-0
+    routers also get the B flag and advertise one /128 into area 0, one with the LA and one with the P option, at
+    metrics that tie at the first border (the "inter-area flip": the first border's inter-area route takes the first
+    LSA's record, and a job that lengthens that router's path alone hands the route to the other at the same metric,
+    with other options).  `spf(csr, root_vertex, nh_words)` gives unperturbed planes, as area_from_planes takes them.
+    Returns a dict:
+      r_area        R's area-1 image;
+      summaries1    area 1's Inter-Area-Prefix / Inter-Area-Router LSAs (LsaKey order): each border's
+                    hspf_ospfv3_net_summaries and hspf_ospfv3_rtr_summaries into area 1 over its update_rib_full at the
+                    unperturbed job, lsa_id numbered per border (nonbackbone_lsas);
+      externals     backbone_view's, plus n_ext /64s of the area-0 ASBR, both E-bit values (drawn from a generator of
+                    its own, so that every other part is as without them);
+      borders       per border (areas, area ids, inter-area LSAs per area) as backbone_view's, the area-0 LSAs holding
+                    the inter-area flip's two;
+      flip          (address bytes, length) of the inter-area flip's /128, and its two advertisers (LA's first);
+      shared        backbone_view's shared /64;
+      asbr          the area-0 ASBR's router id."""
+    from . import ospf_rib
+    from .ospfv2 import _dist_from
+    bids = {RID_BASE + int(i0) for i0, _ in borders}
+    if r is None:
+        r = next(i for i in range(t1.n_routers) if i not in {int(i1) for _, i1 in borders})
+    v = backbone_view(t0, t1, seed, borders=borders, max_paths=max_paths, n_ext_keys=n_ext_keys, r1=r)
+    rng = np.random.default_rng([seed, 0x1F1])
+    # the inter-area flip: two area-0 routers, neither a border nor the ASBR, tying at the first border
+    first = next(a for a in v["borders"][0][0] if a.area_id == 0)
+    fl = Flat(first)
+    d = _dist_from(fl, fl.router_vertex(first.router_id))
+    dist = {int(fl.router_ids[u]): int(d[u]) for u in range(len(fl.router_ids)) if fl.is_router[u] and d[u] < 1 << 40}
+    cand = sorted(x for x in dist if x not in bids and x != v["asbr"])
+    x, y = sorted(int(q) for q in rng.choice(cand, 2, replace=False))
+    M = max(dist[x], dist[y]) + 7
+    key = (ipaddress.IPv6Address((0x20010DB8 << 96) | (0xF3_0000 << 64) | 1).packed, 128)
+    rec = lambda b: (tuple(b), 1, (0, 0, 0))
+    flip_lsas = [(x, 0x900, M - dist[x], 0, rec(key[0]), 128, PFX_LA, 3, 0),
+                 (y, 0x900, M - dist[y], 0, rec(key[0]), 128, PFX_P, 3, 0)]
+    out_borders = []
+    for areas, ids, sums in v["borders"]:
+        areas = list(areas)
+        i0 = ids.index(0)
+        a0 = Ospfv3Area(**{k: getattr(areas[i0], k) for k in areas[i0].__dataclass_fields__})
+        rl = a0.router_lsas.copy()
+        for q in (x, y):
+            rl["flags"][rl["adv_rtr"] == q] |= 0x01
+        a0.router_lsas = rl
+        areas[i0] = a0
+        s0 = sorted([tuple(z) for z in sums[i0].tolist()] + flip_lsas, key=lambda z: (z[7], z[0], z[1]))
+        sums = list(sums)
+        sums[i0] = _lsa_array(s0, ospf_rib.INTER_AREA_LSA_DT)
+        out_borders.append((areas, ids, sums))
+    ext = v["externals"]
+    if n_ext:
+        rng_e = np.random.default_rng([seed, 0x0E1])
+        six = lambda hi, lo=0: ipaddress.IPv6Address((0x20010DB8 << 96) | (hi << 64) | lo).packed
+        more = [(v["asbr"], 0x1000 + q, int(rng_e.integers(1, 40)), 11, rec(six(0xE8_0000 + q)), 64, 0, q % 2, 0)
+                for q in range(n_ext)]
+        ext = _lsa_array(sorted([tuple(z) for z in ext.tolist()] + more, key=lambda z: (z[0], z[1])),
+                         ospf_rib.EXTERNAL6_LSA_DT)
+    sums1 = []
+    for areas, ids, bsums in out_borders:
+        rib_areas = [ospf_rib.RibArea(a.area_id, area_from_planes(a, spf), a.ifaces, s, True)
+                     for a, s in zip(areas, bsums)]
+        sums1 += nonbackbone_lsas(areas[0].router_id, max_paths, rib_areas, ext, ids.index(1))
+    return {"r_area": v["r1_area"], "summaries1": _lsa_array(sorted(sums1, key=lambda z: (z[7], z[0], z[1])),
+                                                             ospf_rib.INTER_AREA_LSA_DT),
+            "externals": ext, "borders": out_borders, "flip": (key[0], key[1], x, y), "shared": v["shared"],
+            "asbr": v["asbr"]}
+
+
+def nonbackbone_lsas(router_id: int, max_paths: int, rib_areas: list, externals, target: int, configs=None) -> list:
+    """What an OSPFv3 border originates into rib_areas[target]: its update_rib_full over rib_areas, then
+    hspf_ospfv3_net_summaries and hspf_ospfv3_rtr_summaries, as INTER_AREA_LSA_DT rows with lsa_id numbered from 1 in
+    output order (Inter-Area-Prefix first)."""
+    from . import ospf_rib
+    cfg = configs if configs is not None else [ospf_rib.area_config()] * len(rib_areas)
+    rib = ospf_rib.update_rib_full_v3(router_id, max_paths, rib_areas, externals)
+    rows = [tuple(z) for z in ospf_rib.net_summaries_v3(router_id, rib, rib_areas, cfg, target).tolist()]
+    rows += [tuple(z) for z in ospf_rib.rtr_summaries_v3(router_id, rib_areas, cfg, target).tolist()]
+    return [(z[0], k + 1) + tuple(z[2:]) for k, z in enumerate(rows)]

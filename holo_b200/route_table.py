@@ -179,7 +179,9 @@ def declare(lib: C.CDLL):
         "hspf_ospfv2_backbone_asbr_delta16": [vp, vp, u32, res16, pvp, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv3_net_summaries": [u32, C.POINTER(ospf_rib.RibStruct), C.POINTER(ospf_rib.RibAreaStruct), vp, u32,
                                       u32, vp, u32, u32p],
+        "hspf_ospfv3_rtr_summaries": [u32, C.POINTER(ospf_rib.RibAreaStruct), vp, u32, u32, vp, u32, u32p],
         "hspf_ospfv3_backbone_table_create": [vp, u32, vp, u32, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv3_nonbackbone_table_create": [vp, u32, vp, vp, u32, vp, u32, pvp, u32, pvp],
         "hspf_ospfv3_backbone_table_prefixes6": [vp, u32p, pvp, C.POINTER(u32p)],
         "hspf_ospfv3_backbone_from_cells": [vp, C.POINTER(ospfv3.AreaStruct), vp, vp, vp, u32,
                                             C.POINTER(ospf_rib.RibStruct)],

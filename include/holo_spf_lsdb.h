@@ -463,10 +463,11 @@ int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_
                                       uint64_t *n_records);
 
 /*
- * Non-backbone router over what-if jobs on the backbone (OSPFv2 only).  The same stage with source and target area
- * swapped: R is an internal router of a non-backbone area A, and a job changes costs in area 0 only.  R's area-A SPT
- * is its unperturbed one; what changes are the type-3 / type-4 LSAs that A's area border routers attached to area 0
- * (the "borders") originate into A, because each border's routes move with the job.  The caller must give every area
+ * Non-backbone router over what-if jobs on the backbone (OSPFv3: hspf_ospfv3_nonbackbone_table_create below).  The
+ * same stage with source and target area swapped: R is an internal router of a non-backbone area A, and a job
+ * changes costs in area 0 only.  R's area-A SPT is its unperturbed one; what changes are the type-3 / type-4 LSAs
+ * that A's area border routers attached to area 0 (the "borders") originate into A, because each border's routes
+ * move with the job.  The caller must give every area
  * border router of A that is attached to area 0 as a border: another one keeps its base LSAs as static records, and
  * the table cannot tell.  The borders' cells of job j come from hspf_ospfv2_abr_rib_cells[16], with each border's
  * area-0 row of the job and row 0 of its other areas.  For job j, with border b's cells decoded to rib_b, the decoded
@@ -529,7 +530,9 @@ int hspf_ospfv2_nonbackbone_table_create(const hspf_ospfv2_flat *flat, uint32_t 
  *   hspf_ospfv3_backbone_table_prefixes6  P, and the IPv6 prefixes / lengths in prefix order (pointers may be NULL);
  *                                HSPF_E_INVAL for an OSPFv2 table.
  *   hspf_ospfv3_backbone_from_cells host: one job's cells -> the table of the contract, a slot winner's prefix options
- *                                read from the winner.  area: R's area-0 image; gathers as hspf_ospfv2_backbone_from_cells.
+ *                                read from the winner.  area: R's image of the table's area (area 0 here, the target
+ *                                area of an hspf_ospfv3_nonbackbone_table_create table); gathers as
+ *                                hspf_ospfv2_backbone_from_cells.
  */
 int hspf_ospfv3_backbone_table_create(const struct hspf_ospfv3_flat *flat, uint32_t router_id,
                                       const hl_ospfv3_inter_area_lsa *summaries, uint32_t n_summaries,
@@ -541,6 +544,44 @@ int hspf_ospfv3_backbone_table_prefixes6(const hspf_ospfv2_backbone_table *t, ui
 int hspf_ospfv3_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const hl_ospfv3_area *area,
                                     const hl_ospf_rib_cell *cells, const uint32_t *gather_v, const uint64_t *gather_nh,
                                     uint32_t n_gather, hl_ospfv3_rib *out);
+
+/*
+ * Non-backbone router over what-if jobs on the backbone, OSPFv3: hspf_ospfv2_nonbackbone_table_create's stage over
+ * Inter-Area-Prefix / Inter-Area-Router LSAs.  R is an internal router of a non-backbone area A, a job changes costs
+ * in area 0 only, and the borders are A's ABRs attached to area 0 (every one of them must be given).  The borders'
+ * cells of job j come from hspf_ospfv3_abr_rib_cells[16], with each border's area-0 row of the job and row 0 of its
+ * other areas.  For job j, with border b's cells decoded to rib_b (hspf_ospfv3_abr_rib_from_cells) over its areas
+ * areas_b, the decoded cells of j equal the affected-prefix routes, prefix options included, of
+ *     hspf_ospfv3_update_rib_full(R, max_paths, [{A, area_from_planes(A, R's row 0), ifaces, S_j, 1}], X)
+ * where S_j is A's Inter-Area-Prefix / Inter-Area-Router LSAs with each border's LSAs replaced by
+ * hspf_ospfv3_net_summaries(rib_b, areas_b, target A) and hspf_ospfv3_rtr_summaries(areas_b, target A), both over
+ * the border's area-0 SPF of the job, in LsaKey order.  A border advertises a route of its cell as the OSPFv2 stage
+ * says (intra-area or inter-area), and its LSA carries the route's prefix options: those of the winning intra-area
+ * record, or of the winning Inter-Area-Prefix record of an inter-area cell (a transit-area record included).  A
+ * slot's winner is n_records + (slot index << 8 | those options), so a border route whose winning LSA changes at an
+ * equal metric, to one with other options, shows as OTHER in the route-delta stage.  Inter-Area-Router slots are the
+ * OSPFv2 stage's type-4 slots: one per (border, area other than A where the ASBR is an E-flag router), an area-0
+ * ASBR's read from the border's area-0 row of the job.  The affected prefixes and the stub-area rules are those of
+ * the OSPFv2 stage, the stub default route being ::/0.
+ *
+ *   hspf_ospfv3_nonbackbone_table_create  host.  flat: R's OSPFv3 area-A flat (A is flat's area id); config: A's
+ *                                configuration; summaries: A's Inter-Area-Prefix / Inter-Area-Router LSAs in LsaKey
+ *                                order; externals: the AS-external LSAs; borders: the borders' OSPFv3 ABR tables.  The
+ *                                result is an hspf_ospfv2_backbone_table marked OSPFv3 and with its target area A; the
+ *                                cells and delta calls of both kinds take it (a table with Inter-Area-Router slots is
+ *                                the asbr calls', as for OSPFv2), and hspf_ospfv3_backbone_from_cells decodes it over
+ *                                R's image of A.  The asbr calls still refuse an OSPFv3 table of area 0.  Refusals:
+ *                                those of hspf_ospfv2_nonbackbone_table_create, over Inter-Area-Prefix /
+ *                                Inter-Area-Router LSAs, with an OSPFv2 border table HSPF_E_INVAL and slot winners that
+ *                                would not fit 32 bits HSPF_E_UNSUPPORTED.  Inter-Area-Prefix LSAs with the NU option
+ *                                are left out.
+ */
+int hspf_ospfv3_nonbackbone_table_create(const struct hspf_ospfv3_flat *flat, uint32_t router_id,
+                                         const struct hl_ospf_area_config *config,
+                                         const hl_ospfv3_inter_area_lsa *summaries, uint32_t n_summaries,
+                                         const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
+                                         const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                         hspf_ospfv2_backbone_table **out);
 
 /*
  * The stages of update_rib_full that follow the per-area SPFs (holo-ospf/src/route.rs:146-193):
@@ -592,12 +633,26 @@ int hspf_ospfv2_net_summaries(uint32_t router_id, const hl_ospfv2_rib *rib, cons
  * lsa_orig_inter_area_network of holo-ospf ospfv3/lsdb.rs:341-386), over hspf_ospfv3_update_rib_full's table: the
  * type-3 rules of hspf_ospfv2_net_summaries, each LSA carrying its route's prefix options (the default route of a stub
  * area: ::/0 at default_cost, options 0).  out[0, *n_out): lsa_type 3, adv_rtr = router_id, lsa_id 0, the prefix, its
- * length, prefix options and metric, in prefix order.  Inter-Area-Router contents are not computed.  HSPF_E_NOMEM
- * with *n_out set when cap is too small.  Host only.
+ * length, prefix options and metric, in prefix order.  Inter-Area-Router contents: hspf_ospfv3_rtr_summaries.
+ * HSPF_E_NOMEM with *n_out set when cap is too small.  Host only.
  */
 int hspf_ospfv3_net_summaries(uint32_t router_id, const hl_ospfv3_rib *rib, const hl_ospfv3_rib_area *areas,
                               const hl_ospf_area_config *config, uint32_t n_areas, uint32_t target,
                               hl_ospfv3_inter_area_lsa *out, uint32_t cap, uint32_t *n_out);
+/*
+ * The Inter-Area-Router contents an OSPFv3 area border router originates into one target area (compute_rtr_summaries,
+ * holo-ospf area.rs:699-740), over the router entries hspf_ospfv3_update_rib_full leaves for the same `areas` (each
+ * area's SPF routers as intra-area entries, then inter-area entries from the Inter-Area-Router LSAs it reads: area 0's
+ * when more than one area is active).  The type-4 rule of hspf_ospfv2_net_summaries: only into a normal area, each
+ * entry of another area with the E flag below LSInfinity, intra-area ones only into the backbone, none with a next
+ * hop on one of the target area's interfaces, an id in two areas keeping the later area's entry.  out[0, *n_out):
+ * lsa_type 4, adv_rtr = router_id, router_id = the ASBR, metric, lsa_id 0, in router-id order.  Nothing when at most
+ * one area is active.  The LSA's options are out of the contract: hl_ospfv3_inter_area_lsa has no field for them,
+ * and update_rib_full does not read them.  HSPF_E_NOMEM with *n_out set when cap is too small.  Host only.
+ */
+int hspf_ospfv3_rtr_summaries(uint32_t router_id, const hl_ospfv3_rib_area *areas, const hl_ospf_area_config *config,
+                              uint32_t n_areas, uint32_t target, hl_ospfv3_inter_area_lsa *out, uint32_t cap,
+                              uint32_t *n_out);
 
 /*
  * update_global_rib (holo-ospf/src/route.rs:833-893): compares the freshly computed table with
