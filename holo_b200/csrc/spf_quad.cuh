@@ -451,6 +451,12 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
         }
         HSPF_QMARK(1);   // SSSP
 
+        // Slot -> vertex map of phase 2, in the ring (dead after the SSSP): the vertex of the first slot
+        // of every bitmap word.  Chains never straddle a word and dummy quads only pad a word's tail,
+        // so the vertex whose chain starts at slot s is vbase[s >> 5] plus the chain starts below s in
+        // its word (~cont bits): a shared lookup instead of a dependent L2 load of vert_of.
+        uint16_t *vbase = reinterpret_cast<uint16_t *>(ring);
+        for (uint32_t w = tid; w < NBW; w += T) vbase[w] = __ldg(&Q.vert_of[w << 5]);
         // hops-0 non-HOP heads of root edges (their out-edges carry first-hop atoms)
         if (tid < S.n_roottab) {
             const uint32_t h = S.rt_target[tid], c = S.rt_cost[tid];
@@ -541,7 +547,8 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
                     if (dv >= U) dv = kInf;                                   // unreached
                     if (v == root || dv == kInf) { cnt = 0; bs = kInf; }
                     if (dv != kInf && g.saturate_at && dv >= g.saturate_at) sat_flag = 1;
-                    const uint32_t fpv = cnt ? (uint32_t)__ldg(&Q.vert_of[bs]) : kInf;
+                    // (bs: the first slot of the parent's chain)
+                    const uint32_t fpv = cnt ? vbase[bs >> 5] + __popc(~cont_s[bs >> 5] & ((1u << (bs & 31)) - 1u)) : kInf;
                     if (narrow) {
                         if (dv != kInf && dv >= 0xFFFFu) narrow_flag = 1;      // does not fit; 0xFFFF means "not on the SPT"
                         o_dist16[v] = (uint16_t)min(dv, 0xFFFFu);
@@ -555,23 +562,42 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
                     if (cnt >= 2) atomicOr(&ecmpbm[v >> 5], 1u << (v & 31));
                 }
             };
-            // two in-quads of a thread in flight (NIQ % 32 == 0: a warp is in range as a whole)
+            // NIQ % 32 == 0: a warp is in range as a whole
             const uint32_t wbase = tid & ~31u;
-            for (uint32_t i0 = 0; i0 + wbase < NIQ; i0 += 2 * T) {
-                const uint32_t ia = i0 + tid, ib = ia + T;
-                const bool hb = i0 + T + wbase < NIQ;                          // warp-uniform
-                const uint2 ma = __ldg(&Q.imeta[ia]);
-                const uint4 ra = __ldg(&Q.iq[ia]);
-                uint2 mb = make_uint2(0xFFFFFFFFu, 0u);
-                uint4 rb = make_uint4(0u, 0u, 0u, 0u);
-                if (hb) { mb = __ldg(&Q.imeta[ib]); rb = __ldg(&Q.iq[ib]); }
-                uint32_t dva, ca, bda, bsa, dvb = kInf, cb = 0, bdb = kInf, bsb = kInf;
-                pull(ia, ma, ra, dva, ca, bda, bsa);
-                if (hb) pull(ib, mb, rb, dvb, cb, bdb, bsb);
-                combine(ma.y & 0xFFu, ca, bda, bsa);
-                if (hb) combine(mb.y & 0xFFu, cb, bdb, bsb);
-                emit_v(ma, dva, ca, bsa);
-                if (hb) emit_v(mb, dvb, cb, bsb);
+            if constexpr (!kOv) {
+                // one in-quad of a thread per iteration, the next one's loads issued before this one's
+                // chain combine and stores
+                uint2 nm = make_uint2(0xFFFFFFFFu, 0u);
+                uint4 nr = make_uint4(0u, 0u, 0u, 0u);
+                if (wbase < NIQ) { nm = __ldg(&Q.imeta[tid]); nr = __ldg(&Q.iq[tid]); }
+                for (uint32_t i = tid; i - lane < NIQ; i += T) {
+                    const uint2 m = nm;
+                    uint32_t dv, cnt, bd, bs;
+                    pull(i, m, nr, dv, cnt, bd, bs);
+                    if (i + T - lane < NIQ) { nm = __ldg(&Q.imeta[i + T]); nr = __ldg(&Q.iq[i + T]); }
+                    combine(m.y & 0xFFu, cnt, bd, bs);
+                    emit_v(m, dv, cnt, bs);
+                }
+            } else {
+                // With overrides the prefetch does not fit 40 registers at 512 threads (ptxas moves the
+                // override patch's record arrays, the SSSP's included, to local memory): two in-quads of
+                // a thread in flight instead.
+                for (uint32_t i0 = 0; i0 + wbase < NIQ; i0 += 2 * T) {
+                    const uint32_t ia = i0 + tid, ib = ia + T;
+                    const bool hb = i0 + T + wbase < NIQ;                          // warp-uniform
+                    const uint2 ma = __ldg(&Q.imeta[ia]);
+                    const uint4 ra = __ldg(&Q.iq[ia]);
+                    uint2 mb = make_uint2(0xFFFFFFFFu, 0u);
+                    uint4 rb = make_uint4(0u, 0u, 0u, 0u);
+                    if (hb) { mb = __ldg(&Q.imeta[ib]); rb = __ldg(&Q.iq[ib]); }
+                    uint32_t dva, ca, bda, bsa, dvb = kInf, cb = 0, bdb = kInf, bsb = kInf;
+                    pull(ia, ma, ra, dva, ca, bda, bsa);
+                    if (hb) pull(ib, mb, rb, dvb, cb, bdb, bsb);
+                    combine(ma.y & 0xFFu, ca, bda, bsa);
+                    if (hb) combine(mb.y & 0xFFu, cb, bdb, bsb);
+                    emit_v(ma, dva, ca, bsa);
+                    if (hb) emit_v(mb, dvb, cb, bsb);
+                }
             }
             if (sat_flag) atomicOr(&S.status, kJsSaturated);
             if (narrow_flag) atomicOr(&S.status, kJsNarrow);
@@ -654,10 +680,17 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
             // two-pass code.
             const uint32_t na = n_atoms;
             uint32_t ovf = 0;
-            for (uint32_t v = tid; v < Vp; v += T) {
-                uint32_t A = v, h = 0;
-                if (v < V && !is_ecmp(v)) {
-                    const uint32_t f = ld_fp(v);
+            for (uint32_t v0 = tid; v0 < Vp; v0 += 4 * T) {      // four first-parent loads in flight
+                uint32_t fk[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint32_t v = v0 + k * T;
+                    fk[k] = (v < V && !is_ecmp(v)) ? ld_fp(v) : kInf;
+                }
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint32_t v = v0 + k * T, f = fk[k];
+                    uint32_t A = v, h = 0;
                     if (f != kInf) {
                         h = is_hop(v) ? 1u : 0u;
                         A = f;
@@ -665,13 +698,13 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
                             // cut: anc = root, but the hops of a hops-0 parent other than the root need
                             // not be 0 (a HOP vertex at distance 0 above it): walk its first parents
                             A = root;
-                            for (uint32_t u = f, k = 0; u != root && u < V && k < V; u = ld_fp(u), ++k)
+                            for (uint32_t u = f, n = 0; u != root && u < V && n < V; u = ld_fp(u), ++n)
                                 h += is_hop(u) ? 1u : 0u;
                         }
                     }
+                    ovf |= h << na;
+                    word[v] = (A << 16) | ((h << na) & 0xFFFFu);
                 }
-                ovf |= h << na;
-                word[v] = (A << 16) | ((h << na) & 0xFFFFu);
             }
             if (tid < 16u) S.seed_of[tid] = (uint16_t)min(seed_v, 0xFFFFu);
             if (tid == 0) S.mbad = 0;
@@ -780,9 +813,15 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
             __syncthreads();
         } else {
             // -- hops: sum of HOP flags over (root, v]; the root and unreached vertices are terminals
-            for (uint32_t v = tid; v < Vp; v += T) {      // (padding words are terminals: no bounds checks in the rounds)
-                const uint32_t f = (v < V) ? ld_fp(v) : kInf;
-                word[v] = (f == kInf) ? (v << 16) : ((f << 16) | (is_hop(v) ? 1u : 0u));
+            for (uint32_t v0 = tid; v0 < Vp; v0 += 4 * T) {      // (padding words are terminals: no bounds checks in the rounds)
+                uint32_t fk[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) fk[k] = (v0 + k * T < V) ? ld_fp(v0 + k * T) : kInf;
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const uint32_t v = v0 + k * T;
+                    word[v] = (fk[k] == kInf) ? (v << 16) : ((fk[k] << 16) | (is_hop(v) ? 1u : 0u));
+                }
             }
             __syncthreads();
             uint32_t jump_rounds = 0;     // rounds in which some vertex still moved
@@ -827,13 +866,16 @@ __global__ void __launch_bounds__(T, 3) spf_quad_kernel(const QuadArgs a) {
             // and every vertex adds the final set of its top.  16 atoms per pass.
             for (uint32_t pass = 0; pass * 16u < n_atoms || pass == 0; ++pass) {
                 // terminals (the root, unreached vertices, ECMP vertices) point at themselves
-                for (uint32_t v = tid; v < Vp; v += T) {
-                    uint32_t A = v;
-                    if (v < V) {
-                        const uint32_t f = ld_fp(v);
-                        if (f != kInf && !is_ecmp(v)) A = hops0(f) ? root : f;
+                for (uint32_t v0 = tid; v0 < Vp; v0 += 4 * T) {
+                    uint32_t fk[4];
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) fk[k] = (v0 + k * T < V) ? ld_fp(v0 + k * T) : kInf;
+#pragma unroll
+                    for (int k = 0; k < 4; ++k) {
+                        const uint32_t v = v0 + k * T, f = fk[k];
+                        const uint32_t A = (f != kInf && !is_ecmp(v)) ? (hops0(f) ? root : f) : v;
+                        word[v] = A << 16;
                     }
-                    word[v] = A << 16;
                 }
                 __syncthreads();
                 if (seed_v != kInf && (tid >> 4) == pass) atomicOr(&word[seed_v], 1u << (tid & 15));
