@@ -253,6 +253,9 @@ struct hspf_ospfv2_backbone_table {
     // in the border's table); a table with type-4 slots is read only by the asbr calls
     uint32_t n_asbr_slots = 0;
     std::vector<std::pair<uint32_t, uint32_t>> asbr_set;
+    // made by a create that re-originates the borders' type-4 / Inter-Area-Router LSAs per job (the asbr and
+    // nonbackbone creates): the asbr calls take an OSPFv3 table of area 0 only with this mark
+    bool asbr = false;
     // OSPFv3 tables (hspf_ospfv3_backbone_table_create): `prefix` is zero-filled (the prefixes are prefix6), and
     // options6 holds the prefix options of each type-3 / type-5 record of the view (index - o3[0]); a slot's entry is
     // a placeholder, its options come from its winner

@@ -352,8 +352,9 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
 // over area 0 without the borders' type-3 LSAs, and per affected prefix R's intra-area records, its static type-3
 // records with one slot per (border, prefix) at the border's place in LsaKey order, and its type-5 records
 // (ospf_backbone_cells.h).  Border tables of the other version are refused (HSPF_E_INVAL).  `asbr`
-// (hspf_ospfv2_backbone_asbr_table_create): the borders' type-4 LSAs are re-originated per job too, as type-4 slots,
-// and the prefixes of the type-5 LSAs they lead to are affected; else a usable one is HSPF_E_UNSUPPORTED.
+// (hspf_ospfv{2,3}_backbone_asbr_table_create): the borders' type-4 / Inter-Area-Router LSAs are re-originated per job
+// too, as type-4 slots, and the prefixes of the type-5 LSAs they lead to are affected; else a usable one is
+// HSPF_E_UNSUPPORTED.  The table keeps the flag (hspf_ospfv2_backbone_table::asbr).
 // `config` (hspf_ospfv{2,3}_nonbackbone_table_create): R is an internal router of the non-backbone area of `flat` with
 // that configuration, the target area A.  The borders re-originate into A their intra-area routes of their other
 // areas and their inter-area routes, and type-4 / Inter-Area-Router LSAs for the ASBRs they reach intra-area outside A
@@ -389,7 +390,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         const uint32_t root = vertex(router_id);
         if (root == kNone || (flags(root) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
         t->router_id = router_id; t->root = root; t->n_vertices = T::n_vertices(f);
-        t->max_paths = f.area->max_paths; t->n_borders = n_borders; t->v3 = T::kV3; t->area_id = ta;
+        t->max_paths = f.area->max_paths; t->n_borders = n_borders; t->v3 = T::kV3; t->area_id = ta; t->asbr = asbr;
         // per border: its area-0 index, its target-area index, its vertex
         std::vector<uint32_t> a0(n_borders), at(n_borders), bv(n_borders);
         std::unordered_map<uint32_t, uint32_t> border_of;           // router id -> border

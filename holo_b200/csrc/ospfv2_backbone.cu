@@ -93,12 +93,27 @@ struct OspfNonBackboneV3Cell : OspfBackboneAsbrCell<Planes> {
     }
 };
 
+// The walk over an OSPFv3 table of area 0 with Inter-Area-Router slots (hspf_ospfv3_backbone_asbr_table_create): slot
+// winners carry prefix options.  A type of its own, so that the kernels above keep their instantiations.
+template <class Planes>
+struct OspfBackboneAsbrV3Cell : OspfBackboneAsbrCell<Planes> {
+    using Base = OspfBackboneCell<Planes, false>;
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
+        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {this->sets, j}};
+        return hspf::ospf_backbone_cell_eval<true, true, false>(pl, this->t, p, rows);
+    }
+};
+
 // Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
-// and for OSPFv3 tables, for OSPFv2 tables with type-4 slots, and for OSPFv2 and OSPFv3 tables of a non-backbone
-// target area.
+// and for OSPFv3 tables, for OSPFv2 and OSPFv3 tables with type-4 / Inter-Area-Router slots, and for OSPFv2 and
+// OSPFv3 tables of a non-backbone target area.
 constexpr uint32_t kBackboneBlocksPerSM = 4;
 constexpr uint32_t kBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kBackboneAsbrBlocksPerSM = 4;
+constexpr uint32_t kBackboneAsbrV3BlocksPerSM = 4;
 constexpr uint32_t kNonBackboneBlocksPerSM = 4;
 constexpr uint32_t kNonBackboneV3BlocksPerSM = 4;
 
@@ -145,14 +160,14 @@ int version_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n
 }
 
 // The cell over a table with type-4 slots: the plane sets the slots name, from each border's planes, row counts and
-// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when it names none.  Of OSPFv3
-// tables only those of a non-backbone target area have such slots (Inter-Area-Router slots).
+// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when it names none.  An OSPFv3
+// table of area 0 is taken only from hspf_ospfv3_backbone_asbr_table_create (Inter-Area-Router slots).
 template <class R>
 int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
                    const uint32_t *const *border_status, const R *const *border_planes,
                    const uint32_t *const *border_n_rows, const uint32_t *const *border_rows, uint32_t n_jobs,
                    OspfBackboneAsbrCell<hspf::PlanesOf<R>> &cell) {
-    if (!t || (t->v3 && !t->area_id)) return HSPF_E_INVAL;
+    if (!t || (t->v3 && !t->area_id && !t->asbr)) return HSPF_E_INVAL;
     if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
     auto &s = cell.sets;
     s.n = (uint32_t)t->asbr_set.size();
@@ -170,11 +185,12 @@ int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const h
     return HSPF_OK;
 }
 
+// The launch of a walk over a table with type-4 / Inter-Area-Router slots or of a non-backbone target area (Cell).
 template <class Cell, uint32_t kBlocks, class R>
-int nonbackbone_cells_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                         const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                         const R *const *border_planes, const uint32_t *const *border_n_rows,
-                         const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+int asbr_cells_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   const R *const *border_planes, const uint32_t *const *border_n_rows,
+                   const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
     Cell cell{};
     if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                                       n_jobs, cell))
@@ -184,12 +200,12 @@ int nonbackbone_cells_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uin
 }
 
 template <class Cell, uint32_t kBlocks, class R>
-int nonbackbone_delta_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                         const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                         const R *const *border_planes, const uint32_t *const *border_n_rows,
-                         const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
-                         const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
-                         uint64_t *n_records) {
+int asbr_delta_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                   const R *const *border_planes, const uint32_t *const *border_n_rows,
+                   const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                   const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                   uint64_t *n_records) {
     Cell cell{};
     if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                                       n_jobs, cell))
@@ -205,10 +221,10 @@ int nonbackbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32
                       const R *const *border_planes, const uint32_t *const *border_n_rows,
                       const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
     using P = hspf::PlanesOf<R>;
-    return t->v3 ? nonbackbone_cells_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
+    return t->v3 ? asbr_cells_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
                        ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                        job_status_out, cells)
-                 : nonbackbone_cells_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
+                 : asbr_cells_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
                        ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                        job_status_out, cells);
 }
@@ -221,10 +237,10 @@ int nonbackbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32
                       const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                       uint64_t *n_records) {
     using P = hspf::PlanesOf<R>;
-    return t->v3 ? nonbackbone_delta_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
+    return t->v3 ? asbr_delta_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
                        ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                        base_cells, n_base, base_of, job_out, records, cap, n_records)
-                 : nonbackbone_delta_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
+                 : asbr_delta_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
                        ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                        base_cells, n_base, base_of, job_out, records, cap, n_records);
 }
@@ -258,17 +274,21 @@ int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t 
 }
 
 // A table without type-4 slots takes the calls above (NULL border planes allowed).  An OSPFv3 table of area 0 is
-// refused.
+// refused unless hspf_ospfv3_backbone_asbr_table_create made it.
 template <class R>
 int backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
                         const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                         const R *const *border_planes, const uint32_t *const *border_n_rows,
                         const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    if (!t || (t->v3 && !t->area_id)) return HSPF_E_INVAL;
+    if (!t || (t->v3 && !t->area_id && !t->asbr)) return HSPF_E_INVAL;
     if (t->area_id)
         return nonbackbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
                                  border_rows, job_status_out, cells);
     if (!t->n_asbr_slots) return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+    if (t->v3)
+        return asbr_cells_as<OspfBackboneAsbrV3Cell<hspf::PlanesOf<R>>, kBackboneAsbrV3BlocksPerSM>(
+            ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+            job_status_out, cells);
     OspfBackboneAsbrCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                                       n_jobs, cell))
@@ -284,13 +304,17 @@ int backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint
                         const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
                         const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                         uint64_t *n_records) {
-    if (!t || (t->v3 && !t->area_id)) return HSPF_E_INVAL;
+    if (!t || (t->v3 && !t->area_id && !t->asbr)) return HSPF_E_INVAL;
     if (t->area_id)
         return nonbackbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
                                  border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
     if (!t->n_asbr_slots)
         return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
                               records, cap, n_records);
+    if (t->v3)
+        return asbr_delta_as<OspfBackboneAsbrV3Cell<hspf::PlanesOf<R>>, kBackboneAsbrV3BlocksPerSM>(
+            ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, base_cells,
+            n_base, base_of, job_out, records, cap, n_records);
     OspfBackboneAsbrCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                                       n_jobs, cell))

@@ -907,6 +907,14 @@ int hspf_ospfv3_backbone_table_create(const hspf_ospfv3_flat *flat, uint32_t rou
     return hspf::build_backbone_table<RibV3>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out);
 }
 
+int hspf_ospfv3_backbone_asbr_table_create(const hspf_ospfv3_flat *flat, uint32_t router_id,
+                                           const hl_ospfv3_inter_area_lsa *sums, uint32_t n_sums,
+                                           const hl_ospfv3_external_lsa *ext, uint32_t n_ext,
+                                           const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                           hspf_ospfv2_backbone_table **out) {
+    return hspf::build_backbone_table<RibV3>(flat, router_id, sums, n_sums, ext, n_ext, borders, n_borders, out, true);
+}
+
 int hspf_ospfv3_nonbackbone_table_create(const hspf_ospfv3_flat *flat, uint32_t router_id,
                                          const hl_ospf_area_config *config, const hl_ospfv3_inter_area_lsa *sums,
                                          uint32_t n_sums, const hl_ospfv3_external_lsa *ext, uint32_t n_ext,

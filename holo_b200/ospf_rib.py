@@ -647,9 +647,11 @@ class BackboneTable:
     EXTERNAL6_LSA_DT, borders: OSPFv3 AbrRibTables); `prefix` and `prefixes6` then hold the IPv6 prefixes
     (ospfv3.IP_DT), `v3` is set, and a slot's winner is n_records + (slot index << 8 | its prefix options).
 
-    asbr=True (OSPFv2): hspf_ospfv2_backbone_asbr_table_create, which re-originates the borders' type-4 LSAs per job
+    asbr=True: hspf_ospfv2_backbone_asbr_table_create (from an OSPFv3 area-0 flat without `config`:
+    hspf_ospfv3_backbone_asbr_table_create), which re-originates the borders' type-4 / Inter-Area-Router LSAs per job
     too; `n_asbr_slots` type-4 slots read `n_asbr_sets` (border, area) plane sets, and a table with type-4 slots is
-    read by backbone_asbr_cells_device / backbone_asbr_delta_device only.
+    read by backbone_asbr_cells_device / backbone_asbr_delta_device only.  An OSPFv3 table of area 0 made without
+    asbr=True is refused by those two.
 
     config=area_config(...): hspf_ospfv2_nonbackbone_table_create (from an ospfv3.Flat:
     hspf_ospfv3_nonbackbone_table_create), the table of an internal router R of the non-backbone area of `flat` (the
@@ -664,8 +666,8 @@ class BackboneTable:
         self.lib = capi.load_library()
         self.flat, self.router_id, self.borders = flat, router_id, list(borders)
         self.v3 = isinstance(flat, ospfv3.Flat)
-        if asbr and self.v3:
-            raise ValueError("type-4 slots are OSPFv2 only")
+        if asbr and self.v3 and (config is not None or int(flat.area.area_id) != 0):
+            raise ValueError("asbr=True takes an OSPFv3 flat of area 0 and no config")
         sum_dt, ext_dt = (INTER_AREA_LSA_DT, EXTERNAL6_LSA_DT) if self.v3 else (SUMMARY_LSA_DT, EXTERNAL_LSA_DT)
         sm = np.ascontiguousarray(summaries if summaries is not None else np.zeros(0, sum_dt), sum_dt)
         ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, ext_dt), ext_dt)
@@ -674,6 +676,7 @@ class BackboneTable:
         h = C.c_void_p()
         self.area_id = int(flat.area.area_id) if config is not None else 0
         create = ("hspf_ospfv3_nonbackbone_table_create" if self.v3 and config is not None else
+                  "hspf_ospfv3_backbone_asbr_table_create" if self.v3 and asbr else
                   "hspf_ospfv3_backbone_table_create" if self.v3 else
                   "hspf_ospfv2_nonbackbone_table_create" if config is not None else
                   "hspf_ospfv2_backbone_asbr_table_create" if asbr else "hspf_ospfv2_backbone_table_create")
@@ -759,10 +762,11 @@ def _border_plane_args(border_planes, border_n_rows, border_rows, keep: list):
 
 def backbone_asbr_cells_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
                                border_planes, border_n_rows, border_rows, status_ptr: int, cells_ptr: int):
-    """hspf_ospfv2_backbone_asbr_cells / _cells16: backbone_cells_device over a table with type-4 slots, plus per
-    border its DEVICE planes (one capi.ResultStruct / Result16Struct per area, as given abr_rib_cells_device, of R's
-    width), its row counts per area, and a device pointer to its rows u32 [n_jobs, n_areas].  The three may be None
-    for a table without type-4 slots."""
+    """hspf_ospfv2_backbone_asbr_cells / _cells16: backbone_cells_device over a table with type-4 / Inter-Area-Router
+    slots (either version; an OSPFv3 table of area 0 from BackboneTable(..., asbr=True) only), plus per border its
+    DEVICE planes (one capi.ResultStruct / Result16Struct per area, as given abr_rib_cells_device, of R's width), its
+    row counts per area, and a device pointer to its rows u32 [n_jobs, n_areas].  The three may be None for a table
+    without type-4 slots."""
     keep = []
     st = _device_ptrs(border_status) if border_status is not None else None
     bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)

@@ -650,7 +650,8 @@ def abr_view(topos: list, seed: int, area_ids=None, roots=None, max_paths: int =
 
 
 def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1, 0), (2, 1), (3, 2)),
-                  max_paths: int = 16, n_ext_keys: int = 3, t2: Topology | None = None, r1: int | None = None):
+                  max_paths: int = 16, n_ext_keys: int = 3, t2: Topology | None = None, r1: int | None = None,
+                  area1_asbrs: int = 0, area1_ext: int = 4):
     """The OSPFv3 twin of ospfv2.backbone_view: a backbone router R of area 0 and the area border routers ("borders")
     of one other area 1, each as its own image.  Seeded.  Area 0 is synth_area(t0) (router i is RID_BASE + i), area 1
     synth_area(t1) with router ids, prefixes and interface sort keys in ranges of its own, except that border (i0, i1)
@@ -670,7 +671,17 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
                     the other record at the same metric, with other options;
       shared        (address bytes, length) of a /64 that is intra-area in area 1 (LA) and area 2 (P) at metrics that
                     tie at the first border (its route there keeps area 1's options, the first of its areas);
-      r1_area       with r1: the area-1 image of router r1 of t1, with area 1's prefixes as the borders see them."""
+      r1_area       with r1: the area-1 image of router r1 of t1, with area 1's prefixes as the borders see them.
+    area1_asbrs = k > 0 (drawn from a generator of its own, so that every other part is as without it): k routers of
+    area 1 get the E flag ("area1_asbrs" in the dict) and area1_ext AS-external /64s each, both E-bit values and a mix
+    of prefix options, on prefixes the next ASBR shares in half, plus the area-0 ASBR's own /64 at one below its
+    type-2 metric (so an area-1 ASBR's LSA wins it while R reaches one).
+    summaries0 then also holds each border's Inter-Area-Router LSAs for those it reaches in area 1, at that distance
+    (what hspf_ospfv3_rtr_summaries gives in the base job), numbered after its Inter-Area-Prefix LSAs.  With k >= 2,
+    "flip_ext" is (address bytes, length, x1, x2) of a /64 that the first two ASBRs advertise as type-1, x1 with the LA
+    and x2 with the P option, at costs that tie through the last border: R's route takes x1's LSA, and a job that cuts
+    x1 off alone hands it to x2's at the same metric, with other options.  A border left out of a backbone table keeps
+    its LSAs as another ABR's static ones."""
     from . import ospf_rib, synth
     from .ospfv2 import _dist_from
     rng = np.random.default_rng(seed)
@@ -734,6 +745,16 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
     a1s = [_with_prefixes(a, adds1) for a in a1s]
     a2 = _with_prefixes(a2, adds2)
     r1_area = _with_prefixes(image(t1, 1, r1, b1map), adds1) if r1 is not None else None
+    asbrs1 = []
+    if area1_asbrs:
+        rng1 = np.random.default_rng([seed, 0x3A5B])
+        cand1 = sorted({int(x["adv_rtr"]) for x in a1s[0].router_lsas} - set(bids))
+        asbrs1 = sorted(cand1[int(i)] for i in rng1.choice(len(cand1), min(area1_asbrs, len(cand1)), replace=False))
+        for a in a1s + ([r1_area] if r1_area is not None else []):
+            rl = a.router_lsas.copy()
+            for x in asbrs1:
+                rl["flags"][rl["adv_rtr"] == x] |= 0x02
+            a.router_lsas = rl
     # each border's Inter-Area-Prefix LSAs into area 0: its other areas' prefixes that are not area 0's
     own0 = {(bytes(int(b) for b in p["addr"]["bytes"]), int(p["len"])) for p in r_area.prefixes}
     sums0 = []
@@ -754,6 +775,15 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
                     best[key] = (m, int(p["options"]))
         for n, (key, (m, opt)) in enumerate(sorted(best.items())):
             sums0.append((bid, n + 1, m, 0, rec(key[0]), key[1], opt, 3, 0))
+    # each border's Inter-Area-Router LSAs into area 0: the area-1 ASBRs it reaches, at that distance
+    n_iap = {bid: sum(1 for x in sums0 if x[0] == bid) for bid in bids}
+    d_last = {}
+    for bid, a in zip(bids, a1s) if asbrs1 else ():
+        d = dists(a)
+        reach = [x for x in asbrs1 if x in d]
+        sums0 += [(bid, n_iap[bid] + k + 1, d[x], x, ((0,) * 16, 0, (0, 0, 0)), 0, 0, 4, 0) for k, x in enumerate(reach)]
+        if bid == max(bids):
+            d_last = d
     sums0.sort(key=lambda x: (x[7], x[0], x[1]))
     summaries0 = np.zeros(len(sums0), ospf_rib.INTER_AREA_LSA_DT)
     for i, x in enumerate(sums0):
@@ -764,6 +794,19 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
     ext = [(asbr, j + 1, int(rng.choice([5, 30])), 7, rec(k[0]), k[1], PFX_P if j == 1 else 0, int(j % 2), 0)
            for j, k in enumerate(keys)]
     ext.append((asbr, len(keys) + 1, 12, 8, rec(six(0xE0_0000)), 64, 0, 1, 0))
+    opts = (0, PFX_P, PFX_LA, PFX_LA | PFX_P)
+    for m, x in enumerate(asbrs1):
+        ext.append((x, 1, 11, 9, rec(six(0xE0_0000)), 64, 0, 1, 0))
+        for q in range(area1_ext):
+            ext.append((x, q + 2, int(rng1.integers(1, 40)), 10 + m, rec(six(0xE9_0000 + m * area1_ext // 2 + q)), 64,
+                        opts[int(rng1.integers(0, len(opts)))], (q + m) % 2, 0))
+    flip_ext = None
+    if len(asbrs1) >= 2 and all(x in d_last for x in asbrs1[:2]):
+        x1, x2 = asbrs1[:2]
+        M = max(d_last[x1], d_last[x2]) + 5
+        flip_ext = (six(0xEA_0000), 64, x1, x2)
+        ext += [(x1, area1_ext + 2, M - d_last[x1], 11, rec(flip_ext[0]), 64, PFX_LA, 0, 0),
+                (x2, area1_ext + 2, M - d_last[x2], 11, rec(flip_ext[0]), 64, PFX_P, 0, 0)]
     externals = np.zeros(len(ext), ospf_rib.EXTERNAL6_LSA_DT)
     for i, x in enumerate(sorted(ext, key=lambda x: (x[0], x[1]))):
         externals[i] = x
@@ -777,6 +820,8 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
             out_borders.append(([a0, a1], [0, 1], [s0, empty]))
     out = {"r_area": r_area, "summaries0": summaries0, "externals": externals, "borders": out_borders,
            "flip": flip, "shared": shared, "asbr": asbr}
+    if area1_asbrs:
+        out["area1_asbrs"], out["flip_ext"] = asbrs1, flip_ext
     if r1 is not None:
         out["r1_area"] = r1_area
     return out

@@ -181,6 +181,7 @@ def declare(lib: C.CDLL):
                                       u32, vp, u32, u32p],
         "hspf_ospfv3_rtr_summaries": [u32, C.POINTER(ospf_rib.RibAreaStruct), vp, u32, u32, vp, u32, u32p],
         "hspf_ospfv3_backbone_table_create": [vp, u32, vp, u32, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv3_backbone_asbr_table_create": [vp, u32, vp, u32, vp, u32, pvp, u32, pvp],
         "hspf_ospfv3_nonbackbone_table_create": [vp, u32, vp, vp, u32, vp, u32, pvp, u32, pvp],
         "hspf_ospfv3_backbone_table_prefixes6": [vp, u32p, pvp, C.POINTER(u32p)],
         "hspf_ospfv3_backbone_from_cells": [vp, C.POINTER(ospfv3.AreaStruct), vp, vp, vp, u32,

@@ -399,7 +399,8 @@ int hspf_ospfv2_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
                                     uint32_t n_gather, hl_ospfv2_rib *out);
 
 /*
- * The same stage with the borders' type-4 LSAs re-originated per job (OSPFv2 only): a border originates one into
+ * The same stage with the borders' type-4 LSAs re-originated per job (OSPFv3: hspf_ospfv3_backbone_asbr_table_create
+ * below): a border originates one into
  * area 0 for router A (an ASBR) when A is a router with the E flag in one of its non-backbone areas that it reaches,
  * below LSInfinity, in the job; its metric is that distance (hspf_ospfv2_net_summaries' type-4 rule; an id in two such
  * areas keeps the later area's).  For job j the decoded cells equal the affected-prefix routes of the update_rib_full
@@ -546,6 +547,45 @@ int hspf_ospfv3_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
                                     uint32_t n_gather, hl_ospfv3_rib *out);
 
 /*
+ * The same OSPFv3 stage with the borders' Inter-Area-Router LSAs re-originated per job: a border originates one into
+ * area 0 for router A (an ASBR) when A is a router with the E flag in one of its non-backbone areas that it reaches,
+ * below LSInfinity, in the job; its metric is that distance (hspf_ospfv3_rtr_summaries' rule; an id in two such areas
+ * keeps the later area's).  For job j, with border b's cells decoded to rib_b over its areas areas_b, the decoded
+ * cells of j equal the affected-prefix routes, prefix options included, of the hspf_ospfv3_update_rib_full above,
+ * with S_j holding each border's Inter-Area-Prefix LSAs from hspf_ospfv3_net_summaries(rib_b, areas_b, target area 0)
+ * AND its Inter-Area-Router LSAs from hspf_ospfv3_rtr_summaries(areas_b, target area 0), in LsaKey order.  R's entry
+ * for A is the last usable Inter-Area-Router LSA, in LsaKey order, whose ABR R reaches (rib_full step 2 replaces the
+ * entry per LSA), not the cheapest.  The options of an Inter-Area-Router LSA are outside the contract, as they are for
+ * hspf_ospfv3_rtr_summaries.  The Inter-Area-Router rules are restated from the reference's code: no recorded
+ * conformance data holds an Inter-Area-Router LSA, so their parity rests on the host restatement alone.
+ *
+ *   hspf_ospfv3_backbone_asbr_table_create  host.  Arguments as hspf_ospfv3_backbone_table_create; the result may hold
+ *                                Inter-Area-Router slots, as hspf_ospfv2_backbone_asbr_table_create's type-4 slots:
+ *                                per ASBR A some border can originate for, the static records of other ABRs and one
+ *                                slot per (border, non-backbone area where A is an E-flag router) at the border's place
+ *                                in LsaKey order.  The affected prefixes add every prefix of a usable AS-external LSA
+ *                                of such an A.  The refusals of hspf_ospfv3_backbone_table_create apply, except the one
+ *                                of a border's Inter-Area-Router LSA, and: HSPF_E_INVAL a usable Inter-Area-Router LSA
+ *                                of a border for a router it cannot originate for (the NU option does not make one
+ *                                unusable: NU leaves out prefixes only); HSPF_E_UNSUPPORTED a router with the E and the
+ *                                B flag in a border's non-backbone area, or slots reading more than 8 (border, area)
+ *                                plane sets.  The table is marked as this call's: hspf_ospfv2_backbone_table_asbr_slots
+ *                                counts its slots, hspf_ospfv3_backbone_from_cells decodes it (an external cell's
+ *                                winner is its AS-external record, whose prefix options the route takes), and the asbr
+ *                                calls above take it.  Those calls refuse an OSPFv3 area-0 table of
+ *                                hspf_ospfv3_backbone_table_create (HSPF_E_INVAL), before any launch.
+ *   hspf_ospfv2_backbone_asbr_cells[16] / _delta[16]  over this table: with Inter-Area-Router slots, the walk above
+ *                                with the arguments and job status rule of the OSPFv2 asbr calls; without slots, the
+ *                                output of hspf_ospfv2_backbone_cells[16] / _delta[16].  The cells and delta calls
+ *                                without asbr refuse a table with slots (HSPF_E_INVAL).
+ */
+int hspf_ospfv3_backbone_asbr_table_create(const struct hspf_ospfv3_flat *flat, uint32_t router_id,
+                                           const hl_ospfv3_inter_area_lsa *summaries, uint32_t n_summaries,
+                                           const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
+                                           const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                           hspf_ospfv2_backbone_table **out);
+
+/*
  * Non-backbone router over what-if jobs on the backbone, OSPFv3: hspf_ospfv2_nonbackbone_table_create's stage over
  * Inter-Area-Prefix / Inter-Area-Router LSAs.  R is an internal router of a non-backbone area A, a job changes costs
  * in area 0 only, and the borders are A's ABRs attached to area 0 (every one of them must be given).  The borders'
@@ -570,7 +610,7 @@ int hspf_ospfv3_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
  *                                result is an hspf_ospfv2_backbone_table marked OSPFv3 and with its target area A; the
  *                                cells and delta calls of both kinds take it (a table with Inter-Area-Router slots is
  *                                the asbr calls', as for OSPFv2), and hspf_ospfv3_backbone_from_cells decodes it over
- *                                R's image of A.  The asbr calls still refuse an OSPFv3 table of area 0.  Refusals:
+ *                                R's image of A.  Refusals:
  *                                those of hspf_ospfv2_nonbackbone_table_create, over Inter-Area-Prefix /
  *                                Inter-Area-Router LSAs, with an OSPFv2 border table HSPF_E_INVAL and slot winners that
  *                                would not fit 32 bits HSPF_E_UNSUPPORTED.  Inter-Area-Prefix LSAs with the NU option
