@@ -85,8 +85,14 @@ HSPF_HD bool abr_transit(const PF &plane, const AbrRibView &t, uint32_t i) {
     return false;
 }
 
-template <class Planes, class PF>
-HSPF_HD CellWords abr_rib_cell_eval(const PF &plane, const AbrRibView &t, uint32_t p) {
+// The slots of a walk without them (kSlots off).
+struct AbrNoSlots {};
+
+// kSlots (hspf_ospfv2_abr_backbone_table_create, ospf_backbone_cells.h: AbrBorderSlots): a type-3 record that step 2
+// reads may be a slot, which `slots.offer` turns into the border's advertisement (or drops), and a type-4 record
+// with Slots::kAsbrSlot in w is a type-4 slot, skipped unless plane.asbr says its border originates.
+template <class Planes, bool kSlots = false, class PF, class Slots = AbrNoSlots>
+HSPF_HD CellWords abr_rib_cell_eval(const PF &plane, const AbrRibView &t, uint32_t p, const Slots &slots = Slots{}) {
     const uint32_t A = t.n_areas, S = t.P + 1;
     const RouteContrib *contribs = reinterpret_cast<const RouteContrib *>(t.recs);
     const uint32_t *o3 = t.off + (size_t)A * S, *o5 = o3 + (size_t)A * S;
@@ -119,9 +125,13 @@ HSPF_HD CellWords abr_rib_cell_eval(const PF &plane, const AbrRibView &t, uint32
             for (uint32_t k = o3[i * S + p]; k < o3[i * S + p + 1]; ++k) {
                 const RibRec r = load_rib_rec(t.recs + k);
                 if (!pl.reached(r.x)) continue;
-                const uint32_t m = pl.d(r.x) + r.y;
+                uint32_t y = r.y, w = k;
+                if constexpr (kSlots) {
+                    if (!slots.offer(r, y, w)) continue;
+                }
+                const uint32_t m = pl.d(r.x) + y;
                 const uint64_t n = pl.n(r.x) << t.base[i];
-                if (win == kNoRecord || m < metric) { win = k; metric = m; mask = n; area = i; }
+                if (win == kNoRecord || m < metric) { win = w; metric = m; mask = n; area = i; }
                 else if (m == metric) mask |= n;
             }
         }
@@ -163,7 +173,11 @@ HSPF_HD CellWords abr_rib_cell_eval(const PF &plane, const AbrRibView &t, uint32
             for (uint32_t j = s.w; j > s.z; --j) {                      // the last type-4 whose ABR is reached
                 const RibRec f = load_rib_rec(t.recs + j - 1);
                 if (!pl.reached(f.x)) continue;
-                m = pl.d(f.x) + f.y; n = pl.n(f.x); found = true;
+                uint32_t fm = f.y;                                      // a border that does not originate: go on
+                if constexpr (kSlots) {
+                    if ((f.w & Slots::kAsbrSlot) && !plane.asbr.originates(f.w & ~Slots::kAsbrSlot, f.y, fm)) continue;
+                }
+                m = pl.d(f.x) + fm; n = pl.n(f.x); found = true;
                 break;
             }
             if (!found) {
@@ -208,6 +222,7 @@ struct hspf_ospfv2_abr_ribtable {
     std::vector<hspf::RibRec> recs;
     std::vector<uint32_t> v_flagged, vl_off;
     std::vector<uint32_t> ext_tag;                 // per type-5 record (index - ext_base)
+    std::vector<uint32_t> group_asbr;              // per ASBR entry group (records ext_end + A g ..): the ASBR's id
     std::vector<std::unordered_map<uint32_t, uint32_t>> rtr_vertex;   // per area: router id -> router vertex
     // OSPFv3 tables (hspf_ospfv3_abr_ribtable_create): each area's table is an OSPFv3 one-area table, `prefix` is
     // zero-filled (the prefixes are prefix6), and options6 holds the prefix options per type-3 / type-5 record

@@ -231,7 +231,67 @@ HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneVi
     return {mask, type2, (uint64_t)win | ((uint64_t)rib_mpf(metric, path, HL_CELL_PRESENT) << 32)};
 }
 
+// An area border router R over jobs inside an area it is not attached to (hspf_ospfv2_abr_backbone_table_create):
+// abr_rib_cell_eval with kSlots over R's row 0 of every area.  Area 0's type-3 ranges hold static records (z
+// kOspfBackboneStatic) and slots as the backbone table's, its type-4 ranges static records and type-4 slots as the
+// asbr table's.  A slot's winner is n_recs + its slot index.
+struct AbrBorderSlots {
+    static constexpr uint32_t kAsbrSlot = kOspfBackboneAsbrSlot;
+    OspfBorderRows rows;
+    const uint32_t *border;       // [4 n_borders] as OspfBackboneView::border (area 0's records and atoms)
+    uint32_t n_recs;
+    // what type-3 record r offers: a static one its own metric, a slot its border's advertisement (false: none)
+    HSPF_HD bool offer(const RibRec &r, uint32_t &metric, uint32_t &winner) const {
+        if (r.z == kOspfBackboneStatic) return true;
+        uint32_t options;
+        if (!border_summary<false>(rows.row[r.z] + r.y, border, r.z, metric, options)) return false;
+        winner = n_recs + r.w;
+        return true;
+    }
+};
+
+// R's planes of area i at row 0, and the job's type-4 plane sets (kept with the planes, as OspfAsbrPlanes).
+template <class Planes, class D, class N>
+struct AbrRow0Planes {
+    const AbrPlaneSet<D, N> &s;
+    OspfAsbrJob<Planes, D> asbr;
+    HSPF_HD Planes operator()(uint32_t i) const { return Planes{s.dist[i], s.hops[i], s.nh[i]}; }
+};
+
+// The OR of R's row-0 status words over its areas.
+template <class D, class N>
+HSPF_HD uint32_t abr_row0_status(const AbrPlaneSet<D, N> &s, uint32_t n_areas) {
+    uint32_t st = 0;
+    for (uint32_t i = 0; i < n_areas; ++i)
+        if (s.status[i]) st |= s.status[i][0];
+    return st;
+}
+
 }  // namespace hspf
+
+// Host + device image of an area border router's affected prefixes over jobs inside another area
+// (include/holo_spf_lsdb.h, hspf_ospfv2_abr_backbone_table_create; ospf_ribtable.h, build_abr_backbone_table).
+struct hspf_ospfv2_abr_backbone_table {
+    // R's table over the affected prefixes.  Its records: every area's intra-area records as R's whole table has them
+    // (the decode's), the type-3 ranges (area 0's with slots), the type-5 ranges, the ASBR entries and type-4 ranges,
+    // then from walk_intra the intra-area records of the affected prefixes again, which `off` names for the walk.
+    hspf_ospfv2_abr_ribtable *abr = nullptr;
+    uint32_t area0 = 0, n_borders = 0, walk_intra = 0;
+    const hspf_ospfv2_abr_ribtable *borders[hspf::kOspfBackboneMaxBorders] = {};
+    std::vector<uint32_t> intra_src;             // per walk intra-area record (index - walk_intra): the decode's record
+    std::vector<uint32_t> slot_rec;              // [n_slots] the record of each slot
+    uint32_t n_asbr_slots = 0;
+    std::vector<std::pair<uint32_t, uint32_t>> asbr_set;   // the type-4 slots' plane sets (border, area index)
+    std::vector<uint32_t> words;                 // abr->off, padded to 16 bytes, then border [4 n_borders]
+    hspf::DeviceRouteTable dev;                  // words, then records
+
+    uint32_t P() const { return (uint32_t)abr->prefix.size(); }
+    uint32_t n_recs() const { return (uint32_t)abr->recs.size(); }
+    size_t border_at() const { return (abr->off.size() + 3) & ~(size_t)3; }
+    hspf::AbrRibView view(const uint32_t *w, const hspf::RibRec *rc) const {
+        return abr->view(w, rc, reinterpret_cast<const uint32_t *>(rc + abr->recs.size()));
+    }
+};
 
 // Host + device image of a backbone router's affected prefixes (include/holo_spf_lsdb.h).
 struct hspf_ospfv2_backbone_table {

@@ -10,9 +10,13 @@
 //                      affected prefixes over its one-area table and its borders' ABR tables (ospf_backbone_cells.h);
 //                      hspf_ospfv{2,3}_nonbackbone_table_create: the same for an internal router of a non-backbone
 //                      area
+//   build_abr_backbone_table  hspf_ospfv2_abr_backbone_table_create: an area border router's affected prefixes over
+//                      its ABR table and the borders' (build_abr_ribtable, and the slot helpers build_backbone_table
+//                      shares)
 //   decode_rib         one job's cells -> its routing table, for hspf_ospfv2_rib_from_cells,
-//                      hspf_ospfv3_rib_from_cells, hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib) and
-//                      hspf_ospfv{2,3}_backbone_from_cells (decode_backbone_rib).  A one-area table decodes as an area
+//                      hspf_ospfv3_rib_from_cells, hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib),
+//                      hspf_ospfv{2,3}_backbone_from_cells (decode_backbone_rib) and
+//                      hspf_ospfv2_abr_backbone_from_cells (decode_abr_backbone_rib).  A one-area table decodes as an area
 //                      border router's table with a single area.
 //
 // For build_rib_records a version trait T provides:
@@ -54,6 +58,7 @@
 //   to_nh(hop, sort), to_hop   a next hop into the merged set, naming its interface's sort key, and back out
 #pragma once
 #include <algorithm>
+#include <array>
 #include <cstdint>
 #include <cstring>
 #include <map>
@@ -322,6 +327,8 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
         for (uint32_t k = 0; k < rec_group.size(); ++k) recs[t->ext_base + k].x = group_base + rec_group[k] * A;
         recs.resize((size_t)group_base + (size_t)G * A);
         for (uint32_t g = 0; g < G; ++g)
+            t->group_asbr.push_back(r0.asbr_id[r0.recs[r0.ext_base + group_rep[g]].x - r0.ext_end]);
+        for (uint32_t g = 0; g < G; ++g)
             for (uint32_t i = 0; i < A; ++i) {
                 const hspf_ospfv2_ribtable &rt = *t->area[i];
                 const RibRec s = rt.recs[rt.recs[rt.ext_base + group_rep[g]].x];
@@ -346,6 +353,93 @@ int build_abr_ribtable(uint32_t router_id, uint32_t n_areas, const typename T::F
     } catch (...) {
         return HSPF_E_UNSUPPORTED;
     }
+}
+
+// ---- the borders' slots, shared by build_backbone_table and build_abr_backbone_table ----------------------------
+using BorderSlots = std::vector<std::pair<uint32_t, uint32_t>>;     // (border, index), in the borders' LsaKey order
+
+inline void sort_by_router_id(BorderSlots &sl, const hspf_ospfv2_abr_ribtable *const *borders) {
+    std::stable_sort(sl.begin(), sl.end(), [&](const std::pair<uint32_t, uint32_t> &x, const std::pair<uint32_t, uint32_t> &y) {
+        return borders[x.first]->router_id < borders[y.first]->router_id;
+    });
+}
+
+template <class K>
+bool has_border(const std::map<K, BorderSlots> &m, const K &key, uint32_t b) {
+    auto it = m.find(key);
+    if (it != m.end())
+        for (const auto &s : it->second)
+            if (s.first == b) return true;
+    return false;
+}
+
+// Type-4 slots: per ASBR id, the (border, area index) pairs of the borders' areas other than the target area ta where
+// it is a router with the E flag, in LsaKey order.  HSPF_E_UNSUPPORTED for such a router with the B flag (its entry
+// would replace an ABR's, as hspf_ospfv2_ribtable_create refuses).
+inline int border_asbr_origins(const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders, uint32_t ta,
+                               std::map<uint32_t, BorderSlots> &orig) {
+    for (uint32_t b = 0; b < n_borders; ++b) {
+        const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+        for (uint32_t i = 0; i < bt.n_areas; ++i) {
+            if (bt.area_id[i] == ta) continue;
+            for (const auto &e : bt.rtr_vertex[i]) {
+                const uint8_t fl = bt.area[i]->vflags[e.second];
+                if (!(fl & HL_RTR_FLAG_E)) continue;
+                if (fl & HL_RTR_FLAG_B) return HSPF_E_UNSUPPORTED;
+                orig[e.first].emplace_back(b, i);
+            }
+        }
+    }
+    for (auto &e : orig) sort_by_router_id(e.second, borders);
+    return HSPF_OK;
+}
+
+// Type-3 slots: per prefix key, the (border, prefix index) pairs of the borders that can advertise it into the target
+// area ta: an intra-area record in one of the border's areas other than ta, or, into a non-backbone area (nb), a
+// type-3 record in its area 0 (index a0[b]); `skip(key)` drops a key.  Sorted into LsaKey order.
+template <class T, class Skip>
+void border_prefix_slots(const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders, const uint32_t *a0,
+                         uint32_t ta, bool nb, Skip skip, std::map<typename T::Key, BorderSlots> &slots) {
+    for (uint32_t b = 0; b < n_borders; ++b) {
+        const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+        const uint32_t P = (uint32_t)bt.prefix.size(), S = P + 1, A = bt.n_areas;
+        for (uint32_t u = 0; u < P; ++u) {
+            bool adv = nb && bt.off[(A + a0[b]) * S + u] != bt.off[(A + a0[b]) * S + u + 1];
+            for (uint32_t i = 0; i < A && !adv; ++i)
+                adv = bt.area_id[i] != ta && bt.off[i * S + u] != bt.off[i * S + u + 1];
+            if (adv && !skip(T::table_key(bt, u))) slots[T::table_key(bt, u)].emplace_back(b, u);
+        }
+    }
+    for (auto &e : slots) sort_by_router_id(e.second, borders);
+}
+
+// A range of static records (in LsaKey order, `adv_rtr(s)` each) with every slot of `sl` at its border's LsaKey place.
+template <class S, class AdvRtr, class PutStatic, class PutSlot>
+void merge_lsakey(const std::vector<S> &statics, AdvRtr adv_rtr, const BorderSlots &sl,
+                  const hspf_ospfv2_abr_ribtable *const *borders, PutStatic put_static, PutSlot put_slot) {
+    size_t k = 0;
+    for (const S &s : statics) {
+        while (k < sl.size() && borders[sl[k].first]->router_id < adv_rtr(s)) put_slot(sl[k++]);
+        put_static(s);
+    }
+    while (k < sl.size()) put_slot(sl[k++]);
+}
+
+// The type-4 slot of (border, area index) o for ASBR `id`, whose border is vertex bv of the table's area; its plane set
+// is added to `sets` when new.
+inline RibRec asbr_slot(const hspf_ospfv2_abr_ribtable *const *borders, uint32_t bv, const std::pair<uint32_t, uint32_t> &o,
+                        uint32_t id, std::map<std::pair<uint32_t, uint32_t>, uint32_t> &set_of,
+                        std::vector<std::pair<uint32_t, uint32_t>> &sets) {
+    auto ins = set_of.emplace(o, (uint32_t)sets.size());
+    if (ins.second) sets.push_back(o);
+    return RibRec{bv, borders[o.first]->rtr_vertex[o.second].at(id), o.first, kOspfBackboneAsbrSlot | ins.first->second};
+}
+
+// Border b's words (OspfBackboneView::border): its intra-area records of area index i, and i's atom bits.
+inline std::array<uint32_t, 4> border_words(const hspf_ospfv2_abr_ribtable &bt, uint32_t i) {
+    const uint32_t lo = bt.intra_base[i], na = bt.n_atoms[i];
+    const uint64_t atoms = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << bt.base[i]);
+    return {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)};
 }
 
 // hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create, argument checks included: R's one-area table
@@ -444,56 +538,21 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                 if (fl & HL_RTR_FLAG_V) return HSPF_E_UNSUPPORTED;
         // type-4 slots: per ASBR id, the (border, area index) pairs of the borders' areas other than the target where
         // it is a router with the E flag, each border's in area order (none into a stub area)
-        std::map<uint32_t, std::vector<std::pair<uint32_t, uint32_t>>> orig;
+        std::map<uint32_t, BorderSlots> orig;
         if (asbr && normal) {
-            for (uint32_t b = 0; b < n_borders; ++b) {
-                const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-                for (uint32_t i = 0; i < bt.n_areas; ++i) {
-                    if (bt.area_id[i] == ta) continue;
-                    for (const auto &e : bt.rtr_vertex[i]) {
-                        const uint8_t fl = bt.area[i]->vflags[e.second];
-                        if (!(fl & HL_RTR_FLAG_E)) continue;
-                        // its entry at R would replace an ABR's (as hspf_ospfv2_ribtable_create refuses)
-                        if (fl & HL_RTR_FLAG_B) return HSPF_E_UNSUPPORTED;
-                        orig[e.first].emplace_back(b, i);
-                    }
-                }
-            }
-            for (auto &e : orig)
-                std::stable_sort(e.second.begin(), e.second.end(), [&](const std::pair<uint32_t, uint32_t> &x,
-                                                                       const std::pair<uint32_t, uint32_t> &y) {
-                    return borders[x.first]->router_id < borders[y.first]->router_id;
-                });
-            for (const auto &x : border_t4) {
-                auto it = orig.find(x.second);
-                bool found = false;
-                if (it != orig.end())
-                    for (const auto &o : it->second) found = found || o.first == x.first;
-                if (!found) return HSPF_E_INVAL;                     // the LSDB disagrees with the border's table
-            }
+            if (const int rc2 = border_asbr_origins(borders, n_borders, ta, orig)) return rc2;
+            for (const auto &x : border_t4)
+                if (!has_border(orig, x.second, x.first)) return HSPF_E_INVAL;   // the LSDB disagrees with the border's table
         }
         // the affected prefixes: each border's prefixes with an intra-area record in one of its areas other than the
         // target (into a non-backbone area also those with a type-3 record in its area 0; none into a totally stubby
         // area, and not a stub area's default route)
-        std::map<Key, std::vector<std::pair<uint32_t, uint32_t>>> slots;   // key -> (border, its prefix index)
-        for (uint32_t b = 0; b < n_borders && (!nb || config->summary); ++b) {
-            const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-            const uint32_t P = (uint32_t)bt.prefix.size(), S = P + 1, A = bt.n_areas;
-            for (uint32_t u = 0; u < P; ++u) {
-                bool adv = nb && bt.off[(A + a0[b]) * S + u] != bt.off[(A + a0[b]) * S + u + 1];
-                for (uint32_t i = 0; i < A && !adv; ++i)
-                    adv = bt.area_id[i] != ta && bt.off[i * S + u] != bt.off[i * S + u + 1];
-                if (nb && !normal && T::table_key(bt, u) == dflt) adv = false;
-                if (adv) slots[T::table_key(bt, u)].emplace_back(b, u);
-            }
-        }
-        for (const auto &x : border_t3) {
-            auto it = slots.find(x.second);
-            bool found = false;
-            if (it != slots.end())
-                for (const auto &s : it->second) found = found || s.first == x.first;
-            if (!found) return HSPF_E_INVAL;                         // the LSDB disagrees with the border's table
-        }
+        std::map<Key, BorderSlots> slots;                            // key -> (border, its prefix index)
+        if (!nb || config->summary)
+            border_prefix_slots<T>(borders, n_borders, a0.data(), ta, nb,
+                                   [&](const Key &k) { return nb && !normal && k == dflt; }, slots);
+        for (const auto &x : border_t3)
+            if (!has_border(slots, x.second, x.first)) return HSPF_E_INVAL;      // the LSDB disagrees with the border's table
         // ... and the prefixes of the type-5 LSAs of an ASBR some border can originate a type-4 LSA for
         const uint32_t *rx = r.off.data() + 2 * (r.prefix.size() + 1);
         if (!orig.empty())
@@ -520,32 +579,25 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         t->prefix.resize(P); t->plen.resize(P);
         if (T::kV3) t->prefix6.resize(P);
         uint32_t u = 0;
+        const std::vector<std::array<uint32_t, 4>> none;
         for (auto &e : slots) {
-            auto &sl = e.second;
-            std::stable_sort(sl.begin(), sl.end(), [&](const std::pair<uint32_t, uint32_t> &x,
-                                                       const std::pair<uint32_t, uint32_t> &y) {
-                return borders[x.first]->router_id < borders[y.first]->router_id;
-            });
             T::set_prefix(*t, u, e.first);
             auto qi = q_of.find(e.first);
             q[u] = qi == q_of.end() ? kNoRecord : qi->second;
             o3[u] = (uint32_t)t->recs.size();
             auto st = statics.find(e.first);
-            size_t k = 0;
-            auto put_slot = [&]() {
-                const uint32_t b = sl[k].first;
-                t->slot_rec.push_back((uint32_t)t->recs.size());
-                t->recs.push_back(RibRec{bv[b], sl[k].second, b, (uint32_t)t->slot_rec.size() - 1});
-                if (T::kV3) t->options6.push_back(0);
-                ++k;
-            };
-            if (st != statics.end())
-                for (const auto &s : st->second) {
-                    while (k < sl.size() && borders[sl[k].first]->router_id < s[0]) put_slot();
+            merge_lsakey(
+                st != statics.end() ? st->second : none, [](const std::array<uint32_t, 4> &s) { return s[0]; },
+                e.second, borders,
+                [&](const std::array<uint32_t, 4> &s) {
                     t->recs.push_back(RibRec{s[1], s[2], kOspfBackboneStatic, 0});
                     if (T::kV3) t->options6.push_back((uint8_t)s[3]);
-                }
-            while (k < sl.size()) put_slot();
+                },
+                [&](const std::pair<uint32_t, uint32_t> &s) {
+                    t->slot_rec.push_back((uint32_t)t->recs.size());
+                    t->recs.push_back(RibRec{bv[s.first], s.second, s.first, (uint32_t)t->slot_rec.size() - 1});
+                    if (T::kV3) t->options6.push_back(0);
+                });
             ++u;
         }
         o3[P] = (uint32_t)t->recs.size();
@@ -575,25 +627,16 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                 const uint32_t id = r.asbr_id[a];
                 auto o = orig.find(id);
                 if (o == orig.end()) continue;
-                const auto &ob = o->second;
                 const auto st = t4.find(id);
                 const uint32_t z = (uint32_t)t->recs.size();
-                size_t k = 0;
-                auto put_slot = [&]() {
-                    const uint32_t b = ob[k].first, i = ob[k].second;
-                    auto ins = set_of.emplace(ob[k], (uint32_t)t->asbr_set.size());
-                    if (ins.second) t->asbr_set.push_back(ob[k]);
-                    t->recs.push_back(RibRec{bv[b], borders[b]->rtr_vertex[i].at(id), b,
-                                             kOspfBackboneAsbrSlot | ins.first->second});
-                    ++t->n_asbr_slots;
-                    ++k;
-                };
-                if (st != t4.end())
-                    for (const auto &x : st->second) {
-                        while (k < ob.size() && borders[ob[k].first]->router_id < x.first) put_slot();
-                        t->recs.push_back(x.second);
-                    }
-                while (k < ob.size()) put_slot();
+                const std::vector<std::pair<uint32_t, RibRec>> none;
+                merge_lsakey(
+                    st != t4.end() ? st->second : none, [](const std::pair<uint32_t, RibRec> &x) { return x.first; },
+                    o->second, borders, [&](const std::pair<uint32_t, RibRec> &x) { t->recs.push_back(x.second); },
+                    [&](const std::pair<uint32_t, uint32_t> &x) {
+                        t->recs.push_back(asbr_slot(borders, bv[x.first], x, id, set_of, t->asbr_set));
+                        ++t->n_asbr_slots;
+                    });
                 RibRec &s = t->recs[r.ext_end + a];
                 s.z = z;
                 s.w = (uint32_t)t->recs.size();
@@ -612,9 +655,8 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         auto opt_end = [&](const hspf_ospfv2_abr_ribtable &bt) { return nb ? bt.t3_end : bt.t3_base[0]; };
         for (uint32_t b = 0; b < n_borders; ++b) {
             const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-            const uint32_t i = at[b], lo = bt.intra_base[i], na = bt.n_atoms[i];
-            const uint64_t atoms = na == 0 ? 0 : ((na == 64 ? ~0ull : ((1ull << na) - 1)) << bt.base[i]);
-            t->words.insert(t->words.end(), {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)});
+            const std::array<uint32_t, 4> bw = border_words(bt, at[b]);
+            t->words.insert(t->words.end(), bw.begin(), bw.end());
             if (T::kV3) {
                 t->words.insert(t->words.end(), {4 * opt_words, 0u, 0u, 0u});
                 opt_words += (opt_end(bt) + 3) / 4;
@@ -643,6 +685,224 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                 if (!opt.empty()) std::memcpy(t->words.data() + at, opt.data(), opt.size());
             }
         }
+        *out = t.release();
+        return HSPF_OK;
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_UNSUPPORTED;
+    }
+}
+
+// hspf_ospfv2_abr_backbone_table_create, argument checks included: an area border router R of area 0 and other areas
+// over jobs inside an area it is not attached to.  R's ABR table (build_abr_ribtable) over its areas, with area 0's
+// summaries without the borders' type-3 / type-4 LSAs, restricted to the affected prefixes: those some border can
+// advertise into area 0, and those of the type-5 LSAs of an ASBR some border can originate a type-4 LSA for.  Area
+// 0's type-3 ranges get the borders' slots and its type-4 ranges their type-4 slots, at the borders' LsaKey places,
+// as build_backbone_table places them (ospf_backbone_cells.h: AbrBorderSlots).
+template <class T>
+int build_abr_backbone_table(uint32_t router_id, uint32_t n_areas, const typename T::Flat *const *flats,
+                             const uint32_t *area_ids, const typename T::Sum *const *summaries,
+                             const uint32_t *n_summaries, const uint8_t *active, const typename T::Ext *ext,
+                             uint32_t n_ext, const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                             hspf_ospfv2_abr_backbone_table **out) {
+    using Key = typename T::Key;
+    using Sum = typename T::Sum;
+    constexpr uint32_t kNone = 0xFFFFFFFFu;
+    if (!out || !flats || !area_ids || n_areas == 0 || !borders || (n_ext && !ext)) return HSPF_E_INVAL;
+    *out = nullptr;
+    if (n_borders == 0 || n_borders > kOspfBackboneMaxBorders) return HSPF_E_INVAL;
+    if (n_areas > kAbrMaxAreas) return HSPF_E_UNSUPPORTED;
+    uint32_t i0 = kNone, n_active = 0;
+    for (uint32_t i = 0; i < n_areas; ++i) {
+        if (!flats[i] || !flats[i]->area) return HSPF_E_INVAL;
+        if (n_summaries && n_summaries[i] && (!summaries || !summaries[i])) return HSPF_E_INVAL;
+        if (area_ids[i] == 0 && i0 == kNone) i0 = i;
+        n_active += (!active || active[i]) ? 1u : 0u;
+    }
+    if (i0 == kNone || (active && !active[i0]) || n_active < 2) return HSPF_E_INVAL;
+    try {
+        std::unique_ptr<hspf_ospfv2_abr_backbone_table, void (*)(hspf_ospfv2_abr_backbone_table *)> t(
+            new hspf_ospfv2_abr_backbone_table(), hspf_ospfv2_abr_backbone_table_free);
+        const typename T::Flat &f = *flats[i0];
+        auto vertex = [&](uint32_t id) { return T::root_vertex(f, id); };
+        auto flags = [&](uint32_t v) { return v == kNone ? (uint8_t)0 : T::router_flags(f, v); };
+        if (!(flags(vertex(router_id)) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
+        // the borders: their area-0 index and their vertex in R's area 0
+        std::vector<uint32_t> a0(n_borders), bv(n_borders);
+        std::unordered_map<uint32_t, uint32_t> border_of;
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            const hspf_ospfv2_abr_ribtable *bt = borders[b];
+            if (!bt || bt->v3 != T::kV3 || bt->router_id == router_id || !border_of.emplace(bt->router_id, b).second)
+                return HSPF_E_INVAL;
+            a0[b] = kNone;
+            for (uint32_t i = 0; i < bt->n_areas && a0[b] == kNone; ++i)
+                if (bt->area_id[i] == 0) a0[b] = i;
+            bv[b] = vertex(bt->router_id);
+            if (a0[b] == kNone || !(flags(bv[b]) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
+            t->borders[b] = bt;
+        }
+        t->n_borders = n_borders;
+        t->area0 = i0;
+        // area 0's summaries without the borders' LSAs, which the slots stand for
+        const uint32_t n0 = n_summaries ? n_summaries[i0] : 0;
+        auto live = [](const Sum &l) { return !l.maxage && l.metric < HL_LSA_INFINITY && !T::skip(l); };
+        std::vector<Sum> rest;
+        std::vector<std::pair<uint32_t, Key>> border_t3;
+        std::vector<std::pair<uint32_t, uint32_t>> border_t4;
+        for (uint32_t k = 0; k < n0; ++k) {
+            const Sum &l = summaries[i0][k];
+            auto it = border_of.find(l.adv_rtr);
+            if (it == border_of.end()) { rest.push_back(l); continue; }
+            if (!live(l)) continue;
+            if (l.lsa_type == 3) border_t3.emplace_back(it->second, T::key(l));
+            if (l.lsa_type == 4) border_t4.emplace_back(it->second, T::asbr_id(l));
+        }
+        std::map<uint32_t, BorderSlots> orig;
+        if (const int rc = border_asbr_origins(borders, n_borders, 0, orig)) return rc;
+        for (const auto &x : border_t4)
+            if (!has_border(orig, x.second, x.first)) return HSPF_E_INVAL;
+        std::map<Key, BorderSlots> slots;
+        border_prefix_slots<T>(borders, n_borders, a0.data(), 0, false, [](const Key &) { return false; }, slots);
+        for (const auto &x : border_t3)
+            if (!has_border(slots, x.second, x.first)) return HSPF_E_INVAL;
+        // R's whole table over those summaries
+        std::vector<const Sum *> sp(n_areas);
+        std::vector<uint32_t> ns(n_areas);
+        for (uint32_t i = 0; i < n_areas; ++i) {
+            sp[i] = i == i0 ? rest.data() : (summaries ? summaries[i] : nullptr);
+            ns[i] = i == i0 ? (uint32_t)rest.size() : (n_summaries ? n_summaries[i] : 0);
+        }
+        hspf_ospfv2_abr_ribtable *full_raw = nullptr;
+        int rc = build_abr_ribtable<T>(router_id, n_areas, flats, area_ids, sp.data(), ns.data(), active, ext, n_ext,
+                                       &full_raw);
+        if (rc) return rc;
+        std::unique_ptr<hspf_ospfv2_abr_ribtable, void (*)(hspf_ospfv2_abr_ribtable *)> full(full_raw,
+                                                                                            hspf_ospfv2_abr_ribtable_free);
+        const hspf_ospfv2_abr_ribtable &F = *full;
+        if (!F.v_flagged.empty()) return HSPF_E_UNSUPPORTED;          // the transit-area step
+        const uint32_t A = n_areas, PF = (uint32_t)F.prefix.size(), SF = PF + 1;
+        const uint32_t G = (uint32_t)F.group_asbr.size();
+        // ... and the prefixes of the type-5 LSAs of an ASBR with type-4 slots
+        std::map<Key, uint32_t> uf;                                  // R's prefix index of a key
+        for (uint32_t u = 0; u < PF; ++u) uf.emplace(T::table_key(F, u), u);
+        const uint32_t *f5 = F.off.data() + 2 * (size_t)A * SF;
+        for (uint32_t u = 0; u < PF; ++u)
+            for (uint32_t k = f5[u]; k < f5[u + 1]; ++k)
+                if (orig.count(F.group_asbr[(F.recs[k].x - F.ext_end) / A])) {
+                    slots[T::table_key(F, u)];
+                    break;
+                }
+        // the table over the affected prefixes
+        std::unique_ptr<hspf_ospfv2_abr_ribtable, void (*)(hspf_ospfv2_abr_ribtable *)> r(new hspf_ospfv2_abr_ribtable(),
+                                                                                         hspf_ospfv2_abr_ribtable_free);
+        r->router_id = F.router_id; r->n_areas = A; r->max_paths = F.max_paths; r->step2 = F.step2; r->v3 = F.v3;
+        r->area = F.area; full->area.clear();                        // the area tables move over
+        r->area_id = F.area_id; r->root = F.root; r->n_vertices = F.n_vertices; r->base = F.base;
+        r->n_atoms = F.n_atoms; r->intra_base = F.intra_base; r->rtr_vertex = F.rtr_vertex;
+        r->group_asbr = F.group_asbr;
+        const uint32_t P = (uint32_t)slots.size(), S = P + 1;
+        std::vector<uint32_t> from(P);                               // R's prefix index of each, or kNone
+        r->prefix.resize(P); r->plen.resize(P);
+        r->area_prefix.assign(A, std::vector<uint32_t>(P, kNoRecord));
+        uint32_t u = 0;
+        for (const auto &e : slots) {
+            T::set_prefix(*r, u, e.first);
+            auto it = uf.find(e.first);
+            from[u] = it == uf.end() ? kNone : it->second;
+            for (uint32_t i = 0; i < A && from[u] != kNone; ++i) r->area_prefix[i][u] = F.area_prefix[i][from[u]];
+            ++u;
+        }
+        r->off.assign((2 * (size_t)A + 1) * S, 0);
+        uint32_t *o3 = r->off.data() + (size_t)A * S, *o5 = o3 + (size_t)A * S;
+        auto &recs = r->recs;
+        recs.assign(F.recs.begin(), F.recs.begin() + F.t3_base[0]);  // every intra-area record, for the decode
+        // R's router id of each area-0 vertex, for the LsaKey order of the static records
+        std::unordered_map<uint32_t, uint32_t> id_of;
+        for (const auto &e : F.rtr_vertex[i0]) id_of.emplace(e.second, e.first);
+        auto adv_rtr = [&](const RibRec &x) { return id_of.at(x.x); };
+        for (uint32_t i = 0; i < A; ++i) {                           // type-3, area 0's with the slots
+            r->t3_base.push_back((uint32_t)recs.size());
+            const uint32_t *g3 = F.off.data() + (A + i) * (size_t)SF;
+            u = 0;
+            for (const auto &e : slots) {
+                o3[i * S + u] = (uint32_t)recs.size();
+                std::vector<RibRec> st;
+                if (from[u] != kNone) st.assign(F.recs.begin() + g3[from[u]], F.recs.begin() + g3[from[u] + 1]);
+                if (i != i0) {
+                    recs.insert(recs.end(), st.begin(), st.end());
+                } else {
+                    merge_lsakey(st, adv_rtr, e.second, borders,
+                                 [&](const RibRec &x) { recs.push_back(RibRec{x.x, x.y, kOspfBackboneStatic, 0}); },
+                                 [&](const std::pair<uint32_t, uint32_t> &s) {
+                                     t->slot_rec.push_back((uint32_t)recs.size());
+                                     recs.push_back(RibRec{bv[s.first], s.second, s.first, (uint32_t)t->slot_rec.size() - 1});
+                                 });
+                }
+                ++u;
+            }
+            o3[i * S + P] = (uint32_t)recs.size();
+        }
+        r->t3_end = (uint32_t)recs.size();
+        // type-5, then the ASBR entries and their type-4 ranges, moved by `shift`
+        r->ext_base = (uint32_t)recs.size();
+        size_t n5 = 0;
+        for (u = 0; u < P; ++u)
+            if (from[u] != kNone) n5 += f5[from[u] + 1] - f5[from[u]];
+        const uint32_t shift = (uint32_t)(recs.size() + n5) - F.ext_end;
+        for (u = 0; u < P; ++u) {
+            o5[u] = (uint32_t)recs.size();
+            if (from[u] == kNone) continue;
+            for (uint32_t k = f5[from[u]]; k < f5[from[u] + 1]; ++k) {
+                recs.push_back(RibRec{F.recs[k].x + shift, F.recs[k].y, F.recs[k].z, F.recs[k].w});
+                r->ext_tag.push_back(F.ext_tag[k - F.ext_base]);
+            }
+        }
+        o5[P] = (uint32_t)recs.size();
+        r->ext_end = o5[P];
+        recs.insert(recs.end(), F.recs.begin() + F.ext_end, F.recs.end());
+        for (uint32_t k = 0; k < G * A; ++k) {
+            recs[r->ext_end + k].z += shift;
+            recs[r->ext_end + k].w += shift;
+        }
+        std::map<std::pair<uint32_t, uint32_t>, uint32_t> set_of;
+        for (uint32_t g = 0; g < G; ++g) {                           // area 0's entry of an ASBR with type-4 slots
+            auto o = orig.find(F.group_asbr[g]);
+            if (o == orig.end()) continue;
+            const RibRec s = recs[r->ext_end + g * A + i0];
+            const std::vector<RibRec> st(recs.begin() + s.z, recs.begin() + s.w);
+            const uint32_t z = (uint32_t)recs.size();
+            merge_lsakey(st, adv_rtr, o->second, borders, [&](const RibRec &x) { recs.push_back(x); },
+                         [&](const std::pair<uint32_t, uint32_t> &x) {
+                             recs.push_back(asbr_slot(borders, bv[x.first], x, o->first, set_of, t->asbr_set));
+                             ++t->n_asbr_slots;
+                         });
+            recs[r->ext_end + g * A + i0] = RibRec{s.x, s.y, z, (uint32_t)recs.size()};
+        }
+        if (t->asbr_set.size() > kOspfBackboneMaxAsbrSets) return HSPF_E_UNSUPPORTED;   // the kernel parameter's
+        // the walk's intra-area ranges: the affected prefixes' records again, each naming its decode record
+        t->walk_intra = (uint32_t)recs.size();
+        for (uint32_t i = 0; i < A; ++i) {
+            for (u = 0; u < P; ++u) {
+                r->off[i * S + u] = (uint32_t)recs.size();
+                if (from[u] == kNone) continue;
+                for (uint32_t k = F.off[i * SF + from[u]]; k < F.off[i * SF + from[u] + 1]; ++k) {
+                    recs.push_back(F.recs[k]);
+                    t->intra_src.push_back(k);
+                }
+            }
+            r->off[i * S + P] = (uint32_t)recs.size();
+        }
+        r->vl_off.assign(A + 1, 0);
+        if (recs.size() >= kNoRecord || !backbone_winners_fit(recs.size(), t->slot_rec.size(), false))
+            return HSPF_E_UNSUPPORTED;
+        t->words = r->off;
+        t->words.resize(((t->words.size() + 3) & ~(size_t)3), 0);
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            const std::array<uint32_t, 4> bw = border_words(*borders[b], a0[b]);
+            t->words.insert(t->words.end(), bw.begin(), bw.end());
+        }
+        t->abr = r.release();
         *out = t.release();
         return HSPF_OK;
     } catch (const std::bad_alloc &) {
@@ -862,6 +1122,34 @@ int decode_abr_rib(const hspf_ospfv2_abr_ribtable *t, const typename T::Area *ar
                               t->base[i], mask, t->area_id[i], &jd[i]});
         }
         return decode_rib(d, cells, out);
+    } catch (const std::bad_alloc &) {
+        return HSPF_E_NOMEM;
+    } catch (...) {
+        return HSPF_E_INVAL;
+    }
+}
+
+// hspf_ospfv2_abr_backbone_from_cells, argument checks included: a slot winner names its type-3 record and a walk
+// intra-area record the decode's, then decode_abr_rib over the table's prefixes.
+template <class T>
+int decode_abr_backbone_rib(const hspf_ospfv2_abr_backbone_table *t, const typename T::Area *areas, uint32_t n_areas,
+                            const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
+                            const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out) {
+    if (!t || !t->abr || !cells || !out) return HSPF_E_INVAL;
+    try {
+        const uint32_t n_recs = t->n_recs();
+        std::vector<hl_ospf_rib_cell> c(cells, cells + t->P());
+        for (hl_ospf_rib_cell &x : c) {
+            if (!(HL_RIB_CELL_FLAGS(x) & HL_CELL_PRESENT)) continue;
+            if (x.winner >= n_recs) {
+                if (HL_RIB_CELL_PATH(x) != HL_PATH_INTER_AREA || x.winner - n_recs >= t->slot_rec.size()) return HSPF_E_INVAL;
+                x.winner = t->slot_rec[x.winner - n_recs];
+            } else if (HL_RIB_CELL_PATH(x) == HL_PATH_INTRA_AREA) {
+                if (x.winner < t->walk_intra || x.winner - t->walk_intra >= t->intra_src.size()) return HSPF_E_INVAL;
+                x.winner = t->intra_src[x.winner - t->walk_intra];
+            }
+        }
+        return decode_abr_rib<T>(t->abr, areas, n_areas, c.data(), gather_area, gather_v, gather_nh, n_gather, out);
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;
     } catch (...) {

@@ -1,0 +1,178 @@
+// Device stage for the routing table of an OSPFv2 area border router over what-if jobs inside an area it is not
+// attached to (include/holo_spf_lsdb.h, hspf_ospfv2_abr_backbone_table_create): update_rib_full at the router, for
+// its affected prefixes, with every border's type-3 and type-4 LSAs in area 0 re-originated for the job.
+//
+// One launch on the ctx stream: one thread per (job, prefix) runs abr_rib_cell_eval with kSlots (ospf_abr_rib_cells.h,
+// ospf_backbone_cells.h: AbrBorderSlots) over the router's row 0 of every area, the job's row of each border's
+// routing-table cells and the job's rows of the plane sets its type-4 slots read; the shared cell kernel or the
+// route-delta stage (route_stage.cuh) stores or compares the 24-byte cells.
+#include <cstring>
+#include <vector>
+
+#include "../../include/holo_spf_lsdb.h"
+#include "ospf_backbone_cells.h"
+#include "route_stage.cuh"
+
+namespace {
+
+using hspf::kOspfBackboneMaxBorders;
+
+template <class Planes>
+struct OspfAbrBackboneCell {
+    using Rows = hspf::ResultPlanes<Planes>;
+    using D = typename Rows::D;
+    using N = typename Rows::N;
+    hspf::AbrRibView t;
+    hspf::AbrPlaneSet<D, N> s;                                    // R's planes of each area; only row 0 is read
+    hspf::OspfAsbrSets<D> sets;                                   // the plane sets the type-4 slots read
+    const hl_ospf_rib_cell *cells[kOspfBackboneMaxBorders];       // [n_jobs][K_b] per border
+    const uint32_t *status[kOspfBackboneMaxBorders];              // [n_jobs] per border, or NULL
+    uint32_t K[kOspfBackboneMaxBorders];
+    const uint32_t *border;                                       // the table's border words
+    uint32_t n_borders, n_recs;
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
+        uint32_t st = hspf::abr_row0_status(s, t.n_areas) | hspf::asbr_job_status(sets, j);
+        for (uint32_t b = 0; b < n_borders; ++b)
+            if (status[b]) st |= status[b][j];
+        return st;
+    }
+    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::AbrBorderSlots sl;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) sl.rows.row[b] = cells[b] + (size_t)j * K[b];
+        sl.border = border;
+        sl.n_recs = n_recs;
+        const hspf::AbrRow0Planes<Planes, D, N> plane{s, {sets, j}};
+        return hspf::abr_rib_cell_eval<Planes, true>(plane, t, p, sl);
+    }
+    __device__ __forceinline__ uint64_t gather(uint32_t, uint32_t, uint32_t) const { return 0; }   // row 0: host side
+    __device__ static hspf::CellWords empty() { return {0, 0, hspf::kNoRecord}; }
+};
+
+// Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6).
+constexpr uint32_t kAbrBackboneBlocksPerSM = 4;
+
+// R's planes, the borders' cells and status words, and the plane sets the type-4 slots name, from each border's
+// planes, row counts and rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when the
+// table has no type-4 slot.
+template <class R>
+int make_cell(const hspf_ospfv2_abr_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
+              const uint32_t *const *border_status, const R *const *border_planes, const uint32_t *const *border_n_rows,
+              const uint32_t *const *border_rows, uint32_t n_jobs, OspfAbrBackboneCell<hspf::PlanesOf<R>> &cell) {
+    if (!t || !t->abr || !t->dev.blob || !planes || !border_cells) return HSPF_E_INVAL;
+    const hspf_ospfv2_abr_ribtable &a = *t->abr;
+    for (uint32_t i = 0; i < a.n_areas; ++i) {
+        typename OspfAbrBackboneCell<hspf::PlanesOf<R>>::Rows p;
+        if (hspf::result_planes(&planes[i], a.n_vertices[i], p) || !p.complete()) return HSPF_E_INVAL;
+        cell.s.dist[i] = p.dist; cell.s.hops[i] = p.hops; cell.s.nh[i] = p.nh; cell.s.status[i] = p.status;
+        cell.s.V[i] = p.V; cell.s.n_rows[i] = 1;
+    }
+    for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
+        cell.cells[b] = nullptr; cell.status[b] = nullptr; cell.K[b] = 0;
+        if (b >= t->n_borders) continue;
+        // the border's cells, 8-byte words of 24-byte cells
+        if (!border_cells[b] || (reinterpret_cast<uintptr_t>(border_cells[b]) & 7u)) return HSPF_E_INVAL;
+        cell.cells[b] = border_cells[b];
+        cell.status[b] = border_status ? border_status[b] : nullptr;
+        cell.K[b] = (uint32_t)t->borders[b]->prefix.size();
+    }
+    auto &s = cell.sets;
+    s.n = (uint32_t)t->asbr_set.size();
+    if (s.n && (!border_planes || !border_n_rows || (n_jobs && !border_rows))) return HSPF_E_INVAL;
+    for (uint32_t k = 0; k < s.n; ++k) {
+        const uint32_t b = t->asbr_set[k].first, i = t->asbr_set[k].second;
+        if (!border_planes[b] || !border_n_rows[b] || (n_jobs && !border_rows[b])) return HSPF_E_INVAL;
+        hspf::ResultPlanes<hspf::PlanesOf<R>> p;
+        if (hspf::result_planes(&border_planes[b][i], t->borders[b]->n_vertices[i], p) || !p.complete())
+            return HSPF_E_INVAL;
+        s.dist[k] = p.dist; s.status[k] = p.status; s.V[k] = p.V;
+        s.rows[k] = border_rows[b]; s.n_rows[k] = border_n_rows[b][i];
+        s.stride[k] = t->borders[b]->n_areas; s.area[k] = i;
+    }
+    cell.n_borders = t->n_borders;
+    cell.n_recs = t->n_recs();
+    cell.t = t->view(t->dev.off, static_cast<const hspf::RibRec *>(t->dev.contribs));
+    cell.border = t->dev.off + t->border_at();
+    return HSPF_OK;
+}
+
+template <class R>
+int abr_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
+                       const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                       const R *const *border_planes, const uint32_t *const *border_n_rows,
+                       const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    OspfAbrBackboneCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                 n_jobs, cell))
+        return rc;
+    return hspf::launch_route_cells<kAbrBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out,
+                                                             0, nullptr, nullptr, nullptr, nullptr);
+}
+
+template <class R>
+int abr_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
+                       const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                       const R *const *border_planes, const uint32_t *const *border_n_rows,
+                       const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
+                       const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                       uint64_t *n_records) {
+    OspfAbrBackboneCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                 n_jobs, cell))
+        return rc;
+    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kAbrBackboneBlocksPerSM>(
+        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+}  // namespace
+
+extern "C" {
+
+int hspf_ospfv2_abr_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_abr_backbone_table *t) {
+    if (!t || !t->abr) return HSPF_E_INVAL;
+    return hspf::upload_route_table(ctx, t->dev, t->words, t->abr->recs.data(),
+                                    t->abr->recs.size() * sizeof(hspf::RibRec));
+}
+
+int hspf_ospfv2_abr_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                   const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                   uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    return abr_backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                              border_rows, job_status_out, cells);
+}
+
+int hspf_ospfv2_abr_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                     const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                     const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                     const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                     uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+    return abr_backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                              border_rows, job_status_out, cells);
+}
+
+int hspf_ospfv2_abr_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                   const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                   uint64_t *n_records) {
+    return abr_backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                              border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+int hspf_ospfv2_abr_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                     const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                     const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                     const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                     const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                     hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                     uint64_t *n_records) {
+    return abr_backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                              border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+}
+
+}  // extern "C"

@@ -1310,6 +1310,52 @@ int hspf_ospfv2_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
 }
 
 
+/* ---- area border router over what-if jobs inside another area (ospf_backbone_cells.h) -------------- */
+
+void hspf_ospfv2_abr_backbone_table_free(hspf_ospfv2_abr_backbone_table *t) {
+    if (!t) return;
+    hspf::release_route_table(t->dev);
+    hspf_ospfv2_abr_ribtable_free(t->abr);
+    delete t;
+}
+
+int hspf_ospfv2_abr_backbone_table_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv2_flat *const *flats,
+                                          const uint32_t *area_ids, const hl_ospfv2_summary_lsa *const *summaries,
+                                          const uint32_t *n_summaries, const uint8_t *active,
+                                          const hl_ospfv2_external_lsa *ext, uint32_t n_ext,
+                                          const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                          hspf_ospfv2_abr_backbone_table **out) {
+    return hspf::build_abr_backbone_table<RibV2>(router_id, n_areas, flats, area_ids, summaries, n_summaries, active,
+                                                 ext, n_ext, borders, n_borders, out);
+}
+
+int hspf_ospfv2_abr_backbone_table_prefixes(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_prefixes,
+                                            const uint32_t **prefix, const uint32_t **plen) {
+    if (!t) return HSPF_E_INVAL;
+    if (n_prefixes) *n_prefixes = t->P();
+    if (prefix) *prefix = t->abr->prefix.data();
+    if (plen) *plen = t->abr->plen.data();
+    return HSPF_OK;
+}
+
+int hspf_ospfv2_abr_backbone_table_records(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_records,
+                                           uint32_t *n_slots, uint32_t *n_asbr_slots, uint32_t *n_asbr_sets) {
+    if (!t) return HSPF_E_INVAL;
+    if (n_records) *n_records = t->n_recs();
+    if (n_slots) *n_slots = (uint32_t)t->slot_rec.size();
+    if (n_asbr_slots) *n_asbr_slots = t->n_asbr_slots;
+    if (n_asbr_sets) *n_asbr_sets = (uint32_t)t->asbr_set.size();
+    return HSPF_OK;
+}
+
+int hspf_ospfv2_abr_backbone_from_cells(const hspf_ospfv2_abr_backbone_table *t, const hl_ospfv2_area *areas,
+                                        uint32_t n_areas, const hl_ospf_rib_cell *cells, const uint32_t *gather_area,
+                                        const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather,
+                                        hl_ospfv2_rib *out) {
+    return hspf::decode_abr_backbone_rib<RibV2>(t, areas, n_areas, cells, gather_area, gather_v, gather_nh, n_gather, out);
+}
+
+
 /* ---- trigger-keyed recomputation (holo_spf_lsdb.h) ---------------------------------------------- */
 
 int hspf_ospfv2_spf_computation_type(const hl_lsa_trigger *tr, uint32_t n, hl_spf_computation *out) {

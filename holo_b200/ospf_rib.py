@@ -814,3 +814,98 @@ def backbone_from_cells_v3(area, t: BackboneTable, cells: np.ndarray, gather_v, 
     return _call_rib(capi.load_library().hspf_ospfv3_backbone_from_cells,
                      (t.handle, C.byref(s), cells.ctypes.data, gv.ctypes.data, gn.ctypes.data, len(gv)),
                      t.n_prefixes, RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)
+
+
+# ---- area border router over what-if jobs inside another area (include/holo_spf_lsdb.h) --------------------------
+class AbrBackboneTable:
+    """hspf_ospfv2_abr_backbone_table of an area border router R of area 0 and other areas: its affected prefixes over
+    what-if jobs inside an area it is not attached to.  `router_id`, `flats`, `area_ids`, `summaries`, `active`,
+    `externals` as for AbrRibTable (area 0's summaries as in R's LSDB); `borders`: the AbrRibTables of the perturbed
+    area's ABRs attached to area 0 (kept alive with this table).  `prefix`, `plen` [n_prefixes]: the affected prefixes
+    in prefix order; a slot's winner is n_records + its slot index (n_slots in all); `n_asbr_slots` type-4 slots read
+    `n_asbr_sets` (border, area) plane sets."""
+
+    def __init__(self, router_id: int, flats: list, area_ids, summaries=None, active=None, externals=None, borders=()):
+        n = len(flats)
+        self.lib = capi.load_library()
+        self.handle = None
+        self.router_id, self.flats, self.area_ids = router_id, list(flats), [int(a) for a in area_ids]
+        self.borders = list(borders)
+        sums = [np.ascontiguousarray(s if s is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
+                for s in (summaries if summaries is not None else [None] * n)]
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        self.summaries, self.externals = sums, ext
+        self.active = [True] * n if active is None else [bool(a) for a in active]
+        self.n_areas = n
+        fl = (C.c_void_p * max(n, 1))(*[f.handle.value for f in flats])
+        ids = np.asarray(self.area_ids or [0], np.uint32)
+        sp = (C.c_void_p * max(n, 1))(*[s.ctypes.data if len(s) else None for s in sums])
+        ns = np.asarray([len(s) for s in sums] or [0], np.uint32)
+        act = np.asarray([int(a) for a in self.active] or [0], np.uint8)
+        bt = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
+        self._keep = (fl, ids, sp, ns, act, sums, ext, flats)
+        h = C.c_void_p()
+        rc = self.lib.hspf_ospfv2_abr_backbone_table_create(router_id, n, fl, ids.ctypes.data, sp, ns.ctypes.data,
+                                                            act.ctypes.data, ext.ctypes.data if len(ext) else None,
+                                                            len(ext), bt, len(self.borders), C.byref(h))
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, "hspf_ospfv2_abr_backbone_table_create failed")
+        self.handle = h
+        np_, pp, pl = C.c_uint32(), C.c_void_p(), C.c_void_p()
+        assert self.lib.hspf_ospfv2_abr_backbone_table_prefixes(h, C.byref(np_), C.byref(pp), C.byref(pl)) == capi.HSPF_OK
+        self.n_prefixes = np_.value
+        self.prefix = route_table.copy_records(pp, self.n_prefixes, np.uint32)
+        self.plen = route_table.copy_records(pl, self.n_prefixes, np.uint32)
+        c = [C.c_uint32() for _ in range(4)]
+        assert self.lib.hspf_ospfv2_abr_backbone_table_records(h, *[C.byref(x) for x in c]) == capi.HSPF_OK
+        self.n_records, self.n_slots, self.n_asbr_slots, self.n_asbr_sets = [x.value for x in c]
+
+    def upload(self, ctx: capi.Context):
+        rc = self.lib.hspf_ospfv2_abr_backbone_table_upload(ctx.handle, self.handle)
+        if rc != capi.HSPF_OK:
+            raise capi.HspfError(rc, ctx.last_error())
+
+    def __del__(self):
+        try:
+            if self.handle:
+                self.lib.hspf_ospfv2_abr_backbone_table_free(self.handle)
+                self.handle = None
+        except Exception:
+            pass
+
+
+def abr_backbone_cells_device(ctx: capi.Context, t: AbrBackboneTable, n_jobs: int, planes: list, border_cells,
+                              border_status, border_planes, border_n_rows, border_rows, status_ptr: int,
+                              cells_ptr: int):
+    """hspf_ospfv2_abr_backbone_cells / _cells16 over DEVICE planes.  planes: R's capi.ResultStruct (nh_words 1) or
+    capi.Result16Struct per area, in the table's order, only row 0 read; border_cells / border_status as
+    backbone_cells_device; border_planes / border_n_rows / border_rows as backbone_asbr_cells_device (None for a table
+    without type-4 slots); status_ptr: device u32 [n_jobs] or 0; cells_ptr: device [n_jobs, t.n_prefixes]
+    RIB_CELL_DT.  Enqueued on the ctx stream; the table must have been uploaded."""
+    keep = []
+    st = _device_ptrs(border_status) if border_status is not None else None
+    bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)
+    route_table.call_stage(ctx, "hspf_ospfv2_abr_backbone_cells", planes[0], t.handle, n_jobs, _planes_array(planes),
+                           _device_ptrs(border_cells), st, bp, bn, br, status_ptr or None, cells_ptr or None)
+
+
+def abr_backbone_delta_device(ctx: capi.Context, t: AbrBackboneTable, n_jobs: int, planes: list, border_cells,
+                              border_status, border_planes, border_n_rows, border_rows, base_ptr: int, n_base: int,
+                              base_of_ptr: int, job_out_ptr: int, records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_ospfv2_abr_backbone_delta / _delta16: the route-delta stage over the same walk (arguments as
+    abr_backbone_cells_device and rib_delta_device)."""
+    keep = []
+    st = _device_ptrs(border_status) if border_status is not None else None
+    bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)
+    route_table.call_stage(ctx, "hspf_ospfv2_abr_backbone_delta", planes[0], t.handle, n_jobs, _planes_array(planes),
+                           _device_ptrs(border_cells), st, bp, bn, br, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+
+
+def abr_backbone_from_cells(areas: list, t: AbrBackboneTable, cells: np.ndarray, gather_area, gather_v,
+                            gather_nh) -> Rib:
+    """hspf_ospfv2_abr_backbone_from_cells (host): one job's cells -> R's routes for the affected prefixes.  areas:
+    R's ospfv2.Ospfv2Area images in the table's order; gathers (area, vertex, nh_mask) of R's row 0.  rc
+    HSPF_E_UNSUPPORTED is returned in the result, as rib_from_cells."""
+    return _call_abr_rib_from_cells(capi.load_library().hspf_ospfv2_abr_backbone_from_cells, ospfv2.AreaStruct, areas,
+                                    t, cells, gather_area, gather_v, gather_nh, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)

@@ -905,6 +905,48 @@ def backbone_view(t0: Topology, t1: Topology, seed: int, r: int = 0, borders=((1
             "shared": shared, "asbr": asbr, "area1_asbrs": asbrs1}
 
 
+def abr_backbone_view(t0: Topology, t1: Topology, t2: Topology, seed: int, r: int = 0, r2: int = 0,
+                      borders=((1, 0), (2, 1), (3, 2)), max_paths: int = 16, n_ext_keys: int = 3, area1_asbrs: int = 0,
+                      area1_ext: int = 4):
+    """An area border router R of area 0 and area 2, and the borders of area 1, each as its own image: backbone_view's
+    domain (areas 0 and 1, the three borders, the area-0 ASBR, with area1_asbrs / area1_ext its area-1 ASBRs and
+    their type-5 and the borders' type-4 LSAs), with R (router r of t0) also router r2 of area 2, synth_area(t2) moved
+    into ranges of its own, and the B flag in both of R's areas.  Seeded; area 2 draws from a generator of its own.
+    Returns a dict:
+      r_areas       R's images [area 0, area 2] (area ids `area_ids` [0, 2]), `summaries` per area: backbone_view's
+                    summaries0 and none for area 2 (R is its only ABR);
+      externals     backbone_view's, plus an area-2 ASBR's ("area2_asbr", the E flag) type-5 LSAs: 0x0E0A0000/24, which
+                    the area-0 ASBR and every area-1 ASBR also advertise, and a /24 of its own;
+      area2_shared  (prefix, mask) of an area-1 stub that is also a stub of an area-2 router (intra-area at R);
+      borders, shared, asbr, area1_asbrs  as backbone_view's (R has the B flag in the borders' area-0 images)."""
+    from . import ospf_rib
+    v = backbone_view(t0, t1, seed, r=r, borders=borders, max_paths=max_paths, n_ext_keys=n_ext_keys,
+                      area1_asbrs=area1_asbrs, area1_ext=area1_ext)
+    rng = np.random.default_rng([seed, 0xAB2])
+    R = RID_BASE + int(r)
+    a2 = _set_flags(_area_remap(synth_area(t2, root=r2, max_paths=max_paths), 2, {RID_BASE + int(r2): R}), {R: 0x01})
+    fl = Flat(a2)
+    d = _dist_from(fl, fl.router_vertex(R))
+    reach = sorted(int(fl.ids[x]) for x in range(len(fl.ids)) if fl.is_router[x] and 0 < d[x] < 1 << 40)
+    t3 = v["summaries0"][v["summaries0"]["lsa_type"] == 3]
+    pick = t3[int(rng.integers(0, len(t3)))]
+    shared2 = (int(pick["lsa_id"]), int(pick["mask"]))
+    a2 = _with_stubs(a2, {reach[int(rng.integers(0, len(reach)))]: [(shared2[0], shared2[1], 1)]})
+    asbr2 = reach[int(rng.integers(0, len(reach)))]
+    a2 = _set_flags(a2, {asbr2: 0x02})
+    ext = [tuple(x) for x in v["externals"].tolist()]
+    ext += [(asbr2, 0x0E0A0000, 0xFFFFFF00, 12, 0, 12, 1, 0, (0, 0)),
+            (asbr2, 0x0E0C0000, 0xFFFFFF00, int(rng.integers(1, 40)), 0, 12, 0, 0, (0, 0))]
+    ext.sort(key=lambda x: (x[0], x[1]))
+    r_area0 = _set_flags(v["r_area"], {R: 0x01})
+    out_borders = [([_set_flags(a, {R: 0x01}) if a.area_id == 0 else a for a in areas], ids, sums)
+                   for areas, ids, sums in v["borders"]]
+    return {"r_areas": [r_area0, a2], "area_ids": [0, 2],
+            "summaries": [v["summaries0"], np.zeros(0, ospf_rib.SUMMARY_LSA_DT)],
+            "externals": np.asarray(ext, ospf_rib.EXTERNAL_LSA_DT), "area2_shared": shared2, "area2_asbr": asbr2,
+            "borders": out_borders, "shared": v["shared"], "asbr": v["asbr"], "area1_asbrs": v["area1_asbrs"]}
+
+
 def nonbackbone_view(t0: Topology, t1: Topology, seed: int, spf, r: int | None = None,
                      borders=((1, 0), (2, 1), (3, 2)), max_paths: int = 16, n_ext_keys: int = 3, n_ext: int = 0):
     """An internal router R of area 1 and the area border routers ("borders") between area 0 and area 1, each as its

@@ -177,6 +177,16 @@ def declare(lib: C.CDLL):
         "hspf_ospfv2_backbone_asbr_cells16": [vp, vp, u32, res16, pvp, pvp, pvp, pvp, pvp, vp, vp],
         "hspf_ospfv2_backbone_asbr_delta": [vp, vp, u32, res, pvp, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv2_backbone_asbr_delta16": [vp, vp, u32, res16, pvp, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_abr_backbone_table_create": [u32, u32, vp, vp, vp, vp, vp, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv2_abr_backbone_table_prefixes": [vp, u32p, pvp, pvp],
+        "hspf_ospfv2_abr_backbone_table_records": [vp, u32p, u32p, u32p, u32p],
+        "hspf_ospfv2_abr_backbone_table_upload": [vp, vp],
+        "hspf_ospfv2_abr_backbone_cells": [vp, vp, u32, vp, pvp, pvp, pvp, pvp, pvp, vp, vp],
+        "hspf_ospfv2_abr_backbone_cells16": [vp, vp, u32, vp, pvp, pvp, pvp, pvp, pvp, vp, vp],
+        "hspf_ospfv2_abr_backbone_delta": [vp, vp, u32, vp, pvp, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_abr_backbone_delta16": [vp, vp, u32, vp, pvp, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_abr_backbone_from_cells": [vp, C.POINTER(ospfv2.AreaStruct), u32, vp, vp, vp, vp, u32,
+                                                C.POINTER(ospf_rib.RibStruct)],
         "hspf_ospfv3_net_summaries": [u32, C.POINTER(ospf_rib.RibStruct), C.POINTER(ospf_rib.RibAreaStruct), vp, u32,
                                       u32, vp, u32, u32p],
         "hspf_ospfv3_rtr_summaries": [u32, C.POINTER(ospf_rib.RibAreaStruct), vp, u32, u32, vp, u32, u32p],
@@ -198,6 +208,7 @@ def declare(lib: C.CDLL):
         for name in ("prefixes", "contributors"):
             getattr(lib, f"{table}_{name}").argtypes = [vp]
             getattr(lib, f"{table}_{name}").restype = u32
-    for table in ("hspf_isis_l1_to_l2_table", "hspf_isis_backbone_table", "hspf_ospfv2_backbone_table"):
+    for table in ("hspf_isis_l1_to_l2_table", "hspf_isis_backbone_table", "hspf_ospfv2_backbone_table",
+                  "hspf_ospfv2_abr_backbone_table"):
         getattr(lib, table + "_free").argtypes = [vp]
         getattr(lib, table + "_free").restype = None

@@ -510,6 +510,97 @@ int hspf_ospfv2_nonbackbone_table_create(const hspf_ospfv2_flat *flat, uint32_t 
                                          hspf_ospfv2_backbone_table **out);
 
 /*
+ * Area border router over what-if jobs inside an area it is not attached to.  R is an ABR of area 0 and at least one
+ * more active area; a job changes costs only inside another area, whose ABRs attached to area 0 are the "borders"
+ * (1..8, each with its ABR table above).  Contract: the jobs perturb no area R is attached to, so each of R's per-area
+ * SPTs is row 0 in every job.  Every ABR of the perturbed area attached to area 0 must be given as a border: another
+ * one keeps its base LSAs as static records, and the table cannot tell.  update_rib_full at R (more than one active
+ * area) reads inter-area routes from area 0's type-3 LSAs only, and ASBR entries of the perturbed area's ASBRs from
+ * the borders' type-4 LSAs in area 0; both move with the job, R's intra-area routes do not.  The table holds R's
+ * affected prefixes: those some border can advertise into area 0 (an intra-area record in one of its non-backbone
+ * areas), and those of a usable type-5 LSA of an ASBR some border can originate a type-4 LSA for.  Every other prefix
+ * of R's table is R's base route in every job.  For job j, with border b's ABR cells of j decoded to rib_b, the
+ * decoded cells of j equal the affected-prefix routes of
+ *     hspf_ospfv2_update_rib_full(R, max_paths, [{A_i.area_id, area_from_planes(A_i, R's row 0 of A_i), ifaces,
+ *         S_i, active_i}], X)
+ * where S_i is area i's type-3/4 LSAs, area 0's with each border's type-3 and type-4 LSAs replaced by
+ * hspf_ospfv2_net_summaries(rib_b, rtrs_b, ..., target area 0), in LsaKey order.  The type-3 rule is the backbone
+ * table's, the type-4 rule the asbr table's.
+ *
+ *   hspf_ospfv2_abr_backbone_table_create  host.  The arguments of hspf_ospfv2_abr_ribtable_create (R's areas in
+ *                                instance order; area 0's summaries as in R's LSDB, borders' LSAs included), plus the
+ *                                borders' OSPFv2 ABR tables, which must outlive the table.  Per affected prefix: R's
+ *                                records as hspf_ospfv2_abr_ribtable_create's, with area 0's type-3 range holding one
+ *                                slot per (border, prefix) and each type-4 range of an ASBR some border can originate
+ *                                for one slot per (border, non-backbone area where the ASBR is an E-flag router), at
+ *                                the borders' LsaKey places.  The refusals of hspf_ospfv2_abr_ribtable_create apply,
+ *                                and: HSPF_E_INVAL R not a B-flag router vertex of its area-0 flat, area 0 missing or
+ *                                inactive, fewer than two active areas, R one of the borders, a border given twice,
+ *                                for OSPFv3, without area 0 or not a B-flag router vertex of R's area-0 flat, a usable
+ *                                type-3 / type-4 LSA of a border in area 0 it cannot originate, 0 or more than 8
+ *                                borders; HSPF_E_UNSUPPORTED a V-flag router in any of R's areas, a router with the E
+ *                                and the B flag in a border's non-backbone area, type-4 slots reading more than 8
+ *                                (border, area) plane sets, winners that do not fit.
+ *   hspf_ospfv2_abr_backbone_table_prefixes  P, and the prefixes / lengths in prefix order (pointers may be NULL).
+ *   hspf_ospfv2_abr_backbone_table_records   the record, slot, type-4 slot and plane-set counts: a slot's winner is
+ *                                n_records + its slot index.
+ *   hspf_ospfv2_abr_backbone_table_upload    copies the table to the ctx's device.
+ *   hspf_ospfv2_abr_backbone_cells[16]  one thread per (job, prefix).  planes: host array of R's n_areas plane structs
+ *                                (device, as given hspf_ospfv2_abr_rib_cells), row 0 read; border_cells /
+ *                                border_status as hspf_ospfv2_backbone_cells; border_planes / border_n_rows /
+ *                                border_rows as hspf_ospfv2_backbone_asbr_cells (NULL for a table without type-4
+ *                                slots).  job_status_out (device u32[n_jobs], may be NULL): the OR of R's row-0 words,
+ *                                the borders' job words and the words of the type-4 rows the job reads, with
+ *                                HSPF_JS_INVALID for a row out of range; a job with a non-zero word gets empty cells.
+ *                                cells[n_jobs][P] (device).  Nothing is launched for 0 jobs.  Enqueued on the ctx
+ *                                stream.
+ *   hspf_ospfv2_abr_backbone_delta[16]  the route-delta stage over the same walk (base cells as hspf_ospfv2_rib_delta).
+ *   hspf_ospfv2_abr_backbone_from_cells host: one job's cells -> exactly the routes of the affected prefixes of the
+ *                                contract.  areas / gathers as hspf_ospfv2_abr_rib_from_cells, of R's row 0.
+ */
+typedef struct hspf_ospfv2_abr_backbone_table hspf_ospfv2_abr_backbone_table;
+int hspf_ospfv2_abr_backbone_table_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv2_flat *const *flats,
+                                          const uint32_t *area_ids, const hl_ospfv2_summary_lsa *const *summaries,
+                                          const uint32_t *n_summaries, const uint8_t *active,
+                                          const hl_ospfv2_external_lsa *externals, uint32_t n_externals,
+                                          const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                          hspf_ospfv2_abr_backbone_table **out);
+void hspf_ospfv2_abr_backbone_table_free(hspf_ospfv2_abr_backbone_table *t);
+int hspf_ospfv2_abr_backbone_table_prefixes(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_prefixes,
+                                            const uint32_t **prefix, const uint32_t **plen);
+int hspf_ospfv2_abr_backbone_table_records(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_records,
+                                           uint32_t *n_slots, uint32_t *n_asbr_slots, uint32_t *n_asbr_sets);
+int hspf_ospfv2_abr_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_abr_backbone_table *t);
+int hspf_ospfv2_abr_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                   const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                   uint32_t *job_status_out, hl_ospf_rib_cell *cells);
+int hspf_ospfv2_abr_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                     const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                     const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                     const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                     uint32_t *job_status_out, hl_ospf_rib_cell *cells);
+int hspf_ospfv2_abr_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const hspf_result *const *border_planes,
+                                   const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                   uint64_t *n_records);
+int hspf_ospfv2_abr_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                     const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                     const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
+                                     const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                     const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
+                                     hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
+                                     uint64_t *n_records);
+int hspf_ospfv2_abr_backbone_from_cells(const hspf_ospfv2_abr_backbone_table *t, const hl_ospfv2_area *areas,
+                                        uint32_t n_areas, const hl_ospf_rib_cell *cells, const uint32_t *gather_area,
+                                        const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather,
+                                        hl_ospfv2_rib *out);
+
+/*
  * The same stage for OSPFv3.  The table is an hspf_ospfv2_backbone_table marked OSPFv3; the cells and delta calls
  * above take it (the table's mark picks the walk), and each version's create and decode refuse the other version's
  * tables (HSPF_E_INVAL).  For job j, with border b's ABR cells of j decoded to rib_b (hspf_ospfv3_abr_rib_from_cells),
