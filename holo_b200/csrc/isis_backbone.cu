@@ -72,25 +72,12 @@ int make_cell(const hspf_isis_backbone_table *t, const R *l2_std, const R *l2_mt
     return HSPF_OK;
 }
 
-template <class R>
-int backbone_cells(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs, const R *l2_std, const R *l2_mt6,
-                   const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
-                   uint32_t *job_status_out, hl_isis_route_cell *cells) {
+template <class R, class Out>
+int backbone(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs, const R *l2_std, const R *l2_mt6,
+             const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status, const Out &out) {
     IsisBackboneCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(t, l2_std, l2_mt6, border_cells, border_status, cell)) return rc;
-    return hspf::launch_route_cells<kBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P, cells, job_status_out, 0,
-                                                          nullptr, nullptr, nullptr, nullptr);
-}
-
-template <class R>
-int backbone_delta(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs, const R *l2_std, const R *l2_mt6,
-                   const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
-                   const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
-                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    IsisBackboneCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, l2_std, l2_mt6, border_cells, border_status, cell)) return rc;
-    return hspf::launch_route_delta<hspf::IsisCellLayout, kBackboneBlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, t->P, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return hspf::launch_route_stage<kBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P, out);
 }
 
 }  // namespace
@@ -107,14 +94,16 @@ int hspf_isis_backbone_cells(hspf_ctx *ctx, const hspf_isis_backbone_table *t, u
                              const hspf_result *l2_std, const hspf_result *l2_mt6,
                              const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
                              uint32_t *job_status_out, hl_isis_route_cell *cells) {
-    return backbone_cells(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status, job_status_out, cells);
+    return backbone(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status,
+                    hspf::CellsOut<hl_isis_route_cell>{cells, job_status_out});
 }
 
 int hspf_isis_backbone_cells16(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs,
                                const hspf_result16 *l2_std, const hspf_result16 *l2_mt6,
                                const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
                                uint32_t *job_status_out, hl_isis_route_cell *cells) {
-    return backbone_cells(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status, job_status_out, cells);
+    return backbone(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status,
+                    hspf::CellsOut<hl_isis_route_cell>{cells, job_status_out});
 }
 
 int hspf_isis_backbone_delta(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs,
@@ -122,8 +111,8 @@ int hspf_isis_backbone_delta(hspf_ctx *ctx, const hspf_isis_backbone_table *t, u
                              const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
                              const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                              hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return backbone_delta(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status, base_cells, n_base, base_of,
-                          job_out, records, cap, n_records);
+    return backbone(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status,
+                    hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_isis_backbone_delta16(hspf_ctx *ctx, const hspf_isis_backbone_table *t, uint32_t n_jobs,
@@ -131,8 +120,8 @@ int hspf_isis_backbone_delta16(hspf_ctx *ctx, const hspf_isis_backbone_table *t,
                                const hl_isis_route_cell *const *border_cells, const uint32_t *const *border_status,
                                const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return backbone_delta(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status, base_cells, n_base, base_of,
-                          job_out, records, cap, n_records);
+    return backbone(ctx, t, n_jobs, l2_std, l2_mt6, border_cells, border_status,
+                    hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

@@ -71,34 +71,15 @@ int make_cell(const hspf_isis_l1_to_l2_table *t, const R *l1_std, const R *l1_mt
     return HSPF_OK;
 }
 
-template <class R>
-int l1_to_l2_cells(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs, const R *l1_std, const R *l1_mt6,
-                   uint32_t n_rows, const uint32_t *rows, uint64_t *summary_out, uint32_t *job_status_out,
-                   hl_isis_route_cell *cells) {
+// The summary pass runs first: the call refuses its output arguments before it.
+template <class R, class Out>
+int l1_to_l2(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs, const R *l1_std, const R *l1_mt6,
+             uint32_t n_rows, const uint32_t *rows, uint64_t *summary_out, const Out &out) {
     IsisL1ToL2Cell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(t, l1_std, l1_mt6, n_rows, n_jobs, rows, summary_out, cell)) return rc;
-    if (!ctx || !cells) return HSPF_E_INVAL;                  // launch_route_cells' checks, before the first launch
+    if (const int rc = hspf::check_route_out(ctx, out, n_jobs, t->K)) return rc;
     if (const int rc = hspf::launch_isis_summaries<kL1ToL2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
-    return hspf::launch_route_cells<kL1ToL2BlocksPerSM>(ctx, t->dev, cell, n_jobs, t->K, cells, job_status_out, 0,
-                                                        nullptr, nullptr, nullptr, nullptr);
-}
-
-template <class R>
-int l1_to_l2_delta(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs, const R *l1_std, const R *l1_mt6,
-                   uint32_t n_rows, const uint32_t *rows, uint64_t *summary_out, const hl_isis_route_cell *base_cells,
-                   uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
-                   uint64_t cap, uint64_t *n_records) {
-    IsisL1ToL2Cell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, l1_std, l1_mt6, n_rows, n_jobs, rows, summary_out, cell)) return rc;
-    // launch_route_delta's checks, before the first launch
-    if (!ctx || !base_cells || !job_out || !n_records || n_base == 0 ||
-        (reinterpret_cast<uintptr_t>(base_cells) & 7u) || (reinterpret_cast<uintptr_t>(job_out) & 3u) ||
-        (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u) ||
-        !hspf::delta_batch_fits(n_jobs, t->K))
-        return HSPF_E_INVAL;
-    if (const int rc = hspf::launch_isis_summaries<kL1ToL2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
-    return hspf::launch_route_delta<hspf::IsisCellLayout, kL1ToL2BlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, t->K, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return hspf::launch_route_stage<kL1ToL2BlocksPerSM>(ctx, t->dev, cell, n_jobs, t->K, out);
 }
 
 }  // namespace
@@ -114,14 +95,16 @@ int hspf_isis_l1_to_l2_cells(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, u
                              const hspf_result *l1_std, const hspf_result *l1_mt6, uint32_t n_l1_rows,
                              const uint32_t *rows, uint64_t *summary_out, uint32_t *job_status_out,
                              hl_isis_route_cell *cells) {
-    return l1_to_l2_cells(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out, job_status_out, cells);
+    return l1_to_l2(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out,
+                    hspf::CellsOut<hl_isis_route_cell>{cells, job_status_out});
 }
 
 int hspf_isis_l1_to_l2_cells16(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs,
                                const hspf_result16 *l1_std, const hspf_result16 *l1_mt6, uint32_t n_l1_rows,
                                const uint32_t *rows, uint64_t *summary_out, uint32_t *job_status_out,
                                hl_isis_route_cell *cells) {
-    return l1_to_l2_cells(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out, job_status_out, cells);
+    return l1_to_l2(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out,
+                    hspf::CellsOut<hl_isis_route_cell>{cells, job_status_out});
 }
 
 int hspf_isis_l1_to_l2_delta(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs,
@@ -129,8 +112,8 @@ int hspf_isis_l1_to_l2_delta(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, u
                              const uint32_t *rows, uint64_t *summary_out, const hl_isis_route_cell *base_cells,
                              uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                              hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return l1_to_l2_delta(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out, base_cells, n_base, base_of,
-                          job_out, records, cap, n_records);
+    return l1_to_l2(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out,
+                    hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_isis_l1_to_l2_delta16(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t, uint32_t n_jobs,
@@ -138,8 +121,8 @@ int hspf_isis_l1_to_l2_delta16(hspf_ctx *ctx, const hspf_isis_l1_to_l2_table *t,
                                const uint32_t *rows, uint64_t *summary_out, const hl_isis_route_cell *base_cells,
                                uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                                hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return l1_to_l2_delta(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out, base_cells, n_base, base_of,
-                          job_out, records, cap, n_records);
+    return l1_to_l2(ctx, t, n_jobs, l1_std, l1_mt6, n_l1_rows, rows, summary_out,
+                    hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

@@ -77,34 +77,16 @@ int make_cell(const hspf_isis_l1l2_ribtable *t, const R *l1_std, const R *l1_mt6
     return HSPF_OK;
 }
 
-template <class R>
-int l1l2_rib_cells(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs, const R *l1_std, const R *l1_mt6,
-                   const R *l2_std, const R *l2_mt6, const uint32_t *n_rows, const uint32_t *rows, uint64_t *summary_out,
-                   uint32_t *job_status_out, hl_isis_route_cell *cells) {
+// The summary pass runs first: the call refuses its output arguments before it.
+template <class R, class Out>
+int l1l2_rib(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs, const R *l1_std, const R *l1_mt6,
+             const R *l2_std, const R *l2_mt6, const uint32_t *n_rows, const uint32_t *rows, uint64_t *summary_out,
+             const Out &out) {
     IsisL1L2Cell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(t, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, n_jobs, rows, summary_out, cell)) return rc;
-    if (!ctx || !cells) return HSPF_E_INVAL;                  // launch_route_cells' checks, before the first launch
+    if (const int rc = hspf::check_route_out(ctx, out, n_jobs, t->P)) return rc;
     if (const int rc = hspf::launch_isis_summaries<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
-    return hspf::launch_route_cells<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P, cells, job_status_out, 0, nullptr,
-                                                      nullptr, nullptr, nullptr);
-}
-
-template <class R>
-int l1l2_rib_delta(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs, const R *l1_std, const R *l1_mt6,
-                   const R *l2_std, const R *l2_mt6, const uint32_t *n_rows, const uint32_t *rows, uint64_t *summary_out,
-                   const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
-                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    IsisL1L2Cell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, n_jobs, rows, summary_out, cell)) return rc;
-    // launch_route_delta's checks, before the first launch
-    if (!ctx || !base_cells || !job_out || !n_records || n_base == 0 ||
-        (reinterpret_cast<uintptr_t>(base_cells) & 7u) || (reinterpret_cast<uintptr_t>(job_out) & 3u) ||
-        (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u) ||
-        !hspf::delta_batch_fits(n_jobs, t->P))
-        return HSPF_E_INVAL;
-    if (const int rc = hspf::launch_isis_summaries<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, summary_out)) return rc;
-    return hspf::launch_route_delta<hspf::IsisCellLayout, kL1L2BlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, t->P, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return hspf::launch_route_stage<kL1L2BlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P, out);
 }
 
 }  // namespace
@@ -120,14 +102,16 @@ int hspf_isis_l1l2_rib_cells(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, ui
                              const hspf_result *l1_mt6, const hspf_result *l2_std, const hspf_result *l2_mt6,
                              const uint32_t *n_rows, const uint32_t *rows, uint64_t *summary_out,
                              uint32_t *job_status_out, hl_isis_route_cell *cells) {
-    return l1l2_rib_cells(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out, job_status_out, cells);
+    return l1l2_rib(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out,
+                    hspf::CellsOut<hl_isis_route_cell>{cells, job_status_out});
 }
 
 int hspf_isis_l1l2_rib_cells16(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs,
                                const hspf_result16 *l1_std, const hspf_result16 *l1_mt6, const hspf_result16 *l2_std,
                                const hspf_result16 *l2_mt6, const uint32_t *n_rows, const uint32_t *rows,
                                uint64_t *summary_out, uint32_t *job_status_out, hl_isis_route_cell *cells) {
-    return l1l2_rib_cells(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out, job_status_out, cells);
+    return l1l2_rib(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out,
+                    hspf::CellsOut<hl_isis_route_cell>{cells, job_status_out});
 }
 
 int hspf_isis_l1l2_rib_delta(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs, const hspf_result *l1_std,
@@ -135,8 +119,8 @@ int hspf_isis_l1l2_rib_delta(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, ui
                              const uint32_t *n_rows, const uint32_t *rows, uint64_t *summary_out,
                              const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                              hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return l1l2_rib_delta(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out, base_cells, n_base,
-                          base_of, job_out, records, cap, n_records);
+    return l1l2_rib(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out,
+                    hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_isis_l1l2_rib_delta16(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, uint32_t n_jobs,
@@ -145,8 +129,8 @@ int hspf_isis_l1l2_rib_delta16(hspf_ctx *ctx, const hspf_isis_l1l2_ribtable *t, 
                                uint64_t *summary_out, const hl_isis_route_cell *base_cells, uint32_t n_base,
                                const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
                                uint64_t cap, uint64_t *n_records) {
-    return l1l2_rib_delta(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out, base_cells, n_base,
-                          base_of, job_out, records, cap, n_records);
+    return l1l2_rib(ctx, t, n_jobs, l1_std, l1_mt6, l2_std, l2_mt6, n_rows, rows, summary_out,
+                    hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

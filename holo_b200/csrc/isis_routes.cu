@@ -40,26 +40,15 @@ int make_cell(const hspf_isis_rtable *rt, const R *std_planes, const R *mt6_plan
     return HSPF_OK;
 }
 
-// The cell kernel keeps __launch_bounds__(256) with no minimum (a minimum of 0); the grid is one wave of 8 blocks
-// per SM, as for the OSPF stage.
-template <class R>
-int routes_batch(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const R *std_planes, const R *mt6_planes,
-                 hl_isis_route_cell *cells) {
+// The cell kernel keeps __launch_bounds__(256) with no minimum (a minimum of 0), the delta passes a minimum of 1;
+// the grid is one wave of 8 blocks per SM, as for the OSPF stage.
+template <class R, class Out>
+int routes(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const R *std_planes, const R *mt6_planes,
+           const Out &out) {
     IsisCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(rt, std_planes, mt6_planes, cell)) return rc;
-    return hspf::launch_route_cells<0, hspf::kRouteBlocksPerSM>(ctx, rt->dev, cell, n_jobs, (uint32_t)rt->prefix.size(),
-                                                                cells, nullptr, 0, nullptr, nullptr, nullptr, nullptr);
-}
-
-template <class R>
-int routes_delta(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const R *std_planes, const R *mt6_planes,
-                 const hl_isis_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
-                 hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    IsisCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(rt, std_planes, mt6_planes, cell)) return rc;
-    return hspf::launch_route_delta<hspf::IsisCellLayout, 1, hspf::kRouteBlocksPerSM>(
-        ctx, rt->dev, cell, n_jobs, (uint32_t)rt->prefix.size(), base_cells, n_base, base_of, job_out, records, cap,
-        n_records);
+    return hspf::launch_route_stage<Out::kDelta ? 1 : 0, hspf::kRouteBlocksPerSM>(ctx, rt->dev, cell, n_jobs,
+                                                                                (uint32_t)rt->prefix.size(), out);
 }
 
 }  // namespace
@@ -73,26 +62,28 @@ int hspf_isis_rtable_upload(hspf_ctx *ctx, hspf_isis_rtable *rt) {
 
 int hspf_isis_routes_batch(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result *std_planes,
                            const hspf_result *mt6_planes, hl_isis_route_cell *cells) {
-    return routes_batch(ctx, rt, n_jobs, std_planes, mt6_planes, cells);
+    return routes(ctx, rt, n_jobs, std_planes, mt6_planes, hspf::CellsOut<hl_isis_route_cell>{cells, nullptr});
 }
 
 int hspf_isis_routes_batch16(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result16 *std_planes,
                              const hspf_result16 *mt6_planes, hl_isis_route_cell *cells) {
-    return routes_batch(ctx, rt, n_jobs, std_planes, mt6_planes, cells);
+    return routes(ctx, rt, n_jobs, std_planes, mt6_planes, hspf::CellsOut<hl_isis_route_cell>{cells, nullptr});
 }
 
 int hspf_isis_routes_delta(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result *std_planes,
                            const hspf_result *mt6_planes, const hl_isis_route_cell *base_cells, uint32_t n_base,
                            const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                            uint64_t *n_records) {
-    return routes_delta(ctx, rt, n_jobs, std_planes, mt6_planes, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return routes(ctx, rt, n_jobs, std_planes, mt6_planes,
+                  hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_isis_routes_delta16(hspf_ctx *ctx, const hspf_isis_rtable *rt, uint32_t n_jobs, const hspf_result16 *std_planes,
                              const hspf_result16 *mt6_planes, const hl_isis_route_cell *base_cells, uint32_t n_base,
                              const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                              uint64_t *n_records) {
-    return routes_delta(ctx, rt, n_jobs, std_planes, mt6_planes, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return routes(ctx, rt, n_jobs, std_planes, mt6_planes,
+                  hspf::DeltaOut<hl_isis_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

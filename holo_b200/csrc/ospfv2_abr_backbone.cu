@@ -11,6 +11,7 @@
 
 #include "../../include/holo_spf_lsdb.h"
 #include "ospf_backbone_cells.h"
+#include "ospf_border_bind.cuh"
 #include "route_stage.cuh"
 
 namespace {
@@ -68,61 +69,25 @@ int make_cell(const hspf_ospfv2_abr_backbone_table *t, const R *planes, const hl
         cell.s.dist[i] = p.dist; cell.s.hops[i] = p.hops; cell.s.nh[i] = p.nh; cell.s.status[i] = p.status;
         cell.s.V[i] = p.V; cell.s.n_rows[i] = 1;
     }
-    for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
-        cell.cells[b] = nullptr; cell.status[b] = nullptr; cell.K[b] = 0;
-        if (b >= t->n_borders) continue;
-        // the border's cells, 8-byte words of 24-byte cells
-        if (!border_cells[b] || (reinterpret_cast<uintptr_t>(border_cells[b]) & 7u)) return HSPF_E_INVAL;
-        cell.cells[b] = border_cells[b];
-        cell.status[b] = border_status ? border_status[b] : nullptr;
-        cell.K[b] = (uint32_t)t->borders[b]->prefix.size();
-    }
-    auto &s = cell.sets;
-    s.n = (uint32_t)t->asbr_set.size();
-    if (s.n && (!border_planes || !border_n_rows || (n_jobs && !border_rows))) return HSPF_E_INVAL;
-    for (uint32_t k = 0; k < s.n; ++k) {
-        const uint32_t b = t->asbr_set[k].first, i = t->asbr_set[k].second;
-        if (!border_planes[b] || !border_n_rows[b] || (n_jobs && !border_rows[b])) return HSPF_E_INVAL;
-        hspf::ResultPlanes<hspf::PlanesOf<R>> p;
-        if (hspf::result_planes(&border_planes[b][i], t->borders[b]->n_vertices[i], p) || !p.complete())
-            return HSPF_E_INVAL;
-        s.dist[k] = p.dist; s.status[k] = p.status; s.V[k] = p.V;
-        s.rows[k] = border_rows[b]; s.n_rows[k] = border_n_rows[b][i];
-        s.stride[k] = t->borders[b]->n_areas; s.area[k] = i;
-    }
-    cell.n_borders = t->n_borders;
+    if (const int rc = hspf::bind_ospf_borders(*t, border_cells, border_status, cell)) return rc;
+    if (const int rc = hspf::bind_ospf_asbr_sets(*t, border_planes, border_n_rows, border_rows, n_jobs, cell))
+        return rc;
     cell.n_recs = t->n_recs();
     cell.t = t->view(t->dev.off, static_cast<const hspf::RibRec *>(t->dev.contribs));
     cell.border = t->dev.off + t->border_at();
     return HSPF_OK;
 }
 
-template <class R>
-int abr_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
-                       const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                       const R *const *border_planes, const uint32_t *const *border_n_rows,
-                       const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+template <class R, class Out>
+int abr_backbone(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
+                 const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                 const R *const *border_planes, const uint32_t *const *border_n_rows,
+                 const uint32_t *const *border_rows, const Out &out) {
     OspfAbrBackboneCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                                  n_jobs, cell))
         return rc;
-    return hspf::launch_route_cells<kAbrBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out,
-                                                             0, nullptr, nullptr, nullptr, nullptr);
-}
-
-template <class R>
-int abr_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
-                       const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                       const R *const *border_planes, const uint32_t *const *border_n_rows,
-                       const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
-                       const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
-                       uint64_t *n_records) {
-    OspfAbrBackboneCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                 n_jobs, cell))
-        return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kAbrBackboneBlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return hspf::launch_route_stage<kAbrBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), out);
 }
 
 }  // namespace
@@ -140,8 +105,8 @@ int hspf_ospfv2_abr_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone
                                    const uint32_t *const *border_status, const hspf_result *const *border_planes,
                                    const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                    uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return abr_backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                              border_rows, job_status_out, cells);
+    return abr_backbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                        hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_abr_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
@@ -149,8 +114,8 @@ int hspf_ospfv2_abr_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbo
                                      const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
                                      const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                      uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return abr_backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                              border_rows, job_status_out, cells);
+    return abr_backbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                        hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_abr_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
@@ -160,8 +125,8 @@ int hspf_ospfv2_abr_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone
                                    const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                    hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                                    uint64_t *n_records) {
-    return abr_backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                              border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return abr_backbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                        hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_abr_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
@@ -171,8 +136,8 @@ int hspf_ospfv2_abr_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbo
                                      const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                      hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                                      uint64_t *n_records) {
-    return abr_backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                              border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return abr_backbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                        hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

@@ -60,25 +60,14 @@ int make_cell(const hspf_ospfv2_abr_ribtable *t, const R *pl, const uint32_t *n_
     return HSPF_OK;
 }
 
-template <class R>
-int abr_rib_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs, const R *pl, const uint32_t *n_rows,
-                  const uint32_t *rows, hl_ospf_rib_cell *cells, uint32_t *status_out, uint32_t n_gather,
-                  const uint32_t *gather_job, const uint32_t *gather_area, const uint32_t *gather_v, uint64_t *gather_nh) {
-    if (n_gather && !gather_area) return HSPF_E_INVAL;
+template <class R, class Out>
+int abr_rib(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs, const R *pl, const uint32_t *n_rows,
+            const uint32_t *rows, const Out &out) {
+    if constexpr (!Out::kDelta)
+        if (out.n_gather && !out.gather_area) return HSPF_E_INVAL;     // a gather names the area of its vertex
     AbrRibCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(t, pl, n_rows, n_jobs, rows, cell)) return rc;
-    return hspf::launch_route_cells<kAbrBlocksPerSM>(ctx, t->dev, cell, n_jobs, cell.t.P, cells, status_out, n_gather,
-                                                     gather_job, gather_area, gather_v, gather_nh);
-}
-
-template <class R>
-int abr_rib_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs, const R *pl, const uint32_t *n_rows,
-                  const uint32_t *rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
-                  hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    AbrRibCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, pl, n_rows, n_jobs, rows, cell)) return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kAbrBlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, cell.t.P, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return hspf::launch_route_stage<kAbrBlocksPerSM>(ctx, t->dev, cell, n_jobs, cell.t.P, out);
 }
 
 }  // namespace
@@ -99,8 +88,9 @@ int hspf_ospfv2_abr_rib_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, 
                               const uint32_t *n_rows, const uint32_t *rows, hl_ospf_rib_cell *cells,
                               uint32_t *job_status_out, uint32_t n_gather, const uint32_t *gather_job,
                               const uint32_t *gather_area, const uint32_t *gather_v, uint64_t *gather_nh) {
-    return abr_rib_cells(ctx, t, n_jobs, pl, n_rows, rows, cells, job_status_out, n_gather, gather_job, gather_area,
-                         gather_v, gather_nh);
+    return abr_rib(ctx, t, n_jobs, pl, n_rows, rows,
+                   hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out, n_gather, gather_job, gather_area, gather_v,
+                                                    gather_nh});
 }
 
 int hspf_ospfv2_abr_rib_cells16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs,
@@ -108,22 +98,25 @@ int hspf_ospfv2_abr_rib_cells16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t
                                 hl_ospf_rib_cell *cells, uint32_t *job_status_out, uint32_t n_gather,
                                 const uint32_t *gather_job, const uint32_t *gather_area, const uint32_t *gather_v,
                                 uint64_t *gather_nh) {
-    return abr_rib_cells(ctx, t, n_jobs, pl, n_rows, rows, cells, job_status_out, n_gather, gather_job, gather_area,
-                         gather_v, gather_nh);
+    return abr_rib(ctx, t, n_jobs, pl, n_rows, rows,
+                   hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out, n_gather, gather_job, gather_area, gather_v,
+                                                    gather_nh});
 }
 
 int hspf_ospfv2_abr_rib_delta(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs, const hspf_result *pl,
                               const uint32_t *n_rows, const uint32_t *rows, const hl_ospf_rib_cell *base_cells,
                               uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                               hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return abr_rib_delta(ctx, t, n_jobs, pl, n_rows, rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return abr_rib(ctx, t, n_jobs, pl, n_rows, rows,
+                   hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_abr_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_abr_ribtable *t, uint32_t n_jobs,
                                 const hspf_result16 *pl, const uint32_t *n_rows, const uint32_t *rows,
                                 const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                 hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return abr_rib_delta(ctx, t, n_jobs, pl, n_rows, rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return abr_rib(ctx, t, n_jobs, pl, n_rows, rows,
+                   hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

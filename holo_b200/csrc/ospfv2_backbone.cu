@@ -13,6 +13,7 @@
 
 #include "../../include/holo_spf_lsdb.h"
 #include "ospf_backbone_cells.h"
+#include "ospf_border_bind.cuh"
 #include "route_stage.cuh"
 
 namespace {
@@ -122,205 +123,75 @@ int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_osp
               const uint32_t *const *border_status, OspfBackboneCell<hspf::PlanesOf<R>, kV3> &cell) {
     if (!t || !t->dev.blob || !border_cells) return HSPF_E_INVAL;
     if (hspf::result_planes(planes, t->n_vertices, cell.pl) || !cell.pl.complete()) return HSPF_E_INVAL;
-    for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
-        cell.cells[b] = nullptr; cell.status[b] = nullptr; cell.K[b] = 0;
-        if (b >= t->n_borders) continue;
-        // the border's cells, 8-byte words of 24-byte cells
-        if (!border_cells[b] || (reinterpret_cast<uintptr_t>(border_cells[b]) & 7u)) return HSPF_E_INVAL;
-        cell.cells[b] = border_cells[b];
-        cell.status[b] = border_status ? border_status[b] : nullptr;
-        cell.K[b] = (uint32_t)t->borders[b]->prefix.size();
-    }
-    cell.n_borders = t->n_borders;
+    if (const int rc = hspf::bind_ospf_borders(*t, border_cells, border_status, cell)) return rc;
     cell.t = t->view(t->dev.off, static_cast<const hspf::RibRec *>(t->dev.contribs));
     return HSPF_OK;
 }
 
-template <bool kV3, class R>
-int version_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+template <bool kV3, class R, class Out>
+int version(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+            const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status, const Out &out) {
     constexpr uint32_t kBlocks = kV3 ? kBackboneV3BlocksPerSM : kBackboneBlocksPerSM;
     OspfBackboneCell<hspf::PlanesOf<R>, kV3> cell{};
     if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    return hspf::launch_route_cells<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out, 0, nullptr,
-                                             nullptr, nullptr, nullptr);
+    return hspf::launch_route_stage<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
 }
 
-template <bool kV3, class R>
-int version_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
-                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    constexpr uint32_t kBlocks = kV3 ? kBackboneV3BlocksPerSM : kBackboneBlocksPerSM;
-    OspfBackboneCell<hspf::PlanesOf<R>, kV3> cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBlocks>(
-        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
-}
-
-// The cell over a table with type-4 slots: the plane sets the slots name, from each border's planes, row counts and
-// rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when it names none.  An OSPFv3
-// table of area 0 is taken only from hspf_ospfv3_backbone_asbr_table_create (Inter-Area-Router slots).
-template <class R>
-int make_asbr_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
-                   const uint32_t *const *border_status, const R *const *border_planes,
-                   const uint32_t *const *border_n_rows, const uint32_t *const *border_rows, uint32_t n_jobs,
-                   OspfBackboneAsbrCell<hspf::PlanesOf<R>> &cell) {
-    if (!t || (t->v3 && !t->area_id && !t->asbr)) return HSPF_E_INVAL;
-    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    auto &s = cell.sets;
-    s.n = (uint32_t)t->asbr_set.size();
-    if (s.n && (!border_planes || !border_n_rows || (n_jobs && !border_rows))) return HSPF_E_INVAL;
-    for (uint32_t k = 0; k < s.n; ++k) {
-        const uint32_t b = t->asbr_set[k].first, i = t->asbr_set[k].second;
-        if (!border_planes[b] || !border_n_rows[b] || (n_jobs && !border_rows[b])) return HSPF_E_INVAL;
-        hspf::ResultPlanes<hspf::PlanesOf<R>> p;
-        if (hspf::result_planes(&border_planes[b][i], t->borders[b]->n_vertices[i], p) || !p.complete())
-            return HSPF_E_INVAL;
-        s.dist[k] = p.dist; s.status[k] = p.status; s.V[k] = p.V;
-        s.rows[k] = border_rows[b]; s.n_rows[k] = border_n_rows[b][i];
-        s.stride[k] = t->borders[b]->n_areas; s.area[k] = i;
-    }
-    return HSPF_OK;
-}
-
-// The launch of a walk over a table with type-4 / Inter-Area-Router slots or of a non-backbone target area (Cell).
-template <class Cell, uint32_t kBlocks, class R>
-int asbr_cells_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   const R *const *border_planes, const uint32_t *const *border_n_rows,
-                   const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+// The launch of a walk over a table with type-4 / Inter-Area-Router slots or of a non-backbone target area (Cell):
+// the cell above plus the plane sets the slots name.
+template <class Cell, uint32_t kBlocks, class R, class Out>
+int asbr_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+            const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+            const R *const *border_planes, const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+            const Out &out) {
     Cell cell{};
-    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                      n_jobs, cell))
+    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
+    if (const int rc = hspf::bind_ospf_asbr_sets(*t, border_planes, border_n_rows, border_rows, n_jobs, cell))
         return rc;
-    return hspf::launch_route_cells<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out, 0, nullptr,
-                                             nullptr, nullptr, nullptr);
-}
-
-template <class Cell, uint32_t kBlocks, class R>
-int asbr_delta_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   const R *const *border_planes, const uint32_t *const *border_n_rows,
-                   const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
-                   const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
-                   uint64_t *n_records) {
-    Cell cell{};
-    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                      n_jobs, cell))
-        return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBlocks>(
-        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return hspf::launch_route_stage<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
 }
 
 // a table of a non-backbone target area: the walk of its version
-template <class R>
-int nonbackbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                      const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                      const R *const *border_planes, const uint32_t *const *border_n_rows,
-                      const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+template <class R, class Out>
+int nonbackbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                const R *const *border_planes, const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                const Out &out) {
     using P = hspf::PlanesOf<R>;
-    return t->v3 ? asbr_cells_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                       job_status_out, cells)
-                 : asbr_cells_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                       job_status_out, cells);
+    return t->v3 ? asbr_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out)
+                 : asbr_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out);
 }
 
-template <class R>
-int nonbackbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                      const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                      const R *const *border_planes, const uint32_t *const *border_n_rows,
-                      const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
-                      const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
-                      uint64_t *n_records) {
-    using P = hspf::PlanesOf<R>;
-    return t->v3 ? asbr_delta_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                       base_cells, n_base, base_of, job_out, records, cap, n_records)
-                 : asbr_delta_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                       base_cells, n_base, base_of, job_out, records, cap, n_records);
-}
-
-// the walk of the table's version and target area; a table with type-4 slots is the asbr calls'
-template <class R>
-int backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+// the walk of the table's version and target area; a table with type-4 slots is backbone_asbr's
+template <class R, class Out>
+int backbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+             const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status, const Out &out) {
     if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
     if (t->area_id)
-        return nonbackbone_cells<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr,
-                                    job_status_out, cells);
-    return t->v3 ? version_cells<true>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells)
-                 : version_cells<false>(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+        return nonbackbone<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr, out);
+    return t->v3 ? version<true>(ctx, t, n_jobs, planes, border_cells, border_status, out)
+                 : version<false>(ctx, t, n_jobs, planes, border_cells, border_status, out);
 }
 
-template <class R>
-int backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                   const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
-                   hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
-    if (t->area_id)
-        return nonbackbone_delta<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr,
-                                    base_cells, n_base, base_of, job_out, records, cap, n_records);
-    return t->v3 ? version_delta<true>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of,
-                                        job_out, records, cap, n_records)
-                 : version_delta<false>(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base,
-                                         base_of, job_out, records, cap, n_records);
-}
-
-// A table without type-4 slots takes the calls above (NULL border planes allowed).  An OSPFv3 table of area 0 is
-// refused unless hspf_ospfv3_backbone_asbr_table_create made it.
-template <class R>
-int backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                        const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                        const R *const *border_planes, const uint32_t *const *border_n_rows,
-                        const uint32_t *const *border_rows, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
+// A table without type-4 slots takes backbone (NULL border planes allowed).  An OSPFv3 table of area 0 is refused
+// unless hspf_ospfv3_backbone_asbr_table_create made it.
+template <class R, class Out>
+int backbone_asbr(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+                  const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                  const R *const *border_planes, const uint32_t *const *border_n_rows,
+                  const uint32_t *const *border_rows, const Out &out) {
     if (!t || (t->v3 && !t->area_id && !t->asbr)) return HSPF_E_INVAL;
     if (t->area_id)
-        return nonbackbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                                 border_rows, job_status_out, cells);
-    if (!t->n_asbr_slots) return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
-    if (t->v3)
-        return asbr_cells_as<OspfBackboneAsbrV3Cell<hspf::PlanesOf<R>>, kBackboneAsbrV3BlocksPerSM>(
-            ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-            job_status_out, cells);
-    OspfBackboneAsbrCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                      n_jobs, cell))
-        return rc;
-    return hspf::launch_route_cells<kBackboneAsbrBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), cells, job_status_out,
-                                                              0, nullptr, nullptr, nullptr, nullptr);
-}
-
-template <class R>
-int backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                        const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                        const R *const *border_planes, const uint32_t *const *border_n_rows,
-                        const uint32_t *const *border_rows, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
-                        const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
-                        uint64_t *n_records) {
-    if (!t || (t->v3 && !t->area_id && !t->asbr)) return HSPF_E_INVAL;
-    if (t->area_id)
-        return nonbackbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                                 border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
-    if (!t->n_asbr_slots)
-        return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
-                              records, cap, n_records);
-    if (t->v3)
-        return asbr_delta_as<OspfBackboneAsbrV3Cell<hspf::PlanesOf<R>>, kBackboneAsbrV3BlocksPerSM>(
-            ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, base_cells,
-            n_base, base_of, job_out, records, cap, n_records);
-    OspfBackboneAsbrCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_asbr_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                      n_jobs, cell))
-        return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kBackboneAsbrBlocksPerSM>(
-        ctx, t->dev, cell, n_jobs, t->P(), base_cells, n_base, base_of, job_out, records, cap, n_records);
+        return nonbackbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                           border_rows, out);
+    if (!t->n_asbr_slots) return backbone(ctx, t, n_jobs, planes, border_cells, border_status, out);
+    using P = hspf::PlanesOf<R>;
+    return t->v3 ? asbr_as<OspfBackboneAsbrV3Cell<P>, kBackboneAsbrV3BlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out)
+                 : asbr_as<OspfBackboneAsbrCell<P>, kBackboneAsbrBlocksPerSM>(
+                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out);
 }
 
 }  // namespace
@@ -335,13 +206,15 @@ int hspf_ospfv2_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_backbone_table 
 int hspf_ospfv2_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
                                const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
                                const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
+                    hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
                                  const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
                                  const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone_cells(ctx, t, n_jobs, planes, border_cells, border_status, job_status_out, cells);
+    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
+                    hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -349,8 +222,8 @@ int hspf_ospfv2_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *
                                const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
                                const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
                                uint64_t cap, uint64_t *n_records) {
-    return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
-                          records, cap, n_records);
+    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
+                    hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -358,8 +231,8 @@ int hspf_ospfv2_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table
                                  const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells,
                                  uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                                  hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return backbone_delta(ctx, t, n_jobs, planes, border_cells, border_status, base_cells, n_base, base_of, job_out,
-                          records, cap, n_records);
+    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
+                    hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -367,8 +240,8 @@ int hspf_ospfv2_backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_ta
                                     const uint32_t *const *border_status, const hspf_result *const *border_planes,
                                     const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                     uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone_asbr_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                               border_rows, job_status_out, cells);
+    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                         hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_asbr_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -376,8 +249,8 @@ int hspf_ospfv2_backbone_asbr_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_
                                       const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
                                       const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                       uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone_asbr_cells(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                               border_rows, job_status_out, cells);
+    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                         hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -387,8 +260,8 @@ int hspf_ospfv2_backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_ta
                                     const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                     hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                                     uint64_t *n_records) {
-    return backbone_asbr_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                               border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                         hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -398,8 +271,8 @@ int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_
                                       const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                       hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                                       uint64_t *n_records) {
-    return backbone_asbr_delta(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                               border_rows, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                         hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

@@ -49,30 +49,19 @@ int make_cell(const hspf_ospfv2_ribtable *rt, const R *pl, uint32_t n_jobs, cons
     return HSPF_OK;
 }
 
-// The cell kernel runs under the route kernels' bound of 8 blocks per SM (see DESIGN.md §4.4 for its registers).
-template <class R>
-int rib_cells(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const R *pl, const uint32_t *roots,
-              hl_ospf_rib_cell *cells, uint32_t *status_out, uint32_t n_gather, const uint32_t *gather_job,
-              const uint32_t *gather_v, uint64_t *gather_nh) {
-    OspfRibCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(rt, pl, n_jobs, roots, cell)) return rc;
-    return hspf::launch_route_cells<hspf::kRouteBlocksPerSM>(ctx, rt->dev, cell, n_jobs, cell.t.P, cells, status_out,
-                                                             n_gather, gather_job, nullptr, gather_v, gather_nh);
-}
-
 // Blocks per SM of the route-delta passes over this walk: their launch bound and their grid.  At the cell kernels'
 // 8 the walk plus the base compare spills 68 bytes in pass A; from 5 down neither pass spills, and of the bounds
 // timed on an H100 this one was fastest (DESIGN.md §4.4, §6).
 constexpr uint32_t kRibDeltaBlocksPerSM = 4;
 
-template <class R>
-int rib_delta(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const R *pl, const uint32_t *roots,
-              const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
-              hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+// The cell kernel runs under the route kernels' bound of 8 blocks per SM (see DESIGN.md §4.4 for its registers).
+template <class R, class Out>
+int rib(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const R *pl, const uint32_t *roots,
+        const Out &out) {
+    constexpr uint32_t kBlocks = Out::kDelta ? kRibDeltaBlocksPerSM : hspf::kRouteBlocksPerSM;
     OspfRibCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(rt, pl, n_jobs, roots, cell)) return rc;
-    return hspf::launch_route_delta<hspf::OspfRibCellLayout, kRibDeltaBlocksPerSM>(
-        ctx, rt->dev, cell, n_jobs, cell.t.P, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return hspf::launch_route_stage<kBlocks>(ctx, rt->dev, cell, n_jobs, cell.t.P, out);
 }
 
 }  // namespace
@@ -91,27 +80,31 @@ int hspf_ospfv2_ribtable_upload(hspf_ctx *ctx, hspf_ospfv2_ribtable *rt) {
 int hspf_ospfv2_rib_cells(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result *pl,
                           const uint32_t *roots, hl_ospf_rib_cell *cells, uint32_t *job_status_out, uint32_t n_gather,
                           const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh) {
-    return rib_cells(ctx, rt, n_jobs, pl, roots, cells, job_status_out, n_gather, gather_job, gather_v, gather_nh);
+    return rib(ctx, rt, n_jobs, pl, roots,
+               hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out, n_gather, gather_job, nullptr, gather_v, gather_nh});
 }
 
 int hspf_ospfv2_rib_cells16(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
                             const uint32_t *roots, hl_ospf_rib_cell *cells, uint32_t *job_status_out, uint32_t n_gather,
                             const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh) {
-    return rib_cells(ctx, rt, n_jobs, pl, roots, cells, job_status_out, n_gather, gather_job, gather_v, gather_nh);
+    return rib(ctx, rt, n_jobs, pl, roots,
+               hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out, n_gather, gather_job, nullptr, gather_v, gather_nh});
 }
 
 int hspf_ospfv2_rib_delta(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result *pl,
                           const uint32_t *roots, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
                           const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                           uint64_t *n_records) {
-    return rib_delta(ctx, rt, n_jobs, pl, roots, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return rib(ctx, rt, n_jobs, pl, roots,
+               hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_rib_delta16(hspf_ctx *ctx, const hspf_ospfv2_ribtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
                             const uint32_t *roots, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
                             const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                             uint64_t *n_records) {
-    return rib_delta(ctx, rt, n_jobs, pl, roots, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return rib(ctx, rt, n_jobs, pl, roots,
+               hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

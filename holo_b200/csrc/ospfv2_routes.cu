@@ -46,25 +46,12 @@ int make_cell(const hspf_ospfv2_rtable *rt, const R *pl, OspfCell<hspf::PlanesOf
 
 // Both the cell kernel and the route-delta passes are bounded to 8 blocks per SM: the walk stays in 32 registers
 // (with a few bytes of spill in delta pass A), so the grid of one wave is resident at once.
-template <class R>
-int routes_batch(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const R *pl, hl_route_cell *cells,
-                 uint32_t n_gather, const uint32_t *gather_job, const uint32_t *gather_v, uint64_t *gather_nh) {
+template <class R, class Out>
+int routes(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const R *pl, const Out &out) {
     OspfCell<hspf::PlanesOf<R>> cell{};
     if (const int rc = make_cell(rt, pl, cell)) return rc;
-    return hspf::launch_route_cells<hspf::kRouteBlocksPerSM>(ctx, rt->dev, cell, n_jobs, (uint32_t)rt->t.prefix.size(),
-                                                             cells, nullptr, n_gather, gather_job, nullptr, gather_v,
-                                                             gather_nh);
-}
-
-template <class R>
-int routes_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const R *pl,
-                 const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
-                 hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    OspfCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(rt, pl, cell)) return rc;
-    return hspf::launch_route_delta<hspf::OspfCellLayout, hspf::kRouteBlocksPerSM>(
-        ctx, rt->dev, cell, n_jobs, (uint32_t)rt->t.prefix.size(), base_cells, n_base, base_of, job_out, records, cap,
-        n_records);
+    return hspf::launch_route_stage<hspf::kRouteBlocksPerSM>(ctx, rt->dev, cell, n_jobs, (uint32_t)rt->t.prefix.size(),
+                                                             out);
 }
 
 struct DevBuf {
@@ -86,25 +73,29 @@ int hspf_ospfv2_rtable_upload(hspf_ctx *ctx, hspf_ospfv2_rtable *rt) {
 int hspf_ospfv2_routes_batch(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result *pl,
                              hl_route_cell *cells, uint32_t n_gather, const uint32_t *gather_job,
                              const uint32_t *gather_v, uint64_t *gather_nh) {
-    return routes_batch(ctx, rt, n_jobs, pl, cells, n_gather, gather_job, gather_v, gather_nh);
+    return routes(ctx, rt, n_jobs, pl,
+                  hspf::CellsOut<hl_route_cell>{cells, nullptr, n_gather, gather_job, nullptr, gather_v, gather_nh});
 }
 
 int hspf_ospfv2_routes_batch16(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
                                hl_route_cell *cells, uint32_t n_gather, const uint32_t *gather_job,
                                const uint32_t *gather_v, uint64_t *gather_nh) {
-    return routes_batch(ctx, rt, n_jobs, pl, cells, n_gather, gather_job, gather_v, gather_nh);
+    return routes(ctx, rt, n_jobs, pl,
+                  hspf::CellsOut<hl_route_cell>{cells, nullptr, n_gather, gather_job, nullptr, gather_v, gather_nh});
 }
 
 int hspf_ospfv2_routes_delta(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result *pl,
                              const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                              hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return routes_delta(ctx, rt, n_jobs, pl, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return routes(ctx, rt, n_jobs, pl,
+                  hspf::DeltaOut<hl_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_routes_delta16(hspf_ctx *ctx, const hspf_ospfv2_rtable *rt, uint32_t n_jobs, const hspf_result16 *pl,
                                const hl_route_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return routes_delta(ctx, rt, n_jobs, pl, base_cells, n_base, base_of, job_out, records, cap, n_records);
+    return routes(ctx, rt, n_jobs, pl,
+                  hspf::DeltaOut<hl_route_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_run_area_batch(hspf_ctx *ctx, const hl_ospfv2_area *area, const uint32_t *root_router_ids, uint32_t n_roots,

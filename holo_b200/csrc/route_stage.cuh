@@ -138,24 +138,82 @@ route_cells_kernel(const Cell cell, uint32_t n_jobs, uint32_t P, CellWords *__re
     store_route_cells(n_jobs, P, cell, Cell::empty(), cells, aligned16);
 }
 
-// Enqueues route_cells_kernel on the ctx stream: n_jobs x P cells, the jobs' status words when status_out is set,
-// n_gather gathers of (gather_job, gather_area (NULL: 0), gather_v).  The grid covers the largest of the three, one
-// wave of kBlocksPerSM blocks per SM at most; kMinBlocks is the kernel's launch bound.
-template <int kMinBlocks, uint32_t kBlocksPerSM = kMinBlocks, class Cell>
-int launch_route_cells(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs, uint32_t P,
-                       void *cells, uint32_t *status_out, uint32_t n_gather, const uint32_t *gather_job,
-                       const uint32_t *gather_area, const uint32_t *gather_v, uint64_t *gather_nh) {
-    if (!ctx || !cells) return HSPF_E_INVAL;
-    if (n_gather && (!gather_job || !gather_v || !gather_nh)) return HSPF_E_INVAL;
-    const uint64_t items = std::max<uint64_t>({(uint64_t)n_jobs * P, status_out ? n_jobs : 0u, n_gather});
+// ---- what a call writes --------------------------------------------------------------------------------------
+// The cells call stores n_jobs x P cells of CellT, the jobs' status words when status_out is set, and n_gather
+// gathers of (gather_job, gather_area (NULL: 0), gather_v) into gather_nh.  The delta call compares the cells with
+// `base` [n_base][P] instead (the route-delta stage below).  Each descriptor takes its cell layout from CellT.
+template <class CellT> struct CellLayoutOf;
+template <> struct CellLayoutOf<hl_route_cell> { using type = OspfCellLayout; };
+template <> struct CellLayoutOf<hl_ospf_rib_cell> { using type = OspfRibCellLayout; };
+template <> struct CellLayoutOf<hl_isis_route_cell> { using type = IsisCellLayout; };
+
+template <class CellT>
+struct CellsOut {
+    static constexpr bool kDelta = false;
+    CellT *cells;
+    uint32_t *status_out;
+    uint32_t n_gather = 0;
+    const uint32_t *gather_job = nullptr, *gather_area = nullptr, *gather_v = nullptr;
+    uint64_t *gather_nh = nullptr;
+};
+
+template <class CellT>
+struct DeltaOut {
+    static constexpr bool kDelta = true;
+    using Layout = typename CellLayoutOf<CellT>::type;
+    const CellT *base;
+    uint32_t n_base;
+    const uint32_t *base_of;             // [n_jobs] base row of each job; NULL: row 0
+    hl_route_delta_job *job_out;
+    hl_route_delta *records;
+    uint64_t cap;
+    uint64_t *n_records;
+};
+
+// The output arguments a call refuses (HSPF_E_INVAL) before its first launch, so that a stage with a launch of its
+// own before the cells or the compare can check them first.
+template <class CellT>
+int check_route_out(const hspf_ctx *ctx, const CellsOut<CellT> &o, uint32_t, uint32_t) {
+    if (!ctx || !o.cells) return HSPF_E_INVAL;
+    if (o.n_gather && (!o.gather_job || !o.gather_v || !o.gather_nh)) return HSPF_E_INVAL;
+    return HSPF_OK;
+}
+
+// The largest batch of one route-delta call: n_jobs x P <= 2^36 cells, at most 2^31 warp tiles.  The delta kernels
+// walk tiles with a 32-bit counter and a stride of the grid's warp count (< 2^31), so tile + stride < 2^32 never
+// wraps; the reciprocal in delta_eval is exact below 2^37.
+constexpr uint64_t kDeltaMaxCells = 1ull << 36;
+inline bool delta_batch_fits(uint32_t n_jobs, uint32_t P) { return (uint64_t)n_jobs * P <= kDeltaMaxCells; }
+
+template <class CellT>
+int check_route_out(const hspf_ctx *ctx, const DeltaOut<CellT> &o, uint32_t n_jobs, uint32_t P) {
+    if (!ctx || !o.base || !o.job_out || !o.n_records || o.n_base == 0 || !delta_batch_fits(n_jobs, P))
+        return HSPF_E_INVAL;
+    // device buffers at their struct alignment
+    if ((reinterpret_cast<uintptr_t>(o.base) & 7u) || (reinterpret_cast<uintptr_t>(o.job_out) & 3u) ||
+        (reinterpret_cast<uintptr_t>(o.n_records) & 7u) || (reinterpret_cast<uintptr_t>(o.records) & 3u))
+        return HSPF_E_INVAL;
+    return HSPF_OK;
+}
+
+// launch_route_stage(ctx, table, cell, n_jobs, P, out) enqueues the cells call or the delta call of `cell` on the
+// ctx stream, as `out` is a CellsOut or a DeltaOut.  kMinBlocks is the kernels' launch bound; the grid is one wave
+// of kBlocksPerSM blocks per SM at most.
+
+// route_cells_kernel over the largest of the cells, the status words and the gathers.
+template <int kMinBlocks, uint32_t kBlocksPerSM = kMinBlocks, class Cell, class CellT>
+int launch_route_stage(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs, uint32_t P,
+                       const CellsOut<CellT> &out) {
+    if (const int rc = check_route_out(ctx, out, n_jobs, P)) return rc;
+    const uint64_t items = std::max<uint64_t>({(uint64_t)n_jobs * P, out.status_out ? n_jobs : 0u, out.n_gather});
     if (items == 0) return HSPF_OK;
     uint32_t blocks = 0;
     const int rc = route_grid(ctx, table, items, kBlocksPerSM, blocks);
     if (rc != HSPF_OK) return rc;
-    const bool aligned16 = (reinterpret_cast<uintptr_t>(cells) & 15u) == 0;
+    const bool aligned16 = (reinterpret_cast<uintptr_t>(out.cells) & 15u) == 0;
     route_cells_kernel<Cell, kMinBlocks><<<blocks, kRouteThreads, 0, static_cast<cudaStream_t>(hspf_stream(ctx))>>>(
-        cell, n_jobs, P, static_cast<CellWords *>(cells), status_out, aligned16, n_gather, gather_job, gather_area,
-        gather_v, gather_nh);
+        cell, n_jobs, P, reinterpret_cast<CellWords *>(out.cells), out.status_out, aligned16, out.n_gather,
+        out.gather_job, out.gather_area, out.gather_v, out.gather_nh);
     if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
     hspf_note_launches(ctx, 1);
     return HSPF_OK;
@@ -188,12 +246,6 @@ __host__ __device__ __forceinline__ uint64_t delta_tiles64(uint32_t n_jobs, uint
     return ((uint64_t)n_jobs * P + 31) / 32;
 }
 
-// The largest batch of one route-delta call: n_jobs x P <= 2^36 cells, at most 2^31 warp tiles.  The delta kernels
-// walk tiles with a 32-bit counter and a stride of the grid's warp count (< 2^31), so tile + stride < 2^32 never
-// wraps; the reciprocal in delta_eval is exact below 2^37.  Every delta entry point refuses a larger batch before
-// its first launch.
-constexpr uint64_t kDeltaMaxCells = 1ull << 36;
-inline bool delta_batch_fits(uint32_t n_jobs, uint32_t P) { return (uint64_t)n_jobs * P <= kDeltaMaxCells; }
 __device__ __forceinline__ uint32_t delta_tiles(const DeltaArgs &a) { return (uint32_t)delta_tiles64(a.n_jobs, a.P); }
 
 // The kind of the cell of `lane` in warp tile `tile` (0 past the end, for a job without a valid base row, and for a
@@ -280,18 +332,13 @@ size_t route_delta_scan_bytes(uint64_t n_tiles);
 cudaError_t route_delta_scan(void *temp, size_t temp_bytes, const uint8_t *cnt, uint64_t *off, uint64_t n_tiles,
                              cudaStream_t st);
 
-// Enqueues the route-delta stage over `cell` on the ctx stream: the summaries and the total are zeroed, then pass A
-// runs; with records, the scan and pass B follow.  `base` holds the base cells [n_base][P].  Both passes are
-// launch-bounded to kMinBlocks blocks per SM, and the grid is one wave of kBlocksPerSM blocks per SM at most.
-template <class Layout, int kMinBlocks, uint32_t kBlocksPerSM = kMinBlocks, class Cell>
-int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs, uint32_t P,
-                       const void *base, uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
-                       hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    if (!ctx || !base || !job_out || !n_records || n_base == 0 || !delta_batch_fits(n_jobs, P)) return HSPF_E_INVAL;
-    // device buffers at their struct alignment
-    if ((reinterpret_cast<uintptr_t>(base) & 7u) || (reinterpret_cast<uintptr_t>(job_out) & 3u) ||
-        (reinterpret_cast<uintptr_t>(n_records) & 7u) || (reinterpret_cast<uintptr_t>(records) & 3u))
-        return HSPF_E_INVAL;
+// The route-delta stage over `cell`: the summaries and the total are zeroed, then pass A runs; with records, the
+// scan and pass B follow.  Both passes are launch-bounded to kMinBlocks blocks per SM.
+template <int kMinBlocks, uint32_t kBlocksPerSM = kMinBlocks, class Cell, class CellT>
+int launch_route_stage(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell &cell, uint32_t n_jobs, uint32_t P,
+                       const DeltaOut<CellT> &out) {
+    using Layout = typename DeltaOut<CellT>::Layout;
+    if (const int rc = check_route_out(ctx, out, n_jobs, P)) return rc;
     const uint64_t total = (uint64_t)n_jobs * P, n_tiles = delta_tiles64(n_jobs, P);
     // the grid covers the cells, or the jobs' status words when there are more jobs than cells
     uint32_t blocks = 0;
@@ -299,13 +346,14 @@ int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell 
     if (rc != HSPF_OK) return rc;
     DeltaArgs a{};
     a.n_jobs = n_jobs; a.P = P; a.inv_p = P ? 1.0 / P : 0.0;
-    a.base = static_cast<const uint64_t *>(base); a.n_base = n_base; a.base_of = base_of;
-    a.job_out = job_out; a.n_records = reinterpret_cast<unsigned long long *>(n_records);
+    a.base = reinterpret_cast<const uint64_t *>(out.base); a.n_base = out.n_base; a.base_of = out.base_of;
+    a.job_out = out.job_out; a.n_records = reinterpret_cast<unsigned long long *>(out.n_records);
     cudaStream_t st = static_cast<cudaStream_t>(hspf_stream(ctx));
-    if (cudaMemsetAsync(n_records, 0, sizeof(uint64_t), st) != cudaSuccess) return HSPF_E_CUDA;
+    if (cudaMemsetAsync(out.n_records, 0, sizeof(uint64_t), st) != cudaSuccess) return HSPF_E_CUDA;
     if (n_jobs == 0) return HSPF_OK;
-    if (cudaMemsetAsync(job_out, 0, (size_t)n_jobs * sizeof(hl_route_delta_job), st) != cudaSuccess) return HSPF_E_CUDA;
-    const bool with_records = records && cap && n_tiles;
+    if (cudaMemsetAsync(out.job_out, 0, (size_t)n_jobs * sizeof(hl_route_delta_job), st) != cudaSuccess)
+        return HSPF_E_CUDA;
+    const bool with_records = out.records && out.cap && n_tiles;
     size_t scan_bytes = 0;
     char *ws = nullptr;
     if (with_records) {
@@ -315,7 +363,7 @@ int launch_route_delta(hspf_ctx *ctx, const DeviceRouteTable &table, const Cell 
         if (!ws) return HSPF_E_NOMEM;
         a.tile_off = reinterpret_cast<const uint64_t *>(ws);
         a.tile_cnt = reinterpret_cast<uint8_t *>(ws + off_bytes);
-        a.records = records; a.cap = cap;
+        a.records = out.records; a.cap = out.cap;
         ws += off_bytes + cnt_bytes;
     }
     route_delta_count_kernel<Layout, Cell, kMinBlocks><<<blocks, kRouteThreads, 0, st>>>(cell, a);
