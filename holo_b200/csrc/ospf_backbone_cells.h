@@ -234,18 +234,20 @@ HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneVi
 // An area border router R over jobs inside an area it is not attached to (hspf_ospfv2_abr_backbone_table_create):
 // abr_rib_cell_eval with kSlots over R's row 0 of every area.  Area 0's type-3 ranges hold static records (z
 // kOspfBackboneStatic) and slots as the backbone table's, its type-4 ranges static records and type-4 slots as the
-// asbr table's.  A slot's winner is n_recs + its slot index.
+// asbr table's.  A slot's winner is n_recs + its slot index; kV3 (hspf_ospfv3_abr_backbone_table_create): n_recs +
+// (slot index << 8 | prefix options), as ospf_backbone_cell_eval<kV3> gives it.
+template <bool kV3 = false>
 struct AbrBorderSlots {
     static constexpr uint32_t kAsbrSlot = kOspfBackboneAsbrSlot;
     OspfBorderRows rows;
-    const uint32_t *border;       // [4 n_borders] as OspfBackboneView::border (area 0's records and atoms)
+    const uint32_t *border;       // [4 n_borders] (OSPFv3: [8 n_borders] and the options bytes) as OspfBackboneView::border
     uint32_t n_recs;
     // what type-3 record r offers: a static one its own metric, a slot its border's advertisement (false: none)
     HSPF_HD bool offer(const RibRec &r, uint32_t &metric, uint32_t &winner) const {
         if (r.z == kOspfBackboneStatic) return true;
         uint32_t options;
-        if (!border_summary<false>(rows.row[r.z] + r.y, border, r.z, metric, options)) return false;
-        winner = n_recs + r.w;
+        if (!border_summary<kV3>(rows.row[r.z] + r.y, border, r.z, metric, options)) return false;
+        winner = kV3 ? n_recs + (r.w << 8 | options) : n_recs + r.w;
         return true;
     }
 };
@@ -270,11 +272,12 @@ HSPF_HD uint32_t abr_row0_status(const AbrPlaneSet<D, N> &s, uint32_t n_areas) {
 }  // namespace hspf
 
 // Host + device image of an area border router's affected prefixes over jobs inside another area
-// (include/holo_spf_lsdb.h, hspf_ospfv2_abr_backbone_table_create; ospf_ribtable.h, build_abr_backbone_table).
+// (include/holo_spf_lsdb.h, hspf_ospfv{2,3}_abr_backbone_table_create; ospf_ribtable.h, build_abr_backbone_table).
 struct hspf_ospfv2_abr_backbone_table {
     // R's table over the affected prefixes.  Its records: every area's intra-area records as R's whole table has them
     // (the decode's), the type-3 ranges (area 0's with slots), the type-5 ranges, the ASBR entries and type-4 ranges,
     // then from walk_intra the intra-area records of the affected prefixes again, which `off` names for the walk.
+    // abr->v3 marks an OSPFv3 table: its options6 holds a placeholder for each slot, whose options come from its winner.
     hspf_ospfv2_abr_ribtable *abr = nullptr;
     uint32_t area0 = 0, n_borders = 0, walk_intra = 0;
     const hspf_ospfv2_abr_ribtable *borders[hspf::kOspfBackboneMaxBorders] = {};
@@ -282,7 +285,8 @@ struct hspf_ospfv2_abr_backbone_table {
     std::vector<uint32_t> slot_rec;              // [n_slots] the record of each slot
     uint32_t n_asbr_slots = 0;
     std::vector<std::pair<uint32_t, uint32_t>> asbr_set;   // the type-4 slots' plane sets (border, area index)
-    std::vector<uint32_t> words;                 // abr->off, padded to 16 bytes, then border [4 n_borders]
+    std::vector<uint32_t> words;                 // abr->off, padded to 16 bytes, then border [4 n_borders] (OSPFv3:
+                                                 // [8 n_borders], then each border's options bytes)
     hspf::DeviceRouteTable dev;                  // words, then records
 
     uint32_t P() const { return (uint32_t)abr->prefix.size(); }

@@ -10,13 +10,13 @@
 //                      affected prefixes over its one-area table and its borders' ABR tables (ospf_backbone_cells.h);
 //                      hspf_ospfv{2,3}_nonbackbone_table_create: the same for an internal router of a non-backbone
 //                      area
-//   build_abr_backbone_table  hspf_ospfv2_abr_backbone_table_create: an area border router's affected prefixes over
-//                      its ABR table and the borders' (build_abr_ribtable, and the slot helpers build_backbone_table
-//                      shares)
+//   build_abr_backbone_table  hspf_ospfv2_abr_backbone_table_create / hspf_ospfv3_abr_backbone_table_create: an area
+//                      border router's affected prefixes over its ABR table and the borders' (build_abr_ribtable, and
+//                      the slot and border-word helpers build_backbone_table shares)
 //   decode_rib         one job's cells -> its routing table, for hspf_ospfv2_rib_from_cells,
 //                      hspf_ospfv3_rib_from_cells, hspf_ospfv{2,3}_abr_rib_from_cells (decode_abr_rib),
 //                      hspf_ospfv{2,3}_backbone_from_cells (decode_backbone_rib) and
-//                      hspf_ospfv2_abr_backbone_from_cells (decode_abr_backbone_rib).  A one-area table decodes as an area
+//                      hspf_ospfv{2,3}_abr_backbone_from_cells (decode_abr_backbone_rib).  A one-area table decodes as an area
 //                      border router's table with a single area.
 //
 // For build_rib_records a version trait T provides:
@@ -442,6 +442,51 @@ inline std::array<uint32_t, 4> border_words(const hspf_ospfv2_abr_ribtable &bt, 
     return {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)};
 }
 
+// Every border's words over its target-area index at[b], appended to `words` (which ends on a 16-byte boundary).
+// OSPFv3 (kV3): 8 words per border, the fifth the byte offset from the first border word of the border's options
+// bytes, which follow all the border words, each border's padded to a word: one per record an advertised cell's
+// winner can be, its intra-area records and, into a non-backbone area (nb), its type-3 records too.  HSPF_E_INVAL when
+// a border's table does not hold those options.
+template <bool kV3>
+int append_border_words(std::vector<uint32_t> &words, const hspf_ospfv2_abr_ribtable *const *borders,
+                        uint32_t n_borders, const uint32_t *at, bool nb) {
+    uint32_t opt_words = (kV3 ? 8 : 4) * n_borders;
+    auto opt_end = [&](const hspf_ospfv2_abr_ribtable &bt) { return nb ? bt.t3_end : bt.t3_base[0]; };
+    for (uint32_t b = 0; b < n_borders; ++b) {
+        const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+        const std::array<uint32_t, 4> bw = border_words(bt, at[b]);
+        words.insert(words.end(), bw.begin(), bw.end());
+        if (kV3) {
+            words.insert(words.end(), {4 * opt_words, 0u, 0u, 0u});
+            opt_words += (opt_end(bt) + 3) / 4;
+        }
+    }
+    if (kV3) {
+        // per border, the prefix options of each intra-area record of its table, as the OSPFv3 intra-area decode
+        // reads them for that winner: the record's entry in its area's intra-area table; into a non-backbone area
+        // also those of each type-3 record (an inter-area cell's winner), the options of its LSA
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            const hspf_ospfv2_abr_ribtable &bt = *borders[b];
+            std::vector<uint8_t> opt;
+            for (uint32_t i = 0; i < bt.n_areas; ++i) {
+                const std::vector<uint8_t> &o = bt.area[i]->intra->t.options6;
+                if (o.size() != bt.area[i]->n_intra || opt.size() != bt.intra_base[i]) return HSPF_E_INVAL;
+                opt.insert(opt.end(), o.begin(), o.end());
+            }
+            if (nb) {
+                const size_t n3 = bt.t3_end - bt.t3_base[0];
+                if (opt.size() != bt.t3_base[0] || bt.options6.size() < n3) return HSPF_E_INVAL;
+                opt.insert(opt.end(), bt.options6.begin(), bt.options6.begin() + n3);
+            }
+            opt.resize(((size_t)opt_end(bt) + 3) & ~(size_t)3, 0);
+            const size_t w = words.size();
+            words.resize(w + opt.size() / 4);
+            if (!opt.empty()) std::memcpy(words.data() + w, opt.data(), opt.size());
+        }
+    }
+    return HSPF_OK;
+}
+
 // hspf_ospfv2_backbone_table_create / hspf_ospfv3_backbone_table_create, argument checks included: R's one-area table
 // over area 0 without the borders' type-3 LSAs, and per affected prefix R's intra-area records, its static type-3
 // records with one slot per (border, prefix) at the border's place in LsaKey order, and its type-5 records
@@ -649,42 +694,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         t->words.insert(t->words.end(), o3.begin(), o3.end());
         t->words.insert(t->words.end(), o5.begin(), o5.end());
         t->words.resize(t->border_at(), 0);
-        uint32_t opt_words = (T::kV3 ? 8 : 4) * n_borders;         // OSPFv3: the options bytes follow the border words
-        // OSPFv3: a border's options bytes, one per record an advertised cell's winner can be: its intra-area records,
-        // and into a non-backbone area its type-3 records too
-        auto opt_end = [&](const hspf_ospfv2_abr_ribtable &bt) { return nb ? bt.t3_end : bt.t3_base[0]; };
-        for (uint32_t b = 0; b < n_borders; ++b) {
-            const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-            const std::array<uint32_t, 4> bw = border_words(bt, at[b]);
-            t->words.insert(t->words.end(), bw.begin(), bw.end());
-            if (T::kV3) {
-                t->words.insert(t->words.end(), {4 * opt_words, 0u, 0u, 0u});
-                opt_words += (opt_end(bt) + 3) / 4;
-            }
-        }
-        if (T::kV3) {
-            // per border, the prefix options of each intra-area record of its table, as the OSPFv3 intra-area decode
-            // reads them for that winner: the record's entry in its area's intra-area table; into a non-backbone area
-            // also those of each type-3 record (an inter-area cell's winner), the options of its LSA
-            for (uint32_t b = 0; b < n_borders; ++b) {
-                const hspf_ospfv2_abr_ribtable &bt = *borders[b];
-                std::vector<uint8_t> opt;
-                for (uint32_t i = 0; i < bt.n_areas; ++i) {
-                    const std::vector<uint8_t> &o = bt.area[i]->intra->t.options6;
-                    if (o.size() != bt.area[i]->n_intra || opt.size() != bt.intra_base[i]) return HSPF_E_INVAL;
-                    opt.insert(opt.end(), o.begin(), o.end());
-                }
-                if (nb) {
-                    const size_t n3 = bt.t3_end - bt.t3_base[0];
-                    if (opt.size() != bt.t3_base[0] || bt.options6.size() < n3) return HSPF_E_INVAL;
-                    opt.insert(opt.end(), bt.options6.begin(), bt.options6.begin() + n3);
-                }
-                opt.resize(((size_t)opt_end(bt) + 3) & ~(size_t)3, 0);
-                const size_t at = t->words.size();
-                t->words.resize(at + opt.size() / 4);
-                if (!opt.empty()) std::memcpy(t->words.data() + at, opt.data(), opt.size());
-            }
-        }
+        if (const int rc2 = append_border_words<T::kV3>(t->words, borders, n_borders, at.data(), nb)) return rc2;
         *out = t.release();
         return HSPF_OK;
     } catch (const std::bad_alloc &) {
@@ -699,7 +709,9 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
 // summaries without the borders' type-3 / type-4 LSAs, restricted to the affected prefixes: those some border can
 // advertise into area 0, and those of the type-5 LSAs of an ASBR some border can originate a type-4 LSA for.  Area
 // 0's type-3 ranges get the borders' slots and its type-4 ranges their type-4 slots, at the borders' LsaKey places,
-// as build_backbone_table places them (ospf_backbone_cells.h: AbrBorderSlots).
+// as build_backbone_table places them (ospf_backbone_cells.h: AbrBorderSlots).  OSPFv3
+// (hspf_ospfv3_abr_backbone_table_create): the restricted table carries its IPv6 prefixes and the options of its
+// type-3 / type-5 records, and the border words carry each border's options bytes, as build_backbone_table's do.
 template <class T>
 int build_abr_backbone_table(uint32_t router_id, uint32_t n_areas, const typename T::Flat *const *flats,
                              const uint32_t *area_ids, const typename T::Sum *const *summaries,
@@ -804,6 +816,7 @@ int build_abr_backbone_table(uint32_t router_id, uint32_t n_areas, const typenam
         const uint32_t P = (uint32_t)slots.size(), S = P + 1;
         std::vector<uint32_t> from(P);                               // R's prefix index of each, or kNone
         r->prefix.resize(P); r->plen.resize(P);
+        if (T::kV3) r->prefix6.resize(P);
         r->area_prefix.assign(A, std::vector<uint32_t>(P, kNoRecord));
         uint32_t u = 0;
         for (const auto &e : slots) {
@@ -821,22 +834,30 @@ int build_abr_backbone_table(uint32_t router_id, uint32_t n_areas, const typenam
         std::unordered_map<uint32_t, uint32_t> id_of;
         for (const auto &e : F.rtr_vertex[i0]) id_of.emplace(e.second, e.first);
         auto adv_rtr = [&](const RibRec &x) { return id_of.at(x.x); };
+        // OSPFv3: options6 holds each type-3 / type-5 record's prefix options (index - t3_base[0]), R's for a static
+        // one and a placeholder for a slot, whose options come from its winner
+        auto put = [&](const RibRec &x, uint32_t k) {
+            recs.push_back(x);
+            if (T::kV3) r->options6.push_back(F.options6[k - F.t3_base[0]]);
+        };
         for (uint32_t i = 0; i < A; ++i) {                           // type-3, area 0's with the slots
             r->t3_base.push_back((uint32_t)recs.size());
             const uint32_t *g3 = F.off.data() + (A + i) * (size_t)SF;
             u = 0;
             for (const auto &e : slots) {
                 o3[i * S + u] = (uint32_t)recs.size();
-                std::vector<RibRec> st;
-                if (from[u] != kNone) st.assign(F.recs.begin() + g3[from[u]], F.recs.begin() + g3[from[u] + 1]);
+                std::vector<uint32_t> st;                            // R's records of the prefix
+                if (from[u] != kNone)
+                    for (uint32_t k = g3[from[u]]; k < g3[from[u] + 1]; ++k) st.push_back(k);
                 if (i != i0) {
-                    recs.insert(recs.end(), st.begin(), st.end());
+                    for (uint32_t k : st) put(F.recs[k], k);
                 } else {
-                    merge_lsakey(st, adv_rtr, e.second, borders,
-                                 [&](const RibRec &x) { recs.push_back(RibRec{x.x, x.y, kOspfBackboneStatic, 0}); },
+                    merge_lsakey(st, [&](uint32_t k) { return adv_rtr(F.recs[k]); }, e.second, borders,
+                                 [&](uint32_t k) { put(RibRec{F.recs[k].x, F.recs[k].y, kOspfBackboneStatic, 0}, k); },
                                  [&](const std::pair<uint32_t, uint32_t> &s) {
                                      t->slot_rec.push_back((uint32_t)recs.size());
                                      recs.push_back(RibRec{bv[s.first], s.second, s.first, (uint32_t)t->slot_rec.size() - 1});
+                                     if (T::kV3) r->options6.push_back(0);
                                  });
                 }
                 ++u;
@@ -854,7 +875,7 @@ int build_abr_backbone_table(uint32_t router_id, uint32_t n_areas, const typenam
             o5[u] = (uint32_t)recs.size();
             if (from[u] == kNone) continue;
             for (uint32_t k = f5[from[u]]; k < f5[from[u] + 1]; ++k) {
-                recs.push_back(RibRec{F.recs[k].x + shift, F.recs[k].y, F.recs[k].z, F.recs[k].w});
+                put(RibRec{F.recs[k].x + shift, F.recs[k].y, F.recs[k].z, F.recs[k].w}, k);
                 r->ext_tag.push_back(F.ext_tag[k - F.ext_base]);
             }
         }
@@ -894,14 +915,11 @@ int build_abr_backbone_table(uint32_t router_id, uint32_t n_areas, const typenam
             r->off[i * S + P] = (uint32_t)recs.size();
         }
         r->vl_off.assign(A + 1, 0);
-        if (recs.size() >= kNoRecord || !backbone_winners_fit(recs.size(), t->slot_rec.size(), false))
+        if (recs.size() >= kNoRecord || !backbone_winners_fit(recs.size(), t->slot_rec.size(), T::kV3))
             return HSPF_E_UNSUPPORTED;
         t->words = r->off;
         t->words.resize(((t->words.size() + 3) & ~(size_t)3), 0);
-        for (uint32_t b = 0; b < n_borders; ++b) {
-            const std::array<uint32_t, 4> bw = border_words(*borders[b], a0[b]);
-            t->words.insert(t->words.end(), bw.begin(), bw.end());
-        }
+        if (const int rc2 = append_border_words<T::kV3>(t->words, borders, n_borders, a0.data(), false)) return rc2;
         t->abr = r.release();
         *out = t.release();
         return HSPF_OK;
@@ -1089,11 +1107,13 @@ int decode_one_area_rib(const typename T::Area *a, const hspf_ospfv2_ribtable &r
 
 // hspf_ospfv2_abr_rib_from_cells / hspf_ospfv3_abr_rib_from_cells, argument checks included: each area's job
 // decode over its own gathers, and the decode of the router's table over them.  A table of the other version is
-// refused (HSPF_E_INVAL).
+// refused (HSPF_E_INVAL).  `options` (OSPFv3): the prefix options of each type-3 / type-5 record (index -
+// t3_base[0]) the routes take, the table's own when NULL.
 template <class T>
 int decode_abr_rib(const hspf_ospfv2_abr_ribtable *t, const typename T::Area *areas, uint32_t n_areas,
                    const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
-                   const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out) {
+                   const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out,
+                   const uint8_t *options = nullptr) {
     if (!t || t->v3 != T::kV3 || !areas || !cells || !out || n_areas != t->n_areas ||
         (n_gather && (!gather_area || !gather_v || !gather_nh)))
         return HSPF_E_INVAL;
@@ -1102,7 +1122,8 @@ int decode_abr_rib(const hspf_ospfv2_abr_ribtable *t, const typename T::Area *ar
         const uint32_t A = n_areas, P = (uint32_t)t->plen.size(), S = P + 1;
         std::vector<typename T::JobDecode> jd(A);
         RibDecode<T> d{{}, P, t->prefix.data(), t->plen.data(), t->prefix6.data(), t->off.data() + 2 * (size_t)A * S,
-                       t->ext_tag.data(), t->ext_base, t->max_paths, t->options6.data(), t->t3_base[0]};
+                       t->ext_tag.data(), t->ext_base, t->max_paths, options ? options : t->options6.data(),
+                       t->t3_base[0]};
         for (uint32_t i = 0; i < A; ++i) {
             const typename T::Area &a = areas[i];
             if (a.router_id != t->router_id || a.area_id != t->area_id[i] || a.max_paths != t->max_paths) return HSPF_E_INVAL;
@@ -1129,27 +1150,34 @@ int decode_abr_rib(const hspf_ospfv2_abr_ribtable *t, const typename T::Area *ar
     }
 }
 
-// hspf_ospfv2_abr_backbone_from_cells, argument checks included: a slot winner names its type-3 record and a walk
-// intra-area record the decode's, then decode_abr_rib over the table's prefixes.
+// hspf_ospfv2_abr_backbone_from_cells / hspf_ospfv3_abr_backbone_from_cells, argument checks included: a slot winner
+// names its type-3 record (OSPFv3: and carries the options the route takes, written into this job's copy of the
+// table's options) and a walk intra-area record the decode's, then decode_abr_rib over the table's prefixes.  A table
+// of the other version is refused (HSPF_E_INVAL).
 template <class T>
 int decode_abr_backbone_rib(const hspf_ospfv2_abr_backbone_table *t, const typename T::Area *areas, uint32_t n_areas,
                             const hl_ospf_rib_cell *cells, const uint32_t *gather_area, const uint32_t *gather_v,
                             const uint64_t *gather_nh, uint32_t n_gather, typename T::Rib *out) {
-    if (!t || !t->abr || !cells || !out) return HSPF_E_INVAL;
+    if (!t || !t->abr || t->abr->v3 != T::kV3 || !cells || !out) return HSPF_E_INVAL;
     try {
         const uint32_t n_recs = t->n_recs();
         std::vector<hl_ospf_rib_cell> c(cells, cells + t->P());
+        std::vector<uint8_t> options(t->abr->options6);
         for (hl_ospf_rib_cell &x : c) {
             if (!(HL_RIB_CELL_FLAGS(x) & HL_CELL_PRESENT)) continue;
             if (x.winner >= n_recs) {
-                if (HL_RIB_CELL_PATH(x) != HL_PATH_INTER_AREA || x.winner - n_recs >= t->slot_rec.size()) return HSPF_E_INVAL;
-                x.winner = t->slot_rec[x.winner - n_recs];
+                uint32_t s = x.winner - n_recs, opt = 0;
+                if (T::kV3) { opt = s & 0xFFu; s >>= 8; }
+                if (HL_RIB_CELL_PATH(x) != HL_PATH_INTER_AREA || s >= t->slot_rec.size()) return HSPF_E_INVAL;
+                x.winner = t->slot_rec[s];
+                if (T::kV3) options[x.winner - t->abr->t3_base[0]] = (uint8_t)opt;
             } else if (HL_RIB_CELL_PATH(x) == HL_PATH_INTRA_AREA) {
                 if (x.winner < t->walk_intra || x.winner - t->walk_intra >= t->intra_src.size()) return HSPF_E_INVAL;
                 x.winner = t->intra_src[x.winner - t->walk_intra];
             }
         }
-        return decode_abr_rib<T>(t->abr, areas, n_areas, c.data(), gather_area, gather_v, gather_nh, n_gather, out);
+        return decode_abr_rib<T>(t->abr, areas, n_areas, c.data(), gather_area, gather_v, gather_nh, n_gather, out,
+                                 T::kV3 ? options.data() : nullptr);
     } catch (const std::bad_alloc &) {
         return HSPF_E_NOMEM;
     } catch (...) {

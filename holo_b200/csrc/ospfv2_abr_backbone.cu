@@ -1,6 +1,8 @@
-// Device stage for the routing table of an OSPFv2 area border router over what-if jobs inside an area it is not
-// attached to (include/holo_spf_lsdb.h, hspf_ospfv2_abr_backbone_table_create): update_rib_full at the router, for
-// its affected prefixes, with every border's type-3 and type-4 LSAs in area 0 re-originated for the job.
+// Device stage for the routing table of an OSPF area border router over what-if jobs inside an area it is not
+// attached to (include/holo_spf_lsdb.h, hspf_ospfv2_abr_backbone_table_create / hspf_ospfv3_abr_backbone_table_create):
+// update_rib_full at the router, for its affected prefixes, with every border's type-3 / Inter-Area-Prefix and type-4
+// / Inter-Area-Router LSAs in area 0 re-originated for the job.  The entry points serve OSPFv2 and OSPFv3 tables
+// alike: the table's version mark (abr->v3) picks the walk's instantiation.
 //
 // One launch on the ctx stream: one thread per (job, prefix) runs abr_rib_cell_eval with kSlots (ospf_abr_rib_cells.h,
 // ospf_backbone_cells.h: AbrBorderSlots) over the router's row 0 of every area, the job's row of each border's
@@ -18,8 +20,8 @@ namespace {
 
 using hspf::kOspfBackboneMaxBorders;
 
-template <class Planes>
-struct OspfAbrBackboneCell {
+template <class Planes, bool kV3>
+struct OspfAbrBackboneCellOf {
     using Rows = hspf::ResultPlanes<Planes>;
     using D = typename Rows::D;
     using N = typename Rows::N;
@@ -39,7 +41,7 @@ struct OspfAbrBackboneCell {
     }
     __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
     __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::AbrBorderSlots sl;
+        hspf::AbrBorderSlots<kV3> sl;
 #pragma unroll
         for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) sl.rows.row[b] = cells[b] + (size_t)j * K[b];
         sl.border = border;
@@ -51,20 +53,29 @@ struct OspfAbrBackboneCell {
     __device__ static hspf::CellWords empty() { return {0, 0, hspf::kNoRecord}; }
 };
 
-// Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6).
+// The walk over an OSPFv2 table, and over an OSPFv3 one, whose slot winners carry prefix options.  Types of their own,
+// so that each has its own kernels and launch bound.
+template <class Planes>
+struct OspfAbrBackboneCell : OspfAbrBackboneCellOf<Planes, false> {};
+template <class Planes>
+struct OspfAbrBackboneV3Cell : OspfAbrBackboneCellOf<Planes, true> {};
+
+// Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2 and
+// for OSPFv3 tables.
 constexpr uint32_t kAbrBackboneBlocksPerSM = 4;
+constexpr uint32_t kAbrBackboneV3BlocksPerSM = 4;
 
 // R's planes, the borders' cells and status words, and the plane sets the type-4 slots name, from each border's
 // planes, row counts and rows (border_planes[b][i], border_n_rows[b][i], border_rows[b]), which may be NULL when the
 // table has no type-4 slot.
-template <class R>
+template <class R, class Cell>
 int make_cell(const hspf_ospfv2_abr_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
               const uint32_t *const *border_status, const R *const *border_planes, const uint32_t *const *border_n_rows,
-              const uint32_t *const *border_rows, uint32_t n_jobs, OspfAbrBackboneCell<hspf::PlanesOf<R>> &cell) {
+              const uint32_t *const *border_rows, uint32_t n_jobs, Cell &cell) {
     if (!t || !t->abr || !t->dev.blob || !planes || !border_cells) return HSPF_E_INVAL;
     const hspf_ospfv2_abr_ribtable &a = *t->abr;
     for (uint32_t i = 0; i < a.n_areas; ++i) {
-        typename OspfAbrBackboneCell<hspf::PlanesOf<R>>::Rows p;
+        typename Cell::Rows p;
         if (hspf::result_planes(&planes[i], a.n_vertices[i], p) || !p.complete()) return HSPF_E_INVAL;
         cell.s.dist[i] = p.dist; cell.s.hops[i] = p.hops; cell.s.nh[i] = p.nh; cell.s.status[i] = p.status;
         cell.s.V[i] = p.V; cell.s.n_rows[i] = 1;
@@ -78,16 +89,32 @@ int make_cell(const hspf_ospfv2_abr_backbone_table *t, const R *planes, const hl
     return HSPF_OK;
 }
 
+template <class Cell, uint32_t kBlocks, class R, class Out>
+int abr_backbone_as(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
+                    const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+                    const R *const *border_planes, const uint32_t *const *border_n_rows,
+                    const uint32_t *const *border_rows, const Out &out) {
+    Cell cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
+                                 n_jobs, cell))
+        return rc;
+    return hspf::launch_route_stage<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
+}
+
+// the walk of the table's version
 template <class R, class Out>
 int abr_backbone(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
                  const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                  const R *const *border_planes, const uint32_t *const *border_n_rows,
                  const uint32_t *const *border_rows, const Out &out) {
-    OspfAbrBackboneCell<hspf::PlanesOf<R>> cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                                 n_jobs, cell))
-        return rc;
-    return hspf::launch_route_stage<kAbrBackboneBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), out);
+    if (!t || !t->abr) return HSPF_E_INVAL;
+    using P = hspf::PlanesOf<R>;
+    return t->abr->v3 ? abr_backbone_as<OspfAbrBackboneV3Cell<P>, kAbrBackboneV3BlocksPerSM>(
+                            ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                            border_rows, out)
+                      : abr_backbone_as<OspfAbrBackboneCell<P>, kAbrBackboneBlocksPerSM>(
+                            ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
+                            border_rows, out);
 }
 
 }  // namespace

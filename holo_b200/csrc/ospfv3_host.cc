@@ -942,4 +942,35 @@ int hspf_ospfv3_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
     return hspf::decode_backbone_rib<RibV3>(t, a, cells, gather_v, gather_nh, n_gather, out);
 }
 
+
+/* ---- area border router over what-if jobs inside another area (ospf_backbone_cells.h) -------------------------- */
+
+int hspf_ospfv3_abr_backbone_table_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv3_flat *const *flats,
+                                          const uint32_t *area_ids, const hl_ospfv3_inter_area_lsa *const *summaries,
+                                          const uint32_t *n_summaries, const uint8_t *active,
+                                          const hl_ospfv3_external_lsa *ext, uint32_t n_ext,
+                                          const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                          hspf_ospfv2_abr_backbone_table **out) {
+    return hspf::build_abr_backbone_table<RibV3>(router_id, n_areas, flats, area_ids, summaries, n_summaries, active,
+                                                 ext, n_ext, borders, n_borders, out);
+}
+
+int hspf_ospfv3_abr_backbone_table_prefixes6(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_prefixes,
+                                             const hl_ip_addr **prefixes, const uint32_t **lens) {
+    if (!t || !t->abr || !t->abr->v3) return HSPF_E_INVAL;
+    if (n_prefixes) *n_prefixes = t->P();
+    if (prefixes) *prefixes = t->abr->prefix6.data();
+    if (lens) *lens = t->abr->plen.data();
+    return HSPF_OK;
+}
+
+// The decode of R's table over the affected prefixes: a slot winner names its Inter-Area-Prefix record and carries the
+// route's prefix options.
+int hspf_ospfv3_abr_backbone_from_cells(const hspf_ospfv2_abr_backbone_table *t, const hl_ospfv3_area *areas,
+                                        uint32_t n_areas, const hl_ospf_rib_cell *cells, const uint32_t *gather_area,
+                                        const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather,
+                                        hl_ospfv3_rib *out) {
+    return hspf::decode_abr_backbone_rib<RibV3>(t, areas, n_areas, cells, gather_area, gather_v, gather_nh, n_gather, out);
+}
+
 }  // extern "C"

@@ -823,17 +823,24 @@ class AbrBackboneTable:
     `externals` as for AbrRibTable (area 0's summaries as in R's LSDB); `borders`: the AbrRibTables of the perturbed
     area's ABRs attached to area 0 (kept alive with this table).  `prefix`, `plen` [n_prefixes]: the affected prefixes
     in prefix order; a slot's winner is n_records + its slot index (n_slots in all); `n_asbr_slots` type-4 slots read
-    `n_asbr_sets` (border, area) plane sets."""
+    `n_asbr_sets` (border, area) plane sets.
+
+    From ospfv3.Flat areas the table is hspf_ospfv3_abr_backbone_table_create's (summaries: INTER_AREA_LSA_DT,
+    externals: EXTERNAL6_LSA_DT, borders: OSPFv3 AbrRibTables); `prefix` and `prefixes6` then hold the IPv6 prefixes
+    (ospfv3.IP_DT), `v3` is set, and a slot's winner is n_records + (slot index << 8 | its prefix options)."""
 
     def __init__(self, router_id: int, flats: list, area_ids, summaries=None, active=None, externals=None, borders=()):
+        from . import ospfv3
         n = len(flats)
         self.lib = capi.load_library()
         self.handle = None
         self.router_id, self.flats, self.area_ids = router_id, list(flats), [int(a) for a in area_ids]
         self.borders = list(borders)
-        sums = [np.ascontiguousarray(s if s is not None else np.zeros(0, SUMMARY_LSA_DT), SUMMARY_LSA_DT)
+        self.v3 = bool(flats) and isinstance(flats[0], ospfv3.Flat)
+        sum_dt, ext_dt = (INTER_AREA_LSA_DT, EXTERNAL6_LSA_DT) if self.v3 else (SUMMARY_LSA_DT, EXTERNAL_LSA_DT)
+        sums = [np.ascontiguousarray(s if s is not None else np.zeros(0, sum_dt), sum_dt)
                 for s in (summaries if summaries is not None else [None] * n)]
-        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, EXTERNAL_LSA_DT), EXTERNAL_LSA_DT)
+        ext = np.ascontiguousarray(externals if externals is not None else np.zeros(0, ext_dt), ext_dt)
         self.summaries, self.externals = sums, ext
         self.active = [True] * n if active is None else [bool(a) for a in active]
         self.n_areas = n
@@ -845,11 +852,12 @@ class AbrBackboneTable:
         bt = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
         self._keep = (fl, ids, sp, ns, act, sums, ext, flats)
         h = C.c_void_p()
-        rc = self.lib.hspf_ospfv2_abr_backbone_table_create(router_id, n, fl, ids.ctypes.data, sp, ns.ctypes.data,
-                                                            act.ctypes.data, ext.ctypes.data if len(ext) else None,
-                                                            len(ext), bt, len(self.borders), C.byref(h))
+        create = "hspf_ospfv3_abr_backbone_table_create" if self.v3 else "hspf_ospfv2_abr_backbone_table_create"
+        rc = getattr(self.lib, create)(router_id, n, fl, ids.ctypes.data, sp, ns.ctypes.data, act.ctypes.data,
+                                       ext.ctypes.data if len(ext) else None, len(ext), bt, len(self.borders),
+                                       C.byref(h))
         if rc != capi.HSPF_OK:
-            raise capi.HspfError(rc, "hspf_ospfv2_abr_backbone_table_create failed")
+            raise capi.HspfError(rc, create + " failed")
         self.handle = h
         np_, pp, pl = C.c_uint32(), C.c_void_p(), C.c_void_p()
         assert self.lib.hspf_ospfv2_abr_backbone_table_prefixes(h, C.byref(np_), C.byref(pp), C.byref(pl)) == capi.HSPF_OK
@@ -859,6 +867,13 @@ class AbrBackboneTable:
         c = [C.c_uint32() for _ in range(4)]
         assert self.lib.hspf_ospfv2_abr_backbone_table_records(h, *[C.byref(x) for x in c]) == capi.HSPF_OK
         self.n_records, self.n_slots, self.n_asbr_slots, self.n_asbr_sets = [x.value for x in c]
+        if self.v3:
+            p6 = C.c_void_p()
+            rc = self.lib.hspf_ospfv3_abr_backbone_table_prefixes6(h, None, C.byref(p6), None)
+            if rc != capi.HSPF_OK:
+                raise capi.HspfError(rc, "hspf_ospfv3_abr_backbone_table_prefixes6 failed")
+            self.prefixes6 = route_table.copy_records(p6, self.n_prefixes, ospfv3.IP_DT)
+            self.prefix = self.prefixes6
 
     def upload(self, ctx: capi.Context):
         rc = self.lib.hspf_ospfv2_abr_backbone_table_upload(ctx.handle, self.handle)
@@ -909,3 +924,14 @@ def abr_backbone_from_cells(areas: list, t: AbrBackboneTable, cells: np.ndarray,
     HSPF_E_UNSUPPORTED is returned in the result, as rib_from_cells."""
     return _call_abr_rib_from_cells(capi.load_library().hspf_ospfv2_abr_backbone_from_cells, ospfv2.AreaStruct, areas,
                                     t, cells, gather_area, gather_v, gather_nh, RIB_ROUTE_DT, ospfv2.NEXTHOP_DT)
+
+
+def abr_backbone_from_cells_v3(areas: list, t: AbrBackboneTable, cells: np.ndarray, gather_area, gather_v,
+                               gather_nh) -> Rib:
+    """hspf_ospfv3_abr_backbone_from_cells (host): one job's cells over an OSPFv3 AbrBackboneTable -> R's routes for
+    the affected prefixes, prefix options included (RIB_ROUTE6_DT routes, ospfv3.NEXTHOP6_DT next hops).  areas: R's
+    ospfv3.Ospfv3Area images in the table's order; gathers (area, vertex, nh_mask) of R's row 0.  rc
+    HSPF_E_UNSUPPORTED is returned in the result, as rib_from_cells."""
+    from . import ospfv3
+    return _call_abr_rib_from_cells(capi.load_library().hspf_ospfv3_abr_backbone_from_cells, ospfv3.AreaStruct, areas,
+                                    t, cells, gather_area, gather_v, gather_nh, RIB_ROUTE6_DT, ospfv3.NEXTHOP6_DT)

@@ -834,6 +834,73 @@ def _lsa_array(rows, dt):
     return out
 
 
+def abr_backbone_view(t0: Topology, t1: Topology, t2: Topology, seed: int, r: int = 0, r2: int = 0,
+                      borders=((1, 0), (2, 1), (3, 2)), max_paths: int = 16, n_ext_keys: int = 3, area1_asbrs: int = 0,
+                      area1_ext: int = 4):
+    """The OSPFv3 twin of ospfv2.abr_backbone_view: an area border router R of area 0 and of an area only R borders,
+    and the borders of area 1, each as its own image: backbone_view's domain (areas 0 and 1, the three borders, the
+    first also in area 2, the area-0 ASBR, with area1_asbrs / area1_ext its area-1 ASBRs, their AS-external LSAs and the
+    borders' Inter-Area-Router LSAs), with R (router r of t0) also router r2 of synth_area(t2) as area 3 (area 2 is the
+    first border's), in ranges of its own, and the B flag in both of R's areas.  Seeded; area 3 draws from a generator
+    of its own.  Returns a dict:
+      r_areas       R's images [area 0, area 3] (area ids `area_ids` [0, 3]), `summaries` per area: backbone_view's
+                    summaries0 and none for area 3 (R is its only ABR);
+      externals     backbone_view's, plus an area-3 ASBR's ("area3_asbr", the E flag) AS-external LSAs: the area-0 ASBR's
+                    own /64, which every area-1 ASBR also advertises, and a /64 of its own ("area3_ext");
+      area3_shared  (address bytes, length) of a prefix the borders advertise into area 0 that is also a prefix of an
+                    area-3 router (intra-area at R);
+      flip          backbone_view's option flip: a /128 two area-1 routers advertise with the LA and the P option, at
+                    metrics that tie at the first border;
+      borders, shared, asbr, area1_asbrs, flip_ext  as backbone_view's (R has the B flag in the borders' area-0 images)."""
+    from . import ospf_rib
+    from .ospfv2 import _dist_from
+    v = backbone_view(t0, t1, seed, r=r, borders=borders, max_paths=max_paths, n_ext_keys=n_ext_keys,
+                      area1_asbrs=area1_asbrs, area1_ext=area1_ext)
+    rng = np.random.default_rng([seed, 0xAB3])
+    six = lambda hi, lo=0: ipaddress.IPv6Address((0x20010DB8 << 96) | (hi << 64) | lo).packed
+    rec = lambda b: (tuple(b), 1, (0, 0, 0))
+    R = RID_BASE + int(r)
+
+    def with_b(a, rids, bit=0x01):
+        a = Ospfv3Area(**{k: getattr(a, k) for k in a.__dataclass_fields__})
+        rl = a.router_lsas.copy()
+        for x in rids:
+            rl["flags"][rl["adv_rtr"] == x] |= bit
+        a.router_lsas = rl
+        return a
+    rids = [R if i == r2 else RID_BASE + i + (3 << 20) for i in range(t2.n_routers)]
+    a3 = synth_area(t2, root=r2, max_paths=max_paths, rids=rids, area_id=3)
+    pb = a3.prefixes["addr"]["bytes"]
+    pb[:, 5] = pb[:, 5] + 3
+    a3.prefixes["addr"]["bytes"] = pb
+    ifs = a3.ifaces.copy()
+    ifs["sort_key"] += 3000
+    ifs["ifindex"] += 3000
+    a3.ifaces = ifs
+    a3 = with_b(a3, [R])
+    fl = Flat(a3)
+    d = _dist_from(fl, fl.router_vertex(R))
+    reach = sorted(int(fl.router_ids[x]) for x in range(len(fl.router_ids)) if fl.is_router[x] and 0 < d[x] < 1 << 40)
+    t3 = v["summaries0"][v["summaries0"]["lsa_type"] == 3]
+    pick = t3[int(rng.integers(0, len(t3)))]
+    shared3 = (bytes(int(b) for b in pick["prefix"]["bytes"]), int(pick["len"]))
+    a3 = _with_prefixes(a3, {reach[int(rng.integers(0, len(reach)))]: [(shared3[0], shared3[1], 0, 1)]})
+    asbr3 = reach[int(rng.integers(0, len(reach)))]
+    a3 = with_b(a3, [asbr3], 0x02)
+    own3 = (six(0xE3_0000), 64)
+    ext = [tuple(x) for x in v["externals"].tolist()]
+    ext += [(asbr3, 1, 12, 12, rec(six(0xE0_0000)), 64, 0, 1, 0),
+            (asbr3, 2, int(rng.integers(1, 40)), 12, rec(own3[0]), 64, PFX_P, 0, 0)]
+    out_borders = [([with_b(a, [R]) if a.area_id == 0 else a for a in areas], ids, sums)
+                   for areas, ids, sums in v["borders"]]
+    return {"r_areas": [with_b(v["r_area"], [R]), a3], "area_ids": [0, 3],
+            "summaries": [v["summaries0"], np.zeros(0, ospf_rib.INTER_AREA_LSA_DT)],
+            "externals": _lsa_array(sorted(ext, key=lambda x: (x[0], x[1])), ospf_rib.EXTERNAL6_LSA_DT),
+            "area3_shared": shared3, "area3_asbr": asbr3, "area3_ext": own3, "borders": out_borders,
+            "shared": v["shared"], "flip": v["flip"], "asbr": v["asbr"], "area1_asbrs": v.get("area1_asbrs", []),
+            "flip_ext": v.get("flip_ext")}
+
+
 def nonbackbone_view(t0: Topology, t1: Topology, seed: int, spf, r: int | None = None,
                      borders=((1, 0), (2, 1), (3, 2)), max_paths: int = 16, n_ext_keys: int = 3, n_ext: int = 0):
     """The OSPFv3 twin of ospfv2.nonbackbone_view: an internal router R of area 1 and the area border routers

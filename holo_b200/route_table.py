@@ -196,6 +196,10 @@ def declare(lib: C.CDLL):
         "hspf_ospfv3_backbone_table_prefixes6": [vp, u32p, pvp, C.POINTER(u32p)],
         "hspf_ospfv3_backbone_from_cells": [vp, C.POINTER(ospfv3.AreaStruct), vp, vp, vp, u32,
                                             C.POINTER(ospf_rib.RibStruct)],
+        "hspf_ospfv3_abr_backbone_table_create": [u32, u32, vp, vp, vp, vp, vp, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv3_abr_backbone_table_prefixes6": [vp, u32p, pvp, C.POINTER(u32p)],
+        "hspf_ospfv3_abr_backbone_from_cells": [vp, C.POINTER(ospfv3.AreaStruct), u32, vp, vp, vp, vp, u32,
+                                                C.POINTER(ospf_rib.RibStruct)],
         "hspf_isis_backbone_from_cells": [C.POINTER(isis.InstanceStruct), vp, vp, C.POINTER(isis.JobPlanesStruct), vp,
                                           vp, C.POINTER(isis.RibStruct)],
     }

@@ -543,7 +543,8 @@ int hspf_ospfv2_nonbackbone_table_create(const hspf_ospfv2_flat *flat, uint32_t 
  *                                (border, area) plane sets, winners that do not fit.
  *   hspf_ospfv2_abr_backbone_table_prefixes  P, and the prefixes / lengths in prefix order (pointers may be NULL).
  *   hspf_ospfv2_abr_backbone_table_records   the record, slot, type-4 slot and plane-set counts: a slot's winner is
- *                                n_records + its slot index.
+ *                                n_records + its slot index (an OSPFv3 table's, hspf_ospfv3_abr_backbone_table_create:
+ *                                n_records + (slot index << 8 | prefix options)).
  *   hspf_ospfv2_abr_backbone_table_upload    copies the table to the ctx's device.
  *   hspf_ospfv2_abr_backbone_cells[16]  one thread per (job, prefix).  planes: host array of R's n_areas plane structs
  *                                (device, as given hspf_ospfv2_abr_rib_cells), row 0 read; border_cells /
@@ -557,6 +558,7 @@ int hspf_ospfv2_nonbackbone_table_create(const hspf_ospfv2_flat *flat, uint32_t 
  *   hspf_ospfv2_abr_backbone_delta[16]  the route-delta stage over the same walk (base cells as hspf_ospfv2_rib_delta).
  *   hspf_ospfv2_abr_backbone_from_cells host: one job's cells -> exactly the routes of the affected prefixes of the
  *                                contract.  areas / gathers as hspf_ospfv2_abr_rib_from_cells, of R's row 0.
+ *                                HSPF_E_INVAL for an OSPFv3 table (hspf_ospfv3_abr_backbone_from_cells decodes those).
  */
 typedef struct hspf_ospfv2_abr_backbone_table hspf_ospfv2_abr_backbone_table;
 int hspf_ospfv2_abr_backbone_table_create(uint32_t router_id, uint32_t n_areas, const hspf_ospfv2_flat *const *flats,
@@ -713,6 +715,53 @@ int hspf_ospfv3_nonbackbone_table_create(const struct hspf_ospfv3_flat *flat, ui
                                          const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
                                          const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
                                          hspf_ospfv2_backbone_table **out);
+
+/*
+ * Area border router over what-if jobs inside an area it is not attached to, OSPFv3: the
+ * hspf_ospfv2_abr_backbone_table_create stage over Inter-Area-Prefix / Inter-Area-Router LSAs, with the same
+ * contract on jobs and borders.  The borders' cells of job j come from hspf_ospfv2_abr_rib_cells[16] over their
+ * hspf_ospfv3_abr_ribtable_create tables, with each border's row of the perturbed area for the job and row 0 of its
+ * other areas.  For job j, with border b's cells of j decoded to rib_b (hspf_ospfv3_abr_rib_from_cells) over its areas
+ * areas_b, the decoded cells of j equal the affected-prefix routes, prefix options included, of
+ *     hspf_ospfv3_update_rib_full(R, max_paths, [{A_i.area_id, area_from_planes(A_i, R's row 0 of A_i), ifaces,
+ *         S_i, active_i}], X)
+ * where S_i is area i's Inter-Area-Prefix / Inter-Area-Router LSAs, area 0's with each border's own replaced by
+ * hspf_ospfv3_net_summaries(rib_b, areas_b, target area 0) and hspf_ospfv3_rtr_summaries(areas_b, target area 0), in
+ * LsaKey order.  A border advertises a route as the OSPFv2 stage says, and its LSA carries the prefix options of the
+ * border cell's winning intra-area record; the Inter-Area-Router slots are the OSPFv2 stage's type-4 slots.  The
+ * options of an Inter-Area-Router LSA are outside the contract, as they are for hspf_ospfv3_rtr_summaries.
+ *
+ *   hspf_ospfv3_abr_backbone_table_create  host.  The arguments of hspf_ospfv3_abr_ribtable_create (R's OSPFv3 areas in
+ *                                instance order; area 0's LSAs as in R's LSDB, borders' LSAs included), plus the
+ *                                borders' OSPFv3 ABR tables, which must outlive the table.  The result is an
+ *                                hspf_ospfv2_abr_backbone_table marked OSPFv3: hspf_ospfv2_abr_backbone_table_free /
+ *                                _records / _upload and hspf_ospfv2_abr_backbone_cells[16] / _delta[16] take it (the
+ *                                mark picks the walk), and a slot's winner is n_records + (slot index << 8 | the prefix
+ *                                options of the border's LSA): a border route that changes record at an equal metric,
+ *                                to one with other options, changes R's winner, and the route-delta stage reports
+ *                                OTHER.  Refusals: those of the OSPFv2 call, with an OSPFv2 border table HSPF_E_INVAL
+ *                                and slot winners that would not fit 32 bits HSPF_E_UNSUPPORTED.  Inter-Area-Prefix
+ *                                LSAs with the NU option are left out, a border's included.
+ *   hspf_ospfv3_abr_backbone_table_prefixes6  P, and the IPv6 prefixes / lengths in prefix order (pointers may be
+ *                                NULL); HSPF_E_INVAL for an OSPFv2 table.
+ *   hspf_ospfv3_abr_backbone_from_cells  host: one job's cells -> exactly the routes of the affected prefixes of the
+ *                                contract, a slot winner's prefix options read from the winner.  areas: R's
+ *                                hl_ospfv3_area images in the table's order; gathers as
+ *                                hspf_ospfv2_abr_backbone_from_cells.  The create and decode of each version refuse a
+ *                                table of the other (HSPF_E_INVAL).
+ */
+int hspf_ospfv3_abr_backbone_table_create(uint32_t router_id, uint32_t n_areas, const struct hspf_ospfv3_flat *const *flats,
+                                          const uint32_t *area_ids, const hl_ospfv3_inter_area_lsa *const *summaries,
+                                          const uint32_t *n_summaries, const uint8_t *active,
+                                          const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
+                                          const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
+                                          hspf_ospfv2_abr_backbone_table **out);
+int hspf_ospfv3_abr_backbone_table_prefixes6(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_prefixes,
+                                             const hl_ip_addr **prefixes, const uint32_t **lens);
+int hspf_ospfv3_abr_backbone_from_cells(const hspf_ospfv2_abr_backbone_table *t, const hl_ospfv3_area *areas,
+                                        uint32_t n_areas, const hl_ospf_rib_cell *cells, const uint32_t *gather_area,
+                                        const uint32_t *gather_v, const uint64_t *gather_nh, uint32_t n_gather,
+                                        hl_ospfv3_rib *out);
 
 /*
  * The stages of update_rib_full that follow the per-area SPFs (holo-ospf/src/route.rs:146-193):
