@@ -269,6 +269,64 @@ HSPF_HD uint32_t abr_row0_status(const AbrPlaneSet<D, N> &s, uint32_t n_areas) {
     return st;
 }
 
+// ---- a non-backbone router over jobs inside another non-backbone area (hspf_ospfv2_third_area_table_create) --------
+// R is an internal router of area 2, the jobs perturb area 1, and the borders are area 2's ABRs attached to area 0
+// (C), each an hspf_ospfv2_abr_backbone_table over area 1's ABRs (B).  A type-3 slot reads C's cell of the job as a
+// kNonBackbone slot does.  When area 1 holds an ASBR A, C's area-0 entry for A is inter-area, through the B's type-4
+// LSAs, and moves with the job; so does the metric of the type-4 LSA C originates for A into area 2.  R's type-4 range
+// for A then holds one chain slot per C, at C's place in LsaKey order:
+//   chain slot: x C's vertex, y the group's index among C's groups with type-4 slots, z C, w kOspfBackboneAsbrSlot | C
+// and the walk reads C's entry of the job (abr_asbr_entry below, stored by hspf_ospfv2_abr_backbone_asbr_entries).
+constexpr uint32_t kOspfNoEntry = 0xFFFFFFFFu;        // an entry C does not originate a type-4 LSA for
+
+// C's area-0 entry of an ASBR, as rib_full step 2 leaves it and compute_rtr_summaries re-originates it into a normal
+// area: the last type-4 record of the entry's range (`e`, an ASBR entry record of C's area 0) whose ABR C reaches and,
+// for a type-4 slot, whose border originates (asbr), else the ASBR's own vertex with the E flag; its metric, or
+// kOspfNoEntry when there is none or it is not below LSInfinity.  The same loop as abr_rib_cell_eval's step 4 for one
+// area, kept apart so that the kernels over that walk keep their code.
+template <class Planes, class D>
+HSPF_HD uint32_t abr_asbr_entry(const Planes &pl, const OspfAsbrJob<Planes, D> &asbr, const RibRec *recs, uint32_t e) {
+    const RibRec s = load_rib_rec(recs + e);
+    uint32_t m = kOspfNoEntry;
+    bool found = false;
+    for (uint32_t k = s.w; k > s.z && !found; --k) {
+        const RibRec f = load_rib_rec(recs + k - 1);
+        if (!pl.reached(f.x)) continue;
+        uint32_t fm = f.y;
+        if ((f.w & kOspfBackboneAsbrSlot) && !asbr.originates(f.w & ~kOspfBackboneAsbrSlot, f.y, fm)) continue;
+        m = pl.d(f.x) + fm; found = true;
+    }
+    if (!found && s.y && pl.reached(s.x)) m = pl.d(s.x);
+    return m < HL_LSA_INFINITY ? m : kOspfNoEntry;
+}
+
+// Each C's entries of the jobs, u32 [n_jobs][G[b]] (kOspfNoEntry: no type-4 LSA), and their status words (may be NULL).
+struct OspfChainSet {
+    const uint32_t *entries[kOspfBackboneMaxBorders];
+    const uint32_t *status[kOspfBackboneMaxBorders];
+    uint32_t G[kOspfBackboneMaxBorders];
+};
+
+// One job of the set, as OspfAsbrJob: whether C (b) originates a type-4 LSA for its group g, and at what metric.
+struct OspfChainJob {
+    const OspfChainSet &s;
+    uint32_t j;
+    HSPF_HD bool originates(uint32_t b, uint32_t g, uint32_t &metric) const {
+#if defined(__CUDA_ARCH__)
+        metric = __ldg(s.entries[b] + (size_t)j * s.G[b] + g);
+#else
+        metric = s.entries[b][(size_t)j * s.G[b] + g];
+#endif
+        return metric != kOspfNoEntry;
+    }
+};
+
+// R's planes of a job over a table with chain slots, with the job's entries beside them (as OspfAsbrPlanes).
+template <class Planes>
+struct OspfThirdAreaPlanes : Planes {
+    OspfChainJob asbr;
+};
+
 }  // namespace hspf
 
 // Host + device image of an area border router's affected prefixes over jobs inside another area
@@ -288,6 +346,10 @@ struct hspf_ospfv2_abr_backbone_table {
     std::vector<uint32_t> words;                 // abr->off, padded to 16 bytes, then border [4 n_borders] (OSPFv3:
                                                  // [8 n_borders], then each border's options bytes)
     hspf::DeviceRouteTable dev;                  // words, then records
+    // the ASBR entry groups whose area-0 type-4 range holds type-4 slots, ascending: the entries
+    // hspf_ospfv2_abr_backbone_asbr_entries computes, and the chain slots of a third-area table
+    std::vector<uint32_t> asbr_group, asbr_group_id;   // ... and each one's ASBR id
+    hspf::DeviceRouteTable entry_dev;            // per such group its area-0 entry record (uploaded when there is one)
 
     uint32_t P() const { return (uint32_t)abr->prefix.size(); }
     uint32_t n_recs() const { return (uint32_t)abr->recs.size(); }
@@ -326,6 +388,10 @@ struct hspf_ospfv2_backbone_table {
     bool v3 = false;
     std::vector<hl_ip_addr> prefix6;
     std::vector<uint8_t> options6;
+    // hspf_ospfv2_third_area_table_create: the borders are C tables (borders[b] is third[b]->abr), and the type-4
+    // slots are chain slots (n_asbr_slots of them, no plane set), read by the third-area calls only
+    bool third_area = false;
+    const hspf_ospfv2_abr_backbone_table *third[hspf::kOspfBackboneMaxBorders] = {};
     hspf::DeviceRouteTable dev;                  // hspf_ospfv2_backbone_table_upload: words, then records
 
     uint32_t P() const { return (uint32_t)prefix.size(); }

@@ -442,6 +442,17 @@ inline std::array<uint32_t, 4> border_words(const hspf_ospfv2_abr_ribtable &bt, 
     return {lo, lo + bt.area[i]->n_intra, (uint32_t)atoms, (uint32_t)(atoms >> 32)};
 }
 
+// Border C's words over a third-area table (build_backbone_table with `third`): the walk's intra-area records of
+// area index i of C's restricted table (an intra-area winner of C's cells is one of those), and i's atom bits.
+inline std::array<uint32_t, 4> walk_border_words(const hspf_ospfv2_abr_backbone_table &c, uint32_t i) {
+    const hspf_ospfv2_abr_ribtable &a = *c.abr;
+    const size_t S = a.prefix.size() + 1;
+    std::array<uint32_t, 4> w = border_words(a, i);
+    w[0] = a.off[i * S];
+    w[1] = a.off[i * S + S - 1];
+    return w;
+}
+
 // Every border's words over its target-area index at[b], appended to `words` (which ends on a 16-byte boundary).
 // OSPFv3 (kV3): 8 words per border, the fifth the byte offset from the first border word of the border's options
 // bytes, which follow all the border words, each border's padded to a word: one per record an advertised cell's
@@ -500,16 +511,22 @@ int append_border_words(std::vector<uint32_t> &words, const hspf_ospfv2_abr_ribt
 // (plane sets of any of those areas, area 0 included); in a stub area the default route stays static and no type-4
 // LSA is originated, and a totally stubby area has no slot.  OSPFv3: a border's options bytes also cover its type-3
 // records, so that an inter-area cell's winner gives the options of the LSA the border copies them from.
+// `third` (OSPFv2 with `config`, build_third_area_table): borders[b] is third[b]->abr, C's table restricted to its
+// affected prefixes.  A C LSA for a key outside C's prefixes, or a type-4 LSA for an ASBR without type-4 slots in C's
+// table, stays a static record; the type-4 slots are chain slots (ospf_backbone_cells.h: OspfChainJob), one per (C,
+// group of C with type-4 slots), and the border words name C's walk intra-area records (walk_border_words).
 template <class T>
 int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const typename T::Sum *sums, uint32_t n_sums,
                          const typename T::Ext *ext, uint32_t n_ext, const hspf_ospfv2_abr_ribtable *const *borders,
                          uint32_t n_borders, hspf_ospfv2_backbone_table **out, bool asbr = false,
-                         const hl_ospf_area_config *config = nullptr) {
+                         const hl_ospf_area_config *config = nullptr,
+                         const hspf_ospfv2_abr_backbone_table *const *third = nullptr) {
     using Key = typename T::Key;
     using Sum = typename T::Sum;
     constexpr uint32_t kNone = 0xFFFFFFFFu;
     if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext) || !borders) return HSPF_E_INVAL;
     *out = nullptr;
+    if (third && (T::kV3 || !config)) return HSPF_E_INVAL;
     const bool nb = config != nullptr;                            // a non-backbone target area
     const uint32_t ta = nb ? flat->area->area_id : 0;
     if (nb) {
@@ -530,6 +547,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         if (root == kNone || (flags(root) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
         t->router_id = router_id; t->root = root; t->n_vertices = T::n_vertices(f);
         t->max_paths = f.area->max_paths; t->n_borders = n_borders; t->v3 = T::kV3; t->area_id = ta; t->asbr = asbr;
+        t->third_area = third != nullptr;
         // per border: its area-0 index, its target-area index, its vertex
         std::vector<uint32_t> a0(n_borders), at(n_borders), bv(n_borders);
         std::unordered_map<uint32_t, uint32_t> border_of;           // router id -> border
@@ -545,6 +563,12 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
             bv[b] = vertex(bt->router_id);
             if (a0[b] == kNone || at[b] == kNone || !(flags(bv[b]) & HL_RTR_FLAG_B)) return HSPF_E_INVAL;
             t->borders[b] = bt;
+            if (third) {
+                t->third[b] = third[b];
+                // a border of C's that is a router of R's area is an ABR of both areas
+                for (uint32_t k = 0; k < third[b]->n_borders; ++k)
+                    if (vertex(third[b]->borders[k]->router_id) != kNone) return HSPF_E_UNSUPPORTED;
+            }
             if (nb) {
                 // an inter-area router entry at the border (from another ABR's type-4 LSA in area 0) would be
                 // re-originated into A at a distance the job moves
@@ -564,10 +588,23 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         std::vector<Sum> rest;
         std::vector<std::pair<uint32_t, Key>> border_t3;            // (border, prefix key) of the borders' LSAs
         std::vector<std::pair<uint32_t, uint32_t>> border_t4;       // (border, ASBR id)
+        // third: per C, the keys of its prefixes and the ASBRs of its groups with type-4 slots (chain ids)
+        std::vector<std::map<Key, uint32_t>> c_keys(third ? n_borders : 0);
+        std::vector<std::map<uint32_t, uint32_t>> c_ids(third ? n_borders : 0);
+        for (uint32_t b = 0; third && b < n_borders; ++b) {
+            const hspf_ospfv2_abr_ribtable &ca = *borders[b];
+            for (uint32_t u = 0; u < (uint32_t)ca.prefix.size(); ++u) c_keys[b].emplace(T::table_key(ca, u), u);
+            for (uint32_t g = 0; g < (uint32_t)third[b]->asbr_group.size(); ++g)
+                c_ids[b].emplace(ca.group_asbr[third[b]->asbr_group[g]], g);
+        }
+        auto stays = [&](uint32_t b, const Sum &l) {                 // a C LSA the job cannot move
+            if (!third) return false;
+            return l.lsa_type == 3 ? !c_keys[b].count(T::key(l)) : !c_ids[b].count(T::asbr_id(l));
+        };
         for (uint32_t i = 0; i < n_sums; ++i) {
             const Sum &l = sums[i];
             auto it = border_of.find(l.adv_rtr);
-            if (it == border_of.end() || stub_default(l)) { rest.push_back(l); continue; }
+            if (it == border_of.end() || stub_default(l) || stays(it->second, l)) { rest.push_back(l); continue; }
             if (!live(l)) continue;
             if (l.lsa_type == 4) {                                   // re-originated per job too
                 if (!asbr) return HSPF_E_UNSUPPORTED;
@@ -585,7 +622,13 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         // it is a router with the E flag, each border's in area order (none into a stub area)
         std::map<uint32_t, BorderSlots> orig;
         if (asbr && normal) {
-            if (const int rc2 = border_asbr_origins(borders, n_borders, ta, orig)) return rc2;
+            if (third) {                                             // chain slots: C's groups with type-4 slots
+                for (uint32_t b = 0; b < n_borders; ++b)
+                    for (const auto &e : c_ids[b]) orig[e.first].emplace_back(b, e.second);
+                for (auto &e : orig) sort_by_router_id(e.second, borders);
+            } else if (const int rc2 = border_asbr_origins(borders, n_borders, ta, orig)) {
+                return rc2;
+            }
             for (const auto &x : border_t4)
                 if (!has_border(orig, x.second, x.first)) return HSPF_E_INVAL;   // the LSDB disagrees with the border's table
         }
@@ -679,7 +722,8 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
                     st != t4.end() ? st->second : none, [](const std::pair<uint32_t, RibRec> &x) { return x.first; },
                     o->second, borders, [&](const std::pair<uint32_t, RibRec> &x) { t->recs.push_back(x.second); },
                     [&](const std::pair<uint32_t, uint32_t> &x) {
-                        t->recs.push_back(asbr_slot(borders, bv[x.first], x, id, set_of, t->asbr_set));
+                        t->recs.push_back(third ? RibRec{bv[x.first], x.second, x.first, kOspfBackboneAsbrSlot | x.first}
+                                                : asbr_slot(borders, bv[x.first], x, id, set_of, t->asbr_set));
                         ++t->n_asbr_slots;
                     });
                 RibRec &s = t->recs[r.ext_end + a];
@@ -694,7 +738,14 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         t->words.insert(t->words.end(), o3.begin(), o3.end());
         t->words.insert(t->words.end(), o5.begin(), o5.end());
         t->words.resize(t->border_at(), 0);
-        if (const int rc2 = append_border_words<T::kV3>(t->words, borders, n_borders, at.data(), nb)) return rc2;
+        if (third) {
+            for (uint32_t b = 0; b < n_borders; ++b) {
+                const std::array<uint32_t, 4> bw = walk_border_words(*third[b], at[b]);
+                t->words.insert(t->words.end(), bw.begin(), bw.end());
+            }
+        } else if (const int rc2 = append_border_words<T::kV3>(t->words, borders, n_borders, at.data(), nb)) {
+            return rc2;
+        }
         *out = t.release();
         return HSPF_OK;
     } catch (const std::bad_alloc &) {
@@ -702,6 +753,26 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
     } catch (...) {
         return HSPF_E_UNSUPPORTED;
     }
+}
+
+// hspf_ospfv2_third_area_table_create, argument checks included: an internal router R of a non-backbone area over
+// jobs inside another non-backbone area.  The borders are R's area's ABRs attached to area 0 (C), each an OSPFv2
+// abr_backbone table over the perturbed area's ABRs; the table is build_backbone_table's `config` path over the C's
+// restricted tables, with `third` (chain slots, the walk's border words).
+template <class T>
+int build_third_area_table(const typename T::Flat *flat, uint32_t router_id, const hl_ospf_area_config *config,
+                           const typename T::Sum *sums, uint32_t n_sums, const typename T::Ext *ext, uint32_t n_ext,
+                           const hspf_ospfv2_abr_backbone_table *const *borders, uint32_t n_borders,
+                           hspf_ospfv2_backbone_table **out) {
+    if (out) *out = nullptr;
+    if (!config || !borders || n_borders == 0 || n_borders > kOspfBackboneMaxBorders) return HSPF_E_INVAL;
+    const hspf_ospfv2_abr_ribtable *abr[kOspfBackboneMaxBorders];
+    for (uint32_t b = 0; b < n_borders; ++b) {
+        if (!borders[b] || !borders[b]->abr) return HSPF_E_INVAL;
+        abr[b] = borders[b]->abr;
+    }
+    return build_backbone_table<T>(flat, router_id, sums, n_sums, ext, n_ext, abr, n_borders, out, true, config,
+                                   borders);
 }
 
 // hspf_ospfv2_abr_backbone_table_create, argument checks included: an area border router R of area 0 and other areas
@@ -899,6 +970,8 @@ int build_abr_backbone_table(uint32_t router_id, uint32_t n_areas, const typenam
                              ++t->n_asbr_slots;
                          });
             recs[r->ext_end + g * A + i0] = RibRec{s.x, s.y, z, (uint32_t)recs.size()};
+            t->asbr_group.push_back(g);
+            t->asbr_group_id.push_back(o->first);
         }
         if (t->asbr_set.size() > kOspfBackboneMaxAsbrSets) return HSPF_E_UNSUPPORTED;   // the kernel parameter's
         // the walk's intra-area ranges: the affected prefixes' records again, each naming its decode record

@@ -117,14 +117,101 @@ int abr_backbone(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_
                             border_rows, out);
 }
 
+// ---- C's ASBR entries per job (hspf_ospfv2_abr_backbone_asbr_entries) ----------------------------------------------
+// C's area-0 planes (row 0) and the plane sets its type-4 slots read; group k's entry record is group_rec[k].
+template <class D, class N>
+struct AbrEntryArgs {
+    hspf::AbrPlaneSet<D, N> s;
+    hspf::OspfAsbrSets<D> sets;
+    const hspf::RibRec *recs;
+    const uint32_t *group_rec;
+    uint32_t n_areas, area0, G;
+};
+
+// One thread per (job, group), then per job its status word: C's row-0 words and the job's rows' words.  A job with a
+// non-zero word gets kOspfNoEntry.
+template <class Planes, class D, class N>
+__global__ void __launch_bounds__(hspf::kRouteThreads)
+abr_asbr_entries_kernel(const AbrEntryArgs<D, N> a, uint32_t n_jobs, uint32_t *__restrict__ status_out,
+                        uint32_t *__restrict__ entries) {
+    const uint64_t stride = (uint64_t)gridDim.x * blockDim.x, first = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    const uint32_t row0 = hspf::abr_row0_status(a.s, a.n_areas);
+    if (status_out)
+        for (uint64_t j = first; j < n_jobs; j += stride) status_out[j] = row0 | hspf::asbr_job_status(a.sets, (uint32_t)j);
+    const uint64_t total = (uint64_t)n_jobs * a.G;
+    for (uint64_t idx = first; idx < total; idx += stride) {
+        const uint32_t j = (uint32_t)(idx / a.G), k = (uint32_t)(idx - (uint64_t)j * a.G);
+        uint32_t m = hspf::kOspfNoEntry;
+        if (!(row0 | hspf::asbr_job_status(a.sets, j))) {
+            const Planes pl{a.s.dist[a.area0], a.s.hops[a.area0], a.s.nh[a.area0]};
+            const hspf::OspfAsbrJob<Planes, D> asbr{a.sets, j};
+            m = hspf::abr_asbr_entry(pl, asbr, a.recs, __ldg(a.group_rec + k));
+        }
+        entries[idx] = m;
+    }
+}
+
+template <class R>
+int asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
+                 const R *const *border_planes, const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                 uint32_t *job_status_out, uint32_t *entries) {
+    using P = hspf::PlanesOf<R>;
+    using Rows = hspf::ResultPlanes<P>;
+    if (!ctx || !t || !t->abr || t->abr->v3 || !t->dev.blob || !planes) return HSPF_E_INVAL;
+    const uint32_t G = (uint32_t)t->asbr_group.size();
+    if ((n_jobs && G && !entries) || (reinterpret_cast<uintptr_t>(entries) & 3u) ||
+        (reinterpret_cast<uintptr_t>(job_status_out) & 3u) || (G && !t->entry_dev.blob))
+        return HSPF_E_INVAL;
+    const hspf_ospfv2_abr_ribtable &a = *t->abr;
+    AbrEntryArgs<typename Rows::D, typename Rows::N> args{};
+    for (uint32_t i = 0; i < a.n_areas; ++i) {
+        Rows p;
+        if (hspf::result_planes(&planes[i], a.n_vertices[i], p) || !p.complete()) return HSPF_E_INVAL;
+        args.s.dist[i] = p.dist; args.s.hops[i] = p.hops; args.s.nh[i] = p.nh; args.s.status[i] = p.status;
+        args.s.V[i] = p.V; args.s.n_rows[i] = 1;
+    }
+    if (const int rc = hspf::bind_ospf_asbr_sets(*t, border_planes, border_n_rows, border_rows, n_jobs, args)) return rc;
+    args.recs = static_cast<const hspf::RibRec *>(t->dev.contribs);
+    args.group_rec = t->entry_dev.off;
+    args.n_areas = a.n_areas; args.area0 = t->area0; args.G = G;
+    const uint64_t items = std::max<uint64_t>((uint64_t)n_jobs * G, job_status_out ? n_jobs : 0u);
+    if (items == 0) return HSPF_OK;
+    uint32_t blocks = 0;
+    if (const int rc = hspf::route_grid(ctx, t->dev, items, hspf::kRouteBlocksPerSM, blocks)) return rc;
+    abr_asbr_entries_kernel<P><<<blocks, hspf::kRouteThreads, 0, static_cast<cudaStream_t>(hspf_stream(ctx))>>>(
+        args, n_jobs, job_status_out, entries);
+    if (cudaGetLastError() != cudaSuccess) return HSPF_E_CUDA;
+    hspf_note_launches(ctx, 1);
+    return HSPF_OK;
+}
+
 }  // namespace
 
 extern "C" {
 
 int hspf_ospfv2_abr_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_abr_backbone_table *t) {
     if (!t || !t->abr) return HSPF_E_INVAL;
-    return hspf::upload_route_table(ctx, t->dev, t->words, t->abr->recs.data(),
-                                    t->abr->recs.size() * sizeof(hspf::RibRec));
+    const int rc = hspf::upload_route_table(ctx, t->dev, t->words, t->abr->recs.data(),
+                                            t->abr->recs.size() * sizeof(hspf::RibRec));
+    if (rc || t->asbr_group.empty() || t->abr->v3) return rc;
+    // the entry record of each group with type-4 slots, for hspf_ospfv2_abr_backbone_asbr_entries (OSPFv2 only)
+    std::vector<uint32_t> rec;
+    for (uint32_t g : t->asbr_group) rec.push_back(t->abr->ext_end + g * t->abr->n_areas + t->area0);
+    return hspf::upload_route_table(ctx, t->entry_dev, rec, nullptr, 0);
+}
+
+int hspf_ospfv2_abr_backbone_asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                          const hspf_result *planes, const hspf_result *const *border_planes,
+                                          const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                          uint32_t *job_status_out, uint32_t *entries) {
+    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries);
+}
+
+int hspf_ospfv2_abr_backbone_asbr_entries16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                            const hspf_result16 *planes, const hspf_result16 *const *border_planes,
+                                            const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                            uint32_t *job_status_out, uint32_t *entries) {
+    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries);
 }
 
 int hspf_ospfv2_abr_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,

@@ -108,15 +108,39 @@ struct OspfBackboneAsbrV3Cell : OspfBackboneAsbrCell<Planes> {
     }
 };
 
+// The walk over a third-area table with chain slots (hspf_ospfv2_third_area_table_create): the kNonBackbone walk, with
+// each chain slot reading its border's entries of the job, whose status words enter the job's.  A type of its own, so
+// that the kernels above keep their instantiations.
+template <class Planes>
+struct OspfThirdAreaCell : OspfBackboneCell<Planes, false> {
+    using Base = OspfBackboneCell<Planes, false>;
+    hspf::OspfChainSet chain;
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
+        uint32_t s = Base::status_word(j);
+        for (uint32_t b = 0; b < this->n_borders; ++b)
+            if (chain.status[b]) s |= chain.status[b][j];
+        return s;
+    }
+    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
+        const hspf::OspfThirdAreaPlanes<Planes> pl{this->pl.job(0), {chain, j}};
+        return hspf::ospf_backbone_cell_eval<false, true, true>(pl, this->t, p, rows);
+    }
+};
+
 // Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
-// and for OSPFv3 tables, for OSPFv2 and OSPFv3 tables with type-4 / Inter-Area-Router slots, and for OSPFv2 and
-// OSPFv3 tables of a non-backbone target area.
+// and for OSPFv3 tables, for OSPFv2 and OSPFv3 tables with type-4 / Inter-Area-Router slots, for OSPFv2 and OSPFv3
+// tables of a non-backbone target area, and for third-area tables with chain slots.
 constexpr uint32_t kBackboneBlocksPerSM = 4;
 constexpr uint32_t kBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kBackboneAsbrBlocksPerSM = 4;
 constexpr uint32_t kBackboneAsbrV3BlocksPerSM = 4;
 constexpr uint32_t kNonBackboneBlocksPerSM = 4;
 constexpr uint32_t kNonBackboneV3BlocksPerSM = 4;
+constexpr uint32_t kThirdAreaBlocksPerSM = 4;
 
 template <class R, bool kV3>
 int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
@@ -164,6 +188,31 @@ int nonbackbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_j
                        ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out);
 }
 
+// A third-area table: with chain slots the OspfThirdAreaCell walk over each border's entries (border_entries[b] u32
+// [n_jobs][G_b], NULL allowed for a border with no group and for a table without chain slots), else the plain
+// kNonBackbone walk.
+template <class R, class Out>
+int third_area(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+               const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+               const uint32_t *const *border_entries, const uint32_t *const *border_entry_status, const Out &out) {
+    if (!t || !t->third_area) return HSPF_E_INVAL;
+    if (!t->n_asbr_slots)
+        return nonbackbone<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr, out);
+    OspfThirdAreaCell<hspf::PlanesOf<R>> cell{};
+    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
+    if (!border_entries) return HSPF_E_INVAL;
+    for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
+        cell.chain.entries[b] = nullptr; cell.chain.status[b] = nullptr; cell.chain.G[b] = 0;
+        if (b >= t->n_borders) continue;
+        cell.chain.G[b] = (uint32_t)t->third[b]->asbr_group.size();
+        cell.chain.entries[b] = border_entries[b];
+        cell.chain.status[b] = border_entry_status ? border_entry_status[b] : nullptr;
+        if (cell.chain.G[b] && (!border_entries[b] || (reinterpret_cast<uintptr_t>(border_entries[b]) & 3u)))
+            return HSPF_E_INVAL;
+    }
+    return hspf::launch_route_stage<kThirdAreaBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), out);
+}
+
 // the walk of the table's version and target area; a table with type-4 slots is backbone_asbr's
 template <class R, class Out>
 int backbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
@@ -182,7 +231,8 @@ int backbone_asbr(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n
                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                   const R *const *border_planes, const uint32_t *const *border_n_rows,
                   const uint32_t *const *border_rows, const Out &out) {
-    if (!t || (t->v3 && !t->area_id && !t->asbr)) return HSPF_E_INVAL;
+    // a third-area table's type-4 slots are chain slots, which only the third-area calls read
+    if (!t || (t->v3 && !t->area_id && !t->asbr) || (t->third_area && t->n_asbr_slots)) return HSPF_E_INVAL;
     if (t->area_id)
         return nonbackbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
                            border_rows, out);
@@ -273,6 +323,44 @@ int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_
                                       uint64_t *n_records) {
     return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
                          hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+}
+
+int hspf_ospfv2_third_area_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                 const uint32_t *const *border_entry_status, uint32_t *job_status_out,
+                                 hl_ospf_rib_cell *cells) {
+    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
+                      hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+}
+
+int hspf_ospfv2_third_area_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                   const uint32_t *const *border_entry_status, uint32_t *job_status_out,
+                                   hl_ospf_rib_cell *cells) {
+    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
+                      hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+}
+
+int hspf_ospfv2_third_area_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                 const uint32_t *const *border_entry_status, const hl_ospf_rib_cell *base_cells,
+                                 uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                                 hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
+                      hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+}
+
+int hspf_ospfv2_third_area_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                   const uint32_t *const *border_entry_status, const hl_ospf_rib_cell *base_cells,
+                                   uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                                   hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
+    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
+                      hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

@@ -1279,6 +1279,15 @@ int hspf_ospfv2_nonbackbone_table_create(const hspf_ospfv2_flat *flat, uint32_t 
                                              config);
 }
 
+int hspf_ospfv2_third_area_table_create(const hspf_ospfv2_flat *flat, uint32_t router_id,
+                                        const hl_ospf_area_config *config, const hl_ospfv2_summary_lsa *sums,
+                                        uint32_t n_sums, const hl_ospfv2_external_lsa *ext, uint32_t n_ext,
+                                        const hspf_ospfv2_abr_backbone_table *const *borders, uint32_t n_borders,
+                                        hspf_ospfv2_backbone_table **out) {
+    return hspf::build_third_area_table<RibV2>(flat, router_id, config, sums, n_sums, ext, n_ext, borders, n_borders,
+                                               out);
+}
+
 int hspf_ospfv2_backbone_table_asbr_slots(const hspf_ospfv2_backbone_table *t, uint32_t *n_slots, uint32_t *n_sets) {
     if (!t) return HSPF_E_INVAL;
     if (n_slots) *n_slots = t->n_asbr_slots;
@@ -1315,6 +1324,7 @@ int hspf_ospfv2_backbone_from_cells(const hspf_ospfv2_backbone_table *t, const h
 void hspf_ospfv2_abr_backbone_table_free(hspf_ospfv2_abr_backbone_table *t) {
     if (!t) return;
     hspf::release_route_table(t->dev);
+    hspf::release_route_table(t->entry_dev);
     hspf_ospfv2_abr_ribtable_free(t->abr);
     delete t;
 }
@@ -1345,6 +1355,14 @@ int hspf_ospfv2_abr_backbone_table_records(const hspf_ospfv2_abr_backbone_table 
     if (n_slots) *n_slots = (uint32_t)t->slot_rec.size();
     if (n_asbr_slots) *n_asbr_slots = t->n_asbr_slots;
     if (n_asbr_sets) *n_asbr_sets = (uint32_t)t->asbr_set.size();
+    return HSPF_OK;
+}
+
+int hspf_ospfv2_abr_backbone_table_asbrs(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_groups,
+                                         const uint32_t **asbr_ids) {
+    if (!t || !t->abr) return HSPF_E_INVAL;
+    if (n_groups) *n_groups = (uint32_t)t->asbr_group.size();
+    if (asbr_ids) *asbr_ids = t->asbr_group_id.data();
     return HSPF_OK;
 }
 

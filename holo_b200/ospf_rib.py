@@ -658,7 +658,13 @@ class BackboneTable:
     target area, `area_id`) over what-if jobs on the backbone; `summaries` are that area's type-3/4 (Inter-Area-Prefix
     / Inter-Area-Router) LSAs, `config` its configuration, and the borders' type-4 LSAs are re-originated per job as
     with asbr=True.  The device calls of both kinds take it; backbone_from_cells (backbone_from_cells_v3) decodes it
-    over R's image of the area."""
+    over R's image of the area.
+
+    config=area_config(...) with AbrBackboneTable borders: hspf_ospfv2_third_area_table_create, the table of an
+    internal router R of a non-backbone area over what-if jobs inside another non-backbone area; the borders are R's
+    area's ABRs attached to area 0, each over the perturbed area's ABRs.  `third_area` is set; `n_asbr_slots` are chain
+    slots, which read the borders' abr_backbone_asbr_entries_device output through third_area_cells_device /
+    third_area_delta_device; a table without them also runs through the backbone calls."""
 
     def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=(), asbr: bool = False,
                  config=None):
@@ -675,7 +681,11 @@ class BackboneTable:
         arr = (C.c_void_p * max(len(self.borders), 1))(*[b.handle.value for b in self.borders])
         h = C.c_void_p()
         self.area_id = int(flat.area.area_id) if config is not None else 0
-        create = ("hspf_ospfv3_nonbackbone_table_create" if self.v3 and config is not None else
+        self.third_area = bool(self.borders) and all(isinstance(b, AbrBackboneTable) for b in self.borders)
+        if not self.third_area and any(isinstance(b, AbrBackboneTable) for b in self.borders):
+            raise ValueError("borders are all AbrBackboneTables (a third-area table) or none is")
+        create = ("hspf_ospfv2_third_area_table_create" if self.third_area else
+                  "hspf_ospfv3_nonbackbone_table_create" if self.v3 and config is not None else
                   "hspf_ospfv3_backbone_asbr_table_create" if self.v3 and asbr else
                   "hspf_ospfv3_backbone_table_create" if self.v3 else
                   "hspf_ospfv2_nonbackbone_table_create" if config is not None else
@@ -685,6 +695,8 @@ class BackboneTable:
         if config is not None:
             self.config = np.array([config], AREA_CONFIG_DT)
             args = (self.config.ctypes.data,) + args
+        elif self.third_area:
+            args = (None,) + args
         rc = getattr(self.lib, create)(flat.handle, router_id, *args)
         if rc != capi.HSPF_OK:
             raise capi.HspfError(rc, create + " failed")
@@ -867,6 +879,10 @@ class AbrBackboneTable:
         c = [C.c_uint32() for _ in range(4)]
         assert self.lib.hspf_ospfv2_abr_backbone_table_records(h, *[C.byref(x) for x in c]) == capi.HSPF_OK
         self.n_records, self.n_slots, self.n_asbr_slots, self.n_asbr_sets = [x.value for x in c]
+        ng, ids = C.c_uint32(), C.POINTER(C.c_uint32)()
+        assert self.lib.hspf_ospfv2_abr_backbone_table_asbrs(h, C.byref(ng), C.byref(ids)) == capi.HSPF_OK
+        # the ASBRs whose area-0 entry moves with the job (abr_backbone_asbr_entries_device's columns)
+        self.asbr_ids = np.ctypeslib.as_array(ids, (ng.value,)).copy() if ng.value else np.zeros(0, np.uint32)
         if self.v3:
             p6 = C.c_void_p()
             rc = self.lib.hspf_ospfv3_abr_backbone_table_prefixes6(h, None, C.byref(p6), None)
@@ -914,6 +930,42 @@ def abr_backbone_delta_device(ctx: capi.Context, t: AbrBackboneTable, n_jobs: in
     bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)
     route_table.call_stage(ctx, "hspf_ospfv2_abr_backbone_delta", planes[0], t.handle, n_jobs, _planes_array(planes),
                            _device_ptrs(border_cells), st, bp, bn, br, base_ptr or None, n_base, base_of_ptr or None,
+                           job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
+
+
+def abr_backbone_asbr_entries_device(ctx: capi.Context, t: AbrBackboneTable, n_jobs: int, planes: list, border_planes,
+                                     border_n_rows, border_rows, status_ptr: int, entries_ptr: int):
+    """hspf_ospfv2_abr_backbone_asbr_entries / _entries16: per job and per ASBR of t.asbr_ids, the metric of the type-4
+    LSA the router originates for it into a normal area other than area 0 (0xFFFFFFFF: none), into device u32
+    [n_jobs, len(t.asbr_ids)] at entries_ptr.  planes / border_* as abr_backbone_cells_device."""
+    keep = []
+    bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)
+    route_table.call_stage(ctx, "hspf_ospfv2_abr_backbone_asbr_entries", planes[0], t.handle, n_jobs,
+                           _planes_array(planes), bp, bn, br, status_ptr or None, entries_ptr or None)
+
+
+def third_area_cells_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
+                            border_entries, border_entry_status, status_ptr: int, cells_ptr: int):
+    """hspf_ospfv2_third_area_cells / _cells16: backbone_cells_device's arguments over a third-area table, plus per
+    border a device pointer to its [n_jobs, G_b] entries (0 allowed without chain slots; None: NULL) and per border
+    the entries call's device u32 [n_jobs] status words or 0 (None: none)."""
+    be = _device_ptrs(border_entries) if border_entries is not None else None
+    es = _device_ptrs(border_entry_status) if border_entry_status is not None else None
+    st = _device_ptrs(border_status) if border_status is not None else None
+    route_table.call_stage(ctx, "hspf_ospfv2_third_area_cells", rs, t.handle, n_jobs, C.byref(rs),
+                           _device_ptrs(border_cells), st, be, es, status_ptr or None, cells_ptr or None)
+
+
+def third_area_delta_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
+                            border_entries, border_entry_status, base_ptr: int, n_base: int, base_of_ptr: int,
+                            job_out_ptr: int, records_ptr: int, cap: int, n_records_ptr: int):
+    """hspf_ospfv2_third_area_delta / _delta16: the route-delta stage over the same walk (arguments as
+    third_area_cells_device and rib_delta_device)."""
+    be = _device_ptrs(border_entries) if border_entries is not None else None
+    es = _device_ptrs(border_entry_status) if border_entry_status is not None else None
+    st = _device_ptrs(border_status) if border_status is not None else None
+    route_table.call_stage(ctx, "hspf_ospfv2_third_area_delta", rs, t.handle, n_jobs, C.byref(rs),
+                           _device_ptrs(border_cells), st, be, es, base_ptr or None, n_base, base_of_ptr or None,
                            job_out_ptr or None, records_ptr or None, cap, n_records_ptr or None)
 
 

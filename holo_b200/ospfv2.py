@@ -947,6 +947,78 @@ def abr_backbone_view(t0: Topology, t1: Topology, t2: Topology, seed: int, r: in
             "borders": out_borders, "shared": v["shared"], "asbr": v["asbr"], "area1_asbrs": v["area1_asbrs"]}
 
 
+def _rerooted(img: Ospfv2Area, fresh: Ospfv2Area) -> Ospfv2Area:
+    """img's LSDB as seen by fresh's root: the root's own fields (router id, interfaces, neighbours) from fresh."""
+    a = Ospfv2Area(**{k: getattr(img, k) for k in img.__dataclass_fields__})
+    for k in ("router_id", "ifaces", "iface_addrs", "nbrs", "ifnames"):
+        setattr(a, k, getattr(fresh, k))
+    return a
+
+
+def third_area_view(t0: Topology, t1: Topology, t2: Topology, seed: int, spf, n_c: int = 2, max_paths: int = 16,
+                    n_ext_keys: int = 3, area1_asbrs: int = 0, area1_ext: int = 4):
+    """An internal router R of area 2, the area border routers C of area 2 and area 0 (n_c of them, 2 or 3), and the
+    borders B of area 1, each as its own image: backbone_view's areas 0 and 1 (its three borders, the area-0 ASBR,
+    area1_asbrs area-1 ASBRs with their type-5 and type-4 LSAs), with synth_area(t2) moved into ranges of area 2 whose
+    routers 0 .. n_c - 1 are the C's (routers 0, then the first routers of t0 past the borders that are not the
+    area-0 ASBR; the B flag in areas 0 and 2) and whose router n_c is R.  Area 2 also holds an ASBR ("area2_asbr") with
+    0x0E0A0000/24 and a /24 of its own, and a stub of an area-1 prefix ("area2_shared").  Seeded; area 2 draws from a
+    generator of its own.  `spf(csr, root_vertex, nh_words)` gives unperturbed planes, as area_from_planes takes them.
+    Returns a dict:
+      r_area        R's area-2 image;
+      summaries2    area 2's type-3/4 LSAs (LsaKey order): each C's hspf_ospfv2_net_summaries into area 2 over its
+                    update_rib_full at the unperturbed job;
+      externals     backbone_view's plus the area-2 ASBR's;
+      c_areas       per C (areas [area 0, area 2], area ids [0, 2], summaries per area: area 0's, none for area 2);
+      borders       per B as backbone_view's (the C's have the B flag in its area-0 image);
+      asbr, area1_asbrs, area2_asbr, area2_shared, shared."""
+    from . import ospf_rib
+    if n_c not in (2, 3):
+        raise ValueError("n_c is 2 or 3")
+    v = backbone_view(t0, t1, seed, r=0, max_paths=max_paths, n_ext_keys=n_ext_keys, area1_asbrs=area1_asbrs,
+                      area1_ext=area1_ext)
+    rng = np.random.default_rng([seed, 0xC3A])
+    c0 = [0] + [i for i in range(4, t0.n_routers) if RID_BASE + i != v["asbr"]][:n_c - 1]
+    cids = [RID_BASE + i for i in c0]
+    cflag = {c: 0x01 for c in cids}
+    idmap = {RID_BASE + k: c for k, c in enumerate(cids)}
+    img2 = lambda i: _set_flags(_area_remap(synth_area(t2, root=i, max_paths=max_paths), 2, idmap), dict(cflag))
+    ra = img2(n_c)
+    fl = Flat(ra)
+    d = _dist_from(fl, fl.router_vertex(ra.router_id))
+    reach = sorted(int(fl.ids[x]) for x in range(len(fl.ids))
+                   if fl.is_router[x] and 0 < d[x] < 1 << 40 and int(fl.ids[x]) not in cids)
+    t3 = v["summaries0"][v["summaries0"]["lsa_type"] == 3]
+    pick = t3[int(rng.integers(0, len(t3)))]
+    shared2 = (int(pick["lsa_id"]), int(pick["mask"]))
+    adds = {reach[int(rng.integers(0, len(reach)))]: [(shared2[0], shared2[1], 1)]}
+    asbr2 = reach[int(rng.integers(0, len(reach)))]
+    area2 = lambda i: _set_flags(_with_stubs(img2(i), adds), {asbr2: 0x02})
+    ext = [tuple(x) for x in v["externals"].tolist()]
+    ext += [(asbr2, 0x0E0A0000, 0xFFFFFF00, 12, 0, 12, 1, 0, (0, 0)),
+            (asbr2, 0x0E0C0000, 0xFFFFFF00, int(rng.integers(1, 40)), 0, 12, 0, 0, (0, 0))]
+    ext.sort(key=lambda x: (x[0], x[1]))
+    externals = np.asarray(ext, ospf_rib.EXTERNAL_LSA_DT)
+    a0 = _set_flags(v["r_area"], dict(cflag))
+    empty = np.zeros(0, ospf_rib.SUMMARY_LSA_DT)
+    c_areas = [([_rerooted(a0, synth_area(t0, root=i, max_paths=max_paths)) if k else a0, area2(k)], [0, 2],
+                [v["summaries0"], empty]) for k, i in enumerate(c0)]
+    sums = []
+    for areas, ids, csums in c_areas:
+        rid = areas[0].router_id
+        rib_areas = [ospf_rib.RibArea(a.area_id, area_from_planes(a, spf), a.ifaces, s, True)
+                     for a, s in zip(areas, csums)]
+        rib = ospf_rib.update_rib_full(rid, max_paths, rib_areas, externals)
+        sums += [tuple(x) for x in ospf_rib.net_summaries(rid, rib, ospf_rib.router_tables(rid, rib_areas), rib_areas,
+                                                          [ospf_rib.area_config()] * 2, 1).tolist()]
+    sums.sort(key=lambda x: (x[4], x[0], x[1]))
+    borders = [([_set_flags(a, dict(cflag)) if a.area_id == 0 else a for a in areas], ids, bs)
+               for areas, ids, bs in v["borders"]]
+    return {"r_area": area2(n_c), "summaries2": np.asarray(sums, ospf_rib.SUMMARY_LSA_DT), "externals": externals,
+            "c_areas": c_areas, "borders": borders, "asbr": v["asbr"], "area1_asbrs": v["area1_asbrs"],
+            "area2_asbr": asbr2, "area2_shared": shared2, "shared": v["shared"]}
+
+
 def nonbackbone_view(t0: Topology, t1: Topology, seed: int, spf, r: int | None = None,
                      borders=((1, 0), (2, 1), (3, 2)), max_paths: int = 16, n_ext_keys: int = 3, n_ext: int = 0):
     """An internal router R of area 1 and the area border routers ("borders") between area 0 and area 1, each as its

@@ -187,6 +187,14 @@ def declare(lib: C.CDLL):
         "hspf_ospfv2_abr_backbone_delta16": [vp, vp, u32, vp, pvp, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv2_abr_backbone_from_cells": [vp, C.POINTER(ospfv2.AreaStruct), u32, vp, vp, vp, vp, u32,
                                                 C.POINTER(ospf_rib.RibStruct)],
+        "hspf_ospfv2_abr_backbone_table_asbrs": [vp, u32p, C.POINTER(u32p)],
+        "hspf_ospfv2_abr_backbone_asbr_entries": [vp, vp, u32, vp, pvp, pvp, pvp, vp, vp],
+        "hspf_ospfv2_abr_backbone_asbr_entries16": [vp, vp, u32, vp, pvp, pvp, pvp, vp, vp],
+        "hspf_ospfv2_third_area_table_create": [vp, u32, vp, vp, u32, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv2_third_area_cells": [vp, vp, u32, res, pvp, pvp, pvp, pvp, vp, vp],
+        "hspf_ospfv2_third_area_cells16": [vp, vp, u32, res16, pvp, pvp, pvp, pvp, vp, vp],
+        "hspf_ospfv2_third_area_delta": [vp, vp, u32, res, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
+        "hspf_ospfv2_third_area_delta16": [vp, vp, u32, res16, pvp, pvp, pvp, pvp, vp, u32, vp, vp, vp, u64, vp],
         "hspf_ospfv3_net_summaries": [u32, C.POINTER(ospf_rib.RibStruct), C.POINTER(ospf_rib.RibAreaStruct), vp, u32,
                                       u32, vp, u32, u32p],
         "hspf_ospfv3_rtr_summaries": [u32, C.POINTER(ospf_rib.RibAreaStruct), vp, u32, u32, vp, u32, u32p],

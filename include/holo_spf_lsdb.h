@@ -603,6 +603,111 @@ int hspf_ospfv2_abr_backbone_from_cells(const hspf_ospfv2_abr_backbone_table *t,
                                         hl_ospfv2_rib *out);
 
 /*
+ * The ASBR entries of an area border router C of the table above, per job, for a router of another area of C's
+ * (OSPFv2).  When the perturbed area holds an ASBR A, C's area-0 entry for A is inter-area, through the borders'
+ * type-4 LSAs in area 0, and C re-originates it into its normal areas other than area 0 (compute_rtr_summaries: E
+ * flag, below LSInfinity) at a metric that moves with the job.  The "groups" are the ASBRs whose area-0 type-4 range in
+ * C's table holds type-4 slots.
+ *
+ *   hspf_ospfv2_abr_backbone_table_asbrs  the group count G and the groups' ASBR ids, ascending by group (pointer may
+ *                                be NULL).  HSPF_E_INVAL for no table.
+ *   hspf_ospfv2_abr_backbone_asbr_entries[16]  one thread per (job, group).  planes, border_planes, border_n_rows and
+ *                                border_rows as hspf_ospfv2_abr_backbone_cells[16].  entries (device u32
+ *                                [n_jobs][G]): C's area-0 entry metric for the group's ASBR in the job, the metric
+ *                                of the type-4 LSA C originates for it into a normal area, or 0xFFFFFFFF when C
+ *                                originates none: the type-4 rows of hspf_ospfv2_net_summaries(rib_C, rtrs_C, ...,
+ *                                target a normal area other than area 0) over C's routing table of the job.
+ *                                job_status_out (device u32[n_jobs], may be NULL): the OR of C's row-0 words and the
+ *                                words of the type-4 rows the job reads, HSPF_JS_INVALID for a row out of range; a job
+ *                                with a non-zero word gets 0xFFFFFFFF entries.  HSPF_E_INVAL: an OSPFv3 table, a table
+ *                                not uploaded, entries or job_status_out not 4-byte aligned.  Nothing is launched for
+ *                                0 jobs.  Enqueued on the ctx stream.
+ */
+int hspf_ospfv2_abr_backbone_table_asbrs(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_groups,
+                                         const uint32_t **asbr_ids);
+int hspf_ospfv2_abr_backbone_asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                          const hspf_result *planes, const hspf_result *const *border_planes,
+                                          const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                          uint32_t *job_status_out, uint32_t *entries);
+int hspf_ospfv2_abr_backbone_asbr_entries16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                            const hspf_result16 *planes, const hspf_result16 *const *border_planes,
+                                            const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                            uint32_t *job_status_out, uint32_t *entries);
+
+/*
+ * Non-backbone router over what-if jobs inside another non-backbone area (OSPFv2).  R is an internal router of a
+ * non-backbone area A2; a job changes costs only inside another non-backbone area A1.  The "borders" are A2's area
+ * border routers attached to area 0 (C, 1..8), none attached to A1, each given as its hspf_ospfv2_abr_backbone_table
+ * over A1's ABRs attached to area 0 (B).  Every ABR of A2 attached to area 0 must be given as a border: another one
+ * keeps its base LSAs as static records, and the table cannot tell.  R's area-A2 SPT is row 0 in every job.  What
+ * moves are the type-3 / type-4 LSAs the C's originate into A2: each C's routes move with the B's LSAs in area 0.  For
+ * job j, with C's cells of j (hspf_ospfv2_abr_backbone_cells[16]) decoded to rib_C, the decoded cells of j equal the
+ * affected-prefix routes of
+ *     hspf_ospfv2_update_rib_full(R, max_paths, [{A2, area_from_planes(A2, R's row 0), ifaces, S_j, 1}], X)
+ * where S_j is A2's type-3/4 LSAs with each C's LSAs replaced by hspf_ospfv2_net_summaries(rib_C, rtrs_C, ..., target
+ * A2), in LsaKey order.  A C's type-3 LSA can move only for a prefix of C's table (C's affected prefixes); any other
+ * LSA of C stays a static record.  A C advertises a route of its cell as into a non-backbone area above.  When A1
+ * holds an ASBR A, each C's type-4 LSA for A into a normal A2 moves too: in R's type-4 range for A it is a chain slot
+ * at C's LsaKey place, which reads C's entries of the job (hspf_ospfv2_abr_backbone_asbr_entries[16]), and the
+ * prefixes of A's type-5 LSAs are affected.  The affected prefixes are every prefix of some C's table that C can
+ * advertise into A2, plus those.  Every other prefix of R's table is R's base route in every job.  Stub and totally
+ * stubby areas are handled as by hspf_ospfv2_nonbackbone_table_create; the chain rule is restated from the reference's
+ * code: no recorded conformance data holds a type-4 LSA.
+ *
+ *   hspf_ospfv2_third_area_table_create  host.  flat: R's area-A2 flat; config: A2's configuration; summaries: A2's
+ *                                type-3/4 LSAs in LsaKey order; externals: the AS-external LSAs; borders: the C's
+ *                                OSPFv2 abr_backbone tables, which must outlive the table.  The result is an
+ *                                hspf_ospfv2_backbone_table marked as a third-area table: hspf_ospfv2_backbone_table_*
+ *                                (asbr_slots: the chain slot count and 0 plane sets), _upload and
+ *                                hspf_ospfv2_backbone_from_cells take it.  HSPF_E_INVAL: a flat of area 0, a NULL
+ *                                config, R missing from the flat or with the B flag, 0 or more than 8 borders, a border
+ *                                given twice, for OSPFv3, among them R, without area 0 or A2, or not a B-flag router
+ *                                vertex of the flat, a usable type-3 LSA of a C in A2 for a prefix of C's table it cannot
+ *                                advertise.  HSPF_E_UNSUPPORTED: an NSSA, a V-flag router in A2, a B that is a router of
+ *                                A2, a usable type-4 LSA of another ABR in a C's area-0 summaries, winners that do not
+ *                                fit.
+ *   hspf_ospfv2_third_area_cells[16]  the arguments of hspf_ospfv2_backbone_cells[16] (border_cells: each C's cells
+ *                                of the job) plus border_entries (per border a device u32 [n_jobs][G_b] of its
+ *                                entries, NULL allowed for a border without groups and for a table without chain
+ *                                slots) and border_entry_status (per border the entries call's device u32[n_jobs]
+ *                                words or NULL; the array may be NULL).  A job's status word ORs R's row-0 word, each
+ *                                C's cell status and entries status; a job with a non-zero word gets empty cells.
+ *                                HSPF_E_INVAL for a table that is not a third-area one.  A table without chain slots
+ *                                also runs through hspf_ospfv2_backbone[_asbr]_cells[16] / _delta[16]; those refuse a
+ *                                third-area table with chain slots (HSPF_E_INVAL), before any launch.  Nothing is
+ *                                launched for 0 jobs.  Enqueued on the ctx stream.
+ *   hspf_ospfv2_third_area_delta[16]  the route-delta stage over the same walk (base cells as hspf_ospfv2_rib_delta).
+ */
+int hspf_ospfv2_third_area_table_create(const hspf_ospfv2_flat *flat, uint32_t router_id,
+                                        const struct hl_ospf_area_config *config,
+                                        const hl_ospfv2_summary_lsa *summaries, uint32_t n_summaries,
+                                        const hl_ospfv2_external_lsa *externals, uint32_t n_externals,
+                                        const hspf_ospfv2_abr_backbone_table *const *borders, uint32_t n_borders,
+                                        hspf_ospfv2_backbone_table **out);
+int hspf_ospfv2_third_area_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                 const uint32_t *const *border_entry_status, uint32_t *job_status_out,
+                                 hl_ospf_rib_cell *cells);
+int hspf_ospfv2_third_area_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                   const uint32_t *const *border_entry_status, uint32_t *job_status_out,
+                                   hl_ospf_rib_cell *cells);
+int hspf_ospfv2_third_area_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                 const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
+                                 const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                 const uint32_t *const *border_entry_status, const hl_ospf_rib_cell *base_cells,
+                                 uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                                 hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+int hspf_ospfv2_third_area_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
+                                   const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
+                                   const uint32_t *const *border_status, const uint32_t *const *border_entries,
+                                   const uint32_t *const *border_entry_status, const hl_ospf_rib_cell *base_cells,
+                                   uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
+                                   hl_route_delta *records, uint64_t cap, uint64_t *n_records);
+
+/*
  * The same stage for OSPFv3.  The table is an hspf_ospfv2_backbone_table marked OSPFv3; the cells and delta calls
  * above take it (the table's mark picks the walk), and each version's create and decode refuse the other version's
  * tables (HSPF_E_INVAL).  For job j, with border b's ABR cells of j decoded to rib_b (hspf_ospfv3_abr_rib_from_cells),

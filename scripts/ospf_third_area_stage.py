@@ -1,0 +1,326 @@
+#!/usr/bin/env python
+"""The OSPFv2 stage of an internal router of a non-backbone area over what-if jobs inside another non-backbone area
+(hspf_ospfv2_abr_backbone_asbr_entries, hspf_ospfv2_third_area_cells / hspf_ospfv2_third_area_delta) on a 10 000-job
+what-if batch inside area 1; device only:
+python scripts/ospf_third_area_stage.py [--jobs 10000] [--reps 10] [--out profiles/h100_C5_third_area.json]
+
+Domain (ospfv2.third_area_view, seed 0xC5, n_c=2, area1_asbrs=2, area1_ext=1000): C5's LSDB as area 0, a 2 000-router
+area 1 with three area border routers (B) and two ASBRs with about 1 000 type-5 LSAs each, and a 2 000-router area 2
+with two area border routers (C) and R, an internal router of area 2.  Job 0 is unperturbed; job j > 0 disables one
+router-to-router link of area 1 (both directions).  The whole chain runs on the device: each B's area SPT batches
+(one row per job in area 1) and ABR cells (hspf_ospfv2_abr_rib_cells); each C's row 0, abr_backbone cells and ASBR
+entries over them; R's row 0, then R's calls over the C's cells and entries.
+
+The launch bound of R's kernels (kThirdAreaBlocksPerSM in csrc/ospfv2_backbone.cu) is timed against the other bound
+in the same run: a second copy of the library, built into a temporary directory with the other value, runs the same
+calls on its own copy of R's table over the same C tables, planes, cells and entries, alternating with the first.
+The entries call is timed in the same loop.  CUDA-event medians over `--reps` alternating launches after warm-up; the
+card's name and power limit are read (not set) in the same run, with the device memory the run holds.  Outside the
+timed region: both builds' cells are byte-identical and the delta's total equals a count over the stored cells.  Host
+figure (a CPU measurement): per job, the host chain the stage replaces (each B's area_from_planes + update_rib_full +
+router tables + net_summaries into area 0, each C's over those into area 2, then R's update_rib_full), timed over a
+few jobs."""
+import argparse
+import ctypes as C
+import json
+import re
+import shutil
+import subprocess
+import sys
+import tempfile
+import time
+from pathlib import Path
+
+import numpy as np
+
+ROOT = Path(__file__).resolve().parent.parent
+sys.path.insert(0, str(ROOT))
+CONST = "kThirdAreaBlocksPerSM"
+
+
+def build_variant(bound: int, tmp: Path) -> Path:
+    """libholo_spf.so with kThirdAreaBlocksPerSM = bound, built from a copy of the sources in `tmp`."""
+    from holo_b200 import build
+    src = tmp / "holo_b200" / "csrc"
+    shutil.copytree(build.CSRC, src)
+    shutil.copytree(build.ROOT / "include", tmp / "include")
+    cu = src / "ospfv2_backbone.cu"
+    text, n = re.subn(rf"constexpr uint32_t {CONST} = \d+;", f"constexpr uint32_t {CONST} = {bound};", cu.read_text())
+    assert n == 1
+    cu.write_text(text)
+    out = tmp / "libholo_spf_variant.so"
+    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
+    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *build.NVCC_FLAGS, "-o", str(out), *map(str, srcs)], check=True,
+                   capture_output=True)
+    return out
+
+
+def current_bound() -> int:
+    return int(re.search(rf"constexpr uint32_t {CONST} = (\d+);",
+                         (ROOT / "holo_b200" / "csrc" / "ospfv2_backbone.cu").read_text()).group(1))
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--out", default="")
+    ap.add_argument("--jobs", type=int, default=10000)
+    ap.add_argument("--reps", type=int, default=10)
+    ap.add_argument("--host-jobs", type=int, default=2)
+    args = ap.parse_args()
+    import torch
+    if not torch.cuda.is_available():
+        sys.exit("ospf_third_area_stage.py: no CUDA device; this measurement runs on the GPU only")
+    from holo_b200 import capi, ospf_rib, ospfv2, route_table, synth
+    from holo_b200.route_table import DELTA_JOB_DT, DELTA_DT
+
+    ctx = capi.Context(0)
+    dev = torch.device("cuda", 0)
+    n = args.jobs
+    rng = np.random.default_rng(0xC5)
+    u32p, u16p, u64p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16), C.POINTER(C.c_uint64)
+    keep = []
+
+    def spt_batch(csr, root, ov):
+        m = len(ov)
+        g = ctx.upload(csr)
+        off = np.zeros(m + 1, np.int64)
+        ed, co = [], []
+        for j, o in enumerate(ov):
+            for e, cst in o:
+                ed.append(e); co.append(cst)
+            off[j + 1] = len(ed)
+        t = [torch.full((m,), root, dtype=torch.int32, device=dev), torch.from_numpy(off.astype(np.int32)).to(dev),
+             torch.from_numpy(np.asarray(ed or [0], np.uint32).view(np.int32).copy()).to(dev),
+             torch.from_numpy(np.asarray(co or [0], np.uint32).view(np.int32).copy()).to(dev)]
+        js = capi.JobsStruct()
+        js.n_jobs, js.roots, js.ov_off, js.ov_edge, js.ov_cost = m, *(C.cast(x.data_ptr(), u32p) for x in t)
+        V = csr.n_vertices
+        pl = [torch.empty(m * V, dtype=torch.int32, device=dev), torch.empty(m * V, dtype=torch.int16, device=dev),
+              torch.empty(m * V, dtype=torch.int64, device=dev), torch.zeros(m, dtype=torch.int32, device=dev)]
+        rs = capi.ResultStruct()
+        rs.dist, rs.hops = C.cast(pl[0].data_ptr(), u32p), C.cast(pl[1].data_ptr(), u16p)
+        rs.nh_mask, rs.nh_words = C.cast(pl[2].data_ptr(), u64p), 1
+        rs.job_status = C.cast(pl[3].data_ptr(), u32p)
+        keep.extend([g, t, pl, js])
+        ctx.run_device(g, js, rs, sync=False)
+        return rs, pl
+
+    def host_planes(pl, row, V):
+        d = pl[0].view(torch.int32).reshape(-1, V)[row].cpu().numpy().view(np.uint32)
+        hh = pl[1].reshape(-1, V)[row].cpu().numpy().view(np.uint16)
+        m = pl[2].reshape(-1, V)[row].cpu().numpy().view(np.uint64)
+        return d, hh, m
+
+    def device_spf(csr, root, nhw):
+        """Unperturbed planes of one root, for the view's base-job summaries."""
+        _rs, pl = spt_batch(csr, root, [[]])
+        ctx.sync()
+        d, hh, m = host_planes(pl, 0, csr.n_vertices)
+        return d, hh, np.pad(m[:, None], ((0, 0), (0, nhw - 1)))
+
+    t0 = synth.random_topology(10000, 40000, synth.SEED_BASE + 5, cost_choices=[10, 20], lan_fraction=0.05)
+    t1 = synth.random_topology(2000, 8000, synth.SEED_BASE + 850, cost_choices=[10, 20], lan_fraction=0.05)
+    t2 = synth.random_topology(2000, 8000, synth.SEED_BASE + 851, cost_choices=[10, 20], lan_fraction=0.05)
+    v = ospfv2.third_area_view(t0, t1, t2, 0xC5, device_spf, n_c=2, area1_asbrs=2, area1_ext=1000)
+
+    # the jobs: one link of area 1 per job, named by its end points' ids
+    i1 = [b[1].index(1) for b in v["borders"]]
+    f1 = ospfv2.Flat(v["borders"][0][0][i1[0]])
+    src = np.repeat(np.arange(f1.csr.n_vertices), np.diff(f1.csr.row_ptr))
+    links = sorted({tuple(sorted((int(f1.ids[src[e]]), int(f1.ids[f1.csr.col[e]])))) for e in range(f1.csr.n_edges)
+                    if f1.link_index[e] != 0xFFFFFFFF})
+    job_links = [None] + [links[int(rng.integers(len(links)))] for _ in range(n - 1)]
+    tables, border_cells, flats_all, planes_all, border_rs, border_nrows, border_rows = [], [], [], [], [], [], []
+    for b, (areas, ids, sums) in enumerate(v["borders"]):
+        flats = [ospfv2.Flat(a) for a in areas]
+        rt = ospf_rib.AbrRibTable(areas[0].router_id, flats, ids, sums, None, v["externals"])
+        rt.upload(ctx)
+        f = flats[i1[b]]
+        s = np.repeat(np.arange(f.csr.n_vertices), np.diff(f.csr.row_ptr))
+        by_pair = {}
+        for e in range(f.csr.n_edges):
+            by_pair.setdefault(tuple(sorted((int(f.ids[s[e]]), int(f.ids[f.csr.col[e]])))), []).append(e)
+        rs_list, n_rows, pls = [], [], []
+        for i, fl in enumerate(flats):
+            root = fl.router_vertex(areas[0].router_id)
+            ov = [[]] if i != i1[b] else [[(e, capi.COST_DISABLED) for e in by_pair.get(l, [])] if l else [] for l in job_links]
+            rs, pl = spt_batch(fl.csr, root, ov)
+            rs_list.append(rs); n_rows.append(len(ov)); pls.append(pl)
+        rows = np.zeros((n, 2), np.uint32)
+        rows[:, i1[b]] = np.arange(n)
+        d_rows = torch.from_numpy(rows.view(np.int32).reshape(-1).copy()).to(dev)
+        cells = torch.empty(n * rt.n_prefixes * 24, dtype=torch.uint8, device=dev)
+        ospf_rib.abr_rib_cells_device(ctx, rt, n, rs_list, n_rows, d_rows.data_ptr(), cells.data_ptr())
+        keep += [d_rows, rs_list]
+        border_rs.append(rs_list)
+        border_nrows.append(n_rows)
+        border_rows.append(d_rows.data_ptr())
+        tables.append(rt); border_cells.append(cells); flats_all.append(flats); planes_all.append(pls)
+    bc = [c.data_ptr() for c in border_cells]
+    # the C's: row 0 of each area, abr_backbone cells over the B's, and their ASBR entries
+    ctables, c_rs, c_pl, c_cells, c_ent, c_est = [], [], [], [], [], []
+    for areas, ids, sums in v["c_areas"]:
+        flats = [ospfv2.Flat(a) for a in areas]
+        rl, pl_ = [], []
+        for a, f in zip(areas, flats):
+            rs, pl = spt_batch(f.csr, f.router_vertex(a.router_id), [[]])
+            rl.append(rs); pl_.append(pl)
+        ct = ospf_rib.AbrBackboneTable(areas[0].router_id, flats, ids, sums, None, v["externals"], tables)
+        ct.upload(ctx)
+        out = torch.empty(n * ct.n_prefixes * 24, dtype=torch.uint8, device=dev)
+        ospf_rib.abr_backbone_cells_device(ctx, ct, n, rl, bc, None, border_rs, border_nrows, border_rows, 0,
+                                           out.data_ptr())
+        G = len(ct.asbr_ids)
+        assert G > 0
+        ent = torch.empty(n * G, dtype=torch.int32, device=dev)
+        est = torch.empty(n, dtype=torch.int32, device=dev)
+        ospf_rib.abr_backbone_asbr_entries_device(ctx, ct, n, rl, border_rs, border_nrows, border_rows, est.data_ptr(),
+                                                  ent.data_ptr())
+        ctables.append(ct); c_rs.append(rl); c_pl.append(pl_); c_cells.append(out); c_ent.append(ent); c_est.append(est)
+    ra = v["r_area"]
+    rf = ospfv2.Flat(ra)
+    r_rs, r_pl = spt_batch(rf.csr, rf.router_vertex(ra.router_id), [[]])
+    tt = ospf_rib.BackboneTable(rf, ra.router_id, v["summaries2"], v["externals"], ctables,
+                                config=ospf_rib.area_config())
+    assert tt.third_area and tt.n_asbr_slots > 0
+    tt.upload(ctx)
+    ctx.sync()
+    assert not any(x.any().item() for x in c_est)
+    P = tt.n_prefixes
+
+    cur = current_bound()
+    other = 8 if cur == 4 else 4
+    libv = C.CDLL(str(build_variant(other, Path(tempfile.mkdtemp(prefix="third_area_bound_")))))
+    route_table.declare(libv)
+    # the variant's own copy of R's table, over the same flat and C tables
+    hv = C.c_void_p()
+    carr = (C.c_void_p * len(ctables))(*[x.handle.value for x in ctables])
+    sm, ext = tt.summaries, tt.externals
+    assert libv.hspf_ospfv2_third_area_table_create(rf.handle, ra.router_id, tt.config.ctypes.data, sm.ctypes.data,
+                                                    len(sm), ext.ctypes.data, len(ext), carr, len(ctables),
+                                                    C.byref(hv)) == 0
+    assert libv.hspf_ospfv2_backbone_table_upload(ctx.handle, hv) == 0
+    handles = {cur: (ctx.lib, tt.handle), other: (libv, hv)}
+    cells = {b: torch.empty(n * P * 24, dtype=torch.uint8, device=dev) for b in (4, 8)}
+    job_out = torch.zeros(n * DELTA_JOB_DT.itemsize, dtype=torch.uint8, device=dev)
+    total = torch.zeros(1, dtype=torch.int64, device=dev)
+    cca = (C.c_void_p * len(c_cells))(*[x.data_ptr() for x in c_cells])
+    cea = (C.c_void_p * len(c_ent))(*[x.data_ptr() for x in c_ent])
+    cesa = (C.c_void_p * len(c_est))(*[x.data_ptr() for x in c_est])
+
+    def cell_launch(b):
+        lib, h = handles[b]
+        return lambda: lib.hspf_ospfv2_third_area_cells(ctx.handle, h, n, C.byref(r_rs), cca, None, cea, cesa, None,
+                                                        cells[b].data_ptr())
+
+    cell_launch(4)(); cell_launch(8)()
+    ctx.sync()
+    same_bounds = bool(torch.equal(cells[4], cells[8]))
+    base = cells[cur][: P * 24].clone()
+    lib, h = handles[cur]
+    assert lib.hspf_ospfv2_third_area_delta(ctx.handle, h, n, C.byref(r_rs), cca, None, cea, cesa, base.data_ptr(), 1,
+                                            None, job_out.data_ptr(), None, 0, total.data_ptr()) == 0
+    ctx.sync()
+    cap = int(total.cpu()[0])
+    w = cells[cur].view(torch.int64).reshape(n, P, 3)
+    changed = int((w != w[0:1]).any(dim=2).sum().item())
+    recs = torch.empty(max(cap, 1) * DELTA_DT.itemsize, dtype=torch.uint8, device=dev)
+    entries_moved = int(sum(int((e.reshape(n, -1) != e.reshape(n, -1)[0:1]).any(dim=1).sum().item()) for e in c_ent))
+
+    def delta(b, with_records):
+        lib, h = handles[b]
+        return lambda: lib.hspf_ospfv2_third_area_delta(ctx.handle, h, n, C.byref(r_rs), cca, None, cea, cesa,
+                                                        base.data_ptr(), 1, None, job_out.data_ptr(),
+                                                        recs.data_ptr() if with_records else None,
+                                                        cap if with_records else 0, total.data_ptr())
+
+    def entries(k):
+        ct, rl = ctables[k], c_rs[k]
+        return lambda: ospf_rib.abr_backbone_asbr_entries_device(ctx, ct, n, rl, border_rs, border_nrows, border_rows,
+                                                                 c_est[k].data_ptr(), c_ent[k].data_ptr())
+
+    work = {f"asbr_entries_c{k}": entries(k) for k in range(len(ctables))}
+    for b in (4, 8):
+        work[f"third_area_cells_bound{b}"] = cell_launch(b)
+        work[f"third_area_delta_summaries_bound{b}"] = delta(b, False)
+        work[f"third_area_delta_records_bound{b}"] = delta(b, True)
+    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
+    for _ in range(2):
+        for fn in work.values():
+            fn()
+    ctx.sync()
+    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
+          for k in work}
+    for r in range(args.reps):
+        for k, fn in work.items():
+            ev[k][r][0].record(stream)
+            fn()
+            ev[k][r][1].record(stream)
+    ctx.sync()
+    med = {k: float(np.median([a.elapsed_time(b) for a, b in ev[k]])) for k in work}
+    held = torch.cuda.memory_allocated(dev)
+    free, total_mem = torch.cuda.mem_get_info()
+
+    # host chain per job (CPU), over the device planes read back
+    def spf_of(a, p):
+        return ospfv2.area_from_planes(a, lambda csr, root, nhw: (p[0], p[1], np.pad(p[2][:, None], ((0, 0), (0, nhw - 1)))))
+
+    cfg = [ospf_rib.area_config()] * 2
+    host_ms = []
+    cp = [[host_planes(pl, 0, ospfv2.Flat(a).csr.n_vertices) for pl, a in zip(pls, areas)]
+          for pls, (areas, _i, _s) in zip(c_pl, v["c_areas"])]
+    rp = host_planes(r_pl, 0, rf.csr.n_vertices)
+    bids = {int(x.router_id) for x in tables}
+    cids = {int(x.router_id) for x in ctables}
+    for j in range(1, 1 + args.host_jobs):
+        t = time.perf_counter()
+        new0 = [s for s in v["c_areas"][0][2][0] if int(s["adv_rtr"]) not in bids]
+        for b, (areas, ids, sums) in enumerate(v["borders"]):
+            rab = []
+            for i, a in enumerate(areas):
+                p = host_planes(planes_all[b][i], j if i == i1[b] else 0, flats_all[b][i].csr.n_vertices)
+                rab.append(ospf_rib.RibArea(a.area_id, spf_of(a, p), a.ifaces, sums[i], True))
+            rid = areas[0].router_id
+            rib = ospf_rib.update_rib_full(rid, areas[0].max_paths, rab, v["externals"])
+            new0 += list(ospf_rib.net_summaries(rid, rib, ospf_rib.router_tables(rid, rab), rab, cfg, ids.index(0)))
+        s0 = np.array(new0, ospf_rib.SUMMARY_LSA_DT)
+        s0 = s0[np.lexsort((s0["lsa_id"], s0["adv_rtr"], s0["lsa_type"]))]
+        new2 = [s for s in v["summaries2"] if int(s["adv_rtr"]) not in cids]
+        for (areas, ids, sums), pls in zip(v["c_areas"], cp):
+            rac = [ospf_rib.RibArea(a.area_id, spf_of(a, p), a.ifaces, s0 if a.area_id == 0 else ss, True)
+                   for a, p, ss in zip(areas, pls, sums)]
+            rid = areas[0].router_id
+            rib = ospf_rib.update_rib_full(rid, areas[0].max_paths, rac, v["externals"])
+            new2 += list(ospf_rib.net_summaries(rid, rib, ospf_rib.router_tables(rid, rac), rac, cfg, ids.index(2)))
+        s2 = np.array(new2, ospf_rib.SUMMARY_LSA_DT)
+        s2 = s2[np.lexsort((s2["lsa_id"], s2["adv_rtr"], s2["lsa_type"]))]
+        ospf_rib.update_rib_full(ra.router_id, ra.max_paths, [ospf_rib.RibArea(2, spf_of(ra, rp), ra.ifaces, s2, True)],
+                                 v["externals"])
+        host_ms.append((time.perf_counter() - t) * 1e3)
+
+    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
+                       capture_output=True, text=True).stdout.strip().splitlines()
+    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    out = {
+        "stage": "hspf_ospfv2_abr_backbone_asbr_entries, hspf_ospfv2_third_area_cells / hspf_ospfv2_third_area_delta",
+        "workload": {"area0": "C5: 10000 routers, 40000 links, costs {10, 20}, 5 % LANs", "area1": "2000 routers",
+                     "area2": "2000 routers (R's area)", "area1_asbrs": len(v["area1_asbrs"]),
+                     "externals": len(v["externals"]), "b_borders": len(tables), "c_borders": len(ctables),
+                     "jobs": n, "affected_prefixes": P, "slots": tt.n_slots, "chain_slots": tt.n_asbr_slots,
+                     "c_keys": [x.n_prefixes for x in ctables], "c_asbr_groups": [len(x.asbr_ids) for x in ctables],
+                     "b_keys": [x.n_prefixes for x in tables]},
+        "card": card, "power_limit": power, "reps": args.reps, "median_ms": med, "launch_bound": cur,
+        "other_bound": other, "cells_equal_other_bound": same_bounds,
+        "delta_total": cap, "delta_total_equals_changed_cells": cap == changed,
+        "jobs_with_moved_entries": entries_moved,
+        "device_memory_allocated_gib": held / 2**30, "device_memory_in_use_gib": (total_mem - free) / 2**30,
+        "host_chain_ms_per_job": float(np.median(host_ms)), "host_jobs_timed": len(host_ms),
+        "note": "device figures are CUDA-event medians of alternating launches; the host chain is a CPU figure",
+    }
+    print(json.dumps(out))
+    if args.out:
+        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+
+
+if __name__ == "__main__":
+    main()
