@@ -21,39 +21,13 @@ with that chain.  Fails without a GPU.
 """
 import argparse
 import ctypes as C
-import json
-import re
-import shutil
-import subprocess
-import sys
-import tempfile
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
+import stage_bench
 
-CONST = "kBackboneBlocksPerSM"
-
-
-def build_variant(bound: int, tmp: Path) -> Path:
-    """libholo_spf.so with kBackboneBlocksPerSM = bound, built from a copy of the sources in `tmp`."""
-    from holo_b200 import build
-    src = tmp / "holo_b200" / "csrc"                 # the sources include ../../include
-    shutil.copytree(build.CSRC, src)
-    shutil.copytree(build.ROOT / "include", tmp / "include")
-    cu = src / "isis_backbone.cu"
-    text, n = re.subn(rf"constexpr uint32_t {CONST} = \d+;", f"constexpr uint32_t {CONST} = {bound};", cu.read_text())
-    assert n == 1
-    cu.write_text(text)
-    out = tmp / "libholo_spf_variant.so"
-    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
-    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *build.NVCC_FLAGS, "-o", str(out), *map(str, srcs)], check=True,
-                   capture_output=True)
-    return out
+BOUND = ("isis_backbone.cu", "kBackboneBlocksPerSM")
 
 
 def main():
@@ -66,10 +40,8 @@ def main():
     ap.add_argument("--host-sample", type=int, default=5)
     ap.add_argument("--variant", default="", help="a prebuilt library with the other launch bound")
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("isis_backbone_stage.py: no CUDA device; this measurement runs on the GPU only")
-    from holo_b200 import build, capi, isis, route_table, synth
+    torch = stage_bench.require_gpu("isis_backbone_stage.py")
+    from holo_b200 import capi, isis, route_table, synth
     from holo_b200.route_table import DELTA_DT, DELTA_JOB_DT
     from test_isis_backbone_cells import restrict, same_rib, spliced
     from test_isis_l1l2_rib_cells import topology_flat
@@ -119,9 +91,9 @@ def main():
     bcells = [b["cells"].data_ptr() for b in borders]
 
     # the other launch bound, from a copy of the library, with its own tables over the same instances
-    cur = int(re.search(rf"{CONST} = (\d+);", (build.CSRC / "isis_backbone.cu").read_text()).group(1))
+    cur = stage_bench.launch_bound(*BOUND)
     other = 4 if cur == 8 else 8
-    libv = C.CDLL(args.variant or str(build_variant(other, Path(tempfile.mkdtemp(prefix="backbone_bound_")))))
+    libv = C.CDLL(args.variant or str(stage_bench.build_variant(*BOUND, other, "backbone_bound_")))
     route_table.declare(libv)
     keep = []
     for b in borders:
@@ -183,8 +155,7 @@ def main():
             z.synchronize()
             times[k].append(a.elapsed_time(z))
     med = {k: float(np.median(x)) for k, x in times.items()}
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    gpu = ", ".join(stage_bench.card_and_power())
     # outside the timed region: the delta against the stored cells, sampled jobs against the host chain
     border_launch()
     cell_launch(cur)
@@ -248,10 +219,7 @@ def main():
                delta_records=tw, delta_checked_jobs=n, sampled_jobs_decoded=len(sample),
                host_ms_per_job_chain=host_ms, host_sample_jobs=len(jobs),
                host_note="host measurement (CPU of the GPU machine), not an H100 figure")
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
     for rv, tv in keep:
         libv.hspf_isis_l1_to_l2_table_free(tv)
         libv.hspf_isis_l1l2_ribtable_free(rv)

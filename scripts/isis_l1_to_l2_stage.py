@@ -19,39 +19,13 @@ and sampled jobs are decoded and compared with the host function.  Fails without
 """
 import argparse
 import ctypes as C
-import json
-import re
-import shutil
-import subprocess
-import sys
-import tempfile
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
+import stage_bench
 
-CONST = "kL1ToL2BlocksPerSM"
-
-
-def build_variant(bound: int, tmp: Path) -> Path:
-    """libholo_spf.so with kL1ToL2BlocksPerSM = bound, built from a copy of the sources in `tmp`."""
-    from holo_b200 import build
-    src = tmp / "holo_b200" / "csrc"                 # the sources include ../../include
-    shutil.copytree(build.CSRC, src)
-    shutil.copytree(build.ROOT / "include", tmp / "include")
-    cu = src / "isis_l1_to_l2.cu"
-    text, n = re.subn(rf"constexpr uint32_t {CONST} = \d+;", f"constexpr uint32_t {CONST} = {bound};", cu.read_text())
-    assert n == 1
-    cu.write_text(text)
-    out = tmp / "libholo_spf_variant.so"
-    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
-    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *build.NVCC_FLAGS, "-o", str(out), *map(str, srcs)], check=True,
-                   capture_output=True)
-    return out
+BOUND = ("isis_l1_to_l2.cu", "kL1ToL2BlocksPerSM")
 
 
 def main():
@@ -63,10 +37,8 @@ def main():
     ap.add_argument("--host-sample", type=int, default=20)
     ap.add_argument("--variant", default="", help="a prebuilt library with the other launch bound")
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("isis_l1_to_l2_stage.py: no CUDA device; this measurement runs on the GPU only")
-    from holo_b200 import build, capi, isis, route_table, synth
+    torch = stage_bench.require_gpu("isis_l1_to_l2_stage.py")
+    from holo_b200 import capi, isis, route_table, synth
     from holo_b200.route_table import DELTA_DT, DELTA_JOB_DT
     from test_isis_l1_to_l2_cells import host
     from test_isis_l1l2_rib_cells import topology_flat
@@ -104,9 +76,9 @@ def main():
     st = torch.cuda.ExternalStream(ctx.lib.hspf_stream(ctx.handle))
 
     # the other launch bound, from a copy of the library, with its own tables over the same instances
-    cur = int(re.search(rf"{CONST} = (\d+);", (build.CSRC / "isis_l1_to_l2.cu").read_text()).group(1))
+    cur = stage_bench.launch_bound(*BOUND)
     other = 4 if cur == 8 else 8
-    libv = C.CDLL(args.variant or str(build_variant(other, Path(tempfile.mkdtemp(prefix="l1_to_l2_bound_")))))
+    libv = C.CDLL(args.variant or str(stage_bench.build_variant(*BOUND, other, "l1_to_l2_bound_")))
     route_table.declare(libv)
     s1, s2 = isis.instance_struct(v["l1"]), isis.instance_struct(v["l2"])
     rv, tv = C.c_void_p(), C.c_void_p()
@@ -157,8 +129,7 @@ def main():
             z.synchronize()
             times[k].append(a.elapsed_time(z))
     med = {k: float(np.median(x)) for k, x in times.items()}
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    gpu = ", ".join(stage_bench.card_and_power())
     cell_launch(cur)
     cell_launch(other)
     ctx.sync()
@@ -197,10 +168,7 @@ def main():
                delta_records=tw, delta_checked_jobs=n, sampled_jobs_decoded=len(sample),
                host_ms_per_job_spt_from_planes_plus_l1_to_l2=host_ms, host_sample_jobs=len(jobs),
                host_note="host measurement (CPU of the GPU machine), not an H100 figure")
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
     ctx.close()
 
 

@@ -20,37 +20,12 @@ host chain.  Fails without a GPU.
 """
 import argparse
 import ctypes as C
-import json
-import re
-import shutil
-import subprocess
-import sys
-import tempfile
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
+import stage_bench
 
-
-def build_variant(bound: int, tmp: Path) -> Path:
-    """libholo_spf.so with kL1L2BlocksPerSM = bound, built from a copy of the sources in `tmp`."""
-    from holo_b200 import build
-    src = tmp / "holo_b200" / "csrc"                 # the sources include ../../include
-    shutil.copytree(build.CSRC, src)
-    shutil.copytree(build.ROOT / "include", tmp / "include")
-    cu = src / "isis_l1l2_rib.cu"
-    text, n = re.subn(r"constexpr uint32_t kL1L2BlocksPerSM = \d+;", f"constexpr uint32_t kL1L2BlocksPerSM = {bound};",
-                      cu.read_text())
-    assert n == 1
-    cu.write_text(text)
-    out = tmp / "libholo_spf_variant.so"
-    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
-    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *build.NVCC_FLAGS, "-o", str(out), *map(str, srcs)], check=True,
-                   capture_output=True)
-    return out
+BOUND = ("isis_l1l2_rib.cu", "kL1L2BlocksPerSM")
 
 
 def main():
@@ -60,9 +35,7 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--l1", type=int, default=2000)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("isis_l1l2_rib_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("isis_l1l2_rib_stage.py")
     from holo_b200 import capi, isis, route_table, synth
     from holo_b200.route_table import DELTA_DT, DELTA_JOB_DT
     from test_isis_l1l2_rib_cells import chain, level_routes, same_rib, topology_flat, without
@@ -106,10 +79,9 @@ def main():
         tops[k].run()
 
     # the other launch bound, from a copy of the library, with its own table over the same instances
-    from holo_b200 import build
-    cur = int(re.search(r"kL1L2BlocksPerSM = (\d+);", (build.CSRC / "isis_l1l2_rib.cu").read_text()).group(1))
+    cur = stage_bench.launch_bound(*BOUND)
     other = 4 if cur == 8 else 8
-    libv = C.CDLL(str(build_variant(other, Path(tempfile.mkdtemp(prefix="l1l2_bound_")))))
+    libv = C.CDLL(str(stage_bench.build_variant(*BOUND, other, "l1l2_bound_")))
     route_table.declare(libv)
     s1, s2 = isis.instance_struct(v["l1"]), isis.instance_struct(v["l2"])
     hv = C.c_void_p()
@@ -196,16 +168,12 @@ def main():
         got = isis.l1l2_rib_from_cells(v["l1"], v["l2"], t, ch[j], wh[j], planes, o)
         want, _ = chain(level_routes(v["l1"], o[0]), level_routes(without(v["l2"], v["l2_derived"]), o[2]), v["cfg"])
         same_rib(got, want)
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                         capture_output=True, text=True).stdout.strip()
+    gpu = ", ".join(stage_bench.card_and_power())
     out = dict(gpu=gpu, workload="C3 as the L2 backbone + a 2 000-system L1 area, 16 summaries", jobs=n, prefixes=P, summaries=S, l1_vertices=t.n_vertices[0][0], l2_vertices=t.n_vertices[1][0],
                spt_rows=n_rows, reps=args.reps, median_ms=med,
                profiler_kernel_ms=kern, launch_bound=cur, other_bound=other, cells_equal_other_bound=same_bounds, delta_records=tw, sampled_jobs_decoded=3,
                delta_checked_jobs=n)
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
     ctx.close()
 
 

@@ -14,17 +14,12 @@ job's adjacency.  Fails without a GPU.
 """
 import argparse
 import ctypes as C
-import json
-import subprocess
 import sys
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
+import stage_bench
 
 DATASHEET_GBS = 3350.0        # H100 SXM HBM3, NVIDIA data sheet
 
@@ -35,12 +30,11 @@ def main():
     ap.add_argument("--jobs", type=int, default=10000)
     ap.add_argument("--reps", type=int, default=10)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("isis_route_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("isis_route_stage.py")
     from bench import adjacency_edges
     from holo_b200 import capi, isis, synth
     from isis_synth import synth_instance
+    from test_isis_route_cells_gpu import DeviceTopology
 
     t = synth.random_topology(10000, 40000, synth.SEED_BASE + 3, cost_lo=1, cost_hi=1000)
     inst = synth_instance(t, 0)
@@ -58,29 +52,10 @@ def main():
     assert rt.root[isis.TOPO_STD] == root and rt.n_vertices[isis.TOPO_STD] == csr.n_vertices
     assert rt.root[isis.TOPO_MT6] == isis.NO_ROOT
     rt.upload(ctx)
-    g = ctx.upload(csr)
+    top = DeviceTopology(ctx, csr, root, n, ov)
     V, P, K = csr.n_vertices, rt.n_prefixes, rt.n_contributors
-    u16p, u32p, u64p = C.POINTER(C.c_uint16), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)
-
-    d_roots = torch.full((n,), root, dtype=torch.int32, device=dev)
-    off = np.zeros(n + 1, np.int64)
-    off[1:] = np.cumsum([len(o) for o in ov])
-    d_off = torch.from_numpy(off).to(torch.int32).to(dev)
-    d_ed = torch.from_numpy(np.asarray([e for o in ov for e, _ in o], np.uint32).view(np.int32).copy()).to(dev)
-    d_co = torch.from_numpy(np.asarray([c for o in ov for _, c in o], np.uint32).view(np.int32).copy()).to(dev)
-    js = capi.JobsStruct()
-    js.n_jobs = n
-    js.roots = C.cast(d_roots.data_ptr(), u32p)
-    js.ov_off, js.ov_edge, js.ov_cost = (C.cast(x.data_ptr(), u32p) for x in (d_off, d_ed, d_co))
-    dist = torch.empty(n * V, dtype=torch.int32, device=dev)
-    hops = torch.empty(n * V, dtype=torch.int16, device=dev)
-    nh = torch.empty(n * V, dtype=torch.int64, device=dev)
-    status = torch.zeros(n, dtype=torch.int32, device=dev)
+    u16p, u32p = C.POINTER(C.c_uint16), C.POINTER(C.c_uint32)
     cells = torch.empty(n * P * isis.CELL_DT.itemsize, dtype=torch.uint8, device=dev)
-    rs = capi.ResultStruct()
-    rs.dist, rs.hops = C.cast(dist.data_ptr(), u32p), C.cast(hops.data_ptr(), u16p)
-    rs.nh_mask, rs.nh_words = C.cast(nh.data_ptr(), u64p), 1
-    rs.job_status = C.cast(status.data_ptr(), u32p)
     torch.cuda.synchronize()
 
     stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
@@ -89,10 +64,10 @@ def main():
     def launch(e=None):
         if e:
             e[0].record(stream)
-        ctx.run_device(g, js, rs, sync=False)
+        ctx.run_device(top.g, top.js, top.rs, sync=False)
         if e:
             e[1].record(stream)
-        isis.routes_batch_device(ctx, rt, n, rs, None, cells.data_ptr())
+        isis.routes_batch_device(ctx, rt, n, top.rs, None, cells.data_ptr())
         if e:
             e[2].record(stream)
 
@@ -106,7 +81,7 @@ def main():
     rk = [b.elapsed_time(c) for _, b, c in ev]
 
     # ---- outside the timed region: status, one job decoded against compute_routes on the changed LSDB
-    st = status.cpu().numpy()
+    st = top.status.cpu().numpy()
     single = {}
     for k in range(t.n_p2p):
         key = tuple(sorted((int(t.p2p_a[k]), int(t.p2p_b[k]))))
@@ -114,8 +89,7 @@ def main():
     j = next(j for j in range(n) if single[tuple(sorted((int(t.p2p_a[j % len(pair)]), int(t.p2p_b[j % len(pair)]))))] == 1)
     a, b = int(t.p2p_a[j % len(pair)]), int(t.p2p_b[j % len(pair)])
     row = np.frombuffer(cells[j * P * 24:(j + 1) * P * 24].cpu().numpy().tobytes(), isis.CELL_DT)
-    dj = dist[j * V:(j + 1) * V].cpu().numpy().view(np.uint32).copy()
-    hj = hops[j * V:(j + 1) * V].cpu().numpy().view(np.uint16).copy()
+    dj, hj, _ = top.planes(j)
     t0 = time.perf_counter()
     got = isis.routes_from_cells(inst, rt, row, (dj, hj), None, ov[j])
     decode_ms = (time.perf_counter() - t0) * 1e3
@@ -136,9 +110,7 @@ def main():
         host_ms.append((time.perf_counter() - t0) * 1e3)
     assert r.rc == capi.HSPF_OK
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     cell_bytes = n * P * isis.CELL_DT.itemsize
     contrib_bytes = n * (K * 16 + P * 8)                      # every job reads its prefixes' records and offsets
     rk_ms, spt_ms = float(np.median(rk)), float(np.median(spt))
@@ -163,11 +135,7 @@ def main():
         "decode_check": {"job": j, "removed_adjacency": [a, b], "equal_to_compute_routes": bool(decode_ok),
                          "routes": int(len(got.routes))},
     }
-    line = json.dumps(out)
-    print(line)
-    if args.out:
-        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
     ctx.close()
     if not decode_ok:
         sys.exit("decoded cells differ from compute_routes")

@@ -18,38 +18,14 @@ total and every record), and sampled jobs decode to the host stages (area_from_p
 planes."""
 import argparse
 import ctypes as C
-import json
-import re
 import shutil
-import subprocess
-import sys
-import tempfile
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
+import stage_bench
 
-
-def build_variant(bound: int, tmp: Path) -> Path:
-    """libholo_spf.so with kAbrBlocksPerSM = bound, built from a copy of the sources in `tmp`."""
-    from holo_b200 import build
-    src = tmp / "holo_b200" / "csrc"                 # the sources include ../../include
-    shutil.copytree(build.CSRC, src)
-    shutil.copytree(build.ROOT / "include", tmp / "include")
-    cu = src / "ospfv2_abr_rib_cells.cu"
-    text, n = re.subn(r"constexpr uint32_t kAbrBlocksPerSM = \d+;", f"constexpr uint32_t kAbrBlocksPerSM = {bound};",
-                      cu.read_text())
-    assert n == 1
-    cu.write_text(text)
-    out = tmp / "libholo_spf_variant.so"
-    flags = [f for f in build.NVCC_FLAGS]
-    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
-    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *flags, "-o", str(out), *map(str, srcs)], check=True,
-                   capture_output=True)
-    return out
+BOUND = ("ospfv2_abr_rib_cells.cu", "kAbrBlocksPerSM")
 
 
 def torch_delta(cells, base, status, chunk=256):
@@ -93,11 +69,10 @@ def main():
     ap.add_argument("--jobs", type=int, default=10000)
     ap.add_argument("--reps", type=int, default=10)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ospf_abr_rib_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("ospf_abr_rib_stage.py")
     from holo_b200 import capi, ospf_rib, ospfv2, route_table, synth
     from holo_b200.route_table import DELTA_DT, DELTA_JOB_DT
+    from test_isis_route_cells_gpu import DeviceTopology
 
     t_setup = time.perf_counter()
     kw = dict(n_abr=16, n_asbr=16, n_inter=10000, n_ext=5000, n_overlap=3000, n_fresh=2000, n_ext_only=1000)
@@ -126,60 +101,27 @@ def main():
             e, r = pairs[int(rng.integers(len(pairs)))]
             rows[j, i] = len(ovs[i])
             ovs[i].append([(e, capi.COST_DISABLED), (r, capi.COST_DISABLED)])
-    u32p, u16p, u64p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16), C.POINTER(C.c_uint64)
-    keep, spt, rs_list, n_rows = [], [], [], []
-
-    def spt_batch(csr, root, ov):
-        m = len(ov)
-        g = ctx.upload(csr)
-        off = np.zeros(m + 1, np.int64)
-        ed, co = [], []
-        for j, o in enumerate(ov):
-            for e, cst in o:
-                ed.append(e); co.append(cst)
-            off[j + 1] = len(ed)
-        t = [torch.full((m,), root, dtype=torch.int32, device=dev), torch.from_numpy(off.astype(np.int32)).to(dev),
-             torch.from_numpy(np.asarray(ed or [0], np.uint32).view(np.int32).copy()).to(dev),
-             torch.from_numpy(np.asarray(co or [0], np.uint32).view(np.int32).copy()).to(dev)]
-        js = capi.JobsStruct()
-        js.n_jobs, js.roots, js.ov_off, js.ov_edge, js.ov_cost = m, *(C.cast(x.data_ptr(), u32p) for x in t)
-        V = csr.n_vertices
-        pl = [torch.empty(m * V, dtype=torch.int32, device=dev), torch.empty(m * V, dtype=torch.int16, device=dev),
-              torch.empty(m * V, dtype=torch.int64, device=dev), torch.zeros(m, dtype=torch.int32, device=dev)]
-        rs = capi.ResultStruct()
-        rs.dist, rs.hops = C.cast(pl[0].data_ptr(), u32p), C.cast(pl[1].data_ptr(), u16p)
-        rs.nh_mask, rs.nh_words = C.cast(pl[2].data_ptr(), u64p), 1
-        rs.job_status = C.cast(pl[3].data_ptr(), u32p)
-        keep.extend([g, t, pl, js])
-        return g, js, rs, pl
-
-    planes = []
-    for i in range(A):
-        g, js, rs, pl = spt_batch(flats[i].csr, rvs[i], ovs[i])
-        spt.append((g, js, rs))
-        rs_list.append(rs)
-        planes.append(pl)
-        n_rows.append(len(ovs[i]))
+    tops = [DeviceTopology(ctx, flats[i].csr, rvs[i], len(ovs[i]), ovs[i]) for i in range(A)]
+    rs_list, n_rows = [top.rs for top in tops], [top.n for top in tops]
     # the one-area stage for comparison: area 0's rows rooted at an internal router of area 0
     a0 = areas[0]
     internal = next(int(r) for r, fl in zip(a0.router_lsas["adv_rtr"], a0.router_lsas["flags"])
                     if not fl & 0x01 and flats[0].router_vertex(int(r)) != 0xFFFFFFFF)
     iv = flats[0].router_vertex(internal)
-    g_in, js_in, rs_in, pl_in = spt_batch(flats[0].csr, iv, ovs[0])
+    top_in = DeviceTopology(ctx, flats[0].csr, iv, len(ovs[0]), ovs[0])
     rt1 = ospf_rib.RibTable(flats[0], a0.area_id, sums[0], ext)
     rt1.upload(ctx)
     m0 = len(ovs[0])
     d_roots_in = torch.full((m0,), iv, dtype=torch.int32, device=dev)
     cells1 = torch.empty(m0 * rt1.n_prefixes * 24, dtype=torch.uint8, device=dev)
-    for g, js, rs in spt:
-        ctx.run_device(g, js, rs, sync=False)
-    ctx.run_device(g_in, js_in, rs_in, sync=False)
+    for top in tops + [top_in]:
+        top.run()
     ctx.sync()
     d_rows = torch.from_numpy(rows.view(np.int32).reshape(-1).copy()).to(dev)
 
     # the other launch bound, from a copy of the library
-    tmp = Path(tempfile.mkdtemp(prefix="abr_bound_"))
-    lib8 = C.CDLL(str(build_variant(8, tmp)))
+    lib8_path = stage_bench.build_variant(*BOUND, 8, "abr_bound_")
+    lib8 = C.CDLL(str(lib8_path))
     route_table.declare(lib8)
     fl_, ids_, sp_, ns_, act_, _s, ext_, _f = rt._keep
     h8 = C.c_void_p()
@@ -215,8 +157,8 @@ def main():
                                                      1, None, job_out.data_ptr(), recs.data_ptr() if with_records else None,
                                                      cap if with_records else 0, total.data_ptr())
 
-    variants = {f"spt_batch_area{i}": (lambda g=g, js=js, rs=rs: ctx.run_device(g, js, rs, sync=False))
-                for i, (g, js, rs) in enumerate(spt)}
+    variants = {f"spt_batch_area{i}": (lambda t=top: ctx.run_device(t.g, t.js, t.rs, sync=False))
+                for i, top in enumerate(tops)}
     variants.update({
         "abr_rib_cells_kernel_bound4": abr_cells(lib4, rt.handle, 4),
         "abr_rib_cells_kernel_bound8": abr_cells(lib8, h8, 8),
@@ -225,22 +167,9 @@ def main():
         "abr_rib_delta_records_bound4": delta(lib4, rt.handle, True),
         "abr_rib_delta_records_bound8": delta(lib8, h8, True),
         "ospf_rib_cells_kernel_area0_internal_root": lambda: ospf_rib.rib_cells_device(
-            ctx, rt1, m0, rs_in, d_roots_in.data_ptr(), cells1.data_ptr()),
+            ctx, rt1, m0, top_in.rs, d_roots_in.data_ptr(), cells1.data_ptr()),
     })
-    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
-    for _ in range(2):
-        for fn in variants.values():
-            fn()
-    ctx.sync()
-    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
-          for k in variants}
-    for r in range(args.reps):
-        for k, fn in variants.items():
-            ev[k][r][0].record(stream)
-            fn()
-            ev[k][r][1].record(stream)
-    ctx.sync()
-    ms = {k: [a.elapsed_time(b) for a, b in e] for k, e in ev.items()}
+    ms = stage_bench.time_alternating(ctx, variants, args.reps, 2)
     med = {k: float(np.median(v)) for k, v in ms.items()}
 
     # ---- outside the timed region
@@ -267,11 +196,7 @@ def main():
         cj = cells[4][j * P * 24: (j + 1) * P * 24].cpu().numpy().view(ospf_rib.RIB_CELL_DT)
         p, ga, gv, gn = [], [], [], []
         for i in range(A):
-            V = flats[i].csr.n_vertices
-            r = int(rows[j, i])
-            d = planes[i][0][r * V: (r + 1) * V].cpu().numpy().view(np.uint32).copy()
-            h = planes[i][1][r * V: (r + 1) * V].cpu().numpy().view(np.uint16).copy()
-            m = planes[i][2][r * V: (r + 1) * V].cpu().numpy().view(np.uint64).copy()
+            d, h, m = tops[i].planes(int(rows[j, i]))
             p.append((d, h, m))
             f, rv = flats[i], rvs[i]
             nets = sorted({int(v) for v in f.csr.col[f.csr.row_ptr[rv]: f.csr.row_ptr[rv + 1]] if not f.is_router[v]})
@@ -280,21 +205,15 @@ def main():
         got = ospf_rib.abr_rib_from_cells(areas, rt, cj, ga, gv, gn)
         t_dec = time.perf_counter() - t0
         t0 = time.perf_counter()
-        ra = []
-        for i, a in enumerate(areas):
-            m4 = np.zeros((len(p[i][0]), 4), np.uint64)
-            m4[:, 0] = p[i][2]
-            spf = ospfv2.area_from_planes(a, lambda c, r, w, d=p[i][0], h=p[i][1], m4=m4: (d, h, m4[:, :w]))
-            ra.append(ospf_rib.RibArea(a.area_id, spf, a.ifaces, sums[i]))
+        ra = [ospf_rib.RibArea(a.area_id, stage_bench.spf_from_planes("ospfv2", a, p[i]), a.ifaces, sums[i])
+              for i, a in enumerate(areas)]
         want = ospf_rib.update_rib_full(ospfv2.ABR_ROUTER_ID, a0.max_paths, ra, ext)
         t_host = time.perf_counter() - t0
         ok = (status[j] == 0 and got.rc == 0 and got.routes.tobytes() == want.routes.tobytes()
               and got.nexthops.tobytes() == want.nexthops.tobytes())
         decoded.append({"job": int(j), "rows": [int(x) for x in rows[j]], "routes": int(len(got.routes)), "equal": bool(ok),
                         "decode_s": round(t_dec, 4), "host_stages_s": round(t_host, 4)})
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     out = {
         "workload": f"ABR {ospfv2.ABR_ROUTER_ID:#x} of ospfv2.abr_view(seed 0xC5): area 0 = C5 (10000 routers, 40000 directed "
                     f"adjacencies, costs {{10, 20}}, 5 % on LANs) with inter_area_view({kw}); areas 1, 2 = synth_area of "
@@ -308,13 +227,9 @@ def main():
         "cells_bound4_equal_bound8": same_bounds, "delta_checks": checks, "sampled_decodes": decoded,
         "setup_s": round(time.perf_counter() - t_setup, 1),
     }
-    text = json.dumps(out, indent=1)
-    print(json.dumps({k: out[k] for k in ("card", "power_limit", "median_ms", "cells_bound4_equal_bound8", "delta_checks",
-                                          "changes", "prefixes", "areas")}, indent=1))
+    stage_bench.write_json(out, args.out)
     print("decodes equal:", all(d["equal"] for d in decoded))
-    if args.out:
-        Path(args.out).write_text(text + "\n")
-    shutil.rmtree(tmp, ignore_errors=True)
+    shutil.rmtree(lib8_path.parent, ignore_errors=True)
 
 
 if __name__ == "__main__":

@@ -25,44 +25,14 @@ the host chain the stage replaces (each border's area_from_planes + update_rib_f
 into area 1, type 3 and type 4, then R's update_rib_full), timed over a few jobs."""
 import argparse
 import ctypes as C
-import json
-import re
-import shutil
-import subprocess
 import sys
-import tempfile
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-CONST = "kNonBackboneBlocksPerSM"
+import stage_bench
 
-
-def build_variant(bound: int, tmp: Path) -> Path:
-    """libholo_spf.so with kNonBackboneBlocksPerSM = bound, built from a copy of the sources in `tmp`."""
-    from holo_b200 import build
-    src = tmp / "holo_b200" / "csrc"
-    shutil.copytree(build.CSRC, src)
-    shutil.copytree(build.ROOT / "include", tmp / "include")
-    cu = src / "ospfv2_backbone.cu"
-    text, n = re.subn(rf"constexpr uint32_t {CONST} = \d+;", f"constexpr uint32_t {CONST} = {bound};", cu.read_text())
-    assert n == 1
-    cu.write_text(text)
-    out = tmp / "libholo_spf_variant.so"
-    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
-    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *build.NVCC_FLAGS, "-o", str(out), *map(str, srcs)], check=True,
-                   capture_output=True)
-    return out
-
-
-def current_bound() -> int:
-    return int(re.search(rf"constexpr uint32_t {CONST} = (\d+);",
-                         (ROOT / "holo_b200" / "csrc" / "ospfv2_backbone.cu").read_text()).group(1))
-
-
+BOUND = ("ospfv2_backbone.cu", "kNonBackboneBlocksPerSM")
 
 
 def main():
@@ -74,51 +44,19 @@ def main():
     ap.add_argument("--v0", type=int, default=10000, help="area-0 routers (C5: 10000)")
     ap.add_argument("--v1", type=int, default=2000, help="area-1 routers")
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ospf_nonbackbone_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("ospf_nonbackbone_stage.py")
     from holo_b200 import capi, ospf_rib, ospfv2, route_table, synth
     from holo_b200.route_table import DELTA_JOB_DT, DELTA_DT
+    from test_isis_route_cells_gpu import DeviceTopology
 
     ctx = capi.Context(0)
     dev = torch.device("cuda", 0)
 
-    def device_spf(csr, root, nhw):
-        g = ctx.upload(csr)
-        r = ctx.run(g, np.array([root], np.uint32))
-        g.free()
-        return r.dist[0], r.hops[0], np.pad(r.nh_mask[0], ((0, 0), (0, nhw - r.nh_mask.shape[2])))
-
     t0 = synth.random_topology(args.v0, 4 * args.v0, synth.SEED_BASE + 5, cost_choices=[10, 20], lan_fraction=0.05)
     t1 = synth.random_topology(args.v1, 4 * args.v1, synth.SEED_BASE + 850, cost_choices=[10, 20], lan_fraction=0.05)
-    v = ospfv2.nonbackbone_view(t0, t1, 0xC5, device_spf, n_ext=2000)
+    v = ospfv2.nonbackbone_view(t0, t1, 0xC5, stage_bench.root_spf(ctx), n_ext=2000)
     rng = np.random.default_rng(0xC5)
-    u32p, u16p, u64p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16), C.POINTER(C.c_uint64)
     keep = []
-
-    def spt_batch(csr, root, ov):
-        m = len(ov)
-        g = ctx.upload(csr)
-        off = np.zeros(m + 1, np.int64)
-        ed, co = [], []
-        for j, o in enumerate(ov):
-            for e, cst in o:
-                ed.append(e); co.append(cst)
-            off[j + 1] = len(ed)
-        t = [torch.full((m,), root, dtype=torch.int32, device=dev), torch.from_numpy(off.astype(np.int32)).to(dev),
-             torch.from_numpy(np.asarray(ed or [0], np.uint32).view(np.int32).copy()).to(dev),
-             torch.from_numpy(np.asarray(co or [0], np.uint32).view(np.int32).copy()).to(dev)]
-        js = capi.JobsStruct()
-        js.n_jobs, js.roots, js.ov_off, js.ov_edge, js.ov_cost = m, *(C.cast(x.data_ptr(), u32p) for x in t)
-        V = csr.n_vertices
-        pl = [torch.empty(m * V, dtype=torch.int32, device=dev), torch.empty(m * V, dtype=torch.int16, device=dev),
-              torch.empty(m * V, dtype=torch.int64, device=dev), torch.zeros(m, dtype=torch.int32, device=dev)]
-        rs = capi.ResultStruct()
-        rs.dist, rs.hops = C.cast(pl[0].data_ptr(), u32p), C.cast(pl[1].data_ptr(), u16p)
-        rs.nh_mask, rs.nh_words = C.cast(pl[2].data_ptr(), u64p), 1
-        rs.job_status = C.cast(pl[3].data_ptr(), u32p)
-        keep.extend([g, t, pl, js])
-        return rs, pl, lambda: ctx.run_device(g, js, rs, sync=False)
 
     # the tables, R's table and the jobs' size before any batch: how many jobs fit
     tables, flats_all = [], []
@@ -147,7 +85,7 @@ def main():
                     if f0.link_index[e] != 0xFFFFFFFF and f0.is_router[f0.csr.col[e]]})
     job_links = [None] + [(links[int(rng.integers(len(links)))], int(rng.choice([capi.COST_DISABLED, 35])))
                           for _ in range(n - 1)]
-    border_cells, planes_all, border_rs, border_nrows, border_rows, spt_runs, abr_runs = [], [], [], [], [], [], []
+    border_cells, tops_all, border_rs, border_nrows, border_rows, spt_runs, abr_runs = [], [], [], [], [], [], []
     for b, (areas, ids, sums) in enumerate(v["borders"]):
         flats, rt = flats_all[b], tables[b]
         f = flats[i0[b]]
@@ -155,15 +93,15 @@ def main():
         by_pair = {}
         for e in range(f.csr.n_edges):
             by_pair.setdefault(tuple(sorted((int(f.ids[s[e]]), int(f.ids[f.csr.col[e]])))), []).append(e)
-        rs_list, n_rows, pls = [], [], []
+        rs_list, n_rows, tops = [], [], []
         for i, fl in enumerate(flats):
             root = fl.router_vertex(areas[0].router_id)
             ov = [[]] if i != i0[b] else [[(e, jl[1]) for e in by_pair.get(jl[0], [])] if jl else [] for jl in job_links]
-            rs, pl, run = spt_batch(fl.csr, root, ov)
-            run()
+            top = DeviceTopology(ctx, fl.csr, root, len(ov), ov)
+            top.run()
             if i == i0[b]:
-                spt_runs.append(run)
-            rs_list.append(rs); n_rows.append(len(ov)); pls.append(pl)
+                spt_runs.append(lambda t=top: ctx.run_device(t.g, t.js, t.rs, sync=False))
+            rs_list.append(top.rs); n_rows.append(top.n); tops.append(top)
         rows = np.zeros((n, len(areas)), np.uint32)
         rows[:, i0[b]] = np.arange(n)
         d_rows = torch.from_numpy(rows.view(np.int32).reshape(-1).copy()).to(dev)
@@ -176,15 +114,16 @@ def main():
         border_rs.append((capi.ResultStruct * len(rs_list))(*rs_list))
         border_nrows.append(np.asarray(n_rows, np.uint32))
         border_rows.append(d_rows.data_ptr())
-        border_cells.append(cells); planes_all.append(pls)
-    rs_r, pl_r, run_r = spt_batch(r_flat.csr, rv, [[]])
-    run_r()
+        border_cells.append(cells); tops_all.append(tops)
+    rtop = DeviceTopology(ctx, r_flat.csr, rv, 1, [[]])
+    rtop.run()
+    rs_r = rtop.rs
     ctx.sync()
     bc = [c.data_ptr() for c in border_cells]
 
-    cur = current_bound()
+    cur = stage_bench.launch_bound(*BOUND)
     other = 8 if cur == 4 else 4
-    libv = C.CDLL(str(build_variant(other, Path(tempfile.mkdtemp(prefix="nonbackbone_bound_")))))
+    libv = C.CDLL(str(stage_bench.build_variant(*BOUND, other, "nonbackbone_bound_")))
     route_table.declare(libv)
     # the variant's own tables over the same images
     vt = []
@@ -245,34 +184,12 @@ def main():
         work[f"nonbackbone_cells_bound{b}"] = cell_launch(b)
         work[f"nonbackbone_delta_summaries_bound{b}"] = delta(b, False)
         work[f"nonbackbone_delta_records_bound{b}"] = delta(b, True)
-    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
-    for _ in range(2):
-        for fn in work.values():
-            fn()
-    ctx.sync()
-    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
-          for k in work}
-    for r in range(args.reps):
-        for k, fn in work.items():
-            ev[k][r][0].record(stream)
-            fn()
-            ev[k][r][1].record(stream)
-    ctx.sync()
-    med = {k: float(np.median([a.elapsed_time(b) for a, b in ev[k]])) for k in work}
+    med = {k: float(np.median(x)) for k, x in stage_bench.time_alternating(ctx, work, args.reps, 2).items()}
     same_after = bool(torch.equal(cells[4], cells[8]))
 
     # host chain per job (CPU), over the device planes read back
-    def host_planes(pl, row, V):
-        d = pl[0].view(torch.int32).reshape(-1, V)[row].cpu().numpy().view(np.uint32)
-        hh = pl[1].reshape(-1, V)[row].cpu().numpy().view(np.uint16)
-        m = pl[2].reshape(-1, V)[row].cpu().numpy().view(np.uint64)
-        return d, hh, m
-
-    def spf_of(a, p):
-        return ospfv2.area_from_planes(a, lambda csr, root, nhw: (p[0], p[1], np.pad(p[2][:, None], ((0, 0), (0, nhw - 1)))))
-
     host_ms = []
-    rp = host_planes(pl_r, 0, r_flat.csr.n_vertices)
+    rp = rtop.planes(0)
     bids = {int(x.router_id) for x in tables}
     for j in range(1, 1 + min(args.host_jobs, n - 1)):
         t = time.perf_counter()
@@ -280,21 +197,20 @@ def main():
         for b, (areas, ids, sums) in enumerate(v["borders"]):
             ra = []
             for i, a in enumerate(areas):
-                p = host_planes(planes_all[b][i], j if i == i0[b] else 0, flats_all[b][i].csr.n_vertices)
-                ra.append(ospf_rib.RibArea(a.area_id, spf_of(a, p), a.ifaces, sums[i], True))
+                spf = stage_bench.spf_from_planes("ospfv2", a, tops_all[b][i].planes(j if i == i0[b] else 0))
+                ra.append(ospf_rib.RibArea(a.area_id, spf, a.ifaces, sums[i], True))
             rid = areas[0].router_id
             rib = ospf_rib.update_rib_full(rid, areas[0].max_paths, ra, v["externals"])
             new += list(ospf_rib.net_summaries(rid, rib, ospf_rib.router_tables(rid, ra), ra,
                                                [ospf_rib.area_config()] * len(areas), ids.index(1)))
         s = np.array(new, ospf_rib.SUMMARY_LSA_DT)
         s = s[np.lexsort((s["lsa_id"], s["adv_rtr"], s["lsa_type"]))]
-        ospf_rib.update_rib_full(r_area.router_id, r_area.max_paths,
-                                 [ospf_rib.RibArea(1, spf_of(r_area, rp), r_area.ifaces, s, True)], v["externals"])
+        r_spf = stage_bench.spf_from_planes("ospfv2", r_area, rp)
+        ospf_rib.update_rib_full(r_area.router_id, r_area.max_paths, [ospf_rib.RibArea(1, r_spf, r_area.ifaces, s, True)],
+                                 v["externals"])
         host_ms.append((time.perf_counter() - t) * 1e3)
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     out = {
         "stage": "hspf_ospfv2_nonbackbone_table_create + hspf_ospfv2_backbone_asbr_cells / _delta",
         "workload": {"area0": f"{args.v0} routers, {4 * args.v0} links, costs {{10, 20}}, 5 % LANs",
@@ -311,9 +227,7 @@ def main():
         "note": "device figures are CUDA-event medians of alternating launches; the host chain is a CPU figure",
     }
     print(f"device memory held: {held / 2**30:.1f} GiB ({n} jobs)", file=sys.stderr)
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
 
 
 if __name__ == "__main__":

@@ -11,16 +11,12 @@ same run; the host stages (area_from_planes + update_rib_full) are timed per roo
 jobs are decoded and compared with the host stages over the same planes."""
 import argparse
 import ctypes as C
-import json
-import subprocess
 import sys
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
+import stage_bench
 
 DATASHEET_GBS = 3350.0            # H100 SXM5 HBM3
 
@@ -31,9 +27,7 @@ def main():
     ap.add_argument("--roots", type=int, default=1000)
     ap.add_argument("--reps", type=int, default=10)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ospf_rib_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("ospf_rib_stage.py")
     from holo_b200 import capi, ospf_rib, ospfv2, synth
 
     kw = dict(n_abr=16, n_asbr=16, n_inter=10000, n_ext=5000, n_overlap=3000, n_fresh=2000, n_ext_only=1000)
@@ -81,20 +75,7 @@ def main():
         "ospf_rib_cells_kernel": lambda: ospf_rib.rib_cells_device(ctx, rt, n, rs, d_roots.data_ptr(), rib_cells.data_ptr(),
                                                                    st_out.data_ptr()),
     }
-    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
-    for _ in range(3):
-        for fn in variants.values():
-            fn()
-    ctx.sync()
-    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
-          for k in variants}
-    for r in range(args.reps):
-        for k, fn in variants.items():
-            ev[k][r][0].record(stream)
-            fn()
-            ev[k][r][1].record(stream)
-    ctx.sync()
-    ms = {k: [a.elapsed_time(b) for a, b in e] for k, e in ev.items()}
+    ms = stage_bench.time_alternating(ctx, variants, args.reps, 3)
     med = {k: float(np.median(v)) for k, v in ms.items()}
 
     # ---- outside the timed region: sampled jobs decoded against the host stages over the same planes
@@ -127,9 +108,7 @@ def main():
         kinds += np.bincount(got.routes["path_type"], minlength=4)[:4]
         checks.append({"job": int(j), "root": int(a.router_id), "routes": int(len(got.routes)), "equal": bool(ok)})
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     K = rt.n_contributors
     rib_bytes = {"cell_writes": n * P * 24, "records": n * K * 16, "offsets": n * P * 12,
                  "note": "records and offsets are re-read by every job and mostly stay in L2; plane gathers not counted"}
@@ -155,10 +134,7 @@ def main():
                                           "type2": int(kinds[3])},
         "cross_check_against_host_stages": checks,
     }
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
     ctx.close()
     if not all(c["equal"] for c in checks):
         sys.exit("ospf_rib_stage.py: a decoded job differs from the host stages")

@@ -22,42 +22,13 @@ router tables + net_summaries into area 0, each C's over those into area 2, then
 few jobs."""
 import argparse
 import ctypes as C
-import json
-import re
-import shutil
-import subprocess
-import sys
-import tempfile
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-CONST = "kThirdAreaBlocksPerSM"
+import stage_bench
 
-
-def build_variant(bound: int, tmp: Path) -> Path:
-    """libholo_spf.so with kThirdAreaBlocksPerSM = bound, built from a copy of the sources in `tmp`."""
-    from holo_b200 import build
-    src = tmp / "holo_b200" / "csrc"
-    shutil.copytree(build.CSRC, src)
-    shutil.copytree(build.ROOT / "include", tmp / "include")
-    cu = src / "ospfv2_backbone.cu"
-    text, n = re.subn(rf"constexpr uint32_t {CONST} = \d+;", f"constexpr uint32_t {CONST} = {bound};", cu.read_text())
-    assert n == 1
-    cu.write_text(text)
-    out = tmp / "libholo_spf_variant.so"
-    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
-    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *build.NVCC_FLAGS, "-o", str(out), *map(str, srcs)], check=True,
-                   capture_output=True)
-    return out
-
-
-def current_bound() -> int:
-    return int(re.search(rf"constexpr uint32_t {CONST} = (\d+);",
-                         (ROOT / "holo_b200" / "csrc" / "ospfv2_backbone.cu").read_text()).group(1))
+BOUND = ("ospfv2_backbone.cu", "kThirdAreaBlocksPerSM")
 
 
 def main():
@@ -67,61 +38,21 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--host-jobs", type=int, default=2)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ospf_third_area_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("ospf_third_area_stage.py")
     from holo_b200 import capi, ospf_rib, ospfv2, route_table, synth
     from holo_b200.route_table import DELTA_JOB_DT, DELTA_DT
+    from test_isis_route_cells_gpu import DeviceTopology
 
     ctx = capi.Context(0)
     dev = torch.device("cuda", 0)
     n = args.jobs
     rng = np.random.default_rng(0xC5)
-    u32p, u16p, u64p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16), C.POINTER(C.c_uint64)
     keep = []
-
-    def spt_batch(csr, root, ov):
-        m = len(ov)
-        g = ctx.upload(csr)
-        off = np.zeros(m + 1, np.int64)
-        ed, co = [], []
-        for j, o in enumerate(ov):
-            for e, cst in o:
-                ed.append(e); co.append(cst)
-            off[j + 1] = len(ed)
-        t = [torch.full((m,), root, dtype=torch.int32, device=dev), torch.from_numpy(off.astype(np.int32)).to(dev),
-             torch.from_numpy(np.asarray(ed or [0], np.uint32).view(np.int32).copy()).to(dev),
-             torch.from_numpy(np.asarray(co or [0], np.uint32).view(np.int32).copy()).to(dev)]
-        js = capi.JobsStruct()
-        js.n_jobs, js.roots, js.ov_off, js.ov_edge, js.ov_cost = m, *(C.cast(x.data_ptr(), u32p) for x in t)
-        V = csr.n_vertices
-        pl = [torch.empty(m * V, dtype=torch.int32, device=dev), torch.empty(m * V, dtype=torch.int16, device=dev),
-              torch.empty(m * V, dtype=torch.int64, device=dev), torch.zeros(m, dtype=torch.int32, device=dev)]
-        rs = capi.ResultStruct()
-        rs.dist, rs.hops = C.cast(pl[0].data_ptr(), u32p), C.cast(pl[1].data_ptr(), u16p)
-        rs.nh_mask, rs.nh_words = C.cast(pl[2].data_ptr(), u64p), 1
-        rs.job_status = C.cast(pl[3].data_ptr(), u32p)
-        keep.extend([g, t, pl, js])
-        ctx.run_device(g, js, rs, sync=False)
-        return rs, pl
-
-    def host_planes(pl, row, V):
-        d = pl[0].view(torch.int32).reshape(-1, V)[row].cpu().numpy().view(np.uint32)
-        hh = pl[1].reshape(-1, V)[row].cpu().numpy().view(np.uint16)
-        m = pl[2].reshape(-1, V)[row].cpu().numpy().view(np.uint64)
-        return d, hh, m
-
-    def device_spf(csr, root, nhw):
-        """Unperturbed planes of one root, for the view's base-job summaries."""
-        _rs, pl = spt_batch(csr, root, [[]])
-        ctx.sync()
-        d, hh, m = host_planes(pl, 0, csr.n_vertices)
-        return d, hh, np.pad(m[:, None], ((0, 0), (0, nhw - 1)))
 
     t0 = synth.random_topology(10000, 40000, synth.SEED_BASE + 5, cost_choices=[10, 20], lan_fraction=0.05)
     t1 = synth.random_topology(2000, 8000, synth.SEED_BASE + 850, cost_choices=[10, 20], lan_fraction=0.05)
     t2 = synth.random_topology(2000, 8000, synth.SEED_BASE + 851, cost_choices=[10, 20], lan_fraction=0.05)
-    v = ospfv2.third_area_view(t0, t1, t2, 0xC5, device_spf, n_c=2, area1_asbrs=2, area1_ext=1000)
+    v = ospfv2.third_area_view(t0, t1, t2, 0xC5, stage_bench.root_spf(ctx), n_c=2, area1_asbrs=2, area1_ext=1000)
 
     # the jobs: one link of area 1 per job, named by its end points' ids
     i1 = [b[1].index(1) for b in v["borders"]]
@@ -130,7 +61,7 @@ def main():
     links = sorted({tuple(sorted((int(f1.ids[src[e]]), int(f1.ids[f1.csr.col[e]])))) for e in range(f1.csr.n_edges)
                     if f1.link_index[e] != 0xFFFFFFFF})
     job_links = [None] + [links[int(rng.integers(len(links)))] for _ in range(n - 1)]
-    tables, border_cells, flats_all, planes_all, border_rs, border_nrows, border_rows = [], [], [], [], [], [], []
+    tables, border_cells, flats_all, tops_all, border_rs, border_nrows, border_rows = [], [], [], [], [], [], []
     for b, (areas, ids, sums) in enumerate(v["borders"]):
         flats = [ospfv2.Flat(a) for a in areas]
         rt = ospf_rib.AbrRibTable(areas[0].router_id, flats, ids, sums, None, v["externals"])
@@ -140,12 +71,13 @@ def main():
         by_pair = {}
         for e in range(f.csr.n_edges):
             by_pair.setdefault(tuple(sorted((int(f.ids[s[e]]), int(f.ids[f.csr.col[e]])))), []).append(e)
-        rs_list, n_rows, pls = [], [], []
+        rs_list, n_rows, tops = [], [], []
         for i, fl in enumerate(flats):
             root = fl.router_vertex(areas[0].router_id)
             ov = [[]] if i != i1[b] else [[(e, capi.COST_DISABLED) for e in by_pair.get(l, [])] if l else [] for l in job_links]
-            rs, pl = spt_batch(fl.csr, root, ov)
-            rs_list.append(rs); n_rows.append(len(ov)); pls.append(pl)
+            top = DeviceTopology(ctx, fl.csr, root, len(ov), ov)
+            top.run()
+            rs_list.append(top.rs); n_rows.append(top.n); tops.append(top)
         rows = np.zeros((n, 2), np.uint32)
         rows[:, i1[b]] = np.arange(n)
         d_rows = torch.from_numpy(rows.view(np.int32).reshape(-1).copy()).to(dev)
@@ -155,16 +87,16 @@ def main():
         border_rs.append(rs_list)
         border_nrows.append(n_rows)
         border_rows.append(d_rows.data_ptr())
-        tables.append(rt); border_cells.append(cells); flats_all.append(flats); planes_all.append(pls)
+        tables.append(rt); border_cells.append(cells); flats_all.append(flats); tops_all.append(tops)
     bc = [c.data_ptr() for c in border_cells]
     # the C's: row 0 of each area, abr_backbone cells over the B's, and their ASBR entries
-    ctables, c_rs, c_pl, c_cells, c_ent, c_est = [], [], [], [], [], []
+    ctables, c_rs, c_tops, c_cells, c_ent, c_est = [], [], [], [], [], []
     for areas, ids, sums in v["c_areas"]:
         flats = [ospfv2.Flat(a) for a in areas]
-        rl, pl_ = [], []
-        for a, f in zip(areas, flats):
-            rs, pl = spt_batch(f.csr, f.router_vertex(a.router_id), [[]])
-            rl.append(rs); pl_.append(pl)
+        tops = [DeviceTopology(ctx, f.csr, f.router_vertex(a.router_id), 1, [[]]) for a, f in zip(areas, flats)]
+        for top in tops:
+            top.run()
+        rl = [top.rs for top in tops]
         ct = ospf_rib.AbrBackboneTable(areas[0].router_id, flats, ids, sums, None, v["externals"], tables)
         ct.upload(ctx)
         out = torch.empty(n * ct.n_prefixes * 24, dtype=torch.uint8, device=dev)
@@ -176,10 +108,12 @@ def main():
         est = torch.empty(n, dtype=torch.int32, device=dev)
         ospf_rib.abr_backbone_asbr_entries_device(ctx, ct, n, rl, border_rs, border_nrows, border_rows, est.data_ptr(),
                                                   ent.data_ptr())
-        ctables.append(ct); c_rs.append(rl); c_pl.append(pl_); c_cells.append(out); c_ent.append(ent); c_est.append(est)
+        ctables.append(ct); c_rs.append(rl); c_tops.append(tops); c_cells.append(out); c_ent.append(ent); c_est.append(est)
     ra = v["r_area"]
     rf = ospfv2.Flat(ra)
-    r_rs, r_pl = spt_batch(rf.csr, rf.router_vertex(ra.router_id), [[]])
+    rtop = DeviceTopology(ctx, rf.csr, rf.router_vertex(ra.router_id), 1, [[]])
+    rtop.run()
+    r_rs = rtop.rs
     tt = ospf_rib.BackboneTable(rf, ra.router_id, v["summaries2"], v["externals"], ctables,
                                 config=ospf_rib.area_config())
     assert tt.third_area and tt.n_asbr_slots > 0
@@ -188,9 +122,9 @@ def main():
     assert not any(x.any().item() for x in c_est)
     P = tt.n_prefixes
 
-    cur = current_bound()
+    cur = stage_bench.launch_bound(*BOUND)
     other = 8 if cur == 4 else 4
-    libv = C.CDLL(str(build_variant(other, Path(tempfile.mkdtemp(prefix="third_area_bound_")))))
+    libv = C.CDLL(str(stage_bench.build_variant(*BOUND, other, "third_area_bound_")))
     route_table.declare(libv)
     # the variant's own copy of R's table, over the same flat and C tables
     hv = C.c_void_p()
@@ -244,32 +178,16 @@ def main():
         work[f"third_area_cells_bound{b}"] = cell_launch(b)
         work[f"third_area_delta_summaries_bound{b}"] = delta(b, False)
         work[f"third_area_delta_records_bound{b}"] = delta(b, True)
-    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
-    for _ in range(2):
-        for fn in work.values():
-            fn()
-    ctx.sync()
-    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
-          for k in work}
-    for r in range(args.reps):
-        for k, fn in work.items():
-            ev[k][r][0].record(stream)
-            fn()
-            ev[k][r][1].record(stream)
-    ctx.sync()
-    med = {k: float(np.median([a.elapsed_time(b) for a, b in ev[k]])) for k in work}
+    med = {k: float(np.median(x)) for k, x in stage_bench.time_alternating(ctx, work, args.reps, 2).items()}
     held = torch.cuda.memory_allocated(dev)
     free, total_mem = torch.cuda.mem_get_info()
 
     # host chain per job (CPU), over the device planes read back
-    def spf_of(a, p):
-        return ospfv2.area_from_planes(a, lambda csr, root, nhw: (p[0], p[1], np.pad(p[2][:, None], ((0, 0), (0, nhw - 1)))))
 
     cfg = [ospf_rib.area_config()] * 2
     host_ms = []
-    cp = [[host_planes(pl, 0, ospfv2.Flat(a).csr.n_vertices) for pl, a in zip(pls, areas)]
-          for pls, (areas, _i, _s) in zip(c_pl, v["c_areas"])]
-    rp = host_planes(r_pl, 0, rf.csr.n_vertices)
+    cp = [[top.planes(0) for top in tops] for tops in c_tops]
+    rp = rtop.planes(0)
     bids = {int(x.router_id) for x in tables}
     cids = {int(x.router_id) for x in ctables}
     for j in range(1, 1 + args.host_jobs):
@@ -278,8 +196,8 @@ def main():
         for b, (areas, ids, sums) in enumerate(v["borders"]):
             rab = []
             for i, a in enumerate(areas):
-                p = host_planes(planes_all[b][i], j if i == i1[b] else 0, flats_all[b][i].csr.n_vertices)
-                rab.append(ospf_rib.RibArea(a.area_id, spf_of(a, p), a.ifaces, sums[i], True))
+                spf = stage_bench.spf_from_planes("ospfv2", a, tops_all[b][i].planes(j if i == i1[b] else 0))
+                rab.append(ospf_rib.RibArea(a.area_id, spf, a.ifaces, sums[i], True))
             rid = areas[0].router_id
             rib = ospf_rib.update_rib_full(rid, areas[0].max_paths, rab, v["externals"])
             new0 += list(ospf_rib.net_summaries(rid, rib, ospf_rib.router_tables(rid, rab), rab, cfg, ids.index(0)))
@@ -287,20 +205,19 @@ def main():
         s0 = s0[np.lexsort((s0["lsa_id"], s0["adv_rtr"], s0["lsa_type"]))]
         new2 = [s for s in v["summaries2"] if int(s["adv_rtr"]) not in cids]
         for (areas, ids, sums), pls in zip(v["c_areas"], cp):
-            rac = [ospf_rib.RibArea(a.area_id, spf_of(a, p), a.ifaces, s0 if a.area_id == 0 else ss, True)
-                   for a, p, ss in zip(areas, pls, sums)]
+            rac = [ospf_rib.RibArea(a.area_id, stage_bench.spf_from_planes("ospfv2", a, p), a.ifaces,
+                                    s0 if a.area_id == 0 else ss, True) for a, p, ss in zip(areas, pls, sums)]
             rid = areas[0].router_id
             rib = ospf_rib.update_rib_full(rid, areas[0].max_paths, rac, v["externals"])
             new2 += list(ospf_rib.net_summaries(rid, rib, ospf_rib.router_tables(rid, rac), rac, cfg, ids.index(2)))
         s2 = np.array(new2, ospf_rib.SUMMARY_LSA_DT)
         s2 = s2[np.lexsort((s2["lsa_id"], s2["adv_rtr"], s2["lsa_type"]))]
-        ospf_rib.update_rib_full(ra.router_id, ra.max_paths, [ospf_rib.RibArea(2, spf_of(ra, rp), ra.ifaces, s2, True)],
+        r_spf = stage_bench.spf_from_planes("ospfv2", ra, rp)
+        ospf_rib.update_rib_full(ra.router_id, ra.max_paths, [ospf_rib.RibArea(2, r_spf, ra.ifaces, s2, True)],
                                  v["externals"])
         host_ms.append((time.perf_counter() - t) * 1e3)
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     out = {
         "stage": "hspf_ospfv2_abr_backbone_asbr_entries, hspf_ospfv2_third_area_cells / hspf_ospfv2_third_area_delta",
         "workload": {"area0": "C5: 10000 routers, 40000 links, costs {10, 20}, 5 % LANs", "area1": "2000 routers",
@@ -317,9 +234,7 @@ def main():
         "host_chain_ms_per_job": float(np.median(host_ms)), "host_jobs_timed": len(host_ms),
         "note": "device figures are CUDA-event medians of alternating launches; the host chain is a CPU figure",
     }
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
 
 
 if __name__ == "__main__":

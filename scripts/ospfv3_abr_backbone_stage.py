@@ -21,42 +21,13 @@ update_rib_full_v3 + net_summaries_v3 + rtr_summaries_v3, then R's update_rib_fu
 a few jobs."""
 import argparse
 import ctypes as C
-import json
-import re
-import shutil
-import subprocess
-import sys
-import tempfile
 import time
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-CONST = "kAbrBackboneV3BlocksPerSM"
+import stage_bench
 
-
-def build_variant(bound: int, tmp: Path) -> Path:
-    """libholo_spf.so with kAbrBackboneV3BlocksPerSM = bound, built from a copy of the sources in `tmp`."""
-    from holo_b200 import build
-    src = tmp / "holo_b200" / "csrc"
-    shutil.copytree(build.CSRC, src)
-    shutil.copytree(build.ROOT / "include", tmp / "include")
-    cu = src / "ospfv2_abr_backbone.cu"
-    text, n = re.subn(rf"constexpr uint32_t {CONST} = \d+;", f"constexpr uint32_t {CONST} = {bound};", cu.read_text())
-    assert n == 1
-    cu.write_text(text)
-    out = tmp / "libholo_spf_variant.so"
-    srcs = sorted(list(src.glob("*.cu")) + list(src.glob("*.cc")))
-    subprocess.run([build.os.environ.get("NVCC", "nvcc"), *build.NVCC_FLAGS, "-o", str(out), *map(str, srcs)], check=True,
-                   capture_output=True)
-    return out
-
-
-def current_bound() -> int:
-    return int(re.search(rf"constexpr uint32_t {CONST} = (\d+);",
-                         (ROOT / "holo_b200" / "csrc" / "ospfv2_abr_backbone.cu").read_text()).group(1))
+BOUND = ("ospfv2_abr_backbone.cu", "kAbrBackboneV3BlocksPerSM")
 
 
 def main():
@@ -66,11 +37,10 @@ def main():
     ap.add_argument("--reps", type=int, default=10)
     ap.add_argument("--host-jobs", type=int, default=2)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ospfv3_abr_backbone_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("ospfv3_abr_backbone_stage.py")
     from holo_b200 import capi, ospf_rib, ospfv3, route_table, synth
     from holo_b200.route_table import DELTA_JOB_DT, DELTA_DT
+    from test_isis_route_cells_gpu import DeviceTopology
 
     t0 = synth.random_topology(10000, 40000, synth.SEED_BASE + 5, cost_choices=[10, 20], lan_fraction=0.05)
     t1 = synth.random_topology(2000, 8000, synth.SEED_BASE + 850, cost_choices=[10, 20], lan_fraction=0.05)
@@ -80,33 +50,7 @@ def main():
     dev = torch.device("cuda", 0)
     n = args.jobs
     rng = np.random.default_rng(0xC5)
-    u32p, u16p, u64p = C.POINTER(C.c_uint32), C.POINTER(C.c_uint16), C.POINTER(C.c_uint64)
     keep = []
-
-    def spt_batch(csr, root, ov):
-        m = len(ov)
-        g = ctx.upload(csr)
-        off = np.zeros(m + 1, np.int64)
-        ed, co = [], []
-        for j, o in enumerate(ov):
-            for e, cst in o:
-                ed.append(e); co.append(cst)
-            off[j + 1] = len(ed)
-        t = [torch.full((m,), root, dtype=torch.int32, device=dev), torch.from_numpy(off.astype(np.int32)).to(dev),
-             torch.from_numpy(np.asarray(ed or [0], np.uint32).view(np.int32).copy()).to(dev),
-             torch.from_numpy(np.asarray(co or [0], np.uint32).view(np.int32).copy()).to(dev)]
-        js = capi.JobsStruct()
-        js.n_jobs, js.roots, js.ov_off, js.ov_edge, js.ov_cost = m, *(C.cast(x.data_ptr(), u32p) for x in t)
-        V = csr.n_vertices
-        pl = [torch.empty(m * V, dtype=torch.int32, device=dev), torch.empty(m * V, dtype=torch.int16, device=dev),
-              torch.empty(m * V, dtype=torch.int64, device=dev), torch.zeros(m, dtype=torch.int32, device=dev)]
-        rs = capi.ResultStruct()
-        rs.dist, rs.hops = C.cast(pl[0].data_ptr(), u32p), C.cast(pl[1].data_ptr(), u16p)
-        rs.nh_mask, rs.nh_words = C.cast(pl[2].data_ptr(), u64p), 1
-        rs.job_status = C.cast(pl[3].data_ptr(), u32p)
-        keep.extend([g, t, pl, js])
-        ctx.run_device(g, js, rs, sync=False)
-        return rs, pl
 
     # the jobs: one link of the area per job, named by its end points' ids
     bareas = [b[0] for b in v["borders"]]
@@ -116,7 +60,7 @@ def main():
     links = sorted({tuple(sorted((int(f1.router_ids[src[e]]), int(f1.router_ids[f1.csr.col[e]]))))
                     for e in range(f1.csr.n_edges) if f1.is_router[src[e]] and f1.is_router[f1.csr.col[e]]})
     job_links = [None] + [links[int(rng.integers(len(links)))] for _ in range(n - 1)]
-    tables, border_cells, flats_all, planes_all, border_rs, border_nrows, border_rows = [], [], [], [], [], [], []
+    tables, border_cells, flats_all, tops_all, border_rs, border_nrows, border_rows = [], [], [], [], [], [], []
     for b, (areas, ids, sums) in enumerate(v["borders"]):
         flats = [ospfv3.Flat(a) for a in areas]
         rt = ospf_rib.AbrRibTable(areas[0].router_id, flats, ids, sums, None, v["externals"])
@@ -127,12 +71,13 @@ def main():
         for e in range(f.csr.n_edges):
             if f.is_router[s[e]] and f.is_router[f.csr.col[e]]:
                 by_pair.setdefault(tuple(sorted((int(f.router_ids[s[e]]), int(f.router_ids[f.csr.col[e]])))), []).append(e)
-        rs_list, n_rows, pls = [], [], []
+        rs_list, n_rows, tops = [], [], []
         for i, fl in enumerate(flats):
             root = fl.router_vertex(areas[0].router_id)
             ov = [[]] if i != i1[b] else [[(e, capi.COST_DISABLED) for e in by_pair.get(l, [])] if l else [] for l in job_links]
-            rs, pl = spt_batch(fl.csr, root, ov)
-            rs_list.append(rs); n_rows.append(len(ov)); pls.append(pl)
+            top = DeviceTopology(ctx, fl.csr, root, len(ov), ov)
+            top.run()
+            rs_list.append(top.rs); n_rows.append(top.n); tops.append(top)
         rows = np.zeros((n, len(areas)), np.uint32)
         rows[:, i1[b]] = np.arange(n)
         d_rows = torch.from_numpy(rows.view(np.int32).reshape(-1).copy()).to(dev)
@@ -142,25 +87,24 @@ def main():
         border_rs.append((capi.ResultStruct * len(rs_list))(*rs_list))
         border_nrows.append(np.asarray(n_rows, np.uint32))
         border_rows.append(d_rows.data_ptr())
-        tables.append(rt); border_cells.append(cells); flats_all.append(flats); planes_all.append(pls)
+        tables.append(rt); border_cells.append(cells); flats_all.append(flats); tops_all.append(tops)
     r_areas = v["r_areas"]
     r_flats = [ospfv3.Flat(a) for a in r_areas]
-    r_rs, r_pl = [], []
-    for a, f in zip(r_areas, r_flats):
-        rs, pl = spt_batch(f.csr, f.router_vertex(a.router_id), [[]])
-        r_rs.append(rs); r_pl.append(pl)
+    r_tops = [DeviceTopology(ctx, f.csr, f.router_vertex(a.router_id), 1, [[]]) for a, f in zip(r_areas, r_flats)]
+    for top in r_tops:
+        top.run()
     bt = ospf_rib.AbrBackboneTable(r_areas[0].router_id, r_flats, v["area_ids"], v["summaries"], None, v["externals"],
                                    tables)
     assert bt.v3 and bt.n_asbr_slots > 0
     bt.upload(ctx)
-    r_arr = (capi.ResultStruct * len(r_rs))(*r_rs)
+    r_arr = (capi.ResultStruct * len(r_tops))(*[top.rs for top in r_tops])
     ctx.sync()
     P = bt.n_prefixes
     bc = [c.data_ptr() for c in border_cells]
 
-    cur = current_bound()
+    cur = stage_bench.launch_bound(*BOUND)
     other = 8 if cur == 4 else 4
-    libv = C.CDLL(str(build_variant(other, Path(tempfile.mkdtemp(prefix="abr_backbone_v3_bound_")))))
+    libv = C.CDLL(str(stage_bench.build_variant(*BOUND, other, "abr_backbone_v3_bound_")))
     route_table.declare(libv)
     # the variant's own tables over the same images
     vt = []
@@ -218,33 +162,11 @@ def main():
         work[f"abr_backbone_cells_bound{b}"] = cell_launch(b)
         work[f"abr_backbone_delta_summaries_bound{b}"] = delta(b, False)
         work[f"abr_backbone_delta_records_bound{b}"] = delta(b, True)
-    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
-    for _ in range(2):
-        for fn in work.values():
-            fn()
-    ctx.sync()
-    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
-          for k in work}
-    for r in range(args.reps):
-        for k, fn in work.items():
-            ev[k][r][0].record(stream)
-            fn()
-            ev[k][r][1].record(stream)
-    ctx.sync()
-    med = {k: float(np.median([a.elapsed_time(b) for a, b in ev[k]])) for k in work}
+    med = {k: float(np.median(x)) for k, x in stage_bench.time_alternating(ctx, work, args.reps, 2).items()}
 
     # host chain per job (CPU), over the device planes read back
-    def host_planes(pl, row, V):
-        d = pl[0].view(torch.int32).reshape(-1, V)[row].cpu().numpy().view(np.uint32)
-        hh = pl[1].reshape(-1, V)[row].cpu().numpy().view(np.uint16)
-        m = pl[2].reshape(-1, V)[row].cpu().numpy().view(np.uint64)
-        return d, hh, m
-
-    def spf_of(a, p):
-        return ospfv3.area_from_planes(a, lambda csr, root, nhw: (p[0], p[1], np.pad(p[2][:, None], ((0, 0), (0, nhw - 1)))))
-
     host_ms = []
-    rp = [host_planes(pl, 0, f.csr.n_vertices) for pl, f in zip(r_pl, r_flats)]
+    rp = [top.planes(0) for top in r_tops]
     bids = {int(x.router_id) for x in tables}
     for j in range(1, 1 + args.host_jobs):
         t = time.perf_counter()
@@ -252,19 +174,18 @@ def main():
         for b, (areas, ids, sums) in enumerate(v["borders"]):
             ra = []
             for i, a in enumerate(areas):
-                p = host_planes(planes_all[b][i], j if i == i1[b] else 0, flats_all[b][i].csr.n_vertices)
-                ra.append(ospf_rib.RibArea(a.area_id, spf_of(a, p), a.ifaces, sums[i], True))
+                spf = stage_bench.spf_from_planes("ospfv3", a, tops_all[b][i].planes(j if i == i1[b] else 0))
+                ra.append(ospf_rib.RibArea(a.area_id, spf, a.ifaces, sums[i], True))
             new += ospfv3.nonbackbone_lsas(areas[0].router_id, areas[0].max_paths, ra, v["externals"], ids.index(0))
         s = np.array(new, ospf_rib.INTER_AREA_LSA_DT)
         s = s[np.lexsort((s["lsa_id"], s["adv_rtr"], s["lsa_type"]))]
         ospf_rib.update_rib_full_v3(r_areas[0].router_id, r_areas[0].max_paths,
-                                 [ospf_rib.RibArea(a.area_id, spf_of(a, p), a.ifaces, s if a.area_id == 0 else ss, True)
+                                 [ospf_rib.RibArea(a.area_id, stage_bench.spf_from_planes("ospfv3", a, p), a.ifaces,
+                                                   s if a.area_id == 0 else ss, True)
                                   for a, p, ss in zip(r_areas, rp, v["summaries"])], v["externals"])
         host_ms.append((time.perf_counter() - t) * 1e3)
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     out = {
         "stage": "hspf_ospfv3_abr_backbone_table_create, hspf_ospfv2_abr_backbone_cells / _delta (OSPFv3 table)",
         "workload": {"area0": "C5 as OSPFv3: 10000 routers, 40000 links, costs {10, 20}, 5 % LANs",
@@ -279,9 +200,7 @@ def main():
         "host_chain_ms_per_job": float(np.median(host_ms)), "host_jobs_timed": len(host_ms),
         "note": "device figures are CUDA-event medians of alternating launches; the host chain is a CPU figure",
     }
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
 
 
 if __name__ == "__main__":

@@ -20,16 +20,11 @@ tables.  Fails without a GPU.
 """
 import argparse
 import ctypes as C
-import json
-import subprocess
 import sys
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "scripts"))
+import stage_bench
 
 
 def link_pairs(flat):
@@ -48,12 +43,11 @@ def main():
     ap.add_argument("--jobs", type=int, default=10000)
     ap.add_argument("--reps", type=int, default=10)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("ospfv3_rib_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("ospfv3_rib_stage.py")
     from holo_b200 import capi, ospf_rib, ospfv3, synth
     from ospf_rib_delta_stage import torch_delta
     from holo_b200.route_table import DELTA_DT, DELTA_GAINED, DELTA_JOB_DT, DELTA_LOST, DELTA_METRIC
+    from test_isis_route_cells_gpu import DeviceTopology
 
     kw = dict(n_abr=16, n_asbr=16, n_inter=10000, n_ext=5000, n_overlap=3000, n_fresh=2000, n_ext_only=1000)
     t = synth.random_topology(10000, 40000, synth.SEED_BASE + 5, cost_choices=[10, 20], lan_fraction=0.05)
@@ -80,31 +74,16 @@ def main():
     dev = torch.device("cuda", 0)
     rt = ospf_rib.RibTable(flat, 1, sums, ext)
     rt.upload(ctx)
-    g = ctx.upload(csr)
     P = rt.n_prefixes
-    u16p, u32p, u64p = C.POINTER(C.c_uint16), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)
+    top = DeviceTopology(ctx, csr, rv, n, [[]] + [[(e, capi.COST_DISABLED) for e in pr] for pr in cut])
+    rs = top.rs
     d_roots = torch.full((n,), rv, dtype=torch.int32, device=dev)
-    js = capi.JobsStruct()
-    js.n_jobs, js.roots = n, C.cast(d_roots.data_ptr(), u32p)
-    off = np.arange(n + 1, dtype=np.int64) * 2 - 2
-    off[0] = 0
-    ed = np.asarray([e for pr in cut for e in pr], np.uint32)
-    d_off = torch.from_numpy(off.astype(np.int32)).to(dev)
-    d_ed = torch.from_numpy(ed.view(np.int32).copy()).to(dev)
-    d_co = torch.from_numpy(np.full(len(ed), capi.COST_DISABLED, np.uint32).view(np.int32).copy()).to(dev)
-    js.ov_off, js.ov_edge, js.ov_cost = (C.cast(x.data_ptr(), u32p) for x in (d_off, d_ed, d_co))
-    planes = [torch.empty(n * V, dtype=torch.int32, device=dev), torch.empty(n * V, dtype=torch.int16, device=dev),
-              torch.empty(n * V, dtype=torch.int64, device=dev), torch.zeros(n, dtype=torch.int32, device=dev)]
-    rs = capi.ResultStruct()
-    rs.dist, rs.hops = C.cast(planes[0].data_ptr(), u32p), C.cast(planes[1].data_ptr(), u16p)
-    rs.nh_mask, rs.nh_words = C.cast(planes[2].data_ptr(), u64p), 1
-    rs.job_status = C.cast(planes[3].data_ptr(), u32p)
     cells = torch.empty(n * P * 24, dtype=torch.uint8, device=dev)
     st_out = torch.zeros(n, dtype=torch.int32, device=dev)
     job_out = torch.empty(n * DELTA_JOB_DT.itemsize, dtype=torch.uint8, device=dev)
     total = torch.zeros(1, dtype=torch.int64, device=dev)
-    torch.cuda.synchronize()
-    ctx.run_device(g, js, rs, sync=True)
+    top.run()
+    ctx.sync()
     # the base row: job 0's cells (no override)
     ospf_rib.rib_cells_device(ctx, rt, n, rs, d_roots.data_ptr(), cells.data_ptr(), st_out.data_ptr())
     base = cells[: P * 24].clone()
@@ -124,36 +103,23 @@ def main():
     n_changes = int(total.item())
     records = torch.empty(max(n_changes, 1) * DELTA_DT.itemsize, dtype=torch.uint8, device=dev)
     variants = {
-        "spt_batch": lambda: ctx.run_device(g, js, rs, sync=False),
+        "spt_batch": lambda: ctx.run_device(top.g, top.js, rs, sync=False),
         "ospf_rib_cells_kernel": run_cells,
         "delta_summary": lambda: delta_call(fn_a),
         "delta_records": lambda: delta_call(fn_a, records, n_changes),
     }
-    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
-    for _ in range(3):                                       # warm-up: modules, kernels, workspace, caches
-        for fn in variants.values():
-            fn()
-    ctx.sync()
-    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
-          for k in variants}
-    for r in range(args.reps):                               # alternating, so that clocks and heat are shared
-        for k, fn in variants.items():
-            ev[k][r][0].record(stream)
-            fn()
-            ev[k][r][1].record(stream)
-    ctx.sync()
-    ms = {k: [a.elapsed_time(b) for a, b in e] for k, e in ev.items()}
+    ms = stage_bench.time_alternating(ctx, variants, args.reps, 3)
     med = {k: float(np.median(v)) for k, v in ms.items()}
 
     # ---- outside the timed region: the delta against torch's comparison of the stored cells, every job
     check = {"jobs": n}
-    ctx.run_device(g, js, rs, sync=True)
+    ctx.run_device(top.g, top.js, rs, sync=True)
     run_cells()
     records.fill_(0xAB)
     delta_call(fn_a, records, n_changes)
     ctx.sync()
     jo_t, rec_t, tot = job_out.clone(), records.clone(), int(total.item())
-    status = planes[3].clone()
+    status = top.status.clone()
     counts, want = torch_delta(cells, base, n, P)
     jo = jo_t.view(torch.int32).view(n, 8)
     rec = rec_t[: n_changes * DELTA_DT.itemsize].view(torch.int32).view(n_changes, 4)
@@ -166,7 +132,7 @@ def main():
     # ---- sampled jobs decoded; their records tied to the decoded tables
     host_cells = lambda j: cells[j * P * 24:(j + 1) * P * 24].cpu().numpy().view(ospf_rib.RIB_CELL_DT)
     nets = sorted({int(v) for v in csr.col[csr.row_ptr[rv]: csr.row_ptr[rv + 1]] if not flat.is_router[v]})
-    nh = planes[2].view(n, V)
+    nh = top.nh.view(n, V)
     key = lambda p, ln: (bytes(p["bytes"].tolist()), int(ln))
     index = {key(p, ln): i for i, (p, ln) in enumerate(zip(rt.prefix, rt.plen))}
 
@@ -196,9 +162,7 @@ def main():
         ties.append({"job": int(j), "decoded": True, "records": int(len(r)), "equal": bool(ok)})
     check["sampled_decodes_tie"] = all(x.get("equal", False) for x in ties)
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     kinds = {name: int(jo[:, i].sum().item()) for i, name in enumerate(("changed", "lost", "gained", "metric", "nexthops",
                                                                         "other"))}
     out = {
@@ -220,10 +184,7 @@ def main():
         "cross_check_against_torch": check,
         "sampled_decodes": ties,
     }
-    print(json.dumps(out))
-    if args.out:
-        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
+    stage_bench.write_json(out, args.out)
     ctx.close()
     if not (check["total"] and check["summaries"] and check["records"] and check["sampled_decodes_tie"]):
         sys.exit("ospfv3_rib_stage.py: a cross-check failed")

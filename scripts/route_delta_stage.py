@@ -15,17 +15,11 @@ row done with torch on the device, for every job: summaries, total and every rec
     python scripts/route_delta_stage.py [--out FILE] [--jobs N] [--reps R]
 """
 import argparse
-import ctypes as C
-import json
-import subprocess
 import sys
-from pathlib import Path
 
 import numpy as np
 
-ROOT = Path(__file__).resolve().parent.parent
-sys.path.insert(0, str(ROOT))
-sys.path.insert(0, str(ROOT / "tests"))
+import stage_bench
 
 DATASHEET_GBS = 3350.0        # H100 SXM HBM3, NVIDIA data sheet
 
@@ -64,13 +58,12 @@ def main():
     ap.add_argument("--jobs", type=int, default=10000)
     ap.add_argument("--reps", type=int, default=10)
     args = ap.parse_args()
-    import torch
-    if not torch.cuda.is_available():
-        sys.exit("route_delta_stage.py: no CUDA device; this measurement runs on the GPU only")
+    torch = stage_bench.require_gpu("route_delta_stage.py")
     from bench import adjacency_edges
     from holo_b200 import capi, isis, synth
     from holo_b200.route_table import DELTA_DT, DELTA_JOB_DT
     from isis_synth import synth_instance
+    from test_isis_route_cells_gpu import DeviceTopology
 
     t = synth.random_topology(10000, 40000, synth.SEED_BASE + 3, cost_lo=1, cost_hi=1000)
     inst = synth_instance(t, 0)
@@ -87,38 +80,14 @@ def main():
     assert rt.root[isis.TOPO_STD] == root and rt.n_vertices[isis.TOPO_STD] == csr.n_vertices
     assert rt.root[isis.TOPO_MT6] == isis.NO_ROOT
     rt.upload(ctx)
-    g = ctx.upload(csr)
     V, P, K = csr.n_vertices, rt.n_prefixes, rt.n_contributors
-    u16p, u32p, u64p = C.POINTER(C.c_uint16), C.POINTER(C.c_uint32), C.POINTER(C.c_uint64)
-
-    def batch(k, overrides):
-        d_roots = torch.full((k,), root, dtype=torch.int32, device=dev)
-        js = capi.JobsStruct()
-        js.n_jobs, js.roots = k, C.cast(d_roots.data_ptr(), u32p)
-        keep = [d_roots]
-        if overrides:
-            off = np.zeros(k + 1, np.int64)
-            off[1:] = np.cumsum([len(o) for o in overrides])
-            d_off = torch.from_numpy(off).to(torch.int32).to(dev)
-            d_ed = torch.from_numpy(np.asarray([e for o in overrides for e, _ in o], np.uint32).view(np.int32).copy()).to(dev)
-            d_co = torch.from_numpy(np.asarray([c for o in overrides for _, c in o], np.uint32).view(np.int32).copy()).to(dev)
-            js.ov_off, js.ov_edge, js.ov_cost = (C.cast(x.data_ptr(), u32p) for x in (d_off, d_ed, d_co))
-            keep += [d_off, d_ed, d_co]
-        planes = [torch.empty(k * V, dtype=torch.int32, device=dev), torch.empty(k * V, dtype=torch.int16, device=dev),
-                  torch.empty(k * V, dtype=torch.int64, device=dev), torch.zeros(k, dtype=torch.int32, device=dev)]
-        rs = capi.ResultStruct()
-        rs.dist, rs.hops = C.cast(planes[0].data_ptr(), u32p), C.cast(planes[1].data_ptr(), u16p)
-        rs.nh_mask, rs.nh_words = C.cast(planes[2].data_ptr(), u64p), 1
-        rs.job_status = C.cast(planes[3].data_ptr(), u32p)
-        torch.cuda.synchronize()
-        ctx.run_device(g, js, rs, sync=True)
-        return rs, keep + planes
-
-    base_rs, base_keep = batch(1, None)
+    base_top = DeviceTopology(ctx, csr, root, 1)
+    base_top.run()
     base = torch.empty(P * 24, dtype=torch.uint8, device=dev)
-    isis.routes_batch_device(ctx, rt, 1, base_rs, None, base.data_ptr())
-    rs, keep = batch(n, ov)
-    status = keep[-1]
+    isis.routes_batch_device(ctx, rt, 1, base_top.rs, None, base.data_ptr())
+    top = DeviceTopology(ctx, csr, root, n, ov)
+    top.run()
+    rs, status = top.rs, top.status
     cells = torch.empty(n * P * 24, dtype=torch.uint8, device=dev)
     job_out = torch.empty(n * DELTA_JOB_DT.itemsize, dtype=torch.uint8, device=dev)
     total = torch.zeros(1, dtype=torch.int64, device=dev)
@@ -136,20 +105,7 @@ def main():
     n_changes = int(total.item())
     records = torch.empty(max(n_changes, 1) * DELTA_DT.itemsize, dtype=torch.uint8, device=dev)
     variants = {"cells": run_cells, "delta_summary": run_delta, "delta_records": lambda: run_delta(records, n_changes)}
-    stream = torch.cuda.ExternalStream(ctx.stream, device=dev)
-    for _ in range(3):                                       # warm-up: modules, kernels, workspace, caches
-        for fn in variants.values():
-            fn()
-    ctx.sync()
-    ev = {k: [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(args.reps)]
-          for k in variants}
-    for r in range(args.reps):                               # alternating, so that clocks and heat are shared
-        for k, fn in variants.items():
-            ev[k][r][0].record(stream)
-            fn()
-            ev[k][r][1].record(stream)
-    ctx.sync()
-    ms = {k: [a.elapsed_time(b) for a, b in e] for k, e in ev.items()}
+    ms = stage_bench.time_alternating(ctx, variants, args.reps, 3)
 
     # ---- outside the timed region: the delta against torch's comparison of the stored cells, every job
     run_cells()
@@ -171,9 +127,7 @@ def main():
     per_job = jo[:, 0].cpu().numpy()
     kinds = {name: int(jo[:, i].sum().item()) for i, name in enumerate(("changed", "lost", "gained", "metric", "nexthops", "other"))}
 
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    card, power = (q[0].split(", ") + ["?"])[:2] if q else (torch.cuda.get_device_name(0), "?")
+    card, power = stage_bench.card_and_power()
     n_tiles = (n * P + 31) // 32
     contrib = n * (K * 16 + P * 8)                            # every job reads its prefixes' records and offsets
     gathers = n * K * 14                                      # dist + hops + nh_mask of each contributor's vertex
@@ -210,12 +164,8 @@ def main():
         "datasheet_bw_GBps": DATASHEET_GBS,
         "cross_check_against_torch": check,
     }
-    line = json.dumps(out)
-    print(line)
-    if args.out:
-        Path(args.out).parent.mkdir(parents=True, exist_ok=True)
-        Path(args.out).write_text(json.dumps(out, indent=1) + "\n")
-    del base_keep, keep
+    stage_bench.write_json(out, args.out)
+    del base_top, top
     ctx.close()
     if not ok:
         sys.exit("the delta differs from torch's comparison of the stored cells")
