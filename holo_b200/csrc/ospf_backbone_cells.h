@@ -49,7 +49,8 @@ inline bool backbone_winners_fit(uint64_t n_recs, uint64_t n_slots, bool v3) {
 // What the walk reads of a table.  Per border b, border[4 b ..] (OSPFv2) or border[8 b ..] (OSPFv3): its area-0
 // intra-area records [lo, hi) and its area-0 atom bits (low word, high word); OSPFv3 adds the byte offset, from
 // `border`, of the border's options bytes, one per intra-area record of its table (the winner of an intra-area cell
-// indexes them), then three zero words.
+// indexes them), then three zero words (an OSPFv3 third-area table: C's record count, then two zero words, and C's
+// options bytes cover every record index below that count).
 struct OspfBackboneView {
     const uint32_t *oi;           // [PR + 1] R's intra-area ranges (R's one-area table)
     const uint32_t *q;            // [P] the prefix's index in R's one-area table, kNoRecord if none
@@ -129,7 +130,12 @@ struct OspfAsbrPlanes : Planes {
 // metric and, for OSPFv3 (kV3), the prefix options of the cell's winner.  Into area 0 only an intra-area route is
 // advertised; into a non-backbone area (kNonBackbone, hspf_ospfv2_nonbackbone_table_create) an inter-area one too
 // (compute_net_summaries).  The border words name the target area's intra-area records and atoms.
-template <bool kV3, bool kNonBackbone = false>
+// kSlotWinners (OSPFv3 third-area tables, hspf_ospfv3_third_area_table_create): the border's cells are those of an
+// OSPFv3 abr_backbone table, whose inter-area winners from its own slots are n_recs_C + (slot << 8 | options).  The
+// border's sixth word is n_recs_C: a winner at or above it carries its options in the low byte of winner - n_recs_C,
+// and a record winner (an intra-area walk record, a static Inter-Area-Prefix record) reads them from the options
+// bytes.
+template <bool kV3, bool kNonBackbone = false, bool kSlotWinners = false>
 HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, uint32_t b, uint32_t &metric,
                             uint32_t &options) {
     constexpr uint32_t kStride = kV3 ? 2 : 1;                          // 16-byte groups per border
@@ -151,7 +157,19 @@ HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, u
                      (winner < bb.x || winner >= bb.y) && !(nh & atoms0) && metric < HL_LSA_INFINITY;
     if constexpr (kV3) {
         options = 0;
-        if (adv) {
+        if constexpr (kSlotWinners) {
+            if (adv) {
+#if defined(__CUDA_ARCH__)
+                const uint2 ow = __ldg(reinterpret_cast<const uint2 *>(border + 8 * b + 4));
+                options = winner >= ow.y ? ((winner - ow.y) & 0xFFu)
+                                         : __ldg(reinterpret_cast<const uint8_t *>(border) + ow.x + winner);
+#else
+                const uint32_t n = border[8 * b + 5];
+                options = winner >= n ? ((winner - n) & 0xFFu)
+                                      : reinterpret_cast<const uint8_t *>(border)[border[8 * b + 4] + winner];
+#endif
+            }
+        } else if (adv) {
 #if defined(__CUDA_ARCH__)
             options = __ldg(reinterpret_cast<const uint8_t *>(border) + __ldg(border + 8 * b + 4) + winner);
 #else
@@ -165,7 +183,8 @@ HSPF_HD bool border_summary(const hl_ospf_rib_cell *c, const uint32_t *border, u
 // kV3: the table is an OSPFv3 one (hspf_ospfv3_backbone_table_create), whose slot winners carry prefix options.
 // kAsbr: the table's type-4 ranges hold slots, read through pl.asbr (pl an OspfAsbrPlanes of the job).
 // kNonBackbone: the table's target area is not area 0 (border_summary).
-template <bool kV3 = false, bool kAsbr = false, bool kNonBackbone = false, class Planes>
+// kSlotWinners: the borders' cells may hold OSPFv3 slot winners (border_summary; an OSPFv3 third-area table).
+template <bool kV3 = false, bool kAsbr = false, bool kNonBackbone = false, bool kSlotWinners = false, class Planes>
 HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneView &t, uint32_t p,
                                           const OspfBorderRows &rows) {
     const RouteContrib *contribs = reinterpret_cast<const RouteContrib *>(t.recs);
@@ -182,7 +201,8 @@ HSPF_HD CellWords ospf_backbone_cell_eval(const Planes &pl, const OspfBackboneVi
         if (!pl.reached(r.x)) continue;
         uint32_t y = r.y, w = i, options = 0;
         if (r.z != kOspfBackboneStatic) {
-            if (!border_summary<kV3, kNonBackbone>(rows.row[r.z] + r.y, t.border, r.z, y, options)) continue;
+            if (!border_summary<kV3, kNonBackbone, kSlotWinners>(rows.row[r.z] + r.y, t.border, r.z, y, options))
+                continue;
             w = kV3 ? t.n_recs + (r.w << 8 | options) : t.n_recs + r.w;
         }
         const uint32_t m = pl.d(r.x) + y;
@@ -277,6 +297,10 @@ HSPF_HD uint32_t abr_row0_status(const AbrPlaneSet<D, N> &s, uint32_t n_areas) {
 // for A then holds one chain slot per C, at C's place in LsaKey order:
 //   chain slot: x C's vertex, y the group's index among C's groups with type-4 slots, z C, w kOspfBackboneAsbrSlot | C
 // and the walk reads C's entry of the job (abr_asbr_entry below, stored by hspf_ospfv2_abr_backbone_asbr_entries).
+// OSPFv3 (hspf_ospfv3_third_area_table_create): C copies its route's prefix options into the Inter-Area-Prefix LSA it
+// originates, and C's inter-area routes come from the B's slots, whose winners carry the options (n_recs_C + (slot << 8
+// | options)); the walk reads them with kSlotWinners (border_summary).  C's Inter-Area-Router ranges hold the same
+// records as OSPFv2's type-4 ranges, so abr_asbr_entry serves both versions.
 constexpr uint32_t kOspfNoEntry = 0xFFFFFFFFu;        // an entry C does not originate a type-4 LSA for
 
 // C's area-0 entry of an ASBR, as rib_full step 2 leaves it and compute_rtr_summaries re-originates it into a normal
@@ -389,7 +413,8 @@ struct hspf_ospfv2_backbone_table {
     std::vector<hl_ip_addr> prefix6;
     std::vector<uint8_t> options6;
     // hspf_ospfv2_third_area_table_create: the borders are C tables (borders[b] is third[b]->abr), and the type-4
-    // slots are chain slots (n_asbr_slots of them, no plane set), read by the third-area calls only
+    // slots are chain slots (n_asbr_slots of them, no plane set), read by the third-area calls only; an OSPFv3 one
+    // (hspf_ospfv3_third_area_table_create, v3 set) is read by the third-area calls only, with or without them
     bool third_area = false;
     const hspf_ospfv2_abr_backbone_table *third[hspf::kOspfBackboneMaxBorders] = {};
     hspf::DeviceRouteTable dev;                  // hspf_ospfv2_backbone_table_upload: words, then records

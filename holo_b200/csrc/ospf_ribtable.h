@@ -453,6 +453,52 @@ inline std::array<uint32_t, 4> walk_border_words(const hspf_ospfv2_abr_backbone_
     return w;
 }
 
+// Every C's walk_border_words over its target-area index at[b], appended to `words` (which ends on a 16-byte
+// boundary).  OSPFv3 (kV3): 8 words per C, the fifth the byte offset from the first border word of C's options bytes
+// and the sixth C's record count (border_summary with kSlotWinners), then every C's options bytes, each padded to a
+// word: one per record index below that count, the prefix options of a walk intra-area record (its decode record's
+// entry in its area's intra-area table) and of a type-3 record (C's options6), 0 for any other.  HSPF_E_INVAL when a
+// C's table does not hold those options.
+template <bool kV3>
+int append_walk_border_words(std::vector<uint32_t> &words, const hspf_ospfv2_abr_backbone_table *const *cs,
+                             uint32_t n_borders, const uint32_t *at) {
+    uint32_t opt_words = (kV3 ? 8 : 4) * n_borders;
+    for (uint32_t b = 0; b < n_borders; ++b) {
+        const std::array<uint32_t, 4> bw = walk_border_words(*cs[b], at[b]);
+        words.insert(words.end(), bw.begin(), bw.end());
+        if (kV3) {
+            const uint32_t n = cs[b]->n_recs();
+            words.insert(words.end(), {4 * opt_words, n, 0u, 0u});
+            opt_words += (n + 3) / 4;
+        }
+    }
+    if (kV3) {
+        for (uint32_t b = 0; b < n_borders; ++b) {
+            const hspf_ospfv2_abr_backbone_table &c = *cs[b];
+            const hspf_ospfv2_abr_ribtable &a = *c.abr;
+            const uint32_t n = c.n_recs();
+            std::vector<uint8_t> opt(((size_t)n + 3) & ~(size_t)3, 0);
+            if (a.t3_base.empty() || a.options6.size() < a.t3_end - a.t3_base[0] ||
+                c.intra_src.size() != n - c.walk_intra)
+                return HSPF_E_INVAL;
+            for (uint32_t k = a.t3_base[0]; k < a.t3_end; ++k) opt[k] = a.options6[k - a.t3_base[0]];
+            for (uint32_t k = c.walk_intra; k < n; ++k) {
+                const uint32_t src = c.intra_src[k - c.walk_intra];
+                uint32_t i = 0;
+                while (i < a.n_areas && !(src >= a.intra_base[i] && src < a.intra_base[i] + a.area[i]->n_intra)) ++i;
+                if (i == a.n_areas) return HSPF_E_INVAL;
+                const std::vector<uint8_t> &o = a.area[i]->intra->t.options6;
+                if (o.size() != a.area[i]->n_intra) return HSPF_E_INVAL;
+                opt[k] = o[src - a.intra_base[i]];
+            }
+            const size_t w = words.size();
+            words.resize(w + opt.size() / 4);
+            if (!opt.empty()) std::memcpy(words.data() + w, opt.data(), opt.size());
+        }
+    }
+    return HSPF_OK;
+}
+
 // Every border's words over its target-area index at[b], appended to `words` (which ends on a 16-byte boundary).
 // OSPFv3 (kV3): 8 words per border, the fifth the byte offset from the first border word of the border's options
 // bytes, which follow all the border words, each border's padded to a word: one per record an advertised cell's
@@ -511,10 +557,11 @@ int append_border_words(std::vector<uint32_t> &words, const hspf_ospfv2_abr_ribt
 // (plane sets of any of those areas, area 0 included); in a stub area the default route stays static and no type-4
 // LSA is originated, and a totally stubby area has no slot.  OSPFv3: a border's options bytes also cover its type-3
 // records, so that an inter-area cell's winner gives the options of the LSA the border copies them from.
-// `third` (OSPFv2 with `config`, build_third_area_table): borders[b] is third[b]->abr, C's table restricted to its
-// affected prefixes.  A C LSA for a key outside C's prefixes, or a type-4 LSA for an ASBR without type-4 slots in C's
-// table, stays a static record; the type-4 slots are chain slots (ospf_backbone_cells.h: OspfChainJob), one per (C,
-// group of C with type-4 slots), and the border words name C's walk intra-area records (walk_border_words).
+// `third` (with `config`, build_third_area_table): borders[b] is third[b]->abr, C's table restricted to its affected
+// prefixes.  A C LSA for a key outside C's prefixes, or a type-4 / Inter-Area-Router LSA for an ASBR without type-4
+// slots in C's table, stays a static record; the type-4 slots are chain slots (ospf_backbone_cells.h: OspfChainJob),
+// one per (C, group of C with type-4 slots), and the border words name C's walk intra-area records
+// (append_walk_border_words; OSPFv3: with C's record count and options bytes, which its slot winners need).
 template <class T>
 int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const typename T::Sum *sums, uint32_t n_sums,
                          const typename T::Ext *ext, uint32_t n_ext, const hspf_ospfv2_abr_ribtable *const *borders,
@@ -526,7 +573,7 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
     constexpr uint32_t kNone = 0xFFFFFFFFu;
     if (!flat || !flat->area || !out || (n_sums && !sums) || (n_ext && !ext) || !borders) return HSPF_E_INVAL;
     *out = nullptr;
-    if (third && (T::kV3 || !config)) return HSPF_E_INVAL;
+    if (third && !config) return HSPF_E_INVAL;
     const bool nb = config != nullptr;                            // a non-backbone target area
     const uint32_t ta = nb ? flat->area->area_id : 0;
     if (nb) {
@@ -738,14 +785,9 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
         t->words.insert(t->words.end(), o3.begin(), o3.end());
         t->words.insert(t->words.end(), o5.begin(), o5.end());
         t->words.resize(t->border_at(), 0);
-        if (third) {
-            for (uint32_t b = 0; b < n_borders; ++b) {
-                const std::array<uint32_t, 4> bw = walk_border_words(*third[b], at[b]);
-                t->words.insert(t->words.end(), bw.begin(), bw.end());
-            }
-        } else if (const int rc2 = append_border_words<T::kV3>(t->words, borders, n_borders, at.data(), nb)) {
+        if (const int rc2 = third ? append_walk_border_words<T::kV3>(t->words, third, n_borders, at.data())
+                                  : append_border_words<T::kV3>(t->words, borders, n_borders, at.data(), nb))
             return rc2;
-        }
         *out = t.release();
         return HSPF_OK;
     } catch (const std::bad_alloc &) {
@@ -755,10 +797,11 @@ int build_backbone_table(const typename T::Flat *flat, uint32_t router_id, const
     }
 }
 
-// hspf_ospfv2_third_area_table_create, argument checks included: an internal router R of a non-backbone area over
-// jobs inside another non-backbone area.  The borders are R's area's ABRs attached to area 0 (C), each an OSPFv2
-// abr_backbone table over the perturbed area's ABRs; the table is build_backbone_table's `config` path over the C's
-// restricted tables, with `third` (chain slots, the walk's border words).
+// hspf_ospfv2_third_area_table_create / hspf_ospfv3_third_area_table_create, argument checks included: an internal
+// router R of a non-backbone area over jobs inside another non-backbone area.  The borders are R's area's ABRs attached
+// to area 0 (C), each an abr_backbone table of R's version over the perturbed area's ABRs (another version's is
+// HSPF_E_INVAL); the table is build_backbone_table's `config` path over the C's restricted tables, with `third` (chain
+// slots, the walk's border words).
 template <class T>
 int build_third_area_table(const typename T::Flat *flat, uint32_t router_id, const hl_ospf_area_config *config,
                            const typename T::Sum *sums, uint32_t n_sums, const typename T::Ext *ext, uint32_t n_ext,
@@ -768,7 +811,7 @@ int build_third_area_table(const typename T::Flat *flat, uint32_t router_id, con
     if (!config || !borders || n_borders == 0 || n_borders > kOspfBackboneMaxBorders) return HSPF_E_INVAL;
     const hspf_ospfv2_abr_ribtable *abr[kOspfBackboneMaxBorders];
     for (uint32_t b = 0; b < n_borders; ++b) {
-        if (!borders[b] || !borders[b]->abr) return HSPF_E_INVAL;
+        if (!borders[b] || !borders[b]->abr || borders[b]->abr->v3 != T::kV3) return HSPF_E_INVAL;
         abr[b] = borders[b]->abr;
     }
     return build_backbone_table<T>(flat, router_id, sums, n_sums, ext, n_ext, abr, n_borders, out, true, config,

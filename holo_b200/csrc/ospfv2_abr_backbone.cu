@@ -151,13 +151,15 @@ abr_asbr_entries_kernel(const AbrEntryArgs<D, N> a, uint32_t n_jobs, uint32_t *_
     }
 }
 
+// Either version's table (v3: the version the call takes): an OSPFv3 table's Inter-Area-Router ranges hold the records
+// of OSPFv2's type-4 ranges, so one instantiation of the kernel serves both.
 template <class R>
 int asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs, const R *planes,
                  const R *const *border_planes, const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
-                 uint32_t *job_status_out, uint32_t *entries) {
+                 uint32_t *job_status_out, uint32_t *entries, bool v3) {
     using P = hspf::PlanesOf<R>;
     using Rows = hspf::ResultPlanes<P>;
-    if (!ctx || !t || !t->abr || t->abr->v3 || !t->dev.blob || !planes) return HSPF_E_INVAL;
+    if (!ctx || !t || !t->abr || t->abr->v3 != v3 || !t->dev.blob || !planes) return HSPF_E_INVAL;
     const uint32_t G = (uint32_t)t->asbr_group.size();
     if ((n_jobs && G && !entries) || (reinterpret_cast<uintptr_t>(entries) & 3u) ||
         (reinterpret_cast<uintptr_t>(job_status_out) & 3u) || (G && !t->entry_dev.blob))
@@ -193,8 +195,8 @@ int hspf_ospfv2_abr_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_abr_backbon
     if (!t || !t->abr) return HSPF_E_INVAL;
     const int rc = hspf::upload_route_table(ctx, t->dev, t->words, t->abr->recs.data(),
                                             t->abr->recs.size() * sizeof(hspf::RibRec));
-    if (rc || t->asbr_group.empty() || t->abr->v3) return rc;
-    // the entry record of each group with type-4 slots, for hspf_ospfv2_abr_backbone_asbr_entries (OSPFv2 only)
+    if (rc || t->asbr_group.empty()) return rc;
+    // the entry record of each group with type-4 slots, for hspf_ospfv{2,3}_abr_backbone_asbr_entries
     std::vector<uint32_t> rec;
     for (uint32_t g : t->asbr_group) rec.push_back(t->abr->ext_end + g * t->abr->n_areas + t->area0);
     return hspf::upload_route_table(ctx, t->entry_dev, rec, nullptr, 0);
@@ -204,14 +206,32 @@ int hspf_ospfv2_abr_backbone_asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_b
                                           const hspf_result *planes, const hspf_result *const *border_planes,
                                           const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                           uint32_t *job_status_out, uint32_t *entries) {
-    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries);
+    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries,
+                        false);
 }
 
 int hspf_ospfv2_abr_backbone_asbr_entries16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
                                             const hspf_result16 *planes, const hspf_result16 *const *border_planes,
                                             const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                             uint32_t *job_status_out, uint32_t *entries) {
-    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries);
+    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries,
+                        false);
+}
+
+int hspf_ospfv3_abr_backbone_asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                          const hspf_result *planes, const hspf_result *const *border_planes,
+                                          const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                          uint32_t *job_status_out, uint32_t *entries) {
+    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries,
+                        true);
+}
+
+int hspf_ospfv3_abr_backbone_asbr_entries16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                            const hspf_result16 *planes, const hspf_result16 *const *border_planes,
+                                            const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                            uint32_t *job_status_out, uint32_t *entries) {
+    return asbr_entries(ctx, t, n_jobs, planes, border_planes, border_n_rows, border_rows, job_status_out, entries,
+                        true);
 }
 
 int hspf_ospfv2_abr_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,

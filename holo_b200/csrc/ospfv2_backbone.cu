@@ -1,9 +1,10 @@
 // Device stage for the routing table of an OSPF backbone router over what-if jobs inside other areas
 // (include/holo_spf_lsdb.h, "backbone router over what-if jobs inside other areas"): update_rib_full at the router,
 // for its affected prefixes, with every border's type-3 / Inter-Area-Prefix LSAs in area 0 re-originated for the job.
-// The entry points serve OSPFv2 and OSPFv3 tables alike, and tables of an internal router of a non-backbone area over
-// jobs on the backbone (hspf_ospfv{2,3}_nonbackbone_table_create): the table's marks (version, target area) pick the
-// walk's instantiation.
+// The entry points serve OSPFv2 and OSPFv3 tables alike, tables of an internal router of a non-backbone area over
+// jobs on the backbone (hspf_ospfv{2,3}_nonbackbone_table_create) and over jobs inside another non-backbone area
+// (hspf_ospfv{2,3}_third_area_table_create): the table's marks (version, target area, third area) pick the walk's
+// instantiation.
 //
 // One launch on the ctx stream: one thread per (job, prefix) runs ospf_backbone_cell_eval (ospf_backbone_cells.h)
 // over the router's unperturbed area-0 planes (row 0) and the job's row of each border's routing-table cells, and
@@ -131,9 +132,24 @@ struct OspfThirdAreaCell : OspfBackboneCell<Planes, false> {
     }
 };
 
+// The walk over an OSPFv3 third-area table (hspf_ospfv3_third_area_table_create), with or without chain slots: the C
+// cells' inter-area winners may be OSPFv3 slot winners, whose options ride in their low byte (kSlotWinners), and R's
+// slot winners carry those options.  A type of its own, so that the kernels above keep their instantiations.
+template <class Planes>
+struct OspfThirdAreaV3Cell : OspfThirdAreaCell<Planes> {
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
+        const hspf::OspfThirdAreaPlanes<Planes> pl{this->pl.job(0), {this->chain, j}};
+        return hspf::ospf_backbone_cell_eval<true, true, true, true>(pl, this->t, p, rows);
+    }
+};
+
 // Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
 // and for OSPFv3 tables, for OSPFv2 and OSPFv3 tables with type-4 / Inter-Area-Router slots, for OSPFv2 and OSPFv3
-// tables of a non-backbone target area, and for third-area tables with chain slots.
+// tables of a non-backbone target area, for OSPFv2 third-area tables with chain slots, and for OSPFv3 third-area
+// tables.
 constexpr uint32_t kBackboneBlocksPerSM = 4;
 constexpr uint32_t kBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kBackboneAsbrBlocksPerSM = 4;
@@ -141,6 +157,7 @@ constexpr uint32_t kBackboneAsbrV3BlocksPerSM = 4;
 constexpr uint32_t kNonBackboneBlocksPerSM = 4;
 constexpr uint32_t kNonBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kThirdAreaBlocksPerSM = 4;
+constexpr uint32_t kThirdAreaV3BlocksPerSM = 4;
 
 template <class R, bool kV3>
 int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
@@ -188,36 +205,50 @@ int nonbackbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_j
                        ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out);
 }
 
-// A third-area table: with chain slots the OspfThirdAreaCell walk over each border's entries (border_entries[b] u32
-// [n_jobs][G_b], NULL allowed for a border with no group and for a table without chain slots), else the plain
-// kNonBackbone walk.
-template <class R, class Out>
-int third_area(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-               const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-               const uint32_t *const *border_entries, const uint32_t *const *border_entry_status, const Out &out) {
-    if (!t || !t->third_area) return HSPF_E_INVAL;
-    if (!t->n_asbr_slots)
-        return nonbackbone<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr, out);
-    OspfThirdAreaCell<hspf::PlanesOf<R>> cell{};
+// The launch of a third-area walk (Cell) over each border's entries (border_entries[b] u32 [n_jobs][G_b], NULL allowed
+// for a border with no group; the array may be NULL for a table without chain slots, which reads no entries).
+template <class Cell, uint32_t kBlocks, class R, class Out>
+int chain_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+             const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+             const uint32_t *const *border_entries, const uint32_t *const *border_entry_status, const Out &out) {
+    Cell cell{};
     if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    if (!border_entries) return HSPF_E_INVAL;
+    if (t->n_asbr_slots && !border_entries) return HSPF_E_INVAL;
     for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
         cell.chain.entries[b] = nullptr; cell.chain.status[b] = nullptr; cell.chain.G[b] = 0;
-        if (b >= t->n_borders) continue;
+        if (b >= t->n_borders || !t->n_asbr_slots) continue;
         cell.chain.G[b] = (uint32_t)t->third[b]->asbr_group.size();
         cell.chain.entries[b] = border_entries[b];
         cell.chain.status[b] = border_entry_status ? border_entry_status[b] : nullptr;
         if (cell.chain.G[b] && (!border_entries[b] || (reinterpret_cast<uintptr_t>(border_entries[b]) & 3u)))
             return HSPF_E_INVAL;
     }
-    return hspf::launch_route_stage<kThirdAreaBlocksPerSM>(ctx, t->dev, cell, n_jobs, t->P(), out);
+    return hspf::launch_route_stage<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
+}
+
+// A third-area table.  OSPFv2: with chain slots the OspfThirdAreaCell walk, else the plain kNonBackbone walk.  OSPFv3:
+// the OspfThirdAreaV3Cell walk, with or without chain slots (the kNonBackbone walks cannot read C's slot winners).
+template <class R, class Out>
+int third_area(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+               const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
+               const uint32_t *const *border_entries, const uint32_t *const *border_entry_status, const Out &out) {
+    if (!t || !t->third_area) return HSPF_E_INVAL;
+    using P = hspf::PlanesOf<R>;
+    if (t->v3)
+        return chain_as<OspfThirdAreaV3Cell<P>, kThirdAreaV3BlocksPerSM>(
+            ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status, out);
+    if (!t->n_asbr_slots)
+        return nonbackbone<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr, out);
+    return chain_as<OspfThirdAreaCell<P>, kThirdAreaBlocksPerSM>(ctx, t, n_jobs, planes, border_cells, border_status,
+                                                                 border_entries, border_entry_status, out);
 }
 
 // the walk of the table's version and target area; a table with type-4 slots is backbone_asbr's
 template <class R, class Out>
 int backbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
              const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status, const Out &out) {
-    if (!t || t->n_asbr_slots) return HSPF_E_INVAL;
+    // an OSPFv3 third-area table's C cells hold slot winners, which only the third-area calls read
+    if (!t || t->n_asbr_slots || (t->third_area && t->v3)) return HSPF_E_INVAL;
     if (t->area_id)
         return nonbackbone<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr, out);
     return t->v3 ? version<true>(ctx, t, n_jobs, planes, border_cells, border_status, out)
@@ -231,8 +262,10 @@ int backbone_asbr(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n
                   const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
                   const R *const *border_planes, const uint32_t *const *border_n_rows,
                   const uint32_t *const *border_rows, const Out &out) {
-    // a third-area table's type-4 slots are chain slots, which only the third-area calls read
-    if (!t || (t->v3 && !t->area_id && !t->asbr) || (t->third_area && t->n_asbr_slots)) return HSPF_E_INVAL;
+    // a third-area table's type-4 slots are chain slots, and an OSPFv3 one's C cells hold slot winners: only the
+    // third-area calls read those
+    if (!t || (t->v3 && !t->area_id && !t->asbr) || (t->third_area && (t->n_asbr_slots || t->v3)))
+        return HSPF_E_INVAL;
     if (t->area_id)
         return nonbackbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
                            border_rows, out);

@@ -925,6 +925,15 @@ int hspf_ospfv3_nonbackbone_table_create(const hspf_ospfv3_flat *flat, uint32_t 
                                              config);
 }
 
+int hspf_ospfv3_third_area_table_create(const hspf_ospfv3_flat *flat, uint32_t router_id,
+                                        const hl_ospf_area_config *config, const hl_ospfv3_inter_area_lsa *sums,
+                                        uint32_t n_sums, const hl_ospfv3_external_lsa *ext, uint32_t n_ext,
+                                        const hspf_ospfv2_abr_backbone_table *const *borders, uint32_t n_borders,
+                                        hspf_ospfv2_backbone_table **out) {
+    return hspf::build_third_area_table<RibV3>(flat, router_id, config, sums, n_sums, ext, n_ext, borders, n_borders,
+                                               out);
+}
+
 int hspf_ospfv3_backbone_table_prefixes6(const hspf_ospfv2_backbone_table *t, uint32_t *n_prefixes,
                                          const hl_ip_addr **prefixes, const uint32_t **lens) {
     if (!t || !t->v3) return HSPF_E_INVAL;

@@ -664,7 +664,10 @@ class BackboneTable:
     internal router R of a non-backbone area over what-if jobs inside another non-backbone area; the borders are R's
     area's ABRs attached to area 0, each over the perturbed area's ABRs.  `third_area` is set; `n_asbr_slots` are chain
     slots, which read the borders' abr_backbone_asbr_entries_device output through third_area_cells_device /
-    third_area_delta_device; a table without them also runs through the backbone calls."""
+    third_area_delta_device; a table without them also runs through the backbone calls.  From an ospfv3.Flat with
+    OSPFv3 AbrBackboneTable borders: hspf_ospfv3_third_area_table_create, whose cells only the third-area calls read
+    (its borders' cells hold OSPFv3 slot winners); backbone_from_cells_v3 decodes it.  A flat and borders of different
+    versions raise ValueError (a list that mixes versions is refused by the create, HSPF_E_INVAL)."""
 
     def __init__(self, flat, router_id: int, summaries=None, externals=None, borders=(), asbr: bool = False,
                  config=None):
@@ -684,7 +687,10 @@ class BackboneTable:
         self.third_area = bool(self.borders) and all(isinstance(b, AbrBackboneTable) for b in self.borders)
         if not self.third_area and any(isinstance(b, AbrBackboneTable) for b in self.borders):
             raise ValueError("borders are all AbrBackboneTables (a third-area table) or none is")
-        create = ("hspf_ospfv2_third_area_table_create" if self.third_area else
+        if self.third_area and all(b.v3 != self.v3 for b in self.borders):
+            raise ValueError("a third-area table's flat and borders are of one OSPF version")
+        create = ("hspf_ospfv3_third_area_table_create" if self.third_area and self.v3 else
+                  "hspf_ospfv2_third_area_table_create" if self.third_area else
                   "hspf_ospfv3_nonbackbone_table_create" if self.v3 and config is not None else
                   "hspf_ospfv3_backbone_asbr_table_create" if self.v3 and asbr else
                   "hspf_ospfv3_backbone_table_create" if self.v3 else
@@ -935,18 +941,21 @@ def abr_backbone_delta_device(ctx: capi.Context, t: AbrBackboneTable, n_jobs: in
 
 def abr_backbone_asbr_entries_device(ctx: capi.Context, t: AbrBackboneTable, n_jobs: int, planes: list, border_planes,
                                      border_n_rows, border_rows, status_ptr: int, entries_ptr: int):
-    """hspf_ospfv2_abr_backbone_asbr_entries / _entries16: per job and per ASBR of t.asbr_ids, the metric of the type-4
-    LSA the router originates for it into a normal area other than area 0 (0xFFFFFFFF: none), into device u32
-    [n_jobs, len(t.asbr_ids)] at entries_ptr.  planes / border_* as abr_backbone_cells_device."""
+    """hspf_ospfv2_abr_backbone_asbr_entries / _entries16 (an OSPFv3 table: hspf_ospfv3_abr_backbone_asbr_entries /
+    _entries16): per job and per ASBR of t.asbr_ids, the metric of the type-4 / Inter-Area-Router LSA the router
+    originates for it into a normal area other than area 0 (0xFFFFFFFF: none), into device u32 [n_jobs,
+    len(t.asbr_ids)] at entries_ptr.  planes / border_* as abr_backbone_cells_device."""
     keep = []
     bp, bn, br = _border_plane_args(border_planes, border_n_rows, border_rows, keep)
-    route_table.call_stage(ctx, "hspf_ospfv2_abr_backbone_asbr_entries", planes[0], t.handle, n_jobs,
+    name = "hspf_ospfv3_abr_backbone_asbr_entries" if t.v3 else "hspf_ospfv2_abr_backbone_asbr_entries"
+    route_table.call_stage(ctx, name, planes[0], t.handle, n_jobs,
                            _planes_array(planes), bp, bn, br, status_ptr or None, entries_ptr or None)
 
 
 def third_area_cells_device(ctx: capi.Context, t: BackboneTable, n_jobs: int, rs, border_cells, border_status,
                             border_entries, border_entry_status, status_ptr: int, cells_ptr: int):
-    """hspf_ospfv2_third_area_cells / _cells16: backbone_cells_device's arguments over a third-area table, plus per
+    """hspf_ospfv2_third_area_cells / _cells16: backbone_cells_device's arguments over a third-area table (either
+    version; the table's mark picks the walk), plus per
     border a device pointer to its [n_jobs, G_b] entries (0 allowed without chain slots; None: NULL) and per border
     the entries call's device u32 [n_jobs] status words or 0 (None: none)."""
     be = _device_ptrs(border_entries) if border_entries is not None else None

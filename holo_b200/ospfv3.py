@@ -985,3 +985,94 @@ def nonbackbone_lsas(router_id: int, max_paths: int, rib_areas: list, externals,
     rows = [tuple(z) for z in ospf_rib.net_summaries_v3(router_id, rib, rib_areas, cfg, target).tolist()]
     rows += [tuple(z) for z in ospf_rib.rtr_summaries_v3(router_id, rib_areas, cfg, target).tolist()]
     return [(z[0], k + 1) + tuple(z[2:]) for k, z in enumerate(rows)]
+
+
+def third_area_view(t0: Topology, t1: Topology, t3: Topology, seed: int, spf, n_c: int = 2, max_paths: int = 16,
+                    n_ext_keys: int = 3, area1_asbrs: int = 0, area1_ext: int = 4):
+    """The OSPFv3 twin of ospfv2.third_area_view: an internal router R of a non-backbone area, the area border routers
+    C of that area and area 0 (n_c of them, 2 or 3), and the borders B of area 1, each as its own image.  Areas 0 and 1
+    are backbone_view's (its three B's, the first also in area 2, the area-0 ASBR, area1_asbrs area-1 ASBRs with their
+    AS-external and Inter-Area-Router LSAs); R's area is area 3, synth_area(t3) in ranges of its own, whose routers
+    0 .. n_c - 1 are the C's (routers 0, then the first routers of t0 past the borders that are not the area-0 ASBR; the
+    B flag in areas 0 and 3) and whose router n_c is R.  Area 3 also holds an ASBR ("area3_asbr", the E flag) with a
+    /64 of its own, and a router that also advertises a prefix the B's advertise into area 0 ("area3_shared").  Seeded;
+    area 3 draws from a generator of its own, so that every other generator's output stays as it was.
+    `spf(csr, root_vertex, nh_words)` gives unperturbed planes, as area_from_planes takes them.  Returns a dict:
+      r_area        R's area-3 image;
+      summaries3    area 3's Inter-Area-Prefix / Inter-Area-Router LSAs (LsaKey order): each C's
+                    hspf_ospfv3_net_summaries and hspf_ospfv3_rtr_summaries into area 3 over its update_rib_full at the
+                    unperturbed job (nonbackbone_lsas);
+      externals     backbone_view's plus the area-3 ASBR's;
+      c_areas       per C (areas [area 0, area 3], area ids [0, 3], summaries per area: area 0's, none for area 3);
+      borders       per B as backbone_view's (the C's have the B flag in its area-0 image);
+      asbr, area1_asbrs, area3_asbr, area3_shared, flip, flip_ext, shared."""
+    from . import ospf_rib
+    from .ospfv2 import _dist_from
+    if n_c not in (2, 3):
+        raise ValueError("n_c is 2 or 3")
+    v = backbone_view(t0, t1, seed, r=0, max_paths=max_paths, n_ext_keys=n_ext_keys, area1_asbrs=area1_asbrs,
+                      area1_ext=area1_ext)
+    rng = np.random.default_rng([seed, 0xC3B])
+    six = lambda hi, lo=0: ipaddress.IPv6Address((0x20010DB8 << 96) | (hi << 64) | lo).packed
+    rec = lambda b: (tuple(b), 1, (0, 0, 0))
+    c0 = [0] + [i for i in range(4, t0.n_routers) if RID_BASE + i != v["asbr"]][:n_c - 1]
+    cids = [RID_BASE + i for i in c0]
+
+    def with_flags(a, bits):
+        a = Ospfv3Area(**{k: getattr(a, k) for k in a.__dataclass_fields__})
+        rl = a.router_lsas.copy()
+        for x, b in bits.items():
+            rl["flags"][rl["adv_rtr"] == x] |= b
+        a.router_lsas = rl
+        return a
+
+    cflag = {c: 0x01 for c in cids}
+
+    def img3(i):
+        rids = [cids[k] if k < n_c else RID_BASE + k + (3 << 20) for k in range(t3.n_routers)]
+        a = synth_area(t3, root=i, max_paths=max_paths, rids=rids, area_id=3)
+        pb = a.prefixes["addr"]["bytes"]
+        pb[:, 5] = pb[:, 5] + 3
+        a.prefixes["addr"]["bytes"] = pb
+        ifs = a.ifaces.copy()
+        ifs["sort_key"] += 3000
+        ifs["ifindex"] += 3000
+        a.ifaces = ifs
+        return with_flags(a, cflag)
+
+    ra = img3(n_c)
+    fl = Flat(ra)
+    d = _dist_from(fl, fl.router_vertex(ra.router_id))
+    reach = sorted(int(fl.router_ids[x]) for x in range(len(fl.router_ids))
+                   if fl.is_router[x] and 0 < d[x] < 1 << 40 and int(fl.router_ids[x]) not in cids)
+    t3s = v["summaries0"][v["summaries0"]["lsa_type"] == 3]
+    pick = t3s[int(rng.integers(0, len(t3s)))]
+    shared3 = (bytes(int(b) for b in pick["prefix"]["bytes"]), int(pick["len"]))
+    adds = {reach[int(rng.integers(0, len(reach)))]: [(shared3[0], shared3[1], 0, 1)]}
+    asbr3 = reach[int(rng.integers(0, len(reach)))]
+    area3 = lambda i: with_flags(_with_prefixes(img3(i), adds), {asbr3: 0x02})
+    own3 = (six(0xE3_0000), 64)
+    ext = [tuple(x) for x in v["externals"].tolist()]
+    ext += [(asbr3, 1, int(rng.integers(1, 40)), 12, rec(own3[0]), 64, PFX_P, 0, 0)]
+    externals = _lsa_array(sorted(ext, key=lambda x: (x[0], x[1])), ospf_rib.EXTERNAL6_LSA_DT)
+    bits0 = dict(cflag)
+    bits0.update({RID_BASE + int(i0): 0x01 for i0 in (1, 2, 3)})
+    bits0[v["asbr"]] = 0x02
+
+    def area0(i):
+        return with_flags(v["r_area"], cflag) if i == 0 else \
+            with_flags(synth_area(t0, root=i, max_paths=max_paths, area_id=0), bits0)
+    empty = np.zeros(0, ospf_rib.INTER_AREA_LSA_DT)
+    c_areas = [([area0(i), area3(k)], [0, 3], [v["summaries0"], empty]) for k, i in enumerate(c0)]
+    sums = []
+    for areas, ids, csums in c_areas:
+        rib_areas = [ospf_rib.RibArea(a.area_id, area_from_planes(a, spf), a.ifaces, s, True)
+                     for a, s in zip(areas, csums)]
+        sums += nonbackbone_lsas(areas[0].router_id, max_paths, rib_areas, externals, 1)
+    borders = [([with_flags(a, cflag) if a.area_id == 0 else a for a in areas], ids, bs)
+               for areas, ids, bs in v["borders"]]
+    return {"r_area": area3(n_c), "summaries3": _lsa_array(sorted(sums, key=lambda z: (z[7], z[0], z[1])),
+                                                           ospf_rib.INTER_AREA_LSA_DT),
+            "externals": externals, "c_areas": c_areas, "borders": borders, "asbr": v["asbr"],
+            "area1_asbrs": v.get("area1_asbrs", []), "area3_asbr": asbr3, "area3_shared": shared3,
+            "flip": v["flip"], "flip_ext": v.get("flip_ext"), "shared": v["shared"]}

@@ -201,6 +201,9 @@ def declare(lib: C.CDLL):
         "hspf_ospfv3_backbone_table_create": [vp, u32, vp, u32, vp, u32, pvp, u32, pvp],
         "hspf_ospfv3_backbone_asbr_table_create": [vp, u32, vp, u32, vp, u32, pvp, u32, pvp],
         "hspf_ospfv3_nonbackbone_table_create": [vp, u32, vp, vp, u32, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv3_third_area_table_create": [vp, u32, vp, vp, u32, vp, u32, pvp, u32, pvp],
+        "hspf_ospfv3_abr_backbone_asbr_entries": [vp, vp, u32, vp, pvp, pvp, pvp, vp, vp],
+        "hspf_ospfv3_abr_backbone_asbr_entries16": [vp, vp, u32, vp, pvp, pvp, pvp, vp, vp],
         "hspf_ospfv3_backbone_table_prefixes6": [vp, u32p, pvp, C.POINTER(u32p)],
         "hspf_ospfv3_backbone_from_cells": [vp, C.POINTER(ospfv3.AreaStruct), vp, vp, vp, u32,
                                             C.POINTER(ospf_rib.RibStruct)],

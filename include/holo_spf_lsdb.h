@@ -619,9 +619,10 @@ int hspf_ospfv2_abr_backbone_from_cells(const hspf_ospfv2_abr_backbone_table *t,
  *                                target a normal area other than area 0) over C's routing table of the job.
  *                                job_status_out (device u32[n_jobs], may be NULL): the OR of C's row-0 words and the
  *                                words of the type-4 rows the job reads, HSPF_JS_INVALID for a row out of range; a job
- *                                with a non-zero word gets 0xFFFFFFFF entries.  HSPF_E_INVAL: an OSPFv3 table, a table
- *                                not uploaded, entries or job_status_out not 4-byte aligned.  Nothing is launched for
- *                                0 jobs.  Enqueued on the ctx stream.
+ *                                with a non-zero word gets 0xFFFFFFFF entries.  HSPF_E_INVAL: an OSPFv3 table
+ *                                (hspf_ospfv3_abr_backbone_asbr_entries[16] takes those), a table not uploaded,
+ *                                entries or job_status_out not 4-byte aligned.  Nothing is launched for 0 jobs.
+ *                                Enqueued on the ctx stream.
  */
 int hspf_ospfv2_abr_backbone_table_asbrs(const hspf_ospfv2_abr_backbone_table *t, uint32_t *n_groups,
                                          const uint32_t **asbr_ids);
@@ -820,6 +821,63 @@ int hspf_ospfv3_nonbackbone_table_create(const struct hspf_ospfv3_flat *flat, ui
                                          const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
                                          const hspf_ospfv2_abr_ribtable *const *borders, uint32_t n_borders,
                                          hspf_ospfv2_backbone_table **out);
+
+/*
+ * Non-backbone router over what-if jobs inside another non-backbone area, OSPFv3: the
+ * hspf_ospfv2_third_area_table_create stage over Inter-Area-Prefix / Inter-Area-Router LSAs, with the same contract on
+ * jobs, borders (the C's, each an hspf_ospfv3_abr_backbone_table_create table over A1's ABRs) and affected prefixes.
+ * For job j, with C's cells of j (hspf_ospfv2_abr_backbone_cells[16] over its OSPFv3 table) decoded to rib_C
+ * (hspf_ospfv3_abr_backbone_from_cells), the decoded cells of j equal the affected-prefix routes, prefix options
+ * included, of
+ *     hspf_ospfv3_update_rib_full(R, max_paths, [{A2, area_from_planes(A2, R's row 0), ifaces, S_j, 1}], X)
+ * where S_j is A2's Inter-Area-Prefix / Inter-Area-Router LSAs with each C's replaced by
+ * hspf_ospfv3_net_summaries(rib_C, areas_C, target A2) and hspf_ospfv3_rtr_summaries(areas_C, target A2), in LsaKey
+ * order; that is the three-step host chain: each B's update_rib_full, net and rtr summaries into area 0 spliced into
+ * C's area 0; each C's same chain over those LSAs into A2; update_rib_full at R.  A C's Inter-Area-Prefix LSA carries
+ * the prefix options of C's route: those of its winning intra-area record or Inter-Area-Prefix record, and for a route
+ * through a B's slot those the B copied from its own route, which C's cell winner carries (n_recs_C + (slot << 8 |
+ * options)).  R's slot winner is n_records + (slot index << 8 | those options), so a B route that changes record at an
+ * equal metric, to one with other options, changes R's winner through C, and the route-delta stage reports OTHER.  When
+ * A1 holds an ASBR A, each C's Inter-Area-Router LSA for A into a normal A2 is a chain slot, as for OSPFv2, reading C's
+ * entries of the job (hspf_ospfv3_abr_backbone_asbr_entries[16]).  The options of an Inter-Area-Router LSA are outside
+ * the contract, as they are for hspf_ospfv3_rtr_summaries.
+ *
+ *   hspf_ospfv3_third_area_table_create  host.  The arguments of hspf_ospfv2_third_area_table_create over OSPFv3: R's
+ *                                area-A2 flat, A2's configuration, A2's Inter-Area-Prefix / Inter-Area-Router LSAs in
+ *                                LsaKey order, the AS-external LSAs, and the C's OSPFv3 abr_backbone tables, which must
+ *                                outlive the table.  The result is an hspf_ospfv2_backbone_table marked OSPFv3 and as a
+ *                                third-area table: hspf_ospfv2_backbone_table_* (asbr_slots: the chain slot count and 0
+ *                                plane sets), _upload, hspf_ospfv3_backbone_table_prefixes6 and
+ *                                hspf_ospfv3_backbone_from_cells take it (an external route reached through a chain
+ *                                slot decodes as any external route).  Refusals: those of the OSPFv2 call, with an
+ *                                OSPFv2 border table HSPF_E_INVAL (and the OSPFv2 call refuses an OSPFv3 one) and slot
+ *                                winners that would not fit 32 bits (n_records + (slots << 8)) HSPF_E_UNSUPPORTED.
+ *                                Inter-Area-Prefix LSAs with the NU option are left out.
+ *   hspf_ospfv2_third_area_cells[16] / _delta[16]  take it; its version mark picks the walk, which reads C's slot
+ *                                winners, with or without chain slots.  The status-word rule is the OSPFv2 one: a job's
+ *                                word ORs R's row-0 word, each C's cell status and entries status, and a job with a
+ *                                non-zero word gets empty cells.  hspf_ospfv2_backbone[_asbr]_cells[16] / _delta[16]
+ *                                refuse an OSPFv3 third-area table, with or without chain slots (HSPF_E_INVAL), before
+ *                                any launch: their walks cannot read C's slot winners.
+ *   hspf_ospfv3_abr_backbone_asbr_entries[16]  hspf_ospfv2_abr_backbone_asbr_entries[16] over an OSPFv3 C table (the
+ *                                Inter-Area-Router rows of hspf_ospfv3_rtr_summaries(areas_C, target a normal area
+ *                                other than area 0) over C's areas of the job); hspf_ospfv2_abr_backbone_table_asbrs
+ *                                names its groups.  HSPF_E_INVAL: an OSPFv2 table, and the OSPFv2 call's refusals.
+ */
+int hspf_ospfv3_third_area_table_create(const struct hspf_ospfv3_flat *flat, uint32_t router_id,
+                                        const struct hl_ospf_area_config *config,
+                                        const hl_ospfv3_inter_area_lsa *summaries, uint32_t n_summaries,
+                                        const hl_ospfv3_external_lsa *externals, uint32_t n_externals,
+                                        const hspf_ospfv2_abr_backbone_table *const *borders, uint32_t n_borders,
+                                        hspf_ospfv2_backbone_table **out);
+int hspf_ospfv3_abr_backbone_asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                          const hspf_result *planes, const hspf_result *const *border_planes,
+                                          const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                          uint32_t *job_status_out, uint32_t *entries);
+int hspf_ospfv3_abr_backbone_asbr_entries16(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_t n_jobs,
+                                            const hspf_result16 *planes, const hspf_result16 *const *border_planes,
+                                            const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
+                                            uint32_t *job_status_out, uint32_t *entries);
 
 /*
  * Area border router over what-if jobs inside an area it is not attached to, OSPFv3: the
