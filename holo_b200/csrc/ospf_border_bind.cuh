@@ -1,5 +1,6 @@
 // Host set-up shared by the OSPF backbone stages (ospfv2_backbone.cu, ospfv2_abr_backbone.cu): binding the
-// borders' routing-table cells and the plane sets of the type-4 slots into a stage's cell functor.  nvcc only.
+// borders' routing-table cells and the plane sets of the type-4 slots into a stage's cell functor, and an area border
+// router's row-0 planes of every area.  nvcc only.
 #pragma once
 #include "../../include/holo_spf_lsdb.h"
 #include "ospf_backbone_cells.h"
@@ -41,6 +42,18 @@ int bind_ospf_asbr_sets(const Table &t, const R *const *border_planes, const uin
         s.dist[k] = p.dist; s.status[k] = p.status; s.V[k] = p.V;
         s.rows[k] = border_rows[b]; s.n_rows[k] = border_n_rows[b][i];
         s.stride[k] = t.borders[b]->n_areas; s.area[k] = i;
+    }
+    return HSPF_OK;
+}
+
+// An area border router's planes of each area (planes[i], a.n_vertices[i] vertices) into s, one row each (row 0).
+template <class AbrTable, class R, class D, class N>
+int bind_abr_row0_planes(const AbrTable &a, const R *planes, AbrPlaneSet<D, N> &s) {
+    for (uint32_t i = 0; i < a.n_areas; ++i) {
+        ResultPlanes<PlanesOf<R>> p;
+        if (result_planes(&planes[i], a.n_vertices[i], p) || !p.complete()) return HSPF_E_INVAL;
+        s.dist[i] = p.dist; s.hops[i] = p.hops; s.nh[i] = p.nh; s.status[i] = p.status;
+        s.V[i] = p.V; s.n_rows[i] = 1;
     }
     return HSPF_OK;
 }

@@ -73,13 +73,7 @@ int make_cell(const hspf_ospfv2_abr_backbone_table *t, const R *planes, const hl
               const uint32_t *const *border_status, const R *const *border_planes, const uint32_t *const *border_n_rows,
               const uint32_t *const *border_rows, uint32_t n_jobs, Cell &cell) {
     if (!t || !t->abr || !t->dev.blob || !planes || !border_cells) return HSPF_E_INVAL;
-    const hspf_ospfv2_abr_ribtable &a = *t->abr;
-    for (uint32_t i = 0; i < a.n_areas; ++i) {
-        typename Cell::Rows p;
-        if (hspf::result_planes(&planes[i], a.n_vertices[i], p) || !p.complete()) return HSPF_E_INVAL;
-        cell.s.dist[i] = p.dist; cell.s.hops[i] = p.hops; cell.s.nh[i] = p.nh; cell.s.status[i] = p.status;
-        cell.s.V[i] = p.V; cell.s.n_rows[i] = 1;
-    }
+    if (const int rc = hspf::bind_abr_row0_planes(*t->abr, planes, cell.s)) return rc;
     if (const int rc = hspf::bind_ospf_borders(*t, border_cells, border_status, cell)) return rc;
     if (const int rc = hspf::bind_ospf_asbr_sets(*t, border_planes, border_n_rows, border_rows, n_jobs, cell))
         return rc;
@@ -164,18 +158,12 @@ int asbr_entries(hspf_ctx *ctx, const hspf_ospfv2_abr_backbone_table *t, uint32_
     if ((n_jobs && G && !entries) || (reinterpret_cast<uintptr_t>(entries) & 3u) ||
         (reinterpret_cast<uintptr_t>(job_status_out) & 3u) || (G && !t->entry_dev.blob))
         return HSPF_E_INVAL;
-    const hspf_ospfv2_abr_ribtable &a = *t->abr;
     AbrEntryArgs<typename Rows::D, typename Rows::N> args{};
-    for (uint32_t i = 0; i < a.n_areas; ++i) {
-        Rows p;
-        if (hspf::result_planes(&planes[i], a.n_vertices[i], p) || !p.complete()) return HSPF_E_INVAL;
-        args.s.dist[i] = p.dist; args.s.hops[i] = p.hops; args.s.nh[i] = p.nh; args.s.status[i] = p.status;
-        args.s.V[i] = p.V; args.s.n_rows[i] = 1;
-    }
+    if (const int rc = hspf::bind_abr_row0_planes(*t->abr, planes, args.s)) return rc;
     if (const int rc = hspf::bind_ospf_asbr_sets(*t, border_planes, border_n_rows, border_rows, n_jobs, args)) return rc;
     args.recs = static_cast<const hspf::RibRec *>(t->dev.contribs);
     args.group_rec = t->entry_dev.off;
-    args.n_areas = a.n_areas; args.area0 = t->area0; args.G = G;
+    args.n_areas = t->abr->n_areas; args.area0 = t->area0; args.G = G;
     const uint64_t items = std::max<uint64_t>((uint64_t)n_jobs * G, job_status_out ? n_jobs : 0u);
     if (items == 0) return HSPF_OK;
     uint32_t blocks = 0;

@@ -3,8 +3,8 @@
 // for its affected prefixes, with every border's type-3 / Inter-Area-Prefix LSAs in area 0 re-originated for the job.
 // The entry points serve OSPFv2 and OSPFv3 tables alike, tables of an internal router of a non-backbone area over
 // jobs on the backbone (hspf_ospfv{2,3}_nonbackbone_table_create) and over jobs inside another non-backbone area
-// (hspf_ospfv{2,3}_third_area_table_create): the table's marks (version, target area, third area) pick the walk's
-// instantiation.
+// (hspf_ospfv{2,3}_third_area_table_create): the call's family and the table's marks (version, target area, slots,
+// third area) pick the walk (pick_walk).
 //
 // One launch on the ctx stream: one thread per (job, prefix) runs ospf_backbone_cell_eval (ospf_backbone_cells.h)
 // over the router's unperturbed area-0 planes (row 0) and the job's row of each border's routing-table cells, and
@@ -21,135 +21,87 @@ namespace {
 
 using hspf::kOspfBackboneMaxBorders;
 
-template <class Planes, bool kV3>
-struct OspfBackboneCell {
-    using Rows = hspf::ResultPlanes<Planes>;
+// What every walk reads: R's area-0 planes and each border's routing-table cells.
+template <class Planes>
+struct OspfBackboneCore {
     hspf::OspfBackboneView t;
-    Rows pl;                                                      // R's area-0 batch; only row 0 is read
+    hspf::ResultPlanes<Planes> pl;                                // R's area-0 batch; only row 0 is read
     const hl_ospf_rib_cell *cells[kOspfBackboneMaxBorders];       // [n_jobs][K_b] per border
     const uint32_t *status[kOspfBackboneMaxBorders];              // [n_jobs] per border, or NULL
     uint32_t K[kOspfBackboneMaxBorders];
     uint32_t n_borders;
-    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
-        uint32_t s = pl.status_word(0);
-        for (uint32_t b = 0; b < n_borders; ++b)
-            if (status[b]) s |= status[b][j];
+};
+
+// A call's arguments for a side input, NULL where its family takes none: the asbr calls' plane sets per border
+// (border_planes[b][i], border_n_rows[b][i], border_rows[b]) and the third-area calls' entries per border
+// (border_entries[b] u32 [n_jobs][G_b], border_entry_status[b] [n_jobs]).
+template <class R>
+struct SideArgs {
+    const R *const *border_planes;
+    const uint32_t *const *border_n_rows, *const *border_rows;
+    const uint32_t *const *border_entries, *const *border_entry_status;
+};
+
+// A walk's side input: what rides with R's planes of the job into ospf_backbone_cell_eval, and what it ORs into the
+// job's status word after the borders' words.  The plain walks have none.
+template <class Planes>
+struct NoSide {
+    template <class R>
+    int bind(const hspf_ospfv2_backbone_table &, const SideArgs<R> &, uint32_t) { return HSPF_OK; }
+    __device__ __forceinline__ uint32_t or_status(const OspfBackboneCore<Planes> &, uint32_t s, uint32_t) const {
         return s;
     }
-    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
-    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::OspfBorderRows rows;
-#pragma unroll
-        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = cells[b] + (size_t)j * K[b];
-        return hspf::ospf_backbone_cell_eval<kV3>(pl.job(0), t, p, rows);
-    }
-    __device__ __forceinline__ uint64_t gather(uint32_t, uint32_t, uint32_t) const { return 0; }   // row 0: host side
-    __device__ static hspf::CellWords empty() { return {0, 0, hspf::kNoRecord}; }
+    __device__ __forceinline__ Planes planes(const Planes &pl, uint32_t) const { return pl; }
 };
 
-// The walk over a table with type-4 slots (hspf_ospfv2_backbone_asbr_table_create): the same, plus the plane sets the
-// slots read, whose rows enter the job's status word.
+// The plane sets the type-4 / Inter-Area-Router slots read; the job's row of each enters its status word.
 template <class Planes>
-struct OspfBackboneAsbrCell : OspfBackboneCell<Planes, false> {
-    using Base = OspfBackboneCell<Planes, false>;
-    hspf::OspfAsbrSets<typename Base::Rows::D> sets;
-    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
-        return Base::status_word(j) | hspf::asbr_job_status(sets, j);
+struct AsbrSide {
+    using D = typename hspf::ResultPlanes<Planes>::D;
+    hspf::OspfAsbrSets<D> sets;
+    template <class R>
+    int bind(const hspf_ospfv2_backbone_table &t, const SideArgs<R> &a, uint32_t n_jobs) {
+        return hspf::bind_ospf_asbr_sets(t, a.border_planes, a.border_n_rows, a.border_rows, n_jobs, *this);
     }
-    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
-    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::OspfBorderRows rows;
-#pragma unroll
-        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
-        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {sets, j}};
-        return hspf::ospf_backbone_cell_eval<false, true>(pl, this->t, p, rows);
+    __device__ __forceinline__ uint32_t or_status(const OspfBackboneCore<Planes> &, uint32_t s, uint32_t j) const {
+        return s | hspf::asbr_job_status(sets, j);
+    }
+    __device__ __forceinline__ hspf::OspfAsbrPlanes<Planes, D> planes(const Planes &pl, uint32_t j) const {
+        return {pl, {sets, j}};
     }
 };
 
-// The walk over a table whose target area is not area 0 (hspf_ospfv2_nonbackbone_table_create), with or without
-// type-4 slots (the cells and delta calls of both kinds take it): the borders also advertise their inter-area routes, and a plane set may be a border's area 0.
+// Each border's entries of the job, which its chain slots read (a third-area table); their status words enter the
+// job's.  A border with no group may have NULL entries, and a table without chain slots reads none (the array may be
+// NULL).
 template <class Planes>
-struct OspfNonBackboneCell : OspfBackboneAsbrCell<Planes> {
-    using Base = OspfBackboneCell<Planes, false>;
-    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::OspfBorderRows rows;
-#pragma unroll
-        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
-        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {this->sets, j}};
-        return hspf::ospf_backbone_cell_eval<false, true, true>(pl, this->t, p, rows);
-    }
-};
-
-// The same over an OSPFv3 table (hspf_ospfv3_nonbackbone_table_create): slot winners carry prefix options, and a
-// plane set is a border's area 0 read for an Inter-Area-Router slot.  A type of its own, so that the OSPFv2 kernels
-// above keep their instantiations.
-template <class Planes>
-struct OspfNonBackboneV3Cell : OspfBackboneAsbrCell<Planes> {
-    using Base = OspfBackboneCell<Planes, false>;
-    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::OspfBorderRows rows;
-#pragma unroll
-        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
-        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {this->sets, j}};
-        return hspf::ospf_backbone_cell_eval<true, true, true>(pl, this->t, p, rows);
-    }
-};
-
-// The walk over an OSPFv3 table of area 0 with Inter-Area-Router slots (hspf_ospfv3_backbone_asbr_table_create): slot
-// winners carry prefix options.  A type of its own, so that the kernels above keep their instantiations.
-template <class Planes>
-struct OspfBackboneAsbrV3Cell : OspfBackboneAsbrCell<Planes> {
-    using Base = OspfBackboneCell<Planes, false>;
-    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::OspfBorderRows rows;
-#pragma unroll
-        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
-        const hspf::OspfAsbrPlanes<Planes, typename Base::Rows::D> pl{this->pl.job(0), {this->sets, j}};
-        return hspf::ospf_backbone_cell_eval<true, true, false>(pl, this->t, p, rows);
-    }
-};
-
-// The walk over a third-area table with chain slots (hspf_ospfv2_third_area_table_create): the kNonBackbone walk, with
-// each chain slot reading its border's entries of the job, whose status words enter the job's.  A type of its own, so
-// that the kernels above keep their instantiations.
-template <class Planes>
-struct OspfThirdAreaCell : OspfBackboneCell<Planes, false> {
-    using Base = OspfBackboneCell<Planes, false>;
+struct ChainSide {
     hspf::OspfChainSet chain;
-    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
-        uint32_t s = Base::status_word(j);
-        for (uint32_t b = 0; b < this->n_borders; ++b)
+    template <class R>
+    int bind(const hspf_ospfv2_backbone_table &t, const SideArgs<R> &a, uint32_t) {
+        if (t.n_asbr_slots && !a.border_entries) return HSPF_E_INVAL;
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
+            chain.entries[b] = nullptr; chain.status[b] = nullptr; chain.G[b] = 0;
+            if (b >= t.n_borders || !t.n_asbr_slots) continue;
+            chain.G[b] = (uint32_t)t.third[b]->asbr_group.size();
+            chain.entries[b] = a.border_entries[b];
+            chain.status[b] = a.border_entry_status ? a.border_entry_status[b] : nullptr;
+            if (chain.G[b] && (!a.border_entries[b] || (reinterpret_cast<uintptr_t>(a.border_entries[b]) & 3u)))
+                return HSPF_E_INVAL;
+        }
+        return HSPF_OK;
+    }
+    __device__ __forceinline__ uint32_t or_status(const OspfBackboneCore<Planes> &c, uint32_t s, uint32_t j) const {
+        for (uint32_t b = 0; b < c.n_borders; ++b)
             if (chain.status[b]) s |= chain.status[b][j];
         return s;
     }
-    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
-    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::OspfBorderRows rows;
-#pragma unroll
-        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
-        const hspf::OspfThirdAreaPlanes<Planes> pl{this->pl.job(0), {chain, j}};
-        return hspf::ospf_backbone_cell_eval<false, true, true>(pl, this->t, p, rows);
+    __device__ __forceinline__ hspf::OspfThirdAreaPlanes<Planes> planes(const Planes &pl, uint32_t j) const {
+        return {pl, {chain, j}};
     }
 };
 
-// The walk over an OSPFv3 third-area table (hspf_ospfv3_third_area_table_create), with or without chain slots: the C
-// cells' inter-area winners may be OSPFv3 slot winners, whose options ride in their low byte (kSlotWinners), and R's
-// slot winners carry those options.  A type of its own, so that the kernels above keep their instantiations.
-template <class Planes>
-struct OspfThirdAreaV3Cell : OspfThirdAreaCell<Planes> {
-    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
-        hspf::OspfBorderRows rows;
-#pragma unroll
-        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
-        const hspf::OspfThirdAreaPlanes<Planes> pl{this->pl.job(0), {this->chain, j}};
-        return hspf::ospf_backbone_cell_eval<true, true, true, true>(pl, this->t, p, rows);
-    }
-};
-
-// Blocks per SM of the kernels over this walk: their launch bound and their grid (DESIGN.md §4.4, §6), for OSPFv2
-// and for OSPFv3 tables, for OSPFv2 and OSPFv3 tables with type-4 / Inter-Area-Router slots, for OSPFv2 and OSPFv3
-// tables of a non-backbone target area, for OSPFv2 third-area tables with chain slots, and for OSPFv3 third-area
-// tables.
+// Blocks per SM of each walk's kernels: their launch bound and their grid (DESIGN.md §4.4, §6).
 constexpr uint32_t kBackboneBlocksPerSM = 4;
 constexpr uint32_t kBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kBackboneAsbrBlocksPerSM = 4;
@@ -159,122 +111,102 @@ constexpr uint32_t kNonBackboneV3BlocksPerSM = 4;
 constexpr uint32_t kThirdAreaBlocksPerSM = 4;
 constexpr uint32_t kThirdAreaV3BlocksPerSM = 4;
 
-template <class R, bool kV3>
-int make_cell(const hspf_ospfv2_backbone_table *t, const R *planes, const hl_ospf_rib_cell *const *border_cells,
-              const uint32_t *const *border_status, OspfBackboneCell<hspf::PlanesOf<R>, kV3> &cell) {
-    if (!t || !t->dev.blob || !border_cells) return HSPF_E_INVAL;
-    if (hspf::result_planes(planes, t->n_vertices, cell.pl) || !cell.pl.complete()) return HSPF_E_INVAL;
-    if (const int rc = hspf::bind_ospf_borders(*t, border_cells, border_status, cell)) return rc;
-    cell.t = t->view(t->dev.off, static_cast<const hspf::RibRec *>(t->dev.contribs));
-    return HSPF_OK;
-}
+// A walk: the flags it runs ospf_backbone_cell_eval with, its side input and its kernels' launch bound.
+template <bool V3, bool Asbr, bool NonBackbone, bool SlotWinners, template <class> class S, uint32_t Blocks>
+struct Walk {
+    static constexpr bool kV3 = V3, kAsbr = Asbr, kNonBackbone = NonBackbone, kSlotWinners = SlotWinners;
+    template <class Planes> using Side = S<Planes>;
+    static constexpr uint32_t kBlocks = Blocks;
+};
 
-template <bool kV3, class R, class Out>
-int version(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-            const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status, const Out &out) {
-    constexpr uint32_t kBlocks = kV3 ? kBackboneV3BlocksPerSM : kBackboneBlocksPerSM;
-    OspfBackboneCell<hspf::PlanesOf<R>, kV3> cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    return hspf::launch_route_stage<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
-}
+// Tables of area 0 (hspf_ospfv{2,3}_backbone_table_create), and those with type-4 / Inter-Area-Router slots
+// (hspf_ospfv{2,3}_backbone_asbr_table_create).
+struct WalkBackbone : Walk<false, false, false, false, NoSide, kBackboneBlocksPerSM> {};
+struct WalkBackboneV3 : Walk<true, false, false, false, NoSide, kBackboneV3BlocksPerSM> {};
+struct WalkBackboneAsbr : Walk<false, true, false, false, AsbrSide, kBackboneAsbrBlocksPerSM> {};
+struct WalkBackboneAsbrV3 : Walk<true, true, false, false, AsbrSide, kBackboneAsbrV3BlocksPerSM> {};
+// Tables of a non-backbone target area (hspf_ospfv{2,3}_nonbackbone_table_create), with or without slots: the borders
+// also advertise their inter-area routes, and a plane set may be a border's area 0.
+struct WalkNonBackbone : Walk<false, true, true, false, AsbrSide, kNonBackboneBlocksPerSM> {};
+struct WalkNonBackboneV3 : Walk<true, true, true, false, AsbrSide, kNonBackboneV3BlocksPerSM> {};
+// Third-area tables (hspf_ospfv{2,3}_third_area_table_create): the kNonBackbone walk over chain slots.  An OSPFv3
+// one's C cells may hold OSPFv3 slot winners, whose options ride in their low byte (kSlotWinners).
+struct WalkThirdArea : Walk<false, true, true, false, ChainSide, kThirdAreaBlocksPerSM> {};
+struct WalkThirdAreaV3 : Walk<true, true, true, true, ChainSide, kThirdAreaV3BlocksPerSM> {};
 
-// The launch of a walk over a table with type-4 / Inter-Area-Router slots or of a non-backbone target area (Cell):
-// the cell above plus the plane sets the slots name.
-template <class Cell, uint32_t kBlocks, class R, class Out>
-int asbr_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-            const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-            const R *const *border_planes, const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
-            const Out &out) {
-    Cell cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    if (const int rc = hspf::bind_ospf_asbr_sets(*t, border_planes, border_n_rows, border_rows, n_jobs, cell))
-        return rc;
-    return hspf::launch_route_stage<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
-}
-
-// a table of a non-backbone target area: the walk of its version
-template <class R, class Out>
-int nonbackbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                const R *const *border_planes, const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
-                const Out &out) {
-    using P = hspf::PlanesOf<R>;
-    return t->v3 ? asbr_as<OspfNonBackboneV3Cell<P>, kNonBackboneV3BlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out)
-                 : asbr_as<OspfNonBackboneCell<P>, kNonBackboneBlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out);
-}
-
-// The launch of a third-area walk (Cell) over each border's entries (border_entries[b] u32 [n_jobs][G_b], NULL allowed
-// for a border with no group; the array may be NULL for a table without chain slots, which reads no entries).
-template <class Cell, uint32_t kBlocks, class R, class Out>
-int chain_as(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-             const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-             const uint32_t *const *border_entries, const uint32_t *const *border_entry_status, const Out &out) {
-    Cell cell{};
-    if (const int rc = make_cell(t, planes, border_cells, border_status, cell)) return rc;
-    if (t->n_asbr_slots && !border_entries) return HSPF_E_INVAL;
-    for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) {
-        cell.chain.entries[b] = nullptr; cell.chain.status[b] = nullptr; cell.chain.G[b] = 0;
-        if (b >= t->n_borders || !t->n_asbr_slots) continue;
-        cell.chain.G[b] = (uint32_t)t->third[b]->asbr_group.size();
-        cell.chain.entries[b] = border_entries[b];
-        cell.chain.status[b] = border_entry_status ? border_entry_status[b] : nullptr;
-        if (cell.chain.G[b] && (!border_entries[b] || (reinterpret_cast<uintptr_t>(border_entries[b]) & 3u)))
-            return HSPF_E_INVAL;
+// The cell functor of walk W (route_stage.cuh).  A job's status word ORs R's row-0 word, the borders' words, then
+// the side input's.  Every walk is its own instantiation, with kernels of its own, so a walk added later leaves the
+// others' code alone.
+template <class Planes, class W>
+struct OspfBackboneWalkCell : OspfBackboneCore<Planes>, W::template Side<Planes> {
+    __device__ __forceinline__ uint32_t border_status(uint32_t j) const {
+        uint32_t s = this->pl.status_word(0);
+        for (uint32_t b = 0; b < this->n_borders; ++b)
+            if (this->status[b]) s |= this->status[b][j];
+        return s;
     }
-    return hspf::launch_route_stage<kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
+    __device__ __forceinline__ uint32_t status_word(uint32_t j) const {
+        return this->or_status(*this, border_status(j), j);
+    }
+    __device__ __forceinline__ bool refused(uint32_t j) const { return status_word(j) != 0; }
+    __device__ __forceinline__ hspf::CellWords operator()(uint32_t j, uint32_t p) const {
+        hspf::OspfBorderRows rows;
+#pragma unroll
+        for (uint32_t b = 0; b < kOspfBackboneMaxBorders; ++b) rows.row[b] = this->cells[b] + (size_t)j * this->K[b];
+        return hspf::ospf_backbone_cell_eval<W::kV3, W::kAsbr, W::kNonBackbone, W::kSlotWinners>(
+            this->planes(this->pl.job(0), j), this->t, p, rows);
+    }
+    __device__ __forceinline__ uint64_t gather(uint32_t, uint32_t, uint32_t) const { return 0; }   // row 0: host side
+    __device__ static hspf::CellWords empty() { return {0, 0, hspf::kNoRecord}; }
+};
+
+// The families of entry points: hspf_ospfv2_backbone_*, hspf_ospfv2_backbone_asbr_* and hspf_ospfv2_third_area_*.
+enum class Call { kBackbone, kAsbr, kThirdArea };
+
+// The walk a call of the family runs over t, picked from the table's marks and handed to run as a tag; HSPF_E_INVAL
+// for a table the family refuses.
+template <class F>
+int pick_walk(const hspf_ospfv2_backbone_table *t, Call call, F &&run) {
+    if (!t) return HSPF_E_INVAL;
+    switch (call) {
+    case Call::kBackbone:
+        // a table with type-4 slots is the asbr calls'; an OSPFv3 third-area table's C cells hold slot winners, which
+        // only the third-area calls read
+        if (t->n_asbr_slots || (t->third_area && t->v3)) return HSPF_E_INVAL;
+        if (t->area_id) return t->v3 ? run(WalkNonBackboneV3{}) : run(WalkNonBackbone{});
+        return t->v3 ? run(WalkBackboneV3{}) : run(WalkBackbone{});
+    case Call::kAsbr:
+        // an OSPFv3 table of area 0 only from hspf_ospfv3_backbone_asbr_table_create; a third-area table's type-4
+        // slots are chain slots, and an OSPFv3 one's C cells hold slot winners
+        if ((t->v3 && !t->area_id && !t->asbr) || (t->third_area && (t->n_asbr_slots || t->v3))) return HSPF_E_INVAL;
+        if (t->area_id) return t->v3 ? run(WalkNonBackboneV3{}) : run(WalkNonBackbone{});
+        if (!t->n_asbr_slots) return t->v3 ? run(WalkBackboneV3{}) : run(WalkBackbone{});   // border planes unread
+        return t->v3 ? run(WalkBackboneAsbrV3{}) : run(WalkBackboneAsbr{});
+    case Call::kThirdArea:
+        // an OSPFv3 table with or without chain slots: the kNonBackbone walks cannot read C's slot winners
+        if (!t->third_area) return HSPF_E_INVAL;
+        if (t->v3) return run(WalkThirdAreaV3{});
+        return t->n_asbr_slots ? run(WalkThirdArea{}) : run(WalkNonBackbone{});
+    }
+    return HSPF_E_INVAL;
 }
 
-// A third-area table.  OSPFv2: with chain slots the OspfThirdAreaCell walk, else the plain kNonBackbone walk.  OSPFv3:
-// the OspfThirdAreaV3Cell walk, with or without chain slots (the kNonBackbone walks cannot read C's slot winners).
+// A call: its walk, then R's planes, the borders' cells and status words and the walk's side input into the cell,
+// then the launch.
 template <class R, class Out>
-int third_area(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-               const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-               const uint32_t *const *border_entries, const uint32_t *const *border_entry_status, const Out &out) {
-    if (!t || !t->third_area) return HSPF_E_INVAL;
-    using P = hspf::PlanesOf<R>;
-    if (t->v3)
-        return chain_as<OspfThirdAreaV3Cell<P>, kThirdAreaV3BlocksPerSM>(
-            ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status, out);
-    if (!t->n_asbr_slots)
-        return nonbackbone<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr, out);
-    return chain_as<OspfThirdAreaCell<P>, kThirdAreaBlocksPerSM>(ctx, t, n_jobs, planes, border_cells, border_status,
-                                                                 border_entries, border_entry_status, out);
-}
-
-// the walk of the table's version and target area; a table with type-4 slots is backbone_asbr's
-template <class R, class Out>
-int backbone(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-             const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status, const Out &out) {
-    // an OSPFv3 third-area table's C cells hold slot winners, which only the third-area calls read
-    if (!t || t->n_asbr_slots || (t->third_area && t->v3)) return HSPF_E_INVAL;
-    if (t->area_id)
-        return nonbackbone<R>(ctx, t, n_jobs, planes, border_cells, border_status, nullptr, nullptr, nullptr, out);
-    return t->v3 ? version<true>(ctx, t, n_jobs, planes, border_cells, border_status, out)
-                 : version<false>(ctx, t, n_jobs, planes, border_cells, border_status, out);
-}
-
-// A table without type-4 slots takes backbone (NULL border planes allowed).  An OSPFv3 table of area 0 is refused
-// unless hspf_ospfv3_backbone_asbr_table_create made it.
-template <class R, class Out>
-int backbone_asbr(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
-                  const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status,
-                  const R *const *border_planes, const uint32_t *const *border_n_rows,
-                  const uint32_t *const *border_rows, const Out &out) {
-    // a third-area table's type-4 slots are chain slots, and an OSPFv3 one's C cells hold slot winners: only the
-    // third-area calls read those
-    if (!t || (t->v3 && !t->area_id && !t->asbr) || (t->third_area && (t->n_asbr_slots || t->v3)))
-        return HSPF_E_INVAL;
-    if (t->area_id)
-        return nonbackbone(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows,
-                           border_rows, out);
-    if (!t->n_asbr_slots) return backbone(ctx, t, n_jobs, planes, border_cells, border_status, out);
-    using P = hspf::PlanesOf<R>;
-    return t->v3 ? asbr_as<OspfBackboneAsbrV3Cell<P>, kBackboneAsbrV3BlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out)
-                 : asbr_as<OspfBackboneAsbrCell<P>, kBackboneAsbrBlocksPerSM>(
-                       ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows, out);
+int stage(hspf_ctx *ctx, Call call, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs, const R *planes,
+          const hl_ospf_rib_cell *const *border_cells, const uint32_t *const *border_status, const SideArgs<R> &side,
+          const Out &out) {
+    return pick_walk(t, call, [&](auto walk) {
+        using W = decltype(walk);
+        OspfBackboneWalkCell<hspf::PlanesOf<R>, W> cell{};
+        if (!t->dev.blob || !border_cells) return HSPF_E_INVAL;
+        if (hspf::result_planes(planes, t->n_vertices, cell.pl) || !cell.pl.complete()) return HSPF_E_INVAL;
+        if (const int rc = hspf::bind_ospf_borders(*t, border_cells, border_status, cell)) return rc;
+        cell.t = t->view(t->dev.off, static_cast<const hspf::RibRec *>(t->dev.contribs));
+        if (const int rc = cell.bind(*t, side, n_jobs)) return rc;
+        return hspf::launch_route_stage<W::kBlocks>(ctx, t->dev, cell, n_jobs, t->P(), out);
+    });
 }
 
 }  // namespace
@@ -289,15 +221,15 @@ int hspf_ospfv2_backbone_table_upload(hspf_ctx *ctx, hspf_ospfv2_backbone_table 
 int hspf_ospfv2_backbone_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
                                const hspf_result *planes, const hl_ospf_rib_cell *const *border_cells,
                                const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
-                    hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+    return stage(ctx, Call::kBackbone, t, n_jobs, planes, border_cells, border_status, {},
+                 hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
                                  const hspf_result16 *planes, const hl_ospf_rib_cell *const *border_cells,
                                  const uint32_t *const *border_status, uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
-                    hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+    return stage(ctx, Call::kBackbone, t, n_jobs, planes, border_cells, border_status, {},
+                 hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -305,8 +237,8 @@ int hspf_ospfv2_backbone_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *
                                const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells, uint32_t n_base,
                                const uint32_t *base_of, hl_route_delta_job *job_out, hl_route_delta *records,
                                uint64_t cap, uint64_t *n_records) {
-    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
-                    hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+    return stage(ctx, Call::kBackbone, t, n_jobs, planes, border_cells, border_status, {},
+                 hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -314,8 +246,8 @@ int hspf_ospfv2_backbone_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table
                                  const uint32_t *const *border_status, const hl_ospf_rib_cell *base_cells,
                                  uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                                  hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return backbone(ctx, t, n_jobs, planes, border_cells, border_status,
-                    hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+    return stage(ctx, Call::kBackbone, t, n_jobs, planes, border_cells, border_status, {},
+                 hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -323,8 +255,8 @@ int hspf_ospfv2_backbone_asbr_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_ta
                                     const uint32_t *const *border_status, const hspf_result *const *border_planes,
                                     const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                     uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                         hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+    return stage(ctx, Call::kAsbr, t, n_jobs, planes, border_cells, border_status,
+                 {border_planes, border_n_rows, border_rows}, hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_asbr_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -332,8 +264,8 @@ int hspf_ospfv2_backbone_asbr_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_
                                       const uint32_t *const *border_status, const hspf_result16 *const *border_planes,
                                       const uint32_t *const *border_n_rows, const uint32_t *const *border_rows,
                                       uint32_t *job_status_out, hl_ospf_rib_cell *cells) {
-    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                         hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+    return stage(ctx, Call::kAsbr, t, n_jobs, planes, border_cells, border_status,
+                 {border_planes, border_n_rows, border_rows}, hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -343,8 +275,9 @@ int hspf_ospfv2_backbone_asbr_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_ta
                                     const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                     hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                                     uint64_t *n_records) {
-    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                         hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+    return stage(ctx, Call::kAsbr, t, n_jobs, planes, border_cells, border_status,
+                 {border_planes, border_n_rows, border_rows},
+                 hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -354,8 +287,9 @@ int hspf_ospfv2_backbone_asbr_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_
                                       const hl_ospf_rib_cell *base_cells, uint32_t n_base, const uint32_t *base_of,
                                       hl_route_delta_job *job_out, hl_route_delta *records, uint64_t cap,
                                       uint64_t *n_records) {
-    return backbone_asbr(ctx, t, n_jobs, planes, border_cells, border_status, border_planes, border_n_rows, border_rows,
-                         hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+    return stage(ctx, Call::kAsbr, t, n_jobs, planes, border_cells, border_status,
+                 {border_planes, border_n_rows, border_rows},
+                 hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_third_area_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -363,8 +297,9 @@ int hspf_ospfv2_third_area_cells(hspf_ctx *ctx, const hspf_ospfv2_backbone_table
                                  const uint32_t *const *border_status, const uint32_t *const *border_entries,
                                  const uint32_t *const *border_entry_status, uint32_t *job_status_out,
                                  hl_ospf_rib_cell *cells) {
-    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
-                      hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+    return stage(ctx, Call::kThirdArea, t, n_jobs, planes, border_cells, border_status,
+                 {nullptr, nullptr, nullptr, border_entries, border_entry_status},
+                 hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_third_area_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -372,8 +307,9 @@ int hspf_ospfv2_third_area_cells16(hspf_ctx *ctx, const hspf_ospfv2_backbone_tab
                                    const uint32_t *const *border_status, const uint32_t *const *border_entries,
                                    const uint32_t *const *border_entry_status, uint32_t *job_status_out,
                                    hl_ospf_rib_cell *cells) {
-    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
-                      hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
+    return stage(ctx, Call::kThirdArea, t, n_jobs, planes, border_cells, border_status,
+                 {nullptr, nullptr, nullptr, border_entries, border_entry_status},
+                 hspf::CellsOut<hl_ospf_rib_cell>{cells, job_status_out});
 }
 
 int hspf_ospfv2_third_area_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -382,8 +318,9 @@ int hspf_ospfv2_third_area_delta(hspf_ctx *ctx, const hspf_ospfv2_backbone_table
                                  const uint32_t *const *border_entry_status, const hl_ospf_rib_cell *base_cells,
                                  uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                                  hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
-                      hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+    return stage(ctx, Call::kThirdArea, t, n_jobs, planes, border_cells, border_status,
+                 {nullptr, nullptr, nullptr, border_entries, border_entry_status},
+                 hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 int hspf_ospfv2_third_area_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_table *t, uint32_t n_jobs,
@@ -392,8 +329,9 @@ int hspf_ospfv2_third_area_delta16(hspf_ctx *ctx, const hspf_ospfv2_backbone_tab
                                    const uint32_t *const *border_entry_status, const hl_ospf_rib_cell *base_cells,
                                    uint32_t n_base, const uint32_t *base_of, hl_route_delta_job *job_out,
                                    hl_route_delta *records, uint64_t cap, uint64_t *n_records) {
-    return third_area(ctx, t, n_jobs, planes, border_cells, border_status, border_entries, border_entry_status,
-                      hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
+    return stage(ctx, Call::kThirdArea, t, n_jobs, planes, border_cells, border_status,
+                 {nullptr, nullptr, nullptr, border_entries, border_entry_status},
+                 hspf::DeltaOut<hl_ospf_rib_cell>{base_cells, n_base, base_of, job_out, records, cap, n_records});
 }
 
 }  // extern "C"

@@ -105,7 +105,7 @@ def main():
     cur = stage_bench.launch_bound(*BOUND)
     other = 8 if cur == 4 else 4
     lib_path, log = stage_bench.build_variant(*BOUND, other, "backbone_asbr_v3_bound_", ptxas=True)
-    regs_other = stage_bench.ptxas_registers(log, lambda k: "OspfBackboneAsbrV3Cell" in k)
+    regs_other = stage_bench.ptxas_registers(log, lambda k: "WalkBackboneAsbrV3" in k)
     libv = C.CDLL(str(lib_path))
     route_table.declare(libv)
     # the variant's own tables over the same images

@@ -98,7 +98,7 @@ def main():
     cur = stage_bench.launch_bound(*BOUND)
     other = 8 if cur == 4 else 4
     lib_path, log = stage_bench.build_variant(*BOUND, other, "backbone_v3_bound_", ptxas=True)
-    regs_other = stage_bench.ptxas_registers(log, lambda k: "OspfBackboneCell" in k and "Lb1E" in k)
+    regs_other = stage_bench.ptxas_registers(log, lambda k: "WalkBackboneV3" in k)
     libv = C.CDLL(str(lib_path))
     route_table.declare(libv)
     # the variant's own tables over the same images
